@@ -1,12 +1,13 @@
 """Batch fisheye undistortion on the GPU -- counterpart of the reference's Tools/undistort.py:25-77.
 
-The undistortion map is built once on the device and never leaves it; each image then costs one
-upload, one gather kernel and one download.  Decoding / encoding image files stays on the host with
-cv2, as in the reference.  The command line accepts the reference's flags with the same defaults;
-boolean flags additionally understand 0/1/true/false (the reference's ``type=bool`` turns every
-non-empty string into True), and ``-fused 1`` evaluates the camera model inside the gather kernel
-instead of keeping a map in HBM; ``-workers N`` sizes the decode/encode thread pool that overlaps
-the image files' JPEG/PNG work with the GPU calls.
+The undistortion map is built once on the device and never leaves it.  With ``-dstformat jpg`` (the
+default) each image costs one upload, one gather kernel and the device JPEG encoder, and only the
+compressed stream comes back -- the same bytes cv2.imwrite writes; other formats download the image and
+encode it with cv2 as the reference does.  Decoding the source files stays on the host with cv2.  The
+command line accepts the reference's flags with the same defaults; boolean flags additionally understand
+0/1/true/false (the reference's ``type=bool`` turns every non-empty string into True), and ``-fused 1``
+evaluates the camera model inside the gather kernel instead of keeping a map in HBM; ``-workers N`` sizes
+the thread pool that decodes source files and writes finished ones while the GPU calls run.
 """
 from __future__ import annotations
 
@@ -66,10 +67,13 @@ def build_undistorter(opts) -> ops.Undistorter:
     return ops.Undistorter(K, D, P, size, fused=opts.fused)
 
 
+def _write_bytes(path, data):
+    with open(path, "wb") as f:
+        f.write(data)
+
+
 def _save(cv2, opts, stem_in_save_dir, bare_stem, img):
-    if opts.dstformat == "jpg":
-        cv2.imwrite(stem_in_save_dir + ".jpg", img, [cv2.IMWRITE_JPEG_QUALITY, opts.quality])
-    elif opts.dstformat == "png":
+    if opts.dstformat == "png":
         cv2.imwrite(stem_in_save_dir + ".png", img, [cv2.IMWRITE_PNG_COMPRESSION, opts.quality])
     else:   # the reference writes other formats next to the working directory
         cv2.imwrite(bare_stem + "." + opts.dstformat, img)
@@ -77,9 +81,11 @@ def _save(cv2, opts, stem_in_save_dir, bare_stem, img):
 
 def run_directory(opts, undistorter, cv2):
     """Decode -> undistort -> encode over a directory, overlapped: a thread pool decodes the next files
-    and encodes finished ones (cv2 releases the GIL in imread/imwrite) while the GPU call for the current
-    image runs on the calling thread.  Files are processed and numbered in ``os.listdir`` order exactly as
-    the reference's serial loop does (:59-77); at most ``2 * workers`` decoded images are held at a time."""
+    and writes finished ones (cv2 releases the GIL in imread/imwrite) while the GPU call for the current
+    image runs on the calling thread.  For ``-dstformat jpg`` that call is ``undistorter.jpeg`` -- undistort
+    and encode on the device, the pool only writes the bytes; other formats are encoded by cv2 in the pool.
+    Files are processed and numbered in ``os.listdir`` order exactly as the reference's serial loop does
+    (:59-77); at most ``2 * workers`` decoded images are held at a time."""
     from collections import deque
     from concurrent.futures import ThreadPoolExecutor
 
@@ -87,6 +93,7 @@ def run_directory(opts, undistorter, cv2):
     entries = [e for e in os.listdir(opts.path_read) if e[-4:] == suffix]
     workers = max(1, int(opts.workers))
     written, encodes = [], deque()
+    device_jpeg = opts.dstformat == "jpg"
     with ThreadPoolExecutor(max_workers=workers) as pool:
         decodes, upcoming = deque(), iter(entries)
 
@@ -102,12 +109,18 @@ def run_directory(opts, undistorter, cv2):
         while decodes:
             entry, pending = decodes.popleft()
             top_up()
-            result = undistorter(pending.result())
+            if device_jpeg:
+                result = undistorter.jpeg(pending.result(), opts.quality)
+            else:
+                result = undistorter(pending.result())
             if opts.name is not None:
                 entry = "{}_{:04d}.{}".format(opts.name, counter, opts.srcformat)
                 counter += 1
             stem = entry[:-4]
-            encodes.append(pool.submit(_save, cv2, opts, os.path.join(opts.path_save, stem), stem, result))
+            if device_jpeg:
+                encodes.append(pool.submit(_write_bytes, os.path.join(opts.path_save, stem) + ".jpg", result))
+            else:
+                encodes.append(pool.submit(_save, cv2, opts, os.path.join(opts.path_save, stem), stem, result))
             while len(encodes) > 2 * workers:
                 encodes.popleft().result()
             written.append(entry)

@@ -74,6 +74,11 @@ SIGNATURES = {
     "bevk_shard_compose": (C.c_int, [_p, _p, C.c_int, _p, _p]),
     "bevk_jpeg_decode": (C.c_int, [_p, C.POINTER(_p), C.POINTER(C.c_uint64), C.c_int, C.c_int, C.c_int, _p, C.c_int64]),
     "bevk_bev_run_jpeg": (C.c_int, [_p, C.POINTER(_p), C.POINTER(C.c_uint64), C.c_int, _p, C.c_int, _p]),
+    "bevk_jpeg_encode_bound": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_uint64)]),
+    "bevk_jpeg_encode": (C.c_int, [_p, _p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, _p, C.c_uint64,
+                                   C.POINTER(C.c_uint64)]),
+    "bevk_undistort_jpeg": (C.c_int, [_p, C.c_int, _p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, _p, C.c_uint64,
+                                      C.POINTER(C.c_uint64)]),
     "bevk_graph_begin": (C.c_int, [_p]),
     "bevk_graph_end": (C.c_int, [_p, C.POINTER(C.c_int)]),
     "bevk_graph_launch": (C.c_int, [_p, C.c_int, C.c_int]),

@@ -24,6 +24,9 @@
 #include "bevk_bev_tma.cuh"
 #include "bevk_plan_tma.cuh"
 #include "bevk_shard.cuh"
+#include "bevk_jpeg_enc.cuh"
+
+#include <cub/device/device_scan.cuh>
 
 #include <dlfcn.h>
 #include <nvtx3/nvToolsExt.h>   // header-only: ranges cost nothing unless a profiler injects itself
@@ -197,6 +200,13 @@ struct bevk_ctx {
   // nvJPEG ingest (bevk_jpeg_decode): library handle + decoder state, created on first use
   void* jpeg_handle = nullptr; void* jpeg_state = nullptr;
   DevBuf d_jpeg_frames, d_jpeg_canvas;
+  // JPEG encoder (bevk_jpeg_encode): header and tables of the last (width, height, quality), work buffers
+  struct JpegEnc {
+    int w = 0, h = 0, q = -1;
+    uint8_t header[jpeg::kHeaderBytes];
+    DevBuf d_header, d_tabs, coef, bits, offs, dcdiff, words, ffcnt, ffscan, scan_tmp, out, meta;
+    std::vector<unsigned long long> sizes;
+  } enc;
   // CUDA graphs captured from the device-pointer entry points (bevk_graph_*)
   bool capturing = false;
   long long capture_launches0 = 0;
@@ -257,6 +267,9 @@ int bevk_ctx_destroy(bevk_ctx* c) {
                     &c->d_hsv, &c->d_frames, &c->d_ptrs, &c->d_canvas, &c->d_car, &c->d_vsum, &c->d_delta, &c->d_csum,
                     &c->d_spans, &c->d_bal, &c->d_bal_ptrs, &c->d_user_ptrs, &c->d_ttiles, &c->d_titems, &c->d_tlut,
                     &c->d_stack_ptrs, &c->d_jpeg_frames, &c->d_jpeg_canvas, &c->d_unit_counter})
+    b->release();
+  for (DevBuf* b : {&c->enc.d_header, &c->enc.d_tabs, &c->enc.coef, &c->enc.bits, &c->enc.offs, &c->enc.dcdiff, &c->enc.words,
+                    &c->enc.ffcnt, &c->enc.ffscan, &c->enc.scan_tmp, &c->enc.out, &c->enc.meta})
     b->release();
   for (auto& m : c->maps) m.d.release();
   shard_release(c);
@@ -442,15 +455,12 @@ int bevk_undistorter_maps(bevk_ctx* c, int slot, int16_t* map1, uint16_t* map2) 
   return BEVK_OK;
 }
 
-int bevk_undistort(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
-                   uint8_t* dst, int dw, int dh, int64_t dstride, int interp) {
-  RET(use(c));
-  if (slot < 0 || slot >= 8 || !c->und[slot].valid) return fail(BEVK_ERR_ARG, "undistorter slot %d not set", slot);
+// Upload a host frame and gather the slot's undistorted image into c->s_dst (dense, row pitch dw * channels).
+static int undistort_to_scratch(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
+                                int interp) {
   Undistorter& u = c->und[slot];
-  if (dw != u.cm.w || dh != u.cm.h)   // the caller sized dst for another map: never write past it
-    return fail(BEVK_ERR_ARG, "undistorter slot %d holds a %dx%d map, the caller expects %dx%d", slot, u.cm.w, u.cm.h, dw, dh);
+  const int dw = u.cm.w, dh = u.cm.h;
   RET(check_image(src, sw, sh, sstride, channels, "src"));
-  RET(check_image(dst, dw, dh, dstride, channels, "dst"));
   if (interp != BEVK_INTER_LINEAR && interp != BEVK_INTER_NEAREST) return fail(BEVK_ERR_UNSUPPORTED, "interp %d", interp);
   RET(upload_image(c, c->s_src, src, sw, sh, sstride, channels));
   RET(c->s_dst.ensure((size_t)dw * dh * channels));
@@ -464,6 +474,18 @@ int bevk_undistort(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, in
     a.map1 = u.map1.as<short2>(); a.map2 = u.map2.as<unsigned short>();
     RET(launch_gather<0>(c, a, channels, interp));
   }
+  return BEVK_OK;
+}
+
+int bevk_undistort(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
+                   uint8_t* dst, int dw, int dh, int64_t dstride, int interp) {
+  RET(use(c));
+  if (slot < 0 || slot >= 8 || !c->und[slot].valid) return fail(BEVK_ERR_ARG, "undistorter slot %d not set", slot);
+  Undistorter& u = c->und[slot];
+  if (dw != u.cm.w || dh != u.cm.h)   // the caller sized dst for another map: never write past it
+    return fail(BEVK_ERR_ARG, "undistorter slot %d holds a %dx%d map, the caller expects %dx%d", slot, u.cm.w, u.cm.h, dw, dh);
+  RET(check_image(dst, dw, dh, dstride, channels, "dst"));
+  RET(undistort_to_scratch(c, slot, src, sw, sh, sstride, channels, interp));
   return download_image(c, c->s_dst, dst, dw, dh, dstride, channels);
 }
 
@@ -1726,6 +1748,123 @@ int bevk_bev_run_jpeg(bevk_ctx* c, const uint8_t* const* jpegs, const uint64_t* 
   CU(cudaMemcpyAsync(out, c->d_jpeg_canvas.p, cbytes * batch, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaStreamSynchronize(c->stream));
   return BEVK_OK;
+}
+
+// ------------------------------------------------------------------ JPEG encode on the device (bevk_jpeg_enc.cuh)
+// The reference writes its results with cv2.imwrite (Tools/undistort.py:72-73, surroundBEV.py:340): D2H of the whole
+// image, then libjpeg-turbo on a host core.  Here the encoder runs on the device and only the streams cross PCIe.
+int bevk_jpeg_encode_bound(int width, int height, uint64_t* bytes) {
+  if (!bytes) return fail(BEVK_ERR_ARG, "null bytes");
+  if (width < 1 || height < 1 || width > jpeg::kMaxDim || height > jpeg::kMaxDim)
+    return fail(BEVK_ERR_ARG, "bad JPEG size %dx%d (1..%d)", width, height, jpeg::kMaxDim);
+  *bytes = jpeg::encode_bound(width, height);
+  return BEVK_OK;
+}
+
+static int jpeg_encode_device(bevk_ctx* c, const void* d_images, int64_t istride, int64_t pitch, int n, int w, int h, int quality,
+                              uint8_t* out, uint64_t capacity, uint64_t* sizes) {
+  using namespace jpeg;
+  auto& e = c->enc;
+  if (c->capturing) return fail(BEVK_ERR_ARG, "bevk_jpeg_encode synchronises and cannot be captured into a graph");
+  const int q = clamp_quality(quality);
+  if (w != e.w || h != e.h || q != e.q) {   // header + tables depend on (w, h, quality) only
+    Tables t;
+    make_tables(q, &t);
+    make_header(w, h, q, e.header);
+    RET(e.d_header.ensure(kHeaderBytes));
+    RET(e.d_tabs.ensure(sizeof(Tables)));
+    CU(cudaMemcpyAsync(e.d_header.p, e.header, kHeaderBytes, cudaMemcpyHostToDevice, c->stream));   // pageable: staged
+    CU(cudaMemcpyAsync(e.d_tabs.p, &t, sizeof t, cudaMemcpyHostToDevice, c->stream));               // before returning
+    e.w = w; e.h = h; e.q = q;
+  }
+  const Geom g = geom(w, h);
+  const long long nblk = blocks_per_image(g), nb = nblk * n;
+  const long long words_img = ((long long)((entropy_bound_bits(w, h) + 31) / 32) + 3) & ~3ll;   // 16-byte aligned regions
+  const int chunks = (int)((words_img * 4 + kChunk - 1) / kChunk);
+  const long long nch = (long long)n * chunks;
+  if (nb > INT_MAX || nch > INT_MAX) return fail(BEVK_ERR_ARG, "batch of %d %dx%d images is too large for one call", n, w, h);
+  RET(e.coef.ensure((size_t)nb * 128));
+  RET(e.bits.ensure((size_t)nb * 8));
+  RET(e.offs.ensure((size_t)nb * 8));
+  RET(e.dcdiff.ensure((size_t)nb * 4));
+  RET(e.words.ensure((size_t)(n * words_img * 4)));
+  const size_t ffcap = e.ffcnt.cap;
+  RET(e.ffcnt.ensure((size_t)nch * 4));
+  if (e.ffcnt.cap != ffcap) CU(cudaMemsetAsync(e.ffcnt.p, 0, e.ffcnt.cap, c->stream));
+  RET(e.ffscan.ensure((size_t)nch * 4));
+  RET(e.out.ensure((size_t)n * encode_bound(w, h)));
+  RET(e.meta.ensure((size_t)n * 16));
+  size_t tmp1 = 0, tmp2 = 0;
+  CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp1, e.bits.as<unsigned long long>(), e.offs.as<unsigned long long>(), (int)nb));
+  CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp2, e.ffcnt.as<unsigned>(), e.ffscan.as<unsigned>(), (int)nch));
+  const size_t tmp = std::max(tmp1, tmp2);
+  RET(e.scan_tmp.ensure(tmp));
+
+  EncArgs a{};
+  a.img = reinterpret_cast<const uint8_t*>(d_images); a.istride = istride; a.pitch = pitch; a.n = n; a.g = g; a.nblk = nblk;
+  a.tabs = e.d_tabs.as<Tables>(); a.coef = e.coef.as<int16_t>(); a.bits = e.bits.as<unsigned long long>();
+  a.offs = e.offs.as<unsigned long long>(); a.dcdiff = e.dcdiff.as<int>(); a.words = e.words.as<uint32_t>(); a.words_img = words_img;
+  a.chunks_img = chunks; a.ffcnt = e.ffcnt.as<unsigned>(); a.ffscan = e.ffscan.as<unsigned>(); a.header = e.d_header.as<uint8_t>();
+  a.out = e.out.as<uint8_t>(); a.out_off = e.meta.as<unsigned long long>(); a.sizes = e.meta.as<unsigned long long>() + n;
+  const unsigned gb = (unsigned)((nb + kBlockThreads - 1) / kBlockThreads), gc = (unsigned)((nch + 255) / 256);
+  CU(cudaEventRecord(c->ev0, c->stream));
+  k_jpeg_blocks<<<gb, kBlockThreads, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  k_jpeg_dc<<<gb, kBlockThreads, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  CU(cub::DeviceScan::ExclusiveSum(e.scan_tmp.p, tmp1, a.bits, a.offs, (int)nb, c->stream));
+  k_jpeg_zero<<<c->n_sm * 4, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  k_jpeg_pack<<<gb, kBlockThreads, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  k_jpeg_ffcount<<<gc, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  CU(cub::DeviceScan::ExclusiveSum(e.scan_tmp.p, tmp2, a.ffcnt, a.ffscan, (int)nch, c->stream));
+  k_jpeg_layout<<<1, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  k_jpeg_stuff<<<gc, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  CU(cudaEventRecord(c->ev1, c->stream));
+  c->timed = true;
+  e.sizes.resize(n);
+  CU(cudaMemcpyAsync(e.sizes.data(), a.sizes, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  unsigned long long total = 0;
+  for (int i = 0; i < n; ++i) {
+    sizes[i] = e.sizes[i];
+    total += e.sizes[i];
+  }
+  if (total > capacity)
+    return fail(BEVK_ERR_ARG, "the %d JPEG streams take %llu bytes, capacity is %llu", n, total, (unsigned long long)capacity);
+  CU(cudaMemcpyAsync(out, e.out.p, total, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  return BEVK_OK;
+}
+
+int bevk_jpeg_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, int64_t row_stride, int n, int width, int height,
+                     int quality, uint8_t* out, uint64_t capacity, uint64_t* sizes) {
+  NvtxRange nvtx_call("bevk_jpeg_encode (device images -> host JPEG streams)");
+  RET(use(c));
+  if (!d_images || !out || !sizes || n < 1) return fail(BEVK_ERR_ARG, "bad argument");
+  uint64_t bound = 0;
+  RET(bevk_jpeg_encode_bound(width, height, &bound));
+  if (row_stride < (int64_t)width * 3) return fail(BEVK_ERR_ARG, "row stride %lld < %d bytes", (long long)row_stride, width * 3);
+  if (n > 1 && image_stride < (int64_t)(height - 1) * row_stride + width * 3)
+    return fail(BEVK_ERR_ARG, "image stride %lld is smaller than one image", (long long)image_stride);
+  return jpeg_encode_device(c, d_images, image_stride, row_stride, n, width, height, quality, out, capacity, sizes);
+}
+
+int bevk_undistort_jpeg(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int interp, int quality,
+                        uint8_t* out, uint64_t capacity, uint64_t* size) {
+  NvtxRange nvtx_call("bevk_undistort_jpeg (host frame -> undistorted JPEG)");
+  RET(use(c));
+  if (slot < 0 || slot >= 8 || !c->und[slot].valid) return fail(BEVK_ERR_ARG, "undistorter slot %d not set", slot);
+  if (!out || !size) return fail(BEVK_ERR_ARG, "bad argument");
+  const int dw = c->und[slot].cm.w, dh = c->und[slot].cm.h;
+  uint64_t bound = 0;
+  RET(bevk_jpeg_encode_bound(dw, dh, &bound));
+  RET(undistort_to_scratch(c, slot, src, sw, sh, sstride, 3, interp));
+  return jpeg_encode_device(c, c->s_dst.p, 0, (int64_t)dw * 3, 1, dw, dh, quality, out, capacity, size);
 }
 
 // ------------------------------------------------------------------ CUDA graphs

@@ -1,0 +1,553 @@
+// bevk_jpeg_enc.cuh -- baseline JPEG encoder on the device (sm_90a), byte-identical to cv2.imwrite / cv2.imencode.
+//
+// cv2 writes JPEG through libjpeg-turbo's baseline compressor: fixed Annex K Huffman tables, 4:2:0, islow integer DCT,
+// no restart markers.  That path is integer arithmetic end to end with no data-dependent choices, so the stream can be
+// reproduced byte for byte:
+//   colour     Y/Cb/Cr from BGR with libjpeg's 16-bit fixed-point constants (jccolor.c)
+//   edges      luma replicated to whole blocks; chroma sources replicated to 16*ceil(W/16) columns, row pairs clamped
+//              to H-1, chroma rows past ceil(H/2) repeat the last chroma row (jcsample.c h2v2 + jcprepct.c)
+//   dummies    luma blocks outside ceil(W/8) x ceil(H/8) inside an MCU: AC 0, DC = quantised DC of the block before
+//              it in the MCU (jccoefct.c)
+//   FDCT       jfdctint.c (CONST_BITS 13, PASS1_BITS 2), output scaled by 8; quantised as sign * ((|c| + d/2) / d)
+//   entropy    DC differences per component in scan order, AC (run, size) with ZRL / EOB, 0xFF stuffing, 1-bit pad
+// Everything per block is __host__ __device__: tests/host/jpeg_enc.cu runs the same functions serially over a whole
+// image and compares the stream with live cv2.imencode.
+//
+// Device pipeline for n equal-sized images (bevk_api.cu: jpeg_encode_device):
+//   k_jpeg_blocks  one thread per 8x8 block: BGR -> samples with the edge rules, FDCT, quantise, int16 zigzag
+//                  coefficients (768 B per MCU) and the block's AC bit count
+//   k_jpeg_dc      DC differences (dummy blocks resolved), bits per block
+//   scan           exclusive sum of bits per block (CUB): every block's bit offset in its image's stream
+//   k_jpeg_zero    clears the used words of each image's bit buffer
+//   k_jpeg_pack    every block writes its codes at its offset; words shared with neighbours take atomicOr
+//   k_jpeg_ffcount 0xFF bytes per 128-byte chunk; scan (CUB); k_jpeg_layout: stream sizes, compact offsets, header + EOI
+//   k_jpeg_stuff   chunk copy with a 0x00 after every 0xFF, into the compacted output
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+#include <string.h>
+
+namespace bevk {
+namespace jpeg {
+
+constexpr int kHeaderBytes = 623;             // SOI + APP0 + 2 DQT + SOF0 + 4 DHT + SOS
+constexpr int kMaxBlockBits = 11 + 11 + 63 * (16 + 10);   // DC code + value, 63 AC codes (<= 16 bits) + values (<= 10)
+constexpr int kChunk = 128;                   // bytes per thread of the stuffing pass
+constexpr int kMaxDim = 65500;                // JPEG_MAX_DIMENSION of libjpeg
+
+// Per-quality tables the kernels read (built on the host, copied into shared memory per CTA).
+struct Tables {
+  uint32_t ac[2][256];     // (length << 16) | code per AC symbol (run << 4 | size); [0] luma, [1] chroma
+  uint32_t dc[2][12];      // the same per DC category
+  uint16_t qdiv[2][64];    // 8 * quantisation step, natural order
+  uint8_t zz[64];          // zigzag index -> natural index
+};
+
+// ------------------------------------------------------------------ geometry
+struct Geom {
+  int W, H, mcux, mcuy, wb, hb;   // MCUs across / down, luma blocks across / down that hold image samples
+};
+__host__ __device__ inline Geom geom(int W, int H) {
+  Geom g;
+  g.W = W; g.H = H;
+  g.mcux = (W + 15) / 16; g.mcuy = (H + 15) / 16;
+  g.wb = (W + 7) / 8; g.hb = (H + 7) / 8;
+  return g;
+}
+// blocks of one image in scan order: MCU raster, per MCU Y00 Y01 Y10 Y11 Cb Cr
+__host__ __device__ inline long long blocks_per_image(const Geom& g) { return (long long)g.mcux * g.mcuy * 6; }
+
+// luma block k (0..3) of MCU (mx, my) lies outside the image's blocks: a dummy (AC 0, DC of the block before it)
+__host__ __device__ inline bool is_dummy(const Geom& g, int mx, int my, int k) {
+  return k < 4 && (2 * mx + (k & 1) >= g.wb || 2 * my + (k >> 1) >= g.hb);
+}
+
+// cv2's IMWRITE_JPEG_QUALITY clamp to [0, 100], then libjpeg's jpeg_quality_scaling maps 0 to 1
+__host__ __device__ inline int clamp_quality(int q) { return q <= 0 ? 1 : q > 100 ? 100 : q; }
+
+// ------------------------------------------------------------------ colour conversion and sampling (jccolor.c, jcsample.c)
+__host__ __device__ inline int ycc_y(int b, int g, int r) { return (19595 * r + 38470 * g + 7471 * b + 32768) >> 16; }
+__host__ __device__ inline int ycc_cb(int b, int g, int r) { return (-11059 * r - 21709 * g + 32768 * b + (128 << 16) + 32767) >> 16; }
+__host__ __device__ inline int ycc_cr(int b, int g, int r) { return (32768 * r - 27439 * g - 5329 * b + (128 << 16) + 32767) >> 16; }
+
+__host__ __device__ inline int ld8(const uint8_t* p) {
+#ifdef __CUDA_ARCH__
+  return __ldg(p);
+#else
+  return *p;
+#endif
+}
+
+// Sample (r, c) of block k of MCU (mx, my): luma (k < 4) or Cb (k == 4) / Cr (k == 5) after 2x2 subsampling.
+__host__ __device__ inline int block_sample(const uint8_t* img, long long pitch, const Geom& g, int mx, int my, int k, int r,
+                                            int c) {
+  if (k < 4) {
+    int x = (2 * mx + (k & 1)) * 8 + c, y = (2 * my + (k >> 1)) * 8 + r;
+    x = x < g.W ? x : g.W - 1;
+    y = y < g.H ? y : g.H - 1;
+    const uint8_t* p = img + y * pitch + 3ll * x;
+    return ycc_y(ld8(p), ld8(p + 1), ld8(p + 2));
+  }
+  const int last = (g.H + 1) / 2 - 1;                    // chroma rows past ceil(H/2) repeat the last one
+  int cy = my * 8 + r;
+  cy = cy < last ? cy : last;
+  const int cx = mx * 8 + c;
+  const int x0 = 2 * cx < g.W ? 2 * cx : g.W - 1, x1 = 2 * cx + 1 < g.W ? 2 * cx + 1 : g.W - 1;
+  const int y0 = 2 * cy < g.H ? 2 * cy : g.H - 1, y1 = 2 * cy + 1 < g.H ? 2 * cy + 1 : g.H - 1;
+  int s = 0;
+  const int xs[2] = {x0, x1}, ys[2] = {y0, y1};
+  for (int i = 0; i < 2; ++i)
+    for (int j = 0; j < 2; ++j) {
+      const uint8_t* p = img + ys[i] * pitch + 3ll * xs[j];
+      const int b = ld8(p), gg = ld8(p + 1), rr = ld8(p + 2);
+      s += k == 4 ? ycc_cb(b, gg, rr) : ycc_cr(b, gg, rr);
+    }
+  return (s + 1 + (c & 1)) >> 2;                         // h2v2_downsample's alternating bias 1, 2
+}
+
+// The 64 samples of a block, level-shifted (sample - 128), natural order.
+__host__ __device__ inline void load_block(const uint8_t* img, long long pitch, const Geom& g, int mx, int my, int k, int* d) {
+  for (int r = 0; r < 8; ++r)
+    for (int c = 0; c < 8; ++c) d[r * 8 + c] = block_sample(img, pitch, g, mx, my, k, r, c) - 128;
+}
+
+// ------------------------------------------------------------------ forward DCT (jfdctint.c, islow) and quantisation
+__host__ __device__ inline int descale(int x, int n) { return (x + (1 << (n - 1))) >> n; }
+
+template <int PASS>
+__host__ __device__ inline void fdct_line(int* p, int step) {
+  constexpr int CB = 13, P1 = 2, SH = PASS == 0 ? CB - P1 : CB + P1;
+  const int t0 = p[0] + p[7 * step], t7 = p[0] - p[7 * step];
+  const int t1 = p[step] + p[6 * step], t6 = p[step] - p[6 * step];
+  const int t2 = p[2 * step] + p[5 * step], t5 = p[2 * step] - p[5 * step];
+  const int t3 = p[3 * step] + p[4 * step], t4 = p[3 * step] - p[4 * step];
+  const int t10 = t0 + t3, t13 = t0 - t3, t11 = t1 + t2, t12 = t1 - t2;
+  if (PASS == 0) {
+    p[0] = (t10 + t11) * (1 << P1);
+    p[4 * step] = (t10 - t11) * (1 << P1);
+  } else {
+    p[0] = descale(t10 + t11, P1);
+    p[4 * step] = descale(t10 - t11, P1);
+  }
+  int z1 = (t12 + t13) * 4433;
+  p[2 * step] = descale(z1 + t13 * 6270, SH);
+  p[6 * step] = descale(z1 - t12 * 15137, SH);
+  z1 = t4 + t7;
+  int z2 = t5 + t6, z3 = t4 + t6, z4 = t5 + t7;
+  const int z5 = (z3 + z4) * 9633;
+  const int a4 = t4 * 2446, a5 = t5 * 16819, a6 = t6 * 25172, a7 = t7 * 12299;
+  z1 *= -7373; z2 *= -20995; z3 *= -16069; z4 *= -3196;
+  z3 += z5; z4 += z5;
+  p[7 * step] = descale(a4 + z1 + z3, SH);
+  p[5 * step] = descale(a5 + z2 + z4, SH);
+  p[3 * step] = descale(a6 + z2 + z3, SH);
+  p[step] = descale(a7 + z1 + z4, SH);
+}
+
+// In place on 64 level-shifted samples (natural order); the result is the DCT scaled by 8.
+__host__ __device__ inline void fdct_islow(int* d) {
+  for (int r = 0; r < 8; ++r) fdct_line<0>(d + 8 * r, 1);
+  for (int c = 0; c < 8; ++c) fdct_line<1>(d + c, 8);
+}
+
+// In place, natural order: sign(c) * ((|c| + d/2) / d) with d = 8 * Q[k]
+__host__ __device__ inline void quantise(int* d, const uint16_t* qdiv) {
+  for (int k = 0; k < 64; ++k) {
+    const int q = qdiv[k], v = d[k];
+    const int a = ((v < 0 ? -v : v) + (q >> 1)) / q;
+    d[k] = v < 0 ? -a : a;
+  }
+}
+
+// ------------------------------------------------------------------ Huffman coding of one block
+__host__ __device__ inline int nbits(int a) {   // size category of |v| = a
+#ifdef __CUDA_ARCH__
+  return 32 - __clz(a);
+#else
+  return a ? 32 - __builtin_clz((unsigned)a) : 0;
+#endif
+}
+
+template <class Sink>
+__host__ __device__ inline void put_sym(Sink& s, uint32_t e) { s.put(e & 0xffffu, (int)(e >> 16)); }
+
+template <class Sink>
+__host__ __device__ inline void emit_dc(int diff, const uint32_t* dc, Sink& s) {
+  const int n = nbits(diff < 0 ? -diff : diff);
+  put_sym(s, dc[n]);
+  if (n) s.put((uint32_t)(diff < 0 ? diff - 1 : diff) & ((1u << n) - 1u), n);
+}
+
+// coefficient accessors for emit_ac: quantised natural-order ints read through the zigzag table, or stored zigzag int16
+struct ZigzagOf {
+  const int* d;
+  const uint8_t* zz;
+  __host__ __device__ int operator()(int j) const { return d[zz[j]]; }
+};
+struct Zigzag16 {
+  const int16_t* c;
+  __host__ __device__ int operator()(int j) const {
+#ifdef __CUDA_ARCH__
+    return __ldg(c + j);
+#else
+    return c[j];
+#endif
+  }
+};
+
+// get(i) = zigzag coefficient i (1..63)
+template <class Get, class Sink>
+__host__ __device__ inline void emit_ac(const Get& get, const uint32_t* ac, Sink& s) {
+  int run = 0;
+  for (int i = 1; i < 64; ++i) {
+    const int v = get(i);
+    if (v == 0) { ++run; continue; }
+    for (; run > 15; run -= 16) put_sym(s, ac[0xf0]);     // ZRL
+    const int n = nbits(v < 0 ? -v : v);
+    put_sym(s, ac[(run << 4) | n]);
+    s.put((uint32_t)(v < 0 ? v - 1 : v) & ((1u << n) - 1u), n);
+    run = 0;
+  }
+  if (run) put_sym(s, ac[0x00]);                          // EOB
+}
+
+struct BitCount {
+  unsigned n = 0;
+  __host__ __device__ void put(uint32_t, int len) { n += (unsigned)len; }
+};
+
+// MSB-first bit writer into 32-bit words whose bytes sit in stream order in memory.  Writers of neighbouring blocks
+// share the words at their boundaries, so the device form ORs atomically into a zeroed buffer.
+struct BitWriter {
+  uint32_t* words;
+  long long w;        // word the next full 32 bits go to
+  uint64_t acc = 0;
+  int n;              // bits pending in acc (the first word starts with `start % 32` zero bits)
+  __host__ __device__ BitWriter(uint32_t* base, unsigned long long start) : words(base), w((long long)(start >> 5)), n((int)(start & 31)) {}
+  __host__ __device__ static void or_word(uint32_t* p, uint32_t v) {
+#ifdef __CUDA_ARCH__
+    atomicOr(p, __byte_perm(v, 0, 0x0123));
+#else
+    *p |= __builtin_bswap32(v);
+#endif
+  }
+  __host__ __device__ void put(uint32_t code, int len) {   // len <= 16
+    acc = (acc << len) | code;
+    n += len;
+    if (n >= 32) {
+      n -= 32;
+      or_word(words + w++, (uint32_t)(acc >> n));
+    }
+  }
+  __host__ __device__ void flush() {
+    if (n > 0) or_word(words + w, (uint32_t)(acc << (32 - n)));
+  }
+};
+
+// Stream bytes with a 0x00 after every 0xFF (the entropy-coded segment's byte stuffing).
+__host__ __device__ inline int count_ff(const uint8_t* p, int n) {
+  int k = 0;
+  for (int i = 0; i < n; ++i) k += p[i] == 0xff;
+  return k;
+}
+__host__ __device__ inline int stuff_copy(const uint8_t* p, int n, uint8_t* out) {
+  int o = 0;
+  for (int i = 0; i < n; ++i) {
+    out[o++] = p[i];
+    if (p[i] == 0xff) out[o++] = 0;
+  }
+  return o;
+}
+
+// Worst-case stream size: header, every block at its longest code, all of it doubled by stuffing, pad, EOI.
+__host__ __device__ inline unsigned long long entropy_bound_bits(int W, int H) {
+  return (unsigned long long)blocks_per_image(geom(W, H)) * kMaxBlockBits + 7;
+}
+__host__ __device__ inline unsigned long long encode_bound(int W, int H) {
+  return kHeaderBytes + 2 * (entropy_bound_bits(W, H) / 8) + 2;
+}
+
+// ------------------------------------------------------------------ host: tables and header (jcparam.c, Annex K)
+namespace annex_k {
+static const uint8_t kLumaQ[64] = {16, 11, 10, 16, 24, 40, 51, 61, 12, 12, 14, 19, 26, 58, 60, 55, 14, 13, 16, 24, 40, 57,
+                                   69, 56, 14, 17, 22, 29, 51, 87, 80, 62, 18, 22, 37, 56, 68, 109, 103, 77, 24, 35, 55, 64,
+                                   81, 104, 113, 92, 49, 64, 78, 87, 103, 121, 120, 101, 72, 92, 95, 98, 112, 100, 103, 99};
+static const uint8_t kChromaQ[64] = {17, 18, 24, 47, 99, 99, 99, 99, 18, 21, 26, 66, 99, 99, 99, 99, 24, 26, 56, 99, 99, 99,
+                                     99, 99, 47, 66, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99,
+                                     99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99};
+static const uint8_t kZigzag[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
+                                    41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
+                                    30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
+// BITS (codes per length 1..16) and HUFFVAL of K.3 (DC) and K.5 (AC), luma then chroma
+static const uint8_t kDcBits[2][16] = {{0, 1, 5, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0}, {0, 3, 1, 1, 1, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0}};
+static const uint8_t kDcVals[12] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11};
+static const uint8_t kAcBits[2][16] = {{0, 2, 1, 3, 3, 2, 4, 3, 5, 5, 4, 4, 0, 0, 1, 0x7d}, {0, 2, 1, 2, 4, 4, 3, 4, 7, 5, 4, 4, 0, 1, 2, 0x77}};
+static const uint8_t kAcVals[2][162] = {
+    {0x01, 0x02, 0x03, 0x00, 0x04, 0x11, 0x05, 0x12, 0x21, 0x31, 0x41, 0x06, 0x13, 0x51, 0x61, 0x07, 0x22, 0x71, 0x14,
+     0x32, 0x81, 0x91, 0xa1, 0x08, 0x23, 0x42, 0xb1, 0xc1, 0x15, 0x52, 0xd1, 0xf0, 0x24, 0x33, 0x62, 0x72, 0x82, 0x09,
+     0x0a, 0x16, 0x17, 0x18, 0x19, 0x1a, 0x25, 0x26, 0x27, 0x28, 0x29, 0x2a, 0x34, 0x35, 0x36, 0x37, 0x38, 0x39, 0x3a,
+     0x43, 0x44, 0x45, 0x46, 0x47, 0x48, 0x49, 0x4a, 0x53, 0x54, 0x55, 0x56, 0x57, 0x58, 0x59, 0x5a, 0x63, 0x64, 0x65,
+     0x66, 0x67, 0x68, 0x69, 0x6a, 0x73, 0x74, 0x75, 0x76, 0x77, 0x78, 0x79, 0x7a, 0x83, 0x84, 0x85, 0x86, 0x87, 0x88,
+     0x89, 0x8a, 0x92, 0x93, 0x94, 0x95, 0x96, 0x97, 0x98, 0x99, 0x9a, 0xa2, 0xa3, 0xa4, 0xa5, 0xa6, 0xa7, 0xa8, 0xa9,
+     0xaa, 0xb2, 0xb3, 0xb4, 0xb5, 0xb6, 0xb7, 0xb8, 0xb9, 0xba, 0xc2, 0xc3, 0xc4, 0xc5, 0xc6, 0xc7, 0xc8, 0xc9, 0xca,
+     0xd2, 0xd3, 0xd4, 0xd5, 0xd6, 0xd7, 0xd8, 0xd9, 0xda, 0xe1, 0xe2, 0xe3, 0xe4, 0xe5, 0xe6, 0xe7, 0xe8, 0xe9, 0xea,
+     0xf1, 0xf2, 0xf3, 0xf4, 0xf5, 0xf6, 0xf7, 0xf8, 0xf9, 0xfa},
+    {0x00, 0x01, 0x02, 0x03, 0x11, 0x04, 0x05, 0x21, 0x31, 0x06, 0x12, 0x41, 0x51, 0x07, 0x61, 0x71, 0x13, 0x22, 0x32,
+     0x81, 0x08, 0x14, 0x42, 0x91, 0xa1, 0xb1, 0xc1, 0x09, 0x23, 0x33, 0x52, 0xf0, 0x15, 0x62, 0x72, 0xd1, 0x0a, 0x16,
+     0x24, 0x34, 0xe1, 0x25, 0xf1, 0x17, 0x18, 0x19, 0x1a, 0x26, 0x27, 0x28, 0x29, 0x2a, 0x35, 0x36, 0x37, 0x38, 0x39,
+     0x3a, 0x43, 0x44, 0x45, 0x46, 0x47, 0x48, 0x49, 0x4a, 0x53, 0x54, 0x55, 0x56, 0x57, 0x58, 0x59, 0x5a, 0x63, 0x64,
+     0x65, 0x66, 0x67, 0x68, 0x69, 0x6a, 0x73, 0x74, 0x75, 0x76, 0x77, 0x78, 0x79, 0x7a, 0x82, 0x83, 0x84, 0x85, 0x86,
+     0x87, 0x88, 0x89, 0x8a, 0x92, 0x93, 0x94, 0x95, 0x96, 0x97, 0x98, 0x99, 0x9a, 0xa2, 0xa3, 0xa4, 0xa5, 0xa6, 0xa7,
+     0xa8, 0xa9, 0xaa, 0xb2, 0xb3, 0xb4, 0xb5, 0xb6, 0xb7, 0xb8, 0xb9, 0xba, 0xc2, 0xc3, 0xc4, 0xc5, 0xc6, 0xc7, 0xc8,
+     0xc9, 0xca, 0xd2, 0xd3, 0xd4, 0xd5, 0xd6, 0xd7, 0xd8, 0xd9, 0xda, 0xe2, 0xe3, 0xe4, 0xe5, 0xe6, 0xe7, 0xe8, 0xe9,
+     0xea, 0xf2, 0xf3, 0xf4, 0xf5, 0xf6, 0xf7, 0xf8, 0xf9, 0xfa}};
+}  // namespace annex_k
+
+// jpeg_quality_scaling + jpeg_add_quant_table(force_baseline): natural-order steps of table t (0 luma, 1 chroma)
+inline void quant_steps(int quality, int t, int* q) {
+  const int qq = clamp_quality(quality), scale = qq < 50 ? 5000 / qq : 200 - 2 * qq;
+  const uint8_t* base = t ? annex_k::kChromaQ : annex_k::kLumaQ;
+  for (int k = 0; k < 64; ++k) {
+    const int v = (base[k] * scale + 50) / 100;
+    q[k] = v < 1 ? 1 : v > 255 ? 255 : v;
+  }
+}
+
+// Canonical code assignment (Annex C): (length << 16) | code per symbol
+inline void huff_codes(const uint8_t* bits, const uint8_t* vals, uint32_t* table, int n_table) {
+  for (int i = 0; i < n_table; ++i) table[i] = 0;
+  uint32_t code = 0;
+  int k = 0;
+  for (int len = 1; len <= 16; ++len) {
+    for (int i = 0; i < bits[len - 1]; ++i) table[vals[k++]] = ((uint32_t)len << 16) | code++;
+    code <<= 1;
+  }
+}
+
+inline void make_tables(int quality, Tables* t) {
+  memset(t, 0, sizeof *t);
+  for (int c = 0; c < 2; ++c) {
+    int q[64];
+    quant_steps(quality, c, q);
+    for (int k = 0; k < 64; ++k) t->qdiv[c][k] = (uint16_t)(8 * q[k]);
+    huff_codes(annex_k::kDcBits[c], annex_k::kDcVals, t->dc[c], 12);
+    huff_codes(annex_k::kAcBits[c], annex_k::kAcVals[c], t->ac[c], 256);
+  }
+  memcpy(t->zz, annex_k::kZigzag, 64);
+}
+
+// SOI, APP0 (JFIF 1.01, no units, 1x1), DQT 0 and DQT 1, SOF0 (Y 2x2 table 0, Cb/Cr 1x1 table 1),
+// DHT DC0 AC0 DC1 AC1, SOS (Y 0/0, Cb 1/1, Cr 1/1, Ss 0 Se 63 Ah/Al 0): kHeaderBytes bytes
+inline void make_header(int W, int H, int quality, uint8_t* out) {
+  uint8_t* p = out;
+  auto b = [&](int v) { *p++ = (uint8_t)v; };
+  auto w16 = [&](int v) { b(v >> 8); b(v & 255); };
+  b(0xff); b(0xd8);
+  b(0xff); b(0xe0); w16(16);
+  for (const char ch : {'J', 'F', 'I', 'F', '\0'}) b(ch);
+  b(1); b(1); b(0); w16(1); w16(1); b(0); b(0);
+  for (int t = 0; t < 2; ++t) {
+    int q[64];
+    quant_steps(quality, t, q);
+    b(0xff); b(0xdb); w16(67); b(t);
+    for (int k = 0; k < 64; ++k) b(q[annex_k::kZigzag[k]]);
+  }
+  b(0xff); b(0xc0); w16(17); b(8); w16(H); w16(W); b(3);
+  b(1); b(0x22); b(0);
+  b(2); b(0x11); b(1);
+  b(3); b(0x11); b(1);
+  for (int t = 0; t < 2; ++t) {
+    for (int cls = 0; cls < 2; ++cls) {
+      const uint8_t* bits = cls ? annex_k::kAcBits[t] : annex_k::kDcBits[t];
+      const uint8_t* vals = cls ? annex_k::kAcVals[t] : annex_k::kDcVals;
+      int n = 0;
+      for (int i = 0; i < 16; ++i) n += bits[i];
+      b(0xff); b(0xc4); w16(2 + 1 + 16 + n); b((cls << 4) | t);
+      for (int i = 0; i < 16; ++i) b(bits[i]);
+      for (int i = 0; i < n; ++i) b(vals[i]);
+    }
+  }
+  b(0xff); b(0xda); w16(12); b(3);
+  b(1); b(0x00);
+  b(2); b(0x11);
+  b(3); b(0x11);
+  b(0); b(63); b(0);
+}
+
+// ------------------------------------------------------------------ device pipeline
+struct EncArgs {
+  const uint8_t* img;            // image i at img + i * istride, rows at pitch, BGR
+  long long istride, pitch;
+  int n;
+  Geom g;
+  long long nblk;                // blocks per image
+  const Tables* tabs;
+  int16_t* coef;                 // [n * nblk][64] zigzag
+  unsigned long long* bits;      // [n * nblk] bits per block
+  unsigned long long* offs;      // [n * nblk] exclusive scan of bits (over the whole batch)
+  int* dcdiff;                   // [n * nblk]
+  uint32_t* words;               // image i's entropy bits at words + i * words_img
+  long long words_img;
+  int chunks_img;                // kChunk-byte chunks per image region
+  unsigned* ffcnt;               // [n * chunks_img] 0xFF bytes per chunk
+  unsigned* ffscan;              // exclusive scan of ffcnt (over the whole batch)
+  const uint8_t* header;         // kHeaderBytes
+  uint8_t* out;                  // compacted streams
+  unsigned long long* out_off;   // [n]
+  unsigned long long* sizes;     // [n]
+};
+
+constexpr int kBlockThreads = 128;
+constexpr int kBlockPad = 65;    // ints per thread's block in shared memory: odd stride, conflict-free
+
+__device__ inline void load_tables(Tables* s, const Tables* g) {
+  const uint32_t* src = reinterpret_cast<const uint32_t*>(g);
+  uint32_t* dst = reinterpret_cast<uint32_t*>(s);
+  for (int i = threadIdx.x; i < (int)(sizeof(Tables) / 4); i += blockDim.x) dst[i] = src[i];
+}
+
+// bits of image i's entropy-coded data, without the pad
+__device__ inline unsigned long long image_bits(const EncArgs& a, int i) {
+  const long long last = (long long)(i + 1) * a.nblk - 1;
+  return a.offs[last] + a.bits[last] - a.offs[(long long)i * a.nblk];
+}
+
+__global__ void __launch_bounds__(kBlockThreads) k_jpeg_blocks(EncArgs a) {
+  __shared__ Tables st;
+  __shared__ int sblk[kBlockThreads * kBlockPad];
+  load_tables(&st, a.tabs);
+  __syncthreads();
+  const long long b = (long long)blockIdx.x * kBlockThreads + threadIdx.x;
+  if (b >= a.nblk * a.n) return;
+  const int i = (int)(b / a.nblk);
+  const long long local = b - i * a.nblk;
+  const int m = (int)(local / 6), k = (int)(local - 6ll * m);
+  const int mx = m % a.g.mcux, my = m / a.g.mcux;
+  int16_t* out = a.coef + b * 64;
+  const int t = k < 4 ? 0 : 1;
+  if (is_dummy(a.g, mx, my, k)) {
+    uint4* o = reinterpret_cast<uint4*>(out);
+    for (int j = 0; j < 8; ++j) o[j] = make_uint4(0, 0, 0, 0);
+    a.bits[b] = st.ac[0][0] >> 16;                         // EOB only
+    return;
+  }
+  int* d = sblk + threadIdx.x * kBlockPad;
+  load_block(a.img + i * a.istride, a.pitch, a.g, mx, my, k, d);
+  fdct_islow(d);
+  quantise(d, st.qdiv[t]);
+  const uint8_t* zz = st.zz;
+  BitCount cnt;
+  emit_ac(ZigzagOf{d, zz}, st.ac[t], cnt);
+  for (int j = 0; j < 64; j += 2) {
+    const unsigned lo = (uint16_t)d[zz[j]], hi = (uint16_t)d[zz[j + 1]];
+    reinterpret_cast<unsigned*>(out)[j >> 1] = lo | (hi << 16);
+  }
+  a.bits[b] = cnt.n;
+}
+
+// quantised DC of block k of MCU m (image-local block index base): a dummy takes the DC of the block before it
+__device__ inline int resolved_dc(const EncArgs& a, long long mcu_base, int mx, int my, int k) {
+  while (k > 0 && is_dummy(a.g, mx, my, k)) --k;
+  return a.coef[(mcu_base + k) * 64];
+}
+
+__global__ void k_jpeg_dc(EncArgs a) {
+  const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= a.nblk * a.n) return;
+  const int i = (int)(b / a.nblk);
+  const long long local = b - i * a.nblk;
+  const int m = (int)(local / 6), k = (int)(local - 6ll * m);
+  const int mx = m % a.g.mcux, my = m / a.g.mcux;
+  const long long base = b - k;                           // block 0 of this MCU
+  const int dc = resolved_dc(a, base, mx, my, k);
+  int pred = 0;
+  if (k > 0 && k < 4) pred = resolved_dc(a, base, mx, my, k - 1);
+  else if (m > 0) {
+    const int pm = m - 1;
+    pred = resolved_dc(a, base - 6, pm % a.g.mcux, pm / a.g.mcux, k == 0 ? 3 : k);
+  }
+  const int diff = dc - pred;
+  a.dcdiff[b] = diff;
+  BitCount cnt;
+  emit_dc(diff, a.tabs->dc[k < 4 ? 0 : 1], cnt);
+  a.bits[b] += cnt.n;
+}
+
+// clear the words image i's bits will occupy (the pad stays inside the last one)
+__global__ void k_jpeg_zero(EncArgs a) {
+  for (int i = 0; i < a.n; ++i) {
+    const long long used = (long long)((image_bits(a, i) + 31) >> 5);
+    uint32_t* w = a.words + i * a.words_img;
+    for (long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x; j < used; j += (long long)gridDim.x * blockDim.x) w[j] = 0;
+  }
+}
+
+__global__ void __launch_bounds__(kBlockThreads) k_jpeg_pack(EncArgs a) {
+  __shared__ Tables st;
+  load_tables(&st, a.tabs);
+  __syncthreads();
+  const long long b = (long long)blockIdx.x * kBlockThreads + threadIdx.x;
+  if (b >= a.nblk * a.n) return;
+  const int i = (int)(b / a.nblk);
+  const long long local = b - i * a.nblk;
+  const int t = (int)(local % 6) < 4 ? 0 : 1;
+  const unsigned long long start = a.offs[b] - a.offs[(long long)i * a.nblk];
+  BitWriter wr(a.words + i * a.words_img, start);
+  emit_dc(a.dcdiff[b], st.dc[t], wr);
+  emit_ac(Zigzag16{a.coef + b * 64}, st.ac[t], wr);
+  if (local == a.nblk - 1) {                              // the image's last block pads its last byte with 1 bits
+    const int pad = (int)((8 - ((start + a.bits[b]) & 7)) & 7);
+    if (pad) wr.put((1u << pad) - 1u, pad);
+  }
+  wr.flush();
+}
+
+__global__ void k_jpeg_ffcount(EncArgs a) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (long long)a.n * a.chunks_img) return;
+  const int i = (int)(t / a.chunks_img), c = (int)(t - (long long)i * a.chunks_img);
+  const long long nbytes = (long long)((image_bits(a, i) + 7) >> 3), off = (long long)c * kChunk;
+  if (off >= nbytes) return;   // unused chunks keep stale counts: only differences within an image are ever read
+  const uint8_t* p = reinterpret_cast<const uint8_t*>(a.words + i * a.words_img) + off;
+  a.ffcnt[t] = (unsigned)count_ff(p, (int)(nbytes - off < kChunk ? nbytes - off : kChunk));
+}
+
+// one CTA: stream sizes and compacted offsets, then every image's header and EOI
+__global__ void k_jpeg_layout(EncArgs a) {
+  if (threadIdx.x == 0) {
+    unsigned long long off = 0;
+    for (int i = 0; i < a.n; ++i) {
+      const unsigned long long nbytes = (image_bits(a, i) + 7) >> 3;
+      const long long c0 = (long long)i * a.chunks_img, cl = c0 + (long long)((nbytes + kChunk - 1) / kChunk) - 1;
+      const unsigned ff = a.ffscan[cl] + a.ffcnt[cl] - a.ffscan[c0];
+      const unsigned long long size = kHeaderBytes + nbytes + ff + 2;
+      a.out_off[i] = off;
+      a.sizes[i] = size;
+      off += size;
+    }
+  }
+  __syncthreads();
+  for (long long j = threadIdx.x; j < (long long)a.n * kHeaderBytes; j += blockDim.x) {
+    const int i = (int)(j / kHeaderBytes), h = (int)(j - (long long)i * kHeaderBytes);
+    a.out[a.out_off[i] + h] = a.header[h];
+  }
+  for (int i = threadIdx.x; i < a.n; i += blockDim.x) {
+    uint8_t* e = a.out + a.out_off[i] + a.sizes[i] - 2;
+    e[0] = 0xff;
+    e[1] = 0xd9;
+  }
+}
+
+__global__ void k_jpeg_stuff(EncArgs a) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (long long)a.n * a.chunks_img) return;
+  const int i = (int)(t / a.chunks_img), c = (int)(t - (long long)i * a.chunks_img);
+  const long long nbytes = (long long)((image_bits(a, i) + 7) >> 3), off = (long long)c * kChunk;
+  if (off >= nbytes) return;
+  const uint8_t* p = reinterpret_cast<const uint8_t*>(a.words + i * a.words_img) + off;
+  uint8_t* o = a.out + a.out_off[i] + kHeaderBytes + off + (a.ffscan[t] - a.ffscan[(long long)i * a.chunks_img]);
+  stuff_copy(p, (int)(nbytes - off < kChunk ? nbytes - off : kChunk), o);
+}
+
+}  // namespace jpeg
+}  // namespace bevk

@@ -89,6 +89,68 @@ def jpeg_decode(jpegs, width: int, height: int, out=None, ctx: L.Context | None 
     return out
 
 
+def jpeg_encode_bound(width: int, height: int) -> int:
+    """Largest JPEG stream bevk_jpeg_encode can produce for a width x height image."""
+    n = C.c_uint64()
+    L.check(L.load().bevk_jpeg_encode_bound(int(width), int(height), C.byref(n)))
+    return n.value
+
+
+def _cuda_bgr_batch(arr):
+    """(device pointer, n, h, w, image stride, row stride) of a uint8 CUDA array [H][W][3] or [N][H][W][3] whose pixels
+    are dense (3-byte pixels, 1-byte channels); rows and images may be padded."""
+    iface = arr.__cuda_array_interface__
+    shape = tuple(iface["shape"])
+    if iface["typestr"] not in ("|u1", "<u1", "=u1"):
+        raise L.BevkError(f"CUDA array must be uint8, got typestr {iface['typestr']}")
+    if len(shape) not in (3, 4) or shape[-1] != 3:
+        raise L.BevkError(f"jpeg_encode takes uint8[H][W][3] or uint8[N][H][W][3] BGR images, got shape {shape}")
+    strides = iface.get("strides")
+    if strides is None:
+        strides = tuple(int(np.prod(shape[i + 1:])) for i in range(len(shape)))
+    if len(shape) == 3:
+        shape, strides = (1,) + shape, (0,) + tuple(strides)
+    n, h, w, _ = shape
+    if strides[3] != 1 or (w > 1 and strides[2] != 3):
+        raise L.BevkError("CUDA images must have dense BGR pixels (strides 3 and 1 along width and channels)")
+    ptr = iface["data"][0]
+    if not ptr:
+        raise L.BevkError("CUDA array has a null data pointer")
+    row = strides[1] if h > 1 else 3 * w
+    img = strides[0] if n > 1 else h * row
+    return int(ptr), n, h, w, int(img), int(row)
+
+
+def jpeg_encode(images, quality: int = 95, ctx: L.Context | None = None) -> list[bytes]:
+    """cv2.imencode('.jpg', img, [cv2.IMWRITE_JPEG_QUALITY, quality]) on the GPU, byte for byte, for one uint8[H][W][3]
+    BGR image or a batch uint8[N][H][W][3].  CUDA arrays (``__cuda_array_interface__``, e.g. the torch canvases of
+    BevEngine.run_cuda) are read in place, on torch's current stream; NumPy input is uploaded once.  Returns one
+    ``bytes`` per image -- what cv2.imwrite would write to a .jpg file."""
+    ctx = ctx or L.default_context()
+    from .sharding import _torch_current_stream
+    keep = images
+    if not hasattr(images, "__cuda_array_interface__"):
+        a = np.asarray(images)
+        if a.dtype != np.uint8 or a.ndim not in (3, 4) or a.shape[-1] != 3:
+            raise L.BevkError(f"jpeg_encode takes uint8[H][W][3] or uint8[N][H][W][3] BGR images, got {a.dtype} {a.shape}")
+        import torch
+        keep = torch.from_numpy(np.ascontiguousarray(a)).to(torch.device("cuda", ctx.device))
+    ptr, n, h, w, img_stride, row_stride = _cuda_bgr_batch(keep)
+    if n < 1:
+        return []
+    cap = n * jpeg_encode_bound(w, h)
+    out = np.empty(cap, np.uint8)          # pages are only touched where streams land
+    sizes = (C.c_uint64 * n)()
+    with ctx.on_stream(_torch_current_stream(ctx.device)):
+        L.check(ctx.lib.bevk_jpeg_encode(ctx.h, C.c_void_p(ptr), img_stride, row_stride, n, w, h, int(quality), L.vptr(out),
+                                         cap, sizes))
+    res, off = [], 0
+    for s in sizes:
+        res.append(out[off:off + s].tobytes())
+        off += s
+    return res
+
+
 def remap(src: np.ndarray, map1: np.ndarray, map2: np.ndarray | None, interpolation: int = INTER_LINEAR,
           ctx: L.Context | None = None, out: np.ndarray | None = None) -> np.ndarray:
     """cv2.remap with CV_16SC2 (+CV_16UC1) maps, BORDER_CONSTANT 0."""
@@ -235,6 +297,20 @@ class Undistorter:
         L.check(self.ctx.lib.bevk_undistort(self.ctx.h, self.slot, L.vptr(img), sw, sh, ss, ch, L.vptr(out), self.w, self.h,
                                             self.w * ch, _interp(interpolation)))
         return out
+
+    def jpeg(self, src: np.ndarray, quality: int = 95, interpolation: int = INTER_LINEAR) -> bytes:
+        """The undistorted image as the bytes cv2.imwrite(path, self(src), [IMWRITE_JPEG_QUALITY, quality]) writes to a .jpg
+        file; the image itself never leaves the GPU.  src: uint8[h][w][3] BGR."""
+        self._live()
+        img, sw, sh, ss, ch = L.image_view(src)
+        if ch != 3 or src.ndim != 3:
+            raise L.BevkError("Undistorter.jpeg takes uint8[h][w][3] BGR images")
+        if getattr(self, "_jpeg_buf", None) is None:
+            self._jpeg_buf = np.empty(jpeg_encode_bound(self.w, self.h), np.uint8)
+        size = C.c_uint64()
+        L.check(self.ctx.lib.bevk_undistort_jpeg(self.ctx.h, self.slot, L.vptr(img), sw, sh, ss, _interp(interpolation),
+                                                 int(quality), L.vptr(self._jpeg_buf), self._jpeg_buf.size, C.byref(size)))
+        return self._jpeg_buf[:size.value].tobytes()
 
 
 class BevEngine:

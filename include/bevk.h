@@ -241,6 +241,23 @@ int bevk_jpeg_decode(bevk_ctx *ctx, const uint8_t *const *jpegs, const uint64_t 
 int bevk_bev_run_jpeg(bevk_ctx *ctx, const uint8_t *const *jpegs, const uint64_t *sizes, int batch, const uint8_t *car, int flags,
                       uint8_t *out);
 
+/* ---- JPEG encode on the device ------------------------------------------------------------------------------------
+ * Replaces cv2.imwrite(path, img, [IMWRITE_JPEG_QUALITY, q]) at the end of the path (Tools/undistort.py:72-73,
+ * surroundBEV.py:340): the streams are byte-identical to cv2's (libjpeg-turbo baseline: 4:2:0, islow DCT, Annex K
+ * Huffman tables, JFIF 1.01 header, no restart markers), and only the compressed bytes cross PCIe.
+ * bevk_jpeg_encode_bound: the largest stream a width x height image can produce (sizes the caller's buffer).          */
+int bevk_jpeg_encode_bound(int width, int height, uint64_t *bytes);
+/* n DEVICE images, 3-channel BGR, image i at d_images + i * image_stride, rows row_stride bytes apart (any pitch >= 3 *
+ * width).  quality is clamped as cv2 does (to [0, 100]; 0 acts as 1; cv2's default is 95).  The streams are written
+ * back to back into HOST memory at out, their sizes to sizes[n]; the call synchronises.  When they need more than
+ * capacity bytes the call fails with BEVK_ERR_ARG, still fills sizes[], and writes nothing to out.                    */
+int bevk_jpeg_encode(bevk_ctx *ctx, const void *d_images, int64_t image_stride, int64_t row_stride, int n, int width, int height,
+                     int quality, uint8_t *out, uint64_t capacity, uint64_t *sizes);
+/* bevk_undistort (3 channels) followed by the encoder: Tools/undistort.py:65-73 (imread'ed frame -> remap -> imwrite)
+ * without the undistorted image ever leaving the device.  Works with map and fused slots; capacity as above.          */
+int bevk_undistort_jpeg(bevk_ctx *ctx, int slot, const uint8_t *src, int sw, int sh, int64_t sstride, int interp, int quality,
+                        uint8_t *out, uint64_t capacity, uint64_t *size);
+
 /* ---- CUDA graphs over the device-pointer entry points ------------------------------------------------
  * Everything the "_device" / "_stack" / "_frames" entry points enqueue on the ctx stream between begin and end is
  * captured (stream capture) instead of executed, instantiated once, and replayed `times` times by one call --
@@ -254,7 +271,7 @@ int bevk_graph_launch(bevk_ctx *ctx, int graph_id, int times);
 int bevk_graph_destroy(bevk_ctx *ctx, int graph_id);
 /* Kernel launches issued by this ctx since creation (bench "gpu_launches"). */
 int64_t bevk_launch_count(bevk_ctx *ctx);
-/* Milliseconds spent in the last bevk_bev_run_device call's kernels, measured with
+/* Milliseconds spent in the last bevk_bev_run_device or bevk_jpeg_encode call's kernels, measured with
  * CUDA events on the ctx stream (synchronises). */
 int bevk_last_kernel_ms(bevk_ctx *ctx, float *ms);
 

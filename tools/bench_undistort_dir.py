@@ -1,7 +1,9 @@
 #!/usr/bin/env python
-"""Tools/undistort.py end to end on a directory (SURVEY 8f-3): images/s of the GPU tool (decode / encode thread pool
-around the device call) next to the reference's serial loop (Tools/undistort.py:59-77: cv2.imread -> cv2.remap ->
-cv2.imwrite per file, restated in oracle/cv2_path.py terms) on the same host.  One JSON line.
+"""Tools/undistort.py end to end on a directory (SURVEY 8f-3): images/s of the GPU tool (decode thread pool around the
+device call, which undistorts and encodes the JPEG on the GPU; the pool writes the bytes) next to the reference's serial
+loop (Tools/undistort.py:59-77: cv2.imread -> cv2.remap -> cv2.imwrite per file, restated in oracle/cv2_path.py terms)
+on the same host.  ``files_byte_identical``: every file of the reference loop's sample equals the GPU tool's file byte
+for byte.  One JSON line.
 
     python tools/bench_undistort_dir.py [--files 400] [--workers 16]
 """
@@ -56,10 +58,12 @@ def main():
             cv2.imwrite(os.path.join(ref_dst, name), out, [cv2.IMWRITE_JPEG_QUALITY, 100])
         dr = time.perf_counter() - t1
         same = bool((cv2.imread(os.path.join(dst, sample[0])) == cv2.imread(os.path.join(ref_dst, sample[0]))).all())
+        identical = all(open(os.path.join(dst, n), "rb").read() == open(os.path.join(ref_dst, n), "rb").read() for n in sample)
         print(json.dumps({"tool": "Tools/undistort.py on a directory of 1280x1024 JPEGs (decode + undistort + encode, quality 100)",
                           "files": len(written), "workers": a.workers, "gpu_tool_images_per_s": len(written) / dt,
                           "reference_loop_images_per_s": len(sample) / dr, "reference_sample": len(sample),
-                          "cv2_threads": cv2.getNumThreads(), "os_cpu_count": os.cpu_count(), "outputs_identical": same}))
+                          "cv2_threads": cv2.getNumThreads(), "os_cpu_count": os.cpu_count(), "outputs_identical": same,
+                          "files_byte_identical": identical}))
     finally:
         for d in (src, dst, ref_dst):
             shutil.rmtree(d, ignore_errors=True)
