@@ -536,6 +536,8 @@ int bevk_bev_configure(bevk_ctx* c, int n_cam, int fw, int fh, int bw, int bh) {
   if (n_cam < 1 || n_cam > BEVK_MAX_CAMERAS) return fail(BEVK_ERR_ARG, "n_cam %d out of range", n_cam);
   if (fw <= 0 || fh <= 0 || bw <= 0 || bh <= 0) return fail(BEVK_ERR_ARG, "bad geometry");
   if (fw > 32767 || fh > 32767) return fail(BEVK_ERR_UNSUPPORTED, "frames larger than 32767 px");
+  // k_bev_tma passes a tile's origin to its consumers as x | y << 16: the last tile of a 65536-px row starts at 65504
+  if (bw > 65536 || bh > 65536) return fail(BEVK_ERR_UNSUPPORTED, "canvas %d x %d: wider or taller than 65536 px", bw, bh);
   if ((long long)fw * fh * 3 + 16 > 0xffffffffLL) return fail(BEVK_ERR_UNSUPPORTED, "frame too large for 32-bit offsets");
   c->n_cam = n_cam; c->FW = fw; c->FH = fh; c->BW = bw; c->BH = bh;
   c->bev_interp = BEVK_INTER_LINEAR;
@@ -724,11 +726,13 @@ int bevk_bev_finalize(bevk_ctx* c) {
   // ---- the TMA-staged kernel's plan (frames whose row pitch is a multiple of 16 bytes)
   c->tma_planned = false;
   c->tma_cfg = 0;
-  if (const char* env = getenv("BEVK_TMA_CFG")) {
-    int fs = 0, st = 0, eg = 0;
+  if (const char* env = getenv("BEVK_TMA_CFG")) {   // "FS,slots,groups" of a built configuration; anything else is an error
+    int fs = 0, st = 0, eg = 0, found = -1;
     if (sscanf(env, "%d,%d,%d", &fs, &st, &eg) == 3)
       for (int i = 0; i < kNumTmaConfigs; ++i)
-        if (kTmaConfigs[i].fs == fs && kTmaConfigs[i].stages == st && kTmaConfigs[i].eg == eg) c->tma_cfg = i;
+        if (kTmaConfigs[i].fs == fs && kTmaConfigs[i].stages == st && kTmaConfigs[i].eg == eg) found = i;
+    if (found < 0) return fail(BEVK_ERR_ARG, "BEVK_TMA_CFG=%s matches no built configuration (BEVK_TMA_CONFIGS)", env);
+    c->tma_cfg = found;
   }
   c->tma_stage_bytes = kTmaConfigs[c->tma_cfg].fs;
   c->tma_backoff_ns = 0;

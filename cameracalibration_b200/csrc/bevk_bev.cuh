@@ -102,6 +102,16 @@ __host__ __device__ __forceinline__ unsigned tile_row_word(const unsigned* acc_r
   tile_word_src(w, p, sel);
   return lane_perm(acc_row[p], acc_row[p + 1], sel);
 }
+// May a write-out use 32-bit stores to the output and 32-bit loads of the car?  Row pitch, frame-set stride, window
+// origin AND the caller's pointers must all be multiples of 4 (a canvas at buf + 1 is legal input; a misaligned word
+// store is not).  k_bev, k_bev_tma's producer and its consumers decide with this one function: the producer derives
+// D_ROWS from it, so the three must agree.  k_gain tests the same.
+template <class Params>
+__host__ __device__ __forceinline__ bool out_words_ok(const Params& P) {
+  return (P.out_pitch & 3) == 0 && (P.canvas_bytes & 3) == 0 && (P.ox & 3) == 0 &&
+         ((reinterpret_cast<uintptr_t>(P.out) | reinterpret_cast<uintptr_t>(P.car)) & 3) == 0;
+}
+
 // Interior write-out of k_bev_tma, who stores what: warp `wrp` owns tile rows wrp, wrp+8, wrp+16, wrp+24 (the rows it
 // accumulates with lanes along canvas x); lane l < 24 stores word l of each of them.
 __host__ __device__ __forceinline__ int tile_out_row32(int wrp, int i) { return wrp + 8 * i; }                 // i = 0..3
@@ -236,7 +246,7 @@ __global__ void __launch_bounds__(256, BEVK_MIN_CTAS) k_bev(BevParams P) {
     const int gy = tile.y + row, gx = tile.x + chunk * 4;
     const bool inb = (gy < P.oy1) && (gx < P.ox1);
     const size_t pix_off = (size_t)(gy - P.oy) * P.out_pitch + (size_t)(gx - P.ox) * 3;
-    const bool full = inb && (gx + 4 <= P.ox1) && (P.out_pitch % 4 == 0) && (P.canvas_bytes % 4 == 0) && (P.ox % 4 == 0);
+    const bool full = inb && (gx + 4 <= P.ox1) && out_words_ok(P);
     const int npx = inb ? min(4, P.ox1 - gx) : 0;
     unsigned c0 = 0, c1 = 0, c2 = 0;
     if (!BAL && P.car && full) {

@@ -427,7 +427,7 @@ __global__ void __launch_bounds__(TMA_THREADS, MINCTAS) k_bev_tma(const TmaParam
 #endif
       };
       const bool filtered = P.cam_lo > 0 || P.cam_hi < 8;   // BEVK_MAX_CAMERAS
-      const bool words_ok = !BAL && (P.out_pitch & 3) == 0 && (P.canvas_bytes & 3) == 0 && (P.ox & 3) == 0;   // as the consumers decide
+      const bool words_ok = !BAL && out_words_ok(P);   // as the consumers decide
       bool prev_generic = false;   // the previous unit left through the generic write-out (reads across the warps' rows)
       // Units are handed out dynamically (one atomic per unit, only this thread needs it: the consumers follow the ring):
       // unit u = tile u / groups of the cost-sorted tile list, frame-set group u % groups -- heavy tiles first, so the
@@ -517,7 +517,7 @@ __global__ void __launch_bounds__(TMA_THREADS, MINCTAS) k_bev_tma(const TmaParam
   const unsigned posx = acc_u32 + 4u * (unsigned)(wrp * ACC_WPITCH + lane);   // lanes along canvas x: line k*8+wrp is a row
   const unsigned posy = acc_u32 + 4u * (unsigned)(lane * ACC_WPITCH + wrp);   // lanes along canvas y: line k*8+wrp is a column
   const unsigned ent0 = stage0 + ENT_OFF + (unsigned)t * 16u;
-  const bool words_ok = !BAL && (P.out_pitch & 3) == 0 && (P.canvas_bytes & 3) == 0 && (P.ox & 3) == 0;
+  const bool words_ok = !BAL && out_words_ok(P);   // as the producer decided (D_ROWS)
   unsigned s = 0, ph = 0;
 #ifdef BEVK_TRACE
   unsigned tn = 0;
@@ -605,7 +605,7 @@ __global__ void __launch_bounds__(TMA_THREADS, MINCTAS) k_bev_tma(const TmaParam
     const int gy = tile.y + row, gx = tile.x + chunk * 4;
     const bool inb = (gy < P.oy1) && (gx < P.ox1);
     const size_t pix_off = (size_t)(gy - P.oy) * P.out_pitch + (size_t)(gx - P.ox) * 3;
-    const bool full = inb && (gx + 4 <= P.ox1) && (P.out_pitch % 4 == 0) && (P.canvas_bytes % 4 == 0) && (P.ox % 4 == 0);
+    const bool full = inb && (gx + 4 <= P.ox1) && out_words_ok(P);
     const int npx = inb ? min(4, P.ox1 - gx) : 0;
     unsigned c0 = 0, c1 = 0, c2 = 0;
     if (!BAL && P.car && full) {

@@ -100,6 +100,7 @@ int bevk_warp_maps(bevk_ctx *ctx, const int16_t *map1, const uint16_t *map2, int
                    const double H[9], int dw, int dh, int16_t *out1, uint16_t *out2);
 
 /* ---- the BEV engine (BevGenerator, surroundBEV.py:282-325) ----------------- */
+/* frames up to 32767 px a side, canvases up to 65536 (BEVK_ERR_UNSUPPORTED beyond) */
 int bevk_bev_configure(bevk_ctx *ctx, int n_cam, int frame_w, int frame_h, int bev_w, int bev_h);
 /* Camera.__init__ (surroundBEV.py:82-108): K, D, P = camera_mat_dst, undistorted
  * size (und_w x und_h) and H.  Builds the camera's BEV LUT on the device with the

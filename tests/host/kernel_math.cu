@@ -216,7 +216,8 @@ static int mode_balance() {
 // BALANCE sequence (V sums, offsets, balanced row spans, gather, channel sums, gains, car), without threads.
 // in.bin : int32 NC FW FH BW BH nearest balance has_car; per camera map1 int16[BH*BW*2], map2 uint16[BH*BW],
 //          mask u8[BH*BW]; NC frames u8[FH*FW*3]; car u8[BH*BW*3] if has_car.   out.bin: canvas u8[BH*BW*3]
-static int mode_bev(const char* in_path, const char* out_path, int tma_stage_bytes /* 0: round-1 gather plan */, int max_groups = 4) {
+static int mode_bev(const char* in_path, const char* out_path, int tma_stage_bytes /* 0: round-1 gather plan */, int max_groups = 4,
+                    int max_mult = 4) {
   FILE* f = fopen(in_path, "rb");
   if (!f) return 5;
   int hd[8];
@@ -281,8 +282,34 @@ static int mode_bev(const char* in_path, const char* out_path, int tma_stage_byt
       std::vector<const unsigned short*> p2(NC);
       std::vector<const uint8_t*> pm(NC);
       for (int k = 0; k < NC; ++k) { p1[k] = m1[k].data(); p2[k] = m2[k].data(); pm[k] = mk[k].data(); }
-      build_tma_plan(NC, FW, FH, BW, BH, nearest != 0, p1.data(), p2.data(), pm.data(), tma_stage_bytes, true, tp, max_groups);
+      build_tma_plan(NC, FW, FH, BW, BH, nearest != 0, p1.data(), p2.data(), pm.data(), tma_stage_bytes, true, tp, max_groups,
+                     max_mult);
     }
+    // what the plan contains, by the kinds of work k_bev_tma distinguishes (tests/test_host_bev_fuzz.py sums these)
+    long long n_fs[3] = {0, 0, 0}, n_gather = 0, n_slow = 0, n_nosat = 0, n_sat = 0, n_full = 0, n_orient[2] = {0, 0};
+    long long n_empty = 0, n_edge = 0;
+    for (const int4& tile : tp.tiles) {
+      n_empty += tile.w == 0;
+      n_edge += tile.x + TILE > BW || tile.y + TILE > BH;
+      for (int it = tile.z; it < tile.z + tile.w; ++it) {
+        const TmaItem& item = tp.items[it];
+        if (item.flags & ITEM_GATHER) {
+          ++n_gather;
+          for (int i = item.k0 * 256; i < item.k1 * 256; ++i) {
+            const uint4 e = tp.lut[(size_t)item.lut_block * (TILE * TILE) + i];
+            n_slow += (e.w & T_ACTIVE) && (e.w & T_SLOW);
+          }
+        } else {
+          ++n_fs[item.fs_bytes == tma_stage_bytes ? 0 : (item.fs_bytes == 2 * tma_stage_bytes ? 1 : 2)];
+        }
+        ++((item.flags & ITEM_NOSAT) ? n_nosat : n_sat);
+        n_full += (item.flags & ITEM_FULL) != 0;
+        ++n_orient[item.orient ? 1 : 0];
+      }
+    }
+    printf("tma kinds: fs1=%lld fs2=%lld fs4=%lld gather=%lld gather_slow=%lld nosat=%lld sat=%lld full=%lld orient0=%lld orient1=%lld "
+           "empty_tiles=%lld edge_tiles=%lld\n", n_fs[0], n_fs[1], n_fs[2], n_gather, n_slow, n_nosat, n_sat, n_full, n_orient[0],
+           n_orient[1], n_empty, n_edge);
     std::vector<uint8_t> stage((size_t)4 * tma_stage_bytes + 16, 0xEE);   // one ring slot = 4 FS
     for (const int4& tile : tp.tiles) {
       unsigned acc[ACC_WORDS];
@@ -474,8 +501,8 @@ int main(int argc, char** argv) {
   if (argc == 9 && !strcmp(argv[1], "gather"))
     return mode_gather(atoi(argv[2]), atoi(argv[3]), atoi(argv[4]), atoi(argv[5]), atoi(argv[6]), argv[7], argv[8]);
   if (argc == 4 && !strcmp(argv[1], "bev")) return mode_bev(argv[2], argv[3], 0);
-  if ((argc == 5 || argc == 6) && !strcmp(argv[1], "bevtma")) {
-    const int r = mode_bev(argv[2], argv[3], atoi(argv[4]), argc == 6 ? atoi(argv[5]) : 4);
+  if (argc >= 5 && argc <= 7 && !strcmp(argv[1], "bevtma")) {   // bevtma <in> <out> <stage bytes> [max groups [max mult]]
+    const int r = mode_bev(argv[2], argv[3], atoi(argv[4]), argc >= 6 ? atoi(argv[5]) : 4, argc == 7 ? atoi(argv[6]) : 4);
     return r ? r : (fails ? 1 : 0);
   }
   if (argc == 2 && !strcmp(argv[1], "balance")) return mode_balance();

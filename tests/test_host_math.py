@@ -198,6 +198,7 @@ def test_balance_scalar_code_on_the_host(exe, fx):
 
 
 # ------------------------------------------------------------------ the whole BEV path on the CPU
+from tests.bev_cases import blob, oracle, random_case  # noqa: E402
 from tests.helpers import NAMES, h16  # noqa: E402
 
 
@@ -343,37 +344,12 @@ def test_bev_path_on_the_host_eight_cameras(exe, tmp_path, fx):
     assert (out == want).all(), info
 
 
-def _fuzz_case(rng, case):
-    """Random geometry, maps (sometimes at the int16 extremes), masks and frames -> (input blob, cv2-based expectation)."""
-    NC = int(rng.integers(1, 4))
-    FW, FH = int(rng.integers(8, 90)), int(rng.integers(8, 70))
-    BW, BH = int(rng.integers(5, 80)), int(rng.integers(5, 75))
-    nearest = bool(case % 3 == 2)
-    blob = [np.array([NC, FW, FH, BW, BH, int(nearest), 0, 0], np.int32).tobytes()]
-    frames, maps, masks = [], [], []
-    for _ in range(NC):
-        lo, hi = (-6, 6) if case % 4 else (-40000, 40000)
-        m1 = np.stack([rng.integers(lo, FW + hi, (BH, BW)), rng.integers(lo, FH + hi, (BH, BW))], -1).clip(-32768, 32767).astype(np.int16)
-        m2 = rng.integers(0, 1024, (BH, BW)).astype(np.uint16)
-        kind = rng.integers(0, 3)
-        mask = (rng.integers(0, 2, (BH, BW)) * 255 if kind == 0 else rng.integers(0, 256, (BH, BW)) if kind == 1
-                else np.full((BH, BW), 255)).astype(np.uint8)
-        maps.append((m1, m2)); masks.append(mask)
-        frames.append(rng.integers(0, 256, (FH, FW, 3), dtype=np.uint8))
-        blob += [m1.tobytes(), m2.tobytes(), mask.tobytes()]
-    blob += [f.tobytes() for f in frames]
-    want = np.zeros((BH, BW, 3), np.uint8)
-    for f, (m1, m2), mask in zip(frames, maps, masks):
-        warped = cv2.remap(f, m1, m2, cv2.INTER_NEAREST if nearest else cv2.INTER_LINEAR)
-        want = cv2.add(want, R.apply_blend(warped, mask))
-    return b"".join(blob), want
-
-
 def _run_fuzz(exe_path, tmp_path, n_cases, env=None):
     rng = np.random.default_rng(500)
     for case in range(n_cases):
-        blob, want = _fuzz_case(rng, case)
-        (tmp_path / "fz_in.bin").write_bytes(blob)
+        c = random_case(rng, case)
+        want = oracle(c, 0)
+        (tmp_path / "fz_in.bin").write_bytes(blob(c))
         r = subprocess.run([str(exe_path), "bev", str(tmp_path / "fz_in.bin"), str(tmp_path / "fz_out.bin")], capture_output=True,
                            text=True, timeout=300, env=env)
         assert r.returncode == 0, (case, r.stderr[-2000:])
