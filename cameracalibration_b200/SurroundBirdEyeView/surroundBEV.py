@@ -307,6 +307,20 @@ class BevGenerator:
         order, or nested lists of per-frame CUDA arrays) -> CUDA array [n][BH][BW][3]; nothing crosses PCIe."""
         return self.engine.run_cuda(frames, car, self.balance, out, stream)
 
+    def jpeg(self, front, back, left, right, car=None, quality=95):
+        """cv2.imencode('.jpg', self(front, back, left, right, car), [IMWRITE_JPEG_QUALITY, quality]) -- the bytes
+        main()'s cv2.imwrite('./surround.jpg', surround) writes (reference surroundBEV.py:340) -- encoded on the GPU:
+        only the JPEG stream crosses PCIe."""
+        return self.engine.run_to_jpeg([[front, back, left, right]], quality, car, self.balance)[0]
+
+    def jpeg_batch(self, frame_sets, car=None, quality=95):
+        """frame_sets: iterable of (front, back, left, right) host tuples -> one JPEG ``bytes`` per frame-set."""
+        return self.engine.run_to_jpeg([list(fs) for fs in frame_sets], quality, car, self.balance)
+
+    def jpeg_cuda(self, frames, car=None, quality=95):
+        """Frame-sets already on the GPU (as run_cuda takes them) -> one JPEG ``bytes`` per frame-set."""
+        return self.engine.cuda_to_jpeg(frames, quality, car, self.balance)
+
 
 FRAME_WIDTH, FRAME_HEIGHT, BEV_WIDTH, BEV_HEIGHT = _geo.FW, _geo.FH, _geo.BW, _geo.BH
 CAR_WIDTH, CAR_HEIGHT, FOCAL_SCALE, SIZE_SCALE = _geo.CW, _geo.CH, _geo.FS, _geo.SS

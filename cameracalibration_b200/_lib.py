@@ -79,6 +79,9 @@ SIGNATURES = {
                                    C.POINTER(C.c_uint64)]),
     "bevk_undistort_jpeg": (C.c_int, [_p, C.c_int, _p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, _p, C.c_uint64,
                                       C.POINTER(C.c_uint64)]),
+    "bevk_bev_run_to_jpeg": (C.c_int, [_p, C.POINTER(_p), C.c_int64, C.c_int, _p, C.c_int, C.c_int, _p, C.c_uint64,
+                                       C.POINTER(C.c_uint64)]),
+    "bevk_bev_frames_to_jpeg": (C.c_int, [_p, C.POINTER(_p), C.c_int, _p, C.c_int, C.c_int, _p, C.c_uint64, C.POINTER(C.c_uint64)]),
     "bevk_graph_begin": (C.c_int, [_p]),
     "bevk_graph_end": (C.c_int, [_p, C.POINTER(C.c_int)]),
     "bevk_graph_launch": (C.c_int, [_p, C.c_int, C.c_int]),

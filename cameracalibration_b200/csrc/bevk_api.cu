@@ -200,12 +200,17 @@ struct bevk_ctx {
   // nvJPEG ingest (bevk_jpeg_decode): library handle + decoder state, created on first use
   void* jpeg_handle = nullptr; void* jpeg_state = nullptr;
   DevBuf d_jpeg_frames, d_jpeg_canvas;
-  // JPEG encoder (bevk_jpeg_encode): header and tables of the last (width, height, quality), work buffers
+  // JPEG encoder (bevk_jpeg_encode): header and tables of the last (width, height, quality), work buffers.  The
+  // compacted streams, their layout and their sizes are double-buffered (two slots), so that one batch can be encoded
+  // while the streams of the one before are still being copied out on out_stream.
   struct JpegEnc {
     int w = 0, h = 0, q = -1;
     uint8_t header[jpeg::kHeaderBytes];
-    DevBuf d_header, d_tabs, coef, bits, offs, dcdiff, words, ffcnt, ffscan, scan_tmp, out, meta;
-    std::vector<unsigned long long> sizes;
+    DevBuf d_header, d_tabs, coef, bits, offs, dcdiff, words, ffcnt, ffscan, scan_tmp, out[2], meta[2];
+    unsigned long long* h_sizes[2] = {nullptr, nullptr};   // page-locked copies of a slot's stream sizes
+    size_t h_sizes_cap[2] = {0, 0};
+    cudaStream_t out_stream = nullptr;                      // D2H of the streams
+    cudaEvent_t ev_sizes[2] = {nullptr, nullptr}, ev_out_free[2] = {nullptr, nullptr};
   } enc;
   // CUDA graphs captured from the device-pointer entry points (bevk_graph_*)
   bool capturing = false;
@@ -269,8 +274,17 @@ int bevk_ctx_destroy(bevk_ctx* c) {
                     &c->d_stack_ptrs, &c->d_jpeg_frames, &c->d_jpeg_canvas, &c->d_unit_counter})
     b->release();
   for (DevBuf* b : {&c->enc.d_header, &c->enc.d_tabs, &c->enc.coef, &c->enc.bits, &c->enc.offs, &c->enc.dcdiff, &c->enc.words,
-                    &c->enc.ffcnt, &c->enc.ffscan, &c->enc.scan_tmp, &c->enc.out, &c->enc.meta})
+                    &c->enc.ffcnt, &c->enc.ffscan, &c->enc.scan_tmp, &c->enc.out[0], &c->enc.out[1], &c->enc.meta[0],
+                    &c->enc.meta[1]})
     b->release();
+  if (c->enc.out_stream) {
+    cudaStreamSynchronize(c->enc.out_stream);
+    for (int i = 0; i < 2; ++i) {
+      cudaEventDestroy(c->enc.ev_sizes[i]); cudaEventDestroy(c->enc.ev_out_free[i]);
+      if (c->enc.h_sizes[i]) cudaFreeHost(c->enc.h_sizes[i]);
+    }
+    cudaStreamDestroy(c->enc.out_stream);
+  }
   for (auto& m : c->maps) m.d.release();
   shard_release(c);
   jpeg_release(c);
@@ -957,6 +971,10 @@ struct OutWin {
   uint8_t* peer[SHARD_MAX_RANKS] = {}; int world = 0; long long src_off = 0;
 };
 
+// run_device flag, not part of the ABI: with BALANCE, stop at the raw composed canvas and its channel sums (d_csum).  The
+// encoder's GainSrc applies the gains and the car, so k_gain does not run.  (Without BALANCE the write-out adds the car.)
+constexpr int kFlagRawBalance = 1 << 30;
+
 static int run_device(bevk_ctx* c, FrameSrc src, int batch, const void* d_car, int flags, void* d_out, int cam_lo, int cam_hi,
                       const OutWin* win = nullptr) {
   NvtxRange nvtx_render("bevk render (fused BEV kernels)");
@@ -1055,7 +1073,7 @@ static int run_device(bevk_ctx* c, FrameSrc src, int batch, const void* d_car, i
     LAUNCHED(c);
     c->last_path = 1;
   }
-  if (bal) {
+  if (bal && !(flags & kFlagRawBalance)) {
     const int gblocks = (int)std::max<long long>(1, std::min<long long>(P.canvas_bytes / (12 * 256) + 1, c->n_sm * 8 / std::max(1, std::min(batch, 64)) + 1));
     k_gain<<<dim3(gblocks, batch), 256, 0, c->stream>>>(P.out, P.canvas_bytes, (double)c->BW * (double)c->BH,
                                                         c->d_csum.as<unsigned long long>(), P.car);
@@ -1086,18 +1104,17 @@ static bool affine_table(const void* const* frames, size_t n, long long* stride)
   return true;
 }
 
-int bevk_bev_run_frames(bevk_ctx* c, const void* const* frames, int batch, const void* d_car, int flags, void* d_out) {
-  RET(use(c));
-  if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
-  if (!frames || !d_out) return fail(BEVK_ERR_ARG, "null pointer");
+// The frames of a host table of device pointers as run_device reads them: a frame stack when the table describes one
+// (no table upload at all), else the ctx's device copy of the table, uploaded only when its contents change.
+static int frames_src(bevk_ctx* c, const void* const* frames, int batch, FrameSrc* src) {
   if (batch < 1) return fail(BEVK_ERR_ARG, "batch must be >= 1");
   const size_t n = (size_t)batch * c->n_cam;
   for (size_t i = 0; i < n; ++i)
     if (!frames[i] || (reinterpret_cast<uintptr_t>(frames[i]) & 3)) return fail(BEVK_ERR_ARG, "frame %zu null or not 4-byte aligned", i);
   long long stride = 0;
-  if (c->tma_planned && affine_table(frames, n, &stride)) {   // no table upload at all
-    c->timed = true;
-    return run_device(c, stack_src(frames[0], stride), batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
+  if (c->tma_planned && affine_table(frames, n, &stride)) {
+    *src = stack_src(frames[0], stride);
+    return BEVK_OK;
   }
   if (c->user_tab.size() != n || memcmp(c->user_tab.data(), frames, n * sizeof(void*)) != 0) {
     RET(c->d_user_ptrs.ensure(n * sizeof(void*)));
@@ -1109,8 +1126,18 @@ int bevk_bev_run_frames(bevk_ctx* c, const void* const* frames, int batch, const
       return fail(BEVK_ERR_CUDA, "frame table upload: %s", cudaGetErrorString(e));
     }
   }
+  *src = table_src(c->d_user_ptrs.p);
+  return BEVK_OK;
+}
+
+int bevk_bev_run_frames(bevk_ctx* c, const void* const* frames, int batch, const void* d_car, int flags, void* d_out) {
+  RET(use(c));
+  if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
+  if (!frames || !d_out) return fail(BEVK_ERR_ARG, "null pointer");
+  FrameSrc src;
+  RET(frames_src(c, frames, batch, &src));
   c->timed = true;
-  return run_device(c, table_src(c->d_user_ptrs.p), batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
+  return run_device(c, src, batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
 }
 
 static int check_stack(bevk_ctx* c, const void* d_frames, int64_t frame_stride) {
@@ -1161,21 +1188,30 @@ int bevk_sat_sum_device(bevk_ctx* c, const void* const* parts, int n, uint64_t b
   return BEVK_OK;
 }
 
-int bevk_bev_run(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, int batch, const uint8_t* car, int flags,
-                 uint8_t* out) {
-  NvtxRange nvtx_call("bevk_bev_run (host frames -> host canvases)");
-  RET(use(c));
+// Host frames into the two halves of the ctx staging stack (d_frames), chunk by chunk on the copy stream: the state one
+// call of bevk_bev_run / bevk_bev_run_to_jpeg shares between its chunks.
+struct HostIngest {
+  size_t row = 0, fbytes = 0, fpad = 0, cbytes = 0;
+  int chunk = 0;
+  bool zero_copy = false;
+  std::vector<const uint8_t*> dev_view;   // zero-copy: device views of the page-locked frames
+};
+
+static int ingest_setup(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, int batch, const uint8_t* car, int flags,
+                        HostIngest* h) {
   if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
-  if (!srcs || !out) return fail(BEVK_ERR_ARG, "null host pointer");
+  if (!srcs) return fail(BEVK_ERR_ARG, "null host pointer");
   if (batch < 1) return fail(BEVK_ERR_ARG, "batch must be >= 1");
   const size_t row = (size_t)c->FW * 3, fbytes = row * c->FH, fpad = (fbytes + 255) & ~size_t(255);
   if (src_stride < (int64_t)row) return fail(BEVK_ERR_ARG, "src_stride %lld < row bytes", (long long)src_stride);
   const size_t cbytes = (size_t)c->BW * c->BH * 3;
+  h->row = row; h->fbytes = fbytes; h->fpad = fpad; h->cbytes = cbytes;
   // Two-deep pipeline over chunks of frame-sets: the H2D copies of chunk i+1 run on the copy
   // stream while chunk i is rendered and its canvases go back on the main stream, so the two
   // PCIe directions overlap and the kernel hides under the copies.
   int chunk = std::min(batch, 4);   // 4 frame-sets = one kernel work group; finer chunks shorten pipeline fill / drain
   if (const char* env = getenv("BEVK_CHUNK")) chunk = std::max(1, std::min(std::min(batch, 8), atoi(env)));
+  h->chunk = chunk;
   const size_t set_frames = (size_t)c->n_cam;
   RET(c->d_frames.ensure(fpad * set_frames * chunk * 2));
   RET(c->d_ptrs.ensure(sizeof(void*) * set_frames * chunk * 2));
@@ -1203,20 +1239,19 @@ int bevk_bev_run(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, in
   // or a previous call's D2H that still reads the canvases) has been ordered
   CU(cudaEventRecord(c->ev_free[0], c->stream));
   CU(cudaEventRecord(c->ev_free[1], c->stream));
-  int half = 0;
   // Page-locked host frames whose rows are 16-byte friendly are ingested by k_fetch_spans (the SMs read
   // only the sampled row spans over PCIe); anything else goes through DMA copies.
   bool zero_copy = !(flags & BEVK_FLAG_BALANCE) && (row % 16 == 0) && (src_stride % 16 == 0) && c->zero_copy_ok;
-  std::vector<const uint8_t*> dev_view((size_t)batch * c->n_cam, nullptr);
+  h->dev_view.assign((size_t)batch * c->n_cam, nullptr);
   if (zero_copy) {
-    for (size_t i = 0; i < dev_view.size() && zero_copy; ++i) {
+    for (size_t i = 0; i < h->dev_view.size() && zero_copy; ++i) {
       cudaPointerAttributes at{};
       if (!srcs[i] || cudaPointerGetAttributes(&at, srcs[i]) != cudaSuccess || at.type != cudaMemoryTypeHost || !at.devicePointer ||
           (reinterpret_cast<uintptr_t>(at.devicePointer) & 15)) {
         zero_copy = false;
         cudaGetLastError();   // a pageable pointer makes cudaPointerGetAttributes fail on old drivers: not an error here
       } else {
-        dev_view[i] = static_cast<const uint8_t*>(at.devicePointer);
+        h->dev_view[i] = static_cast<const uint8_t*>(at.devicePointer);
       }
     }
   }
@@ -1224,59 +1259,81 @@ int bevk_bev_run(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, in
     RET(c->d_hptrs.ensure(sizeof(void*) * set_frames * chunk * 2));
     if (!c->h_hptrs) CU(cudaHostAlloc(reinterpret_cast<void**>(&c->h_hptrs), sizeof(void*) * BEVK_MAX_CAMERAS * 8 * 2, cudaHostAllocDefault));
   }
+  h->zero_copy = zero_copy;
   c->last_h2d_bytes = 0;
-  for (int b0 = 0; b0 < batch; b0 += chunk, half ^= 1) {
-    const int nb = std::min(chunk, batch - b0);
-    uint8_t* dframes = c->d_frames.as<uint8_t>() + (size_t)half * chunk * set_frames * fpad;
-    std::unique_ptr<NvtxRange> nvtx_ingest(new NvtxRange("bevk ingest (H2D / zero-copy spans)"));
-    CU(cudaStreamWaitEvent(c->copy_stream, c->ev_free[half], 0));   // this half's previous chunk has been rendered
-    if (zero_copy) {
-      const uint8_t** hp = c->h_hptrs + (size_t)half * chunk * set_frames;
-      // the pinned pointer staging area of this half was consumed by the copy two chunks ago (ordered by ev_free + stream order)
-      CU(cudaEventSynchronize(c->ev_hp[half]));
-      for (int i = 0; i < nb * c->n_cam; ++i) hp[i] = dev_view[(size_t)b0 * c->n_cam + i];
-      const uint8_t** dhp = c->d_hptrs.as<const uint8_t*>() + (size_t)half * chunk * set_frames;
-      CU(cudaMemcpyAsync(dhp, hp, sizeof(void*) * nb * c->n_cam, cudaMemcpyHostToDevice, c->copy_stream));
-      CU(cudaEventRecord(c->ev_hp[half], c->copy_stream));
-      k_fetch_spans<<<dim3(c->FH, nb * c->n_cam), 128, 0, c->copy_stream>>>(
-          dhp, c->d_ptrs.as<uint8_t*>() + (size_t)half * chunk * set_frames, c->d_spans.as<int2>(), c->n_cam, c->FH,
-          (long long)src_stride, (int)row);
-      LAUNCHED(c);
-      c->last_h2d_bytes += (long long)c->span_fetch_bytes * nb;
-    }
-    for (int i = 0; i < nb * c->n_cam && !zero_copy; ++i) {
-      const uint8_t* s = srcs[(size_t)b0 * c->n_cam + i];
-      if (!s) return fail(BEVK_ERR_ARG, "null frame pointer %d", b0 * c->n_cam + i);
-      uint8_t* d = dframes + (size_t)i * fpad;
-      if (flags & BEVK_FLAG_BALANCE) {   // luminance_balance averages V over the whole raw frame: everything goes up
-        if ((size_t)src_stride == row) CU(cudaMemcpyAsync(d, s, fbytes, cudaMemcpyHostToDevice, c->copy_stream));
-        else CU(cudaMemcpy2DAsync(d, row, s, (size_t)src_stride, row, c->FH, cudaMemcpyHostToDevice, c->copy_stream));
-        c->last_h2d_bytes += (long long)fbytes;
-      } else {                           // only the rectangle of the frame this camera's LUT can sample
-        for (int bnd = 0; bnd < c->n_bands; ++bnd) {
-          const int* bx = c->cam_box[i % c->n_cam][bnd];
-          if (bx[1] > bx[0]) {
-            CU(cudaMemcpy2DAsync(d + (size_t)bx[0] * row + bx[2], row, s + (size_t)bx[0] * src_stride + bx[2],
-                                 (size_t)src_stride, (size_t)(bx[3] - bx[2]), (size_t)(bx[1] - bx[0]), cudaMemcpyHostToDevice,
-                                 c->copy_stream));
-            c->last_h2d_bytes += (long long)(bx[3] - bx[2]) * (bx[1] - bx[0]);
-          }
+  return BEVK_OK;
+}
+
+// Frame-sets [b0, b0 + nb) into staging half `half` on the copy stream, and the main stream made to wait for them.  *fsrc:
+// the staged frames as run_device reads them (a frame stack, so the TMA-staged kernel serves them too).
+static int ingest_chunk(bevk_ctx* c, const HostIngest& h, const uint8_t* const* srcs, int64_t src_stride, int flags, int b0, int nb,
+                        int half, FrameSrc* fsrc) {
+  const size_t set_frames = (size_t)c->n_cam, row = h.row, fbytes = h.fbytes, fpad = h.fpad;
+  const int chunk = h.chunk;
+  uint8_t* dframes = c->d_frames.as<uint8_t>() + (size_t)half * chunk * set_frames * fpad;
+  NvtxRange nvtx_ingest("bevk ingest (H2D / zero-copy spans)");
+  CU(cudaStreamWaitEvent(c->copy_stream, c->ev_free[half], 0));   // this half's previous chunk has been rendered
+  if (h.zero_copy) {
+    const uint8_t** hp = c->h_hptrs + (size_t)half * chunk * set_frames;
+    // the pinned pointer staging area of this half was consumed by the copy two chunks ago (ordered by ev_free + stream order)
+    CU(cudaEventSynchronize(c->ev_hp[half]));
+    for (int i = 0; i < nb * c->n_cam; ++i) hp[i] = h.dev_view[(size_t)b0 * c->n_cam + i];
+    const uint8_t** dhp = c->d_hptrs.as<const uint8_t*>() + (size_t)half * chunk * set_frames;
+    CU(cudaMemcpyAsync(dhp, hp, sizeof(void*) * nb * c->n_cam, cudaMemcpyHostToDevice, c->copy_stream));
+    CU(cudaEventRecord(c->ev_hp[half], c->copy_stream));
+    k_fetch_spans<<<dim3(c->FH, nb * c->n_cam), 128, 0, c->copy_stream>>>(
+        dhp, c->d_ptrs.as<uint8_t*>() + (size_t)half * chunk * set_frames, c->d_spans.as<int2>(), c->n_cam, c->FH,
+        (long long)src_stride, (int)row);
+    LAUNCHED(c);
+    c->last_h2d_bytes += (long long)c->span_fetch_bytes * nb;
+  }
+  for (int i = 0; i < nb * c->n_cam && !h.zero_copy; ++i) {
+    const uint8_t* s = srcs[(size_t)b0 * c->n_cam + i];
+    if (!s) return fail(BEVK_ERR_ARG, "null frame pointer %d", b0 * c->n_cam + i);
+    uint8_t* d = dframes + (size_t)i * fpad;
+    if (flags & BEVK_FLAG_BALANCE) {   // luminance_balance averages V over the whole raw frame: everything goes up
+      if ((size_t)src_stride == row) CU(cudaMemcpyAsync(d, s, fbytes, cudaMemcpyHostToDevice, c->copy_stream));
+      else CU(cudaMemcpy2DAsync(d, row, s, (size_t)src_stride, row, c->FH, cudaMemcpyHostToDevice, c->copy_stream));
+      c->last_h2d_bytes += (long long)fbytes;
+    } else {                           // only the rectangle of the frame this camera's LUT can sample
+      for (int bnd = 0; bnd < c->n_bands; ++bnd) {
+        const int* bx = c->cam_box[i % c->n_cam][bnd];
+        if (bx[1] > bx[0]) {
+          CU(cudaMemcpy2DAsync(d + (size_t)bx[0] * row + bx[2], row, s + (size_t)bx[0] * src_stride + bx[2],
+                               (size_t)src_stride, (size_t)(bx[3] - bx[2]), (size_t)(bx[1] - bx[0]), cudaMemcpyHostToDevice,
+                               c->copy_stream));
+          c->last_h2d_bytes += (long long)(bx[3] - bx[2]) * (bx[1] - bx[0]);
         }
       }
     }
-    CU(cudaEventRecord(c->ev_in[half], c->copy_stream));
-    nvtx_ingest.reset();
-    CU(cudaStreamWaitEvent(c->stream, c->ev_in[half], 0));
+  }
+  CU(cudaEventRecord(c->ev_in[half], c->copy_stream));
+  CU(cudaStreamWaitEvent(c->stream, c->ev_in[half], 0));
+  *fsrc = stack_src(dframes, (long long)fpad);
+  fsrc->table = c->d_ptrs.as<const uint8_t*>() + (size_t)half * chunk * set_frames;
+  return BEVK_OK;
+}
+
+int bevk_bev_run(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, int batch, const uint8_t* car, int flags,
+                 uint8_t* out) {
+  NvtxRange nvtx_call("bevk_bev_run (host frames -> host canvases)");
+  RET(use(c));
+  if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
+  if (!srcs || !out) return fail(BEVK_ERR_ARG, "null host pointer");
+  HostIngest h;
+  RET(ingest_setup(c, srcs, src_stride, batch, car, flags, &h));
+  int half = 0;
+  for (int b0 = 0; b0 < batch; b0 += h.chunk, half ^= 1) {
+    const int nb = std::min(h.chunk, batch - b0);
+    FrameSrc fsrc;
+    RET(ingest_chunk(c, h, srcs, src_stride, flags, b0, nb, half, &fsrc));
     c->timed = false;
-    uint8_t* dcanvas = c->d_canvas.as<uint8_t>() + (size_t)half * chunk * cbytes;
-    const void* dptrs = c->d_ptrs.as<const uint8_t*>() + (size_t)half * chunk * set_frames;
-    FrameSrc fsrc = stack_src(dframes, (long long)fpad);   // the staging buffers are a frame stack: TMA-staged kernel
-    fsrc.table = dptrs;
+    uint8_t* dcanvas = c->d_canvas.as<uint8_t>() + (size_t)half * h.chunk * h.cbytes;
     RET(run_device(c, fsrc, nb, car ? c->d_car.p : nullptr, flags, dcanvas, 0, BEVK_MAX_CAMERAS));
     CU(cudaEventRecord(c->ev_free[half], c->stream));               // frames of this half are free again
     {
       NvtxRange nvtx_d2h("bevk read-back (D2H canvases)");
-      CU(cudaMemcpyAsync(out + (size_t)b0 * cbytes, dcanvas, cbytes * nb, cudaMemcpyDeviceToHost, c->stream));
+      CU(cudaMemcpyAsync(out + (size_t)b0 * h.cbytes, dcanvas, h.cbytes * nb, cudaMemcpyDeviceToHost, c->stream));
     }
   }
   CU(cudaStreamSynchronize(c->stream));
@@ -1765,11 +1822,34 @@ int bevk_jpeg_encode_bound(int width, int height, uint64_t* bytes) {
   return BEVK_OK;
 }
 
-static int jpeg_encode_device(bevk_ctx* c, const void* d_images, int64_t istride, int64_t pitch, int n, int w, int h, int quality,
-                              uint8_t* out, uint64_t capacity, uint64_t* sizes) {
+// What the encoder reads: n images at img + i * istride, rows pitch bytes apart.  With csum they are raw BEV canvases
+// under BALANCE (GainSrc): colour balance from their channel sums csum[3 * i ...] and the car (NULL or a dense canvas)
+// are applied as the blocks are loaded.
+struct JpegIn {
+  const void* img = nullptr;
+  long long istride = 0, pitch = 0;
+  const unsigned long long* csum = nullptr;
+  const uint8_t* car = nullptr;
+};
+
+static int jpeg_streams(bevk_ctx* c) {
+  auto& e = c->enc;
+  if (e.out_stream) return BEVK_OK;
+  CU(cudaStreamCreateWithFlags(&e.out_stream, cudaStreamNonBlocking));
+  for (int i = 0; i < 2; ++i) {
+    CU(cudaEventCreateWithFlags(&e.ev_sizes[i], cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&e.ev_out_free[i], cudaEventDisableTiming));
+  }
+  return BEVK_OK;
+}
+
+// Enqueue the encoder over n w x h images into slot s on the ctx stream: every kernel, then the D2H of the stream sizes
+// into page-locked memory and ev_sizes[s].  jpeg_collect(s) finishes the batch.  The per-block work buffers are single:
+// batches use them one after the other in stream order.
+static int jpeg_enqueue(bevk_ctx* c, int s, const JpegIn& in, int n, int w, int h, int quality) {
   using namespace jpeg;
   auto& e = c->enc;
-  if (c->capturing) return fail(BEVK_ERR_ARG, "bevk_jpeg_encode synchronises and cannot be captured into a graph");
+  RET(jpeg_streams(c));
   const int q = clamp_quality(quality);
   if (w != e.w || h != e.h || q != e.q) {   // header + tables depend on (w, h, quality) only
     Tables t;
@@ -1796,8 +1876,14 @@ static int jpeg_encode_device(bevk_ctx* c, const void* d_images, int64_t istride
   RET(e.ffcnt.ensure((size_t)nch * 4));
   if (e.ffcnt.cap != ffcap) CU(cudaMemsetAsync(e.ffcnt.p, 0, e.ffcnt.cap, c->stream));
   RET(e.ffscan.ensure((size_t)nch * 4));
-  RET(e.out.ensure((size_t)n * encode_bound(w, h)));
-  RET(e.meta.ensure((size_t)n * 16));
+  RET(e.out[s].ensure((size_t)n * encode_bound(w, h)));
+  RET(e.meta[s].ensure((size_t)n * 16));
+  if (e.h_sizes_cap[s] < (size_t)n) {
+    if (e.h_sizes[s]) CU(cudaFreeHost(e.h_sizes[s]));      // jpeg_collect waited for its last copy
+    e.h_sizes[s] = nullptr; e.h_sizes_cap[s] = 0;
+    CU(cudaHostAlloc(reinterpret_cast<void**>(&e.h_sizes[s]), (size_t)n * 8, cudaHostAllocDefault));
+    e.h_sizes_cap[s] = (size_t)n;
+  }
   size_t tmp1 = 0, tmp2 = 0;
   CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp1, e.bits.as<unsigned long long>(), e.offs.as<unsigned long long>(), (int)nb));
   CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp2, e.ffcnt.as<unsigned>(), e.ffscan.as<unsigned>(), (int)nch));
@@ -1805,14 +1891,22 @@ static int jpeg_encode_device(bevk_ctx* c, const void* d_images, int64_t istride
   RET(e.scan_tmp.ensure(tmp));
 
   EncArgs a{};
-  a.img = reinterpret_cast<const uint8_t*>(d_images); a.istride = istride; a.pitch = pitch; a.n = n; a.g = g; a.nblk = nblk;
+  a.img = reinterpret_cast<const uint8_t*>(in.img); a.istride = in.istride; a.pitch = in.pitch; a.n = n; a.g = g; a.nblk = nblk;
   a.tabs = e.d_tabs.as<Tables>(); a.coef = e.coef.as<int16_t>(); a.bits = e.bits.as<unsigned long long>();
   a.offs = e.offs.as<unsigned long long>(); a.dcdiff = e.dcdiff.as<int>(); a.words = e.words.as<uint32_t>(); a.words_img = words_img;
   a.chunks_img = chunks; a.ffcnt = e.ffcnt.as<unsigned>(); a.ffscan = e.ffscan.as<unsigned>(); a.header = e.d_header.as<uint8_t>();
-  a.out = e.out.as<uint8_t>(); a.out_off = e.meta.as<unsigned long long>(); a.sizes = e.meta.as<unsigned long long>() + n;
+  a.out = e.out[s].as<uint8_t>(); a.out_off = e.meta[s].as<unsigned long long>(); a.sizes = e.meta[s].as<unsigned long long>() + n;
+  a.csum = in.csum; a.npix = (double)w * (double)h; a.car = in.car;
   const unsigned gb = (unsigned)((nb + kBlockThreads - 1) / kBlockThreads), gc = (unsigned)((nch + 255) / 256);
+  CU(cudaStreamWaitEvent(c->stream, e.ev_out_free[s], 0));   // the slot's previous streams have been copied out
   CU(cudaEventRecord(c->ev0, c->stream));
-  k_jpeg_blocks<<<gb, kBlockThreads, 0, c->stream>>>(a);
+  if (in.csum) {
+    const size_t gsmem = (size_t)gain_images_per_cta(nblk, n) * 768;
+    CU(cudaFuncSetAttribute(k_jpeg_blocks<GainSrc>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gsmem));
+    k_jpeg_blocks<GainSrc><<<gb, kBlockThreads, gsmem, c->stream>>>(a);
+  } else {
+    k_jpeg_blocks<PlainSrc><<<gb, kBlockThreads, 0, c->stream>>>(a);
+  }
   LAUNCHED(c);
   k_jpeg_dc<<<gb, kBlockThreads, 0, c->stream>>>(a);
   LAUNCHED(c);
@@ -1830,19 +1924,133 @@ static int jpeg_encode_device(bevk_ctx* c, const void* d_images, int64_t istride
   LAUNCHED(c);
   CU(cudaEventRecord(c->ev1, c->stream));
   c->timed = true;
-  e.sizes.resize(n);
-  CU(cudaMemcpyAsync(e.sizes.data(), a.sizes, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  unsigned long long total = 0;
-  for (int i = 0; i < n; ++i) {
-    sizes[i] = e.sizes[i];
-    total += e.sizes[i];
-  }
-  if (total > capacity)
-    return fail(BEVK_ERR_ARG, "the %d JPEG streams take %llu bytes, capacity is %llu", n, total, (unsigned long long)capacity);
-  CU(cudaMemcpyAsync(out, e.out.p, total, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
+  CU(cudaMemcpyAsync(e.h_sizes[s], a.sizes, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaEventRecord(e.ev_sizes[s], c->stream));
   return BEVK_OK;
+}
+
+// Finish slot s's batch of n: wait for its sizes, store them in sizes[n], and copy streams to the host at out + *used on
+// out_stream (not synchronised).  whole: all of the batch's streams or none; otherwise the leading streams that still fit
+// in capacity, none once *full (an earlier stream did not fit).  *used grows by the bytes copied.
+static int jpeg_collect(bevk_ctx* c, int s, int n, uint8_t* out, uint64_t capacity, bool whole, uint64_t* sizes, uint64_t* used,
+                        bool* full) {
+  auto& e = c->enc;
+  CU(cudaEventSynchronize(e.ev_sizes[s]));
+  unsigned long long fit = 0, all = 0;
+  for (int i = 0; i < n; ++i) {
+    sizes[i] = e.h_sizes[s][i];
+    all += sizes[i];
+    if (!*full && *used + fit + sizes[i] <= capacity) fit += sizes[i];
+    else *full = true;
+  }
+  if (whole && fit < all) fit = 0;
+  if (fit) {
+    CU(cudaStreamWaitEvent(e.out_stream, e.ev_sizes[s], 0));
+    CU(cudaMemcpyAsync(out + *used, e.out[s].p, fit, cudaMemcpyDeviceToHost, e.out_stream));
+    CU(cudaEventRecord(e.ev_out_free[s], e.out_stream));
+  }
+  *used += fit;
+  return BEVK_OK;
+}
+
+static int capacity_error(int n, const uint64_t* sizes, uint64_t capacity) {
+  unsigned long long total = 0;
+  for (int i = 0; i < n; ++i) total += sizes[i];
+  return fail(BEVK_ERR_ARG, "the %d JPEG streams take %llu bytes, capacity is %llu", n, total, (unsigned long long)capacity);
+}
+
+static int jpeg_encode_device(bevk_ctx* c, const JpegIn& in, int n, int w, int h, int quality, uint8_t* out, uint64_t capacity,
+                              uint64_t* sizes) {
+  if (c->capturing) return fail(BEVK_ERR_ARG, "bevk_jpeg_encode synchronises and cannot be captured into a graph");
+  RET(jpeg_enqueue(c, 0, in, n, w, h, quality));
+  uint64_t used = 0;
+  bool full = false;
+  RET(jpeg_collect(c, 0, n, out, capacity, true, sizes, &used, &full));
+  CU(cudaStreamSynchronize(c->enc.out_stream));
+  return full ? capacity_error(n, sizes, capacity) : BEVK_OK;
+}
+
+// ------------------------------------------------------------------ BEV canvases straight to JPEG (surroundBEV.py:340)
+// BevGenerator.__call__ then cv2.imencode: each chunk of frame-sets is rendered into ctx scratch and encoded there, and
+// only the streams come back.  Under BALANCE the canvases stay raw and the encoder applies colour balance and the car
+// (GainSrc), so k_gain does not run and the balanced canvas is never written.  The streams of chunk i are collected
+// (wait for their sizes, D2H on the encoder's out_stream) after chunk i+1 has been enqueued, into the other slot.
+static int to_jpeg_check(bevk_ctx* c, uint8_t* out, uint64_t* sizes) {
+  if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
+  if (!out || !sizes) return fail(BEVK_ERR_ARG, "null host pointer");
+  if (c->capturing) return fail(BEVK_ERR_ARG, "the BEV-to-JPEG calls synchronise and cannot be captured into a graph");
+  uint64_t bound = 0;
+  return bevk_jpeg_encode_bound(c->BW, c->BH, &bound);
+}
+
+static JpegIn canvas_in(bevk_ctx* c, const uint8_t* canvases, int flags, const void* d_car) {
+  JpegIn in;
+  in.img = canvases; in.pitch = (long long)c->BW * 3; in.istride = in.pitch * c->BH;
+  if (flags & BEVK_FLAG_BALANCE) { in.csum = c->d_csum.as<unsigned long long>(); in.car = reinterpret_cast<const uint8_t*>(d_car); }
+  return in;
+}
+
+int bevk_bev_run_to_jpeg(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, int batch, const uint8_t* car, int flags,
+                         int quality, uint8_t* out, uint64_t capacity, uint64_t* sizes) {
+  NvtxRange nvtx_call("bevk_bev_run_to_jpeg (host frames -> host JPEG streams)");
+  RET(use(c));
+  RET(to_jpeg_check(c, out, sizes));
+  HostIngest h;
+  RET(ingest_setup(c, srcs, src_stride, batch, car, flags, &h));
+  const void* d_car = car ? c->d_car.p : nullptr;
+  uint64_t used = 0;
+  bool full = false;
+  int half = 0, prev_b0 = -1, prev_nb = 0;
+  for (int b0 = 0; b0 < batch; b0 += h.chunk, half ^= 1) {
+    const int nb = std::min(h.chunk, batch - b0);
+    FrameSrc fsrc;
+    RET(ingest_chunk(c, h, srcs, src_stride, flags, b0, nb, half, &fsrc));
+    c->timed = false;
+    uint8_t* dcanvas = c->d_canvas.as<uint8_t>() + (size_t)half * h.chunk * h.cbytes;
+    RET(run_device(c, fsrc, nb, d_car, flags | kFlagRawBalance, dcanvas, 0, BEVK_MAX_CAMERAS));
+    CU(cudaEventRecord(c->ev_free[half], c->stream));               // frames of this half are free again
+    RET(jpeg_enqueue(c, half, canvas_in(c, dcanvas, flags, d_car), nb, c->BW, c->BH, quality));
+    if (prev_b0 >= 0) RET(jpeg_collect(c, half ^ 1, prev_nb, out, capacity, false, sizes + prev_b0, &used, &full));
+    prev_b0 = b0; prev_nb = nb;
+  }
+  RET(jpeg_collect(c, half ^ 1, prev_nb, out, capacity, false, sizes + prev_b0, &used, &full));
+  CU(cudaStreamSynchronize(c->enc.out_stream));
+  return full ? capacity_error(batch, sizes, capacity) : BEVK_OK;
+}
+
+int bevk_bev_frames_to_jpeg(bevk_ctx* c, const void* const* frames, int batch, const void* d_car, int flags, int quality,
+                            uint8_t* out, uint64_t capacity, uint64_t* sizes) {
+  NvtxRange nvtx_call("bevk_bev_frames_to_jpeg (device frames -> host JPEG streams)");
+  RET(use(c));
+  RET(to_jpeg_check(c, out, sizes));
+  if (!frames) return fail(BEVK_ERR_ARG, "null pointer");
+  FrameSrc src;
+  RET(frames_src(c, frames, batch, &src));
+  // chunks of frame-sets rendered into one canvas scratch and encoded there, chunk i's streams copied out while chunk
+  // i+1 is rendered and encoded.  8 canvases (24 MB at 1000^2: they stay in the 50 MB L2) beat the whole batch at once
+  // on H100 (DESIGN.md section 4); BEVK_JPEG_CHUNK=n sets another size, 0 the whole batch.
+  int chunk = std::min(batch, 8);
+  if (const char* env = getenv("BEVK_JPEG_CHUNK")) chunk = atoi(env) > 0 ? std::min(batch, atoi(env)) : batch;
+  const size_t cbytes = (size_t)c->BW * c->BH * 3;
+  RET(c->d_canvas.ensure(cbytes * chunk));
+  uint8_t* dcanvas = c->d_canvas.as<uint8_t>();
+  uint64_t used = 0;
+  bool full = false;
+  int slot = 0, prev_b0 = -1, prev_nb = 0;
+  for (int b0 = 0; b0 < batch; b0 += chunk, slot ^= 1) {
+    const int nb = std::min(chunk, batch - b0);
+    FrameSrc part = src;
+    if (part.base) part.base += (long long)b0 * c->n_cam * part.stride;
+    else part.table = reinterpret_cast<const uint8_t* const*>(part.table) + (size_t)b0 * c->n_cam;
+    c->timed = false;
+    RET(run_device(c, part, nb, d_car, flags | kFlagRawBalance, dcanvas, 0, BEVK_MAX_CAMERAS));
+    RET(jpeg_enqueue(c, slot, canvas_in(c, dcanvas, flags, d_car), nb, c->BW, c->BH, quality));
+    if (prev_b0 >= 0) RET(jpeg_collect(c, slot ^ 1, prev_nb, out, capacity, false, sizes + prev_b0, &used, &full));
+    prev_b0 = b0; prev_nb = nb;
+  }
+  RET(jpeg_collect(c, slot ^ 1, prev_nb, out, capacity, false, sizes + prev_b0, &used, &full));
+  CU(cudaStreamSynchronize(c->enc.out_stream));
+  return full ? capacity_error(batch, sizes, capacity) : BEVK_OK;
 }
 
 int bevk_jpeg_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, int64_t row_stride, int n, int width, int height,
@@ -1855,7 +2063,9 @@ int bevk_jpeg_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, in
   if (row_stride < (int64_t)width * 3) return fail(BEVK_ERR_ARG, "row stride %lld < %d bytes", (long long)row_stride, width * 3);
   if (n > 1 && image_stride < (int64_t)(height - 1) * row_stride + width * 3)
     return fail(BEVK_ERR_ARG, "image stride %lld is smaller than one image", (long long)image_stride);
-  return jpeg_encode_device(c, d_images, image_stride, row_stride, n, width, height, quality, out, capacity, sizes);
+  JpegIn in;
+  in.img = d_images; in.istride = image_stride; in.pitch = row_stride;
+  return jpeg_encode_device(c, in, n, width, height, quality, out, capacity, sizes);
 }
 
 int bevk_undistort_jpeg(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int interp, int quality,
@@ -1868,7 +2078,9 @@ int bevk_undistort_jpeg(bevk_ctx* c, int slot, const uint8_t* src, int sw, int s
   uint64_t bound = 0;
   RET(bevk_jpeg_encode_bound(dw, dh, &bound));
   RET(undistort_to_scratch(c, slot, src, sw, sh, sstride, 3, interp));
-  return jpeg_encode_device(c, c->s_dst.p, 0, (int64_t)dw * 3, 1, dw, dh, quality, out, capacity, size);
+  JpegIn in;
+  in.img = c->s_dst.p; in.pitch = (long long)dw * 3;
+  return jpeg_encode_device(c, in, 1, dw, dh, quality, out, capacity, size);
 }
 
 // ------------------------------------------------------------------ CUDA graphs

@@ -13,7 +13,7 @@
 // Everything per block is __host__ __device__: tests/host/jpeg_enc.cu runs the same functions serially over a whole
 // image and compares the stream with live cv2.imencode.
 //
-// Device pipeline for n equal-sized images (bevk_api.cu: jpeg_encode_device):
+// Device pipeline for n equal-sized images (bevk_api.cu: jpeg_enqueue, then jpeg_collect copies the streams out):
 //   k_jpeg_blocks  one thread per 8x8 block: BGR -> samples with the edge rules, FDCT, quantise, int16 zigzag
 //                  coefficients (768 B per MCU) and the block's AC bit count
 //   k_jpeg_dc      DC differences (dummy blocks resolved), bits per block
@@ -22,10 +22,18 @@
 //   k_jpeg_pack    every block writes its codes at its offset; words shared with neighbours take atomicOr
 //   k_jpeg_ffcount 0xFF bytes per 128-byte chunk; scan (CUB); k_jpeg_layout: stream sizes, compact offsets, header + EOI
 //   k_jpeg_stuff   chunk copy with a 0x00 after every 0xFF, into the compacted output
+//
+// With GainSrc (bevk_bev_run_to_jpeg / bevk_bev_frames_to_jpeg under BALANCE) k_jpeg_blocks applies color_balance and
+// the car while it loads a block, so k_gain never runs.  Each CTA builds one gain table per image its blocks touch,
+// keyed by image, in dynamic shared memory (gain_images_per_cta; 768 B each, 2 for canvases of 128 blocks or more).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
+
+#include <type_traits>
+
+#include "bevk_kernels.cuh"   // gray_world_gains, gain_entry
 
 namespace bevk {
 namespace jpeg {
@@ -78,15 +86,46 @@ __host__ __device__ inline int ld8(const uint8_t* p) {
 #endif
 }
 
+// ------------------------------------------------------------------ pixel sources of the load stage
+// The load stage reads pixel (x, y) of the image being encoded through a source: src.bgr(x, y, b, g, r).
+// PlainSrc is the image as stored (bevk_jpeg_encode).
+struct PlainSrc {
+  const uint8_t* img;
+  long long pitch;
+  __host__ __device__ void bgr(int x, int y, int& b, int& g, int& r) const {
+    const uint8_t* p = img + y * pitch + 3ll * x;
+    b = ld8(p); g = ld8(p + 1); r = ld8(p + 2);
+  }
+};
+// GainSrc is a raw composed BEV canvas -- what k_bev<true> / k_bev_tma<true> leave with BALANCE -- as color_balance and
+// the car overlay turn it into the reference's result (surroundBEV.py:322-324): sat(tab[c][v] + car), where tab is
+// k_gain's 3 x 256 table (gray_world_gains + gain_entry of the canvas's channel sums).  The gained canvas never exists.
+struct GainSrc {
+  const uint8_t* img;
+  long long pitch;
+  const uint8_t* tab;     // [3][256]
+  const uint8_t* car;     // NULL, or uint8[H][W][3] at car_pitch
+  long long car_pitch;
+  __host__ __device__ void bgr(int x, int y, int& b, int& g, int& r) const {
+    const uint8_t* p = img + y * pitch + 3ll * x;
+    b = tab[ld8(p)]; g = tab[256 + ld8(p + 1)]; r = tab[512 + ld8(p + 2)];
+    if (car) {
+      const uint8_t* q = car + y * car_pitch + 3ll * x;
+      b += ld8(q); g += ld8(q + 1); r += ld8(q + 2);
+      b = b < 255 ? b : 255; g = g < 255 ? g : 255; r = r < 255 ? r : 255;
+    }
+  }
+};
 // Sample (r, c) of block k of MCU (mx, my): luma (k < 4) or Cb (k == 4) / Cr (k == 5) after 2x2 subsampling.
-__host__ __device__ inline int block_sample(const uint8_t* img, long long pitch, const Geom& g, int mx, int my, int k, int r,
-                                            int c) {
+template <class Src>
+__host__ __device__ inline int block_sample(const Src& src, const Geom& g, int mx, int my, int k, int r, int c) {
   if (k < 4) {
     int x = (2 * mx + (k & 1)) * 8 + c, y = (2 * my + (k >> 1)) * 8 + r;
     x = x < g.W ? x : g.W - 1;
     y = y < g.H ? y : g.H - 1;
-    const uint8_t* p = img + y * pitch + 3ll * x;
-    return ycc_y(ld8(p), ld8(p + 1), ld8(p + 2));
+    int b, gg, rr;
+    src.bgr(x, y, b, gg, rr);
+    return ycc_y(b, gg, rr);
   }
   const int last = (g.H + 1) / 2 - 1;                    // chroma rows past ceil(H/2) repeat the last one
   int cy = my * 8 + r;
@@ -98,17 +137,21 @@ __host__ __device__ inline int block_sample(const uint8_t* img, long long pitch,
   const int xs[2] = {x0, x1}, ys[2] = {y0, y1};
   for (int i = 0; i < 2; ++i)
     for (int j = 0; j < 2; ++j) {
-      const uint8_t* p = img + ys[i] * pitch + 3ll * xs[j];
-      const int b = ld8(p), gg = ld8(p + 1), rr = ld8(p + 2);
+      int b, gg, rr;
+      src.bgr(xs[j], ys[i], b, gg, rr);
       s += k == 4 ? ycc_cb(b, gg, rr) : ycc_cr(b, gg, rr);
     }
   return (s + 1 + (c & 1)) >> 2;                         // h2v2_downsample's alternating bias 1, 2
 }
 
 // The 64 samples of a block, level-shifted (sample - 128), natural order.
-__host__ __device__ inline void load_block(const uint8_t* img, long long pitch, const Geom& g, int mx, int my, int k, int* d) {
+template <class Src>
+__host__ __device__ inline void load_block(const Src& src, const Geom& g, int mx, int my, int k, int* d) {
   for (int r = 0; r < 8; ++r)
-    for (int c = 0; c < 8; ++c) d[r * 8 + c] = block_sample(img, pitch, g, mx, my, k, r, c) - 128;
+    for (int c = 0; c < 8; ++c) d[r * 8 + c] = block_sample(src, g, mx, my, k, r, c) - 128;
+}
+__host__ __device__ inline void load_block(const uint8_t* img, long long pitch, const Geom& g, int mx, int my, int k, int* d) {
+  load_block(PlainSrc{img, pitch}, g, mx, my, k, d);
 }
 
 // ------------------------------------------------------------------ forward DCT (jfdctint.c, islow) and quantisation
@@ -395,6 +438,10 @@ struct EncArgs {
   uint8_t* out;                  // compacted streams
   unsigned long long* out_off;   // [n]
   unsigned long long* sizes;     // [n]
+  // GainSrc only: channel sums of image i at csum + 3 * i, pixels per image, car (NULL or uint8[H][W][3], dense)
+  const unsigned long long* csum;
+  double npix;
+  const uint8_t* car;
 };
 
 constexpr int kBlockThreads = 128;
@@ -412,12 +459,30 @@ __device__ inline unsigned long long image_bits(const EncArgs& a, int i) {
   return a.offs[last] + a.bits[last] - a.offs[(long long)i * a.nblk];
 }
 
+// images whose blocks one CTA of k_jpeg_blocks can touch: the gain tables GainSrc needs per CTA
+__host__ __device__ inline int gain_images_per_cta(long long nblk, int n) {
+  const long long m = (kBlockThreads - 1) / nblk + 2;
+  return (int)(m < n ? m : n);
+}
+
+template <class Src>
 __global__ void __launch_bounds__(kBlockThreads) k_jpeg_blocks(EncArgs a) {
+  constexpr bool kGain = std::is_same<Src, GainSrc>::value;
   __shared__ Tables st;
   __shared__ int sblk[kBlockThreads * kBlockPad];
+  extern __shared__ uint8_t sgain[];                      // GainSrc: [images this CTA touches][3][256]
   load_tables(&st, a.tabs);
-  __syncthreads();
   const long long b = (long long)blockIdx.x * kBlockThreads + threadIdx.x;
+  const int i0 = (int)((long long)blockIdx.x * kBlockThreads / a.nblk);
+  if constexpr (kGain) {
+    const long long last = min((long long)blockIdx.x * kBlockThreads + kBlockThreads, a.nblk * a.n) - 1;
+    for (int i = i0; i <= (int)(last / a.nblk); ++i) {
+      double gain[3];
+      gray_world_gains(a.csum + 3ll * i, a.npix, gain);
+      for (int j = threadIdx.x; j < 768; j += blockDim.x) sgain[(i - i0) * 768 + j] = gain_entry(gain[j >> 8], j & 255);
+    }
+  }
+  __syncthreads();
   if (b >= a.nblk * a.n) return;
   const int i = (int)(b / a.nblk);
   const long long local = b - i * a.nblk;
@@ -432,7 +497,8 @@ __global__ void __launch_bounds__(kBlockThreads) k_jpeg_blocks(EncArgs a) {
     return;
   }
   int* d = sblk + threadIdx.x * kBlockPad;
-  load_block(a.img + i * a.istride, a.pitch, a.g, mx, my, k, d);
+  if constexpr (kGain) load_block(GainSrc{a.img + i * a.istride, a.pitch, sgain + (i - i0) * 768, a.car, 3ll * a.g.W}, a.g, mx, my, k, d);
+  else load_block(PlainSrc{a.img + i * a.istride, a.pitch}, a.g, mx, my, k, d);
   fdct_islow(d);
   quantise(d, st.qdiv[t]);
   const uint8_t* zz = st.zz;

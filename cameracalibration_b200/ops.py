@@ -379,9 +379,23 @@ class BevEngine:
         uint8[batch][BH][BW][3]."""
         if not self.finalized:
             self.finalize()
+        keep, ptrs, stride, batch = self._host_frames(frame_sets, "run()")
+        if out is None:   # a fresh array per call, as the reference returns -- page-locked and recycled (PinnedPool)
+            if getattr(self, "_pool", None) is None:
+                self._pool = L.PinnedPool()
+            out = self._pool.get((batch, self.BH, self.BW, 3))
+        else:
+            out = _out((batch, self.BH, self.BW, 3), out)
+        car, carp = self._host_car(car)
+        L.check(self.ctx.lib.bevk_bev_run(self.ctx.h, ptrs, stride, batch, carp, L.FLAG_BALANCE if balance else 0,
+                                          L.vptr(out)))
+        return out
+
+    def _host_frames(self, frame_sets, what):
+        """(arrays to keep alive, host pointer table, row stride, batch) of host frame-sets laid out as run() takes them."""
         batch = len(frame_sets)
         if batch < 1:
-            raise L.BevkError("run() needs at least one frame-set")
+            raise L.BevkError(f"{what} needs at least one frame-set")
         keep, ptrs, stride = [], (C.c_void_p * (batch * self.n_cam))(), None
         for b, fs in enumerate(frame_sets):
             if len(fs) != self.n_cam:
@@ -397,21 +411,42 @@ class BevEngine:
                         raise L.BevkError("all frames of a call must share one row stride")
                 keep.append(img)
                 ptrs[b * self.n_cam + k] = img.ctypes.data
-        if out is None:   # a fresh array per call, as the reference returns -- page-locked and recycled (PinnedPool)
-            if getattr(self, "_pool", None) is None:
-                self._pool = L.PinnedPool()
-            out = self._pool.get((batch, self.BH, self.BW, 3))
-        else:
-            out = _out((batch, self.BH, self.BW, 3), out)
-        carp = None
-        if car is not None:
-            car = np.ascontiguousarray(car, np.uint8)
-            if car.shape != (self.BH, self.BW, 3):
-                raise L.BevkError("car must be uint8[bev_h][bev_w][3]")
-            carp = L.vptr(car)
-        L.check(self.ctx.lib.bevk_bev_run(self.ctx.h, ptrs, stride, batch, carp, L.FLAG_BALANCE if balance else 0,
-                                          L.vptr(out)))
-        return out
+        return keep, ptrs, stride, batch
+
+    def _host_car(self, car):
+        """(dense car array or None, its pointer or None)."""
+        if car is None:
+            return None, None
+        car = np.ascontiguousarray(car, np.uint8)
+        if car.shape != (self.BH, self.BW, 3):
+            raise L.BevkError("car must be uint8[bev_h][bev_w][3]")
+        return car, L.vptr(car)
+
+    def _streams(self, batch):
+        """Host buffer for `batch` JPEG streams of a canvas (pages are only touched where streams land) and sizes[batch]."""
+        out = np.empty(batch * jpeg_encode_bound(self.BW, self.BH), np.uint8)
+        return out, (C.c_uint64 * batch)()
+
+    @staticmethod
+    def _split(out, sizes):
+        res, off = [], 0
+        for s in sizes:
+            res.append(out[off:off + s].tobytes())
+            off += s
+        return res
+
+    def run_to_jpeg(self, frame_sets, quality: int = 95, car: np.ndarray | None = None, balance: bool = False) -> list[bytes]:
+        """run() followed by cv2.imencode('.jpg', canvas, [IMWRITE_JPEG_QUALITY, quality]) per frame-set, with the
+        encoder on the GPU: only the JPEG streams come back over PCIe.  frame_sets as in run().  Returns one ``bytes``
+        per frame-set, byte-identical to cv2's."""
+        if not self.finalized:
+            self.finalize()
+        keep, ptrs, stride, batch = self._host_frames(frame_sets, "run_to_jpeg()")
+        car, carp = self._host_car(car)
+        out, sizes = self._streams(batch)
+        L.check(self.ctx.lib.bevk_bev_run_to_jpeg(self.ctx.h, ptrs, stride, batch, carp, L.FLAG_BALANCE if balance else 0,
+                                                  int(quality), L.vptr(out), out.size, sizes))
+        return self._split(out, sizes)
 
     def run_jpeg(self, jpeg_sets, car: np.ndarray | None = None, balance: bool = False, out: np.ndarray | None = None):
         """jpeg_sets: list (batch) of lists (n_cam) of JPEG byte strings (the files cv2.imread would open).  The streams
@@ -513,6 +548,42 @@ class BevEngine:
         stream afterwards.  The call does not synchronise.  Returns ``out``."""
         if not self.finalized:
             self.finalize()
+        ptrs = self._cuda_frames(frames)
+        batch = len(ptrs) // self.n_cam
+        if out is None:
+            import torch
+            out = torch.empty((batch, self.BH, self.BW, 3), dtype=torch.uint8, device=torch.device("cuda", self.ctx.device))
+        d_out = _cuda_ptr(out, (batch, self.BH, self.BW, 3))[0]
+        d_car = _cuda_ptr(car, (self.BH, self.BW, 3))[0] if car is not None else None
+        if stream is None:
+            from .sharding import _torch_current_stream
+            stream = _torch_current_stream(self.ctx.device)
+        table = (C.c_void_p * len(ptrs))(*ptrs)
+        with self.ctx.on_stream(stream):
+            L.check(self.ctx.lib.bevk_bev_run_frames(self.ctx.h, table, batch, C.c_void_p(d_car), L.FLAG_BALANCE if balance else 0,
+                                                     C.c_void_p(d_out)))
+        return out
+
+    def cuda_to_jpeg(self, frames, quality: int = 95, car=None, balance: bool = False) -> list[bytes]:
+        """run_cuda() followed by cv2.imencode('.jpg', canvas, [IMWRITE_JPEG_QUALITY, quality]) per frame-set: frames
+        (and car) as run_cuda takes them; the canvases stay in library scratch on the GPU and only the JPEG streams come
+        back.  Runs on torch's current stream and synchronises.  Returns one ``bytes`` per frame-set."""
+        if not self.finalized:
+            self.finalize()
+        ptrs = self._cuda_frames(frames)
+        batch = len(ptrs) // self.n_cam
+        d_car = _cuda_ptr(car, (self.BH, self.BW, 3))[0] if car is not None else None
+        out, sizes = self._streams(batch)
+        from .sharding import _torch_current_stream
+        table = (C.c_void_p * len(ptrs))(*ptrs)
+        with self.ctx.on_stream(_torch_current_stream(self.ctx.device)):
+            L.check(self.ctx.lib.bevk_bev_frames_to_jpeg(self.ctx.h, table, batch, C.c_void_p(d_car),
+                                                         L.FLAG_BALANCE if balance else 0, int(quality), L.vptr(out),
+                                                         out.size, sizes))
+        return self._split(out, sizes)
+
+    def _cuda_frames(self, frames):
+        """Device pointers (frame-set major) of the frames run_cuda takes."""
         frame_shape = (self.FH, self.FW, 3)
         if hasattr(frames, "__cuda_array_interface__"):
             base, shape = _cuda_ptr(frames, None)
@@ -528,19 +599,7 @@ class BevEngine:
                 ptrs += [_cuda_ptr(f, frame_shape)[0] for f in fs]
         if batch < 1:
             raise L.BevkError("batch must be >= 1")
-        if out is None:
-            import torch
-            out = torch.empty((batch, self.BH, self.BW, 3), dtype=torch.uint8, device=torch.device("cuda", self.ctx.device))
-        d_out = _cuda_ptr(out, (batch, self.BH, self.BW, 3))[0]
-        d_car = _cuda_ptr(car, (self.BH, self.BW, 3))[0] if car is not None else None
-        if stream is None:
-            from .sharding import _torch_current_stream
-            stream = _torch_current_stream(self.ctx.device)
-        table = (C.c_void_p * len(ptrs))(*ptrs)
-        with self.ctx.on_stream(stream):
-            L.check(self.ctx.lib.bevk_bev_run_frames(self.ctx.h, table, batch, C.c_void_p(d_car), L.FLAG_BALANCE if balance else 0,
-                                                     C.c_void_p(d_out)))
-        return out
+        return ptrs
 
     def run_device_cams(self, d_srcs_ptr: int, batch: int, cam_lo: int, cam_hi: int, d_out_ptr: int):
         if not self.finalized:

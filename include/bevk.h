@@ -259,6 +259,22 @@ int bevk_jpeg_encode(bevk_ctx *ctx, const void *d_images, int64_t image_stride, 
 int bevk_undistort_jpeg(bevk_ctx *ctx, int slot, const uint8_t *src, int sw, int sh, int64_t sstride, int interp, int quality,
                         uint8_t *out, uint64_t capacity, uint64_t *size);
 
+/* ---- BEV canvases straight to JPEG ----------------------------------------------------------------------------------
+ * BevGenerator.__call__ then cv2.imencode('.jpg', surround, [IMWRITE_JPEG_QUALITY, quality]) (surroundBEV.py:312-325,
+ * :340): each canvas is rendered into library scratch and encoded on the device, and only the streams (byte-identical to
+ * cv2's) cross PCIe.  With BEVK_FLAG_BALANCE the encoder applies colour balance and the car as it loads the raw canvas.
+ * Streams go back to back into host `out`, their sizes into sizes[batch], which is always filled for the whole batch.
+ * Streams leave chunk by chunk, so when they need more than `capacity` bytes the call fails with BEVK_ERR_ARG after
+ * `out` has received the whole streams of the leading frame-sets that fit; nothing is written at or past capacity.
+ * quality is clamped as in bevk_jpeg_encode.  Both calls synchronise and cannot be captured into a graph.
+ * bevk_bev_run_to_jpeg: `batch` HOST frame-sets laid out as in bevk_bev_run (same chunk pipeline and ingest).         */
+int bevk_bev_run_to_jpeg(bevk_ctx *ctx, const uint8_t *const *srcs, int64_t src_stride, int batch, const uint8_t *car, int flags,
+                         int quality, uint8_t *out, uint64_t capacity, uint64_t *sizes);
+/* The same for DEVICE frames given as a host table of device pointers, as in bevk_bev_run_frames (a table that describes a
+ * 16-byte friendly stack takes the TMA-staged kernel).  d_car NULL or device; work runs on the ctx stream.           */
+int bevk_bev_frames_to_jpeg(bevk_ctx *ctx, const void *const *frames, int batch, const void *d_car, int flags, int quality,
+                            uint8_t *out, uint64_t capacity, uint64_t *sizes);
+
 /* ---- CUDA graphs over the device-pointer entry points ------------------------------------------------
  * Everything the "_device" / "_stack" / "_frames" entry points enqueue on the ctx stream between begin and end is
  * captured (stream capture) instead of executed, instantiated once, and replayed `times` times by one call --
