@@ -36,7 +36,10 @@ SIGNATURES = {
     "bevk_undistorter_set": (C.c_int, [_p, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, C.c_int, C.c_int, C.c_int]),
     "bevk_undistorter_maps": (C.c_int, [_p, C.c_int, _p, _p]),
     "bevk_undistort": (C.c_int, [_p, C.c_int, _p, C.c_int, C.c_int, C.c_int64, C.c_int, _p, C.c_int, C.c_int, C.c_int64, C.c_int]),
-    "bevk_warp_perspective": (C.c_int, [_p, _p, C.c_int, C.c_int, C.c_int64, C.c_int, _dp, _p, C.c_int, C.c_int, C.c_int64, C.c_int]),
+    "bevk_undistort_stack": (C.c_int, [_p, C.c_int, _p, C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, _p, C.c_int64,
+                                       C.c_int, C.c_int, C.c_int64, C.c_int]),
+    "bevk_undistort_last_path": (C.c_int, [_p]),
+    "bevk_warp_perspective":(C.c_int, [_p, _p, C.c_int, C.c_int, C.c_int64, C.c_int, _dp, _p, C.c_int, C.c_int, C.c_int64, C.c_int]),
     "bevk_warp_maps": (C.c_int, [_p, _p, _p, C.c_int, C.c_int, _dp, C.c_int, C.c_int, _p, _p]),
     "bevk_bev_configure": (C.c_int, [_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "bevk_bev_set_camera": (C.c_int, [_p, C.c_int, _dp, _dp, _dp, C.c_int, C.c_int, _dp]),
@@ -79,7 +82,9 @@ SIGNATURES = {
                                    C.POINTER(C.c_uint64)]),
     "bevk_undistort_jpeg": (C.c_int, [_p, C.c_int, _p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, _p, C.c_uint64,
                                       C.POINTER(C.c_uint64)]),
-    "bevk_bev_run_to_jpeg": (C.c_int, [_p, C.POINTER(_p), C.c_int64, C.c_int, _p, C.c_int, C.c_int, _p, C.c_uint64,
+    "bevk_undistort_stack_jpeg": (C.c_int, [_p, C.c_int, _p, C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int, _p,
+                                            C.c_uint64, C.POINTER(C.c_uint64)]),
+    "bevk_bev_run_to_jpeg":(C.c_int, [_p, C.POINTER(_p), C.c_int64, C.c_int, _p, C.c_int, C.c_int, _p, C.c_uint64,
                                        C.POINTER(C.c_uint64)]),
     "bevk_bev_frames_to_jpeg": (C.c_int, [_p, C.POINTER(_p), C.c_int, _p, C.c_int, C.c_int, _p, C.c_uint64, C.POINTER(C.c_uint64)]),
     "bevk_graph_begin": (C.c_int, [_p]),

@@ -180,6 +180,7 @@ struct bevk_ctx {
   DevBuf d_stack_ptrs;                      // pointer table of a frame stack (BALANCE pre-passes read frames through a table)
   const void* stack_ptrs_base = nullptr; long long stack_ptrs_stride = 0, stack_ptrs_n = 0;
   int last_path = 0;                        // 1: k_bev (pointer-table gather), 2: k_bev_tma
+  int gather_path = 0;                      // stand-alone gathers: 4 = k_gather4 (word path), 1 = k_gather (byte path)
   // multi-GPU sharding (bevk_shard_*): partition, slab geometry, NCCL communicator
   struct Shard {
     bool configured = false, geometry = false;
@@ -361,24 +362,47 @@ int bevk_undistort_map(bevk_ctx* c, int model, const double K[9], const double* 
 }
 
 // ------------------------------------------------------------------ gather dispatch
+// k_gather4's word path: 32-bit tap loads need every source row to start on a 4-byte boundary (base, row pitch and, over
+// a batch, image stride), and its 32-bit stores the same of the destination (padded rows are fine).  Anything else,
+// e.g. caller memory at an odd address, takes k_gather's byte path.
+static bool gather4_ok(const GatherArgs& a, int channels, int interp, int mode) {
+  const uintptr_t al = reinterpret_cast<uintptr_t>(a.src) | reinterpret_cast<uintptr_t>(a.dst) | (uintptr_t)a.spitch |
+                       (uintptr_t)a.dpitch | (a.n > 1 ? (uintptr_t)(a.sistride | a.distride) : 0);
+  return channels == 3 && interp == BEVK_INTER_LINEAR && (a.dw % 4) == 0 && (al & 3) == 0 &&
+         a.spitch < (1ll << 31) / std::max(1, a.sh) && (mode != 0 || a.map2 != nullptr);
+}
+
+// Enqueue the gather of a.n >= 1 frames.  grid.z = frame groups of GATHER_NB, at most 65535 per launch; a single frame
+// takes k_gather4's single-frame form (NB = 1), which keeps the register count and speed of the one-frame kernel.
 template <int MODE>
-static int launch_gather(bevk_ctx* c, const GatherArgs& a, int channels, int interp) {
-  if (channels == 3 && interp == BEVK_INTER_LINEAR && (a.dw % 4) == 0 && a.dpitch == (long long)a.dw * 3 && (a.spitch % 4) == 0 &&
-      a.spitch < (1ll << 31) / std::max(1, a.sh) && (MODE != 0 || a.map2 != nullptr)) {
-    // 4 output pixels per thread, 32-bit tap loads and 12-byte stores
-    k_gather4<MODE><<<dim3((a.dw / 4 + 31) / 32, (a.dh + 7) / 8), 256, 0, c->stream>>>(a);
-    LAUNCHED(c);
-    return BEVK_OK;
-  }
-  const dim3 g = grid2d(a.dw, a.dh);
+static int launch_gather(bevk_ctx* c, const GatherArgs& a0, int channels, int interp) {
+  const bool words = gather4_ok(a0, channels, interp, MODE);
+  const int per_launch = 65535 * GATHER_NB;
+  for (int f0 = 0; f0 < a0.n; f0 += per_launch) {
+    GatherArgs a = a0;
+    a.n = std::min(per_launch, a0.n - f0);
+    a.src += (long long)f0 * a0.sistride;
+    a.dst += (long long)f0 * a0.distride;
+    const unsigned gz = (unsigned)((a.n + GATHER_NB - 1) / GATHER_NB);
+    if (words) {
+      // 4 output pixels per thread, 32-bit tap loads and 12-byte stores
+      const dim3 g4((a.dw / 4 + 31) / 32, (a.dh + 7) / 8, gz);
+      if (a.n == 1) k_gather4<MODE, 1><<<g4, 256, 0, c->stream>>>(a);
+      else k_gather4<MODE, GATHER_NB><<<g4, 256, 0, c->stream>>>(a);
+      LAUNCHED(c);
+      continue;
+    }
+    const dim3 g((a.dw + 31) / 32, (a.dh + 7) / 8, gz);
 #define GO(C, L) k_gather<MODE, C, L><<<g, 256, 0, c->stream>>>(a)
-  if (interp == BEVK_INTER_LINEAR) {
-    if (channels == 1) GO(1, 1); else if (channels == 3) GO(3, 1); else GO(4, 1);
-  } else {
-    if (channels == 1) GO(1, 0); else if (channels == 3) GO(3, 0); else GO(4, 0);
-  }
+    if (interp == BEVK_INTER_LINEAR) {
+      if (channels == 1) GO(1, 1); else if (channels == 3) GO(3, 1); else GO(4, 1);
+    } else {
+      if (channels == 1) GO(1, 0); else if (channels == 3) GO(3, 0); else GO(4, 0);
+    }
 #undef GO
-  LAUNCHED(c);
+    LAUNCHED(c);
+  }
+  c->gather_path = words ? 4 : 1;
   return BEVK_OK;
 }
 
@@ -421,6 +445,7 @@ int bevk_remap(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride,
   CU(cudaMemcpyAsync(c->s_m1.p, map1, n * 4, cudaMemcpyHostToDevice, c->stream));
   if (map2) CU(cudaMemcpyAsync(c->s_m2.p, map2, n * 2, cudaMemcpyHostToDevice, c->stream));
   GatherArgs a{};
+  a.n = 1;
   a.src = c->s_src.as<uint8_t>(); a.sw = sw; a.sh = sh; a.spitch = (long long)sw * channels;
   a.dst = c->s_dst.as<uint8_t>(); a.dw = dw; a.dh = dh; a.dpitch = (long long)dw * channels;
   a.map1 = c->s_m1.as<short2>(); a.map2 = map2 ? c->s_m2.as<unsigned short>() : nullptr;
@@ -479,6 +504,7 @@ static int undistort_to_scratch(bevk_ctx* c, int slot, const uint8_t* src, int s
   RET(upload_image(c, c->s_src, src, sw, sh, sstride, channels));
   RET(c->s_dst.ensure((size_t)dw * dh * channels));
   GatherArgs a{};
+  a.n = 1;
   a.src = c->s_src.as<uint8_t>(); a.sw = sw; a.sh = sh; a.spitch = (long long)sw * channels;
   a.dst = c->s_dst.as<uint8_t>(); a.dw = dw; a.dh = dh; a.dpitch = (long long)dw * channels;
   if (u.fused) {
@@ -503,6 +529,54 @@ int bevk_undistort(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, in
   return download_image(c, c->s_dst, dst, dw, dh, dstride, channels);
 }
 
+// ------------------------------------------------------------------ undistortion of device frame batches
+// Checks the source side of the bevk_undistort_stack calls and fills a (slot's map or model, n frames of the source);
+// the destination is left to the caller.  An image stride only matters when n > 1.
+static int stack_src_args(bevk_ctx* c, int slot, const void* d_src, int64_t sis, int sw, int sh, int64_t srs, int channels, int n,
+                          int interp, GatherArgs* a) {
+  if (slot < 0 || slot >= 8 || !c->und[slot].valid) return fail(BEVK_ERR_ARG, "undistorter slot %d not set", slot);
+  if (n < 1) return fail(BEVK_ERR_ARG, "n must be >= 1, got %d", n);
+  if (interp != BEVK_INTER_LINEAR && interp != BEVK_INTER_NEAREST) return fail(BEVK_ERR_UNSUPPORTED, "interp %d", interp);
+  RET(check_image(d_src, sw, sh, srs, channels, "src"));
+  if (n > 1 && sis < (int64_t)(sh - 1) * srs + (int64_t)sw * channels)
+    return fail(BEVK_ERR_ARG, "src image stride %lld is smaller than one image", (long long)sis);
+  const Undistorter& u = c->und[slot];
+  *a = GatherArgs{};
+  a->src = reinterpret_cast<const uint8_t*>(d_src); a->sw = sw; a->sh = sh; a->spitch = srs;
+  a->n = n; a->sistride = n > 1 ? sis : 0;
+  a->dw = u.cm.w; a->dh = u.cm.h;
+  if (u.fused) a->cm = u.cm;
+  else { a->map1 = u.map1.as<short2>(); a->map2 = u.map2.as<unsigned short>(); }
+  return BEVK_OK;
+}
+
+static int launch_undistort(bevk_ctx* c, int slot, const GatherArgs& a, int channels, int interp) {
+  return c->und[slot].fused ? launch_gather<1>(c, a, channels, interp) : launch_gather<0>(c, a, channels, interp);
+}
+
+int bevk_undistort_stack(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
+                         int channels, int n, void* d_dst, int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride,
+                         int interp) {
+  RET(use(c));
+  GatherArgs a;
+  RET(stack_src_args(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, interp, &a));
+  if (dw != a.dw || dh != a.dh)   // the caller sized dst for another map: never write past it
+    return fail(BEVK_ERR_ARG, "undistorter slot %d holds a %dx%d map, the caller expects %dx%d", slot, a.dw, a.dh, dw, dh);
+  RET(check_image(d_dst, dw, dh, dst_row_stride, channels, "dst"));
+  const int64_t dimg = (int64_t)(dh - 1) * dst_row_stride + (int64_t)dw * channels;
+  if (n > 1 && dst_image_stride < dimg)
+    return fail(BEVK_ERR_ARG, "dst image stride %lld is smaller than one image", (long long)dst_image_stride);
+  // byte ranges [first, last] of the whole batch on each side: an output that overwrites frames still to be read is refused
+  const uintptr_t s0 = reinterpret_cast<uintptr_t>(d_src), d0 = reinterpret_cast<uintptr_t>(d_dst);
+  const uintptr_t s1 = s0 + (uintptr_t)(n > 1 ? (n - 1) * src_image_stride : 0) + (uintptr_t)((int64_t)(sh - 1) * src_row_stride + (int64_t)sw * channels);
+  const uintptr_t d1 = d0 + (uintptr_t)(n > 1 ? (n - 1) * dst_image_stride : 0) + (uintptr_t)dimg;
+  if (s0 < d1 && d0 < s1) return fail(BEVK_ERR_ARG, "the destination range overlaps the source frames");
+  a.dst = reinterpret_cast<uint8_t*>(d_dst); a.dpitch = dst_row_stride; a.distride = n > 1 ? dst_image_stride : 0;
+  return launch_undistort(c, slot, a, channels, interp);
+}
+
+int bevk_undistort_last_path(bevk_ctx* c) { return c ? c->gather_path : 0; }
+
 // ------------------------------------------------------------------ K4 / K2
 int bevk_warp_perspective(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
                           const double H[9], uint8_t* dst, int dw, int dh, int64_t dstride, int interp) {
@@ -511,6 +585,7 @@ int bevk_warp_perspective(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64
   RET(check_image(dst, dw, dh, dstride, channels, "dst"));
   if (interp != BEVK_INTER_LINEAR && interp != BEVK_INTER_NEAREST) return fail(BEVK_ERR_UNSUPPORTED, "interp %d", interp);
   GatherArgs a{};
+  a.n = 1;
   RET(make_homog(H, &a.hm));
   RET(upload_image(c, c->s_src, src, sw, sh, sstride, channels));
   RET(c->s_dst.ensure((size_t)dw * dh * channels));
@@ -2081,6 +2156,46 @@ int bevk_undistort_jpeg(bevk_ctx* c, int slot, const uint8_t* src, int sw, int s
   JpegIn in;
   in.img = c->s_dst.p; in.pitch = (long long)dw * 3;
   return jpeg_encode_device(c, in, 1, dw, dh, quality, out, capacity, size);
+}
+
+// Device frames -> undistorted -> JPEG, chunk by chunk as bevk_bev_frames_to_jpeg: chunk i+1 is undistorted into the
+// scratch (stream-ordered after chunk i's encoder kernels read it) while chunk i's streams are copied out.
+int bevk_undistort_stack_jpeg(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh,
+                              int64_t src_row_stride, int n, int interp, int quality, uint8_t* out, uint64_t capacity,
+                              uint64_t* sizes) {
+  NvtxRange nvtx_call("bevk_undistort_stack_jpeg (device frames -> undistorted JPEG streams)");
+  RET(use(c));
+  if (!out || !sizes) return fail(BEVK_ERR_ARG, "null host pointer");
+  if (c->capturing) return fail(BEVK_ERR_ARG, "bevk_undistort_stack_jpeg synchronises and cannot be captured into a graph");
+  GatherArgs a;
+  RET(stack_src_args(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, 3, n, interp, &a));
+  const int dw = a.dw, dh = a.dh;
+  uint64_t bound = 0;
+  RET(bevk_jpeg_encode_bound(dw, dh, &bound));
+  // same chunking as bevk_bev_frames_to_jpeg: 8 images by default, BEVK_JPEG_CHUNK=n another size, 0 the whole batch
+  int chunk = std::min(n, 8);
+  if (const char* env = getenv("BEVK_JPEG_CHUNK")) chunk = atoi(env) > 0 ? std::min(n, atoi(env)) : n;
+  const long long ibytes = (long long)dw * dh * 3;
+  RET(c->s_dst.ensure((size_t)ibytes * chunk));
+  uint64_t used = 0;
+  bool full = false;
+  int s = 0, prev_b0 = -1, prev_nb = 0;
+  for (int b0 = 0; b0 < n; b0 += chunk, s ^= 1) {
+    const int nb = std::min(chunk, n - b0);
+    GatherArgs part = a;
+    part.src += (long long)b0 * a.sistride;
+    part.n = nb;
+    part.dst = c->s_dst.as<uint8_t>(); part.dpitch = (long long)dw * 3; part.distride = ibytes;
+    RET(launch_undistort(c, slot, part, 3, interp));
+    JpegIn in;
+    in.img = c->s_dst.p; in.pitch = (long long)dw * 3; in.istride = ibytes;
+    RET(jpeg_enqueue(c, s, in, nb, dw, dh, quality));
+    if (prev_b0 >= 0) RET(jpeg_collect(c, s ^ 1, prev_nb, out, capacity, false, sizes + prev_b0, &used, &full));
+    prev_b0 = b0; prev_nb = nb;
+  }
+  RET(jpeg_collect(c, s ^ 1, prev_nb, out, capacity, false, sizes + prev_b0, &used, &full));
+  CU(cudaStreamSynchronize(c->enc.out_stream));
+  return full ? capacity_error(n, sizes, capacity) : BEVK_OK;
 }
 
 // ------------------------------------------------------------------ CUDA graphs

@@ -3,15 +3,31 @@
 // surroundBEV.py:110-111, intrinsicCalib.py:193-195, undistort.py:66), the same with the camera model
 // evaluated in-kernel (MODE 1) and cv2.warpPerspective (MODE 2; extrinsicCalib.py:166-169).
 // Same tap machinery as the fused BEV kernel (aligned 32-bit words, funnel shift, PRMT, DP2A);
-// each thread produces 12 output bytes and stores them as three 32-bit words.  The generic
-// k_gather stays for 1/4-channel images, INTER_NEAREST and sizes that are not multiples of 4.
+// each thread produces 12 output bytes per frame and stores them as three 32-bit words.  Over a
+// batch it resolves its 4 pixels' taps once and gathers them from NB = GATHER_NB frames (see k_gather).
+// The generic k_gather stays for 1/4-channel images, INTER_NEAREST, sizes that are not multiples
+// of 4 and caller memory that is not 4-byte aligned.
 #pragma once
 #include "bevk_bev.cuh"
 #include "bevk_kernels.cuh"
 
 namespace bevk {
 
-// one output pixel: fixed-point source position -> packed B | G<<8 | R<<16
+// Tap loads of gather_px: read-only global loads.  tests/host/undistort_stack.cu substitutes a loader that records
+// every address it is asked for.
+struct Ldg {
+  __host__ __device__ __forceinline__ static unsigned w32(const uint8_t* p) { return ldg32(p); }
+  __host__ __device__ __forceinline__ static int b8(const uint8_t* p) { return ldg8(p); }
+};
+
+// one output pixel: fixed-point source position -> packed B | G<<8 | R<<16.
+// The word loads read nothing outside the taps' own rows, rounded out to whole 32-bit words, so frames need no
+// slack after them: `inside` means both taps of each row, bytes [off, off + 6) with off = 3 * sx, lie in the row.
+// The loaded words start at off_al = off & ~3 and off_al + 4, and at off_al + 8 only when off % 4 == 3.  Each of
+// them holds a byte of [off, off + 6): off itself; off_al + 4, which is in [off + 1, off + 4]; off_al + 8 = off + 5.
+// With the row's first byte on a 4-byte boundary (src, spitch 4-aligned; checked by the host), every word loaded
+// is therefore one of the row's own words.
+template <class LD = Ldg>
 __host__ __device__ __forceinline__ unsigned gather_px(const uint8_t* __restrict__ src, unsigned spitch, int sw, int sh, int sx, int sy,
                                               unsigned fx, unsigned fy) {
   const bool inside = sx >= 0 && sy >= 0 && sx + 1 < sw && sy + 1 < sh;
@@ -21,8 +37,8 @@ __host__ __device__ __forceinline__ unsigned gather_px(const uint8_t* __restrict
     const bool third = (sh8 == 24u);
     const uint8_t* q0 = src + off_al;
     const uint8_t* q1 = q0 + spitch;
-    const unsigned a0 = ldg32(q0), a1 = ldg32(q0 + 4), a2 = third ? ldg32(q0 + 8) : 0u;
-    const unsigned b0 = ldg32(q1), b1 = ldg32(q1 + 4), b2 = third ? ldg32(q1 + 8) : 0u;
+    const unsigned a0 = LD::w32(q0), a1 = LD::w32(q0 + 4), a2 = third ? LD::w32(q0 + 8) : 0u;
+    const unsigned b0 = LD::w32(q1), b1 = LD::w32(q1 + 4), b2 = third ? LD::w32(q1 + 8) : 0u;
     const unsigned w11 = fx * fy, w01 = (fx << 5) - w11, w10 = (fy << 5) - w11, w00 = 1024u - (fx << 5) - (fy << 5) + w11;
     return interp_fast(sh8, w00 | (w01 << 16), w10 | (w11 << 16), 65536u, a0, a1, a2, b0, b1, b2);
   }
@@ -32,7 +48,7 @@ __host__ __device__ __forceinline__ unsigned gather_px(const uint8_t* __restrict
     const int tx = sx + (t & 1), ty = sy + (t >> 1);
     if ((unsigned)tx < (unsigned)sw && (unsigned)ty < (unsigned)sh) {
       const uint8_t* q = src + (size_t)ty * spitch + 3 * tx;
-      p[t][0] = ldg8(q); p[t][1] = ldg8(q + 1); p[t][2] = ldg8(q + 2);
+      p[t][0] = LD::b8(q); p[t][1] = LD::b8(q + 1); p[t][2] = LD::b8(q + 2);
     } else { p[t][0] = p[t][1] = p[t][2] = 0; }
   }
   const unsigned ob = (unsigned)bilerp_q10(p[0][0], p[1][0], p[2][0], p[3][0], (int)fx, (int)fy);
@@ -41,14 +57,12 @@ __host__ __device__ __forceinline__ unsigned gather_px(const uint8_t* __restrict
   return ob | (og << 8) | (orr << 16);
 }
 
-// Requirements checked by the host: channels == 3, INTER_LINEAR, dw % 4 == 0, dense dst (pitch 3*dw),
-// source pitch % 4 == 0 with 4 bytes of readable slack after the frame (library-owned buffers).
-template <int MODE>
-__global__ void __launch_bounds__(256) k_gather4(GatherArgs a) {
-  const int x4 = (blockIdx.x * 32 + (threadIdx.x & 31)) * 4;
-  const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
-  if (x4 >= a.dw || y >= a.dh) return;
-  unsigned px[4];
+// One thread of k_gather4: output pixels x4 .. x4 + 3 of row y, frames [f0, min(n, f0 + NB)).  Host-capable
+// (tests/host/undistort_stack.cu).  Requirements checked by the host (gather4_ok in bevk_api.cu): channels == 3,
+// INTER_LINEAR, dw % 4 == 0; src, dst, both row pitches and (n > 1) both image strides multiples of 4; spitch * sh < 2^31
+// (gather_px's 32-bit offsets within a frame).
+template <int MODE, int NB, class LD = Ldg>
+__host__ __device__ __forceinline__ void gather4_frames(const GatherArgs& a, int x4, int y, int f0) {
   short mx[4], my[4];
   unsigned short fr[4];
   if (MODE == 0) {
@@ -62,30 +76,52 @@ __global__ void __launch_bounds__(256) k_gather4(GatherArgs a) {
     fr[0] = (unsigned short)(f.x & 0xffffu); fr[1] = (unsigned short)(f.x >> 16);
     fr[2] = (unsigned short)(f.y & 0xffffu); fr[3] = (unsigned short)(f.y >> 16);
   }
+  int sx[4], sy[4];
+  unsigned fx[4], fy[4], px[4];
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
-    int sx, sy;
-    unsigned fx, fy;
     if (MODE == 2) {
       int X, Y;
       warp_point(a.hm, x4 + q, y, (double)TAB, X, Y);
-      sx = sat_i16(X >> INTER_BITS); sy = sat_i16(Y >> INTER_BITS);
-      fx = X & (TAB - 1); fy = Y & (TAB - 1);
+      sx[q] = sat_i16(X >> INTER_BITS); sy[q] = sat_i16(Y >> INTER_BITS);
+      fx[q] = X & (TAB - 1); fy[q] = Y & (TAB - 1);
     } else {
       if (MODE == 1) {
         double u, v;
         undistort_point(a.cm, x4 + q, y, u, v);
         quantise_uv(u, v, mx[q], my[q], fr[q], pack_saturates(a.cm.model, x4 + q, a.cm.w));
       }
-      sx = mx[q]; sy = my[q];
-      fx = fr[q] & (TAB - 1); fy = (fr[q] >> INTER_BITS) & (TAB - 1);
+      sx[q] = mx[q]; sy[q] = my[q];
+      fx[q] = fr[q] & (TAB - 1); fy[q] = (fr[q] >> INTER_BITS) & (TAB - 1);
     }
-    px[q] = gather_px(a.src, (unsigned)a.spitch, a.sw, a.sh, sx, sy, fx, fy);
+    // one frame (launched only for n = 1, so f0 = 0): gather each pixel as soon as its taps are known, as the
+    // single-frame kernel always did -- about half the registers of the batch form, twice the occupancy
+    if (NB == 1) px[q] = gather_px<LD>(a.src, (unsigned)a.spitch, a.sw, a.sh, sx[q], sy[q], fx[q], fy[q]);
   }
-  unsigned* o = reinterpret_cast<unsigned*>(a.dst + (size_t)y * a.dpitch + (size_t)x4 * 3);
-  o[0] = __byte_perm(px[0], px[1], 0x4210);   // B0 G0 R0 B1
-  o[1] = __byte_perm(px[1], px[2], 0x5421);   // G1 R1 B2 G2
-  o[2] = __byte_perm(px[2], px[3], 0x6542);   // R2 B3 G3 R3
+  const int nf = a.n - f0 < NB ? a.n - f0 : NB;
+  const uint8_t* s = a.src + (long long)f0 * a.sistride;
+  uint8_t* d = a.dst + (long long)f0 * a.distride + (long long)y * a.dpitch + (long long)x4 * 3;
+  for (int f = 0; f < nf; ++f, s += a.sistride, d += a.distride) {
+    if (NB != 1) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) px[q] = gather_px<LD>(s, (unsigned)a.spitch, a.sw, a.sh, sx[q], sy[q], fx[q], fy[q]);
+    }
+    unsigned* o = reinterpret_cast<unsigned*>(NB == 1 ? a.dst + (long long)y * a.dpitch + (long long)x4 * 3 : d);
+    o[0] = lane_perm(px[0], px[1], 0x4210);   // B0 G0 R0 B1
+    o[1] = lane_perm(px[1], px[2], 0x5421);   // G1 R1 B2 G2
+    o[2] = lane_perm(px[2], px[3], 0x6542);   // R2 B3 G3 R3
+    if (NB == 1) break;
+  }
+}
+
+// NB = frames per thread: GATHER_NB over a batch, 1 for a single frame (n = 1 then compiles to the single-frame body
+// and keeps its register count and occupancy; the batch form needs about twice the registers).
+template <int MODE, int NB>
+__global__ void __launch_bounds__(256) k_gather4(GatherArgs a) {
+  const int x4 = (blockIdx.x * 32 + (threadIdx.x & 31)) * 4;
+  const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x4 >= a.dw || y >= a.dh) return;
+  gather4_frames<MODE, NB>(a, x4, y, blockIdx.z * NB);
 }
 
 }  // namespace bevk

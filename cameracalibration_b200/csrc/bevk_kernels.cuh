@@ -37,6 +37,9 @@ __global__ void __launch_bounds__(256) k_undistort_map(CamModel cm, short2* __re
 // ---------------------------------------------------------------------------------
 // K3 / K4: generic gather.  MODE 0: maps in HBM, 1: camera model evaluated in-kernel
 // (fused undistort), 2: homography (warpPerspective).
+// Over a batch of n frames: the taps of an output pixel depend on the pixel only, so a thread
+// resolves them once (map load or camera model) and gathers them from GATHER_NB frames of its
+// grid-z slice.  Frame f is read at src + f * sistride and written at dst + f * distride.
 // ---------------------------------------------------------------------------------
 struct GatherArgs {
   const uint8_t* src; int sw, sh; long long spitch;
@@ -44,26 +47,36 @@ struct GatherArgs {
   const short2* map1; const unsigned short* map2;
   CamModel cm;
   Homog hm;
+  int n; long long sistride, distride;   // frames, and the 64-bit image strides of source and destination
 };
 
+// Frames per thread (grid.z = ceil(n / GATHER_NB)); DESIGN.md section 4 has the measurement that chose it.
+#ifndef BEVK_GATHER_NB
+#define BEVK_GATHER_NB 8
+#endif
+constexpr int GATHER_NB = BEVK_GATHER_NB;
+
 template <int C>
-__device__ __forceinline__ void load_px(const uint8_t* __restrict__ src, long long spitch, int sw, int sh,
-                                        int x, int y, int (&p)[C]) {
+__host__ __device__ __forceinline__ void load_px(const uint8_t* __restrict__ src, long long spitch, int sw, int sh,
+                                                 int x, int y, int (&p)[C]) {
   if ((unsigned)x < (unsigned)sw && (unsigned)y < (unsigned)sh) {
     const uint8_t* q = src + (long long)y * spitch + (long long)x * C;
+#ifdef __CUDA_ARCH__
 #pragma unroll
     for (int c = 0; c < C; ++c) p[c] = __ldg(q + c);
+#else
+    for (int c = 0; c < C; ++c) p[c] = q[c];
+#endif
   } else {
 #pragma unroll
     for (int c = 0; c < C; ++c) p[c] = 0;
   }
 }
 
+// One thread of k_gather: output pixel (x, y) of frames [f0, min(n, f0 + GATHER_NB)).  Host-capable, so that
+// tests/host/undistort_stack.cu runs the same frame loop and addressing on a CPU.
 template <int MODE, int C, int LINEAR>
-__global__ void __launch_bounds__(256) k_gather(GatherArgs a) {
-  const int x = blockIdx.x * 32 + (threadIdx.x & 31);
-  const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
-  if (x >= a.dw || y >= a.dh) return;
+__host__ __device__ __forceinline__ void gather_frames(const GatherArgs& a, int x, int y, int f0) {
   int sx, sy, fx = 0, fy = 0;
   if (MODE == 2) {
     int X, Y;
@@ -96,21 +109,33 @@ __global__ void __launch_bounds__(256) k_gather(GatherArgs a) {
       sx += (fx < 16); sy += (fy < 16);
     }
   }
-  uint8_t* o = a.dst + (long long)y * a.dpitch + (long long)x * C;
-  if (LINEAR) {
-    int p00[C], p01[C], p10[C], p11[C];
-    load_px<C>(a.src, a.spitch, a.sw, a.sh, sx, sy, p00);
-    load_px<C>(a.src, a.spitch, a.sw, a.sh, sx + 1, sy, p01);
-    load_px<C>(a.src, a.spitch, a.sw, a.sh, sx, sy + 1, p10);
-    load_px<C>(a.src, a.spitch, a.sw, a.sh, sx + 1, sy + 1, p11);
+  const int nf = a.n - f0 < GATHER_NB ? a.n - f0 : GATHER_NB;
+  const uint8_t* s = a.src + (long long)f0 * a.sistride;
+  uint8_t* o = a.dst + (long long)f0 * a.distride + (long long)y * a.dpitch + (long long)x * C;
+  for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) {
+    if (LINEAR) {
+      int p00[C], p01[C], p10[C], p11[C];
+      load_px<C>(s, a.spitch, a.sw, a.sh, sx, sy, p00);
+      load_px<C>(s, a.spitch, a.sw, a.sh, sx + 1, sy, p01);
+      load_px<C>(s, a.spitch, a.sw, a.sh, sx, sy + 1, p10);
+      load_px<C>(s, a.spitch, a.sw, a.sh, sx + 1, sy + 1, p11);
 #pragma unroll
-    for (int c = 0; c < C; ++c) o[c] = (uint8_t)bilerp_q10(p00[c], p01[c], p10[c], p11[c], fx, fy);
-  } else {
-    int p[C];
-    load_px<C>(a.src, a.spitch, a.sw, a.sh, sx, sy, p);
+      for (int c = 0; c < C; ++c) o[c] = (uint8_t)bilerp_q10(p00[c], p01[c], p10[c], p11[c], fx, fy);
+    } else {
+      int p[C];
+      load_px<C>(s, a.spitch, a.sw, a.sh, sx, sy, p);
 #pragma unroll
-    for (int c = 0; c < C; ++c) o[c] = (uint8_t)p[c];
+      for (int c = 0; c < C; ++c) o[c] = (uint8_t)p[c];
+    }
   }
+}
+
+template <int MODE, int C, int LINEAR>
+__global__ void __launch_bounds__(256) k_gather(GatherArgs a) {
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31);
+  const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x >= a.dw || y >= a.dh) return;
+  gather_frames<MODE, C, LINEAR>(a, x, y, blockIdx.z * GATHER_NB);
 }
 
 // ---------------------------------------------------------------------------------

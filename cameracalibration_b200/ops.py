@@ -121,6 +121,37 @@ def _cuda_bgr_batch(arr):
     return int(ptr), n, h, w, int(img), int(row)
 
 
+def _cuda_images(arr, what):
+    """(device pointer, rank, n, h, w, channels, image stride, row stride) of a uint8 CUDA array [H][W], [H][W][C] or
+    [N][H][W][C] (C in 1, 3, 4) whose pixels are dense (C-byte pixels, 1-byte channels); rows and images may be padded."""
+    iface = getattr(arr, "__cuda_array_interface__", None)
+    if iface is None:
+        raise L.BevkError(f"{what} must be a CUDA array (an object with __cuda_array_interface__), got {type(arr).__name__}")
+    shape = tuple(iface["shape"])
+    if iface["typestr"] not in ("|u1", "<u1", "=u1"):
+        raise L.BevkError(f"{what} must be uint8, got typestr {iface['typestr']}")
+    rank = len(shape)
+    if rank not in (2, 3, 4) or (rank > 2 and shape[-1] not in (1, 3, 4)):
+        raise L.BevkError(f"{what} must be uint8[H][W], [H][W][C] or [N][H][W][C] with C in 1, 3, 4, got shape {shape}")
+    strides = iface.get("strides")
+    if strides is None:
+        strides = tuple(int(np.prod(shape[i + 1:])) for i in range(rank))
+    strides = tuple(int(s) for s in strides)
+    if rank == 2:
+        shape, strides = shape + (1,), strides + (1,)
+    if rank != 4:
+        shape, strides = (1,) + shape, (0,) + strides
+    n, h, w, ch = shape
+    if (ch > 1 and strides[3] != 1) or (w > 1 and strides[2] != ch):
+        raise L.BevkError(f"{what} must have dense pixels (strides {ch} and 1 along width and channels)")
+    ptr = iface["data"][0]
+    if not ptr:
+        raise L.BevkError(f"{what} has a null data pointer")
+    row = strides[1] if h > 1 else w * ch
+    img = strides[0] if n > 1 else h * row
+    return int(ptr), rank, n, h, w, ch, img, row
+
+
 def jpeg_encode(images, quality: int = 95, ctx: L.Context | None = None) -> list[bytes]:
     """cv2.imencode('.jpg', img, [cv2.IMWRITE_JPEG_QUALITY, quality]) on the GPU, byte for byte, for one uint8[H][W][3]
     BGR image or a batch uint8[N][H][W][3].  CUDA arrays (``__cuda_array_interface__``, e.g. the torch canvases of
@@ -291,6 +322,10 @@ class Undistorter:
         return m1, m2
 
     def __call__(self, src: np.ndarray, interpolation: int = INTER_LINEAR, out: np.ndarray | None = None) -> np.ndarray:
+        """cv2.remap(src, map1, map2, interpolation).  A CUDA array (e.g. a torch tensor on the GPU) goes to cuda() and
+        the result stays on the device; NumPy input is uploaded, undistorted and downloaded in one call."""
+        if hasattr(src, "__cuda_array_interface__"):
+            return self.cuda(src, out=out, interpolation=interpolation)
         self._live()
         img, sw, sh, ss, ch = L.image_view(src)
         out = _out((self.h, self.w) if src.ndim == 2 else (self.h, self.w, ch), out)
@@ -311,6 +346,52 @@ class Undistorter:
         L.check(self.ctx.lib.bevk_undistort_jpeg(self.ctx.h, self.slot, L.vptr(img), sw, sh, ss, _interp(interpolation),
                                                  int(quality), L.vptr(self._jpeg_buf), self._jpeg_buf.size, C.byref(size)))
         return self._jpeg_buf[:size.value].tobytes()
+
+    def cuda(self, frames, out=None, interpolation: int = INTER_LINEAR, stream: int | None = None):
+        """Undistort frames that already live on the GPU: no PCIe in the call.
+
+        frames: a uint8 CUDA array (``__cuda_array_interface__``) [H][W] (one grey image), [H][W][C] (one image) or
+        [N][H][W][C] (a batch; a grey batch is [N][H][W][1]), C in 1, 3, 4.  Pixels must be dense; rows and images may
+        be padded.  ``out``: a CUDA array of the matching shape (rows and images may be padded too), default a new torch
+        tensor.  Each output pixel's map entry (or camera model) is read once for several frames of the batch.  Runs on
+        ``stream`` (a raw CUDA stream handle), default torch's current stream, and only enqueues.  Returns ``out``."""
+        self._live()
+        ptr, rank, n, sh, sw, ch, simg, srow = _cuda_images(frames, "frames")
+        shape = {2: (self.h, self.w), 3: (self.h, self.w, ch), 4: (n, self.h, self.w, ch)}[rank]
+        if out is None:
+            import torch
+            out = torch.empty(shape, dtype=torch.uint8, device=torch.device("cuda", self.ctx.device))
+        optr, orank, on, oh, ow, och, oimg, orow = _cuda_images(out, "out")
+        if orank != rank or (on, oh, ow, och) != (n, self.h, self.w, ch):
+            raise L.BevkError(f"out must be a uint8 CUDA array of shape {shape}")
+        if stream is None:
+            from .sharding import _torch_current_stream
+            stream = _torch_current_stream(self.ctx.device)
+        with self.ctx.on_stream(stream):
+            L.check(self.ctx.lib.bevk_undistort_stack(self.ctx.h, self.slot, C.c_void_p(ptr), simg, sw, sh, srow, ch, n,
+                                                      C.c_void_p(optr), oimg, self.w, self.h, orow, _interp(interpolation)))
+        return out
+
+    def cuda_to_jpeg(self, frames, quality: int = 95, interpolation: int = INTER_LINEAR) -> list[bytes]:
+        """cuda() followed by cv2.imencode('.jpg', img, [IMWRITE_JPEG_QUALITY, quality]) per frame, with the encoder on
+        the GPU: the undistorted images stay in library scratch and only the JPEG streams come back.  frames: a uint8
+        CUDA array [H][W][3] or [N][H][W][3] (BGR) laid out as cuda() takes it.  Runs on torch's current stream and
+        synchronises.  Returns one ``bytes`` per frame, byte-identical to cv2's."""
+        self._live()
+        ptr, rank, n, sh, sw, ch, simg, srow = _cuda_images(frames, "frames")
+        if ch != 3 or rank == 2:
+            raise L.BevkError("Undistorter.cuda_to_jpeg takes uint8[H][W][3] or uint8[N][H][W][3] BGR frames")
+        out = np.empty(max(n, 1) * jpeg_encode_bound(self.w, self.h), np.uint8)   # pages are only touched where streams land
+        sizes = (C.c_uint64 * max(n, 1))()
+        from .sharding import _torch_current_stream
+        with self.ctx.on_stream(_torch_current_stream(self.ctx.device)):
+            L.check(self.ctx.lib.bevk_undistort_stack_jpeg(self.ctx.h, self.slot, C.c_void_p(ptr), simg, sw, sh, srow, n,
+                                                           _interp(interpolation), int(quality), L.vptr(out), out.size, sizes))
+        return BevEngine._split(out, sizes)
+
+    def last_path(self) -> str:
+        """Which gather the last call of this ctx launched: 'word' (k_gather4, 4 pixels per thread) or 'byte' (k_gather)."""
+        return {4: "word", 1: "byte"}.get(int(self.ctx.lib.bevk_undistort_last_path(self.ctx.h)), "none")
 
 
 class BevEngine:

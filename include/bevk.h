@@ -89,6 +89,19 @@ int bevk_undistorter_maps(bevk_ctx *ctx, int slot, int16_t *map1, uint16_t *map2
  * a slot that was re-set can never make the library write past dst). */
 int bevk_undistort(bevk_ctx *ctx, int slot, const uint8_t *src, int sw, int sh, int64_t sstride, int channels,
                    uint8_t *dst, int dw, int dh, int64_t dstride, int interp);
+/* n DEVICE frames (frame i at d_src + i*src_image_stride, rows src_row_stride apart, channels 1/3/4) undistorted
+ * through the slot's map or fused model into n DEVICE images (dst_image_stride / dst_row_stride, dw x dh = the slot's
+ * size, checked).  Each output pixel's taps are resolved once (map read or camera model) for several frames.  Row
+ * strides must cover a row, image strides (read when n > 1) an image; a destination range that overlaps the source
+ * range is refused.  3-channel INTER_LINEAR with dw % 4 == 0 takes the 4-pixel word path when both base pointers, both
+ * row strides and (n > 1) both image strides are multiples of 4; otherwise the byte path.  Only enqueues on the ctx
+ * stream; no allocation or synchronisation, so it can be graph-captured. */
+int bevk_undistort_stack(bevk_ctx *ctx, int slot, const void *d_src, int64_t src_image_stride, int sw, int sh,
+                         int64_t src_row_stride, int channels, int n, void *d_dst, int64_t dst_image_stride,
+                         int dw, int dh, int64_t dst_row_stride, int interp);
+/* Which gather the last undistort call (or bevk_remap / bevk_warp_perspective) launched: 4 = k_gather4 (word path),
+ * 1 = k_gather (byte path), 0 = none yet. */
+int bevk_undistort_last_path(bevk_ctx *ctx);
 
 /* ---- K4: cv2.warpPerspective(src, H, (dw,dh), flags=interp), border 0 --------
  *   ExtrinsicCalibration/extrinsicCalib.py:166-169, surroundBEV.py:113-114      */
@@ -230,7 +243,7 @@ int bevk_shard_compose(bevk_ctx *ctx, const void *d_slabs, int batch, const void
 /* ---- JPEG ingest on the device ------------------------------------------------------------------------------
  * Replaces cv2.imread in front of the path (surroundBEV.py:328-332, Tools/undistort.py:65): n baseline JPEG streams
  * (host memory) are decoded by nvJPEG (dlopen'ed on first use) into frames 0..n-1 of a device frame stack, BGR
- * interleaved, row pitch width*3 -- the layout bevk_bev_run_stack and the undistort entry points read.  Only the
+ * interleaved, row pitch width*3 -- the layout bevk_bev_run_stack and bevk_undistort_stack(_jpeg) read.  Only the
  * compressed bytes cross PCIe.  Every stream must decode to width x height.  The pixels are nvJPEG's, which differ from
  * libjpeg-turbo's (cv2) by the decoders' IDCT / upsampling rounding; everything downstream is bit-exact on them.
  * The Huffman stage runs on the calling thread; GPU work is enqueued on the ctx stream. */
@@ -258,6 +271,12 @@ int bevk_jpeg_encode(bevk_ctx *ctx, const void *d_images, int64_t image_stride, 
  * without the undistorted image ever leaving the device.  Works with map and fused slots; capacity as above.          */
 int bevk_undistort_jpeg(bevk_ctx *ctx, int slot, const uint8_t *src, int sw, int sh, int64_t sstride, int interp, int quality,
                         uint8_t *out, uint64_t capacity, uint64_t *size);
+/* bevk_undistort_stack for n 3-channel DEVICE frames, encoded on the device: the streams are byte-identical to
+ * cv2.imencode of the undistorted images, back to back in host `out`; sizes[n] is always filled; capacity rule as
+ * bevk_bev_frames_to_jpeg (below), and the same chunk pipeline (BEVK_JPEG_CHUNK).  Synchronises; cannot be captured. */
+int bevk_undistort_stack_jpeg(bevk_ctx *ctx, int slot, const void *d_src, int64_t src_image_stride, int sw, int sh,
+                              int64_t src_row_stride, int n, int interp, int quality,
+                              uint8_t *out, uint64_t capacity, uint64_t *sizes);
 
 /* ---- BEV canvases straight to JPEG ----------------------------------------------------------------------------------
  * BevGenerator.__call__ then cv2.imencode('.jpg', surround, [IMWRITE_JPEG_QUALITY, quality]) (surroundBEV.py:312-325,
