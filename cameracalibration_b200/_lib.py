@@ -75,6 +75,9 @@ SIGNATURES = {
     "bevk_shard_last_link_bytes": (C.c_int64, [_p]),
     "bevk_shard_render": (C.c_int, [_p, _p, C.c_int64, C.c_int, C.c_int, _p]),
     "bevk_shard_compose": (C.c_int, [_p, _p, C.c_int, _p, _p]),
+    "bevk_shard_vsum": (C.c_int, [_p, _p, C.c_int64, C.c_int, C.c_int, _p]),
+    "bevk_shard_render_balanced": (C.c_int, [_p, _p, C.c_int64, C.c_int, C.c_int, _p, _p]),
+    "bevk_shard_compose_balanced": (C.c_int, [_p, _p, C.c_int, _p, _p]),
     "bevk_jpeg_decode": (C.c_int, [_p, C.POINTER(_p), C.POINTER(C.c_uint64), C.c_int, C.c_int, C.c_int, _p, C.c_int64]),
     "bevk_bev_run_jpeg": (C.c_int, [_p, C.POINTER(_p), C.POINTER(C.c_uint64), C.c_int, _p, C.c_int, _p]),
     "bevk_jpeg_encode_bound": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_uint64)]),

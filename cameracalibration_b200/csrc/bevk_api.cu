@@ -190,6 +190,7 @@ struct bevk_ctx {
     long long slab_bytes = 0;
     void* comm = nullptr;                   // ncclComm_t
     DevBuf d_slabs;
+    DevBuf d_vsums;                         // BALANCE: V sums [world][batch][n_cam], block r from rank r
     long long last_link_bytes = 0;
     // peer-store exchange (bevk_bev_run_scattered): this rank's receive buffer [2 halves][world][own_max][slab_bytes],
     // the same buffer of every peer mapped through CUDA IPC, and a 4-byte-per-rank scratch for the step barrier
@@ -1046,6 +1047,55 @@ struct OutWin {
   uint8_t* peer[SHARD_MAX_RANKS] = {}; int world = 0; long long src_off = 0;
 };
 
+// k_vsum over the frames of camera range `cr` (`nr` of them) through a pointer table: vsum[frame] += its V sum
+static void launch_vsum(bevk_ctx* c, const uint8_t* const* srcs, CamRange cr, int nr, unsigned long long* vsum) {
+  const long long frame_bytes = (long long)c->FW * 3 * c->FH;
+  const int blocks = (int)std::max<long long>(1, std::min<long long>(c->n_sm * 4 / std::max(1, std::min(nr, 64)) + 1, frame_bytes / (48 * 256) + 1));
+  k_vsum<<<dim3(blocks, nr), 256, 0, c->stream>>>(srcs, frame_bytes, vsum, cr);
+}
+
+// BALANCE pre-pass of the fused render: luminance_balance of the frames of cameras [lo, hi) of every frame-set, once
+// per sampled source pixel, into balanced copies (d_bal: frame b * n_cam + cam at the 256-byte padded stride) that the
+// ordinary fused gather then reads; *bal_src describes them.  The V sums come from k_vsum over those frames
+// (vsum_blocks null: single GPU, where the range is every camera), or from the `world` blocks [world][batch][n_cam]
+// that camera-sharded ranks filled with their own cameras' sums and exchanged.  Other cameras' copies are neither
+// written nor read.  The caller checks batch * n_cam <= 65535.
+static int balance_prepass(bevk_ctx* c, FrameSrc src, int batch, int lo, int hi, const unsigned long long* vsum_blocks, int world,
+                           FrameSrc* bal_src) {
+  const int nf = batch * c->n_cam, nr = batch * (hi - lo);
+  const CamRange cr{lo, hi - lo, c->n_cam};
+  RET(c->d_delta.ensure((size_t)nf * 4));
+  if (!vsum_blocks) {
+    RET(c->d_vsum.ensure((size_t)nf * 8));
+    CU(cudaMemsetAsync(c->d_vsum.p, 0, (size_t)nf * 8, c->stream));
+  }
+  const void* table = src.table;
+  if (!table) RET(stack_table(c, src.base, src.stride, nf, &table));
+  const uint8_t* const* srcs = reinterpret_cast<const uint8_t* const*>(table);
+  if (!vsum_blocks) {
+    launch_vsum(c, srcs, cr, nr, c->d_vsum.as<unsigned long long>());
+    LAUNCHED(c);
+    vsum_blocks = c->d_vsum.as<unsigned long long>();
+    world = 1;
+  }
+  k_delta<<<(batch + 127) / 128, 128, 0, c->stream>>>(vsum_blocks, c->n_cam, batch, world, (double)c->FW * (double)c->FH,
+                                                       c->d_delta.as<int>());
+  LAUNCHED(c);
+  const size_t fpad = ((size_t)c->FW * 3 * c->FH + 255) & ~size_t(255);
+  RET(c->d_bal.ensure(fpad * nf));
+  RET(c->d_bal_ptrs.ensure(sizeof(void*) * nf));
+  if (c->bal_ptrs_for != c->d_bal.p || c->bal_ptrs_n != nf || c->bal_ptrs_pad != fpad) {
+    k_fill_ptrs<<<(nf + 255) / 256, 256, 0, c->stream>>>(c->d_bal_ptrs.as<const uint8_t*>(), c->d_bal.as<uint8_t>(), (long long)fpad, nf);
+    LAUNCHED(c);
+    c->bal_ptrs_for = c->d_bal.p; c->bal_ptrs_n = nf; c->bal_ptrs_pad = fpad;
+  }
+  k_lum_spans<<<dim3((c->FH + LUM_ROWS - 1) / LUM_ROWS, nr), 128, 0, c->stream>>>(srcs, c->d_bal_ptrs.as<uint8_t*>(), c->d_spans.as<int2>(), cr,
+                                                                                 c->FW, c->FH, c->d_delta.as<int>(), c->d_hsv.as<int>());
+  LAUNCHED(c);
+  bal_src->table = c->d_bal_ptrs.p; bal_src->base = c->d_bal.as<uint8_t>(); bal_src->stride = (long long)fpad;
+  return BEVK_OK;
+}
+
 // run_device flag, not part of the ABI: with BALANCE, stop at the raw composed canvas and its channel sums (d_csum).  The
 // encoder's GainSrc applies the gains and the car, so k_gain does not run.  (Without BALANCE the write-out adds the car.)
 constexpr int kFlagRawBalance = 1 << 30;
@@ -1078,35 +1128,9 @@ static int run_device(bevk_ctx* c, FrameSrc src, int batch, const void* d_car, i
   if (c->timed && !c->capturing) CU(cudaEventRecord(c->ev0, c->stream));
   FrameSrc gsrc = src;                         // what the fused gather reads
   if (bal) {
-    RET(c->d_vsum.ensure((size_t)nf * 8));
-    RET(c->d_delta.ensure((size_t)nf * 4));
     RET(c->d_csum.ensure((size_t)batch * 24));
-    CU(cudaMemsetAsync(c->d_vsum.p, 0, (size_t)nf * 8, c->stream));
     CU(cudaMemsetAsync(c->d_csum.p, 0, (size_t)batch * 24, c->stream));
-    const void* table = src.table;
-    if (!table) RET(stack_table(c, src.base, src.stride, nf, &table));
-    const uint8_t* const* srcs = reinterpret_cast<const uint8_t* const*>(table);
-    const long long frame_bytes = (long long)P.pitch * c->FH;
-    const int blocks = (int)std::max<long long>(1, std::min<long long>(c->n_sm * 4 / std::max(1, std::min(nf, 64)) + 1, frame_bytes / (48 * 256) + 1));
-    k_vsum<<<dim3(blocks, nf), 256, 0, c->stream>>>(srcs, frame_bytes, c->d_vsum.as<unsigned long long>());
-    LAUNCHED(c);
-    k_delta<<<(batch + 127) / 128, 128, 0, c->stream>>>(c->d_vsum.as<unsigned long long>(), c->n_cam, batch,
-                                                         (double)c->FW * (double)c->FH, c->d_delta.as<int>());
-    LAUNCHED(c);
-    // luminance_balance once per sampled source pixel into balanced frame copies, then the ordinary
-    // fused gather reads those copies
-    const size_t fpad = ((size_t)frame_bytes + 255) & ~size_t(255);
-    RET(c->d_bal.ensure(fpad * nf));
-    RET(c->d_bal_ptrs.ensure(sizeof(void*) * nf));
-    if (c->bal_ptrs_for != c->d_bal.p || c->bal_ptrs_n != nf || c->bal_ptrs_pad != fpad) {
-      k_fill_ptrs<<<(nf + 255) / 256, 256, 0, c->stream>>>(c->d_bal_ptrs.as<const uint8_t*>(), c->d_bal.as<uint8_t>(), (long long)fpad, nf);
-      LAUNCHED(c);
-      c->bal_ptrs_for = c->d_bal.p; c->bal_ptrs_n = nf; c->bal_ptrs_pad = fpad;
-    }
-    k_lum_spans<<<dim3((c->FH + LUM_ROWS - 1) / LUM_ROWS, nf), 128, 0, c->stream>>>(srcs, c->d_bal_ptrs.as<uint8_t*>(), c->d_spans.as<int2>(), c->n_cam,
-                                                       c->FW, c->FH, c->d_delta.as<int>(), c->d_hsv.as<int>());
-    LAUNCHED(c);
-    gsrc.table = c->d_bal_ptrs.p; gsrc.base = c->d_bal.as<uint8_t>(); gsrc.stride = (long long)fpad;
+    RET(balance_prepass(c, src, batch, 0, c->n_cam, nullptr, 1, &gsrc));
     P.csum = c->d_csum.as<unsigned long long>();
   }
   // TMA-staged kernel for frame stacks (16-byte aligned base and stride); pointer-table gather otherwise
@@ -1492,9 +1516,9 @@ int bevk_luminance_balance(bevk_ctx* c, const uint8_t* const* imgs, int n, int w
   const uint8_t* const* d_in = c->d_ptrs.as<const uint8_t*>();
   uint8_t* const* d_out = reinterpret_cast<uint8_t* const*>(c->d_ptrs.as<uint8_t*>() + BEVK_MAX_CAMERAS);
   k_vsum<<<dim3(stream_blocks(c, fbytes / 48 + 1) / n + 1, n), 256, 0, c->stream>>>(d_in, (long long)fbytes,
-                                                                                 c->d_vsum.as<unsigned long long>());
+                                                                                 c->d_vsum.as<unsigned long long>(), CamRange{0, n, n});
   LAUNCHED(c);
-  k_delta<<<1, 32, 0, c->stream>>>(c->d_vsum.as<unsigned long long>(), n, 1, (double)w * (double)h, c->d_delta.as<int>());
+  k_delta<<<1, 32, 0, c->stream>>>(c->d_vsum.as<unsigned long long>(), n, 1, 1, (double)w * (double)h, c->d_delta.as<int>());
   LAUNCHED(c);
   k_lum_apply<<<dim3(stream_blocks(c, (long long)w * h) / n + 1, n), 256, 0, c->stream>>>(d_in, d_out, w, h, c->d_delta.as<int>(),
                                                                                        c->d_hsv.as<int>());
@@ -1559,6 +1583,7 @@ static void shard_release(bevk_ctx* c) {
   if (c->shard.comm && nccl().ok) nccl().CommDestroy(c->shard.comm);
   c->shard.comm = nullptr;
   c->shard.d_slabs.release();
+  c->shard.d_vsums.release();
 }
 
 int bevk_shard_configure(bevk_ctx* c, int policy, int rank, int world) {
@@ -1637,23 +1662,105 @@ static int shard_render(bevk_ctx* c, FrameSrc src, int batch, int as_rank, void*
   return run_device(c, src, batch, nullptr, 0, dst, s.cam_lo[as_rank], s.cam_hi[as_rank], &w);
 }
 
-static int shard_compose(bevk_ctx* c, const void* d_slabs, int batch, const void* d_car, void* d_out, long long rank_stride = 0) {
+// bal: colour balance after the compose -- k_compose_slabs<.., true> writes the raw canvases and their channel sums,
+// then k_gain applies the grey-world gains and the car, as the single-GPU BALANCE render does
+static int shard_compose(bevk_ctx* c, const void* d_slabs, int batch, const void* d_car, void* d_out, long long rank_stride = 0,
+                         bool bal = false) {
   bevk_ctx::Shard& s = c->shard;
   ComposeArgs a{};
   a.slabs = reinterpret_cast<const uint8_t*>(d_slabs); a.slab_bytes = s.slab_bytes; a.world = std::min(s.world, SHARD_MAX_RANKS);
   a.rank_stride = rank_stride ? rank_stride : (long long)batch * s.slab_bytes;
   a.batch = batch; a.BW = c->BW; a.BH = c->BH;
   for (int r = 0; r < a.world; ++r) a.rect[r] = s.rect[r];
-  a.car = reinterpret_cast<const uint8_t*>(d_car); a.out = reinterpret_cast<uint8_t*>(d_out);
-  const bool wide = (c->BW % 8) == 0 && (reinterpret_cast<uintptr_t>(d_out) & 7) == 0 && (!d_car || (reinterpret_cast<uintptr_t>(d_car) & 7) == 0) &&
+  a.car = bal ? nullptr : reinterpret_cast<const uint8_t*>(d_car); a.out = reinterpret_cast<uint8_t*>(d_out);
+  const bool wide = (c->BW % 8) == 0 && (reinterpret_cast<uintptr_t>(d_out) & 7) == 0 && (!a.car || (reinterpret_cast<uintptr_t>(a.car) & 7) == 0) &&
                     (reinterpret_cast<uintptr_t>(d_slabs) & 7) == 0 && (s.slab_bytes & 7) == 0 && (a.rank_stride & 7) == 0;
   if (batch > 65535 || c->BH > 65535 * COMPOSE_ROWS) return fail(BEVK_ERR_UNSUPPORTED, "compose grid too large");
   const int units = wide ? c->BW * 3 / 8 : c->BW * 3;
   const dim3 grid((units + 255) / 256, (c->BH + COMPOSE_ROWS - 1) / COMPOSE_ROWS, batch);
-  if (wide) k_compose_slabs<8><<<grid, 256, 0, c->stream>>>(a);
-  else k_compose_slabs<1><<<grid, 256, 0, c->stream>>>(a);
+  if (!bal) {
+    if (wide) k_compose_slabs<8><<<grid, 256, 0, c->stream>>>(a);
+    else k_compose_slabs<1><<<grid, 256, 0, c->stream>>>(a);
+    LAUNCHED(c);
+    return BEVK_OK;
+  }
+  RET(c->d_csum.ensure((size_t)batch * 24));
+  CU(cudaMemsetAsync(c->d_csum.p, 0, (size_t)batch * 24, c->stream));
+  a.csum = c->d_csum.as<unsigned long long>();
+  if (wide) k_compose_slabs<8, true><<<grid, 256, 0, c->stream>>>(a);
+  else k_compose_slabs<1, true><<<grid, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  const long long canvas_bytes = (long long)c->BW * c->BH * 3;
+  const int gblocks = (int)std::max<long long>(1, std::min<long long>(canvas_bytes / (12 * 256) + 1, c->n_sm * 8 / std::max(1, std::min(batch, 64)) + 1));
+  k_gain<<<dim3(gblocks, batch), 256, 0, c->stream>>>(a.out, canvas_bytes, (double)c->BW * (double)c->BH, a.csum,
+                                                      reinterpret_cast<const uint8_t*>(d_car));
   LAUNCHED(c);
   return BEVK_OK;
+}
+
+// BALANCE limits of a camera-sharded call, checked before anything is enqueued (those of run_device)
+static int shard_balance_limits(bevk_ctx* c, int batch) {
+  if (batch < 1 || batch > 65535) return fail(BEVK_ERR_ARG, "batch %d out of range [1,65535]", batch);
+  if ((long long)batch * c->n_cam > 65535) return fail(BEVK_ERR_ARG, "batch %d x %d cameras exceeds the 65535 frames of a BALANCE call", batch, c->n_cam);
+  return BEVK_OK;
+}
+
+// the V sums of rank `as_rank`'s own cameras into block as_rank of d_vsums[world][batch][n_cam], zero in the other
+// columns; other cameras' frames are never read
+static int shard_vsum(bevk_ctx* c, FrameSrc src, int batch, int as_rank, unsigned long long* d_vsums) {
+  bevk_ctx::Shard& s = c->shard;
+  const int lo = s.cam_lo[as_rank], hi = s.cam_hi[as_rank], nf = batch * c->n_cam;
+  unsigned long long* blk = d_vsums + (size_t)as_rank * nf;
+  CU(cudaMemsetAsync(blk, 0, (size_t)nf * 8, c->stream));
+  if (hi <= lo) return BEVK_OK;   // a rank without cameras sends zeros
+  const void* table = src.table;
+  if (!table) RET(stack_table(c, src.base, src.stride, nf, &table));
+  launch_vsum(c, reinterpret_cast<const uint8_t* const*>(table), CamRange{lo, hi - lo, c->n_cam}, batch * (hi - lo), blk);
+  LAUNCHED(c);
+  return BEVK_OK;
+}
+
+// rank `as_rank`'s slabs under BALANCE: luminance balance of its own cameras from the exchanged V sums, then the
+// ordinary windowed render of the balanced copies
+static int shard_render_balanced(bevk_ctx* c, FrameSrc src, int batch, int as_rank, const unsigned long long* d_vsums, void* d_slabs) {
+  bevk_ctx::Shard& s = c->shard;
+  const SlabRect q = s.rect[as_rank];
+  if (q.ox1 <= q.ox || s.cam_hi[as_rank] <= s.cam_lo[as_rank]) return BEVK_OK;
+  FrameSrc bal;
+  RET(balance_prepass(c, src, batch, s.cam_lo[as_rank], s.cam_hi[as_rank], d_vsums, s.world, &bal));
+  return shard_render(c, bal, batch, as_rank, d_slabs);
+}
+
+int bevk_shard_vsum(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, int as_rank, uint64_t* d_vsums) {
+  RET(use(c));
+  RET(shard_geometry(c));
+  RET(check_stack(c, d_frames, frame_stride));
+  RET(shard_balance_limits(c, batch));
+  if (as_rank < 0 || as_rank >= c->shard.world || as_rank >= SHARD_MAX_RANKS) return fail(BEVK_ERR_ARG, "rank %d out of range", as_rank);
+  if (!d_vsums || (reinterpret_cast<uintptr_t>(d_vsums) & 7)) return fail(BEVK_ERR_ARG, "V-sum buffer null or not 8-byte aligned");
+  return shard_vsum(c, stack_src(d_frames, frame_stride), batch, as_rank, reinterpret_cast<unsigned long long*>(d_vsums));
+}
+
+int bevk_shard_render_balanced(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, int as_rank, const uint64_t* d_vsums,
+                               void* d_slabs) {
+  RET(use(c));
+  RET(shard_geometry(c));
+  RET(check_stack(c, d_frames, frame_stride));
+  RET(shard_balance_limits(c, batch));
+  if (as_rank < 0 || as_rank >= c->shard.world || as_rank >= SHARD_MAX_RANKS) return fail(BEVK_ERR_ARG, "rank %d out of range", as_rank);
+  if (!d_vsums || (reinterpret_cast<uintptr_t>(d_vsums) & 7)) return fail(BEVK_ERR_ARG, "V-sum buffer null or not 8-byte aligned");
+  if (!d_slabs || (reinterpret_cast<uintptr_t>(d_slabs) & 15)) return fail(BEVK_ERR_ARG, "slab buffer null or not 16-byte aligned");
+  c->timed = true;
+  return shard_render_balanced(c, stack_src(d_frames, frame_stride), batch, as_rank,
+                               reinterpret_cast<const unsigned long long*>(d_vsums), d_slabs);
+}
+
+int bevk_shard_compose_balanced(bevk_ctx* c, const void* d_slabs, int batch, const void* d_car, void* d_out) {
+  RET(use(c));
+  RET(shard_geometry(c));
+  if (!d_slabs || !d_out) return fail(BEVK_ERR_ARG, "null device pointer");
+  RET(shard_balance_limits(c, batch));
+  return shard_compose(c, d_slabs, batch, d_car, d_out, 0, true);
 }
 
 int bevk_shard_render(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, int as_rank, void* d_slabs) {
@@ -1673,6 +1780,21 @@ int bevk_shard_compose(bevk_ctx* c, const void* d_slabs, int batch, const void* 
   return shard_compose(c, d_slabs, batch, d_car, d_out);
 }
 
+// this rank's V sums into its block of s.d_vsums, then one in-place all-gather of the blocks (none in a world of one);
+// *received: the bytes that came from the other ranks
+static int shard_exchange_vsums(bevk_ctx* c, FrameSrc src, int batch, long long* received) {
+  bevk_ctx::Shard& s = c->shard;
+  const size_t blk = (size_t)batch * c->n_cam * 8;
+  RET(s.d_vsums.ensure(blk * s.world));
+  RET(shard_vsum(c, src, batch, s.rank, s.d_vsums.as<unsigned long long>()));
+  *received = 0;
+  if (s.world == 1) return BEVK_OK;
+  const int r = nccl().AllGather(s.d_vsums.as<uint8_t>() + blk * s.rank, s.d_vsums.p, blk, kNcclUint8, s.comm, c->stream);
+  if (r != 0) return fail(BEVK_ERR_CUDA, "ncclAllGather (V sums): %s", nccl().GetErrorString(r));
+  *received = (long long)blk * (s.world - 1);
+  return BEVK_OK;
+}
+
 int bevk_bev_run_sharded(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, const void* d_car, int flags, void* d_out) {
   NvtxRange nvtx_call("bevk_bev_run_sharded (render slabs, all-gather, compose)");
   RET(use(c));
@@ -1684,18 +1806,27 @@ int bevk_bev_run_sharded(bevk_ctx* c, const void* d_frames, int64_t frame_stride
     c->timed = true;
     return run_device(c, stack_src(d_frames, frame_stride), batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
   }
-  if (flags & BEVK_FLAG_BALANCE) return fail(BEVK_ERR_UNSUPPORTED, "balance needs every camera's V mean before the warp: not available with camera sharding");
+  const bool bal = (flags & BEVK_FLAG_BALANCE) != 0;
+  if (bal) RET(shard_balance_limits(c, batch));
   if (!s.comm) return fail(BEVK_ERR_ARG, "bevk_shard_connect not called");
   RET(shard_geometry(c));
+  const FrameSrc src = stack_src(d_frames, frame_stride);
   const size_t per_rank = (size_t)batch * s.slab_bytes;
   RET(s.d_slabs.ensure(per_rank * s.world));
   c->timed = false;
-  RET(shard_render(c, stack_src(d_frames, frame_stride), batch, s.rank, s.d_slabs.p));
+  long long vsum_bytes = 0;
+  if (bal) {
+    // luminance_balance needs every camera's V mean: ONE all-gather of the ranks' V-sum blocks before the render
+    RET(shard_exchange_vsums(c, src, batch, &vsum_bytes));
+    RET(shard_render_balanced(c, src, batch, s.rank, s.d_vsums.as<unsigned long long>(), s.d_slabs.p));
+  } else {
+    RET(shard_render(c, src, batch, s.rank, s.d_slabs.p));
+  }
   // ONE all-gather of the slabs (in place: this rank's block is already where it belongs)
   const int r = nccl().AllGather(s.d_slabs.as<uint8_t>() + per_rank * s.rank, s.d_slabs.p, per_rank, kNcclUint8, s.comm, c->stream);
   if (r != 0) return fail(BEVK_ERR_CUDA, "ncclAllGather: %s", nccl().GetErrorString(r));
-  s.last_link_bytes = (long long)per_rank * (s.world - 1);
-  return shard_compose(c, s.d_slabs.p, batch, d_car, d_out);
+  s.last_link_bytes = (long long)per_rank * (s.world - 1) + vsum_bytes;
+  return shard_compose(c, s.d_slabs.p, batch, d_car, d_out, 0, bal);
 }
 
 // ---- camera sharding with peer stores: compute and exchange in one kernel ----------------------------------------
@@ -1756,7 +1887,8 @@ int bevk_bev_run_scattered(bevk_ctx* c, const void* d_frames, int64_t frame_stri
   bevk_ctx::Shard& s = c->shard;
   if (!s.configured || s.policy != BEVK_SHARD_CAMERAS) return fail(BEVK_ERR_ARG, "bevk_shard_configure(CAMERAS) not called");
   RET(check_stack(c, d_frames, frame_stride));
-  if (flags & BEVK_FLAG_BALANCE) return fail(BEVK_ERR_UNSUPPORTED, "balance is not available with camera sharding");
+  const bool bal = (flags & BEVK_FLAG_BALANCE) != 0;
+  if (bal) RET(shard_balance_limits(c, batch));
   RET(shard_geometry(c));
   if (!s.comm && s.world > 1) return fail(BEVK_ERR_ARG, "bevk_shard_connect not called");
   if (!s.attached || batch > s.prepared_batch || (batch + s.world - 1) / s.world != s.own_max)
@@ -1765,24 +1897,30 @@ int bevk_bev_run_scattered(bevk_ctx* c, const void* d_frames, int64_t frame_stri
   if (n_own) *n_own = mine;
   if (mine > 0 && !d_out_own) return fail(BEVK_ERR_ARG, "null output");
   const size_t half = (size_t)s.world * s.own_max * s.slab_bytes, rank_stride = (size_t)s.own_max * s.slab_bytes;
-  const unsigned par = s.step++ & 1u;     // double buffer: a peer may already store step n+1 while this rank composes step n
   const SlabRect q = s.rect[s.rank];
+  const FrameSrc src = stack_src(d_frames, frame_stride);
   s.last_link_bytes = 0;
+  c->timed = false;
+  long long vsum_bytes = 0;
+  if (bal) RET(shard_exchange_vsums(c, src, batch, &vsum_bytes));
+  const unsigned par = s.step++ & 1u;     // double buffer: a peer may already store step n+1 while this rank composes step n
   if (q.ox1 > q.ox && s.cam_hi[s.rank] > s.cam_lo[s.rank]) {
     OutWin w;
     w.pitch = (q.ox1 - q.ox) * 3; w.ox = q.ox; w.oy = q.oy; w.ox1 = q.ox1; w.oy1 = q.oy1; w.stride = s.slab_bytes;
     w.world = s.world; w.src_off = (long long)(par * half + (size_t)s.rank * rank_stride);
     for (int r = 0; r < s.world; ++r) w.peer[r] = reinterpret_cast<uint8_t*>(s.peer_recv[r]);
-    c->timed = false;
-    RET(run_device(c, stack_src(d_frames, frame_stride), batch, nullptr, 0, nullptr, s.cam_lo[s.rank], s.cam_hi[s.rank], &w));
+    FrameSrc rsrc = src;   // BALANCE: the peer-store render reads this rank's balanced copies
+    if (bal) RET(balance_prepass(c, src, batch, s.cam_lo[s.rank], s.cam_hi[s.rank], s.d_vsums.as<unsigned long long>(), s.world, &rsrc));
+    RET(run_device(c, rsrc, batch, nullptr, 0, nullptr, s.cam_lo[s.rank], s.cam_hi[s.rank], &w));
     s.last_link_bytes = (long long)(batch - mine) * s.slab_bytes;   // what this rank stored into its peers
   }
+  s.last_link_bytes += vsum_bytes;
   if (s.world > 1) {   // the step barrier: every rank's stores are complete (its kernel has finished) when this returns on the stream
     int* f = s.d_flag.as<int>();
     const int r = nccl().AllGather(f + SHARD_MAX_RANKS, f, 4, kNcclUint8, s.comm, c->stream);
     if (r != 0) return fail(BEVK_ERR_CUDA, "ncclAllGather (step barrier): %s", nccl().GetErrorString(r));
   }
-  if (mine > 0) RET(shard_compose(c, reinterpret_cast<const uint8_t*>(s.recv) + par * half, mine, d_car, d_out_own, (long long)rank_stride));
+  if (mine > 0) RET(shard_compose(c, reinterpret_cast<const uint8_t*>(s.recv) + par * half, mine, d_car, d_out_own, (long long)rank_stride, bal));
   return BEVK_OK;
 }
 

@@ -277,9 +277,17 @@ __device__ __forceinline__ unsigned vsum_16px(const uint4 a, const uint4 b, cons
   return s;
 }
 
+// The frames of cameras [lo, lo + n) of a frame-set-major stack of n_cam cameras: launch index i (grid y) -> frame
+// (i / n) * n_cam + lo + i % n.  A camera-sharded rank converts only its own cameras; the whole range {0, n_cam, n_cam}
+// is the identity.
+struct CamRange { int lo, n, n_cam; };
+__host__ __device__ __forceinline__ int range_frame(CamRange r, int i) { return (i / r.n) * r.n_cam + r.lo + i % r.n; }
+
+// grid y = frames of the range; vsum[frame] += its V sum
 __global__ void __launch_bounds__(256) k_vsum(const uint8_t* const* __restrict__ frames, long long frame_bytes,
-                                              unsigned long long* __restrict__ vsum) {
-  const uint8_t* f = frames[blockIdx.y];
+                                              unsigned long long* __restrict__ vsum, CamRange cr) {
+  const int fi = range_frame(cr, blockIdx.y);
+  const uint8_t* f = frames[fi];
   const long long n48 = frame_bytes / 48;
   unsigned long long acc = 0;
   if ((reinterpret_cast<uintptr_t>(f) & 15) == 0) {
@@ -307,7 +315,7 @@ __global__ void __launch_bounds__(256) k_vsum(const uint8_t* const* __restrict__
   if (threadIdx.x == 0) {
     unsigned long long t = 0;
     for (int k = 0; k < 8; ++k) t += part[k];
-    atomicAdd(vsum + blockIdx.y, t);
+    atomicAdd(vsum + fi, t);
   }
 }
 
@@ -320,11 +328,26 @@ __host__ __device__ __forceinline__ void lum_deltas(const unsigned long long* vs
   for (int c = 0; c < n_cam; ++c) delta[c] = cv_round(dadd(vmean, -ddiv((double)vsum[c], npix)));
 }
 
-__global__ void k_delta(const unsigned long long* __restrict__ vsum, int n_cam, int batch, double npix,
+// The same from `world` blocks of V sums, block w at vsum + w * block_stride: camera-sharded ranks each fill the
+// columns of their own cameras and leave the others zero, so the column sums are exact and equal the single-GPU sums.
+// world 1 is the single-GPU case.
+__host__ __device__ __forceinline__ void gathered_deltas(const unsigned long long* vsum, long long block_stride, int world,
+                                                         int n_cam, double npix, int* delta) {
+  unsigned long long v[BEVK_MAX_CAMERAS_K];
+  for (int c = 0; c < n_cam; ++c) {
+    unsigned long long s = 0;
+    for (int w = 0; w < world; ++w) s += vsum[w * block_stride + c];
+    v[c] = s;
+  }
+  lum_deltas(v, n_cam, npix, delta);
+}
+
+// vsum: [world][batch][n_cam]
+__global__ void k_delta(const unsigned long long* __restrict__ vsum, int n_cam, int batch, int world, double npix,
                         int* __restrict__ delta) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= batch) return;
-  lum_deltas(vsum + b * n_cam, n_cam, npix, delta + b * n_cam);
+  gathered_deltas(vsum + b * n_cam, (long long)batch * n_cam, world, n_cam, npix, delta + b * n_cam);
 }
 
 // ---------------------------------------------------------------------------------
@@ -480,7 +503,7 @@ __global__ void __launch_bounds__(256) k_lum_apply(const uint8_t* const* __restr
 // can sample.  spans[cam * FH + y] = (first, last+1) source column of row y that any tap of camera
 // `cam` touches (bevk_bev_finalize); everything else in the frame is never read by k_bev, so it
 // is not converted (about 17 % of a frame at the fixture geometry, 4.6x fewer HSV round trips
-// than converting the four taps of every output pixel).  grid = (FH, n_frames).
+// than converting the four taps of every output pixel).  grid = (FH / LUM_ROWS, frames of the camera range `cr`).
 // ---------------------------------------------------------------------------------
 constexpr int LUM_ROWS = 16;   // source rows per CTA
 
@@ -489,10 +512,10 @@ constexpr int LUM_ROWS = 16;   // source rows per CTA
 // memory) that the threads stride through, so that a row with a short span costs nothing and every thread has several
 // independent groups in flight; the sector selection of hsv_roundtrip is branch-free.
 __global__ void __launch_bounds__(128) k_lum_spans(const uint8_t* const* __restrict__ frames, uint8_t* const* __restrict__ outs,
-                                                   const int2* __restrict__ spans, int n_cam, int w, int h,
+                                                   const int2* __restrict__ spans, CamRange cr, int w, int h,
                                                    const int* __restrict__ delta, const int* __restrict__ hsv_tab) {
-  const int f = blockIdx.y, y0 = blockIdx.x * LUM_ROWS, y1 = min(h, y0 + LUM_ROWS), nrows = y1 - y0;
-  const int2* sp_cam = spans + (size_t)(f % n_cam) * h;
+  const int f = range_frame(cr, blockIdx.y), y0 = blockIdx.x * LUM_ROWS, y1 = min(h, y0 + LUM_ROWS), nrows = y1 - y0;
+  const int2* sp_cam = spans + (size_t)(f % cr.n_cam) * h;
   __shared__ int s_tab[512];
   __shared__ int s_pref[LUM_ROWS + 1], s_g0[LUM_ROWS];
   const bool words = (w & 3) == 0 && ((reinterpret_cast<uintptr_t>(frames[f]) | reinterpret_cast<uintptr_t>(outs[f])) & 3) == 0;

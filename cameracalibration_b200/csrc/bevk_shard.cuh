@@ -52,24 +52,26 @@ struct ComposeArgs {
   SlabRect rect[SHARD_MAX_RANKS];
   const uint8_t* car;              // dense canvas or null
   uint8_t* out;                    // [batch][BH][BW][3]
+  unsigned long long* csum;        // BAL: channel sums [batch][3] of the composed canvases (zeroed by the caller)
 };
 
-#ifdef __CUDACC__
 // grid (chunks of 256 units per canvas row, groups of COMPOSE_ROWS canvas rows, frame-sets): no index arithmetic beyond
 // adds.  UNIT bytes per thread and row: 8 when canvas rows are whole 8-byte words (BW % 8 == 0; every slab edge then falls
 // on an 8-byte boundary: tile-aligned x is a multiple of 96 bytes, the canvas edge a multiple of 8), else 1.
 constexpr int COMPOSE_ROWS = 4;
 
-template <int UNIT>
-__global__ void __launch_bounds__(256) k_compose_slabs(ComposeArgs a) {
-  const int b = blockIdx.z;
+// One thread's work: bytes [xb, xb + UNIT) of canvas rows y0 .. y0 + COMPOSE_ROWS - 1 of frame-set b.  Without BAL the
+// car is added.  With BAL the raw canvas is written (colour balance and then the car follow in k_gain) and each byte
+// written is added to sums[channel], the channel being its offset in the canvas row mod 3 (a row starts on a pixel).
+// Host-capable: tests/host/shard_compose.cu drives it over the device's grid.
+template <int UNIT, bool BAL>
+__host__ __device__ __forceinline__ void compose_column(const ComposeArgs& a, int b, int y0, int xb, unsigned* sums) {
   const int row_bytes = a.BW * 3;
-  const int xb = (blockIdx.x * 256 + threadIdx.x) * UNIT;
-  if (xb >= row_bytes) return;
   uint8_t* out = a.out + (size_t)b * row_bytes * a.BH;
+  unsigned rel[3] = {0, 0, 0};     // BAL: sums of the bytes at xb + k, k % 3 == 0, 1, 2
 #pragma unroll
   for (int dy = 0; dy < COMPOSE_ROWS; ++dy) {
-    const int y = blockIdx.y * COMPOSE_ROWS + dy;
+    const int y = y0 + dy;
     if (y >= a.BH) break;
     const size_t off = (size_t)y * row_bytes + xb;
     unsigned lo = 0, hi = 0;
@@ -80,15 +82,65 @@ __global__ void __launch_bounds__(256) k_compose_slabs(ComposeArgs a) {
       if (y < q.oy || y >= q.oy1 || xb < q.ox * 3 || xb >= q.ox1 * 3) continue;
       const uint8_t* p = a.slabs + (size_t)r * a.rank_stride + (size_t)b * a.slab_bytes + (size_t)(y - q.oy) * ((q.ox1 - q.ox) * 3) + (xb - q.ox * 3);
       // plain loads (not the read-only path): in peer-store mode other GPUs wrote this memory
-      if (UNIT == 8) { const uint2 v = *reinterpret_cast<const uint2*>(p); lo = __vaddus4(lo, v.x); hi = __vaddus4(hi, v.y); }
+      if (UNIT == 8) { const uint2 v = *reinterpret_cast<const uint2*>(p); lo = lane_addus4(lo, v.x); hi = lane_addus4(hi, v.y); }
       else lo = min(255u, lo + *p);
     }
-    if (a.car) {
+    if (!BAL && a.car) {
+#ifdef __CUDA_ARCH__
       if (UNIT == 8) { const uint2 v = __ldg(reinterpret_cast<const uint2*>(a.car + off)); lo = __vaddus4(lo, v.x); hi = __vaddus4(hi, v.y); }
       else lo = min(255u, lo + __ldg(a.car + off));
+#else
+      if (UNIT == 8) { const uint2 v = *reinterpret_cast<const uint2*>(a.car + off); lo = lane_addus4(lo, v.x); hi = lane_addus4(hi, v.y); }
+      else lo = min(255u, lo + a.car[off]);
+#endif
     }
     if (UNIT == 8) *reinterpret_cast<uint2*>(out + off) = make_uint2(lo, hi);
     else out[off] = (uint8_t)lo;
+    if (BAL) {
+      if (UNIT == 8) {   // bytes k = 0..3 of lo, 4..7 of hi
+        rel[0] += (lo & 255u) + (lo >> 24) + ((hi >> 16) & 255u);
+        rel[1] += ((lo >> 8) & 255u) + (hi & 255u) + (hi >> 24);
+        rel[2] += ((lo >> 16) & 255u) + ((hi >> 8) & 255u);
+      } else {
+        rel[0] += lo;
+      }
+    }
+  }
+  if (BAL) {
+    const int ph = xb % 3;
+    sums[ph] += rel[0];
+    sums[ph == 2 ? 0 : ph + 1] += rel[1];
+    sums[ph == 0 ? 2 : ph - 1] += rel[2];
+  }
+}
+
+#ifdef __CUDACC__
+// BAL: 32-bit partials per thread (at most COMPOSE_ROWS * 3 * 255 per channel), warp shuffles, then one u64 atomic per
+// channel and CTA (a CTA's sum stays below 256 * COMPOSE_ROWS * 8 * 255 < 2^32).
+template <int UNIT, bool BAL = false>
+__global__ void __launch_bounds__(256) k_compose_slabs(ComposeArgs a) {
+  const int b = blockIdx.z;
+  const int xb = (blockIdx.x * 256 + threadIdx.x) * UNIT;
+  if (!BAL) {
+    if (xb >= a.BW * 3) return;
+    compose_column<UNIT, false>(a, b, blockIdx.y * COMPOSE_ROWS, xb, nullptr);
+    return;
+  }
+  unsigned s[3] = {0, 0, 0};
+  if (xb < a.BW * 3) compose_column<UNIT, true>(a, b, blockIdx.y * COMPOSE_ROWS, xb, s);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    s[0] += __shfl_xor_sync(0xffffffffu, s[0], o);
+    s[1] += __shfl_xor_sync(0xffffffffu, s[1], o);
+    s[2] += __shfl_xor_sync(0xffffffffu, s[2], o);
+  }
+  __shared__ unsigned part[8][3];
+  if ((threadIdx.x & 31) == 0) { part[threadIdx.x >> 5][0] = s[0]; part[threadIdx.x >> 5][1] = s[1]; part[threadIdx.x >> 5][2] = s[2]; }
+  __syncthreads();
+  if (threadIdx.x < 3) {
+    unsigned t = 0;
+    for (int w = 0; w < 8; ++w) t += part[w][threadIdx.x];
+    if (t) atomicAdd(a.csum + 3 * b + threadIdx.x, (unsigned long long)t);
   }
 }
 #endif

@@ -8,8 +8,11 @@ libbevk.so (bevk_shard_* / bevk_bev_run_sharded, include/bevk.h) so that a bindi
   * cameras per GPU ("cameras"): rank r renders cameras [lo_r, hi_r) of every frame-set into a SLAB (the tile-aligned
     bounding box of the union of their masks: 0.9-1.2 MB per frame-set at 1000x1000 instead of the 3 MB canvas), ONE
     ncclAllGather moves the slabs over NVLink, and every rank composes them with the saturating sum.  Exact, because
-    the reference's cv2.add chain (surroundBEV.py:316-320) is order-independent.  balance=True is not available in
-    this mode (luminance_balance needs every camera's V mean before the warp).
+    the reference's cv2.add chain (surroundBEV.py:316-320) is order-independent.  With balance=True each rank first
+    sums V over its own cameras' frames and one all-gather of those uint64 sums ([world][batch][n_cam]) gives every
+    rank every camera's luminance offset (luminance_balance needs all V means before the warp); each rank balances
+    and renders its own cameras, and colour balance runs on the composed canvases.  Every step is exact in integers,
+    so the canvases are byte-identical to the single-GPU render.
     The same policy with the exchange FUSED into the render kernel: ShardedBev.render_scattered -- frame-set b is owned
     by rank b % world, the fused kernel's write-out stores each slab straight into the owner's memory over NVLink (CUDA
     IPC peer mapping), a 4-byte all-gather is the step barrier, each rank composes the canvases it owns.
@@ -139,26 +142,52 @@ class ShardedBev:
         import torch
         return torch.zeros((self.world, batch, self.info()[3]), dtype=torch.uint8, device=torch.device("cuda", self.e.ctx.device))
 
-    def render_slabs(self, frames, as_rank: int, slabs, stream: int | None = None):
-        """The render half of the 'cameras' policy on its own: the slabs of rank `as_rank` into slabs[as_rank]."""
+    def vsum_buffer(self, batch: int):
+        """torch int64 CUDA tensor [world][batch][n_cam], zeroed, for vsums / render_slabs(vsums=...).  The library
+        treats it as uint64; a V sum stays far below 2**63."""
+        import torch
+        return torch.zeros((self.world, batch, self.e.n_cam), dtype=torch.int64, device=torch.device("cuda", self.e.ctx.device))
+
+    def vsums(self, frames, as_rank: int, buf, stream: int | None = None):
+        """The first BALANCE step of the 'cameras' policy on its own: the V sums of rank `as_rank`'s own cameras into
+        buf[as_rank] (zero in the other cameras' columns).  Every block must be filled (an all-gather, or every rank
+        on one GPU) before render_slabs(vsums=buf)."""
+        from . import _lib as L
+        from .ops import _cuda_ptr
+        e = self.e
+        base, shape = _cuda_ptr(frames, None)
+        d_buf = _vsum_ptr(buf, (self.world, shape[0], e.n_cam))
+        with e.ctx.on_stream(_torch_current_stream(e.ctx.device) if stream is None else stream):
+            L.check(e.ctx.lib.bevk_shard_vsum(e.ctx.h, C.c_void_p(base), e.FH * e.FW * 3, shape[0], int(as_rank), C.c_void_p(d_buf)))
+
+    def render_slabs(self, frames, as_rank: int, slabs, stream: int | None = None, vsums=None):
+        """The render half of the 'cameras' policy on its own: the slabs of rank `as_rank` into slabs[as_rank].
+        ``vsums``: the filled vsum_buffer -- render the luminance-balanced slabs (then compose with balance=True)."""
         from . import _lib as L
         from .ops import _cuda_ptr
         e = self.e
         base, shape = _cuda_ptr(frames, None)
         d_slabs = _cuda_ptr(slabs, (self.world, shape[0], self.info()[3]))[0]
         with e.ctx.on_stream(_torch_current_stream(e.ctx.device) if stream is None else stream):
-            L.check(e.ctx.lib.bevk_shard_render(e.ctx.h, C.c_void_p(base), e.FH * e.FW * 3, shape[0], int(as_rank), C.c_void_p(d_slabs)))
+            if vsums is None:
+                L.check(e.ctx.lib.bevk_shard_render(e.ctx.h, C.c_void_p(base), e.FH * e.FW * 3, shape[0], int(as_rank), C.c_void_p(d_slabs)))
+            else:
+                d_vs = _vsum_ptr(vsums, (self.world, shape[0], e.n_cam))
+                L.check(e.ctx.lib.bevk_shard_render_balanced(e.ctx.h, C.c_void_p(base), e.FH * e.FW * 3, shape[0], int(as_rank),
+                                                             C.c_void_p(d_vs), C.c_void_p(d_slabs)))
 
-    def compose(self, slabs, out, car=None, stream: int | None = None):
-        """The compose half: slabs[world][batch][slab_bytes] (+ car) -> out[batch][BH][BW][3]."""
+    def compose(self, slabs, out, car=None, stream: int | None = None, balance: bool = False):
+        """The compose half: slabs[world][batch][slab_bytes] (+ car) -> out[batch][BH][BW][3].  balance=True: colour
+        balance of the composed canvases before the car (slabs rendered with vsums=...)."""
         from . import _lib as L
         from .ops import _cuda_ptr
         e = self.e
         d_slabs, shape = _cuda_ptr(slabs, None)
         d_out = _cuda_ptr(out, (shape[1], e.BH, e.BW, 3))[0]
         d_car = _cuda_ptr(car, (e.BH, e.BW, 3))[0] if car is not None else None
+        fn = e.ctx.lib.bevk_shard_compose_balanced if balance else e.ctx.lib.bevk_shard_compose
         with e.ctx.on_stream(_torch_current_stream(e.ctx.device) if stream is None else stream):
-            L.check(e.ctx.lib.bevk_shard_compose(e.ctx.h, C.c_void_p(d_slabs), shape[1], C.c_void_p(d_car), C.c_void_p(d_out)))
+            L.check(fn(e.ctx.h, C.c_void_p(d_slabs), shape[1], C.c_void_p(d_car), C.c_void_p(d_out)))
         return out
 
     def own_frame_sets(self, batch: int):
@@ -184,12 +213,13 @@ class ShardedBev:
         dist.barrier(group=self.group)      # nobody stores into a peer before every peer has mapped and zeroed its buffer
         self._peers_for = batch
 
-    def render_scattered(self, frames, out_own, car=None, stream: int | None = None):
+    def render_scattered(self, frames, out_own, car=None, stream: int | None = None, balance: bool = False):
         """Policy 'cameras' with peer stores (bevk_bev_run_scattered): every rank renders its cameras' slabs of ALL
         frame-sets of ``frames`` ([batch][n_cam][FH][FW][3]; only its own cameras' frames are read), the fused kernel
         stores each slab straight into the memory of the rank that OWNS the frame-set (b % world) over NVLink, and each
         rank composes its own canvases into ``out_own`` ([ceil(batch / world)][BH][BW][3]; the first
-        len(own_frame_sets(batch)) entries are valid).  Returns the number of canvases written."""
+        len(own_frame_sets(batch)) entries are valid).  balance=True: the V-sum all-gather first, colour balance of the
+        owned canvases last.  Returns the number of canvases written."""
         from . import _lib as L
         from .ops import _cuda_ptr
         e = self.e
@@ -206,13 +236,34 @@ class ShardedBev:
         if stream is None:
             stream = _torch_current_stream(e.ctx.device)
         with e.ctx.on_stream(stream):
-            L.check(e.ctx.lib.bevk_bev_run_scattered(e.ctx.h, C.c_void_p(base), e.FH * e.FW * 3, batch, C.c_void_p(d_car), 0,
-                                                     C.c_void_p(d_out), C.byref(n_own)))
+            L.check(e.ctx.lib.bevk_bev_run_scattered(e.ctx.h, C.c_void_p(base), e.FH * e.FW * 3, batch, C.c_void_p(d_car),
+                                                     L.FLAG_BALANCE if balance else 0, C.c_void_p(d_out), C.byref(n_own)))
         return n_own.value
 
     def link_bytes(self) -> int:
-        """Bytes this rank received over NVLink in the last render()."""
+        """Bytes this rank received (render) or stored into its peers (render_scattered) over NVLink in the last call,
+        the V sums of balance=True included."""
         return int(self.e.ctx.lib.bevk_shard_last_link_bytes(self.e.ctx.h))
+
+
+def _vsum_ptr(buf, shape):
+    """Device pointer of a V-sum buffer: a C-contiguous 8-byte integer CUDA array of `shape` (vsum_buffer's)."""
+    from . import _lib as L
+    cai = getattr(buf, "__cuda_array_interface__", None)
+    if cai is None:
+        raise L.BevkError("V-sum buffer must expose __cuda_array_interface__")
+    if cai["typestr"] not in ("<i8", "<u8"):
+        raise L.BevkError(f"V-sum buffer must hold 8-byte integers, got {cai['typestr']}")
+    if tuple(cai["shape"]) != tuple(shape):
+        raise L.BevkError(f"V-sum buffer shape {tuple(cai['shape'])} != {tuple(shape)}")
+    if cai.get("strides") is not None:
+        want, acc = [], 8
+        for n in reversed(shape):
+            want.insert(0, acc)
+            acc *= n
+        if any(n > 1 and s != w for n, s, w in zip(shape, cai["strides"], want)):
+            raise L.BevkError("V-sum buffer must be C-contiguous")
+    return cai["data"][0]
 
 
 def _torch_current_stream(device: int):

@@ -218,7 +218,11 @@ int bevk_shard_connect(bevk_ctx *ctx, const void *id128, int len);
  * pixels, and the (padded, equal for all ranks) bytes of one frame-set's slab. */
 int bevk_shard_info(bevk_ctx *ctx, int rank, int *cam_lo, int *cam_hi, int32_t rect[4], int64_t *slab_bytes);
 /* BevGenerator.__call__ over a frame stack (see bevk_bev_run_stack) under the configured policy.  CAMERAS: every rank
- * passes the same batch; only the frames of its own cameras are read; every rank ends with all canvases in d_out. */
+ * passes the same batch; only the frames of its own cameras are read; every rank ends with all canvases in d_out.
+ * BEVK_FLAG_BALANCE under CAMERAS: each rank sums V over its own cameras' frames, one all-gather of those sums
+ * (world x batch x n_cam uint64) gives every rank the luminance offsets of every camera, each rank balances and renders
+ * its own cameras, and colour balance (then the car) runs on the composed canvases.  The result is byte-identical to
+ * the single-GPU BALANCE render; batch x n_cam <= 65535. */
 int bevk_bev_run_sharded(bevk_ctx *ctx, const void *d_frames, int64_t frame_stride, int batch, const void *d_car, int flags,
                          void *d_out);
 /* CAMERAS policy, fused compute + exchange: frame-set b is OWNED by rank b % world.  Every rank renders its cameras'
@@ -228,7 +232,8 @@ int bevk_bev_run_sharded(bevk_ctx *ctx, const void *d_frames, int64_t frame_stri
  * (and receives) (world-1)/world of one slab set, instead of receiving world-1 whole slab sets as the all-gather does.
  * Setup after bevk_shard_connect: bevk_shard_prepare(batch) on every rank gives a 64-byte handle; the launcher gathers
  * the handles of all ranks (rank order, world x 64 bytes) and gives them to bevk_shard_attach.  Frames must be a
- * 16-byte friendly stack (the TMA-staged kernel does the stores). */
+ * 16-byte friendly stack (the TMA-staged kernel does the stores).  BEVK_FLAG_BALANCE works as in bevk_bev_run_sharded:
+ * the V-sum all-gather comes first, and each rank colour-balances the canvases it owns. */
 int bevk_shard_prepare(bevk_ctx *ctx, int batch, void *handle64);
 int bevk_shard_attach(bevk_ctx *ctx, const void *handles);
 int bevk_bev_run_scattered(bevk_ctx *ctx, const void *d_frames, int64_t frame_stride, int batch, const void *d_car, int flags,
@@ -239,6 +244,14 @@ int64_t bevk_shard_last_link_bytes(bevk_ctx *ctx);
  * into d_slabs[as_rank][batch][slab_bytes]; compose d_slabs[world][batch][slab_bytes] (+ car) into canvases. */
 int bevk_shard_render(bevk_ctx *ctx, const void *d_frames, int64_t frame_stride, int batch, int as_rank, void *d_slabs);
 int bevk_shard_compose(bevk_ctx *ctx, const void *d_slabs, int batch, const void *d_car, void *d_out);
+/* The BALANCE halves, in this order: bevk_shard_vsum writes block as_rank of d_vsums[world][batch][n_cam] (8-byte
+ * aligned): the V sums of rank as_rank's own cameras, zero in the other columns.  Once every block is there (an
+ * all-gather, or every rank on one GPU), bevk_shard_render_balanced renders rank as_rank's balanced slabs and
+ * bevk_shard_compose_balanced composes, colour-balances and adds the car.  Only enqueue; batch x n_cam <= 65535. */
+int bevk_shard_vsum(bevk_ctx *ctx, const void *d_frames, int64_t frame_stride, int batch, int as_rank, uint64_t *d_vsums);
+int bevk_shard_render_balanced(bevk_ctx *ctx, const void *d_frames, int64_t frame_stride, int batch, int as_rank,
+                               const uint64_t *d_vsums, void *d_slabs);
+int bevk_shard_compose_balanced(bevk_ctx *ctx, const void *d_slabs, int batch, const void *d_car, void *d_out);
 
 /* ---- JPEG ingest on the device ------------------------------------------------------------------------------
  * Replaces cv2.imread in front of the path (surroundBEV.py:328-332, Tools/undistort.py:65): n baseline JPEG streams
