@@ -430,8 +430,8 @@ __global__ void __launch_bounds__(TMA_THREADS, MINCTAS) k_bev_tma(const TmaParam
       const bool words_ok = !BAL && out_words_ok(P);   // as the consumers decide
       bool prev_generic = false;   // the previous unit left through the generic write-out (reads across the warps' rows)
       // Units are handed out dynamically (one atomic per unit, only this thread needs it: the consumers follow the ring):
-      // unit u = tile u / groups of the cost-sorted tile list, frame-set group u % groups -- heavy tiles first, so the
-      // CTAs finish together.  The next unit's id and tile record are fetched while the current unit is being posted.
+      // unit u = tile u / groups of the plan's tile list (a Hilbert curve, cheapest tiles last: tile_order), frame-set
+      // group u % groups.  The next unit's id and tile record are fetched while the current unit is being posted.
       long long unit = (long long)atomicAdd(P.unit_counter, 1u);
       int4 tile = unit < n_units ? __ldg(P.tiles + (int)(unit / groups)) : make_int4(0, 0, 0, 0);
       while (unit < n_units) {

@@ -10,8 +10,8 @@
 //     2 FS (two frame-sets per pass) or 4 FS (one per pass), and only what exceeds 4 FS is a GATHER item (global loads).
 //   * the box pitch is chosen among the next few 16-byte multiples to minimise the shared-memory bank conflicts of the
 //     item's own warp loads (simulated here: the lanes of a warp follow a curved path through the box).
-// Box shapes are quantised to a small menu so that a few dozen tensor maps serve the whole plan.  Tiles are ordered by
-// decreasing estimated cost, so that the persistent CTAs' last rounds are the cheap ones.
+// Box shapes are quantised to a small menu so that a few dozen tensor maps serve the whole plan.  Tiles follow a Hilbert
+// curve for L2 reuse of the source rows, the cheapest ones last so that the persistent CTAs finish together (tile_order).
 #pragma once
 #include <algorithm>
 #include <climits>
@@ -24,6 +24,7 @@ namespace bevk {
 
 struct TmaPlan {
   std::vector<int4> tiles;          // x0, y0, first item, item count
+  std::vector<long long> tile_cost; // estimated cost of each tile (same order as `tiles`)
   std::vector<TmaItem> items;
   std::vector<uint4> lut;           // [block][4][256]
   std::vector<int2> shapes;         // box shapes: (width in 32-bit words, rows)
@@ -61,6 +62,46 @@ inline int lds_wavefronts(const unsigned* word, int n) {
     if (cnt[b] > deg) deg = cnt[b];
   }
   return deg;
+}
+
+// Index of tile (x, y) along the Hilbert curve over an n x n grid (n a power of two)
+inline int hilbert_index(int n, int x, int y) {
+  int d = 0;
+  for (int s = n / 2; s > 0; s /= 2) {
+    const int rx = (x & s) > 0, ry = (y & s) > 0;
+    d += s * s * ((3 * rx) ^ ry);
+    if (ry == 0) {
+      if (rx == 1) { x = n - 1 - x; y = n - 1 - y; }
+      std::swap(x, y);
+    }
+  }
+  return d;
+}
+
+// Order of the tiles, i.e. of k_bev_tma's units (tile u / groups, frame-set group u % groups).  Units run back to back
+// for a tile's frame-set groups and neighbouring tiles read overlapping source rows of the same frames, so the tiles
+// follow a Hilbert curve over the tile grid: what a tile shares with its neighbours is still in L2 when they run.  The
+// cheapest `tail_percent` % of the tiles (empty and light tiles) leave the curve and close the step, heaviest first,
+// so that the persistent CTAs finish together.  tools/l2_model.py compares this order with the alternatives on a model
+// of the step's DRAM traffic (DESIGN.md §4).
+constexpr int TILE_TAIL_PERCENT = 10;
+inline std::vector<int> tile_order(int tx, int ty, const std::vector<long long>& cost, int tail_percent = TILE_TAIL_PERCENT) {
+  const int n_tiles = tx * ty;
+  int n = 1;
+  while (n < tx || n < ty) n *= 2;
+  std::vector<int> h(n_tiles), curve(n_tiles), by_cost(n_tiles);
+  for (int i = 0; i < n_tiles; ++i) { h[i] = hilbert_index(n, i % tx, i / tx); curve[i] = by_cost[i] = i; }
+  std::stable_sort(curve.begin(), curve.end(), [&](int a, int b) { return h[a] < h[b]; });
+  std::stable_sort(by_cost.begin(), by_cost.end(), [&](int a, int b) { return cost[a] > cost[b]; });
+  const int n_tail = (int)((long long)n_tiles * std::max(0, std::min(100, tail_percent)) / 100);
+  std::vector<char> tail(n_tiles, 0);
+  for (int i = n_tiles - n_tail; i < n_tiles; ++i) tail[by_cost[i]] = 1;
+  std::vector<int> out;
+  out.reserve(n_tiles);
+  for (int t : curve)
+    if (!tail[t]) out.push_back(t);
+  for (int i = n_tiles - n_tail; i < n_tiles; ++i) out.push_back(by_cost[i]);
+  return out;
 }
 
 inline void build_tma_plan(int NC, int FW, int FH, int BW, int BH, bool nearest, const short* const* m1,
@@ -241,13 +282,10 @@ inline void build_tma_plan(int NC, int FW, int FH, int BW, int BH, bool nearest,
       out.tiles.push_back(t);
       tile_cost.push_back(item_cost);
     }
-  // heavy tiles first: CTA c takes units c, c + G, c + 2G, ... of each frame-set group, so every CTA gets one tile of
-  // each cost stratum and the last round consists of the cheapest tiles
-  std::vector<int> order(out.tiles.size());
-  for (size_t i = 0; i < order.size(); ++i) order[i] = (int)i;
-  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return tile_cost[a] > tile_cost[b]; });
+  const std::vector<int> order = tile_order(tx, ty, tile_cost);
   std::vector<int4> sorted(out.tiles.size());
-  for (size_t i = 0; i < order.size(); ++i) sorted[i] = out.tiles[order[i]];
+  out.tile_cost.resize(order.size());
+  for (size_t i = 0; i < order.size(); ++i) { sorted[i] = out.tiles[order[i]]; out.tile_cost[i] = tile_cost[order[i]]; }
   out.tiles.swap(sorted);
 }
 
