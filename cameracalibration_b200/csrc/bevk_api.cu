@@ -138,7 +138,6 @@ struct bevk_ctx {
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev_switch = nullptr;
   cudaStream_t copy_stream = nullptr;                      // H2D side of the host-pointer pipeline
   cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_free[2] = {nullptr, nullptr};
-  const void* ptrs_for = nullptr; const void* ptrs_tab = nullptr; long long ptrs_n = 0; size_t ptrs_pad = 0;   // cached frame pointer table
   bool timed = false;
   long long launches = 0;
   DevBuf s_src, s_dst, s_m1, s_m2, s_o1, s_o2;   // scratch for the host-pointer entry points
@@ -160,9 +159,8 @@ struct bevk_ctx {
   int cam_box[BEVK_MAX_CAMERAS][BEVK_MAX_BANDS][4] = {};   // per camera and band: sampled rows [y0,y1), bytes [bx0,bx1)
   DevBuf d_tiles, d_items, d_lut, d_hsv;
   int bev_grid[6] = {0, 0, 0, 0, 0, 0};   // resident CTAs of k_bev<BAL, NB>: index = 3*BAL + {NB=1:0, 4:1, 8:2}
-  DevBuf d_frames, d_ptrs, d_canvas, d_car, d_vsum, d_delta, d_csum;
-  DevBuf d_spans, d_bal, d_bal_ptrs;        // BALANCE: sampled row spans per camera, balanced frame copies + their table
-  const void* bal_ptrs_for = nullptr; long long bal_ptrs_n = 0; size_t bal_ptrs_pad = 0;
+  DevBuf d_frames, d_canvas, d_car, d_vsum, d_delta, d_csum;
+  DevBuf d_spans, d_bal;                    // BALANCE: sampled row spans per camera, balanced frame copies
   DevBuf d_user_ptrs;                       // bevk_bev_run_frames: device copy of the caller's frame table
   std::vector<const void*> user_tab;        // ... and what it currently holds
   // TMA-staged kernel (bevk_bev_tma.cuh): its plan, and the tensor maps of the frame stacks seen recently
@@ -177,9 +175,7 @@ struct bevk_ctx {
   int tma_cfg = 0;                          // index into kTmaConfigs
   int tma_backoff_ns = 0;                   // BEVK_TMA_BACKOFF (read at finalize): producer poll interval when the ring is full
   int tma_grid[kMaxTmaConfigs][4] = {};                  // [config] resident CTAs of k_bev_tma<BAL, NB>: index = 2*BAL + {NB=1:0, 4:1}
-  DevBuf d_stack_ptrs;                      // pointer table of a frame stack (BALANCE pre-passes read frames through a table)
-  const void* stack_ptrs_base = nullptr; long long stack_ptrs_stride = 0, stack_ptrs_n = 0;
-  int last_path = 0;                        // 1: k_bev (pointer-table gather), 2: k_bev_tma
+  int last_path = 0;                        // 1: k_bev (global-offset gather), 2: k_bev_tma
   int gather_path = 0;                      // stand-alone gathers: 4 = k_gather4 (word path), 1 = k_gather (byte path)
   // multi-GPU sharding (bevk_shard_*): partition, slab geometry, NCCL communicator
   struct Shard {
@@ -271,9 +267,9 @@ int bevk_ctx_destroy(bevk_ctx* c) {
   cudaSetDevice(c->device);
   cudaDeviceSynchronize();   // not c->stream: a caller-owned stream handed to bevk_ctx_set_stream may be gone by now
   for (DevBuf* b : {&c->s_src, &c->s_dst, &c->s_m1, &c->s_m2, &c->s_o1, &c->s_o2, &c->d_tiles, &c->d_items, &c->d_lut,
-                    &c->d_hsv, &c->d_frames, &c->d_ptrs, &c->d_canvas, &c->d_car, &c->d_vsum, &c->d_delta, &c->d_csum,
-                    &c->d_spans, &c->d_bal, &c->d_bal_ptrs, &c->d_user_ptrs, &c->d_ttiles, &c->d_titems, &c->d_tlut,
-                    &c->d_stack_ptrs, &c->d_jpeg_frames, &c->d_jpeg_canvas, &c->d_unit_counter})
+                    &c->d_hsv, &c->d_frames, &c->d_canvas, &c->d_car, &c->d_vsum, &c->d_delta, &c->d_csum,
+                    &c->d_spans, &c->d_bal, &c->d_user_ptrs, &c->d_ttiles, &c->d_titems, &c->d_tlut,
+                    &c->d_jpeg_frames, &c->d_jpeg_canvas, &c->d_unit_counter})
     b->release();
   for (DevBuf* b : {&c->enc.d_header, &c->enc.d_tabs, &c->enc.coef, &c->enc.bits, &c->enc.offs, &c->enc.dcdiff, &c->enc.words,
                     &c->enc.ffcnt, &c->enc.ffscan, &c->enc.scan_tmp, &c->enc.out[0], &c->enc.out[1], &c->enc.meta[0],
@@ -633,8 +629,6 @@ int bevk_bev_configure(bevk_ctx* c, int n_cam, int fw, int fh, int bw, int bh) {
   c->bev_interp = BEVK_INTER_LINEAR;
   c->planned = false;
   c->tma_planned = false;
-  // cached pointer tables are keyed on buffer addresses: a new geometry changes the strides behind the same addresses
-  c->ptrs_for = nullptr; c->bal_ptrs_for = nullptr; c->bal_ptrs_n = 0; c->stack_ptrs_base = nullptr;
   for (auto& k : c->cam) { k.has_maps = false; k.has_mask = false; k.mask.clear(); }
   return BEVK_OK;
 }
@@ -746,6 +740,20 @@ static TmaFns tma_fns(int cfg) {
   return TmaFns{{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}};
 }
 
+// OpenCV's 8-bit HSV division tables (color_hsv: sdiv_table / hdiv_table180, hsv_shift = 12), uploaded once per ctx
+static int ensure_hsv(bevk_ctx* c) {
+  if (c->d_hsv.p) return BEVK_OK;
+  std::vector<int> tab(512, 0);
+  for (int i = 1; i < 256; ++i) {
+    tab[i] = (int)std::nearbyint((255 << 12) / (1. * i));
+    tab[256 + i] = (int)std::nearbyint((180 << 12) / (6. * i));
+  }
+  RET(c->d_hsv.ensure(512 * sizeof(int)));
+  CU(cudaMemcpyAsync(c->d_hsv.p, tab.data(), 512 * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  return BEVK_OK;
+}
+
 // Tile-plan compiler: LUT maps + masks -> per-tile item lists and thread-ordered LUT blocks.
 int bevk_bev_finalize(bevk_ctx* c) {
   RET(use(c));
@@ -804,14 +812,7 @@ int bevk_bev_finalize(bevk_ctx* c) {
   c->n_bands = 2;
   if (const char* env = getenv("BEVK_BANDS")) c->n_bands = std::max(1, std::min(BEVK_MAX_BANDS, atoi(env)));
   for (int k = 0; k < NC; ++k) plan_bands(spans.data() + (size_t)k * FH, FW, FH, c->n_bands, c->cam_box[k]);
-  // OpenCV's 8-bit HSV division tables (color_hsv: sdiv_table / hdiv_table180, hsv_shift = 12)
-  std::vector<int> tab(512, 0);
-  for (int i = 1; i < 256; ++i) {
-    tab[i] = (int)std::nearbyint((255 << 12) / (1. * i));
-    tab[256 + i] = (int)std::nearbyint((180 << 12) / (6. * i));
-  }
-  RET(c->d_hsv.ensure(512 * sizeof(int)));
-  CU(cudaMemcpyAsync(c->d_hsv.p, tab.data(), 512 * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  RET(ensure_hsv(c));
   CU(cudaStreamSynchronize(c->stream));
   // ---- the TMA-staged kernel's plan (frames whose row pitch is a multiple of 16 bytes)
   c->tma_planned = false;
@@ -928,13 +929,8 @@ int bevk_bev_host_copy_bytes(bevk_ctx* c, int flags, int64_t* h2d, int64_t* d2h)
 }
 
 // ------------------------------------------------------------------ BEV engine: run
-// Where the frames of a call live: a device table of frame pointers (any layout), or a frame STACK (frame i at
-// base + i * stride), which is what the TMA-staged kernel's 3-D tensor maps describe.
-struct FrameSrc {
-  const void* table = nullptr;
-  const uint8_t* base = nullptr;
-  long long stride = 0;
-};
+// The frames of a call are a Frames (bevk_device.cuh).  Stacks are what the TMA-staged kernel's 3-D tensor maps describe;
+// every other kernel reads either form.
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -986,23 +982,6 @@ static int stack_maps(bevk_ctx* c, const uint8_t* base, long long stride, long l
   return BEVK_OK;
 }
 
-__global__ void k_fill_ptrs(const uint8_t** table, const uint8_t* base, long long stride, int n) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) table[i] = base + (long long)i * stride;
-}
-
-// pointer table of a frame stack (the BALANCE pre-passes and the round-1 gather kernel read frames through a table)
-static int stack_table(bevk_ctx* c, const uint8_t* base, long long stride, int n, const void** table) {
-  RET(c->d_stack_ptrs.ensure(sizeof(void*) * (size_t)n));
-  if (c->stack_ptrs_base != base || c->stack_ptrs_stride != stride || c->stack_ptrs_n < n) {
-    k_fill_ptrs<<<(n + 255) / 256, 256, 0, c->stream>>>(c->d_stack_ptrs.as<const uint8_t*>(), base, stride, n);
-    LAUNCHED(c);
-    c->stack_ptrs_base = base; c->stack_ptrs_stride = stride; c->stack_ptrs_n = n;
-  }
-  *table = c->d_stack_ptrs.p;
-  return BEVK_OK;
-}
-
 static int launch_bev_tma(bevk_ctx* c, const TmaParams& P, int nbu, bool bal) {
   const long long units = c->n_tiles * ((P.batch + nbu - 1) / nbu);
   const int variant = (bal ? 2 : 0) + (nbu == 4 ? 1 : 0);
@@ -1047,8 +1026,8 @@ struct OutWin {
   uint8_t* peer[SHARD_MAX_RANKS] = {}; int world = 0; long long src_off = 0;
 };
 
-// k_vsum over the frames of camera range `cr` (`nr` of them) through a pointer table: vsum[frame] += its V sum
-static void launch_vsum(bevk_ctx* c, const uint8_t* const* srcs, CamRange cr, int nr, unsigned long long* vsum) {
+// k_vsum over the frames of camera range `cr` (`nr` of them): vsum[frame] += its V sum
+static void launch_vsum(bevk_ctx* c, Frames srcs, CamRange cr, int nr, unsigned long long* vsum) {
   const long long frame_bytes = (long long)c->FW * 3 * c->FH;
   const int blocks = (int)std::max<long long>(1, std::min<long long>(c->n_sm * 4 / std::max(1, std::min(nr, 64)) + 1, frame_bytes / (48 * 256) + 1));
   k_vsum<<<dim3(blocks, nr), 256, 0, c->stream>>>(srcs, frame_bytes, vsum, cr);
@@ -1060,20 +1039,15 @@ static void launch_vsum(bevk_ctx* c, const uint8_t* const* srcs, CamRange cr, in
 // (vsum_blocks null: single GPU, where the range is every camera), or from the `world` blocks [world][batch][n_cam]
 // that camera-sharded ranks filled with their own cameras' sums and exchanged.  Other cameras' copies are neither
 // written nor read.  The caller checks batch * n_cam <= 65535.
-static int balance_prepass(bevk_ctx* c, FrameSrc src, int batch, int lo, int hi, const unsigned long long* vsum_blocks, int world,
-                           FrameSrc* bal_src) {
+static int balance_prepass(bevk_ctx* c, Frames src, int batch, int lo, int hi, const unsigned long long* vsum_blocks, int world,
+                           Frames* bal_src) {
   const int nf = batch * c->n_cam, nr = batch * (hi - lo);
   const CamRange cr{lo, hi - lo, c->n_cam};
   RET(c->d_delta.ensure((size_t)nf * 4));
   if (!vsum_blocks) {
     RET(c->d_vsum.ensure((size_t)nf * 8));
     CU(cudaMemsetAsync(c->d_vsum.p, 0, (size_t)nf * 8, c->stream));
-  }
-  const void* table = src.table;
-  if (!table) RET(stack_table(c, src.base, src.stride, nf, &table));
-  const uint8_t* const* srcs = reinterpret_cast<const uint8_t* const*>(table);
-  if (!vsum_blocks) {
-    launch_vsum(c, srcs, cr, nr, c->d_vsum.as<unsigned long long>());
+    launch_vsum(c, src, cr, nr, c->d_vsum.as<unsigned long long>());
     LAUNCHED(c);
     vsum_blocks = c->d_vsum.as<unsigned long long>();
     world = 1;
@@ -1083,16 +1057,11 @@ static int balance_prepass(bevk_ctx* c, FrameSrc src, int batch, int lo, int hi,
   LAUNCHED(c);
   const size_t fpad = ((size_t)c->FW * 3 * c->FH + 255) & ~size_t(255);
   RET(c->d_bal.ensure(fpad * nf));
-  RET(c->d_bal_ptrs.ensure(sizeof(void*) * nf));
-  if (c->bal_ptrs_for != c->d_bal.p || c->bal_ptrs_n != nf || c->bal_ptrs_pad != fpad) {
-    k_fill_ptrs<<<(nf + 255) / 256, 256, 0, c->stream>>>(c->d_bal_ptrs.as<const uint8_t*>(), c->d_bal.as<uint8_t>(), (long long)fpad, nf);
-    LAUNCHED(c);
-    c->bal_ptrs_for = c->d_bal.p; c->bal_ptrs_n = nf; c->bal_ptrs_pad = fpad;
-  }
-  k_lum_spans<<<dim3((c->FH + LUM_ROWS - 1) / LUM_ROWS, nr), 128, 0, c->stream>>>(srcs, c->d_bal_ptrs.as<uint8_t*>(), c->d_spans.as<int2>(), cr,
-                                                                                 c->FW, c->FH, c->d_delta.as<int>(), c->d_hsv.as<int>());
+  k_lum_spans<<<dim3((c->FH + LUM_ROWS - 1) / LUM_ROWS, nr), 128, 0, c->stream>>>(src, c->d_bal.as<uint8_t>(), (long long)fpad,
+                                                                                 c->d_spans.as<int2>(), cr, c->FW, c->FH,
+                                                                                 c->d_delta.as<int>(), c->d_hsv.as<int>());
   LAUNCHED(c);
-  bal_src->table = c->d_bal_ptrs.p; bal_src->base = c->d_bal.as<uint8_t>(); bal_src->stride = (long long)fpad;
+  *bal_src = Frames(c->d_bal.p, (long long)fpad);
   return BEVK_OK;
 }
 
@@ -1100,7 +1069,7 @@ static int balance_prepass(bevk_ctx* c, FrameSrc src, int batch, int lo, int hi,
 // encoder's GainSrc applies the gains and the car, so k_gain does not run.  (Without BALANCE the write-out adds the car.)
 constexpr int kFlagRawBalance = 1 << 30;
 
-static int run_device(bevk_ctx* c, FrameSrc src, int batch, const void* d_car, int flags, void* d_out, int cam_lo, int cam_hi,
+static int run_device(bevk_ctx* c, Frames src, int batch, const void* d_car, int flags, void* d_out, int cam_lo, int cam_hi,
                       const OutWin* win = nullptr) {
   NvtxRange nvtx_render("bevk render (fused BEV kernels)");
   if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
@@ -1126,15 +1095,15 @@ static int run_device(bevk_ctx* c, FrameSrc src, int batch, const void* d_car, i
   int nbu = batch >= 4 ? 4 : 1;
   if (c->nb_override) nbu = c->nb_override;
   if (c->timed && !c->capturing) CU(cudaEventRecord(c->ev0, c->stream));
-  FrameSrc gsrc = src;                         // what the fused gather reads
+  Frames gsrc = src;                           // what the fused gather reads
   if (bal) {
     RET(c->d_csum.ensure((size_t)batch * 24));
     CU(cudaMemsetAsync(c->d_csum.p, 0, (size_t)batch * 24, c->stream));
     RET(balance_prepass(c, src, batch, 0, c->n_cam, nullptr, 1, &gsrc));
     P.csum = c->d_csum.as<unsigned long long>();
   }
-  // TMA-staged kernel for frame stacks (16-byte aligned base and stride); pointer-table gather otherwise
-  const bool use_tma = c->tma_planned && gsrc.base && (reinterpret_cast<uintptr_t>(gsrc.base) & 15) == 0 && (gsrc.stride & 15) == 0 &&
+  // TMA-staged kernel for frame stacks (16-byte aligned base and stride); global-offset gather otherwise
+  const bool use_tma = c->tma_planned && !gsrc.table && (reinterpret_cast<uintptr_t>(gsrc.base) & 15) == 0 && (gsrc.stride & 15) == 0 &&
                        gsrc.stride >= (long long)P.pitch * c->FH && (nbu == 1 || nbu == 4);
   if (use_tma) {
     TmaParams T{};
@@ -1154,8 +1123,7 @@ static int run_device(bevk_ctx* c, FrameSrc src, int batch, const void* d_car, i
     c->last_path = 2;
   } else {
     if (win && win->world) return fail(BEVK_ERR_UNSUPPORTED, "peer-store output needs the TMA-staged kernel (a 16-byte friendly frame stack)");
-    if (!gsrc.table) RET(stack_table(c, gsrc.base, gsrc.stride, nf, &gsrc.table));
-    P.srcs = reinterpret_cast<const uint8_t* const*>(gsrc.table);
+    P.srcs = gsrc;
     const long long units = c->n_tiles * ((batch + nbu - 1) / nbu);
     const int variant = (bal ? 3 : 0) + (nbu == 8 ? 2 : (nbu == 4 ? 1 : 0));
     const unsigned bev_blocks = (unsigned)std::max<long long>(1, std::min<long long>(units, c->bev_grid[variant]));
@@ -1182,13 +1150,10 @@ static int run_device(bevk_ctx* c, FrameSrc src, int batch, const void* d_car, i
   return BEVK_OK;
 }
 
-static FrameSrc table_src(const void* d_srcs) { FrameSrc s; s.table = d_srcs; return s; }
-static FrameSrc stack_src(const void* base, long long stride) { FrameSrc s; s.base = reinterpret_cast<const uint8_t*>(base); s.stride = stride; return s; }
-
 int bevk_bev_run_device(bevk_ctx* c, const void* d_srcs, int batch, const void* d_car, int flags, void* d_out) {
   RET(use(c));
   c->timed = true;
-  return run_device(c, table_src(d_srcs), batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
+  return run_device(c, Frames(d_srcs), batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
 }
 
 // frames[i] == frames[0] + i * stride with a 16-byte friendly stride?  (a frame stack: the TMA-staged kernel applies)
@@ -1205,14 +1170,14 @@ static bool affine_table(const void* const* frames, size_t n, long long* stride)
 
 // The frames of a host table of device pointers as run_device reads them: a frame stack when the table describes one
 // (no table upload at all), else the ctx's device copy of the table, uploaded only when its contents change.
-static int frames_src(bevk_ctx* c, const void* const* frames, int batch, FrameSrc* src) {
+static int frames_src(bevk_ctx* c, const void* const* frames, int batch, Frames* src) {
   if (batch < 1) return fail(BEVK_ERR_ARG, "batch must be >= 1");
   const size_t n = (size_t)batch * c->n_cam;
   for (size_t i = 0; i < n; ++i)
     if (!frames[i] || (reinterpret_cast<uintptr_t>(frames[i]) & 3)) return fail(BEVK_ERR_ARG, "frame %zu null or not 4-byte aligned", i);
   long long stride = 0;
   if (c->tma_planned && affine_table(frames, n, &stride)) {
-    *src = stack_src(frames[0], stride);
+    *src = Frames(frames[0], stride);
     return BEVK_OK;
   }
   if (c->user_tab.size() != n || memcmp(c->user_tab.data(), frames, n * sizeof(void*)) != 0) {
@@ -1225,7 +1190,7 @@ static int frames_src(bevk_ctx* c, const void* const* frames, int batch, FrameSr
       return fail(BEVK_ERR_CUDA, "frame table upload: %s", cudaGetErrorString(e));
     }
   }
-  *src = table_src(c->d_user_ptrs.p);
+  *src = Frames(c->d_user_ptrs.p);
   return BEVK_OK;
 }
 
@@ -1233,7 +1198,7 @@ int bevk_bev_run_frames(bevk_ctx* c, const void* const* frames, int batch, const
   RET(use(c));
   if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
   if (!frames || !d_out) return fail(BEVK_ERR_ARG, "null pointer");
-  FrameSrc src;
+  Frames src;
   RET(frames_src(c, frames, batch, &src));
   c->timed = true;
   return run_device(c, src, batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
@@ -1250,7 +1215,7 @@ int bevk_bev_run_stack(bevk_ctx* c, const void* d_frames, int64_t frame_stride, 
   RET(use(c));
   RET(check_stack(c, d_frames, frame_stride));
   c->timed = true;
-  return run_device(c, stack_src(d_frames, frame_stride), batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
+  return run_device(c, Frames(d_frames, frame_stride), batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
 }
 
 int bevk_bev_run_stack_cams(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, int cam_lo, int cam_hi, void* d_out) {
@@ -1258,7 +1223,7 @@ int bevk_bev_run_stack_cams(bevk_ctx* c, const void* d_frames, int64_t frame_str
   RET(check_stack(c, d_frames, frame_stride));
   if (cam_lo < 0 || cam_hi > c->n_cam || cam_lo > cam_hi) return fail(BEVK_ERR_ARG, "bad camera range [%d,%d)", cam_lo, cam_hi);
   c->timed = true;
-  return run_device(c, stack_src(d_frames, frame_stride), batch, nullptr, 0, d_out, cam_lo, cam_hi);
+  return run_device(c, Frames(d_frames, frame_stride), batch, nullptr, 0, d_out, cam_lo, cam_hi);
 }
 
 int bevk_bev_last_path(bevk_ctx* c) { return c ? c->last_path : 0; }
@@ -1267,7 +1232,7 @@ int bevk_bev_run_device_cams(bevk_ctx* c, const void* d_srcs, int batch, int cam
   RET(use(c));
   if (cam_lo < 0 || cam_hi > c->n_cam || cam_lo > cam_hi) return fail(BEVK_ERR_ARG, "bad camera range [%d,%d)", cam_lo, cam_hi);
   c->timed = true;
-  return run_device(c, table_src(d_srcs), batch, nullptr, 0, d_out, cam_lo, cam_hi);
+  return run_device(c, Frames(d_srcs), batch, nullptr, 0, d_out, cam_lo, cam_hi);
 }
 
 int bevk_sat_sum_device(bevk_ctx* c, const void* const* parts, int n, uint64_t bytes, const void* d_car, void* d_out) {
@@ -1313,7 +1278,6 @@ static int ingest_setup(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_str
   h->chunk = chunk;
   const size_t set_frames = (size_t)c->n_cam;
   RET(c->d_frames.ensure(fpad * set_frames * chunk * 2));
-  RET(c->d_ptrs.ensure(sizeof(void*) * set_frames * chunk * 2));
   RET(c->d_canvas.ensure(cbytes * chunk * 2));
   if (!c->copy_stream) {
     CU(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
@@ -1326,13 +1290,6 @@ static int ingest_setup(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_str
   if (car) {
     RET(c->d_car.ensure(cbytes));
     CU(cudaMemcpyAsync(c->d_car.p, car, cbytes, cudaMemcpyHostToDevice, c->stream));
-  }
-  if (c->ptrs_for != c->d_frames.p || c->ptrs_tab != c->d_ptrs.p || c->ptrs_n != (long long)(set_frames * chunk * 2) || c->ptrs_pad != fpad) {
-    std::vector<const uint8_t*> ptrs(set_frames * chunk * 2);
-    for (size_t i = 0; i < ptrs.size(); ++i) ptrs[i] = c->d_frames.as<uint8_t>() + i * fpad;
-    CU(cudaMemcpyAsync(c->d_ptrs.p, ptrs.data(), ptrs.size() * sizeof(void*), cudaMemcpyHostToDevice, c->stream));
-    CU(cudaStreamSynchronize(c->stream));   // ptrs is a stack-lifetime staging vector
-    c->ptrs_for = c->d_frames.p; c->ptrs_tab = c->d_ptrs.p; c->ptrs_n = (long long)ptrs.size(); c->ptrs_pad = fpad;
   }
   // the copy stream must not start before work already queued on the main stream (e.g. the car upload,
   // or a previous call's D2H that still reads the canvases) has been ordered
@@ -1366,7 +1323,7 @@ static int ingest_setup(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_str
 // Frame-sets [b0, b0 + nb) into staging half `half` on the copy stream, and the main stream made to wait for them.  *fsrc:
 // the staged frames as run_device reads them (a frame stack, so the TMA-staged kernel serves them too).
 static int ingest_chunk(bevk_ctx* c, const HostIngest& h, const uint8_t* const* srcs, int64_t src_stride, int flags, int b0, int nb,
-                        int half, FrameSrc* fsrc) {
+                        int half, Frames* fsrc) {
   const size_t set_frames = (size_t)c->n_cam, row = h.row, fbytes = h.fbytes, fpad = h.fpad;
   const int chunk = h.chunk;
   uint8_t* dframes = c->d_frames.as<uint8_t>() + (size_t)half * chunk * set_frames * fpad;
@@ -1381,8 +1338,7 @@ static int ingest_chunk(bevk_ctx* c, const HostIngest& h, const uint8_t* const* 
     CU(cudaMemcpyAsync(dhp, hp, sizeof(void*) * nb * c->n_cam, cudaMemcpyHostToDevice, c->copy_stream));
     CU(cudaEventRecord(c->ev_hp[half], c->copy_stream));
     k_fetch_spans<<<dim3(c->FH, nb * c->n_cam), 128, 0, c->copy_stream>>>(
-        dhp, c->d_ptrs.as<uint8_t*>() + (size_t)half * chunk * set_frames, c->d_spans.as<int2>(), c->n_cam, c->FH,
-        (long long)src_stride, (int)row);
+        dhp, dframes, (long long)fpad, c->d_spans.as<int2>(), c->n_cam, c->FH, (long long)src_stride, (int)row);
     LAUNCHED(c);
     c->last_h2d_bytes += (long long)c->span_fetch_bytes * nb;
   }
@@ -1408,8 +1364,7 @@ static int ingest_chunk(bevk_ctx* c, const HostIngest& h, const uint8_t* const* 
   }
   CU(cudaEventRecord(c->ev_in[half], c->copy_stream));
   CU(cudaStreamWaitEvent(c->stream, c->ev_in[half], 0));
-  *fsrc = stack_src(dframes, (long long)fpad);
-  fsrc->table = c->d_ptrs.as<const uint8_t*>() + (size_t)half * chunk * set_frames;
+  *fsrc = Frames(dframes, (long long)fpad);
   return BEVK_OK;
 }
 
@@ -1424,7 +1379,7 @@ int bevk_bev_run(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, in
   int half = 0;
   for (int b0 = 0; b0 < batch; b0 += h.chunk, half ^= 1) {
     const int nb = std::min(h.chunk, batch - b0);
-    FrameSrc fsrc;
+    Frames fsrc;
     RET(ingest_chunk(c, h, srcs, src_stride, flags, b0, nb, half, &fsrc));
     c->timed = false;
     uint8_t* dcanvas = c->d_canvas.as<uint8_t>() + (size_t)half * h.chunk * h.cbytes;
@@ -1440,19 +1395,6 @@ int bevk_bev_run(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, in
 }
 
 // ------------------------------------------------------------------ stand-alone helpers
-static int ensure_hsv(bevk_ctx* c) {
-  if (c->d_hsv.p) return BEVK_OK;
-  std::vector<int> tab(512, 0);
-  for (int i = 1; i < 256; ++i) {
-    tab[i] = (int)std::nearbyint((255 << 12) / (1. * i));
-    tab[256 + i] = (int)std::nearbyint((180 << 12) / (6. * i));
-  }
-  RET(c->d_hsv.ensure(512 * sizeof(int)));
-  CU(cudaMemcpyAsync(c->d_hsv.p, tab.data(), 512 * sizeof(int), cudaMemcpyHostToDevice, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return BEVK_OK;
-}
-
 static int stream_blocks(const bevk_ctx* c, long long n_items) {
   return (int)std::max<long long>(1, std::min<long long>(c->n_sm * 8LL, (n_items + 255) / 256));
 }
@@ -1500,32 +1442,26 @@ int bevk_luminance_balance(bevk_ctx* c, const uint8_t* const* imgs, int n, int w
   const size_t fbytes = (size_t)w * h * 3, fpad = (fbytes + 255) & ~size_t(255);
   RET(c->s_src.ensure(fpad * n));
   RET(c->s_dst.ensure(fpad * n));
-  RET(c->d_ptrs.ensure(sizeof(void*) * 2 * BEVK_MAX_CAMERAS));
-  c->ptrs_for = nullptr;   // the BEV host path's cached pointer table is overwritten below
   RET(c->d_vsum.ensure(8 * n));
   RET(c->d_delta.ensure(4 * n));
-  const uint8_t* ptrs[2 * BEVK_MAX_CAMERAS];
+  uint8_t* const d_in = c->s_src.as<uint8_t>();
+  uint8_t* const d_out = c->s_dst.as<uint8_t>();
   for (int i = 0; i < n; ++i) {
     if (!imgs[i] || !outs[i]) return fail(BEVK_ERR_ARG, "null frame %d", i);
-    ptrs[i] = c->s_src.as<uint8_t>() + i * fpad;
-    ptrs[BEVK_MAX_CAMERAS + i] = c->s_dst.as<uint8_t>() + i * fpad;
-    CU(cudaMemcpyAsync(const_cast<uint8_t*>(ptrs[i]), imgs[i], fbytes, cudaMemcpyHostToDevice, c->stream));
+    CU(cudaMemcpyAsync(d_in + i * fpad, imgs[i], fbytes, cudaMemcpyHostToDevice, c->stream));
   }
-  CU(cudaMemcpyAsync(c->d_ptrs.p, ptrs, sizeof ptrs, cudaMemcpyHostToDevice, c->stream));
   CU(cudaMemsetAsync(c->d_vsum.p, 0, 8 * n, c->stream));
-  const uint8_t* const* d_in = c->d_ptrs.as<const uint8_t*>();
-  uint8_t* const* d_out = reinterpret_cast<uint8_t* const*>(c->d_ptrs.as<uint8_t*>() + BEVK_MAX_CAMERAS);
-  k_vsum<<<dim3(stream_blocks(c, fbytes / 48 + 1) / n + 1, n), 256, 0, c->stream>>>(d_in, (long long)fbytes,
+  k_vsum<<<dim3(stream_blocks(c, fbytes / 48 + 1) / n + 1, n), 256, 0, c->stream>>>(Frames(d_in, (long long)fpad), (long long)fbytes,
                                                                                  c->d_vsum.as<unsigned long long>(), CamRange{0, n, n});
   LAUNCHED(c);
   k_delta<<<1, 32, 0, c->stream>>>(c->d_vsum.as<unsigned long long>(), n, 1, 1, (double)w * (double)h, c->d_delta.as<int>());
   LAUNCHED(c);
-  k_lum_apply<<<dim3(stream_blocks(c, (long long)w * h) / n + 1, n), 256, 0, c->stream>>>(d_in, d_out, w, h, c->d_delta.as<int>(),
-                                                                                       c->d_hsv.as<int>());
+  k_lum_apply<<<dim3(stream_blocks(c, (long long)w * h) / n + 1, n), 256, 0, c->stream>>>(d_in, d_out, (long long)fpad, w, h,
+                                                                                       c->d_delta.as<int>(), c->d_hsv.as<int>());
   LAUNCHED(c);
   for (int i = 0; i < n; ++i)
-    CU(cudaMemcpyAsync(outs[i], ptrs[BEVK_MAX_CAMERAS + i], fbytes, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));   // also keeps the stack-resident ptrs[] alive long enough
+    CU(cudaMemcpyAsync(outs[i], d_out + i * fpad, fbytes, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
   return BEVK_OK;
 }
 
@@ -1652,7 +1588,7 @@ int bevk_shard_info(bevk_ctx* c, int rank, int* cam_lo, int* cam_hi, int32_t rec
 }
 
 // rank `as_rank`'s slabs of `batch` frame-sets into d_slabs[as_rank][batch][slab_bytes]
-static int shard_render(bevk_ctx* c, FrameSrc src, int batch, int as_rank, void* d_slabs) {
+static int shard_render(bevk_ctx* c, Frames src, int batch, int as_rank, void* d_slabs) {
   bevk_ctx::Shard& s = c->shard;
   const SlabRect q = s.rect[as_rank];
   uint8_t* dst = reinterpret_cast<uint8_t*>(d_slabs) + (size_t)as_rank * batch * s.slab_bytes;
@@ -1707,26 +1643,24 @@ static int shard_balance_limits(bevk_ctx* c, int batch) {
 
 // the V sums of rank `as_rank`'s own cameras into block as_rank of d_vsums[world][batch][n_cam], zero in the other
 // columns; other cameras' frames are never read
-static int shard_vsum(bevk_ctx* c, FrameSrc src, int batch, int as_rank, unsigned long long* d_vsums) {
+static int shard_vsum(bevk_ctx* c, Frames src, int batch, int as_rank, unsigned long long* d_vsums) {
   bevk_ctx::Shard& s = c->shard;
   const int lo = s.cam_lo[as_rank], hi = s.cam_hi[as_rank], nf = batch * c->n_cam;
   unsigned long long* blk = d_vsums + (size_t)as_rank * nf;
   CU(cudaMemsetAsync(blk, 0, (size_t)nf * 8, c->stream));
   if (hi <= lo) return BEVK_OK;   // a rank without cameras sends zeros
-  const void* table = src.table;
-  if (!table) RET(stack_table(c, src.base, src.stride, nf, &table));
-  launch_vsum(c, reinterpret_cast<const uint8_t* const*>(table), CamRange{lo, hi - lo, c->n_cam}, batch * (hi - lo), blk);
+  launch_vsum(c, src, CamRange{lo, hi - lo, c->n_cam}, batch * (hi - lo), blk);
   LAUNCHED(c);
   return BEVK_OK;
 }
 
 // rank `as_rank`'s slabs under BALANCE: luminance balance of its own cameras from the exchanged V sums, then the
 // ordinary windowed render of the balanced copies
-static int shard_render_balanced(bevk_ctx* c, FrameSrc src, int batch, int as_rank, const unsigned long long* d_vsums, void* d_slabs) {
+static int shard_render_balanced(bevk_ctx* c, Frames src, int batch, int as_rank, const unsigned long long* d_vsums, void* d_slabs) {
   bevk_ctx::Shard& s = c->shard;
   const SlabRect q = s.rect[as_rank];
   if (q.ox1 <= q.ox || s.cam_hi[as_rank] <= s.cam_lo[as_rank]) return BEVK_OK;
-  FrameSrc bal;
+  Frames bal;
   RET(balance_prepass(c, src, batch, s.cam_lo[as_rank], s.cam_hi[as_rank], d_vsums, s.world, &bal));
   return shard_render(c, bal, batch, as_rank, d_slabs);
 }
@@ -1738,7 +1672,7 @@ int bevk_shard_vsum(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int
   RET(shard_balance_limits(c, batch));
   if (as_rank < 0 || as_rank >= c->shard.world || as_rank >= SHARD_MAX_RANKS) return fail(BEVK_ERR_ARG, "rank %d out of range", as_rank);
   if (!d_vsums || (reinterpret_cast<uintptr_t>(d_vsums) & 7)) return fail(BEVK_ERR_ARG, "V-sum buffer null or not 8-byte aligned");
-  return shard_vsum(c, stack_src(d_frames, frame_stride), batch, as_rank, reinterpret_cast<unsigned long long*>(d_vsums));
+  return shard_vsum(c, Frames(d_frames, frame_stride), batch, as_rank, reinterpret_cast<unsigned long long*>(d_vsums));
 }
 
 int bevk_shard_render_balanced(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, int as_rank, const uint64_t* d_vsums,
@@ -1751,7 +1685,7 @@ int bevk_shard_render_balanced(bevk_ctx* c, const void* d_frames, int64_t frame_
   if (!d_vsums || (reinterpret_cast<uintptr_t>(d_vsums) & 7)) return fail(BEVK_ERR_ARG, "V-sum buffer null or not 8-byte aligned");
   if (!d_slabs || (reinterpret_cast<uintptr_t>(d_slabs) & 15)) return fail(BEVK_ERR_ARG, "slab buffer null or not 16-byte aligned");
   c->timed = true;
-  return shard_render_balanced(c, stack_src(d_frames, frame_stride), batch, as_rank,
+  return shard_render_balanced(c, Frames(d_frames, frame_stride), batch, as_rank,
                                reinterpret_cast<const unsigned long long*>(d_vsums), d_slabs);
 }
 
@@ -1770,7 +1704,7 @@ int bevk_shard_render(bevk_ctx* c, const void* d_frames, int64_t frame_stride, i
   if (as_rank < 0 || as_rank >= c->shard.world || as_rank >= SHARD_MAX_RANKS) return fail(BEVK_ERR_ARG, "rank %d out of range", as_rank);
   if (!d_slabs || (reinterpret_cast<uintptr_t>(d_slabs) & 15)) return fail(BEVK_ERR_ARG, "slab buffer null or not 16-byte aligned");
   c->timed = true;
-  return shard_render(c, stack_src(d_frames, frame_stride), batch, as_rank, d_slabs);
+  return shard_render(c, Frames(d_frames, frame_stride), batch, as_rank, d_slabs);
 }
 
 int bevk_shard_compose(bevk_ctx* c, const void* d_slabs, int batch, const void* d_car, void* d_out) {
@@ -1782,7 +1716,7 @@ int bevk_shard_compose(bevk_ctx* c, const void* d_slabs, int batch, const void* 
 
 // this rank's V sums into its block of s.d_vsums, then one in-place all-gather of the blocks (none in a world of one);
 // *received: the bytes that came from the other ranks
-static int shard_exchange_vsums(bevk_ctx* c, FrameSrc src, int batch, long long* received) {
+static int shard_exchange_vsums(bevk_ctx* c, Frames src, int batch, long long* received) {
   bevk_ctx::Shard& s = c->shard;
   const size_t blk = (size_t)batch * c->n_cam * 8;
   RET(s.d_vsums.ensure(blk * s.world));
@@ -1804,13 +1738,13 @@ int bevk_bev_run_sharded(bevk_ctx* c, const void* d_frames, int64_t frame_stride
   s.last_link_bytes = 0;
   if (s.policy == BEVK_SHARD_FRAMES || s.world == 1) {   // every rank renders its own frame-sets: no exchange
     c->timed = true;
-    return run_device(c, stack_src(d_frames, frame_stride), batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
+    return run_device(c, Frames(d_frames, frame_stride), batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
   }
   const bool bal = (flags & BEVK_FLAG_BALANCE) != 0;
   if (bal) RET(shard_balance_limits(c, batch));
   if (!s.comm) return fail(BEVK_ERR_ARG, "bevk_shard_connect not called");
   RET(shard_geometry(c));
-  const FrameSrc src = stack_src(d_frames, frame_stride);
+  const Frames src = Frames(d_frames, frame_stride);
   const size_t per_rank = (size_t)batch * s.slab_bytes;
   RET(s.d_slabs.ensure(per_rank * s.world));
   c->timed = false;
@@ -1898,7 +1832,7 @@ int bevk_bev_run_scattered(bevk_ctx* c, const void* d_frames, int64_t frame_stri
   if (mine > 0 && !d_out_own) return fail(BEVK_ERR_ARG, "null output");
   const size_t half = (size_t)s.world * s.own_max * s.slab_bytes, rank_stride = (size_t)s.own_max * s.slab_bytes;
   const SlabRect q = s.rect[s.rank];
-  const FrameSrc src = stack_src(d_frames, frame_stride);
+  const Frames src = Frames(d_frames, frame_stride);
   s.last_link_bytes = 0;
   c->timed = false;
   long long vsum_bytes = 0;
@@ -1909,7 +1843,7 @@ int bevk_bev_run_scattered(bevk_ctx* c, const void* d_frames, int64_t frame_stri
     w.pitch = (q.ox1 - q.ox) * 3; w.ox = q.ox; w.oy = q.oy; w.ox1 = q.ox1; w.oy1 = q.oy1; w.stride = s.slab_bytes;
     w.world = s.world; w.src_off = (long long)(par * half + (size_t)s.rank * rank_stride);
     for (int r = 0; r < s.world; ++r) w.peer[r] = reinterpret_cast<uint8_t*>(s.peer_recv[r]);
-    FrameSrc rsrc = src;   // BALANCE: the peer-store render reads this rank's balanced copies
+    Frames rsrc = src;   // BALANCE: the peer-store render reads this rank's balanced copies
     if (bal) RET(balance_prepass(c, src, batch, s.cam_lo[s.rank], s.cam_hi[s.rank], s.d_vsums.as<unsigned long long>(), s.world, &rsrc));
     RET(run_device(c, rsrc, batch, nullptr, 0, nullptr, s.cam_lo[s.rank], s.cam_hi[s.rank], &w));
     s.last_link_bytes = (long long)(batch - mine) * s.slab_bytes;   // what this rank stored into its peers
@@ -2017,7 +1951,7 @@ int bevk_bev_run_jpeg(bevk_ctx* c, const uint8_t* const* jpegs, const uint64_t* 
     CU(cudaMemcpyAsync(c->d_car.p, car, cbytes, cudaMemcpyHostToDevice, c->stream));
   }
   c->timed = false;
-  RET(run_device(c, stack_src(c->d_jpeg_frames.p, (long long)fpad), batch, car ? c->d_car.p : nullptr, flags, c->d_jpeg_canvas.p, 0,
+  RET(run_device(c, Frames(c->d_jpeg_frames.p, (long long)fpad), batch, car ? c->d_car.p : nullptr, flags, c->d_jpeg_canvas.p, 0,
                  BEVK_MAX_CAMERAS));
   CU(cudaMemcpyAsync(out, c->d_jpeg_canvas.p, cbytes * batch, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaStreamSynchronize(c->stream));
@@ -2216,7 +2150,7 @@ int bevk_bev_run_to_jpeg(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_st
   int half = 0, prev_b0 = -1, prev_nb = 0;
   for (int b0 = 0; b0 < batch; b0 += h.chunk, half ^= 1) {
     const int nb = std::min(h.chunk, batch - b0);
-    FrameSrc fsrc;
+    Frames fsrc;
     RET(ingest_chunk(c, h, srcs, src_stride, flags, b0, nb, half, &fsrc));
     c->timed = false;
     uint8_t* dcanvas = c->d_canvas.as<uint8_t>() + (size_t)half * h.chunk * h.cbytes;
@@ -2237,7 +2171,7 @@ int bevk_bev_frames_to_jpeg(bevk_ctx* c, const void* const* frames, int batch, c
   RET(use(c));
   RET(to_jpeg_check(c, out, sizes));
   if (!frames) return fail(BEVK_ERR_ARG, "null pointer");
-  FrameSrc src;
+  Frames src;
   RET(frames_src(c, frames, batch, &src));
   // chunks of frame-sets rendered into one canvas scratch and encoded there, chunk i's streams copied out while chunk
   // i+1 is rendered and encoded.  8 canvases (24 MB at 1000^2: they stay in the 50 MB L2) beat the whole batch at once
@@ -2252,9 +2186,9 @@ int bevk_bev_frames_to_jpeg(bevk_ctx* c, const void* const* frames, int batch, c
   int slot = 0, prev_b0 = -1, prev_nb = 0;
   for (int b0 = 0; b0 < batch; b0 += chunk, slot ^= 1) {
     const int nb = std::min(chunk, batch - b0);
-    FrameSrc part = src;
-    if (part.base) part.base += (long long)b0 * c->n_cam * part.stride;
-    else part.table = reinterpret_cast<const uint8_t* const*>(part.table) + (size_t)b0 * c->n_cam;
+    Frames part = src;
+    if (part.table) part.table += (size_t)b0 * c->n_cam;
+    else part.base += (long long)b0 * c->n_cam * part.stride;
     c->timed = false;
     RET(run_device(c, part, nb, d_car, flags | kFlagRawBalance, dcanvas, 0, BEVK_MAX_CAMERAS));
     RET(jpeg_enqueue(c, slot, canvas_in(c, dcanvas, flags, d_car), nb, c->BW, c->BH, quality));

@@ -43,7 +43,7 @@ struct BevItem {
 };
 
 struct BevParams {
-  const uint8_t* const* srcs;   // device array [batch * n_cam] of dense BGR frames
+  Frames srcs;                  // the batch * n_cam dense BGR frames
   int n_cam, FW, FH;
   unsigned pitch;               // source row pitch in bytes (= 3*FW)
   const int4* tiles;            // x0, y0, first item, item count
@@ -188,7 +188,7 @@ __global__ void __launch_bounds__(256, BEVK_MIN_CTAS) k_bev(BevParams P) {
 #pragma unroll
       for (int j = 0; j < NB; ++j) {
         const int b = b0 + (j < nb ? j : 0);   // j >= nb aliases frame-set b0: computed, never written out
-        src[j] = P.srcs[b * P.n_cam + item.cam];
+        src[j] = P.srcs.frame(b * P.n_cam + item.cam);
       }
       const int pos = item.orient ? posy : posx, step = item.orient ? stepy : stepx;
       uint4 nxt = __ldg(L);

@@ -14,6 +14,19 @@ namespace bevk {
 constexpr int INTER_BITS = 5;
 constexpr int TAB = 32;
 
+// Where the frames of a call live, for the host and the kernels alike: a frame STACK (frame i at base + i * stride), or a
+// device table of frame pointers for frames that really are scattered.  Kernels take it by value, so a captured CUDA
+// graph keeps the addresses it was captured with.
+struct Frames {
+  const uint8_t* const* table = nullptr;
+  const uint8_t* base = nullptr;
+  long long stride = 0;
+  Frames() = default;
+  explicit Frames(const void* d_table) : table(static_cast<const uint8_t* const*>(d_table)) {}
+  Frames(const void* d_base, long long frame_stride) : base(static_cast<const uint8_t*>(d_base)), stride(frame_stride) {}
+  __host__ __device__ __forceinline__ const uint8_t* frame(long long i) const { return table ? table[i] : base + i * stride; }
+};
+
 struct CamModel {      // cv2.fisheye / cv2 initUndistortRectifyMap inputs, pre-digested on the host
   double iR[9];        // inv(P * R), R = I
   double k[5];         // fisheye: k1..k4 ; pinhole: k1,k2,p1,p2,k3

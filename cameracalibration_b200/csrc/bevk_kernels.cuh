@@ -283,11 +283,11 @@ __device__ __forceinline__ unsigned vsum_16px(const uint4 a, const uint4 b, cons
 struct CamRange { int lo, n, n_cam; };
 __host__ __device__ __forceinline__ int range_frame(CamRange r, int i) { return (i / r.n) * r.n_cam + r.lo + i % r.n; }
 
-// grid y = frames of the range; vsum[frame] += its V sum
-__global__ void __launch_bounds__(256) k_vsum(const uint8_t* const* __restrict__ frames, long long frame_bytes,
-                                              unsigned long long* __restrict__ vsum, CamRange cr) {
+// grid y = frames of the range; vsum[frame] += its V sum.  A streaming reduction: 8 CTAs (a full SM of threads) per SM.
+__global__ void __launch_bounds__(256, 8) k_vsum(Frames frames, long long frame_bytes, unsigned long long* __restrict__ vsum,
+                                                 CamRange cr) {
   const int fi = range_frame(cr, blockIdx.y);
-  const uint8_t* f = frames[fi];
+  const uint8_t* f = frames.frame(fi);
   const long long n48 = frame_bytes / 48;
   unsigned long long acc = 0;
   if ((reinterpret_cast<uintptr_t>(f) & 15) == 0) {
@@ -480,15 +480,15 @@ __global__ void __launch_bounds__(256) k_chan_sum(const uint8_t* __restrict__ im
   if ((threadIdx.x & 31) == 0) { atomicAdd(csum, sb); atomicAdd(csum + 1, sg); atomicAdd(csum + 2, sr); }
 }
 
-// grid.y = frame index; delta[frame] from k_delta
-__global__ void __launch_bounds__(256) k_lum_apply(const uint8_t* const* __restrict__ frames, uint8_t* const* __restrict__ outs,
+// grid.y = frame index; frame i of the input and output stacks at in / out + i * frame_stride; delta[frame] from k_delta
+__global__ void __launch_bounds__(256) k_lum_apply(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, long long frame_stride,
                                                    int w, int h, const int* __restrict__ delta,
                                                    const int* __restrict__ hsv_tab) {
   __shared__ int s_tab[512];
   for (int i = threadIdx.x; i < 512; i += 256) s_tab[i] = hsv_tab[i];
   __syncthreads();
-  const uint8_t* f = frames[blockIdx.y];
-  uint8_t* o = outs[blockIdx.y];
+  const uint8_t* f = in + blockIdx.y * frame_stride;
+  uint8_t* o = out + blockIdx.y * frame_stride;
   const int d = delta[blockIdx.y], tail = w - (w % 32);
   const long long npx = (long long)w * h;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < npx; i += (long long)gridDim.x * blockDim.x) {
@@ -510,15 +510,18 @@ constexpr int LUM_ROWS = 16;   // source rows per CTA
 // One CTA converts the sampled spans of LUM_ROWS consecutive source rows of one frame.  The work items -- groups of 4
 // pixels = 3 aligned words in, 3 out -- of all its rows form ONE flat list (prefix sums of the rows' group counts in shared
 // memory) that the threads stride through, so that a row with a short span costs nothing and every thread has several
-// independent groups in flight; the sector selection of hsv_roundtrip is branch-free.
-__global__ void __launch_bounds__(128) k_lum_spans(const uint8_t* const* __restrict__ frames, uint8_t* const* __restrict__ outs,
+// independent groups in flight; the sector selection of hsv_roundtrip is branch-free.  Frame f's balanced copy goes to
+// out_base + f * out_stride.
+__global__ void __launch_bounds__(128) k_lum_spans(Frames in, uint8_t* __restrict__ out_base, long long out_stride,
                                                    const int2* __restrict__ spans, CamRange cr, int w, int h,
                                                    const int* __restrict__ delta, const int* __restrict__ hsv_tab) {
   const int f = range_frame(cr, blockIdx.y), y0 = blockIdx.x * LUM_ROWS, y1 = min(h, y0 + LUM_ROWS), nrows = y1 - y0;
   const int2* sp_cam = spans + (size_t)(f % cr.n_cam) * h;
+  const uint8_t* const frame = in.frame(f);
+  uint8_t* const out = out_base + f * out_stride;
   __shared__ int s_tab[512];
   __shared__ int s_pref[LUM_ROWS + 1], s_g0[LUM_ROWS];
-  const bool words = (w & 3) == 0 && ((reinterpret_cast<uintptr_t>(frames[f]) | reinterpret_cast<uintptr_t>(outs[f])) & 3) == 0;
+  const bool words = (w & 3) == 0 && ((reinterpret_cast<uintptr_t>(frame) | reinterpret_cast<uintptr_t>(out)) & 3) == 0;
   if (threadIdx.x == 0) {
     // groups cover each span rounded out to multiples of 4 pixels: the extra pixels are converted too, which nobody samples
     int acc = 0;
@@ -537,8 +540,8 @@ __global__ void __launch_bounds__(128) k_lum_spans(const uint8_t* const* __restr
   const int d = delta[f], tail = w - (w % 32);
   if (words) {
     const size_t row_words = (size_t)w * 3 / 4;
-    const unsigned* src0 = reinterpret_cast<const unsigned*>(frames[f]) + (size_t)y0 * row_words;
-    unsigned* dst0 = reinterpret_cast<unsigned*>(outs[f]) + (size_t)y0 * row_words;
+    const unsigned* src0 = reinterpret_cast<const unsigned*>(frame) + (size_t)y0 * row_words;
+    unsigned* dst0 = reinterpret_cast<unsigned*>(out) + (size_t)y0 * row_words;
     int r = 0;
 #pragma unroll 2
     for (int i = threadIdx.x; i < total; i += 128) {
@@ -560,8 +563,8 @@ __global__ void __launch_bounds__(128) k_lum_spans(const uint8_t* const* __restr
   } else {
     for (int y = y0; y < y1; ++y) {
       const int2 sp = sp_cam[y];
-      const uint8_t* src = frames[f] + (size_t)y * w * 3;
-      uint8_t* dst = outs[f] + (size_t)y * w * 3;
+      const uint8_t* src = frame + (size_t)y * w * 3;
+      uint8_t* dst = out + (size_t)y * w * 3;
       for (int x = sp.x + threadIdx.x; x < sp.y; x += 128) {
         int b = src[3 * x], g = src[3 * x + 1], r = src[3 * x + 2];
         hsv_roundtrip(b, g, r, d, x >= tail, s_tab, s_tab + 256);
@@ -575,18 +578,19 @@ __global__ void __launch_bounds__(128) k_lum_spans(const uint8_t* const* __restr
 // Host -> device ingest for page-locked (mapped) host frames: instead of DMA rectangles, the SMs
 // read exactly the sampled row spans of every frame straight out of host memory (zero-copy, 16-byte
 // vectors, coalesced) and write them into the device frame buffers.  Moves ~17 % of each frame
-// over PCIe instead of the 23-34 % a band / bounding-box DMA needs.  grid = (FH, n_frames).
+// over PCIe instead of the 23-34 % a band / bounding-box DMA needs.  grid = (FH, n_frames); frame f goes to
+// dev_frames + f * dev_stride.
 // ---------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) k_fetch_spans(const uint8_t* const* __restrict__ host_frames, uint8_t* const* __restrict__ dev_frames,
-                                                     const int2* __restrict__ spans, int n_cam, int h, long long host_stride,
-                                                     int row_bytes) {
+__global__ void __launch_bounds__(128) k_fetch_spans(const uint8_t* const* __restrict__ host_frames, uint8_t* __restrict__ dev_frames,
+                                                     long long dev_stride, const int2* __restrict__ spans, int n_cam, int h,
+                                                     long long host_stride, int row_bytes) {
   const int y = blockIdx.x, f = blockIdx.y;
   const int2 sp = spans[(f % n_cam) * h + y];
   if (sp.y <= sp.x) return;
   // 16-byte window around the span (+4 px each side for the aligned word reads of the gather)
   const int b0 = max(0, 3 * sp.x - 12) & ~15, b1 = min(row_bytes, (3 * sp.y + 12 + 15) & ~15);
   const uint4* src = reinterpret_cast<const uint4*>(host_frames[f] + (size_t)y * host_stride + b0);
-  uint4* dst = reinterpret_cast<uint4*>(dev_frames[f] + (size_t)y * row_bytes + b0);
+  uint4* dst = reinterpret_cast<uint4*>(dev_frames + f * dev_stride + (size_t)y * row_bytes + b0);
   for (int i = threadIdx.x; i < (b1 - b0) >> 4; i += 128) dst[i] = src[i];
 }
 
