@@ -15,6 +15,8 @@ INTER_NEAREST, INTER_LINEAR = 0, 1
 MAPS_UNDISTORT, MAPS_BEV = 0, 1
 MODEL_FISHEYE, MODEL_PINHOLE = 0, 1
 FLAG_BALANCE = 1
+FLAG_NV12, FLAG_I420 = 2, 4          # YUV 4:2:0 frames (cv2's single-buffer layout), bevk_bev_run / _run_stack only
+PIXEL_FORMATS = {"bgr": 0, "nv12": FLAG_NV12, "i420": FLAG_I420}
 SHARD_FRAMES, SHARD_CAMERAS = 0, 1
 MAX_CAMERAS = 8
 

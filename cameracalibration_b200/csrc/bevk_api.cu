@@ -157,6 +157,11 @@ struct bevk_ctx {
   long long span_fetch_bytes = 0;           // bytes k_fetch_spans moves per frame-set
   long long last_h2d_bytes = 0;             // host->device bytes of the last bevk_bev_run call
   int cam_box[BEVK_MAX_CAMERAS][BEVK_MAX_BANDS][4] = {};   // per camera and band: sampled rows [y0,y1), bytes [bx0,bx1)
+  // YUV sources, per format (NV12, I420): page-locked ingest windows [camera][FH*3/2] and their bytes per frame-set, and
+  // the DMA rectangles of pageable frames per camera
+  DevBuf d_yuv_win[2];
+  long long yuv_fetch_bytes[2] = {0, 0};
+  std::vector<int4> yuv_rects[2][BEVK_MAX_CAMERAS];
   DevBuf d_tiles, d_items, d_lut, d_hsv;
   int bev_grid[6] = {0, 0, 0, 0, 0, 0};   // resident CTAs of k_bev<BAL, NB>: index = 3*BAL + {NB=1:0, 4:1, 8:2}
   DevBuf d_frames, d_canvas, d_car, d_vsum, d_delta, d_csum;
@@ -812,6 +817,20 @@ int bevk_bev_finalize(bevk_ctx* c) {
   c->n_bands = 2;
   if (const char* env = getenv("BEVK_BANDS")) c->n_bands = std::max(1, std::min(BEVK_MAX_BANDS, atoi(env)));
   for (int k = 0; k < NC; ++k) plan_bands(spans.data() + (size_t)k * FH, FW, FH, c->n_bands, c->cam_box[k]);
+  if (FW % 2 == 0 && FH % 2 == 0) {   // YUV 4:2:0 ingest of the same spans (odd sizes: YUV calls are refused)
+    const int rows = FH * 3 / 2;
+    std::vector<int4> win((size_t)NC * rows);
+    for (int fmt = YUV_NV12; fmt <= YUV_I420; ++fmt) {
+      for (int k = 0; k < NC; ++k) {
+        yuv_windows(fmt, spans.data() + (size_t)k * FH, FW, FH, win.data() + (size_t)k * rows);
+        yuv_dma_rects(fmt, c->cam_box[k], c->n_bands, FW, FH, c->yuv_rects[fmt - 1][k]);
+      }
+      c->yuv_fetch_bytes[fmt - 1] = yuv_window_bytes(win.data(), NC * rows);
+      RET(c->d_yuv_win[fmt - 1].ensure(win.size() * sizeof(int4)));
+      CU(cudaMemcpyAsync(c->d_yuv_win[fmt - 1].p, win.data(), win.size() * sizeof(int4), cudaMemcpyHostToDevice, c->stream));
+      CU(cudaStreamSynchronize(c->stream));   // win is reused for the next format
+    }
+  }
   RET(ensure_hsv(c));
   CU(cudaStreamSynchronize(c->stream));
   // ---- the TMA-staged kernel's plan (frames whose row pitch is a multiple of 16 bytes)
@@ -914,12 +933,35 @@ int bevk_bev_tma_plan_info(bevk_ctx* c, int64_t* n_items, int64_t* n_shapes, int
 
 int64_t bevk_bev_last_h2d_bytes(bevk_ctx* c) { return c ? c->last_h2d_bytes : 0; }
 
+// Source pixel format of a call from its flags: 0 = BGR, YUV_NV12, YUV_I420.  YUV needs even frame sizes, as cv2 does.
+static int pixel_format(bevk_ctx* c, int flags, int* fmt) {
+  const int yuv = flags & (BEVK_FLAG_NV12 | BEVK_FLAG_I420);
+  *fmt = 0;
+  if (!yuv) return BEVK_OK;
+  if (yuv == (BEVK_FLAG_NV12 | BEVK_FLAG_I420)) return fail(BEVK_ERR_ARG, "BEVK_FLAG_NV12 and BEVK_FLAG_I420 are exclusive");
+  if ((c->FW | c->FH) & 1) return fail(BEVK_ERR_UNSUPPORTED, "YUV 4:2:0 frames need an even size, not %d x %d", c->FW, c->FH);
+  *fmt = yuv == BEVK_FLAG_NV12 ? YUV_NV12 : YUV_I420;
+  return BEVK_OK;
+}
+
+// Entry points that read BGR frames only refuse the YUV flags rather than read a YUV buffer as BGR.
+static int bgr_only(int flags, const char* fn) {
+  if (flags & (BEVK_FLAG_NV12 | BEVK_FLAG_I420)) return fail(BEVK_ERR_UNSUPPORTED, "%s takes BGR frames only (no YUV flags)", fn);
+  return BEVK_OK;
+}
+
 int bevk_bev_host_copy_bytes(bevk_ctx* c, int flags, int64_t* h2d, int64_t* d2h) {
   RET(use(c));
   if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
+  int fmt = 0;
+  RET(pixel_format(c, flags, &fmt));
   int64_t up = 0;
   for (int k = 0; k < c->n_cam; ++k) {
-    if (flags & BEVK_FLAG_BALANCE) { up += (int64_t)c->FW * c->FH * 3; continue; }
+    if (flags & BEVK_FLAG_BALANCE) { up += (int64_t)c->FW * c->FH * (fmt ? 3 : 6) / 2; continue; }
+    if (fmt) {
+      for (const int4& r : c->yuv_rects[fmt - 1][k]) up += (int64_t)r.y * r.w;
+      continue;
+    }
     for (int bnd = 0; bnd < c->n_bands; ++bnd)
       up += (int64_t)(c->cam_box[k][bnd][1] - c->cam_box[k][bnd][0]) * (c->cam_box[k][bnd][3] - c->cam_box[k][bnd][2]);
   }
@@ -1065,6 +1107,42 @@ static int balance_prepass(bevk_ctx* c, Frames src, int batch, int lo, int hi, c
   return BEVK_OK;
 }
 
+// YUV pre-pass of the fused render: the sampled spans of every frame converted to BGR (and, with BALANCE, balanced) into
+// the copy stack d_bal, laid out as balance_prepass leaves it; *bgr_src describes it.  With BALANCE the V sums come from
+// k_vsum_yuv over the whole converted frames first.  The caller checks batch * n_cam <= 65535.
+template <int FMT>
+static int yuv_prepass_fmt(bevk_ctx* c, Frames src, int batch, bool bal, Frames* bgr_src) {
+  const int nf = batch * c->n_cam;
+  const CamRange cr{0, c->n_cam, c->n_cam};
+  if (bal) {
+    RET(c->d_delta.ensure((size_t)nf * 4));
+    RET(c->d_vsum.ensure((size_t)nf * 8));
+    CU(cudaMemsetAsync(c->d_vsum.p, 0, (size_t)nf * 8, c->stream));
+    const int blocks = std::max(1, std::min(c->FH / 2, c->n_sm * 4 / std::max(1, std::min(nf, 64)) + 1));
+    k_vsum_yuv<FMT><<<dim3(blocks, nf), 256, 0, c->stream>>>(src, c->FW, c->FH, c->d_vsum.as<unsigned long long>(), cr);
+    LAUNCHED(c);
+    k_delta<<<(batch + 127) / 128, 128, 0, c->stream>>>(c->d_vsum.as<unsigned long long>(), c->n_cam, batch, 1,
+                                                         (double)c->FW * (double)c->FH, c->d_delta.as<int>());
+    LAUNCHED(c);
+  }
+  const size_t fpad = ((size_t)c->FW * 3 * c->FH + 255) & ~size_t(255);
+  RET(c->d_bal.ensure(fpad * nf));
+  const dim3 grid((c->FH + LUM_ROWS - 1) / LUM_ROWS, nf);
+  if (bal)
+    k_yuv_spans<FMT, true><<<grid, 128, 0, c->stream>>>(src, c->d_bal.as<uint8_t>(), (long long)fpad, c->d_spans.as<int2>(), cr,
+                                                        c->FW, c->FH, c->d_delta.as<int>(), c->d_hsv.as<int>());
+  else
+    k_yuv_spans<FMT, false><<<grid, 128, 0, c->stream>>>(src, c->d_bal.as<uint8_t>(), (long long)fpad, c->d_spans.as<int2>(), cr,
+                                                         c->FW, c->FH, nullptr, nullptr);
+  LAUNCHED(c);
+  *bgr_src = Frames(c->d_bal.p, (long long)fpad);
+  return BEVK_OK;
+}
+
+static int yuv_prepass(bevk_ctx* c, int fmt, Frames src, int batch, bool bal, Frames* bgr_src) {
+  return fmt == YUV_NV12 ? yuv_prepass_fmt<YUV_NV12>(c, src, batch, bal, bgr_src) : yuv_prepass_fmt<YUV_I420>(c, src, batch, bal, bgr_src);
+}
+
 // run_device flag, not part of the ABI: with BALANCE, stop at the raw composed canvas and its channel sums (d_csum).  The
 // encoder's GainSrc applies the gains and the car, so k_gain does not run.  (Without BALANCE the write-out adds the car.)
 constexpr int kFlagRawBalance = 1 << 30;
@@ -1077,7 +1155,11 @@ static int run_device(bevk_ctx* c, Frames src, int batch, const void* d_car, int
   if (batch < 1 || batch > 65535) return fail(BEVK_ERR_ARG, "batch %d out of range [1,65535]", batch);
   const bool bal = (flags & BEVK_FLAG_BALANCE) != 0;
   const int nf = batch * c->n_cam;
-  if (bal && nf > 65535) return fail(BEVK_ERR_ARG, "batch %d x %d cameras exceeds the 65535 frames of a BALANCE call", batch, c->n_cam);
+  int fmt = 0;
+  RET(pixel_format(c, flags, &fmt));
+  if ((bal || fmt) && nf > 65535)
+    return fail(BEVK_ERR_ARG, "batch %d x %d cameras exceeds the 65535 frames of a BALANCE or YUV call", batch, c->n_cam);
+  if (fmt && (win || cam_lo != 0 || cam_hi < c->n_cam)) return fail(BEVK_ERR_UNSUPPORTED, "YUV frames render whole canvases only");
   BevParams P{};
   P.n_cam = c->n_cam; P.FW = c->FW; P.FH = c->FH; P.pitch = (unsigned)c->FW * 3u;
   P.tiles = c->d_tiles.as<int4>(); P.items = c->d_items.as<BevItem>(); P.lut = c->d_lut.as<uint4>();
@@ -1099,9 +1181,10 @@ static int run_device(bevk_ctx* c, Frames src, int batch, const void* d_car, int
   if (bal) {
     RET(c->d_csum.ensure((size_t)batch * 24));
     CU(cudaMemsetAsync(c->d_csum.p, 0, (size_t)batch * 24, c->stream));
-    RET(balance_prepass(c, src, batch, 0, c->n_cam, nullptr, 1, &gsrc));
+    if (!fmt) RET(balance_prepass(c, src, batch, 0, c->n_cam, nullptr, 1, &gsrc));
     P.csum = c->d_csum.as<unsigned long long>();
   }
+  if (fmt) RET(yuv_prepass(c, fmt, src, batch, bal, &gsrc));   // BGR copies of the sampled spans (balanced with BALANCE)
   // TMA-staged kernel for frame stacks (16-byte aligned base and stride); global-offset gather otherwise
   const bool use_tma = c->tma_planned && !gsrc.table && (reinterpret_cast<uintptr_t>(gsrc.base) & 15) == 0 && (gsrc.stride & 15) == 0 &&
                        gsrc.stride >= (long long)P.pitch * c->FH && (nbu == 1 || nbu == 4);
@@ -1152,6 +1235,7 @@ static int run_device(bevk_ctx* c, Frames src, int batch, const void* d_car, int
 
 int bevk_bev_run_device(bevk_ctx* c, const void* d_srcs, int batch, const void* d_car, int flags, void* d_out) {
   RET(use(c));
+  RET(bgr_only(flags, "bevk_bev_run_device"));
   c->timed = true;
   return run_device(c, Frames(d_srcs), batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
 }
@@ -1198,6 +1282,7 @@ int bevk_bev_run_frames(bevk_ctx* c, const void* const* frames, int batch, const
   RET(use(c));
   if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
   if (!frames || !d_out) return fail(BEVK_ERR_ARG, "null pointer");
+  RET(bgr_only(flags, "bevk_bev_run_frames"));
   Frames src;
   RET(frames_src(c, frames, batch, &src));
   c->timed = true;
@@ -1213,7 +1298,15 @@ static int check_stack(bevk_ctx* c, const void* d_frames, int64_t frame_stride) 
 
 int bevk_bev_run_stack(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, const void* d_car, int flags, void* d_out) {
   RET(use(c));
-  RET(check_stack(c, d_frames, frame_stride));
+  int fmt = 0;
+  RET(pixel_format(c, flags, &fmt));
+  if (fmt) {   // YUV frames are read byte- or word-wise by k_vsum_yuv / k_yuv_spans only: any base and stride will do
+    if (!d_frames) return fail(BEVK_ERR_ARG, "null frame stack");
+    if (frame_stride < (int64_t)c->FW * c->FH * 3 / 2)
+      return fail(BEVK_ERR_ARG, "frame_stride %lld smaller than a YUV 4:2:0 frame", (long long)frame_stride);
+  } else {
+    RET(check_stack(c, d_frames, frame_stride));
+  }
   c->timed = true;
   return run_device(c, Frames(d_frames, frame_stride), batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
 }
@@ -1256,6 +1349,7 @@ int bevk_sat_sum_device(bevk_ctx* c, const void* const* parts, int n, uint64_t b
 // call of bevk_bev_run / bevk_bev_run_to_jpeg shares between its chunks.
 struct HostIngest {
   size_t row = 0, fbytes = 0, fpad = 0, cbytes = 0;
+  int fmt = 0, rows = 0;                  // pixel format (0 = BGR) and buffer rows of a frame (FH; FH * 3 / 2 for YUV)
   int chunk = 0;
   bool zero_copy = false;
   std::vector<const uint8_t*> dev_view;   // zero-copy: device views of the page-locked frames
@@ -1266,10 +1360,14 @@ static int ingest_setup(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_str
   if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
   if (!srcs) return fail(BEVK_ERR_ARG, "null host pointer");
   if (batch < 1) return fail(BEVK_ERR_ARG, "batch must be >= 1");
-  const size_t row = (size_t)c->FW * 3, fbytes = row * c->FH, fpad = (fbytes + 255) & ~size_t(255);
+  int fmt = 0;
+  RET(pixel_format(c, flags, &fmt));
+  // a YUV frame is uint8[FH * 3 / 2][FW] at the same row stride; it is staged as it is and converted on the device
+  const int rows = fmt ? c->FH * 3 / 2 : c->FH;
+  const size_t row = (size_t)c->FW * (fmt ? 1 : 3), fbytes = row * rows, fpad = (fbytes + 255) & ~size_t(255);
   if (src_stride < (int64_t)row) return fail(BEVK_ERR_ARG, "src_stride %lld < row bytes", (long long)src_stride);
   const size_t cbytes = (size_t)c->BW * c->BH * 3;
-  h->row = row; h->fbytes = fbytes; h->fpad = fpad; h->cbytes = cbytes;
+  h->row = row; h->fbytes = fbytes; h->fpad = fpad; h->cbytes = cbytes; h->fmt = fmt; h->rows = rows;
   // Two-deep pipeline over chunks of frame-sets: the H2D copies of chunk i+1 run on the copy
   // stream while chunk i is rendered and its canvases go back on the main stream, so the two
   // PCIe directions overlap and the kernel hides under the copies.
@@ -1337,10 +1435,16 @@ static int ingest_chunk(bevk_ctx* c, const HostIngest& h, const uint8_t* const* 
     const uint8_t** dhp = c->d_hptrs.as<const uint8_t*>() + (size_t)half * chunk * set_frames;
     CU(cudaMemcpyAsync(dhp, hp, sizeof(void*) * nb * c->n_cam, cudaMemcpyHostToDevice, c->copy_stream));
     CU(cudaEventRecord(c->ev_hp[half], c->copy_stream));
-    k_fetch_spans<<<dim3(c->FH, nb * c->n_cam), 128, 0, c->copy_stream>>>(
-        dhp, dframes, (long long)fpad, c->d_spans.as<int2>(), c->n_cam, c->FH, (long long)src_stride, (int)row);
+    if (h.fmt) {
+      k_fetch_yuv<<<dim3(h.rows, nb * c->n_cam), 128, 0, c->copy_stream>>>(
+          dhp, dframes, (long long)fpad, c->d_yuv_win[h.fmt - 1].as<int4>(), c->n_cam, h.rows, (long long)src_stride, (int)row);
+      c->last_h2d_bytes += (long long)c->yuv_fetch_bytes[h.fmt - 1] * nb;
+    } else {
+      k_fetch_spans<<<dim3(c->FH, nb * c->n_cam), 128, 0, c->copy_stream>>>(
+          dhp, dframes, (long long)fpad, c->d_spans.as<int2>(), c->n_cam, c->FH, (long long)src_stride, (int)row);
+      c->last_h2d_bytes += (long long)c->span_fetch_bytes * nb;
+    }
     LAUNCHED(c);
-    c->last_h2d_bytes += (long long)c->span_fetch_bytes * nb;
   }
   for (int i = 0; i < nb * c->n_cam && !h.zero_copy; ++i) {
     const uint8_t* s = srcs[(size_t)b0 * c->n_cam + i];
@@ -1348,8 +1452,14 @@ static int ingest_chunk(bevk_ctx* c, const HostIngest& h, const uint8_t* const* 
     uint8_t* d = dframes + (size_t)i * fpad;
     if (flags & BEVK_FLAG_BALANCE) {   // luminance_balance averages V over the whole raw frame: everything goes up
       if ((size_t)src_stride == row) CU(cudaMemcpyAsync(d, s, fbytes, cudaMemcpyHostToDevice, c->copy_stream));
-      else CU(cudaMemcpy2DAsync(d, row, s, (size_t)src_stride, row, c->FH, cudaMemcpyHostToDevice, c->copy_stream));
+      else CU(cudaMemcpy2DAsync(d, row, s, (size_t)src_stride, row, h.rows, cudaMemcpyHostToDevice, c->copy_stream));
       c->last_h2d_bytes += (long long)fbytes;
+    } else if (h.fmt) {                // the Y rows of this camera's band boxes and their chroma rows (yuv_dma_rects)
+      for (const int4& r : c->yuv_rects[h.fmt - 1][i % c->n_cam]) {
+        CU(cudaMemcpy2DAsync(d + (size_t)r.x * row + r.z, row, s + (size_t)r.x * src_stride + r.z, (size_t)src_stride, (size_t)r.w,
+                             (size_t)r.y, cudaMemcpyHostToDevice, c->copy_stream));
+        c->last_h2d_bytes += (long long)r.y * r.w;
+      }
     } else {                           // only the rectangle of the frame this camera's LUT can sample
       for (int bnd = 0; bnd < c->n_bands; ++bnd) {
         const int* bx = c->cam_box[i % c->n_cam][bnd];
@@ -1732,6 +1842,7 @@ static int shard_exchange_vsums(bevk_ctx* c, Frames src, int batch, long long* r
 int bevk_bev_run_sharded(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, const void* d_car, int flags, void* d_out) {
   NvtxRange nvtx_call("bevk_bev_run_sharded (render slabs, all-gather, compose)");
   RET(use(c));
+  RET(bgr_only(flags, "bevk_bev_run_sharded"));
   if (!c->shard.configured) return fail(BEVK_ERR_ARG, "bevk_shard_configure not called");
   RET(check_stack(c, d_frames, frame_stride));
   bevk_ctx::Shard& s = c->shard;
@@ -1818,6 +1929,7 @@ int bevk_bev_run_scattered(bevk_ctx* c, const void* d_frames, int64_t frame_stri
                            void* d_out_own, int* n_own) {
   NvtxRange nvtx_call("bevk_bev_run_scattered (render with peer stores, barrier, compose own)");
   RET(use(c));
+  RET(bgr_only(flags, "bevk_bev_run_scattered"));
   bevk_ctx::Shard& s = c->shard;
   if (!s.configured || s.policy != BEVK_SHARD_CAMERAS) return fail(BEVK_ERR_ARG, "bevk_shard_configure(CAMERAS) not called");
   RET(check_stack(c, d_frames, frame_stride));
@@ -1939,6 +2051,7 @@ int bevk_bev_run_jpeg(bevk_ctx* c, const uint8_t* const* jpegs, const uint64_t* 
                       uint8_t* out) {
   NvtxRange nvtx_call("bevk_bev_run_jpeg (JPEG streams -> host canvases)");
   RET(use(c));
+  RET(bgr_only(flags, "bevk_bev_run_jpeg"));
   if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
   if (!jpegs || !sizes || !out || batch < 1) return fail(BEVK_ERR_ARG, "bad argument");
   const size_t fbytes = (size_t)c->FW * c->FH * 3, fpad = (fbytes + 255) & ~size_t(255), cbytes = (size_t)c->BW * c->BH * 3;
@@ -2141,6 +2254,7 @@ int bevk_bev_run_to_jpeg(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_st
                          int quality, uint8_t* out, uint64_t capacity, uint64_t* sizes) {
   NvtxRange nvtx_call("bevk_bev_run_to_jpeg (host frames -> host JPEG streams)");
   RET(use(c));
+  RET(bgr_only(flags, "bevk_bev_run_to_jpeg"));
   RET(to_jpeg_check(c, out, sizes));
   HostIngest h;
   RET(ingest_setup(c, srcs, src_stride, batch, car, flags, &h));
@@ -2169,6 +2283,7 @@ int bevk_bev_frames_to_jpeg(bevk_ctx* c, const void* const* frames, int batch, c
                             uint8_t* out, uint64_t capacity, uint64_t* sizes) {
   NvtxRange nvtx_call("bevk_bev_frames_to_jpeg (device frames -> host JPEG streams)");
   RET(use(c));
+  RET(bgr_only(flags, "bevk_bev_frames_to_jpeg"));
   RET(to_jpeg_check(c, out, sizes));
   if (!frames) return fail(BEVK_ERR_ARG, "null pointer");
   Frames src;

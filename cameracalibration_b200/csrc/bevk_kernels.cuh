@@ -575,6 +575,192 @@ __global__ void __launch_bounds__(128) k_lum_spans(Frames in, uint8_t* __restric
 }
 
 // ---------------------------------------------------------------------------------
+// YUV 4:2:0 sources (NV12, I420).  A frame is cv2's single-buffer layout: a uint8[FH*3/2][FW] image (FW, FH even) whose
+// first FH rows are the Y plane.  NV12: then FH/2 rows of interleaved U,V.  I420: then the U plane and the V plane, each
+// FW/2 x FH/2 and packed, so two chroma rows share a buffer row: chroma row k (U rows 0..FH/2-1, then the V rows) starts
+// at buffer row FH + k/2, column (k & 1) * FW/2 -- which is also where cv2 looks for it in a buffer with padded rows.
+// The colour conversion runs once per sampled source pixel into the same copy stack the BALANCE pre-pass fills; the
+// fused render then reads BGR from there as it always does.
+// ---------------------------------------------------------------------------------
+enum { YUV_NV12 = 1, YUV_I420 = 2 };
+
+// cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420), OpenCV 4.x's fixed-point form (20 fraction bits), with U, V the chroma
+// samples of pixel (x/2, y/2).  One definition for the kernels and the CPU tests.
+__host__ __device__ __forceinline__ void yuv_bgr(int Y, int U, int V, int& b, int& g, int& r) {
+  const int y = max(0, Y - 16) * 1220542, u = U - 128, v = V - 128, h = 1 << 19;
+  b = min(255, max(0, (y + h + 2116026 * u) >> 20));
+  g = min(255, max(0, (y + h - 852492 * v - 409993 * u) >> 20));
+  r = min(255, max(0, (y + h + 1673527 * v) >> 20));
+}
+
+// Byte offsets of chroma row cy of a frame whose rows are `pitch` bytes apart: the U and V samples of pixel x are at
+// u + step * (x/2) and v + step * (x/2), step = yuv_chroma_step<FMT>.
+template <int FMT>
+__host__ __device__ __forceinline__ void yuv_chroma_rows(int FW, int FH, long long pitch, int cy, long long& u, long long& v) {
+  if (FMT == YUV_NV12) {
+    u = (long long)(FH + cy) * pitch;
+    v = u + 1;
+  } else {
+    const int ku = cy, kv = FH / 2 + cy;
+    u = (long long)(FH + ku / 2) * pitch + (ku & 1) * (FW / 2);
+    v = (long long)(FH + kv / 2) * pitch + (kv & 1) * (FW / 2);
+  }
+}
+template <int FMT>
+__host__ __device__ __forceinline__ constexpr int yuv_chroma_step() { return FMT == YUV_NV12 ? 2 : 1; }
+
+__host__ __device__ __forceinline__ int ld_u8(const uint8_t* p) {
+#ifdef __CUDA_ARCH__
+  return __ldg(p);
+#else
+  return *p;
+#endif
+}
+
+// The 4-pixel groups [g0, g1) that cover span sp of a row (k_lum_spans' rule); a group's pixels at or past FW (the last
+// group of a row when FW % 4 == 2) are not converted.
+__host__ __device__ __forceinline__ void span_groups(int2 sp, int& g0, int& g1) {
+  g0 = sp.x >> 2;
+  g1 = sp.y > sp.x ? (sp.y + 3) >> 2 : g0;
+}
+
+// One work item of k_yuv_spans: group g of row y of frame f (rows FW bytes apart), converted to BGR in c[3 * px + {0,1,2}]
+// and, with BAL, luminance-balanced by delta d (tab: the HSV division tables).  Returns the number of pixels (4 or 2).
+template <int FMT, bool BAL>
+__host__ __device__ __forceinline__ int yuv_group(const uint8_t* __restrict__ f, int FW, int FH, int y, int g, int d,
+                                                  const int* __restrict__ tab, int (&c)[12]) {
+  const int x0 = 4 * g, n = min(4, FW - x0);
+  long long uo, vo;
+  yuv_chroma_rows<FMT>(FW, FH, FW, y >> 1, uo, vo);
+  const uint8_t* yr = f + (long long)y * FW + x0;
+  const uint8_t* ur = f + uo + yuv_chroma_step<FMT>() * (x0 >> 1);
+  const uint8_t* vr = f + vo + yuv_chroma_step<FMT>() * (x0 >> 1);
+  int Y[4] = {0, 0, 0, 0}, U[2] = {128, 128}, V[2] = {128, 128};
+#ifdef __CUDA_ARCH__
+  if (n == 4 && (reinterpret_cast<uintptr_t>(yr) & 3) == 0) {
+    const unsigned w = __ldg(reinterpret_cast<const unsigned*>(yr));
+#pragma unroll
+    for (int k = 0; k < 4; ++k) Y[k] = (w >> (8 * k)) & 255;
+  } else
+#endif
+  {
+    for (int k = 0; k < n; ++k) Y[k] = ld_u8(yr + k);
+  }
+#ifdef __CUDA_ARCH__
+  if (FMT == YUV_NV12 && n == 4 && (reinterpret_cast<uintptr_t>(ur) & 3) == 0) {   // U0 V0 U1 V1
+    const unsigned w = __ldg(reinterpret_cast<const unsigned*>(ur));
+    U[0] = w & 255; V[0] = (w >> 8) & 255; U[1] = (w >> 16) & 255; V[1] = w >> 24;
+  } else
+#endif
+  {
+    for (int k = 0; k < (n >> 1); ++k) { U[k] = ld_u8(ur + yuv_chroma_step<FMT>() * k); V[k] = ld_u8(vr + yuv_chroma_step<FMT>() * k); }
+  }
+  const bool rt = x0 >= FW - (FW % 32);   // luminance_balance's row tail (a multiple of 4: whole groups)
+#pragma unroll
+  for (int px = 0; px < 4; ++px) {
+    yuv_bgr(Y[px], U[px >> 1], V[px >> 1], c[3 * px], c[3 * px + 1], c[3 * px + 2]);
+    if (BAL) hsv_roundtrip(c[3 * px], c[3 * px + 1], c[3 * px + 2], d, rt, tab, tab + 256);
+  }
+  return n;
+}
+
+// The YUV source pre-pass of a fused render: k_lum_spans' work decomposition (one CTA per LUM_ROWS source rows of one
+// frame, the rows' span groups as one flat list), reading Y row y and chroma row y/2 of the frame and writing BGR into
+// the copy stack (frame f at out_base + f * out_stride, rows FW * 3 bytes); with BAL each pixel then takes
+// luminance_balance's HSV round trip with the frame's delta, so a balanced YUV render has no extra pass over the frames.
+template <int FMT, bool BAL>
+__global__ void __launch_bounds__(128) k_yuv_spans(Frames in, uint8_t* __restrict__ out_base, long long out_stride,
+                                                   const int2* __restrict__ spans, CamRange cr, int w, int h,
+                                                   const int* __restrict__ delta, const int* __restrict__ hsv_tab) {
+  const int f = range_frame(cr, blockIdx.y), y0 = blockIdx.x * LUM_ROWS, y1 = min(h, y0 + LUM_ROWS), nrows = y1 - y0;
+  const int2* sp_cam = spans + (size_t)(f % cr.n_cam) * h;
+  const uint8_t* const frame = in.frame(f);
+  uint8_t* const out = out_base + f * out_stride;
+  __shared__ int s_tab[BAL ? 512 : 1];
+  __shared__ int s_pref[LUM_ROWS + 1], s_g0[LUM_ROWS];
+  if (threadIdx.x == 0) {
+    int acc = 0;
+    for (int r = 0; r < nrows; ++r) {
+      int g0, g1;
+      span_groups(sp_cam[y0 + r], g0, g1);
+      s_pref[r] = acc; s_g0[r] = g0;
+      acc += g1 - g0;
+    }
+    for (int r = nrows; r <= LUM_ROWS; ++r) s_pref[r] = acc;
+  }
+  if (BAL)
+    for (int i = threadIdx.x; i < 512; i += 128) s_tab[i] = hsv_tab[i];
+  __syncthreads();
+  const int total = s_pref[LUM_ROWS];
+  if (total == 0) return;
+  const int d = BAL ? delta[f] : 0;
+  const bool words = (w & 3) == 0 && (reinterpret_cast<uintptr_t>(out) & 3) == 0;
+  const size_t row_bytes = (size_t)w * 3;
+  int r = 0;
+#pragma unroll 2
+  for (int i = threadIdx.x; i < total; i += 128) {
+    while (i >= s_pref[r + 1]) ++r;                       // the thread's items are visited in increasing order
+    const int gidx = s_g0[r] + (i - s_pref[r]);
+    int c[12];
+    const int n = yuv_group<FMT, BAL>(frame, w, h, y0 + r, gidx, d, s_tab, c);
+    uint8_t* o = out + (size_t)(y0 + r) * row_bytes + 12 * (size_t)gidx;
+    if (words) {
+      unsigned* o4 = reinterpret_cast<unsigned*>(o);
+      o4[0] = (unsigned)c[0] | ((unsigned)c[1] << 8) | ((unsigned)c[2] << 16) | ((unsigned)c[3] << 24);
+      o4[1] = (unsigned)c[4] | ((unsigned)c[5] << 8) | ((unsigned)c[6] << 16) | ((unsigned)c[7] << 24);
+      o4[2] = (unsigned)c[8] | ((unsigned)c[9] << 8) | ((unsigned)c[10] << 16) | ((unsigned)c[11] << 24);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 12; ++k)
+        if (k < 3 * n) o[k] = (uint8_t)c[k];
+    }
+  }
+}
+
+// V = max(B, G, R) summed over the four pixels that share chroma sample (cx, cy) (frame rows FW bytes apart).
+template <int FMT>
+__host__ __device__ __forceinline__ unsigned yuv_vsum_2x2(const uint8_t* __restrict__ f, int FW, int FH, int cx, int cy) {
+  long long uo, vo;
+  yuv_chroma_rows<FMT>(FW, FH, FW, cy, uo, vo);
+  const int U = ld_u8(f + uo + yuv_chroma_step<FMT>() * cx), V = ld_u8(f + vo + yuv_chroma_step<FMT>() * cx);
+  const uint8_t* y = f + (long long)(2 * cy) * FW + 2 * cx;
+  const int Yv[4] = {ld_u8(y), ld_u8(y + 1), ld_u8(y + FW), ld_u8(y + FW + 1)};
+  unsigned s = 0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    int b, g, r;
+    yuv_bgr(Yv[k], U, V, b, g, r);
+    s += (unsigned)max(b, max(g, r));
+  }
+  return s;
+}
+
+// k_vsum for YUV frames: vsum[frame] += the exact sum of V over the whole converted frame (what luminance_balance sees
+// after cvtColor).  grid = (blocks over chroma rows, frames of the range `cr`).
+template <int FMT>
+__global__ void __launch_bounds__(256, 8) k_vsum_yuv(Frames frames, int w, int h, unsigned long long* __restrict__ vsum,
+                                                     CamRange cr) {
+  const int fi = range_frame(cr, blockIdx.y);
+  const uint8_t* f = frames.frame(fi);
+  unsigned long long acc = 0;
+  for (int cy = blockIdx.x; cy < h / 2; cy += gridDim.x) {
+    unsigned s = 0;   // at most 4 * 255 per sample and FW/2 <= 16384 samples per row: fits 32 bits
+    for (int cx = threadIdx.x; cx < w / 2; cx += blockDim.x) s += yuv_vsum_2x2<FMT>(f, w, h, cx, cy);
+    acc += s;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  __shared__ unsigned long long part[8];
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long t = 0;
+    for (int k = 0; k < 8; ++k) t += part[k];
+    atomicAdd(vsum + fi, t);
+  }
+}
+
+// ---------------------------------------------------------------------------------
 // Host -> device ingest for page-locked (mapped) host frames: instead of DMA rectangles, the SMs
 // read exactly the sampled row spans of every frame straight out of host memory (zero-copy, 16-byte
 // vectors, coalesced) and write them into the device frame buffers.  Moves ~17 % of each frame
@@ -592,6 +778,24 @@ __global__ void __launch_bounds__(128) k_fetch_spans(const uint8_t* const* __res
   const uint4* src = reinterpret_cast<const uint4*>(host_frames[f] + (size_t)y * host_stride + b0);
   uint4* dst = reinterpret_cast<uint4*>(dev_frames + f * dev_stride + (size_t)y * row_bytes + b0);
   for (int i = threadIdx.x; i < (b1 - b0) >> 4; i += 128) dst[i] = src[i];
+}
+
+// The same for page-locked YUV frames: buffer row y of the uint8[FH*3/2][FW] frame brings its one or two 16-byte
+// windows win[camera][y] = (x0, x1, x2, x3), bytes [x0, x1) and [x2, x3) (yuv_windows in bevk_plan.cuh: everything
+// k_yuv_spans reads of the row).  grid = (FH*3/2, n_frames); frame f goes to dev_frames + f * dev_stride, rows
+// row_bytes (= FW) apart.
+__global__ void __launch_bounds__(128) k_fetch_yuv(const uint8_t* const* __restrict__ host_frames, uint8_t* __restrict__ dev_frames,
+                                                   long long dev_stride, const int4* __restrict__ win, int n_cam, int rows,
+                                                   long long host_stride, int row_bytes) {
+  const int y = blockIdx.x, f = blockIdx.y;
+  const int4 wd = win[(size_t)(f % n_cam) * rows + y];
+  const int n1 = (wd.y - wd.x) >> 4, n = n1 + ((wd.w - wd.z) >> 4);
+  const uint8_t* src = host_frames[f] + (size_t)y * host_stride;
+  uint8_t* dst = dev_frames + f * dev_stride + (size_t)y * row_bytes;
+  for (int i = threadIdx.x; i < n; i += 128) {
+    const int off = i < n1 ? wd.x + 16 * i : wd.z + 16 * (i - n1);
+    *reinterpret_cast<uint4*>(dst + off) = *reinterpret_cast<const uint4*>(src + off);
+  }
 }
 
 }  // namespace bevk

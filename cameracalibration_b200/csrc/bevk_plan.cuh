@@ -142,4 +142,78 @@ inline void plan_bands(const int2* spans /* [FH] of one camera */, int FW, int F
   }
 }
 
+// ---- YUV 4:2:0 host ingest (the frame layout is described above k_yuv_spans in bevk_kernels.cuh) -------------------
+// What k_yuv_spans reads of row y: Y bytes [4 g0, min(FW, 4 g1)) of buffer row y (span_groups of the row's span), and of
+// chroma row y/2 the samples of the same pixels: NV12 bytes [4 g0, min(FW, 4 g1)), I420 [2 g0, min(FW/2, 2 g1)) of
+// each plane's row.  Page-locked frames fetch, per buffer row, up to two 16-byte aligned windows that contain those
+// bytes (k_fetch_yuv): a Y row takes the BGR rule in Y bytes (span +- 4 px), a chroma row the union of its two Y rows'
+// spans mapped to chroma bytes and widened and aligned the same way.  win: [FH * 3 / 2] per camera, (x0, x1, x2, x3).
+inline int4 yuv_window(int b0, int b1, int lo, int hi) {   // [b0, b1) widened to 16-byte bounds inside [lo, hi)
+  return make_int4(std::max(lo, b0) & ~15, std::min(hi, (b1 + 15) & ~15), 0, 0);
+}
+
+inline void yuv_windows(int fmt, const int2* spans /* [FH] of one camera */, int FW, int FH, int4* win) {
+  auto uni = [&](int cy, int& x0, int& x1) {     // union of the spans of Y rows 2 cy, 2 cy + 1
+    x0 = INT_MAX; x1 = -1;
+    for (int y = 2 * cy; y < 2 * cy + 2; ++y)
+      if (spans[y].y > spans[y].x) { x0 = std::min(x0, spans[y].x); x1 = std::max(x1, spans[y].y); }
+    return x1 > x0;
+  };
+  for (int y = 0; y < FH; ++y)
+    win[y] = spans[y].y > spans[y].x ? yuv_window(spans[y].x - 4, spans[y].y + 4, 0, FW) : make_int4(0, 0, 0, 0);
+  for (int j = 0; j < FH / 2; ++j) {
+    int4& w = win[FH + j];
+    w = make_int4(0, 0, 0, 0);
+    int x0, x1;
+    if (fmt == 1) {                               // NV12: chroma byte 2 (x/2) (+1) for pixel x
+      if (uni(j, x0, x1)) w = yuv_window(x0 - 4, x1 + 4, 0, FW);
+    } else {                                      // I420: buffer row j holds chroma rows k = 2j (left) and 2j + 1 (right)
+      for (int half = 0; half < 2; ++half) {
+        const int k = 2 * j + half, cy = k < FH / 2 ? k : k - FH / 2, base = half * (FW / 2);
+        if (!uni(cy, x0, x1)) continue;
+        // aligned within the whole buffer row (FW/2 need not be a multiple of 16): a window may reach into the other half
+        const int4 a = yuv_window(base + x0 / 2 - 2, base + (x1 + 1) / 2 + 2, 0, FW);
+        if (w.y <= w.x) w = a;
+        else if (a.x <= w.y) w.y = std::max(w.y, a.y);
+        else { w.z = a.x; w.w = a.y; }
+      }
+    }
+  }
+}
+
+// Bytes of a frame the window list fetches.
+inline long long yuv_window_bytes(const int4* win, int rows) {
+  long long n = 0;
+  for (int y = 0; y < rows; ++y) n += (long long)(win[y].y - win[y].x) + (win[y].w - win[y].z);
+  return n;
+}
+
+// Pageable YUV frames: the DMA rectangles (buffer row, rows, byte column, bytes) of one camera's band boxes (plan_bands,
+// BGR byte columns): the Y rows of each band, and the chroma rows of those rows over the band's pixel columns.
+inline void yuv_dma_rects(int fmt, const int (*box)[4], int n_bands, int FW, int FH, std::vector<int4>& rects) {
+  rects.clear();
+  for (int bnd = 0; bnd < n_bands; ++bnd) {
+    const int* bx = box[bnd];
+    if (bx[1] <= bx[0]) continue;
+    const int y0 = bx[0], y1 = bx[1], x0 = bx[2] / 3, x1 = bx[3] / 3;
+    rects.push_back(make_int4(y0, y1 - y0, x0, x1 - x0));
+    const int c0 = y0 / 2, c1 = (y1 - 1) / 2 + 1;   // chroma rows of Y rows [y0, y1)
+    if (fmt == 1) {
+      const int b0 = x0 & ~1, b1 = std::min(FW, (x1 + 1) & ~1);
+      rects.push_back(make_int4(FH + c0, c1 - c0, b0, b1 - b0));
+    } else {
+      const int p0 = x0 / 2, p1 = std::min(FW / 2, (x1 + 1) / 2);
+      for (int plane = 0; plane < 2; ++plane) {
+        const int k0 = plane * (FH / 2) + c0, k1 = plane * (FH / 2) + c1;   // chroma rows k of the plane
+        for (int odd = 0; odd < 2; ++odd) {                                 // k of one parity share a column offset
+          const int ka = k0 + ((k0 & 1) != odd);
+          if (ka >= k1) continue;
+          const int n = (k1 - ka + 1) / 2;
+          rects.push_back(make_int4(FH + ka / 2, n, odd * (FW / 2) + p0, p1 - p0));
+        }
+      }
+    }
+  }
+}
+
 }  // namespace bevk

@@ -455,12 +455,18 @@ class BevEngine:
         L.check(self.ctx.lib.bevk_bev_plan_info(self.ctx.h, C.byref(a), C.byref(b), C.byref(c)))
         return {"tiles": a.value, "items": b.value, "lut_bytes": c.value}
 
-    def run(self, frame_sets, car: np.ndarray | None = None, balance: bool = False, out: np.ndarray | None = None):
+    def run(self, frame_sets, car: np.ndarray | None = None, balance: bool = False, out: np.ndarray | None = None,
+            pixel_format: str = "bgr"):
         """frame_sets: list (batch) of lists (n_cam) of uint8[FH][FW][3] arrays.  Returns
-        uint8[batch][BH][BW][3]."""
+        uint8[batch][BH][BW][3].
+
+        pixel_format "nv12" / "i420": every frame is a YUV 4:2:0 buffer uint8[FH*3//2][FW] in cv2's layout (rows may be
+        padded); the canvases are those of cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / _I420) followed by the BGR call.
+        The conversion runs on the GPU, and only the bytes the render samples (1.5 per pixel) cross PCIe."""
         if not self.finalized:
             self.finalize()
-        keep, ptrs, stride, batch = self._host_frames(frame_sets, "run()")
+        fmt = self._pixel_format(pixel_format)
+        keep, ptrs, stride, batch = self._host_frames(frame_sets, "run()", fmt)
         if out is None:   # a fresh array per call, as the reference returns -- page-locked and recycled (PinnedPool)
             if getattr(self, "_pool", None) is None:
                 self._pool = L.PinnedPool()
@@ -468,11 +474,30 @@ class BevEngine:
         else:
             out = _out((batch, self.BH, self.BW, 3), out)
         car, carp = self._host_car(car)
-        L.check(self.ctx.lib.bevk_bev_run(self.ctx.h, ptrs, stride, batch, carp, L.FLAG_BALANCE if balance else 0,
+        L.check(self.ctx.lib.bevk_bev_run(self.ctx.h, ptrs, stride, batch, carp, (L.FLAG_BALANCE if balance else 0) | fmt,
                                           L.vptr(out)))
         return out
 
-    def _host_frames(self, frame_sets, what):
+    def _pixel_format(self, pixel_format: str) -> int:
+        """Flag bits of a pixel_format argument ("bgr", "nv12", "i420"); YUV 4:2:0 needs an even frame size."""
+        fmt = L.PIXEL_FORMATS.get(str(pixel_format).lower())
+        if fmt is None:
+            raise L.BevkError(f"pixel_format must be one of {sorted(L.PIXEL_FORMATS)}, got {pixel_format!r}")
+        if fmt and (self.FW % 2 or self.FH % 2):
+            raise L.BevkError(f"{pixel_format} frames need an even frame size, this engine's is {self.FW} x {self.FH}")
+        return fmt
+
+    def _yuv_view(self, f):
+        """A host YUV 4:2:0 frame as bevk_bev_run reads it: uint8[FH*3//2][FW] with contiguous rows."""
+        shape = (self.FH * 3 // 2, self.FW)
+        if not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.shape != shape:
+            got = f"{f.dtype} {f.shape}" if isinstance(f, np.ndarray) else type(f).__name__
+            raise L.BevkError(f"YUV 4:2:0 frames must be uint8{list(shape)} arrays, got {got}")
+        if f.strides[1] != 1 or f.strides[0] < self.FW:
+            f = np.ascontiguousarray(f)
+        return f, f.strides[0]
+
+    def _host_frames(self, frame_sets, what, fmt: int = 0):
         """(arrays to keep alive, host pointer table, row stride, batch) of host frame-sets laid out as run() takes them."""
         batch = len(frame_sets)
         if batch < 1:
@@ -482,8 +507,11 @@ class BevEngine:
             if len(fs) != self.n_cam:
                 raise L.BevkError(f"frame-set {b} has {len(fs)} frames, expected {self.n_cam}")
             for k, f in enumerate(fs):
-                f = self._conform(f)
-                img, w, h, s, ch = L.image_view(f)
+                if fmt:
+                    img, s = self._yuv_view(f)
+                else:
+                    f = self._conform(f)
+                    img, w, h, s, ch = L.image_view(f)
                 if stride is None:
                     stride = s
                 elif s != stride:
@@ -561,12 +589,14 @@ class BevEngine:
         L.check(self.ctx.lib.bevk_bev_run_jpeg(self.ctx.h, ptrs, sizes, batch, carp, L.FLAG_BALANCE if balance else 0, L.vptr(out)))
         return out
 
-    def host_copy_bytes(self, balance: bool = False):
-        """(host->device, device->host) bytes per frame-set that run() moves over PCIe."""
+    def host_copy_bytes(self, balance: bool = False, pixel_format: str = "bgr"):
+        """(host->device, device->host) bytes per frame-set that run() moves over PCIe (pageable frames)."""
         if not self.finalized:
             self.finalize()
+        fmt = self._pixel_format(pixel_format)
         a, b = C.c_int64(), C.c_int64()
-        L.check(self.ctx.lib.bevk_bev_host_copy_bytes(self.ctx.h, L.FLAG_BALANCE if balance else 0, C.byref(a), C.byref(b)))
+        L.check(self.ctx.lib.bevk_bev_host_copy_bytes(self.ctx.h, (L.FLAG_BALANCE if balance else 0) | fmt, C.byref(a),
+                                                      C.byref(b)))
         return a.value, b.value
 
     def last_h2d_bytes(self) -> int:
@@ -594,13 +624,17 @@ class BevEngine:
         L.check(self.ctx.lib.bevk_bev_run_device(self.ctx.h, C.c_void_p(d_srcs_ptr), batch, C.c_void_p(d_car_ptr or None),
                                                  L.FLAG_BALANCE if balance else 0, C.c_void_p(d_out_ptr)))
 
-    def run_stack(self, d_frames_ptr: int, frame_stride: int, batch: int, d_out_ptr: int, d_car_ptr: int = 0, balance: bool = False):
+    def run_stack(self, d_frames_ptr: int, frame_stride: int, batch: int, d_out_ptr: int, d_car_ptr: int = 0, balance: bool = False,
+                  pixel_format: str = "bgr"):
         """Frame stack on the device (frame i at d_frames_ptr + i * frame_stride, i = set * n_cam + camera): the
-        TMA-staged kernel when base and stride are 16-byte aligned.  Only enqueues on the ctx stream."""
+        TMA-staged kernel when base and stride are 16-byte aligned.  Only enqueues on the ctx stream.  pixel_format
+        "nv12" / "i420": dense uint8[FH*3//2][FW] YUV 4:2:0 frames at any base and stride."""
         if not self.finalized:
             self.finalize()
+        fmt = self._pixel_format(pixel_format)
         L.check(self.ctx.lib.bevk_bev_run_stack(self.ctx.h, C.c_void_p(d_frames_ptr), int(frame_stride), batch,
-                                                C.c_void_p(d_car_ptr or None), L.FLAG_BALANCE if balance else 0, C.c_void_p(d_out_ptr)))
+                                                C.c_void_p(d_car_ptr or None), (L.FLAG_BALANCE if balance else 0) | fmt,
+                                                C.c_void_p(d_out_ptr)))
 
     def run_stack_cams(self, d_frames_ptr: int, frame_stride: int, batch: int, cam_lo: int, cam_hi: int, d_out_ptr: int):
         if not self.finalized:
@@ -617,7 +651,8 @@ class BevEngine:
         L.check(self.ctx.lib.bevk_bev_tma_plan_info(self.ctx.h, *[C.byref(x) for x in v]))
         return dict(zip(("items", "shapes", "box_bytes", "tma_entries", "gather_entries"), (x.value for x in v)))
 
-    def run_cuda(self, frames, car=None, balance: bool = False, out=None, stream: int | None = None):
+    def run_cuda(self, frames, car=None, balance: bool = False, out=None, stream: int | None = None,
+                 pixel_format: str = "bgr"):
         """Frames that already live on the GPU (decoder output, torch / CuPy arrays): no PCIe in the call.
 
         frames: one uint8 CUDA array [batch][n_cam][FH][FW][3], or a list (batch) of lists (n_cam) of uint8
@@ -626,9 +661,16 @@ class BevEngine:
         tensor is allocated.  ``stream``: raw CUDA stream handle the work is enqueued on for THIS call; default torch's
         current stream on the engine's device (so that torch kernels that produced ``frames``, this render and whatever
         consumes ``out`` are ordered), or the ctx's own stream when torch is not in use.  The ctx goes back to its previous
-        stream afterwards.  The call does not synchronise.  Returns ``out``."""
+        stream afterwards.  The call does not synchronise.  Returns ``out``.
+
+        pixel_format "nv12" / "i420": frames is one C-contiguous uint8 CUDA array [batch][n_cam][FH*3//2][FW] of YUV
+        4:2:0 frames in cv2's layout (e.g. NVDEC NV12 surfaces); the result is that of cv2.cvtColor to BGR followed by
+        the BGR call, with the conversion done on the GPU."""
         if not self.finalized:
             self.finalize()
+        fmt = self._pixel_format(pixel_format)
+        if fmt:
+            return self._run_cuda_yuv(frames, car, balance, out, stream, fmt, pixel_format)
         ptrs = self._cuda_frames(frames)
         batch = len(ptrs) // self.n_cam
         if out is None:
@@ -643,6 +685,29 @@ class BevEngine:
         with self.ctx.on_stream(stream):
             L.check(self.ctx.lib.bevk_bev_run_frames(self.ctx.h, table, batch, C.c_void_p(d_car), L.FLAG_BALANCE if balance else 0,
                                                      C.c_void_p(d_out)))
+        return out
+
+    def _run_cuda_yuv(self, frames, car, balance, out, stream, fmt, name):
+        """run_cuda() on a YUV 4:2:0 frame stack: bevk_bev_run_stack with a YUV flag."""
+        if not hasattr(frames, "__cuda_array_interface__"):
+            raise L.BevkError(f"{name} frames must be one uint8 CUDA array [batch][{self.n_cam}][{self.FH * 3 // 2}][{self.FW}]")
+        base, shape = _cuda_ptr(frames, None)
+        want = (self.n_cam, self.FH * 3 // 2, self.FW)
+        if len(shape) != 4 or tuple(shape[1:]) != want or shape[0] < 1:
+            raise L.BevkError(f"{name} frames must be uint8[batch][{self.n_cam}][{self.FH * 3 // 2}][{self.FW}], got {tuple(shape)}")
+        batch = shape[0]
+        if out is None:
+            import torch
+            out = torch.empty((batch, self.BH, self.BW, 3), dtype=torch.uint8, device=torch.device("cuda", self.ctx.device))
+        d_out = _cuda_ptr(out, (batch, self.BH, self.BW, 3))[0]
+        d_car = _cuda_ptr(car, (self.BH, self.BW, 3))[0] if car is not None else None
+        if stream is None:
+            from .sharding import _torch_current_stream
+            stream = _torch_current_stream(self.ctx.device)
+        with self.ctx.on_stream(stream):
+            L.check(self.ctx.lib.bevk_bev_run_stack(self.ctx.h, C.c_void_p(base), self.FW * self.FH * 3 // 2, batch,
+                                                    C.c_void_p(d_car), (L.FLAG_BALANCE if balance else 0) | fmt,
+                                                    C.c_void_p(d_out)))
         return out
 
     def cuda_to_jpeg(self, frames, quality: int = 95, car=None, balance: bool = False) -> list[bytes]:

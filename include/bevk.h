@@ -40,7 +40,13 @@ typedef enum {
 enum { BEVK_INTER_NEAREST = 0, BEVK_INTER_LINEAR = 1 };          /* cv2.INTER_* values */
 enum { BEVK_MAPS_UNDISTORT = 0, BEVK_MAPS_BEV = 1 };
 enum { BEVK_MODEL_FISHEYE = 0, BEVK_MODEL_PINHOLE = 1 };
-enum { BEVK_FLAG_BALANCE = 1 };                                   /* bevk_bev_run flags */
+/* bevk_bev_run flags.  BEVK_FLAG_NV12 / BEVK_FLAG_I420 (exclusive; they combine with BALANCE) say the frames are YUV
+ * 4:2:0 in cv2's single-buffer layout, uint8[frame_h*3/2][frame_w] (frame_w, frame_h even, else BEVK_ERR_UNSUPPORTED):
+ * the Y plane, then NV12: interleaved U,V rows; I420: the U plane, then the V plane, each frame_w/2 x frame_h/2 and
+ * packed (two chroma rows per buffer row).  The result is byte for byte cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 /
+ * COLOR_YUV2BGR_I420) followed by the BGR call.  Accepted by bevk_bev_run, bevk_bev_run_stack and
+ * bevk_bev_host_copy_bytes; every other entry point with flags refuses them with BEVK_ERR_UNSUPPORTED. */
+enum { BEVK_FLAG_BALANCE = 1, BEVK_FLAG_NV12 = 2, BEVK_FLAG_I420 = 4 };
 #define BEVK_MAX_CAMERAS 8
 
 int bevk_version(void);
@@ -142,7 +148,12 @@ int bevk_bev_finalize(bevk_ctx *ctx);
  * srcs: batch*n_cam host pointers (frame-set major: set0 cam0..camN-1, set1 ...),
  *       each uint8[frame_h][frame_w][3] with row stride src_stride bytes.
  * car : NULL or uint8[bev_h][bev_w][3] (dense), added after colour balance.
- * out : batch canvases uint8[bev_h][bev_w][3], dense, canvas b at out + b*bev_h*bev_w*3. */
+ * out : batch canvases uint8[bev_h][bev_w][3], dense, canvas b at out + b*bev_h*bev_w*3.
+ * With BEVK_FLAG_NV12 / _I420 each frame is uint8[frame_h*3/2][frame_w] whose rows (Y and chroma alike) are
+ * src_stride bytes apart.  Page-locked frames (frame_w and src_stride multiples of 16, no BALANCE) are read by the SMs
+ * in the 16-byte windows around the sampled Y spans and the matching chroma bytes; pageable ones go up as the band
+ * rectangles of the Y plane plus their chroma rows; with BALANCE whole frames.  On the device the sampled spans are
+ * converted to BGR (and balanced) into a copy stack that the TMA-staged kernel renders from. */
 int bevk_bev_run(bevk_ctx *ctx, const uint8_t *const *srcs, int64_t src_stride, int batch,
                  const uint8_t *car, int flags, uint8_t *out);
 /* Device-resident variant: d_srcs is a DEVICE array of batch*n_cam device pointers
@@ -161,7 +172,11 @@ int bevk_bev_run_frames(bevk_ctx *ctx, const void *const *frames, int batch, con
  * 16-byte aligned base and stride (and a row pitch frame_w*3 that is a multiple of 16) the TMA-staged kernel runs:
  * per (canvas tile, camera) one cp.async.bulk.tensor box per frame-set into shared memory; otherwise the
  * pointer-table gather.  bevk_bev_run_frames takes this path by itself when its table describes a stack, and so
- * does bevk_bev_run for its staging buffers.  Only enqueues on the ctx stream.                           */
+ * does bevk_bev_run for its staging buffers.  Only enqueues on the ctx stream.
+ * With BEVK_FLAG_NV12 / _I420 frame i is the dense uint8[frame_h*3/2][frame_w] YUV frame at d_frames + i * frame_stride
+ * (any base and any stride >= frame_w * frame_h * 3/2); its sampled spans are converted on the device into a 16-byte
+ * friendly BGR copy stack, so the TMA-staged kernel renders them whenever a TMA plan exists.  Still only enqueues, so
+ * it can be captured into a graph (after one eager call of the same shape).                                        */
 int bevk_bev_run_stack(bevk_ctx *ctx, const void *d_frames, int64_t frame_stride, int batch, const void *d_car, int flags,
                        void *d_out);
 /* Per-camera partial canvases for camera-sharded multi-GPU runs: rank r renders only
@@ -188,7 +203,8 @@ int bevk_luminance_balance(bevk_ctx *ctx, const uint8_t *const *imgs, int n, int
 int bevk_bev_plan_info(bevk_ctx *ctx, int64_t *n_tiles, int64_t *n_items, int64_t *lut_bytes);
 /* Bytes bevk_bev_run moves over PCIe per frame-set for the given flags: host->device (without
  * BALANCE only the rectangle of each frame its camera's LUT can sample is uploaded; with BALANCE
- * the whole frames, because the V means cover them) and device->host (the canvas). */
+ * the whole frames, because the V means cover them) and device->host (the canvas).  With a YUV
+ * flag: the Y rectangles and their chroma rows (1.5 bytes per pixel), or whole YUV frames. */
 int bevk_bev_host_copy_bytes(bevk_ctx *ctx, int flags, int64_t *h2d_per_frame_set, int64_t *d2h_per_frame_set);
 /* Host->device bytes the last bevk_bev_run call actually moved (page-locked frames are ingested span
  * by span by the SMs, pageable ones by DMA rectangles, BALANCE uploads whole frames). */
