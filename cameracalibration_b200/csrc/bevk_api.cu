@@ -80,14 +80,22 @@ struct NvtxRange {
 };
 
 // ------------------------------------------------------------------ small helpers
+// bytes rounded up to a multiple of 256: frames in a stack start 256-byte aligned
+static size_t pad256(size_t bytes) { return (bytes + 255) & ~size_t(255); }
+
+// Device memory owned by the ctx: grown by ensure(), freed with its owner.
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { release(); }
   int ensure(size_t n) {
     if (n <= cap) return BEVK_OK;
     if (p) cudaFree(p);
     p = nullptr; cap = 0;
-    n = (n + 255) & ~size_t(255);
+    n = pad256(n);
     CU(cudaMalloc(&p, n + 256));   // 256 B of slack: the kernels' 32-bit tap loads may touch 3 bytes past a frame
     cap = n;
     return BEVK_OK;
@@ -220,6 +228,7 @@ struct bevk_ctx {
   long long capture_launches0 = 0;
   struct Graph { cudaGraph_t g = nullptr; cudaGraphExec_t x = nullptr; long long kernels = 0; };
   std::vector<Graph> graphs;
+  ~bevk_ctx();   // releases every handle that is set: safe on a partly built ctx; the DevBufs free themselves
 };
 
 static int use(bevk_ctx* c) {
@@ -254,8 +263,6 @@ int bevk_ctx_create(int device, bevk_ctx** out) {
   cudaError_t e2 = e1 == cudaSuccess ? cudaEventCreate(&c->ev0) : e1;
   cudaError_t e3 = e2 == cudaSuccess ? cudaEventCreate(&c->ev1) : e2;
   if (e3 != cudaSuccess) {
-    if (c->ev0) cudaEventDestroy(c->ev0);
-    if (c->own) cudaStreamDestroy(c->own);
     delete c;
     return fail(BEVK_ERR_CUDA, "context setup: %s", cudaGetErrorString(e3));
   }
@@ -267,46 +274,38 @@ int bevk_ctx_create(int device, bevk_ctx** out) {
 static void shard_release(bevk_ctx* c);
 static void jpeg_release(bevk_ctx* c);
 
+bevk_ctx::~bevk_ctx() {
+  shard_release(this);
+  jpeg_release(this);
+  for (auto& g : graphs) { if (g.x) cudaGraphExecDestroy(g.x); if (g.g) cudaGraphDestroy(g.g); }
+  for (cudaEvent_t e : {ev0, ev1, ev_switch, ev_in[0], ev_in[1], ev_free[0], ev_free[1], ev_hp[0], ev_hp[1], enc.ev_sizes[0],
+                        enc.ev_sizes[1], enc.ev_out_free[0], enc.ev_out_free[1]})
+    if (e) cudaEventDestroy(e);
+  for (cudaStream_t s : {copy_stream, enc.out_stream, own})
+    if (s) cudaStreamDestroy(s);
+  for (void* p : {(void*)h_hptrs, (void*)enc.h_sizes[0], (void*)enc.h_sizes[1]})
+    if (p) cudaFreeHost(p);
+}
+
 int bevk_ctx_destroy(bevk_ctx* c) {
   if (!c) return BEVK_OK;
   cudaSetDevice(c->device);
   cudaDeviceSynchronize();   // not c->stream: a caller-owned stream handed to bevk_ctx_set_stream may be gone by now
-  for (DevBuf* b : {&c->s_src, &c->s_dst, &c->s_m1, &c->s_m2, &c->s_o1, &c->s_o2, &c->d_tiles, &c->d_items, &c->d_lut,
-                    &c->d_hsv, &c->d_frames, &c->d_canvas, &c->d_car, &c->d_vsum, &c->d_delta, &c->d_csum,
-                    &c->d_spans, &c->d_bal, &c->d_user_ptrs, &c->d_ttiles, &c->d_titems, &c->d_tlut,
-                    &c->d_jpeg_frames, &c->d_jpeg_canvas, &c->d_unit_counter})
-    b->release();
-  for (DevBuf* b : {&c->enc.d_header, &c->enc.d_tabs, &c->enc.coef, &c->enc.bits, &c->enc.offs, &c->enc.dcdiff, &c->enc.words,
-                    &c->enc.ffcnt, &c->enc.ffscan, &c->enc.scan_tmp, &c->enc.out[0], &c->enc.out[1], &c->enc.meta[0],
-                    &c->enc.meta[1]})
-    b->release();
-  if (c->enc.out_stream) {
-    cudaStreamSynchronize(c->enc.out_stream);
-    for (int i = 0; i < 2; ++i) {
-      cudaEventDestroy(c->enc.ev_sizes[i]); cudaEventDestroy(c->enc.ev_out_free[i]);
-      if (c->enc.h_sizes[i]) cudaFreeHost(c->enc.h_sizes[i]);
-    }
-    cudaStreamDestroy(c->enc.out_stream);
-  }
-  for (auto& m : c->maps) m.d.release();
-  shard_release(c);
-  jpeg_release(c);
-  for (auto& g : c->graphs) { if (g.x) cudaGraphExecDestroy(g.x); if (g.g) cudaGraphDestroy(g.g); }
-  for (auto& u : c->und) { u.map1.release(); u.map2.release(); }
-  for (auto& k : c->cam) { k.map1.release(); k.map2.release(); }
-  cudaEventDestroy(c->ev0);
-  cudaEventDestroy(c->ev1);
-  if (c->ev_switch) cudaEventDestroy(c->ev_switch);
-  if (c->copy_stream) {
-    cudaStreamSynchronize(c->copy_stream);
-    for (int i = 0; i < 2; ++i) { cudaEventDestroy(c->ev_in[i]); cudaEventDestroy(c->ev_free[i]); cudaEventDestroy(c->ev_hp[i]); }
-    if (c->h_hptrs) cudaFreeHost(c->h_hptrs);
-    c->d_hptrs.release();
-    cudaStreamDestroy(c->copy_stream);
-  }
-  cudaStreamDestroy(c->own);
   delete c;
   return BEVK_OK;
+}
+
+// A stream and its events, created all or nothing: on failure every handle is destroyed and left null, so that the next
+// call tries again.
+static int create_stream_set(cudaStream_t* s, std::initializer_list<cudaEvent_t*> events) {
+  cudaError_t e = cudaStreamCreateWithFlags(s, cudaStreamNonBlocking);
+  for (cudaEvent_t* ev : events)
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(ev, cudaEventDisableTiming);
+  if (e == cudaSuccess) return BEVK_OK;
+  for (cudaEvent_t* ev : events) { if (*ev) cudaEventDestroy(*ev); *ev = nullptr; }
+  if (*s) cudaStreamDestroy(*s);
+  *s = nullptr;
+  return fail(e == cudaErrorMemoryAllocation ? BEVK_ERR_OOM : BEVK_ERR_CUDA, "stream set-up: %s", cudaGetErrorString(e));
 }
 
 int bevk_ctx_set_stream(bevk_ctx* c, void* s) {
@@ -475,9 +474,14 @@ int bevk_undistorter_set(bevk_ctx* c, int slot, int model, const double K[9], co
   return BEVK_OK;
 }
 
+static int need_undistorter(bevk_ctx* c, int slot) {
+  if (slot < 0 || slot >= 8 || !c->und[slot].valid) return fail(BEVK_ERR_ARG, "undistorter slot %d not set", slot);
+  return BEVK_OK;
+}
+
 int bevk_undistorter_maps(bevk_ctx* c, int slot, int16_t* map1, uint16_t* map2) {
   RET(use(c));
-  if (slot < 0 || slot >= 8 || !c->und[slot].valid) return fail(BEVK_ERR_ARG, "undistorter slot %d not set", slot);
+  RET(need_undistorter(c, slot));
   if (!map1 || !map2) return fail(BEVK_ERR_ARG, "null output map");
   Undistorter& u = c->und[slot];
   const size_t n = (size_t)u.cm.w * u.cm.h;
@@ -522,7 +526,7 @@ static int undistort_to_scratch(bevk_ctx* c, int slot, const uint8_t* src, int s
 int bevk_undistort(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
                    uint8_t* dst, int dw, int dh, int64_t dstride, int interp) {
   RET(use(c));
-  if (slot < 0 || slot >= 8 || !c->und[slot].valid) return fail(BEVK_ERR_ARG, "undistorter slot %d not set", slot);
+  RET(need_undistorter(c, slot));
   Undistorter& u = c->und[slot];
   if (dw != u.cm.w || dh != u.cm.h)   // the caller sized dst for another map: never write past it
     return fail(BEVK_ERR_ARG, "undistorter slot %d holds a %dx%d map, the caller expects %dx%d", slot, u.cm.w, u.cm.h, dw, dh);
@@ -536,7 +540,7 @@ int bevk_undistort(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, in
 // the destination is left to the caller.  An image stride only matters when n > 1.
 static int stack_src_args(bevk_ctx* c, int slot, const void* d_src, int64_t sis, int sw, int sh, int64_t srs, int channels, int n,
                           int interp, GatherArgs* a) {
-  if (slot < 0 || slot >= 8 || !c->und[slot].valid) return fail(BEVK_ERR_ARG, "undistorter slot %d not set", slot);
+  RET(need_undistorter(c, slot));
   if (n < 1) return fail(BEVK_ERR_ARG, "n must be >= 1, got %d", n);
   if (interp != BEVK_INTER_LINEAR && interp != BEVK_INTER_NEAREST) return fail(BEVK_ERR_UNSUPPORTED, "interp %d", interp);
   RET(check_image(d_src, sw, sh, srs, channels, "src"));
@@ -644,6 +648,10 @@ static int need_cam(bevk_ctx* c, int cam) {
   return BEVK_OK;
 }
 
+static int need_plan(bevk_ctx* c) {
+  return c->planned ? BEVK_OK : fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
+}
+
 int bevk_bev_set_camera(bevk_ctx* c, int cam, const double K[9], const double D[4], const double P[9], int und_w,
                         int und_h, const double H[9]) {
   RET(use(c));
@@ -744,6 +752,11 @@ static TmaFns tma_fns(int cfg) {
 #undef X
   return TmaFns{{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}};
 }
+
+// the instantiations of k_bev: index = 3*BAL + {NB=1:0, 4:1, 8:2}
+static const void* const kBevFns[6] = {(const void*)k_bev<false, 1>, (const void*)k_bev<false, 4>, (const void*)k_bev<false, 8>,
+                                       (const void*)k_bev<true, 1>, (const void*)k_bev<true, 4>, (const void*)k_bev<true, 8>};
+static const int kBevNb[6] = {1, 4, 8, 1, 4, 8};
 
 // OpenCV's 8-bit HSV division tables (color_hsv: sdiv_table / hdiv_table180, hsv_shift = 12), uploaded once per ctx
 static int ensure_hsv(bevk_ctx* c) {
@@ -893,14 +906,11 @@ int bevk_bev_finalize(bevk_ctx* c) {
   if (c->bev_grid[0] == 0) {   // persistent grid = resident CTAs of each variant
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, c->device));
-    const void* fn[6] = {(const void*)k_bev<false, 1>, (const void*)k_bev<false, 4>, (const void*)k_bev<false, 8>,
-                         (const void*)k_bev<true, 1>, (const void*)k_bev<true, 4>, (const void*)k_bev<true, 8>};
-    const int nb[6] = {1, 4, 8, 1, 4, 8};
     for (int i = 0; i < 6; ++i) {
       int per_sm = 0;
-      const size_t smem = bev_smem_bytes(i >= 3, nb[i]);
-      CU(cudaFuncSetAttribute(fn[i], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn[i], 256, smem));
+      const size_t smem = bev_smem_bytes(i >= 3, kBevNb[i]);
+      CU(cudaFuncSetAttribute(kBevFns[i], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kBevFns[i], 256, smem));
       c->bev_grid[i] = std::max(1, per_sm) * prop.multiProcessorCount;
     }
   }
@@ -911,7 +921,7 @@ int bevk_bev_finalize(bevk_ctx* c) {
 
 int bevk_bev_plan_info(bevk_ctx* c, int64_t* n_tiles, int64_t* n_items, int64_t* lut_bytes) {
   RET(use(c));
-  if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
+  RET(need_plan(c));
   if (n_tiles) *n_tiles = c->n_tiles;
   if (n_items) *n_items = c->n_items;
   if (lut_bytes) *lut_bytes = c->n_items * TILE * TILE * (int64_t)sizeof(uint4);
@@ -921,7 +931,7 @@ int bevk_bev_plan_info(bevk_ctx* c, int64_t* n_tiles, int64_t* n_items, int64_t*
 int bevk_bev_tma_plan_info(bevk_ctx* c, int64_t* n_items, int64_t* n_shapes, int64_t* box_bytes, int64_t* tma_entries,
                            int64_t* gather_entries) {
   RET(use(c));
-  if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
+  RET(need_plan(c));
   const bool t = c->tma_planned;
   if (n_items) *n_items = t ? c->tma_items : 0;
   if (n_shapes) *n_shapes = t ? (int64_t)c->tma_shapes.size() : 0;
@@ -952,7 +962,7 @@ static int bgr_only(int flags, const char* fn) {
 
 int bevk_bev_host_copy_bytes(bevk_ctx* c, int flags, int64_t* h2d, int64_t* d2h) {
   RET(use(c));
-  if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
+  RET(need_plan(c));
   int fmt = 0;
   RET(pixel_format(c, flags, &fmt));
   int64_t up = 0;
@@ -1075,6 +1085,26 @@ static void launch_vsum(bevk_ctx* c, Frames srcs, CamRange cr, int nr, unsigned 
   k_vsum<<<dim3(blocks, nr), 256, 0, c->stream>>>(srcs, frame_bytes, vsum, cr);
 }
 
+// luminance_balance deltas of `batch` frame-sets into d_delta, from the V-sum blocks [world][batch][n_cam]; without
+// blocks (null) from d_vsum, zeroed and then filled by vsum_kernel(d_vsum), which enqueues one kernel
+template <class VsumLaunch>
+static int lum_deltas(bevk_ctx* c, int batch, const unsigned long long* vsum_blocks, int world, VsumLaunch vsum_kernel) {
+  const int nf = batch * c->n_cam;
+  RET(c->d_delta.ensure((size_t)nf * 4));
+  if (!vsum_blocks) {
+    RET(c->d_vsum.ensure((size_t)nf * 8));
+    CU(cudaMemsetAsync(c->d_vsum.p, 0, (size_t)nf * 8, c->stream));
+    vsum_kernel(c->d_vsum.as<unsigned long long>());
+    LAUNCHED(c);
+    vsum_blocks = c->d_vsum.as<unsigned long long>();
+    world = 1;
+  }
+  k_delta<<<(batch + 127) / 128, 128, 0, c->stream>>>(vsum_blocks, c->n_cam, batch, world, (double)c->FW * (double)c->FH,
+                                                       c->d_delta.as<int>());
+  LAUNCHED(c);
+  return BEVK_OK;
+}
+
 // BALANCE pre-pass of the fused render: luminance_balance of the frames of cameras [lo, hi) of every frame-set, once
 // per sampled source pixel, into balanced copies (d_bal: frame b * n_cam + cam at the 256-byte padded stride) that the
 // ordinary fused gather then reads; *bal_src describes them.  The V sums come from k_vsum over those frames
@@ -1085,19 +1115,8 @@ static int balance_prepass(bevk_ctx* c, Frames src, int batch, int lo, int hi, c
                            Frames* bal_src) {
   const int nf = batch * c->n_cam, nr = batch * (hi - lo);
   const CamRange cr{lo, hi - lo, c->n_cam};
-  RET(c->d_delta.ensure((size_t)nf * 4));
-  if (!vsum_blocks) {
-    RET(c->d_vsum.ensure((size_t)nf * 8));
-    CU(cudaMemsetAsync(c->d_vsum.p, 0, (size_t)nf * 8, c->stream));
-    launch_vsum(c, src, cr, nr, c->d_vsum.as<unsigned long long>());
-    LAUNCHED(c);
-    vsum_blocks = c->d_vsum.as<unsigned long long>();
-    world = 1;
-  }
-  k_delta<<<(batch + 127) / 128, 128, 0, c->stream>>>(vsum_blocks, c->n_cam, batch, world, (double)c->FW * (double)c->FH,
-                                                       c->d_delta.as<int>());
-  LAUNCHED(c);
-  const size_t fpad = ((size_t)c->FW * 3 * c->FH + 255) & ~size_t(255);
+  RET(lum_deltas(c, batch, vsum_blocks, world, [&](unsigned long long* vsum) { launch_vsum(c, src, cr, nr, vsum); }));
+  const size_t fpad = pad256((size_t)c->FW * 3 * c->FH);
   RET(c->d_bal.ensure(fpad * nf));
   k_lum_spans<<<dim3((c->FH + LUM_ROWS - 1) / LUM_ROWS, nr), 128, 0, c->stream>>>(src, c->d_bal.as<uint8_t>(), (long long)fpad,
                                                                                  c->d_spans.as<int2>(), cr, c->FW, c->FH,
@@ -1115,17 +1134,12 @@ static int yuv_prepass_fmt(bevk_ctx* c, Frames src, int batch, bool bal, Frames*
   const int nf = batch * c->n_cam;
   const CamRange cr{0, c->n_cam, c->n_cam};
   if (bal) {
-    RET(c->d_delta.ensure((size_t)nf * 4));
-    RET(c->d_vsum.ensure((size_t)nf * 8));
-    CU(cudaMemsetAsync(c->d_vsum.p, 0, (size_t)nf * 8, c->stream));
     const int blocks = std::max(1, std::min(c->FH / 2, c->n_sm * 4 / std::max(1, std::min(nf, 64)) + 1));
-    k_vsum_yuv<FMT><<<dim3(blocks, nf), 256, 0, c->stream>>>(src, c->FW, c->FH, c->d_vsum.as<unsigned long long>(), cr);
-    LAUNCHED(c);
-    k_delta<<<(batch + 127) / 128, 128, 0, c->stream>>>(c->d_vsum.as<unsigned long long>(), c->n_cam, batch, 1,
-                                                         (double)c->FW * (double)c->FH, c->d_delta.as<int>());
-    LAUNCHED(c);
+    RET(lum_deltas(c, batch, nullptr, 1, [&](unsigned long long* vsum) {
+      k_vsum_yuv<FMT><<<dim3(blocks, nf), 256, 0, c->stream>>>(src, c->FW, c->FH, vsum, cr);
+    }));
   }
-  const size_t fpad = ((size_t)c->FW * 3 * c->FH + 255) & ~size_t(255);
+  const size_t fpad = pad256((size_t)c->FW * 3 * c->FH);
   RET(c->d_bal.ensure(fpad * nf));
   const dim3 grid((c->FH + LUM_ROWS - 1) / LUM_ROWS, nf);
   if (bal)
@@ -1143,6 +1157,15 @@ static int yuv_prepass(bevk_ctx* c, int fmt, Frames src, int batch, bool bal, Fr
   return fmt == YUV_NV12 ? yuv_prepass_fmt<YUV_NV12>(c, src, batch, bal, bgr_src) : yuv_prepass_fmt<YUV_I420>(c, src, batch, bal, bgr_src);
 }
 
+// colour balance of `batch` full canvases from their channel sums, then the car (null: none), in place
+static int launch_gain(bevk_ctx* c, uint8_t* out, int batch, const unsigned long long* csum, const uint8_t* car) {
+  const long long canvas_bytes = (long long)c->BW * c->BH * 3;
+  const int blocks = (int)std::max<long long>(1, std::min<long long>(canvas_bytes / (12 * 256) + 1, c->n_sm * 8 / std::max(1, std::min(batch, 64)) + 1));
+  k_gain<<<dim3(blocks, batch), 256, 0, c->stream>>>(out, canvas_bytes, (double)c->BW * (double)c->BH, csum, car);
+  LAUNCHED(c);
+  return BEVK_OK;
+}
+
 // run_device flag, not part of the ABI: with BALANCE, stop at the raw composed canvas and its channel sums (d_csum).  The
 // encoder's GainSrc applies the gains and the car, so k_gain does not run.  (Without BALANCE the write-out adds the car.)
 constexpr int kFlagRawBalance = 1 << 30;
@@ -1150,7 +1173,7 @@ constexpr int kFlagRawBalance = 1 << 30;
 static int run_device(bevk_ctx* c, Frames src, int batch, const void* d_car, int flags, void* d_out, int cam_lo, int cam_hi,
                       const OutWin* win = nullptr) {
   NvtxRange nvtx_render("bevk render (fused BEV kernels)");
-  if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
+  RET(need_plan(c));
   if ((!src.table && !src.base) || (!d_out && !(win && win->world))) return fail(BEVK_ERR_ARG, "null device pointer");
   if (batch < 1 || batch > 65535) return fail(BEVK_ERR_ARG, "batch %d out of range [1,65535]", batch);
   const bool bal = (flags & BEVK_FLAG_BALANCE) != 0;
@@ -1160,19 +1183,18 @@ static int run_device(bevk_ctx* c, Frames src, int batch, const void* d_car, int
   if ((bal || fmt) && nf > 65535)
     return fail(BEVK_ERR_ARG, "batch %d x %d cameras exceeds the 65535 frames of a BALANCE or YUV call", batch, c->n_cam);
   if (fmt && (win || cam_lo != 0 || cam_hi < c->n_cam)) return fail(BEVK_ERR_UNSUPPORTED, "YUV frames render whole canvases only");
-  BevParams P{};
-  P.n_cam = c->n_cam; P.FW = c->FW; P.FH = c->FH; P.pitch = (unsigned)c->FW * 3u;
-  P.tiles = c->d_tiles.as<int4>(); P.items = c->d_items.as<BevItem>(); P.lut = c->d_lut.as<uint4>();
-  P.out = reinterpret_cast<uint8_t*>(d_out); P.BW = c->BW; P.BH = c->BH;
-  P.canvas_bytes = (long long)c->BW * c->BH * 3;
-  P.out_pitch = c->BW * 3; P.ox = 0; P.oy = 0; P.ox1 = c->BW; P.oy1 = c->BH;
+  RenderParams R{};
+  R.n_cam = c->n_cam; R.FW = c->FW; R.FH = c->FH; R.pitch = (unsigned)c->FW * 3u;
+  R.out = reinterpret_cast<uint8_t*>(d_out); R.BW = c->BW; R.BH = c->BH;
+  R.canvas_bytes = (long long)c->BW * c->BH * 3;
+  R.out_pitch = c->BW * 3; R.ox = 0; R.oy = 0; R.ox1 = c->BW; R.oy1 = c->BH;
   if (win) {
     if (bal || d_car) return fail(BEVK_ERR_ARG, "balance and the car overlay need the full canvas");
-    P.canvas_bytes = win->stride; P.out_pitch = win->pitch; P.ox = win->ox; P.oy = win->oy; P.ox1 = win->ox1; P.oy1 = win->oy1;
+    R.canvas_bytes = win->stride; R.out_pitch = win->pitch; R.ox = win->ox; R.oy = win->oy; R.ox1 = win->ox1; R.oy1 = win->oy1;
   }
-  P.car = reinterpret_cast<const uint8_t*>(d_car);
-  P.cam_lo = cam_lo; P.cam_hi = cam_hi;
-  P.n_tiles = (int)c->n_tiles; P.batch = batch;
+  R.car = reinterpret_cast<const uint8_t*>(d_car);
+  R.cam_lo = cam_lo; R.cam_hi = cam_hi;
+  R.n_tiles = (int)c->n_tiles; R.batch = batch;
   // frame-sets per work unit: 4 amortises the LUT decode over a batch; 1 for single frames
   int nbu = batch >= 4 ? 4 : 1;
   if (c->nb_override) nbu = c->nb_override;
@@ -1182,21 +1204,17 @@ static int run_device(bevk_ctx* c, Frames src, int batch, const void* d_car, int
     RET(c->d_csum.ensure((size_t)batch * 24));
     CU(cudaMemsetAsync(c->d_csum.p, 0, (size_t)batch * 24, c->stream));
     if (!fmt) RET(balance_prepass(c, src, batch, 0, c->n_cam, nullptr, 1, &gsrc));
-    P.csum = c->d_csum.as<unsigned long long>();
+    R.csum = c->d_csum.as<unsigned long long>();
   }
   if (fmt) RET(yuv_prepass(c, fmt, src, batch, bal, &gsrc));   // BGR copies of the sampled spans (balanced with BALANCE)
   // TMA-staged kernel for frame stacks (16-byte aligned base and stride); global-offset gather otherwise
   const bool use_tma = c->tma_planned && !gsrc.table && (reinterpret_cast<uintptr_t>(gsrc.base) & 15) == 0 && (gsrc.stride & 15) == 0 &&
-                       gsrc.stride >= (long long)P.pitch * c->FH && (nbu == 1 || nbu == 4);
+                       gsrc.stride >= (long long)R.pitch * c->FH && (nbu == 1 || nbu == 4);
   if (use_tma) {
-    TmaParams T{};
+    TmaParams T{R};
+    T.tiles = c->d_ttiles.as<int4>(); T.items = c->d_titems.as<TmaItem>(); T.lut = c->d_tlut.as<uint4>();
     RET(stack_maps(c, gsrc.base, gsrc.stride, nf, &T.maps));
     T.base = gsrc.base; T.frame_stride = gsrc.stride;
-    T.n_cam = P.n_cam; T.FW = P.FW; T.FH = P.FH; T.pitch = P.pitch;
-    T.tiles = c->d_ttiles.as<int4>(); T.items = c->d_titems.as<TmaItem>(); T.lut = c->d_tlut.as<uint4>();
-    T.n_tiles = P.n_tiles; T.batch = batch; T.out = P.out; T.BW = P.BW; T.BH = P.BH; T.canvas_bytes = P.canvas_bytes;
-    T.car = P.car; T.csum = P.csum; T.cam_lo = cam_lo; T.cam_hi = cam_hi;
-    T.out_pitch = P.out_pitch; T.ox = P.ox; T.oy = P.oy; T.ox1 = P.ox1; T.oy1 = P.oy1;
     T.backoff_ns = c->tma_backoff_ns;
     if (win && win->world) { for (int r = 0; r < SHARD_MAX_RANKS; ++r) T.peer[r] = win->peer[r]; T.world = win->world; T.src_off = win->src_off; }
     RET(c->d_unit_counter.ensure(256));
@@ -1206,29 +1224,18 @@ static int run_device(bevk_ctx* c, Frames src, int batch, const void* d_car, int
     c->last_path = 2;
   } else {
     if (win && win->world) return fail(BEVK_ERR_UNSUPPORTED, "peer-store output needs the TMA-staged kernel (a 16-byte friendly frame stack)");
+    BevParams P{R};
+    P.tiles = c->d_tiles.as<int4>(); P.items = c->d_items.as<BevItem>(); P.lut = c->d_lut.as<uint4>();
     P.srcs = gsrc;
     const long long units = c->n_tiles * ((batch + nbu - 1) / nbu);
     const int variant = (bal ? 3 : 0) + (nbu == 8 ? 2 : (nbu == 4 ? 1 : 0));
     const unsigned bev_blocks = (unsigned)std::max<long long>(1, std::min<long long>(units, c->bev_grid[variant]));
-    const size_t bev_smem = bev_smem_bytes(bal, nbu);
-    if (bal) {
-      if (nbu == 8) k_bev<true, 8><<<bev_blocks, 256, bev_smem, c->stream>>>(P);
-      else if (nbu == 4) k_bev<true, 4><<<bev_blocks, 256, bev_smem, c->stream>>>(P);
-      else k_bev<true, 1><<<bev_blocks, 256, bev_smem, c->stream>>>(P);
-    } else {
-      if (nbu == 8) k_bev<false, 8><<<bev_blocks, 256, bev_smem, c->stream>>>(P);
-      else if (nbu == 4) k_bev<false, 4><<<bev_blocks, 256, bev_smem, c->stream>>>(P);
-      else k_bev<false, 1><<<bev_blocks, 256, bev_smem, c->stream>>>(P);
-    }
+    void* args[] = {&P};
+    CU(cudaLaunchKernel(kBevFns[variant], dim3(bev_blocks), dim3(256), args, bev_smem_bytes(bal, nbu), c->stream));
     LAUNCHED(c);
     c->last_path = 1;
   }
-  if (bal && !(flags & kFlagRawBalance)) {
-    const int gblocks = (int)std::max<long long>(1, std::min<long long>(P.canvas_bytes / (12 * 256) + 1, c->n_sm * 8 / std::max(1, std::min(batch, 64)) + 1));
-    k_gain<<<dim3(gblocks, batch), 256, 0, c->stream>>>(P.out, P.canvas_bytes, (double)c->BW * (double)c->BH,
-                                                        c->d_csum.as<unsigned long long>(), P.car);
-    LAUNCHED(c);
-  }
+  if (bal && !(flags & kFlagRawBalance)) RET(launch_gain(c, R.out, batch, R.csum, R.car));
   if (c->timed && !c->capturing) CU(cudaEventRecord(c->ev1, c->stream));
   return BEVK_OK;
 }
@@ -1280,7 +1287,7 @@ static int frames_src(bevk_ctx* c, const void* const* frames, int batch, Frames*
 
 int bevk_bev_run_frames(bevk_ctx* c, const void* const* frames, int batch, const void* d_car, int flags, void* d_out) {
   RET(use(c));
-  if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
+  RET(need_plan(c));
   if (!frames || !d_out) return fail(BEVK_ERR_ARG, "null pointer");
   RET(bgr_only(flags, "bevk_bev_run_frames"));
   Frames src;
@@ -1352,19 +1359,31 @@ struct HostIngest {
   int fmt = 0, rows = 0;                  // pixel format (0 = BGR) and buffer rows of a frame (FH; FH * 3 / 2 for YUV)
   int chunk = 0;
   bool zero_copy = false;
+  const void* d_car = nullptr;            // the car overlay on the device, or null
   std::vector<const uint8_t*> dev_view;   // zero-copy: device views of the page-locked frames
 };
 
+// The caller's host car canvas (null: none) into d_car on the ctx stream; *d_car: the device copy, or null.
+static int upload_car(bevk_ctx* c, const uint8_t* car, const void** d_car) {
+  *d_car = nullptr;
+  if (!car) return BEVK_OK;
+  const size_t cbytes = (size_t)c->BW * c->BH * 3;
+  RET(c->d_car.ensure(cbytes));
+  CU(cudaMemcpyAsync(c->d_car.p, car, cbytes, cudaMemcpyHostToDevice, c->stream));
+  *d_car = c->d_car.p;
+  return BEVK_OK;
+}
+
 static int ingest_setup(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, int batch, const uint8_t* car, int flags,
                         HostIngest* h) {
-  if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
+  RET(need_plan(c));
   if (!srcs) return fail(BEVK_ERR_ARG, "null host pointer");
   if (batch < 1) return fail(BEVK_ERR_ARG, "batch must be >= 1");
   int fmt = 0;
   RET(pixel_format(c, flags, &fmt));
   // a YUV frame is uint8[FH * 3 / 2][FW] at the same row stride; it is staged as it is and converted on the device
   const int rows = fmt ? c->FH * 3 / 2 : c->FH;
-  const size_t row = (size_t)c->FW * (fmt ? 1 : 3), fbytes = row * rows, fpad = (fbytes + 255) & ~size_t(255);
+  const size_t row = (size_t)c->FW * (fmt ? 1 : 3), fbytes = row * rows, fpad = pad256(fbytes);
   if (src_stride < (int64_t)row) return fail(BEVK_ERR_ARG, "src_stride %lld < row bytes", (long long)src_stride);
   const size_t cbytes = (size_t)c->BW * c->BH * 3;
   h->row = row; h->fbytes = fbytes; h->fpad = fpad; h->cbytes = cbytes; h->fmt = fmt; h->rows = rows;
@@ -1377,18 +1396,9 @@ static int ingest_setup(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_str
   const size_t set_frames = (size_t)c->n_cam;
   RET(c->d_frames.ensure(fpad * set_frames * chunk * 2));
   RET(c->d_canvas.ensure(cbytes * chunk * 2));
-  if (!c->copy_stream) {
-    CU(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; ++i) {
-      CU(cudaEventCreateWithFlags(&c->ev_in[i], cudaEventDisableTiming));
-      CU(cudaEventCreateWithFlags(&c->ev_free[i], cudaEventDisableTiming));
-      CU(cudaEventCreateWithFlags(&c->ev_hp[i], cudaEventDisableTiming));
-    }
-  }
-  if (car) {
-    RET(c->d_car.ensure(cbytes));
-    CU(cudaMemcpyAsync(c->d_car.p, car, cbytes, cudaMemcpyHostToDevice, c->stream));
-  }
+  if (!c->copy_stream)
+    RET(create_stream_set(&c->copy_stream, {&c->ev_in[0], &c->ev_in[1], &c->ev_free[0], &c->ev_free[1], &c->ev_hp[0], &c->ev_hp[1]}));
+  RET(upload_car(c, car, &h->d_car));
   // the copy stream must not start before work already queued on the main stream (e.g. the car upload,
   // or a previous call's D2H that still reads the canvases) has been ordered
   CU(cudaEventRecord(c->ev_free[0], c->stream));
@@ -1478,27 +1488,33 @@ static int ingest_chunk(bevk_ctx* c, const HostIngest& h, const uint8_t* const* 
   return BEVK_OK;
 }
 
+// One chunk of a host-frame call: frame-sets [b0, b0 + nb) ingested into staging half `half` and rendered into canvas
+// half `half` of d_canvas (*dcanvas), after which the staging half is free again.
+static int render_chunk(bevk_ctx* c, const HostIngest& h, const uint8_t* const* srcs, int64_t src_stride, int flags, int b0, int nb,
+                        int half, uint8_t** dcanvas) {
+  Frames fsrc;
+  RET(ingest_chunk(c, h, srcs, src_stride, flags, b0, nb, half, &fsrc));
+  c->timed = false;
+  *dcanvas = c->d_canvas.as<uint8_t>() + (size_t)half * h.chunk * h.cbytes;
+  RET(run_device(c, fsrc, nb, h.d_car, flags, *dcanvas, 0, BEVK_MAX_CAMERAS));
+  CU(cudaEventRecord(c->ev_free[half], c->stream));
+  return BEVK_OK;
+}
+
 int bevk_bev_run(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, int batch, const uint8_t* car, int flags,
                  uint8_t* out) {
   NvtxRange nvtx_call("bevk_bev_run (host frames -> host canvases)");
   RET(use(c));
-  if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
+  RET(need_plan(c));
   if (!srcs || !out) return fail(BEVK_ERR_ARG, "null host pointer");
   HostIngest h;
   RET(ingest_setup(c, srcs, src_stride, batch, car, flags, &h));
-  int half = 0;
-  for (int b0 = 0; b0 < batch; b0 += h.chunk, half ^= 1) {
+  for (int b0 = 0, half = 0; b0 < batch; b0 += h.chunk, half ^= 1) {
     const int nb = std::min(h.chunk, batch - b0);
-    Frames fsrc;
-    RET(ingest_chunk(c, h, srcs, src_stride, flags, b0, nb, half, &fsrc));
-    c->timed = false;
-    uint8_t* dcanvas = c->d_canvas.as<uint8_t>() + (size_t)half * h.chunk * h.cbytes;
-    RET(run_device(c, fsrc, nb, car ? c->d_car.p : nullptr, flags, dcanvas, 0, BEVK_MAX_CAMERAS));
-    CU(cudaEventRecord(c->ev_free[half], c->stream));               // frames of this half are free again
-    {
-      NvtxRange nvtx_d2h("bevk read-back (D2H canvases)");
-      CU(cudaMemcpyAsync(out + (size_t)b0 * h.cbytes, dcanvas, h.cbytes * nb, cudaMemcpyDeviceToHost, c->stream));
-    }
+    uint8_t* dcanvas = nullptr;
+    RET(render_chunk(c, h, srcs, src_stride, flags, b0, nb, half, &dcanvas));
+    NvtxRange nvtx_d2h("bevk read-back (D2H canvases)");
+    CU(cudaMemcpyAsync(out + (size_t)b0 * h.cbytes, dcanvas, h.cbytes * nb, cudaMemcpyDeviceToHost, c->stream));
   }
   CU(cudaStreamSynchronize(c->stream));
   return BEVK_OK;
@@ -1549,7 +1565,7 @@ int bevk_luminance_balance(bevk_ctx* c, const uint8_t* const* imgs, int n, int w
   RET(use(c));
   if (!imgs || !outs || n < 1 || n > BEVK_MAX_CAMERAS || w <= 0 || h <= 0) return fail(BEVK_ERR_ARG, "bad argument");
   RET(ensure_hsv(c));
-  const size_t fbytes = (size_t)w * h * 3, fpad = (fbytes + 255) & ~size_t(255);
+  const size_t fbytes = (size_t)w * h * 3, fpad = pad256(fbytes);
   RET(c->s_src.ensure(fpad * n));
   RET(c->s_dst.ensure(fpad * n));
   RET(c->d_vsum.ensure(8 * n));
@@ -1647,7 +1663,7 @@ int bevk_shard_configure(bevk_ctx* c, int policy, int rank, int world) {
 static int shard_geometry(bevk_ctx* c) {
   bevk_ctx::Shard& s = c->shard;
   if (!s.configured) return fail(BEVK_ERR_ARG, "bevk_shard_configure not called");
-  if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
+  RET(need_plan(c));
   if (s.geometry) return BEVK_OK;
   std::vector<const uint8_t*> pm(c->n_cam);
   for (int k = 0; k < c->n_cam; ++k) pm[k] = c->cam[k].mask.data();
@@ -1658,7 +1674,7 @@ static int shard_geometry(bevk_ctx* c) {
     const long long bytes = (long long)(s.rect[r].ox1 - s.rect[r].ox) * (s.rect[r].oy1 - s.rect[r].oy) * 3;
     s.slab_bytes = std::max(s.slab_bytes, bytes);
   }
-  s.slab_bytes = (s.slab_bytes + 255) & ~255ll;   // equal counts for the all-gather, 256-byte aligned slabs
+  s.slab_bytes = (long long)pad256(s.slab_bytes);   // equal counts for the all-gather, 256-byte aligned slabs
   s.geometry = true;
   return BEVK_OK;
 }
@@ -1686,10 +1702,32 @@ int bevk_shard_connect(bevk_ctx* c, const void* id, int len) {
   return BEVK_OK;
 }
 
+static int check_rank(bevk_ctx* c, int rank) {
+  if (rank < 0 || rank >= c->shard.world || rank >= SHARD_MAX_RANKS) return fail(BEVK_ERR_ARG, "rank %d out of range", rank);
+  return BEVK_OK;
+}
+
+// a device buffer the caller hands in: not null, and `align`-byte aligned
+static int check_dev_buf(const void* p, int align, const char* what) {
+  if (!p || (reinterpret_cast<uintptr_t>(p) & (align - 1))) return fail(BEVK_ERR_ARG, "%s null or not %d-byte aligned", what, align);
+  return BEVK_OK;
+}
+
+// does rank r render anything?  (a rank without cameras, or whose cameras' masks are empty, contributes nothing)
+static bool has_slab(const bevk_ctx::Shard& s, int r) { return s.rect[r].ox1 > s.rect[r].ox && s.cam_hi[r] > s.cam_lo[r]; }
+
+// the output window of rank r's slabs: its slab rectangle, slab_bytes apart
+static OutWin slab_win(const bevk_ctx::Shard& s, int r) {
+  const SlabRect q = s.rect[r];
+  OutWin w;
+  w.pitch = (q.ox1 - q.ox) * 3; w.ox = q.ox; w.oy = q.oy; w.ox1 = q.ox1; w.oy1 = q.oy1; w.stride = s.slab_bytes;
+  return w;
+}
+
 int bevk_shard_info(bevk_ctx* c, int rank, int* cam_lo, int* cam_hi, int32_t rect[4], int64_t* slab_bytes) {
   RET(use(c));
   RET(shard_geometry(c));
-  if (rank < 0 || rank >= c->shard.world || rank >= SHARD_MAX_RANKS) return fail(BEVK_ERR_ARG, "rank %d out of range", rank);
+  RET(check_rank(c, rank));
   if (cam_lo) *cam_lo = c->shard.cam_lo[rank];
   if (cam_hi) *cam_hi = c->shard.cam_hi[rank];
   if (rect) { rect[0] = c->shard.rect[rank].ox; rect[1] = c->shard.rect[rank].oy; rect[2] = c->shard.rect[rank].ox1; rect[3] = c->shard.rect[rank].oy1; }
@@ -1700,11 +1738,9 @@ int bevk_shard_info(bevk_ctx* c, int rank, int* cam_lo, int* cam_hi, int32_t rec
 // rank `as_rank`'s slabs of `batch` frame-sets into d_slabs[as_rank][batch][slab_bytes]
 static int shard_render(bevk_ctx* c, Frames src, int batch, int as_rank, void* d_slabs) {
   bevk_ctx::Shard& s = c->shard;
-  const SlabRect q = s.rect[as_rank];
   uint8_t* dst = reinterpret_cast<uint8_t*>(d_slabs) + (size_t)as_rank * batch * s.slab_bytes;
-  if (q.ox1 <= q.ox || s.cam_hi[as_rank] <= s.cam_lo[as_rank]) return BEVK_OK;   // a rank without cameras contributes nothing
-  OutWin w;
-  w.pitch = (q.ox1 - q.ox) * 3; w.ox = q.ox; w.oy = q.oy; w.ox1 = q.ox1; w.oy1 = q.oy1; w.stride = s.slab_bytes;
+  if (!has_slab(s, as_rank)) return BEVK_OK;
+  const OutWin w = slab_win(s, as_rank);
   return run_device(c, src, batch, nullptr, 0, dst, s.cam_lo[as_rank], s.cam_hi[as_rank], &w);
 }
 
@@ -1736,12 +1772,7 @@ static int shard_compose(bevk_ctx* c, const void* d_slabs, int batch, const void
   if (wide) k_compose_slabs<8, true><<<grid, 256, 0, c->stream>>>(a);
   else k_compose_slabs<1, true><<<grid, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
-  const long long canvas_bytes = (long long)c->BW * c->BH * 3;
-  const int gblocks = (int)std::max<long long>(1, std::min<long long>(canvas_bytes / (12 * 256) + 1, c->n_sm * 8 / std::max(1, std::min(batch, 64)) + 1));
-  k_gain<<<dim3(gblocks, batch), 256, 0, c->stream>>>(a.out, canvas_bytes, (double)c->BW * (double)c->BH, a.csum,
-                                                      reinterpret_cast<const uint8_t*>(d_car));
-  LAUNCHED(c);
-  return BEVK_OK;
+  return launch_gain(c, a.out, batch, a.csum, reinterpret_cast<const uint8_t*>(d_car));
 }
 
 // BALANCE limits of a camera-sharded call, checked before anything is enqueued (those of run_device)
@@ -1768,8 +1799,7 @@ static int shard_vsum(bevk_ctx* c, Frames src, int batch, int as_rank, unsigned 
 // ordinary windowed render of the balanced copies
 static int shard_render_balanced(bevk_ctx* c, Frames src, int batch, int as_rank, const unsigned long long* d_vsums, void* d_slabs) {
   bevk_ctx::Shard& s = c->shard;
-  const SlabRect q = s.rect[as_rank];
-  if (q.ox1 <= q.ox || s.cam_hi[as_rank] <= s.cam_lo[as_rank]) return BEVK_OK;
+  if (!has_slab(s, as_rank)) return BEVK_OK;
   Frames bal;
   RET(balance_prepass(c, src, batch, s.cam_lo[as_rank], s.cam_hi[as_rank], d_vsums, s.world, &bal));
   return shard_render(c, bal, batch, as_rank, d_slabs);
@@ -1780,8 +1810,8 @@ int bevk_shard_vsum(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int
   RET(shard_geometry(c));
   RET(check_stack(c, d_frames, frame_stride));
   RET(shard_balance_limits(c, batch));
-  if (as_rank < 0 || as_rank >= c->shard.world || as_rank >= SHARD_MAX_RANKS) return fail(BEVK_ERR_ARG, "rank %d out of range", as_rank);
-  if (!d_vsums || (reinterpret_cast<uintptr_t>(d_vsums) & 7)) return fail(BEVK_ERR_ARG, "V-sum buffer null or not 8-byte aligned");
+  RET(check_rank(c, as_rank));
+  RET(check_dev_buf(d_vsums, 8, "V-sum buffer"));
   return shard_vsum(c, Frames(d_frames, frame_stride), batch, as_rank, reinterpret_cast<unsigned long long*>(d_vsums));
 }
 
@@ -1791,9 +1821,9 @@ int bevk_shard_render_balanced(bevk_ctx* c, const void* d_frames, int64_t frame_
   RET(shard_geometry(c));
   RET(check_stack(c, d_frames, frame_stride));
   RET(shard_balance_limits(c, batch));
-  if (as_rank < 0 || as_rank >= c->shard.world || as_rank >= SHARD_MAX_RANKS) return fail(BEVK_ERR_ARG, "rank %d out of range", as_rank);
-  if (!d_vsums || (reinterpret_cast<uintptr_t>(d_vsums) & 7)) return fail(BEVK_ERR_ARG, "V-sum buffer null or not 8-byte aligned");
-  if (!d_slabs || (reinterpret_cast<uintptr_t>(d_slabs) & 15)) return fail(BEVK_ERR_ARG, "slab buffer null or not 16-byte aligned");
+  RET(check_rank(c, as_rank));
+  RET(check_dev_buf(d_vsums, 8, "V-sum buffer"));
+  RET(check_dev_buf(d_slabs, 16, "slab buffer"));
   c->timed = true;
   return shard_render_balanced(c, Frames(d_frames, frame_stride), batch, as_rank,
                                reinterpret_cast<const unsigned long long*>(d_vsums), d_slabs);
@@ -1811,8 +1841,8 @@ int bevk_shard_render(bevk_ctx* c, const void* d_frames, int64_t frame_stride, i
   RET(use(c));
   RET(shard_geometry(c));
   RET(check_stack(c, d_frames, frame_stride));
-  if (as_rank < 0 || as_rank >= c->shard.world || as_rank >= SHARD_MAX_RANKS) return fail(BEVK_ERR_ARG, "rank %d out of range", as_rank);
-  if (!d_slabs || (reinterpret_cast<uintptr_t>(d_slabs) & 15)) return fail(BEVK_ERR_ARG, "slab buffer null or not 16-byte aligned");
+  RET(check_rank(c, as_rank));
+  RET(check_dev_buf(d_slabs, 16, "slab buffer"));
   c->timed = true;
   return shard_render(c, Frames(d_frames, frame_stride), batch, as_rank, d_slabs);
 }
@@ -1943,16 +1973,14 @@ int bevk_bev_run_scattered(bevk_ctx* c, const void* d_frames, int64_t frame_stri
   if (n_own) *n_own = mine;
   if (mine > 0 && !d_out_own) return fail(BEVK_ERR_ARG, "null output");
   const size_t half = (size_t)s.world * s.own_max * s.slab_bytes, rank_stride = (size_t)s.own_max * s.slab_bytes;
-  const SlabRect q = s.rect[s.rank];
   const Frames src = Frames(d_frames, frame_stride);
   s.last_link_bytes = 0;
   c->timed = false;
   long long vsum_bytes = 0;
   if (bal) RET(shard_exchange_vsums(c, src, batch, &vsum_bytes));
   const unsigned par = s.step++ & 1u;     // double buffer: a peer may already store step n+1 while this rank composes step n
-  if (q.ox1 > q.ox && s.cam_hi[s.rank] > s.cam_lo[s.rank]) {
-    OutWin w;
-    w.pitch = (q.ox1 - q.ox) * 3; w.ox = q.ox; w.oy = q.oy; w.ox1 = q.ox1; w.oy1 = q.oy1; w.stride = s.slab_bytes;
+  if (has_slab(s, s.rank)) {
+    OutWin w = slab_win(s, s.rank);
     w.world = s.world; w.src_off = (long long)(par * half + (size_t)s.rank * rank_stride);
     for (int r = 0; r < s.world; ++r) w.peer[r] = reinterpret_cast<uint8_t*>(s.peer_recv[r]);
     Frames rsrc = src;   // BALANCE: the peer-store render reads this rank's balanced copies
@@ -2052,20 +2080,17 @@ int bevk_bev_run_jpeg(bevk_ctx* c, const uint8_t* const* jpegs, const uint64_t* 
   NvtxRange nvtx_call("bevk_bev_run_jpeg (JPEG streams -> host canvases)");
   RET(use(c));
   RET(bgr_only(flags, "bevk_bev_run_jpeg"));
-  if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
+  RET(need_plan(c));
   if (!jpegs || !sizes || !out || batch < 1) return fail(BEVK_ERR_ARG, "bad argument");
-  const size_t fbytes = (size_t)c->FW * c->FH * 3, fpad = (fbytes + 255) & ~size_t(255), cbytes = (size_t)c->BW * c->BH * 3;
+  const size_t fpad = pad256((size_t)c->FW * c->FH * 3), cbytes = (size_t)c->BW * c->BH * 3;
   const int nf = batch * c->n_cam;
   RET(c->d_jpeg_frames.ensure(fpad * nf));
   RET(c->d_jpeg_canvas.ensure(cbytes * batch));
   RET(bevk_jpeg_decode(c, jpegs, sizes, nf, c->FW, c->FH, c->d_jpeg_frames.p, (int64_t)fpad));
-  if (car) {
-    RET(c->d_car.ensure(cbytes));
-    CU(cudaMemcpyAsync(c->d_car.p, car, cbytes, cudaMemcpyHostToDevice, c->stream));
-  }
+  const void* d_car = nullptr;
+  RET(upload_car(c, car, &d_car));
   c->timed = false;
-  RET(run_device(c, Frames(c->d_jpeg_frames.p, (long long)fpad), batch, car ? c->d_car.p : nullptr, flags, c->d_jpeg_canvas.p, 0,
-                 BEVK_MAX_CAMERAS));
+  RET(run_device(c, Frames(c->d_jpeg_frames.p, (long long)fpad), batch, d_car, flags, c->d_jpeg_canvas.p, 0, BEVK_MAX_CAMERAS));
   CU(cudaMemcpyAsync(out, c->d_jpeg_canvas.p, cbytes * batch, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaStreamSynchronize(c->stream));
   return BEVK_OK;
@@ -2092,24 +2117,13 @@ struct JpegIn {
   const uint8_t* car = nullptr;
 };
 
-static int jpeg_streams(bevk_ctx* c) {
-  auto& e = c->enc;
-  if (e.out_stream) return BEVK_OK;
-  CU(cudaStreamCreateWithFlags(&e.out_stream, cudaStreamNonBlocking));
-  for (int i = 0; i < 2; ++i) {
-    CU(cudaEventCreateWithFlags(&e.ev_sizes[i], cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&e.ev_out_free[i], cudaEventDisableTiming));
-  }
-  return BEVK_OK;
-}
-
 // Enqueue the encoder over n w x h images into slot s on the ctx stream: every kernel, then the D2H of the stream sizes
 // into page-locked memory and ev_sizes[s].  jpeg_collect(s) finishes the batch.  The per-block work buffers are single:
 // batches use them one after the other in stream order.
 static int jpeg_enqueue(bevk_ctx* c, int s, const JpegIn& in, int n, int w, int h, int quality) {
   using namespace jpeg;
   auto& e = c->enc;
-  RET(jpeg_streams(c));
+  if (!e.out_stream) RET(create_stream_set(&e.out_stream, {&e.ev_sizes[0], &e.ev_sizes[1], &e.ev_out_free[0], &e.ev_out_free[1]}));
   const int q = clamp_quality(quality);
   if (w != e.w || h != e.h || q != e.q) {   // header + tables depend on (w, h, quality) only
     Tables t;
@@ -2219,24 +2233,52 @@ static int capacity_error(int n, const uint64_t* sizes, uint64_t capacity) {
   return fail(BEVK_ERR_ARG, "the %d JPEG streams take %llu bytes, capacity is %llu", n, total, (unsigned long long)capacity);
 }
 
+// Encode n images chunk by chunk through the two slots.  enqueue(b0, nb, s, &in) enqueues what makes images
+// [b0, b0 + nb) and describes them in `in`; the encoder then runs on them in slot s.  A chunk's streams are collected
+// (wait for their sizes, D2H on out_stream) after the next chunk has been enqueued into the other slot.  whole: all
+// streams or none (a single chunk); otherwise the leading streams that fit in capacity.
+template <class Enqueue>
+static int jpeg_chunks(bevk_ctx* c, int n, int chunk, int w, int h, int quality, bool whole, uint8_t* out, uint64_t capacity,
+                       uint64_t* sizes, Enqueue enqueue) {
+  uint64_t used = 0;
+  bool full = false;
+  int s = 0, prev_b0 = -1, prev_nb = 0;
+  for (int b0 = 0; b0 < n; b0 += chunk, s ^= 1) {
+    const int nb = std::min(chunk, n - b0);
+    JpegIn in;
+    RET(enqueue(b0, nb, s, &in));
+    RET(jpeg_enqueue(c, s, in, nb, w, h, quality));
+    if (prev_b0 >= 0) RET(jpeg_collect(c, s ^ 1, prev_nb, out, capacity, whole, sizes + prev_b0, &used, &full));
+    prev_b0 = b0; prev_nb = nb;
+  }
+  RET(jpeg_collect(c, s ^ 1, prev_nb, out, capacity, whole, sizes + prev_b0, &used, &full));
+  CU(cudaStreamSynchronize(c->enc.out_stream));
+  return full ? capacity_error(n, sizes, capacity) : BEVK_OK;
+}
+
 static int jpeg_encode_device(bevk_ctx* c, const JpegIn& in, int n, int w, int h, int quality, uint8_t* out, uint64_t capacity,
                               uint64_t* sizes) {
   if (c->capturing) return fail(BEVK_ERR_ARG, "bevk_jpeg_encode synchronises and cannot be captured into a graph");
-  RET(jpeg_enqueue(c, 0, in, n, w, h, quality));
-  uint64_t used = 0;
-  bool full = false;
-  RET(jpeg_collect(c, 0, n, out, capacity, true, sizes, &used, &full));
-  CU(cudaStreamSynchronize(c->enc.out_stream));
-  return full ? capacity_error(n, sizes, capacity) : BEVK_OK;
+  return jpeg_chunks(c, n, n, w, h, quality, true, out, capacity, sizes, [&](int, int, int, JpegIn* p) {
+    *p = in;
+    return BEVK_OK;
+  });
+}
+
+// Images per chunk of the chunked device-frame calls.  8 canvases (24 MB at 1000^2: they stay in the 50 MB L2) beat the
+// whole batch at once on H100 (DESIGN.md section 4); BEVK_JPEG_CHUNK=n sets another size, 0 the whole batch.
+static int jpeg_chunk(int n) {
+  int chunk = std::min(n, 8);
+  if (const char* env = getenv("BEVK_JPEG_CHUNK")) chunk = atoi(env) > 0 ? std::min(n, atoi(env)) : n;
+  return chunk;
 }
 
 // ------------------------------------------------------------------ BEV canvases straight to JPEG (surroundBEV.py:340)
 // BevGenerator.__call__ then cv2.imencode: each chunk of frame-sets is rendered into ctx scratch and encoded there, and
 // only the streams come back.  Under BALANCE the canvases stay raw and the encoder applies colour balance and the car
-// (GainSrc), so k_gain does not run and the balanced canvas is never written.  The streams of chunk i are collected
-// (wait for their sizes, D2H on the encoder's out_stream) after chunk i+1 has been enqueued, into the other slot.
+// (GainSrc), so k_gain does not run and the balanced canvas is never written.
 static int to_jpeg_check(bevk_ctx* c, uint8_t* out, uint64_t* sizes) {
-  if (!c->planned) return fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
+  RET(need_plan(c));
   if (!out || !sizes) return fail(BEVK_ERR_ARG, "null host pointer");
   if (c->capturing) return fail(BEVK_ERR_ARG, "the BEV-to-JPEG calls synchronise and cannot be captured into a graph");
   uint64_t bound = 0;
@@ -2258,25 +2300,13 @@ int bevk_bev_run_to_jpeg(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_st
   RET(to_jpeg_check(c, out, sizes));
   HostIngest h;
   RET(ingest_setup(c, srcs, src_stride, batch, car, flags, &h));
-  const void* d_car = car ? c->d_car.p : nullptr;
-  uint64_t used = 0;
-  bool full = false;
-  int half = 0, prev_b0 = -1, prev_nb = 0;
-  for (int b0 = 0; b0 < batch; b0 += h.chunk, half ^= 1) {
-    const int nb = std::min(h.chunk, batch - b0);
-    Frames fsrc;
-    RET(ingest_chunk(c, h, srcs, src_stride, flags, b0, nb, half, &fsrc));
-    c->timed = false;
-    uint8_t* dcanvas = c->d_canvas.as<uint8_t>() + (size_t)half * h.chunk * h.cbytes;
-    RET(run_device(c, fsrc, nb, d_car, flags | kFlagRawBalance, dcanvas, 0, BEVK_MAX_CAMERAS));
-    CU(cudaEventRecord(c->ev_free[half], c->stream));               // frames of this half are free again
-    RET(jpeg_enqueue(c, half, canvas_in(c, dcanvas, flags, d_car), nb, c->BW, c->BH, quality));
-    if (prev_b0 >= 0) RET(jpeg_collect(c, half ^ 1, prev_nb, out, capacity, false, sizes + prev_b0, &used, &full));
-    prev_b0 = b0; prev_nb = nb;
-  }
-  RET(jpeg_collect(c, half ^ 1, prev_nb, out, capacity, false, sizes + prev_b0, &used, &full));
-  CU(cudaStreamSynchronize(c->enc.out_stream));
-  return full ? capacity_error(batch, sizes, capacity) : BEVK_OK;
+  // the ingest chunks are the encoder's: staging half = canvas half = encoder slot
+  return jpeg_chunks(c, batch, h.chunk, c->BW, c->BH, quality, false, out, capacity, sizes, [&](int b0, int nb, int half, JpegIn* in) -> int {
+    uint8_t* dcanvas = nullptr;
+    RET(render_chunk(c, h, srcs, src_stride, flags | kFlagRawBalance, b0, nb, half, &dcanvas));
+    *in = canvas_in(c, dcanvas, flags, h.d_car);
+    return BEVK_OK;
+  });
 }
 
 int bevk_bev_frames_to_jpeg(bevk_ctx* c, const void* const* frames, int batch, const void* d_car, int flags, int quality,
@@ -2288,31 +2318,19 @@ int bevk_bev_frames_to_jpeg(bevk_ctx* c, const void* const* frames, int batch, c
   if (!frames) return fail(BEVK_ERR_ARG, "null pointer");
   Frames src;
   RET(frames_src(c, frames, batch, &src));
-  // chunks of frame-sets rendered into one canvas scratch and encoded there, chunk i's streams copied out while chunk
-  // i+1 is rendered and encoded.  8 canvases (24 MB at 1000^2: they stay in the 50 MB L2) beat the whole batch at once
-  // on H100 (DESIGN.md section 4); BEVK_JPEG_CHUNK=n sets another size, 0 the whole batch.
-  int chunk = std::min(batch, 8);
-  if (const char* env = getenv("BEVK_JPEG_CHUNK")) chunk = atoi(env) > 0 ? std::min(batch, atoi(env)) : batch;
-  const size_t cbytes = (size_t)c->BW * c->BH * 3;
-  RET(c->d_canvas.ensure(cbytes * chunk));
+  // every chunk is rendered into the same canvas scratch: the next render is stream-ordered after the encoder read it
+  const int chunk = jpeg_chunk(batch);
+  RET(c->d_canvas.ensure((size_t)c->BW * c->BH * 3 * chunk));
   uint8_t* dcanvas = c->d_canvas.as<uint8_t>();
-  uint64_t used = 0;
-  bool full = false;
-  int slot = 0, prev_b0 = -1, prev_nb = 0;
-  for (int b0 = 0; b0 < batch; b0 += chunk, slot ^= 1) {
-    const int nb = std::min(chunk, batch - b0);
+  return jpeg_chunks(c, batch, chunk, c->BW, c->BH, quality, false, out, capacity, sizes, [&](int b0, int nb, int, JpegIn* in) -> int {
     Frames part = src;
     if (part.table) part.table += (size_t)b0 * c->n_cam;
     else part.base += (long long)b0 * c->n_cam * part.stride;
     c->timed = false;
     RET(run_device(c, part, nb, d_car, flags | kFlagRawBalance, dcanvas, 0, BEVK_MAX_CAMERAS));
-    RET(jpeg_enqueue(c, slot, canvas_in(c, dcanvas, flags, d_car), nb, c->BW, c->BH, quality));
-    if (prev_b0 >= 0) RET(jpeg_collect(c, slot ^ 1, prev_nb, out, capacity, false, sizes + prev_b0, &used, &full));
-    prev_b0 = b0; prev_nb = nb;
-  }
-  RET(jpeg_collect(c, slot ^ 1, prev_nb, out, capacity, false, sizes + prev_b0, &used, &full));
-  CU(cudaStreamSynchronize(c->enc.out_stream));
-  return full ? capacity_error(batch, sizes, capacity) : BEVK_OK;
+    *in = canvas_in(c, dcanvas, flags, d_car);
+    return BEVK_OK;
+  });
 }
 
 int bevk_jpeg_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, int64_t row_stride, int n, int width, int height,
@@ -2334,7 +2352,7 @@ int bevk_undistort_jpeg(bevk_ctx* c, int slot, const uint8_t* src, int sw, int s
                         uint8_t* out, uint64_t capacity, uint64_t* size) {
   NvtxRange nvtx_call("bevk_undistort_jpeg (host frame -> undistorted JPEG)");
   RET(use(c));
-  if (slot < 0 || slot >= 8 || !c->und[slot].valid) return fail(BEVK_ERR_ARG, "undistorter slot %d not set", slot);
+  RET(need_undistorter(c, slot));
   if (!out || !size) return fail(BEVK_ERR_ARG, "bad argument");
   const int dw = c->und[slot].cm.w, dh = c->und[slot].cm.h;
   uint64_t bound = 0;
@@ -2359,30 +2377,18 @@ int bevk_undistort_stack_jpeg(bevk_ctx* c, int slot, const void* d_src, int64_t 
   const int dw = a.dw, dh = a.dh;
   uint64_t bound = 0;
   RET(bevk_jpeg_encode_bound(dw, dh, &bound));
-  // same chunking as bevk_bev_frames_to_jpeg: 8 images by default, BEVK_JPEG_CHUNK=n another size, 0 the whole batch
-  int chunk = std::min(n, 8);
-  if (const char* env = getenv("BEVK_JPEG_CHUNK")) chunk = atoi(env) > 0 ? std::min(n, atoi(env)) : n;
+  const int chunk = jpeg_chunk(n);
   const long long ibytes = (long long)dw * dh * 3;
   RET(c->s_dst.ensure((size_t)ibytes * chunk));
-  uint64_t used = 0;
-  bool full = false;
-  int s = 0, prev_b0 = -1, prev_nb = 0;
-  for (int b0 = 0; b0 < n; b0 += chunk, s ^= 1) {
-    const int nb = std::min(chunk, n - b0);
+  return jpeg_chunks(c, n, chunk, dw, dh, quality, false, out, capacity, sizes, [&](int b0, int nb, int, JpegIn* in) -> int {
     GatherArgs part = a;
     part.src += (long long)b0 * a.sistride;
     part.n = nb;
     part.dst = c->s_dst.as<uint8_t>(); part.dpitch = (long long)dw * 3; part.distride = ibytes;
     RET(launch_undistort(c, slot, part, 3, interp));
-    JpegIn in;
-    in.img = c->s_dst.p; in.pitch = (long long)dw * 3; in.istride = ibytes;
-    RET(jpeg_enqueue(c, s, in, nb, dw, dh, quality));
-    if (prev_b0 >= 0) RET(jpeg_collect(c, s ^ 1, prev_nb, out, capacity, false, sizes + prev_b0, &used, &full));
-    prev_b0 = b0; prev_nb = nb;
-  }
-  RET(jpeg_collect(c, s ^ 1, prev_nb, out, capacity, false, sizes + prev_b0, &used, &full));
-  CU(cudaStreamSynchronize(c->enc.out_stream));
-  return full ? capacity_error(n, sizes, capacity) : BEVK_OK;
+    in->img = c->s_dst.p; in->pitch = (long long)dw * 3; in->istride = ibytes;
+    return BEVK_OK;
+  });
 }
 
 // ------------------------------------------------------------------ CUDA graphs

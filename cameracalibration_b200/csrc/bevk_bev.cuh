@@ -42,20 +42,28 @@ struct BevItem {
   int cam, orient;         // orient 0: lanes along canvas x, 1: lanes along canvas y
 };
 
-struct BevParams {
-  Frames srcs;                  // the batch * n_cam dense BGR frames
+// The parameters both fused kernels (k_bev, k_bev_tma) take; BevParams and TmaParams add their own plan and sources.
+struct RenderParams {
   int n_cam, FW, FH;
   unsigned pitch;               // source row pitch in bytes (= 3*FW)
-  const int4* tiles;            // x0, y0, first item, item count
-  const BevItem* items;
-  const uint4* lut;             // [item][4][256]
   int n_tiles, batch;
-  uint8_t* out; int BW, BH; long long canvas_bytes;
+  uint8_t* out; int BW, BH; long long canvas_bytes;   // canvas_bytes: stride between the frame-sets' outputs
   const uint8_t* car;
   unsigned long long* csum;     // [batch * 3] channel sums of the composed canvas (BALANCE)
   int cam_lo, cam_hi;
-  // output window (see TmaParams): canvas pixels [ox,ox1) x [oy,oy1) -> out + (y-oy)*out_pitch + (x-ox)*3
+  // output window (camera-sharded runs render only the tile-aligned bounding box of their cameras' masks, a "slab"):
+  // canvas pixels [ox,ox1) x [oy,oy1) go to out + (y-oy)*out_pitch + (x-ox)*3; the full canvas is 0,0,BW,BH, pitch 3*BW
   int out_pitch, ox, oy, ox1, oy1;
+  // k_bev_tma only: producer poll interval while the ring is full (0: spin).  Kept next to oy1, which k_bev_tma loads
+  // together with it as one 8-byte parameter word.
+  int backoff_ns;
+};
+
+struct BevParams : RenderParams {
+  const int4* tiles;            // x0, y0, first item, item count
+  const BevItem* items;
+  const uint4* lut;             // [item][4][256]
+  Frames srcs;                  // the batch * n_cam dense BGR frames
 };
 
 // read-only global loads; the host forms serve tests/host/kernel_math.cu

@@ -55,24 +55,13 @@ struct __align__(16) TmaItem {   // 32 B, read as two 16-byte words
 };
 static_assert(sizeof(TmaItem) == 32, "TmaItem is read as two int4");
 
-struct TmaParams {
-  const uint8_t* maps;           // [n_shapes] CUtensorMap (128 B each) in global memory
-  const uint8_t* base;           // frame 0 of the stack (GATHER items, slow entries)
-  long long frame_stride;        // bytes between consecutive frames
-  int n_cam, FW, FH;
-  unsigned pitch;
+struct TmaParams : RenderParams {
   const int4* tiles;             // x0, y0, first item, item count
   const TmaItem* items;
   const uint4* lut;
-  int n_tiles, batch;
-  uint8_t* out; int BW, BH; long long canvas_bytes;   // canvas_bytes: stride between the frame-sets' outputs
-  const uint8_t* car;
-  unsigned long long* csum;
-  int cam_lo, cam_hi;
-  // output window (camera-sharded runs render only the tile-aligned bounding box of their cameras' masks, a "slab"):
-  // canvas pixels [ox,ox1) x [oy,oy1) go to out + (y-oy)*out_pitch + (x-ox)*3; the full canvas is 0,0,BW,BH, pitch 3*BW
-  int out_pitch, ox, oy, ox1, oy1;
-  int backoff_ns;                // producer poll interval while the ring is full (0: spin)
+  const uint8_t* maps;           // [n_shapes] CUtensorMap (128 B each) in global memory
+  const uint8_t* base;           // frame 0 of the stack (GATHER items, slow entries)
+  long long frame_stride;        // bytes between consecutive frames
   unsigned* unit_counter;        // zeroed before the launch: next unit to hand out
   // camera-sharded runs with peer stores (bevk_bev_run_scattered): the output of frame-set b goes straight into the memory
   // of the rank that owns b -- peer[b % world] + src_off + (b / world) * canvas_bytes -- over NVLink; world == 0: plain `out`
