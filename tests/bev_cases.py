@@ -3,12 +3,15 @@
 interpolation, frame-sets), plus the oracle every consumer compares with: cv2.remap per camera (BORDER_CONSTANT 0),
 the mask weight (restate.apply_blend), the saturating compose in camera order, and -- with BALANCE -- the reference's
 luminance / colour balance restated, then the car.  Maps are given to the engine through set_maps, so the host
-interpreter and the device render exactly the input the oracle sees."""
+interpreter and the device render exactly the input the oracle sees.
+
+yuv_corpus() carries the same kind of cases with NV12 / I420 frames instead (tests/test_host_yuv.py,
+tests/test_gpu_yuv_fuzz.py); its oracle is cv2.cvtColor of every frame followed by the BGR oracle."""
 from __future__ import annotations
 
 import os
 import re
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 from functools import lru_cache
 
 import cv2
@@ -16,6 +19,7 @@ import numpy as np
 
 from oracle import cv2_path as C
 from oracle import restate as R
+from tests import yuv_frames as Y
 
 
 @dataclass
@@ -31,6 +35,7 @@ class Case:
     masks: list                    # per camera uint8[BH][BW]
     sets: list = field(default_factory=list)   # frame-sets: list (batch) of lists (camera) of uint8[FH][FW][3]
     car: np.ndarray | None = None
+    yuv: list | None = None        # YUV corpus: frame-sets of YUV 4:2:0 buffers uint8[FH*3/2][FW] (sets: see yuv_bgr_case)
 
     @property
     def NC(self) -> int:
@@ -188,6 +193,26 @@ def _smooth_maps(rng, k, FW, FH, BW, BH):
     return C.RefCamera(K, D, H, g).bev_maps
 
 
+def _maps(rng, kind, NC, FW, FH, BW, BH):
+    """Per camera (map1, map2) of a case of this kind: smooth fisheye + homography, random local taps within 6 px of the
+    frame, or int16-extreme taps (a band of ordinary ones); local and extreme maps also get the edge taps."""
+    maps = []
+    for k in range(NC):
+        if kind == "smooth":
+            m1, m2 = _smooth_maps(rng, k, FW, FH, BW, BH)
+            m1 = np.array(m1, np.int16)
+        else:
+            lo, hi = (-6, 6) if kind == "local" else (-40000, 40000)
+            m1 = np.stack([rng.integers(lo, FW + hi, (BH, BW)), rng.integers(lo, FH + hi, (BH, BW))], -1)
+            m1 = m1.clip(-32768, 32767).astype(np.int16)
+            if kind == "extreme":   # a band of ordinary taps, so that extreme cases still stage some boxes
+                m1[: BH // 3] = np.stack([rng.integers(0, FW, (BH // 3, BW)), rng.integers(0, FH, (BH // 3, BW))], -1)
+            _edge_taps(rng, m1, FW, FH)
+            m2 = rng.integers(0, 1024, (BH, BW)).astype(np.uint16)
+        maps.append((m1, np.ascontiguousarray(m2, np.uint16)))
+    return maps
+
+
 def _frames(rng, NC, FW, FH, bright, n_sets):
     base = [rng.integers(160 if bright else 0, 256, (FH, FW, 3), dtype=np.uint8) for _ in range(NC)]
     sets = [base]
@@ -215,20 +240,7 @@ def make_case(seed: int, n_sets: int = 9) -> Case:
         BW, BH = _CANVAS[idx % 6]
     NC = 4 if seed % 2 == 0 else int((1, 2, 3, 5, 6, 7, 8)[idx % 7])
     nearest = seed % 5 == 3
-    maps = []
-    for k in range(NC):
-        if kind == "smooth":
-            m1, m2 = _smooth_maps(rng, k, FW, FH, BW, BH)
-            m1 = np.array(m1, np.int16)
-        else:
-            lo, hi = (-6, 6) if kind == "local" else (-40000, 40000)
-            m1 = np.stack([rng.integers(lo, FW + hi, (BH, BW)), rng.integers(lo, FH + hi, (BH, BW))], -1)
-            m1 = m1.clip(-32768, 32767).astype(np.int16)
-            if kind == "extreme":   # a band of ordinary taps, so that extreme cases still stage some boxes
-                m1[: BH // 3] = np.stack([rng.integers(0, FW, (BH // 3, BW)), rng.integers(0, FH, (BH // 3, BW))], -1)
-            _edge_taps(rng, m1, FW, FH)
-            m2 = rng.integers(0, 1024, (BH, BW)).astype(np.uint16)
-        maps.append((m1, np.ascontiguousarray(m2, np.uint16)))
+    maps = _maps(rng, kind, NC, FW, FH, BW, BH)
     masks = _masks(rng, NC, BW, BH, seed)
     bright = seed % 4 in (1, 2)
     sets = _frames(rng, NC, FW, FH, bright, n_sets)
@@ -243,3 +255,71 @@ def corpus():
 
 def case_by_name(name: str) -> Case:
     return next(c for c in corpus() if c.name == name)
+
+
+# ------------------------------------------------------------------ the YUV 4:2:0 corpus
+# Frame-sets per YUV case: a call of up to 9 sets starts at set 0 or set 1, so that consecutive calls on one engine never
+# present the same frame at the same frame index (the copy stack keeps an earlier call's conversion outside the spans).
+N_YUV_SETS = 10
+# The supplement: (kind, FW, FH, (BW, BH), cameras, nearest, bright).  Widths with FW % 4 == 2 (a last group of 2 pixels,
+# a copy-stack pitch that is not a multiple of 4: k_bev's per-tap path), FW % 16 == 4 * k (k_bev on the copy stack, DMA
+# rectangles for page-locked frames) and FW % 32 == 16 (k_bev_tma with the luminance row tail; I420 windows crossing
+# the U / V halves of a buffer row); heights with FH % 4 == 2 (the I420 V plane starts mid-row); 1-8 cameras.
+_YUV_SUPPLEMENT = (
+    ("local", 30, 38, (52, 68), 4, False, False),
+    ("extreme", 98, 54, (77, 45), 4, True, True),
+    ("smooth", 118, 198, (100, 90), 4, False, False),
+    ("smooth", 52, 130, (150, 118), 4, True, False),
+    ("local", 112, 66, (77, 45), 4, False, True),
+    ("smooth", 176, 150, (64, 77), 4, False, False),
+    ("extreme", 80, 42, (96, 64), 4, False, False),
+    ("extreme", 36, 42, (29, 70), 5, False, True),
+    ("local", 30, 26, (23, 17), 6, True, False),
+    ("extreme", 80, 34, (64, 96), 7, False, False),
+    ("smooth", 64, 122, (64, 77), 8, False, True),
+    ("local", 98, 30, (96, 64), 3, False, True),
+    ("extreme", 118, 22, (77, 45), 2, True, False),
+    ("local", 48, 20, (23, 17), 1, False, False),
+)
+
+
+def _yuv_sets(rng, NC, FW, FH, bright):
+    """N_YUV_SETS independent frame-sets of random YUV 4:2:0 buffers (Y < 16 and chroma that saturates the conversion
+    included); bright: Y in [200, 256) (saturating adds in the compose)."""
+    sets = []
+    for _ in range(N_YUV_SETS):
+        fs = [Y.random_yuv(rng, FW, FH) for _ in range(NC)]
+        if bright:
+            for f in fs:
+                f[:FH] = rng.integers(200, 256, (FH, FW), dtype=np.uint8)
+        sets.append(fs)
+    return sets
+
+
+@lru_cache(maxsize=None)
+def yuv_corpus() -> tuple:
+    """The even-sized cases of corpus() (their maps, masks and car; bright frames where the BGR case has them) and the
+    seeded supplement, each with YUV frame-sets in `yuv` and no BGR ones: yuv_bgr_case gives the frames the oracle sees."""
+    out = []
+    for s in range(N_CASES):
+        c = make_case(s)
+        if c.FW % 2 == 0 and c.FH % 2 == 0:
+            rng = np.random.default_rng(2000 + s)
+            out.append(replace(c, sets=[], yuv=_yuv_sets(rng, c.NC, c.FW, c.FH, s % 4 in (1, 2))))
+    for i, (kind, FW, FH, (BW, BH), NC, nearest, bright) in enumerate(_YUV_SUPPLEMENT):
+        rng = np.random.default_rng(3000 + i)
+        maps = _maps(rng, kind, NC, FW, FH, BW, BH)
+        masks = _masks(rng, NC, BW, BH, 100 + i)
+        car = rng.integers(0, 256, (BH, BW, 3), dtype=np.uint8)
+        car[rng.integers(0, 2, (BH, BW)) == 0] = 0
+        out.append(Case(f"yuv_{kind}{i}", kind, FW, FH, BW, BH, nearest, maps, masks, [], car,
+                        _yuv_sets(rng, NC, FW, FH, bright)))
+    return tuple(out)
+
+
+@lru_cache(maxsize=None)
+def yuv_bgr_case(name: str, fmt: str) -> Case:
+    """YUV corpus case `name` with sets = cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420) of its YUV frame-sets: what oracle()
+    and compose() take, and what a BGR render of the same case reads."""
+    c = next(c for c in yuv_corpus() if c.name == name)
+    return replace(c, sets=[[Y.to_bgr(f, fmt) for f in fs] for fs in c.yuv])

@@ -82,13 +82,15 @@ class Want:
             self.memo[k] = B.oracle(self.case, s, balance, car)
         return self.memo[k]
 
-    def check(self, got, balance, car, what):
+    def check(self, got, balance, car, what, sets=None):
+        """got[i] against the oracle of frame-set sets[i] (default: i)."""
         compared = 0
-        for s in range(got.shape[0]):
+        for i in range(got.shape[0]):
+            s = i if sets is None else sets[i]
             w = self(s, balance, car)
             if w is None:          # BALANCE of a canvas with a zero channel mean: the reference divides by zero
                 continue
-            assert (got[s] == w).all(), (self.case.name, what, s, balance, car, int((got[s] != w).sum()))
+            assert (got[i] == w).all(), (self.case.name, what, s, balance, car, int((got[i] != w).sum()))
             compared += 1
         assert compared > 0, (self.case.name, what, "no frame-set has a defined oracle")
         return compared
@@ -103,9 +105,9 @@ def _stack(torch, case, n, pad):
     return torch.from_numpy(host.reshape(-1)).cuda(), stride
 
 
-def _render(torch, e, d, stride, n, car, balance, off=16, car_off=0):
-    """run_stack into a buffer with 0xA5 sentinels: `off` bytes before the output and a whole canvas after it.  The car
-    (if any) is placed at byte `car_off` of its own buffer."""
+def _render(torch, e, d, stride, n, car, balance, off=16, car_off=0, pixel_format="bgr", base=0):
+    """run_stack of the frames at byte `base` of d into a buffer with 0xA5 sentinels: `off` bytes before the output and
+    a whole canvas after it.  The car (if any) is placed at byte `car_off` of its own buffer."""
     cb = e.BW * e.BH * 3
     buf = torch.full((off + (n + 1) * cb,), 0xA5, dtype=torch.uint8, device=d.device)
     cptr = 0
@@ -113,7 +115,7 @@ def _render(torch, e, d, stride, n, car, balance, off=16, car_off=0):
         cbuf = torch.zeros(cb + 16, dtype=torch.uint8, device=d.device)
         cbuf[car_off:car_off + cb] = torch.from_numpy(car.reshape(-1)).to(d.device)
         cptr = cbuf.data_ptr() + car_off
-    e.run_stack(d.data_ptr(), stride, n, buf.data_ptr() + off, cptr, balance)
+    e.run_stack(d.data_ptr() + base, stride, n, buf.data_ptr() + off, cptr, balance, pixel_format=pixel_format)
     e.ctx.sync()
     h = buf.cpu().numpy()
     assert (h[:off] == 0xA5).all() and (h[off + n * cb:] == 0xA5).all(), "bytes written outside the output"
