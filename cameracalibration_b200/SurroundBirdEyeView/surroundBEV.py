@@ -298,17 +298,20 @@ class BevGenerator:
     def __call__(self, front, back, left, right, car=None):
         return self.engine.run([[front, back, left, right]], car, self.balance)[0]
 
-    def run_batch(self, frame_sets, car=None, out=None, pixel_format="bgr"):
+    def run_batch(self, frame_sets, car=None, out=None, pixel_format="bgr", out_format="bgr"):
         """frame_sets: iterable of (front, back, left, right) tuples -> uint8[n][BH][BW][3].  pixel_format "nv12" /
         "i420": the frames are YUV 4:2:0 buffers uint8[FH*3//2][FW] (cv2's layout), converted to BGR on the GPU exactly
-        as cv2.cvtColor does."""
-        return self.engine.run([list(fs) for fs in frame_sets], car, self.balance, out, pixel_format=pixel_format)
+        as cv2.cvtColor does.  out_format "nv12" / "i420": the canvases come back as uint8[n][BH*3//2][BW], each
+        cv2.cvtColor(canvas, COLOR_BGR2YUV_I420) (NV12: U and V interleaved), converted on the GPU."""
+        return self.engine.run([list(fs) for fs in frame_sets], car, self.balance, out, pixel_format=pixel_format,
+                               out_format=out_format)
 
-    def run_cuda(self, frames, car=None, out=None, stream=None, pixel_format="bgr"):
+    def run_cuda(self, frames, car=None, out=None, stream=None, pixel_format="bgr", out_format="bgr"):
         """Frame-sets that are already on the GPU (uint8 CUDA array [n][4][FH][FW][3] in front/back/left/right
         order, or nested lists of per-frame CUDA arrays) -> CUDA array [n][BH][BW][3]; nothing crosses PCIe.
-        pixel_format "nv12" / "i420": one uint8 CUDA array [n][4][FH*3//2][FW] of YUV 4:2:0 frames."""
-        return self.engine.run_cuda(frames, car, self.balance, out, stream, pixel_format=pixel_format)
+        pixel_format "nv12" / "i420": one uint8 CUDA array [n][4][FH*3//2][FW] of YUV 4:2:0 frames.  out_format
+        "nv12" / "i420": the result is uint8[n][BH*3//2][BW] YUV 4:2:0 canvases (see run_batch)."""
+        return self.engine.run_cuda(frames, car, self.balance, out, stream, pixel_format=pixel_format, out_format=out_format)
 
     def jpeg(self, front, back, left, right, car=None, quality=95):
         """cv2.imencode('.jpg', self(front, back, left, right, car), [IMWRITE_JPEG_QUALITY, quality]) -- the bytes

@@ -17,6 +17,8 @@ MODEL_FISHEYE, MODEL_PINHOLE = 0, 1
 FLAG_BALANCE = 1
 FLAG_NV12, FLAG_I420 = 2, 4          # YUV 4:2:0 frames (cv2's single-buffer layout), bevk_bev_run / _run_stack only
 PIXEL_FORMATS = {"bgr": 0, "nv12": FLAG_NV12, "i420": FLAG_I420}
+FLAG_OUT_NV12, FLAG_OUT_I420 = 8, 16  # YUV 4:2:0 canvases uint8[BH*3/2][BW] (cv2.cvtColor(COLOR_BGR2YUV_I420) layout)
+OUT_FORMATS = {"bgr": 0, "nv12": FLAG_OUT_NV12, "i420": FLAG_OUT_I420}
 SHARD_FRAMES, SHARD_CAMERAS = 0, 1
 MAX_CAMERAS = 8
 

@@ -174,6 +174,7 @@ struct bevk_ctx {
   int bev_grid[6] = {0, 0, 0, 0, 0, 0};   // resident CTAs of k_bev<BAL, NB>: index = 3*BAL + {NB=1:0, 4:1, 8:2}
   DevBuf d_frames, d_canvas, d_car, d_vsum, d_delta, d_csum;
   DevBuf d_spans, d_bal;                    // BALANCE: sampled row spans per camera, balanced frame copies
+  DevBuf d_out_bgr, d_out_yuv;              // YUV output: BGR canvases of the device entry points, YUV canvases of bevk_bev_run
   DevBuf d_user_ptrs;                       // bevk_bev_run_frames: device copy of the caller's frame table
   std::vector<const void*> user_tab;        // ... and what it currently holds
   // TMA-staged kernel (bevk_bev_tma.cuh): its plan, and the tensor maps of the frame stacks seen recently
@@ -960,11 +961,30 @@ static int bgr_only(int flags, const char* fn) {
   return BEVK_OK;
 }
 
+// Canvas format of a call from its flags: 0 = BGR, YUV_NV12, YUV_I420.  YUV needs an even canvas, as cv2 does.
+constexpr int kOutFlags = BEVK_FLAG_OUT_NV12 | BEVK_FLAG_OUT_I420;
+static int out_format(bevk_ctx* c, int flags, int* ofmt) {
+  const int o = flags & kOutFlags;
+  *ofmt = 0;
+  if (!o) return BEVK_OK;
+  if (o == kOutFlags) return fail(BEVK_ERR_ARG, "BEVK_FLAG_OUT_NV12 and BEVK_FLAG_OUT_I420 are exclusive");
+  if ((c->BW | c->BH) & 1) return fail(BEVK_ERR_UNSUPPORTED, "YUV 4:2:0 canvases need an even size, not %d x %d", c->BW, c->BH);
+  *ofmt = o == BEVK_FLAG_OUT_NV12 ? YUV_NV12 : YUV_I420;
+  return BEVK_OK;
+}
+
+// Entry points that write BGR canvases only refuse the output flags rather than write BGR where YUV was asked for.
+static int bgr_canvas_only(int flags, const char* fn) {
+  if (flags & kOutFlags) return fail(BEVK_ERR_UNSUPPORTED, "%s writes BGR canvases only (no output flags)", fn);
+  return BEVK_OK;
+}
+
 int bevk_bev_host_copy_bytes(bevk_ctx* c, int flags, int64_t* h2d, int64_t* d2h) {
   RET(use(c));
   RET(need_plan(c));
-  int fmt = 0;
+  int fmt = 0, ofmt = 0;
   RET(pixel_format(c, flags, &fmt));
+  RET(out_format(c, flags, &ofmt));
   int64_t up = 0;
   for (int k = 0; k < c->n_cam; ++k) {
     if (flags & BEVK_FLAG_BALANCE) { up += (int64_t)c->FW * c->FH * (fmt ? 3 : 6) / 2; continue; }
@@ -976,7 +996,7 @@ int bevk_bev_host_copy_bytes(bevk_ctx* c, int flags, int64_t* h2d, int64_t* d2h)
       up += (int64_t)(c->cam_box[k][bnd][1] - c->cam_box[k][bnd][0]) * (c->cam_box[k][bnd][3] - c->cam_box[k][bnd][2]);
   }
   if (h2d) *h2d = up;
-  if (d2h) *d2h = (int64_t)c->BW * c->BH * 3;
+  if (d2h) *d2h = (int64_t)c->BW * c->BH * (ofmt ? 3 : 6) / 2;
   return BEVK_OK;
 }
 
@@ -1240,11 +1260,64 @@ static int run_device(bevk_ctx* c, Frames src, int batch, const void* d_car, int
   return BEVK_OK;
 }
 
+// k_canvas_yuv over `batch` BGR canvases (dense, 4-byte aligned scratch) into `batch` YUV canvases at out (any alignment).
+// csum non-null: the canvases are raw BALANCE renders with those channel sums, and colour balance and the car come first.
+static int launch_canvas_yuv(bevk_ctx* c, int ofmt, const uint8_t* canvases, int batch, const unsigned long long* csum,
+                             const void* d_car, void* out) {
+  CanvasYuvArgs a{canvases, reinterpret_cast<uint8_t*>(out), c->BW, c->BH, csum, csum ? reinterpret_cast<const uint8_t*>(d_car) : nullptr,
+                  (double)c->BW * (double)c->BH};
+  const long long items = (long long)((c->BW + 3) / 4) * (c->BH / 2);
+  const dim3 grid((unsigned)std::max<long long>(1, std::min<long long>(items / 256 + 1, c->n_sm * 8 / std::max(1, std::min(batch, 64)) + 1)),
+                  (unsigned)batch);
+  if (ofmt == YUV_NV12) {
+    if (csum) k_canvas_yuv<YUV_NV12, true><<<grid, 256, 0, c->stream>>>(a);
+    else k_canvas_yuv<YUV_NV12, false><<<grid, 256, 0, c->stream>>>(a);
+  } else {
+    if (csum) k_canvas_yuv<YUV_I420, true><<<grid, 256, 0, c->stream>>>(a);
+    else k_canvas_yuv<YUV_I420, false><<<grid, 256, 0, c->stream>>>(a);
+  }
+  LAUNCHED(c);
+  return BEVK_OK;
+}
+
+// One whole-canvas render in canvas format ofmt (out_format): BGR canvases straight into d_out; YUV ones as BGR into
+// `scratch`, converted from there into d_out by k_canvas_yuv.  With BALANCE the render stops at the raw canvas and the
+// conversion applies colour balance and the car, so k_gain does not run.  The one conversion step of the host and the
+// device entry points.
+static int render_to(bevk_ctx* c, Frames src, int batch, const void* d_car, int flags, int ofmt, uint8_t* scratch, void* d_out) {
+  if (!ofmt) return run_device(c, src, batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
+  RET(run_device(c, src, batch, d_car, (flags & ~kOutFlags) | kFlagRawBalance, scratch, 0, BEVK_MAX_CAMERAS));
+  return launch_canvas_yuv(c, ofmt, scratch, batch, (flags & BEVK_FLAG_BALANCE) ? c->d_csum.as<unsigned long long>() : nullptr,
+                           d_car, d_out);
+}
+
+// The device entry points' render: run_device for BGR canvases; for YUV ones render_to over the whole batch through
+// d_out_bgr.  Rendering in chunks of 8 frame-sets, so that the conversion reads canvases still in L2, was slower: the
+// fused kernels lose more on the smaller batches than the conversion gains (DESIGN.md section 4).  Only enqueues;
+// bevk_last_kernel_ms covers the render and the conversion.
+static int run_canvases(bevk_ctx* c, Frames src, int batch, const void* d_car, int flags, void* d_out) {
+  int ofmt = 0;
+  RET(need_plan(c));
+  RET(out_format(c, flags, &ofmt));
+  if (!ofmt) return run_device(c, src, batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
+  if (!d_out) return fail(BEVK_ERR_ARG, "null device pointer");
+  if (batch < 1 || batch > 65535) return fail(BEVK_ERR_ARG, "batch %d out of range [1,65535]", batch);
+  RET(c->d_out_bgr.ensure((size_t)c->BW * c->BH * 3 * batch));
+  const bool timed = c->timed;
+  if (timed && !c->capturing) CU(cudaEventRecord(c->ev0, c->stream));
+  c->timed = false;   // the render records no events of its own
+  const int rc = render_to(c, src, batch, d_car, flags, ofmt, c->d_out_bgr.as<uint8_t>(), d_out);
+  c->timed = timed;
+  RET(rc);
+  if (timed && !c->capturing) CU(cudaEventRecord(c->ev1, c->stream));
+  return BEVK_OK;
+}
+
 int bevk_bev_run_device(bevk_ctx* c, const void* d_srcs, int batch, const void* d_car, int flags, void* d_out) {
   RET(use(c));
   RET(bgr_only(flags, "bevk_bev_run_device"));
   c->timed = true;
-  return run_device(c, Frames(d_srcs), batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
+  return run_canvases(c, Frames(d_srcs), batch, d_car, flags, d_out);
 }
 
 // frames[i] == frames[0] + i * stride with a 16-byte friendly stride?  (a frame stack: the TMA-staged kernel applies)
@@ -1293,7 +1366,7 @@ int bevk_bev_run_frames(bevk_ctx* c, const void* const* frames, int batch, const
   Frames src;
   RET(frames_src(c, frames, batch, &src));
   c->timed = true;
-  return run_device(c, src, batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
+  return run_canvases(c, src, batch, d_car, flags, d_out);
 }
 
 static int check_stack(bevk_ctx* c, const void* d_frames, int64_t frame_stride) {
@@ -1315,7 +1388,7 @@ int bevk_bev_run_stack(bevk_ctx* c, const void* d_frames, int64_t frame_stride, 
     RET(check_stack(c, d_frames, frame_stride));
   }
   c->timed = true;
-  return run_device(c, Frames(d_frames, frame_stride), batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
+  return run_canvases(c, Frames(d_frames, frame_stride), batch, d_car, flags, d_out);
 }
 
 int bevk_bev_run_stack_cams(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, int cam_lo, int cam_hi, void* d_out) {
@@ -1357,6 +1430,8 @@ int bevk_sat_sum_device(bevk_ctx* c, const void* const* parts, int n, uint64_t b
 struct HostIngest {
   size_t row = 0, fbytes = 0, fpad = 0, cbytes = 0;
   int fmt = 0, rows = 0;                  // pixel format (0 = BGR) and buffer rows of a frame (FH; FH * 3 / 2 for YUV)
+  int ofmt = 0;                           // canvas format (out_format), and the bytes of one canvas in it
+  size_t obytes = 0;
   int chunk = 0;
   bool zero_copy = false;
   const void* d_car = nullptr;            // the car overlay on the device, or null
@@ -1379,14 +1454,16 @@ static int ingest_setup(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_str
   RET(need_plan(c));
   if (!srcs) return fail(BEVK_ERR_ARG, "null host pointer");
   if (batch < 1) return fail(BEVK_ERR_ARG, "batch must be >= 1");
-  int fmt = 0;
+  int fmt = 0, ofmt = 0;
   RET(pixel_format(c, flags, &fmt));
+  RET(out_format(c, flags, &ofmt));
   // a YUV frame is uint8[FH * 3 / 2][FW] at the same row stride; it is staged as it is and converted on the device
   const int rows = fmt ? c->FH * 3 / 2 : c->FH;
   const size_t row = (size_t)c->FW * (fmt ? 1 : 3), fbytes = row * rows, fpad = pad256(fbytes);
   if (src_stride < (int64_t)row) return fail(BEVK_ERR_ARG, "src_stride %lld < row bytes", (long long)src_stride);
   const size_t cbytes = (size_t)c->BW * c->BH * 3;
   h->row = row; h->fbytes = fbytes; h->fpad = fpad; h->cbytes = cbytes; h->fmt = fmt; h->rows = rows;
+  h->ofmt = ofmt; h->obytes = ofmt ? cbytes / 2 : cbytes;
   // Two-deep pipeline over chunks of frame-sets: the H2D copies of chunk i+1 run on the copy
   // stream while chunk i is rendered and its canvases go back on the main stream, so the two
   // PCIe directions overlap and the kernel hides under the copies.
@@ -1396,6 +1473,7 @@ static int ingest_setup(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_str
   const size_t set_frames = (size_t)c->n_cam;
   RET(c->d_frames.ensure(fpad * set_frames * chunk * 2));
   RET(c->d_canvas.ensure(cbytes * chunk * 2));
+  if (ofmt) RET(c->d_out_yuv.ensure(h->obytes * chunk * 2));
   if (!c->copy_stream)
     RET(create_stream_set(&c->copy_stream, {&c->ev_in[0], &c->ev_in[1], &c->ev_free[0], &c->ev_free[1], &c->ev_hp[0], &c->ev_hp[1]}));
   RET(upload_car(c, car, &h->d_car));
@@ -1489,14 +1567,16 @@ static int ingest_chunk(bevk_ctx* c, const HostIngest& h, const uint8_t* const* 
 }
 
 // One chunk of a host-frame call: frame-sets [b0, b0 + nb) ingested into staging half `half` and rendered into canvas
-// half `half` of d_canvas (*dcanvas), after which the staging half is free again.
+// half `half` of d_canvas (*dcanvas), after which the staging half is free again.  With a YUV canvas format the BGR
+// canvases in d_canvas are converted into half `half` of d_out_yuv, and *dcanvas points there.
 static int render_chunk(bevk_ctx* c, const HostIngest& h, const uint8_t* const* srcs, int64_t src_stride, int flags, int b0, int nb,
                         int half, uint8_t** dcanvas) {
   Frames fsrc;
   RET(ingest_chunk(c, h, srcs, src_stride, flags, b0, nb, half, &fsrc));
   c->timed = false;
-  *dcanvas = c->d_canvas.as<uint8_t>() + (size_t)half * h.chunk * h.cbytes;
-  RET(run_device(c, fsrc, nb, h.d_car, flags, *dcanvas, 0, BEVK_MAX_CAMERAS));
+  uint8_t* bgr = c->d_canvas.as<uint8_t>() + (size_t)half * h.chunk * h.cbytes;
+  *dcanvas = h.ofmt ? c->d_out_yuv.as<uint8_t>() + (size_t)half * h.chunk * h.obytes : bgr;
+  RET(render_to(c, fsrc, nb, h.d_car, flags, h.ofmt, bgr, *dcanvas));
   CU(cudaEventRecord(c->ev_free[half], c->stream));
   return BEVK_OK;
 }
@@ -1514,7 +1594,7 @@ int bevk_bev_run(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, in
     uint8_t* dcanvas = nullptr;
     RET(render_chunk(c, h, srcs, src_stride, flags, b0, nb, half, &dcanvas));
     NvtxRange nvtx_d2h("bevk read-back (D2H canvases)");
-    CU(cudaMemcpyAsync(out + (size_t)b0 * h.cbytes, dcanvas, h.cbytes * nb, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaMemcpyAsync(out + (size_t)b0 * h.obytes, dcanvas, h.obytes * nb, cudaMemcpyDeviceToHost, c->stream));
   }
   CU(cudaStreamSynchronize(c->stream));
   return BEVK_OK;
@@ -1873,6 +1953,7 @@ int bevk_bev_run_sharded(bevk_ctx* c, const void* d_frames, int64_t frame_stride
   NvtxRange nvtx_call("bevk_bev_run_sharded (render slabs, all-gather, compose)");
   RET(use(c));
   RET(bgr_only(flags, "bevk_bev_run_sharded"));
+  RET(bgr_canvas_only(flags, "bevk_bev_run_sharded"));
   if (!c->shard.configured) return fail(BEVK_ERR_ARG, "bevk_shard_configure not called");
   RET(check_stack(c, d_frames, frame_stride));
   bevk_ctx::Shard& s = c->shard;
@@ -1960,6 +2041,7 @@ int bevk_bev_run_scattered(bevk_ctx* c, const void* d_frames, int64_t frame_stri
   NvtxRange nvtx_call("bevk_bev_run_scattered (render with peer stores, barrier, compose own)");
   RET(use(c));
   RET(bgr_only(flags, "bevk_bev_run_scattered"));
+  RET(bgr_canvas_only(flags, "bevk_bev_run_scattered"));
   bevk_ctx::Shard& s = c->shard;
   if (!s.configured || s.policy != BEVK_SHARD_CAMERAS) return fail(BEVK_ERR_ARG, "bevk_shard_configure(CAMERAS) not called");
   RET(check_stack(c, d_frames, frame_stride));
@@ -2080,6 +2162,7 @@ int bevk_bev_run_jpeg(bevk_ctx* c, const uint8_t* const* jpegs, const uint64_t* 
   NvtxRange nvtx_call("bevk_bev_run_jpeg (JPEG streams -> host canvases)");
   RET(use(c));
   RET(bgr_only(flags, "bevk_bev_run_jpeg"));
+  RET(bgr_canvas_only(flags, "bevk_bev_run_jpeg"));
   RET(need_plan(c));
   if (!jpegs || !sizes || !out || batch < 1) return fail(BEVK_ERR_ARG, "bad argument");
   const size_t fpad = pad256((size_t)c->FW * c->FH * 3), cbytes = (size_t)c->BW * c->BH * 3;
@@ -2297,6 +2380,7 @@ int bevk_bev_run_to_jpeg(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_st
   NvtxRange nvtx_call("bevk_bev_run_to_jpeg (host frames -> host JPEG streams)");
   RET(use(c));
   RET(bgr_only(flags, "bevk_bev_run_to_jpeg"));
+  RET(bgr_canvas_only(flags, "bevk_bev_run_to_jpeg"));
   RET(to_jpeg_check(c, out, sizes));
   HostIngest h;
   RET(ingest_setup(c, srcs, src_stride, batch, car, flags, &h));
@@ -2314,6 +2398,7 @@ int bevk_bev_frames_to_jpeg(bevk_ctx* c, const void* const* frames, int batch, c
   NvtxRange nvtx_call("bevk_bev_frames_to_jpeg (device frames -> host JPEG streams)");
   RET(use(c));
   RET(bgr_only(flags, "bevk_bev_frames_to_jpeg"));
+  RET(bgr_canvas_only(flags, "bevk_bev_frames_to_jpeg"));
   RET(to_jpeg_check(c, out, sizes));
   if (!frames) return fail(BEVK_ERR_ARG, "null pointer");
   Frames src;

@@ -33,7 +33,7 @@
 
 #include <type_traits>
 
-#include "bevk_kernels.cuh"   // gray_world_gains, gain_entry
+#include "bevk_kernels.cuh"   // gain_table
 
 namespace bevk {
 namespace jpeg {
@@ -476,11 +476,7 @@ __global__ void __launch_bounds__(kBlockThreads) k_jpeg_blocks(EncArgs a) {
   const int i0 = (int)((long long)blockIdx.x * kBlockThreads / a.nblk);
   if constexpr (kGain) {
     const long long last = min((long long)blockIdx.x * kBlockThreads + kBlockThreads, a.nblk * a.n) - 1;
-    for (int i = i0; i <= (int)(last / a.nblk); ++i) {
-      double gain[3];
-      gray_world_gains(a.csum + 3ll * i, a.npix, gain);
-      for (int j = threadIdx.x; j < 768; j += blockDim.x) sgain[(i - i0) * 768 + j] = gain_entry(gain[j >> 8], j & 255);
-    }
+    for (int i = i0; i <= (int)(last / a.nblk); ++i) gain_table(a.csum + 3ll * i, a.npix, sgain + (i - i0) * 768);
   }
   __syncthreads();
   if (b >= a.nblk * a.n) return;

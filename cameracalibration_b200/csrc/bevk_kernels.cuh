@@ -364,17 +364,20 @@ __host__ __device__ __forceinline__ uint8_t gain_entry(double gain, int v) {
   const int r = cv_round(dmul((double)v, gain));   // non-finite -> INT_MIN -> saturates to 0, as on x86
   return (uint8_t)(r < 0 ? 0 : (r > 255 ? 255 : r));
 }
+// The 3 x 256 table of one canvas (channel sums csum[0..2]) into tab[c * 256 + v], filled by the threads of a CTA.  The
+// caller synchronises before reading it.
+__device__ __forceinline__ void gain_table(const unsigned long long* csum, double npix, uint8_t* tab) {
+  double gain[3];
+  gray_world_gains(csum, npix, gain);
+  for (int i = threadIdx.x; i < 768; i += blockDim.x) tab[i] = gain_entry(gain[i >> 8], i & 255);
+}
 
 __global__ void __launch_bounds__(256) k_gain(uint8_t* __restrict__ canvas, long long canvas_bytes, double npix,
                                               const unsigned long long* __restrict__ csum,
                                               const uint8_t* __restrict__ car) {
   __shared__ uint8_t tab[3][256];
   const int b = blockIdx.y;
-  {
-    double gain[3];
-    gray_world_gains(csum + b * 3, npix, gain);
-    for (int i = threadIdx.x; i < 768; i += blockDim.x) tab[i >> 8][i & 255] = gain_entry(gain[i >> 8], i & 255);
-  }
+  gain_table(csum + b * 3, npix, &tab[0][0]);
   __syncthreads();
   uint8_t* cv = canvas + (size_t)b * canvas_bytes;
   // 12-byte (4-pixel) steps keep the channel phase fixed per byte lane
@@ -757,6 +760,151 @@ __global__ void __launch_bounds__(256, 8) k_vsum_yuv(Frames frames, int w, int h
     unsigned long long t = 0;
     for (int k = 0; k < 8; ++k) t += part[k];
     atomicAdd(vsum + fi, t);
+  }
+}
+
+// ---------------------------------------------------------------------------------
+// YUV 4:2:0 canvases (BEVK_FLAG_OUT_NV12 / _I420).  Canvas b is the dense uint8[BH*3/2][BW] buffer (BW, BH even) at
+// out + b * BW*BH*3/2: the Y plane, then NV12: BH/2 rows of interleaved U,V; I420: the U plane, then the V plane, each
+// BW/2 x BH/2 and packed.  Its bytes are cv2.cvtColor(bgr, COLOR_BGR2YUV_I420) of the BGR canvas (NV12: the same planes
+// interleaved), converted by a streaming pass over the rendered BGR canvases.
+// ---------------------------------------------------------------------------------
+// cv2.cvtColor(COLOR_BGR2YUV_I420) of one pixel, OpenCV 4.x's fixed-point form (20 fraction bits).  Over all 2^24 BGR
+// triples Y lies in [16, 235] and U, V in [16, 240], so nothing saturates.  cv2 takes a 2 x 2 block's U and V from its
+// top-left pixel alone.  One definition for the kernel and the CPU tests.
+__host__ __device__ __forceinline__ void bgr_yuv(int b, int g, int r, int& Y, int& U, int& V) {
+  const int hy = (16 << 20) + (1 << 19), hc = (128 << 20) + (1 << 19);
+  Y = (269484 * r + 528482 * g + 102760 * b + hy) >> 20;
+  U = (-155188 * r - 305135 * g + 460324 * b + hc) >> 20;
+  V = (460324 * r - 385875 * g - 74448 * b + hc) >> 20;
+}
+
+struct CanvasYuvArgs {
+  const uint8_t* canvas;                 // BGR canvases, canvas b at canvas + b * BW*BH*3 (library scratch, 4-byte aligned)
+  uint8_t* out;                          // 4:2:0 canvases, canvas b at out + b * BW*BH*3/2 (the caller's: any alignment)
+  int BW, BH;
+  const unsigned long long* csum;        // GAIN: channel sums of the raw canvases, [batch][3]
+  const uint8_t* car;                    // GAIN: null, or the car overlay uint8[BH][BW][3] (any alignment)
+  double npix;                           // GAIN: BW * BH
+};
+
+// May the work items use 32-bit loads and stores?  The BGR rows of a 4-pixel group are then 3 aligned words (BW % 4 == 0
+// and the scratch base aligned), and so are its Y words, its NV12 chroma word and its two I420 chroma halves, when the
+// caller's out (and car) are 4-byte aligned.  BW % 4 == 2 (an odd chroma row width) takes the byte path.
+__host__ __device__ __forceinline__ bool canvas_yuv_words(const CanvasYuvArgs& a) {
+  return (a.BW & 3) == 0 && ((reinterpret_cast<uintptr_t>(a.out) | reinterpret_cast<uintptr_t>(a.car)) & 3) == 0;
+}
+
+__host__ __device__ __forceinline__ unsigned ld_u32(const uint8_t* p) {
+#ifdef __CUDA_ARCH__
+  return __ldg(reinterpret_cast<const unsigned*>(p));
+#else
+  return *reinterpret_cast<const unsigned*>(p);
+#endif
+}
+
+// One work item of k_canvas_yuv: pixels [4g, 4g + 4) (2 at the end of a BW % 4 == 2 row) of canvas rows 2cy and 2cy + 1
+// of canvas b.  Writes their Y bytes, and U and V of the even row's even pixels.  GAIN: the canvas is raw and each
+// byte first goes through tab (gain_table: color_balance), then the car is added with saturation, as k_gain does.
+template <int FMT, bool GAIN>
+__host__ __device__ __forceinline__ void canvas_yuv_item(const CanvasYuvArgs& a, int b, const uint8_t* tab, int cy, int g,
+                                                         bool words) {
+  const int BW = a.BW, x0 = 4 * g, n = min(4, BW - x0);
+  const long long plane = (long long)BW * a.BH, row3 = 3ll * BW;
+  const long long src_off = (long long)(2 * cy) * row3 + 3 * x0;
+  const uint8_t* src = a.canvas + b * 3 * plane + src_off;
+  const uint8_t* car = GAIN && a.car ? a.car + src_off : nullptr;
+  int c[2][12];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    if (words) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const unsigned w = ld_u32(src + r * row3 + 4 * k);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) c[r][4 * k + j] = (w >> (8 * j)) & 255;
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < 12; ++k) c[r][k] = k < 3 * n ? ld_u8(src + r * row3 + k) : 0;
+    }
+    if (GAIN) {
+#pragma unroll
+      for (int k = 0; k < 12; ++k) c[r][k] = tab[(k % 3) * 256 + c[r][k]];
+      if (car) {
+        if (words) {
+#pragma unroll
+          for (int k = 0; k < 3; ++k) {
+            const unsigned w = ld_u32(car + r * row3 + 4 * k);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) c[r][4 * k + j] = min(255, c[r][4 * k + j] + (int)((w >> (8 * j)) & 255));
+          }
+        } else {
+#pragma unroll
+          for (int k = 0; k < 12; ++k)
+            if (k < 3 * n) c[r][k] = min(255, c[r][k] + ld_u8(car + r * row3 + k));
+        }
+      }
+    }
+  }
+  int Y[2][4], U[2], V[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r)
+#pragma unroll
+    for (int p = 0; p < 4; ++p) {
+      int u, v;
+      bgr_yuv(c[r][3 * p], c[r][3 * p + 1], c[r][3 * p + 2], Y[r][p], u, v);
+      if (r == 0 && !(p & 1)) { U[p >> 1] = u; V[p >> 1] = v; }   // the top-left pixel of each 2 x 2 block
+    }
+  uint8_t* o = a.out + b * (3 * plane / 2);
+  uint8_t* y0 = o + (long long)(2 * cy) * BW + x0;
+  uint8_t* u0;
+  uint8_t* v0;
+  if (FMT == YUV_NV12) {
+    u0 = o + plane + (long long)cy * BW + x0;
+    v0 = u0 + 1;
+  } else {
+    u0 = o + plane + (long long)cy * (BW / 2) + (x0 >> 1);
+    v0 = u0 + plane / 4;
+  }
+  if (words) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r)
+      *reinterpret_cast<unsigned*>(y0 + r * BW) =
+          (unsigned)Y[r][0] | ((unsigned)Y[r][1] << 8) | ((unsigned)Y[r][2] << 16) | ((unsigned)Y[r][3] << 24);
+    if (FMT == YUV_NV12) {
+      *reinterpret_cast<unsigned*>(u0) = (unsigned)U[0] | ((unsigned)V[0] << 8) | ((unsigned)U[1] << 16) | ((unsigned)V[1] << 24);
+    } else {
+      *reinterpret_cast<unsigned short*>(u0) = (unsigned short)(U[0] | (U[1] << 8));
+      *reinterpret_cast<unsigned short*>(v0) = (unsigned short)(V[0] | (V[1] << 8));
+    }
+  } else {
+#pragma unroll
+    for (int p = 0; p < 4; ++p)
+      if (p < n) { y0[p] = (uint8_t)Y[0][p]; y0[BW + p] = (uint8_t)Y[1][p]; }
+#pragma unroll
+    for (int k = 0; k < 2; ++k)
+      if (2 * k < n) { u0[yuv_chroma_step<FMT>() * k] = (uint8_t)U[k]; v0[yuv_chroma_step<FMT>() * k] = (uint8_t)V[k]; }
+  }
+}
+
+// The conversion pass: grid = (blocks, batch); the items (4-pixel groups of row pairs) of canvas blockIdx.y, row pair
+// major, are strided over its blocks, so that a warp reads 32 consecutive groups of two rows and writes 32 consecutive Y
+// words per row.  GAIN: the canvases are raw BALANCE renders (run_device's kFlagRawBalance) and each CTA builds the
+// canvas's gain table in shared memory, so k_gain does not run and the balanced BGR canvas is never written.
+template <int FMT, bool GAIN>
+__global__ void __launch_bounds__(256) k_canvas_yuv(CanvasYuvArgs a) {
+  __shared__ uint8_t tab[GAIN ? 768 : 1];
+  const int b = blockIdx.y;
+  if (GAIN) {
+    gain_table(a.csum + 3 * b, a.npix, tab);
+    __syncthreads();
+  }
+  const int ng = (a.BW + 3) >> 2, items = ng * (a.BH >> 1);   // at most 16384 x 32768: fits an int
+  const bool words = canvas_yuv_words(a);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < items; i += gridDim.x * blockDim.x) {
+    const int cy = i / ng;
+    canvas_yuv_item<FMT, GAIN>(a, b, tab, cy, i - cy * ng, words);
   }
 }
 

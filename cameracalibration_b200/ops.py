@@ -456,27 +456,46 @@ class BevEngine:
         return {"tiles": a.value, "items": b.value, "lut_bytes": c.value}
 
     def run(self, frame_sets, car: np.ndarray | None = None, balance: bool = False, out: np.ndarray | None = None,
-            pixel_format: str = "bgr"):
+            pixel_format: str = "bgr", out_format: str = "bgr"):
         """frame_sets: list (batch) of lists (n_cam) of uint8[FH][FW][3] arrays.  Returns
         uint8[batch][BH][BW][3].
 
         pixel_format "nv12" / "i420": every frame is a YUV 4:2:0 buffer uint8[FH*3//2][FW] in cv2's layout (rows may be
         padded); the canvases are those of cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / _I420) followed by the BGR call.
-        The conversion runs on the GPU, and only the bytes the render samples (1.5 per pixel) cross PCIe."""
+        The conversion runs on the GPU, and only the bytes the render samples (1.5 per pixel) cross PCIe.
+
+        out_format "nv12" / "i420": the canvases are returned as YUV 4:2:0, uint8[batch][BH*3//2][BW], each
+        cv2.cvtColor(bgr_canvas, COLOR_BGR2YUV_I420) (NV12: its U and V planes interleaved); the conversion runs on the
+        GPU, so 1.5 bytes per canvas pixel come back instead of 3."""
         if not self.finalized:
             self.finalize()
         fmt = self._pixel_format(pixel_format)
+        ofmt = self._out_format(out_format)
         keep, ptrs, stride, batch = self._host_frames(frame_sets, "run()", fmt)
+        shape = self._canvas_shape(batch, ofmt)
         if out is None:   # a fresh array per call, as the reference returns -- page-locked and recycled (PinnedPool)
             if getattr(self, "_pool", None) is None:
                 self._pool = L.PinnedPool()
-            out = self._pool.get((batch, self.BH, self.BW, 3))
+            out = self._pool.get(shape)
         else:
-            out = _out((batch, self.BH, self.BW, 3), out)
+            out = _out(shape, out)
         car, carp = self._host_car(car)
-        L.check(self.ctx.lib.bevk_bev_run(self.ctx.h, ptrs, stride, batch, carp, (L.FLAG_BALANCE if balance else 0) | fmt,
-                                          L.vptr(out)))
+        L.check(self.ctx.lib.bevk_bev_run(self.ctx.h, ptrs, stride, batch, carp,
+                                          (L.FLAG_BALANCE if balance else 0) | fmt | ofmt, L.vptr(out)))
         return out
+
+    def _out_format(self, out_format: str) -> int:
+        """Flag bits of an out_format argument ("bgr", "nv12", "i420"); YUV 4:2:0 canvases need an even canvas size."""
+        ofmt = L.OUT_FORMATS.get(str(out_format).lower())
+        if ofmt is None:
+            raise L.BevkError(f"out_format must be one of {sorted(L.OUT_FORMATS)}, got {out_format!r}")
+        if ofmt and (self.BW % 2 or self.BH % 2):
+            raise L.BevkError(f"{out_format} canvases need an even canvas size, this engine's is {self.BW} x {self.BH}")
+        return ofmt
+
+    def _canvas_shape(self, batch: int, ofmt: int):
+        """Shape of `batch` canvases in the format of out-format flag bits ofmt."""
+        return (batch, self.BH * 3 // 2, self.BW) if ofmt else (batch, self.BH, self.BW, 3)
 
     def _pixel_format(self, pixel_format: str) -> int:
         """Flag bits of a pixel_format argument ("bgr", "nv12", "i420"); YUV 4:2:0 needs an even frame size."""
@@ -589,14 +608,13 @@ class BevEngine:
         L.check(self.ctx.lib.bevk_bev_run_jpeg(self.ctx.h, ptrs, sizes, batch, carp, L.FLAG_BALANCE if balance else 0, L.vptr(out)))
         return out
 
-    def host_copy_bytes(self, balance: bool = False, pixel_format: str = "bgr"):
+    def host_copy_bytes(self, balance: bool = False, pixel_format: str = "bgr", out_format: str = "bgr"):
         """(host->device, device->host) bytes per frame-set that run() moves over PCIe (pageable frames)."""
         if not self.finalized:
             self.finalize()
-        fmt = self._pixel_format(pixel_format)
+        flags = (L.FLAG_BALANCE if balance else 0) | self._pixel_format(pixel_format) | self._out_format(out_format)
         a, b = C.c_int64(), C.c_int64()
-        L.check(self.ctx.lib.bevk_bev_host_copy_bytes(self.ctx.h, (L.FLAG_BALANCE if balance else 0) | fmt, C.byref(a),
-                                                      C.byref(b)))
+        L.check(self.ctx.lib.bevk_bev_host_copy_bytes(self.ctx.h, flags, C.byref(a), C.byref(b)))
         return a.value, b.value
 
     def last_h2d_bytes(self) -> int:
@@ -618,23 +636,26 @@ class BevEngine:
         return g
 
     # device-resident entry points (raw device pointers, e.g. torch tensors' data_ptr())
-    def run_device(self, d_srcs_ptr: int, batch: int, d_out_ptr: int, d_car_ptr: int = 0, balance: bool = False):
+    def run_device(self, d_srcs_ptr: int, batch: int, d_out_ptr: int, d_car_ptr: int = 0, balance: bool = False,
+                   out_format: str = "bgr"):
+        """out_format "nv12" / "i420": d_out_ptr receives uint8[batch][BH*3//2][BW] YUV 4:2:0 canvases (see run())."""
         if not self.finalized:
             self.finalize()
+        flags = (L.FLAG_BALANCE if balance else 0) | self._out_format(out_format)
         L.check(self.ctx.lib.bevk_bev_run_device(self.ctx.h, C.c_void_p(d_srcs_ptr), batch, C.c_void_p(d_car_ptr or None),
-                                                 L.FLAG_BALANCE if balance else 0, C.c_void_p(d_out_ptr)))
+                                                 flags, C.c_void_p(d_out_ptr)))
 
     def run_stack(self, d_frames_ptr: int, frame_stride: int, batch: int, d_out_ptr: int, d_car_ptr: int = 0, balance: bool = False,
-                  pixel_format: str = "bgr"):
+                  pixel_format: str = "bgr", out_format: str = "bgr"):
         """Frame stack on the device (frame i at d_frames_ptr + i * frame_stride, i = set * n_cam + camera): the
         TMA-staged kernel when base and stride are 16-byte aligned.  Only enqueues on the ctx stream.  pixel_format
-        "nv12" / "i420": dense uint8[FH*3//2][FW] YUV 4:2:0 frames at any base and stride."""
+        "nv12" / "i420": dense uint8[FH*3//2][FW] YUV 4:2:0 frames at any base and stride.  out_format "nv12" / "i420":
+        d_out_ptr receives uint8[batch][BH*3//2][BW] YUV 4:2:0 canvases (see run())."""
         if not self.finalized:
             self.finalize()
-        fmt = self._pixel_format(pixel_format)
+        flags = (L.FLAG_BALANCE if balance else 0) | self._pixel_format(pixel_format) | self._out_format(out_format)
         L.check(self.ctx.lib.bevk_bev_run_stack(self.ctx.h, C.c_void_p(d_frames_ptr), int(frame_stride), batch,
-                                                C.c_void_p(d_car_ptr or None), (L.FLAG_BALANCE if balance else 0) | fmt,
-                                                C.c_void_p(d_out_ptr)))
+                                                C.c_void_p(d_car_ptr or None), flags, C.c_void_p(d_out_ptr)))
 
     def run_stack_cams(self, d_frames_ptr: int, frame_stride: int, batch: int, cam_lo: int, cam_hi: int, d_out_ptr: int):
         if not self.finalized:
@@ -652,7 +673,7 @@ class BevEngine:
         return dict(zip(("items", "shapes", "box_bytes", "tma_entries", "gather_entries"), (x.value for x in v)))
 
     def run_cuda(self, frames, car=None, balance: bool = False, out=None, stream: int | None = None,
-                 pixel_format: str = "bgr"):
+                 pixel_format: str = "bgr", out_format: str = "bgr"):
         """Frames that already live on the GPU (decoder output, torch / CuPy arrays): no PCIe in the call.
 
         frames: one uint8 CUDA array [batch][n_cam][FH][FW][3], or a list (batch) of lists (n_cam) of uint8
@@ -665,29 +686,38 @@ class BevEngine:
 
         pixel_format "nv12" / "i420": frames is one C-contiguous uint8 CUDA array [batch][n_cam][FH*3//2][FW] of YUV
         4:2:0 frames in cv2's layout (e.g. NVDEC NV12 surfaces); the result is that of cv2.cvtColor to BGR followed by
-        the BGR call, with the conversion done on the GPU."""
+        the BGR call, with the conversion done on the GPU.
+
+        out_format "nv12" / "i420": ``out`` is uint8[batch][BH*3//2][BW], YUV 4:2:0 canvases as run() describes them
+        (e.g. for a hardware video encoder's NV12 input)."""
         if not self.finalized:
             self.finalize()
         fmt = self._pixel_format(pixel_format)
+        ofmt = self._out_format(out_format)
         if fmt:
-            return self._run_cuda_yuv(frames, car, balance, out, stream, fmt, pixel_format)
+            return self._run_cuda_yuv(frames, car, balance, out, stream, fmt, pixel_format, ofmt)
         ptrs = self._cuda_frames(frames)
         batch = len(ptrs) // self.n_cam
-        if out is None:
-            import torch
-            out = torch.empty((batch, self.BH, self.BW, 3), dtype=torch.uint8, device=torch.device("cuda", self.ctx.device))
-        d_out = _cuda_ptr(out, (batch, self.BH, self.BW, 3))[0]
+        out, d_out = self._cuda_out(out, batch, ofmt)
         d_car = _cuda_ptr(car, (self.BH, self.BW, 3))[0] if car is not None else None
         if stream is None:
             from .sharding import _torch_current_stream
             stream = _torch_current_stream(self.ctx.device)
         table = (C.c_void_p * len(ptrs))(*ptrs)
         with self.ctx.on_stream(stream):
-            L.check(self.ctx.lib.bevk_bev_run_frames(self.ctx.h, table, batch, C.c_void_p(d_car), L.FLAG_BALANCE if balance else 0,
-                                                     C.c_void_p(d_out)))
+            L.check(self.ctx.lib.bevk_bev_run_frames(self.ctx.h, table, batch, C.c_void_p(d_car),
+                                                     (L.FLAG_BALANCE if balance else 0) | ofmt, C.c_void_p(d_out)))
         return out
 
-    def _run_cuda_yuv(self, frames, car, balance, out, stream, fmt, name):
+    def _cuda_out(self, out, batch, ofmt):
+        """(out, its device pointer) for `batch` canvases in the format of ofmt: a new torch tensor when out is None."""
+        shape = self._canvas_shape(batch, ofmt)
+        if out is None:
+            import torch
+            out = torch.empty(shape, dtype=torch.uint8, device=torch.device("cuda", self.ctx.device))
+        return out, _cuda_ptr(out, shape)[0]
+
+    def _run_cuda_yuv(self, frames, car, balance, out, stream, fmt, name, ofmt=0):
         """run_cuda() on a YUV 4:2:0 frame stack: bevk_bev_run_stack with a YUV flag."""
         if not hasattr(frames, "__cuda_array_interface__"):
             raise L.BevkError(f"{name} frames must be one uint8 CUDA array [batch][{self.n_cam}][{self.FH * 3 // 2}][{self.FW}]")
@@ -696,17 +726,14 @@ class BevEngine:
         if len(shape) != 4 or tuple(shape[1:]) != want or shape[0] < 1:
             raise L.BevkError(f"{name} frames must be uint8[batch][{self.n_cam}][{self.FH * 3 // 2}][{self.FW}], got {tuple(shape)}")
         batch = shape[0]
-        if out is None:
-            import torch
-            out = torch.empty((batch, self.BH, self.BW, 3), dtype=torch.uint8, device=torch.device("cuda", self.ctx.device))
-        d_out = _cuda_ptr(out, (batch, self.BH, self.BW, 3))[0]
+        out, d_out = self._cuda_out(out, batch, ofmt)
         d_car = _cuda_ptr(car, (self.BH, self.BW, 3))[0] if car is not None else None
         if stream is None:
             from .sharding import _torch_current_stream
             stream = _torch_current_stream(self.ctx.device)
         with self.ctx.on_stream(stream):
             L.check(self.ctx.lib.bevk_bev_run_stack(self.ctx.h, C.c_void_p(base), self.FW * self.FH * 3 // 2, batch,
-                                                    C.c_void_p(d_car), (L.FLAG_BALANCE if balance else 0) | fmt,
+                                                    C.c_void_p(d_car), (L.FLAG_BALANCE if balance else 0) | fmt | ofmt,
                                                     C.c_void_p(d_out)))
         return out
 

@@ -45,8 +45,15 @@ enum { BEVK_MODEL_FISHEYE = 0, BEVK_MODEL_PINHOLE = 1 };
  * the Y plane, then NV12: interleaved U,V rows; I420: the U plane, then the V plane, each frame_w/2 x frame_h/2 and
  * packed (two chroma rows per buffer row).  The result is byte for byte cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 /
  * COLOR_YUV2BGR_I420) followed by the BGR call.  Accepted by bevk_bev_run, bevk_bev_run_stack and
+ * bevk_bev_host_copy_bytes; every other entry point with flags refuses them with BEVK_ERR_UNSUPPORTED.
+ * BEVK_FLAG_OUT_NV12 / BEVK_FLAG_OUT_I420 (exclusive: both is BEVK_ERR_ARG; they combine with BALANCE, the car and the
+ * input flags) say the canvases are written as YUV 4:2:0: canvas b is the dense uint8[bev_h*3/2][bev_w] at
+ * out + b * bev_w*bev_h*3/2 (bev_w, bev_h even, else BEVK_ERR_UNSUPPORTED, as cv2 refuses odd sizes), whose bytes are
+ * cv2.cvtColor(bgr, COLOR_BGR2YUV_I420) of the BGR canvas `bgr` the same call writes without the flag (OUT_NV12: the
+ * same Y plane, then the U and V planes interleaved).  The conversion runs on the device, so only 1.5 bytes per canvas
+ * pixel leave it.  Accepted by bevk_bev_run, bevk_bev_run_device, bevk_bev_run_frames, bevk_bev_run_stack and
  * bevk_bev_host_copy_bytes; every other entry point with flags refuses them with BEVK_ERR_UNSUPPORTED. */
-enum { BEVK_FLAG_BALANCE = 1, BEVK_FLAG_NV12 = 2, BEVK_FLAG_I420 = 4 };
+enum { BEVK_FLAG_BALANCE = 1, BEVK_FLAG_NV12 = 2, BEVK_FLAG_I420 = 4, BEVK_FLAG_OUT_NV12 = 8, BEVK_FLAG_OUT_I420 = 16 };
 #define BEVK_MAX_CAMERAS 8
 
 int bevk_version(void);
@@ -148,7 +155,8 @@ int bevk_bev_finalize(bevk_ctx *ctx);
  * srcs: batch*n_cam host pointers (frame-set major: set0 cam0..camN-1, set1 ...),
  *       each uint8[frame_h][frame_w][3] with row stride src_stride bytes.
  * car : NULL or uint8[bev_h][bev_w][3] (dense), added after colour balance.
- * out : batch canvases uint8[bev_h][bev_w][3], dense, canvas b at out + b*bev_h*bev_w*3.
+ * out : batch canvases uint8[bev_h][bev_w][3], dense, canvas b at out + b*bev_h*bev_w*3; with BEVK_FLAG_OUT_NV12 /
+ *       _I420 uint8[bev_h*3/2][bev_w] at out + b*bev_w*bev_h*3/2, converted on the device, so only those bytes come back.
  * With BEVK_FLAG_NV12 / _I420 each frame is uint8[frame_h*3/2][frame_w] whose rows (Y and chroma alike) are
  * src_stride bytes apart.  Page-locked frames (frame_w and src_stride multiples of 16, no BALANCE) are read by the SMs
  * in the 16-byte windows around the sampled Y spans and the matching chroma bytes; pageable ones go up as the band
@@ -176,7 +184,9 @@ int bevk_bev_run_frames(bevk_ctx *ctx, const void *const *frames, int batch, con
  * With BEVK_FLAG_NV12 / _I420 frame i is the dense uint8[frame_h*3/2][frame_w] YUV frame at d_frames + i * frame_stride
  * (any base and any stride >= frame_w * frame_h * 3/2); its sampled spans are converted on the device into a 16-byte
  * friendly BGR copy stack, so the TMA-staged kernel renders them whenever a TMA plan exists.  Still only enqueues, so
- * it can be captured into a graph (after one eager call of the same shape).                                        */
+ * it can be captured into a graph (after one eager call of the same shape).  The same holds with BEVK_FLAG_OUT_NV12 /
+ * _I420 (here and in bevk_bev_run_device / _frames): the BGR canvases are rendered into library scratch and converted
+ * from there into d_out (any alignment).                                                                              */
 int bevk_bev_run_stack(bevk_ctx *ctx, const void *d_frames, int64_t frame_stride, int batch, const void *d_car, int flags,
                        void *d_out);
 /* Per-camera partial canvases for camera-sharded multi-GPU runs: rank r renders only
@@ -204,7 +214,8 @@ int bevk_bev_plan_info(bevk_ctx *ctx, int64_t *n_tiles, int64_t *n_items, int64_
 /* Bytes bevk_bev_run moves over PCIe per frame-set for the given flags: host->device (without
  * BALANCE only the rectangle of each frame its camera's LUT can sample is uploaded; with BALANCE
  * the whole frames, because the V means cover them) and device->host (the canvas).  With a YUV
- * flag: the Y rectangles and their chroma rows (1.5 bytes per pixel), or whole YUV frames. */
+ * flag: the Y rectangles and their chroma rows (1.5 bytes per pixel), or whole YUV frames.  With an
+ * output flag the canvas is bev_w*bev_h*3/2 bytes. */
 int bevk_bev_host_copy_bytes(bevk_ctx *ctx, int flags, int64_t *h2d_per_frame_set, int64_t *d2h_per_frame_set);
 /* Host->device bytes the last bevk_bev_run call actually moved (page-locked frames are ingested span
  * by span by the SMs, pageable ones by DMA rectangles, BALANCE uploads whole frames). */
