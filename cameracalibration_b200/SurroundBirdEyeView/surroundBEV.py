@@ -313,6 +313,13 @@ class BevGenerator:
         "nv12" / "i420": the result is uint8[n][BH*3//2][BW] YUV 4:2:0 canvases (see run_batch)."""
         return self.engine.run_cuda(frames, car, self.balance, out, stream, pixel_format=pixel_format, out_format=out_format)
 
+    def run_cuda_planes(self, y, c=None, v=None, pixel_format="nv12", car=None, out=None, stream=None, out_format="bgr"):
+        """run_cuda on YUV 4:2:0 frame-sets given plane by plane, as a video decoder leaves them on the GPU (pitched
+        rows, each plane at its own address): y uint8 CUDA array [n][4][FH][FW], c [n][4][FH/2][FW] interleaved U,V
+        ("nv12") or [n][4][FH/2][FW/2] U ("i420"), v the V plane ("i420"); or nested lists of per-frame plane tuples.
+        See BevEngine.run_cuda_planes."""
+        return self.engine.run_cuda_planes(y, c, v, pixel_format, car, self.balance, out, stream, out_format=out_format)
+
     def jpeg(self, front, back, left, right, car=None, quality=95):
         """cv2.imencode('.jpg', self(front, back, left, right, car), [IMWRITE_JPEG_QUALITY, quality]) -- the bytes
         main()'s cv2.imwrite('./surround.jpg', surround) writes (reference surroundBEV.py:340) -- encoded on the GPU:

@@ -57,6 +57,9 @@ SIGNATURES = {
     "bevk_bev_run_device": (C.c_int, [_p, _p, C.c_int, _p, C.c_int, _p]),
     "bevk_bev_run_frames": (C.c_int, [_p, _p, C.c_int, _p, C.c_int, _p]),
     "bevk_bev_run_stack": (C.c_int, [_p, _p, C.c_int64, C.c_int, _p, C.c_int, _p]),
+    "bevk_bev_run_yuv_planes": (C.c_int, [_p, _p, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int, _p, C.c_int,
+                                          _p]),
+    "bevk_bev_run_yuv_surfaces": (C.c_int, [_p, C.POINTER(_p), C.POINTER(C.c_int64), C.c_int, _p, C.c_int, _p]),
     "bevk_bev_run_device_cams": (C.c_int, [_p, _p, C.c_int, C.c_int, C.c_int, _p]),
     "bevk_bev_run_stack_cams": (C.c_int, [_p, _p, C.c_int64, C.c_int, C.c_int, C.c_int, _p]),
     "bevk_sat_sum_device": (C.c_int, [_p, C.POINTER(_p), C.c_int, C.c_uint64, _p, _p]),

@@ -177,6 +177,8 @@ struct bevk_ctx {
   DevBuf d_out_bgr, d_out_yuv;              // YUV output: BGR canvases of the device entry points, YUV canvases of bevk_bev_run
   DevBuf d_user_ptrs;                       // bevk_bev_run_frames: device copy of the caller's frame table
   std::vector<const void*> user_tab;        // ... and what it currently holds
+  DevBuf d_yuv_tab;                         // bevk_bev_run_yuv_surfaces: device copy of the plane table, plane-major
+  std::vector<const void*> yuv_tab;         // ... and what it currently holds
   // TMA-staged kernel (bevk_bev_tma.cuh): its plan, and the tensor maps of the frame stacks seen recently
   bool tma_planned = false;
   int tma_stage_bytes = 0;
@@ -1150,31 +1152,34 @@ static int balance_prepass(bevk_ctx* c, Frames src, int batch, int lo, int hi, c
 // the copy stack d_bal, laid out as balance_prepass leaves it; *bgr_src describes it.  With BALANCE the V sums come from
 // k_vsum_yuv over the whole converted frames first.  The caller checks batch * n_cam <= 65535.
 template <int FMT>
-static int yuv_prepass_fmt(bevk_ctx* c, Frames src, int batch, bool bal, Frames* bgr_src) {
+static int yuv_prepass_fmt(bevk_ctx* c, Frames src, const YuvPlanes* planes, int batch, bool bal, Frames* bgr_src) {
   const int nf = batch * c->n_cam;
   const CamRange cr{0, c->n_cam, c->n_cam};
+  const YuvPlanes in = planes ? *planes : yuv_dense_planes<FMT>(src.base, src.stride, c->FW, c->FH);
   if (bal) {
     const int blocks = std::max(1, std::min(c->FH / 2, c->n_sm * 4 / std::max(1, std::min(nf, 64)) + 1));
     RET(lum_deltas(c, batch, nullptr, 1, [&](unsigned long long* vsum) {
-      k_vsum_yuv<FMT><<<dim3(blocks, nf), 256, 0, c->stream>>>(src, c->FW, c->FH, vsum, cr);
+      k_vsum_yuv<FMT><<<dim3(blocks, nf), 256, 0, c->stream>>>(in, c->FW, c->FH, vsum, cr);
     }));
   }
   const size_t fpad = pad256((size_t)c->FW * 3 * c->FH);
   RET(c->d_bal.ensure(fpad * nf));
   const dim3 grid((c->FH + LUM_ROWS - 1) / LUM_ROWS, nf);
   if (bal)
-    k_yuv_spans<FMT, true><<<grid, 128, 0, c->stream>>>(src, c->d_bal.as<uint8_t>(), (long long)fpad, c->d_spans.as<int2>(), cr,
+    k_yuv_spans<FMT, true><<<grid, 128, 0, c->stream>>>(in, c->d_bal.as<uint8_t>(), (long long)fpad, c->d_spans.as<int2>(), cr,
                                                         c->FW, c->FH, c->d_delta.as<int>(), c->d_hsv.as<int>());
   else
-    k_yuv_spans<FMT, false><<<grid, 128, 0, c->stream>>>(src, c->d_bal.as<uint8_t>(), (long long)fpad, c->d_spans.as<int2>(), cr,
+    k_yuv_spans<FMT, false><<<grid, 128, 0, c->stream>>>(in, c->d_bal.as<uint8_t>(), (long long)fpad, c->d_spans.as<int2>(), cr,
                                                          c->FW, c->FH, nullptr, nullptr);
   LAUNCHED(c);
   *bgr_src = Frames(c->d_bal.p, (long long)fpad);
   return BEVK_OK;
 }
 
-static int yuv_prepass(bevk_ctx* c, int fmt, Frames src, int batch, bool bal, Frames* bgr_src) {
-  return fmt == YUV_NV12 ? yuv_prepass_fmt<YUV_NV12>(c, src, batch, bal, bgr_src) : yuv_prepass_fmt<YUV_I420>(c, src, batch, bal, bgr_src);
+// The frames are `planes` when given, else the dense stack src (cv2's single-buffer layout).
+static int yuv_prepass(bevk_ctx* c, int fmt, Frames src, const YuvPlanes* planes, int batch, bool bal, Frames* bgr_src) {
+  return fmt == YUV_NV12 ? yuv_prepass_fmt<YUV_NV12>(c, src, planes, batch, bal, bgr_src)
+                         : yuv_prepass_fmt<YUV_I420>(c, src, planes, batch, bal, bgr_src);
 }
 
 // colour balance of `batch` full canvases from their channel sums, then the car (null: none), in place
@@ -1190,8 +1195,9 @@ static int launch_gain(bevk_ctx* c, uint8_t* out, int batch, const unsigned long
 // encoder's GainSrc applies the gains and the car, so k_gain does not run.  (Without BALANCE the write-out adds the car.)
 constexpr int kFlagRawBalance = 1 << 30;
 
+// YUV frames (BEVK_FLAG_NV12 / _I420) are `planes` when given (src then only has to be non-null), else the dense stack src.
 static int run_device(bevk_ctx* c, Frames src, int batch, const void* d_car, int flags, void* d_out, int cam_lo, int cam_hi,
-                      const OutWin* win = nullptr) {
+                      const OutWin* win = nullptr, const YuvPlanes* planes = nullptr) {
   NvtxRange nvtx_render("bevk render (fused BEV kernels)");
   RET(need_plan(c));
   if ((!src.table && !src.base) || (!d_out && !(win && win->world))) return fail(BEVK_ERR_ARG, "null device pointer");
@@ -1203,6 +1209,7 @@ static int run_device(bevk_ctx* c, Frames src, int batch, const void* d_car, int
   if ((bal || fmt) && nf > 65535)
     return fail(BEVK_ERR_ARG, "batch %d x %d cameras exceeds the 65535 frames of a BALANCE or YUV call", batch, c->n_cam);
   if (fmt && (win || cam_lo != 0 || cam_hi < c->n_cam)) return fail(BEVK_ERR_UNSUPPORTED, "YUV frames render whole canvases only");
+  if (fmt && !planes && src.table) return fail(BEVK_ERR_UNSUPPORTED, "dense YUV frames come as a frame stack");
   RenderParams R{};
   R.n_cam = c->n_cam; R.FW = c->FW; R.FH = c->FH; R.pitch = (unsigned)c->FW * 3u;
   R.out = reinterpret_cast<uint8_t*>(d_out); R.BW = c->BW; R.BH = c->BH;
@@ -1226,7 +1233,7 @@ static int run_device(bevk_ctx* c, Frames src, int batch, const void* d_car, int
     if (!fmt) RET(balance_prepass(c, src, batch, 0, c->n_cam, nullptr, 1, &gsrc));
     R.csum = c->d_csum.as<unsigned long long>();
   }
-  if (fmt) RET(yuv_prepass(c, fmt, src, batch, bal, &gsrc));   // BGR copies of the sampled spans (balanced with BALANCE)
+  if (fmt) RET(yuv_prepass(c, fmt, src, planes, batch, bal, &gsrc));   // BGR copies of the sampled spans (balanced with BALANCE)
   // TMA-staged kernel for frame stacks (16-byte aligned base and stride); global-offset gather otherwise
   const bool use_tma = c->tma_planned && !gsrc.table && (reinterpret_cast<uintptr_t>(gsrc.base) & 15) == 0 && (gsrc.stride & 15) == 0 &&
                        gsrc.stride >= (long long)R.pitch * c->FH && (nbu == 1 || nbu == 4);
@@ -1284,9 +1291,10 @@ static int launch_canvas_yuv(bevk_ctx* c, int ofmt, const uint8_t* canvases, int
 // `scratch`, converted from there into d_out by k_canvas_yuv.  With BALANCE the render stops at the raw canvas and the
 // conversion applies colour balance and the car, so k_gain does not run.  The one conversion step of the host and the
 // device entry points.
-static int render_to(bevk_ctx* c, Frames src, int batch, const void* d_car, int flags, int ofmt, uint8_t* scratch, void* d_out) {
-  if (!ofmt) return run_device(c, src, batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
-  RET(run_device(c, src, batch, d_car, (flags & ~kOutFlags) | kFlagRawBalance, scratch, 0, BEVK_MAX_CAMERAS));
+static int render_to(bevk_ctx* c, Frames src, int batch, const void* d_car, int flags, int ofmt, uint8_t* scratch, void* d_out,
+                     const YuvPlanes* planes = nullptr) {
+  if (!ofmt) return run_device(c, src, batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS, nullptr, planes);
+  RET(run_device(c, src, batch, d_car, (flags & ~kOutFlags) | kFlagRawBalance, scratch, 0, BEVK_MAX_CAMERAS, nullptr, planes));
   return launch_canvas_yuv(c, ofmt, scratch, batch, (flags & BEVK_FLAG_BALANCE) ? c->d_csum.as<unsigned long long>() : nullptr,
                            d_car, d_out);
 }
@@ -1295,18 +1303,19 @@ static int render_to(bevk_ctx* c, Frames src, int batch, const void* d_car, int 
 // d_out_bgr.  Rendering in chunks of 8 frame-sets, so that the conversion reads canvases still in L2, was slower: the
 // fused kernels lose more on the smaller batches than the conversion gains (DESIGN.md section 4).  Only enqueues;
 // bevk_last_kernel_ms covers the render and the conversion.
-static int run_canvases(bevk_ctx* c, Frames src, int batch, const void* d_car, int flags, void* d_out) {
+static int run_canvases(bevk_ctx* c, Frames src, int batch, const void* d_car, int flags, void* d_out,
+                        const YuvPlanes* planes = nullptr) {
   int ofmt = 0;
   RET(need_plan(c));
   RET(out_format(c, flags, &ofmt));
-  if (!ofmt) return run_device(c, src, batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
+  if (!ofmt) return run_device(c, src, batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS, nullptr, planes);
   if (!d_out) return fail(BEVK_ERR_ARG, "null device pointer");
   if (batch < 1 || batch > 65535) return fail(BEVK_ERR_ARG, "batch %d out of range [1,65535]", batch);
   RET(c->d_out_bgr.ensure((size_t)c->BW * c->BH * 3 * batch));
   const bool timed = c->timed;
   if (timed && !c->capturing) CU(cudaEventRecord(c->ev0, c->stream));
   c->timed = false;   // the render records no events of its own
-  const int rc = render_to(c, src, batch, d_car, flags, ofmt, c->d_out_bgr.as<uint8_t>(), d_out);
+  const int rc = render_to(c, src, batch, d_car, flags, ofmt, c->d_out_bgr.as<uint8_t>(), d_out, planes);
   c->timed = timed;
   RET(rc);
   if (timed && !c->capturing) CU(cudaEventRecord(c->ev1, c->stream));
@@ -1389,6 +1398,72 @@ int bevk_bev_run_stack(bevk_ctx* c, const void* d_frames, int64_t frame_stride, 
   }
   c->timed = true;
   return run_canvases(c, Frames(d_frames, frame_stride), batch, d_car, flags, d_out);
+}
+
+// The checks the two plane entry points share, before anything is enqueued: a YUV flag, batch, and pitches that cover
+// their planes' rows (plane 2 only for I420).
+static int check_yuv_planes(bevk_ctx* c, const int64_t* pitch, int batch, int flags, int* fmt, int* n_planes) {
+  RET(need_plan(c));
+  RET(pixel_format(c, flags, fmt));
+  if (!*fmt) return fail(BEVK_ERR_ARG, "YUV planes need BEVK_FLAG_NV12 or BEVK_FLAG_I420");
+  if (!pitch) return fail(BEVK_ERR_ARG, "null pitch array");
+  if (batch < 1 || (long long)batch * c->n_cam > 65535)
+    return fail(BEVK_ERR_ARG, "batch %d x %d cameras out of range [1,65535] frames", batch, c->n_cam);
+  *n_planes = *fmt == YUV_NV12 ? 2 : 3;
+  const int row[3] = {c->FW, *fmt == YUV_NV12 ? c->FW : c->FW / 2, c->FW / 2};
+  for (int p = 0; p < *n_planes; ++p)
+    if (pitch[p] < row[p]) return fail(BEVK_ERR_ARG, "pitch[%d] %lld smaller than the plane's %d-byte rows", p, (long long)pitch[p], row[p]);
+  return BEVK_OK;
+}
+
+int bevk_bev_run_yuv_planes(bevk_ctx* c, const void* d_base, int64_t frame_stride, const int64_t offset[3], const int64_t pitch[3],
+                            int batch, const void* d_car, int flags, void* d_out) {
+  RET(use(c));
+  int fmt = 0, np = 0;
+  RET(check_yuv_planes(c, pitch, batch, flags, &fmt, &np));
+  if (!d_base || !offset) return fail(BEVK_ERR_ARG, "null surface pool or offset array");
+  YuvPlanes planes;
+  for (int p = 0; p < 3; ++p) {
+    const int q = p < np ? p : 1;   // NV12: plane 2 is never read
+    planes.f[p] = Frames(static_cast<const uint8_t*>(d_base) + offset[q], frame_stride);
+    planes.pitch[p] = pitch[q];
+  }
+  c->timed = true;
+  return run_canvases(c, planes.f[0], batch, d_car, flags, d_out, &planes);
+}
+
+int bevk_bev_run_yuv_surfaces(bevk_ctx* c, const void* const* surfaces, const int64_t pitch[3], int batch, const void* d_car,
+                              int flags, void* d_out) {
+  RET(use(c));
+  int fmt = 0, np = 0;
+  RET(check_yuv_planes(c, pitch, batch, flags, &fmt, &np));
+  if (!surfaces) return fail(BEVK_ERR_ARG, "null plane table");
+  const size_t n = (size_t)batch * c->n_cam;
+  std::vector<const void*> tab(3 * n, nullptr);   // plane-major: plane p of frame i at [p * n + i]
+  for (size_t i = 0; i < n; ++i)
+    for (int p = 0; p < np; ++p) {
+      if (!surfaces[3 * i + p]) return fail(BEVK_ERR_ARG, "plane %d of frame %zu is null", p, i);
+      tab[p * n + i] = surfaces[3 * i + p];
+    }
+  if (np == 2) std::copy(tab.begin() + n, tab.begin() + 2 * n, tab.begin() + 2 * n);   // NV12: plane 2 is never read
+  if (c->yuv_tab != tab) {
+    RET(c->d_yuv_tab.ensure(tab.size() * sizeof(void*)));
+    c->yuv_tab = tab;
+    // pageable source: the driver stages it before returning, and stream order protects launches still reading the old table
+    const cudaError_t e = cudaMemcpyAsync(c->d_yuv_tab.p, c->yuv_tab.data(), tab.size() * sizeof(void*), cudaMemcpyHostToDevice, c->stream);
+    if (e != cudaSuccess) {
+      c->yuv_tab.clear();   // nothing cached: the next call uploads again
+      return fail(BEVK_ERR_CUDA, "plane table upload: %s", cudaGetErrorString(e));
+    }
+  }
+  YuvPlanes planes;
+  const void* const* d_tab = c->d_yuv_tab.as<const void*>();
+  for (int p = 0; p < 3; ++p) {
+    planes.f[p] = Frames(d_tab + p * n);
+    planes.pitch[p] = pitch[p < np ? p : 1];
+  }
+  c->timed = true;
+  return run_canvases(c, planes.f[0], batch, d_car, flags, d_out, &planes);
 }
 
 int bevk_bev_run_stack_cams(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, int cam_lo, int cam_hi, void* d_out) {

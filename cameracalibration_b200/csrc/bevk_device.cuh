@@ -22,8 +22,9 @@ struct Frames {
   const uint8_t* base = nullptr;
   long long stride = 0;
   Frames() = default;
-  explicit Frames(const void* d_table) : table(static_cast<const uint8_t* const*>(d_table)) {}
-  Frames(const void* d_base, long long frame_stride) : base(static_cast<const uint8_t*>(d_base)), stride(frame_stride) {}
+  __host__ __device__ explicit Frames(const void* d_table) : table(static_cast<const uint8_t* const*>(d_table)) {}
+  __host__ __device__ Frames(const void* d_base, long long frame_stride)
+      : base(static_cast<const uint8_t*>(d_base)), stride(frame_stride) {}
   __host__ __device__ __forceinline__ const uint8_t* frame(long long i) const { return table ? table[i] : base + i * stride; }
 };
 

@@ -578,10 +578,12 @@ __global__ void __launch_bounds__(128) k_lum_spans(Frames in, uint8_t* __restric
 }
 
 // ---------------------------------------------------------------------------------
-// YUV 4:2:0 sources (NV12, I420).  A frame is cv2's single-buffer layout: a uint8[FH*3/2][FW] image (FW, FH even) whose
-// first FH rows are the Y plane.  NV12: then FH/2 rows of interleaved U,V.  I420: then the U plane and the V plane, each
-// FW/2 x FH/2 and packed, so two chroma rows share a buffer row: chroma row k (U rows 0..FH/2-1, then the V rows) starts
-// at buffer row FH + k/2, column (k & 1) * FW/2 -- which is also where cv2 looks for it in a buffer with padded rows.
+// YUV 4:2:0 sources (NV12, I420), FW and FH even.  The conversion reads a frame through its planes (YuvFrame: a Y plane,
+// then NV12: one plane of interleaved U,V; I420: a U and a V plane), each at its own address and row pitch, as decoder
+// surfaces come.  cv2's single-buffer layout is one instance: a uint8[FH*3/2][FW] image whose first FH rows are the Y
+// plane.  NV12: then FH/2 rows of interleaved U,V.  I420: then the U plane and the V plane, each FW/2 x FH/2 and packed,
+// so two chroma rows share a buffer row: chroma row k (U rows 0..FH/2-1, then the V rows) starts at buffer row FH + k/2,
+// column (k & 1) * FW/2 -- which is also where cv2 looks for it in a buffer with padded rows.
 // The colour conversion runs once per sampled source pixel into the same copy stack the BALANCE pre-pass fills; the
 // fused render then reads BGR from there as it always does.
 // ---------------------------------------------------------------------------------
@@ -612,6 +614,65 @@ __host__ __device__ __forceinline__ void yuv_chroma_rows(int FW, int FH, long lo
 template <int FMT>
 __host__ __device__ __forceinline__ constexpr int yuv_chroma_step() { return FMT == YUV_NV12 ? 2 : 1; }
 
+// The planes of one YUV frame as the conversion reads them: row r of plane p starts at plane[p] + r * pitch[p].  Plane 0
+// is Y (FW bytes a row), plane 1 interleaved U,V (NV12, FW bytes) or U (I420, FW/2), plane 2 V (I420, FW/2; unused for
+// NV12).  Rows may be padded to any pitch and the planes may lie anywhere, as a video decoder's surfaces do.
+struct YuvFrame {
+  const uint8_t* plane[3];
+  long long pitch[3];
+};
+
+// The planes of every frame of a call: plane p of frame i at f[p].frame(i) (a stack or a device table per plane), rows
+// pitch[p] bytes apart.  Kernels take it by value.
+struct YuvPlanes {
+  Frames f[3];
+  long long pitch[3];
+  __host__ __device__ __forceinline__ YuvFrame frame(long long i) const {
+    return YuvFrame{{f[0].frame(i), f[1].frame(i), f[2].frame(i)}, {pitch[0], pitch[1], pitch[2]}};
+  }
+};
+
+// cv2's single-buffer layout uint8[FH*3/2][FW] as planes: byte offsets and pitches of Y, UV / U and V in the buffer.
+// NV12: {0, FH*FW}, pitches {FW, FW}; I420: {0, FH*FW, FH*FW + FH*FW/4}, pitches {FW, FW/2, FW/2} (the packed U and V
+// planes, chroma row k of yuv_chroma_rows at FH*FW + k*FW/2).
+template <int FMT>
+__host__ __device__ __forceinline__ void yuv_dense_layout(int FW, int FH, long long (&off)[3], long long (&pitch)[3]) {
+  const long long y = (long long)FW * FH;
+  off[0] = 0; pitch[0] = FW;
+  if (FMT == YUV_NV12) {
+    off[1] = y; pitch[1] = FW;
+    off[2] = y; pitch[2] = FW;   // unused
+  } else {
+    off[1] = y; pitch[1] = FW / 2;
+    off[2] = y + y / 4; pitch[2] = FW / 2;
+  }
+}
+
+// The dense frames at base + i * stride (cv2's layout) as planes.
+template <int FMT>
+__host__ __device__ __forceinline__ YuvPlanes yuv_dense_planes(const uint8_t* base, long long stride, int FW, int FH) {
+  long long off[3], pitch[3];
+  yuv_dense_layout<FMT>(FW, FH, off, pitch);
+  YuvPlanes p;
+  for (int k = 0; k < 3; ++k) { p.f[k] = Frames(base + off[k], stride); p.pitch[k] = pitch[k]; }
+  return p;
+}
+
+// One dense frame at f (cv2's layout) as planes.
+template <int FMT>
+__host__ __device__ __forceinline__ YuvFrame yuv_dense_frame(const uint8_t* f, int FW, int FH) {
+  long long off[3], pitch[3];
+  yuv_dense_layout<FMT>(FW, FH, off, pitch);
+  return YuvFrame{{f + off[0], f + off[1], f + off[2]}, {pitch[0], pitch[1], pitch[2]}};
+}
+
+// Chroma row cy of a frame: the U and V samples of pixel x are at u + step * (x/2) and v + step * (x/2).
+template <int FMT>
+__host__ __device__ __forceinline__ void yuv_chroma_ptrs(const YuvFrame& fr, int cy, const uint8_t*& u, const uint8_t*& v) {
+  u = fr.plane[1] + (long long)cy * fr.pitch[1];
+  v = FMT == YUV_NV12 ? u + 1 : fr.plane[2] + (long long)cy * fr.pitch[2];
+}
+
 __host__ __device__ __forceinline__ int ld_u8(const uint8_t* p) {
 #ifdef __CUDA_ARCH__
   return __ldg(p);
@@ -627,17 +688,18 @@ __host__ __device__ __forceinline__ void span_groups(int2 sp, int& g0, int& g1) 
   g1 = sp.y > sp.x ? (sp.y + 3) >> 2 : g0;
 }
 
-// One work item of k_yuv_spans: group g of row y of frame f (rows FW bytes apart), converted to BGR in c[3 * px + {0,1,2}]
-// and, with BAL, luminance-balanced by delta d (tab: the HSV division tables).  Returns the number of pixels (4 or 2).
+// One work item of k_yuv_spans: group g of row y of frame fr, converted to BGR in c[3 * px + {0,1,2}] and, with BAL,
+// luminance-balanced by delta d (tab: the HSV division tables).  Returns the number of pixels (4 or 2).  The word loads
+// are chosen per pointer, so an odd base or pitch only costs byte loads.
 template <int FMT, bool BAL>
-__host__ __device__ __forceinline__ int yuv_group(const uint8_t* __restrict__ f, int FW, int FH, int y, int g, int d,
-                                                  const int* __restrict__ tab, int (&c)[12]) {
+__host__ __device__ __forceinline__ int yuv_group(const YuvFrame& fr, int FW, int y, int g, int d, const int* __restrict__ tab,
+                                                  int (&c)[12]) {
   const int x0 = 4 * g, n = min(4, FW - x0);
-  long long uo, vo;
-  yuv_chroma_rows<FMT>(FW, FH, FW, y >> 1, uo, vo);
-  const uint8_t* yr = f + (long long)y * FW + x0;
-  const uint8_t* ur = f + uo + yuv_chroma_step<FMT>() * (x0 >> 1);
-  const uint8_t* vr = f + vo + yuv_chroma_step<FMT>() * (x0 >> 1);
+  const uint8_t *ur, *vr;
+  yuv_chroma_ptrs<FMT>(fr, y >> 1, ur, vr);
+  ur += yuv_chroma_step<FMT>() * (x0 >> 1);
+  vr += yuv_chroma_step<FMT>() * (x0 >> 1);
+  const uint8_t* yr = fr.plane[0] + (long long)y * fr.pitch[0] + x0;
   int Y[4] = {0, 0, 0, 0}, U[2] = {128, 128}, V[2] = {128, 128};
 #ifdef __CUDA_ARCH__
   if (n == 4 && (reinterpret_cast<uintptr_t>(yr) & 3) == 0) {
@@ -667,17 +729,24 @@ __host__ __device__ __forceinline__ int yuv_group(const uint8_t* __restrict__ f,
   return n;
 }
 
+// The same on a dense frame f in cv2's layout (rows FW bytes apart).
+template <int FMT, bool BAL>
+__host__ __device__ __forceinline__ int yuv_group(const uint8_t* __restrict__ f, int FW, int FH, int y, int g, int d,
+                                                  const int* __restrict__ tab, int (&c)[12]) {
+  return yuv_group<FMT, BAL>(yuv_dense_frame<FMT>(f, FW, FH), FW, y, g, d, tab, c);
+}
+
 // The YUV source pre-pass of a fused render: k_lum_spans' work decomposition (one CTA per LUM_ROWS source rows of one
-// frame, the rows' span groups as one flat list), reading Y row y and chroma row y/2 of the frame and writing BGR into
-// the copy stack (frame f at out_base + f * out_stride, rows FW * 3 bytes); with BAL each pixel then takes
+// frame, the rows' span groups as one flat list), reading Y row y and chroma row y/2 of the frame's planes and writing BGR
+// into the copy stack (frame f at out_base + f * out_stride, rows FW * 3 bytes); with BAL each pixel then takes
 // luminance_balance's HSV round trip with the frame's delta, so a balanced YUV render has no extra pass over the frames.
 template <int FMT, bool BAL>
-__global__ void __launch_bounds__(128) k_yuv_spans(Frames in, uint8_t* __restrict__ out_base, long long out_stride,
+__global__ void __launch_bounds__(128) k_yuv_spans(YuvPlanes in, uint8_t* __restrict__ out_base, long long out_stride,
                                                    const int2* __restrict__ spans, CamRange cr, int w, int h,
                                                    const int* __restrict__ delta, const int* __restrict__ hsv_tab) {
   const int f = range_frame(cr, blockIdx.y), y0 = blockIdx.x * LUM_ROWS, y1 = min(h, y0 + LUM_ROWS), nrows = y1 - y0;
   const int2* sp_cam = spans + (size_t)(f % cr.n_cam) * h;
-  const uint8_t* const frame = in.frame(f);
+  const YuvFrame frame = in.frame(f);
   uint8_t* const out = out_base + f * out_stride;
   __shared__ int s_tab[BAL ? 512 : 1];
   __shared__ int s_pref[LUM_ROWS + 1], s_g0[LUM_ROWS];
@@ -705,7 +774,7 @@ __global__ void __launch_bounds__(128) k_yuv_spans(Frames in, uint8_t* __restric
     while (i >= s_pref[r + 1]) ++r;                       // the thread's items are visited in increasing order
     const int gidx = s_g0[r] + (i - s_pref[r]);
     int c[12];
-    const int n = yuv_group<FMT, BAL>(frame, w, h, y0 + r, gidx, d, s_tab, c);
+    const int n = yuv_group<FMT, BAL>(frame, w, y0 + r, gidx, d, s_tab, c);
     uint8_t* o = out + (size_t)(y0 + r) * row_bytes + 12 * (size_t)gidx;
     if (words) {
       unsigned* o4 = reinterpret_cast<unsigned*>(o);
@@ -720,14 +789,15 @@ __global__ void __launch_bounds__(128) k_yuv_spans(Frames in, uint8_t* __restric
   }
 }
 
-// V = max(B, G, R) summed over the four pixels that share chroma sample (cx, cy) (frame rows FW bytes apart).
+// V = max(B, G, R) summed over the four pixels that share chroma sample (cx, cy) of frame fr.
 template <int FMT>
-__host__ __device__ __forceinline__ unsigned yuv_vsum_2x2(const uint8_t* __restrict__ f, int FW, int FH, int cx, int cy) {
-  long long uo, vo;
-  yuv_chroma_rows<FMT>(FW, FH, FW, cy, uo, vo);
-  const int U = ld_u8(f + uo + yuv_chroma_step<FMT>() * cx), V = ld_u8(f + vo + yuv_chroma_step<FMT>() * cx);
-  const uint8_t* y = f + (long long)(2 * cy) * FW + 2 * cx;
-  const int Yv[4] = {ld_u8(y), ld_u8(y + 1), ld_u8(y + FW), ld_u8(y + FW + 1)};
+__host__ __device__ __forceinline__ unsigned yuv_vsum_2x2(const YuvFrame& fr, int cx, int cy) {
+  const uint8_t *ur, *vr;
+  yuv_chroma_ptrs<FMT>(fr, cy, ur, vr);
+  const int U = ld_u8(ur + yuv_chroma_step<FMT>() * cx), V = ld_u8(vr + yuv_chroma_step<FMT>() * cx);
+  const long long yp = fr.pitch[0];
+  const uint8_t* y = fr.plane[0] + (long long)(2 * cy) * yp + 2 * cx;
+  const int Yv[4] = {ld_u8(y), ld_u8(y + 1), ld_u8(y + yp), ld_u8(y + yp + 1)};
   unsigned s = 0;
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
@@ -738,17 +808,23 @@ __host__ __device__ __forceinline__ unsigned yuv_vsum_2x2(const uint8_t* __restr
   return s;
 }
 
+// The same on a dense frame f in cv2's layout (rows FW bytes apart).
+template <int FMT>
+__host__ __device__ __forceinline__ unsigned yuv_vsum_2x2(const uint8_t* __restrict__ f, int FW, int FH, int cx, int cy) {
+  return yuv_vsum_2x2<FMT>(yuv_dense_frame<FMT>(f, FW, FH), cx, cy);
+}
+
 // k_vsum for YUV frames: vsum[frame] += the exact sum of V over the whole converted frame (what luminance_balance sees
 // after cvtColor).  grid = (blocks over chroma rows, frames of the range `cr`).
 template <int FMT>
-__global__ void __launch_bounds__(256, 8) k_vsum_yuv(Frames frames, int w, int h, unsigned long long* __restrict__ vsum,
+__global__ void __launch_bounds__(256, 8) k_vsum_yuv(YuvPlanes frames, int w, int h, unsigned long long* __restrict__ vsum,
                                                      CamRange cr) {
   const int fi = range_frame(cr, blockIdx.y);
-  const uint8_t* f = frames.frame(fi);
+  const YuvFrame f = frames.frame(fi);
   unsigned long long acc = 0;
   for (int cy = blockIdx.x; cy < h / 2; cy += gridDim.x) {
     unsigned s = 0;   // at most 4 * 255 per sample and FW/2 <= 16384 samples per row: fits 32 bits
-    for (int cx = threadIdx.x; cx < w / 2; cx += blockDim.x) s += yuv_vsum_2x2<FMT>(f, w, h, cx, cy);
+    for (int cx = threadIdx.x; cx < w / 2; cx += blockDim.x) s += yuv_vsum_2x2<FMT>(f, cx, cy);
     acc += s;
   }
 #pragma unroll

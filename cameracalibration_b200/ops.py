@@ -72,6 +72,34 @@ def _cuda_ptr(arr, shape):
     return int(ptr), got
 
 
+def _cuda_plane(arr, shape, what):
+    """(device pointer, byte strides) of a uint8 CUDA array of the given shape whose last axis is dense (pixels within a
+    row); the other axes may have any non-negative stride (pitched rows, views of a larger pool)."""
+    iface = getattr(arr, "__cuda_array_interface__", None)
+    if iface is None:
+        raise L.BevkError(f"{what}: expected a CUDA array (an object with __cuda_array_interface__)")
+    got = tuple(iface["shape"])
+    if iface["typestr"] not in ("|u1", "<u1", "=u1"):
+        raise L.BevkError(f"{what} must be uint8, got typestr {iface['typestr']}")
+    if got != tuple(shape):
+        raise L.BevkError(f"{what} must have shape {tuple(shape)}, got {got}")
+    strides = iface.get("strides")
+    if strides is None:
+        strides, step = [], 1
+        for n in reversed(got):
+            strides.insert(0, step)
+            step *= n
+    strides = [int(s) for s in strides]
+    if got[-1] > 1 and strides[-1] != 1:
+        raise L.BevkError(f"{what}: pixels within a row must be dense")
+    if any(s < 0 for s in strides):
+        raise L.BevkError(f"{what}: negative strides are not supported")
+    ptr = iface["data"][0]
+    if not ptr:
+        raise L.BevkError(f"{what} has a null data pointer")
+    return int(ptr), strides[:-1]
+
+
 def jpeg_decode(jpegs, width: int, height: int, out=None, ctx: L.Context | None = None):
     """Decode JPEG byte strings on the GPU (nvJPEG) into a uint8 CUDA frame stack [n][height][width][3] (BGR, what
     cv2.imread's layout is).  ``out``: a CUDA array of that shape; default a new torch tensor.  Enqueued on the ctx
@@ -736,6 +764,96 @@ class BevEngine:
                                                     C.c_void_p(d_car), (L.FLAG_BALANCE if balance else 0) | fmt | ofmt,
                                                     C.c_void_p(d_out)))
         return out
+
+    def run_cuda_planes(self, y, c=None, v=None, pixel_format: str = "nv12", car=None, balance: bool = False, out=None,
+                        stream: int | None = None, out_format: str = "bgr"):
+        """run_cuda() on YUV 4:2:0 frames given plane by plane, as video decoders leave them on the GPU (NVDEC /
+        DeepStream surfaces, FFmpeg CUDA frames' data[] and linesize[]): no repack into cv2's single buffer.
+
+        y: uint8 CUDA array [batch][n_cam][FH][FW]; c: [batch][n_cam][FH/2][FW] of interleaved U,V (pixel_format
+        "nv12") or [batch][n_cam][FH/2][FW/2] of U ("i420"); v: the V plane like c ("i420" only).  Strided views are
+        fine (e.g. slices of one decoder pool): rows may be padded to any pitch, pixels within a row must be dense, and
+        each plane has one row pitch for all frames.  Or y is a list (batch) of lists (n_cam) of per-frame plane tuples
+        (y, c) / (y, u, v) of 2-D CUDA arrays [rows][cols].  When every plane of every frame lies at one common frame
+        stride (a surface pool) the call goes through bevk_bev_run_yuv_planes, otherwise through the plane table of
+        bevk_bev_run_yuv_surfaces.  car, balance, out, stream and out_format as in run_cuda(); the result is that of
+        run_cuda() on the same frames in cv2's single-buffer layout.  Returns ``out``."""
+        if not self.finalized:
+            self.finalize()
+        fmt = self._pixel_format(pixel_format)
+        ofmt = self._out_format(out_format)
+        if not fmt:
+            raise L.BevkError(f"run_cuda_planes takes nv12 or i420 frames, not {pixel_format!r}")
+        planes, pitch = self._yuv_planes(y, c, v, fmt, pixel_format)
+        n = len(planes[0])
+        batch = n // self.n_cam
+        out, d_out = self._cuda_out(out, batch, ofmt)
+        d_car = _cuda_ptr(car, (self.BH, self.BW, 3))[0] if car is not None else None
+        if stream is None:
+            from .sharding import _torch_current_stream
+            stream = _torch_current_stream(self.ctx.device)
+        flags = (L.FLAG_BALANCE if balance else 0) | fmt | ofmt
+        pitches = (C.c_int64 * 3)(*(pitch + [pitch[-1]] * (3 - len(pitch))))
+        strides = {p[i] - p[i - 1] for p in planes for i in range(1, n)}
+        with self.ctx.on_stream(stream):
+            if len(strides) <= 1:   # a surface pool: plane p of frame i at planes[0][0] + i * stride + offset[p]
+                stride = strides.pop() if strides else 0
+                offs = [p[0] - planes[0][0] for p in planes]
+                offsets = (C.c_int64 * 3)(*(offs + [offs[-1]] * (3 - len(offs))))
+                L.check(self.ctx.lib.bevk_bev_run_yuv_planes(self.ctx.h, C.c_void_p(planes[0][0]), stride, offsets, pitches,
+                                                             batch, C.c_void_p(d_car), flags, C.c_void_p(d_out)))
+            else:
+                table = (C.c_void_p * (3 * n))()
+                for i in range(n):
+                    for k, p in enumerate(planes):
+                        table[3 * i + k] = p[i]
+                L.check(self.ctx.lib.bevk_bev_run_yuv_surfaces(self.ctx.h, table, pitches, batch, C.c_void_p(d_car), flags,
+                                                               C.c_void_p(d_out)))
+        return out
+
+    def _yuv_planes(self, y, c, v, fmt, name):
+        """([per plane: device address of the plane of every frame, frame-set major], [row pitch per plane]) of the
+        frames run_cuda_planes takes."""
+        FW, FH, nc = self.FW, self.FH, self.n_cam
+        shapes = [(FH, FW), (FH // 2, FW)] if fmt == L.FLAG_NV12 else [(FH, FW), (FH // 2, FW // 2), (FH // 2, FW // 2)]
+        what = ("y", "uv") if fmt == L.FLAG_NV12 else ("y", "u", "v")
+        if isinstance(y, (list, tuple)):
+            if c is not None or v is not None:
+                raise L.BevkError("with per-frame plane tuples, pass the list alone")
+            frames = []
+            for b, fs in enumerate(y):
+                if len(fs) != nc:
+                    raise L.BevkError(f"frame-set {b} has {len(fs)} frames, expected {nc}")
+                frames += list(fs)
+            if not frames:
+                raise L.BevkError("batch must be >= 1")
+            planes, pitch = [[] for _ in shapes], [None] * len(shapes)
+            for i, f in enumerate(frames):
+                if len(f) != len(shapes):
+                    raise L.BevkError(f"{name} frames are {len(shapes)} planes {what}, frame {i} has {len(f)}")
+                for k, a in enumerate(f):
+                    ptr, strides = _cuda_plane(a, shapes[k], f"{name} plane {what[k]}")
+                    if pitch[k] is None:
+                        pitch[k] = strides[0]
+                    elif strides[0] != pitch[k]:
+                        raise L.BevkError(f"every {what[k]} plane of a call must share one row pitch")
+                    planes[k].append(ptr)
+            return planes, pitch
+        arrs = [y, c] if fmt == L.FLAG_NV12 else [y, c, v]
+        if any(a is None for a in arrs) or (fmt == L.FLAG_NV12 and v is not None):
+            raise L.BevkError(f"{name} frames need the planes {', '.join(what)}")
+        planes, pitch, batch = [], [], None
+        for k, a in enumerate(arrs):
+            iface = getattr(a, "__cuda_array_interface__", None)
+            shape = tuple(iface["shape"]) if iface else ()
+            if len(shape) != 4 or shape[1:] != (nc,) + shapes[k] or shape[0] < 1 or (batch is not None and shape[0] != batch):
+                raise L.BevkError(f"{name} plane {what[k]} must be a uint8 CUDA array [batch][{nc}][{shapes[k][0]}]"
+                                  f"[{shapes[k][1]}], got {shape}")
+            batch = shape[0]
+            ptr, strides = _cuda_plane(a, shape, f"{name} plane {what[k]}")
+            planes.append([ptr + b * strides[0] + j * strides[1] for b in range(batch) for j in range(nc)])
+            pitch.append(strides[2])
+        return planes, pitch
 
     def cuda_to_jpeg(self, frames, quality: int = 95, car=None, balance: bool = False) -> list[bytes]:
         """run_cuda() followed by cv2.imencode('.jpg', canvas, [IMWRITE_JPEG_QUALITY, quality]) per frame-set: frames

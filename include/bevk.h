@@ -45,7 +45,8 @@ enum { BEVK_MODEL_FISHEYE = 0, BEVK_MODEL_PINHOLE = 1 };
  * the Y plane, then NV12: interleaved U,V rows; I420: the U plane, then the V plane, each frame_w/2 x frame_h/2 and
  * packed (two chroma rows per buffer row).  The result is byte for byte cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 /
  * COLOR_YUV2BGR_I420) followed by the BGR call.  Accepted by bevk_bev_run, bevk_bev_run_stack and
- * bevk_bev_host_copy_bytes; every other entry point with flags refuses them with BEVK_ERR_UNSUPPORTED.
+ * bevk_bev_host_copy_bytes, and required by bevk_bev_run_yuv_planes / _surfaces (frames as separate, pitched planes);
+ * every other entry point with flags refuses them with BEVK_ERR_UNSUPPORTED.
  * BEVK_FLAG_OUT_NV12 / BEVK_FLAG_OUT_I420 (exclusive: both is BEVK_ERR_ARG; they combine with BALANCE, the car and the
  * input flags) say the canvases are written as YUV 4:2:0: canvas b is the dense uint8[bev_h*3/2][bev_w] at
  * out + b * bev_w*bev_h*3/2 (bev_w, bev_h even, else BEVK_ERR_UNSUPPORTED, as cv2 refuses odd sizes), whose bytes are
@@ -189,6 +190,25 @@ int bevk_bev_run_frames(bevk_ctx *ctx, const void *const *frames, int batch, con
  * from there into d_out (any alignment).                                                                              */
 int bevk_bev_run_stack(bevk_ctx *ctx, const void *d_frames, int64_t frame_stride, int batch, const void *d_car, int flags,
                        void *d_out);
+/* YUV 4:2:0 frames as a video decoder leaves them on the device (NVDEC / DeepStream surfaces, FFmpeg CUDA frames'
+ * data[] / linesize[]): each plane at its own address, rows padded to their own pitch.  Plane p of frame i (= frame-set
+ * i / n_cam, camera i % n_cam): p = 0 Y (frame_w bytes a row), 1 interleaved U,V (NV12, frame_w bytes) or U (I420,
+ * frame_w/2), 2 V (I420, frame_w/2; not read for NV12); row r of it at <plane address> + r * pitch[p], with pitch[p] >=
+ * the plane's row bytes.  Pixels within a row are dense.  cv2's single buffer is the case offset = {0, w*h, w*h*5/4},
+ * pitch = {w, w/2, w/2} (I420), or offset = {0, w*h}, pitch = {w, w} (NV12).  Needs BEVK_FLAG_NV12 or _I420 (frame_w, frame_h even); combines
+ * with BALANCE, the car and BEVK_FLAG_OUT_*; the result is that of bevk_bev_run_stack on the same frames repacked
+ * densely, with no repack: only the bytes the conversion samples are read (any base, offset, pitch or stride; odd ones
+ * cost byte loads instead of word loads).  Refused with BEVK_ERR_ARG, nothing enqueued: no YUV flag or both, a pitch
+ * below its plane's row bytes, a null plane, batch * n_cam > 65535.  Only enqueues on the ctx stream, so it can be
+ * captured into a graph (after one eager call of the same shape).
+ * Surface pool: plane p of frame i at d_base + i * frame_stride + offset[p] (a plane may lie before d_base's Y plane). */
+int bevk_bev_run_yuv_planes(bevk_ctx *ctx, const void *d_base, int64_t frame_stride, const int64_t offset[3],
+                            const int64_t pitch[3], int batch, const void *d_car, int flags, void *d_out);
+/* Scattered surfaces: planes[3*i + p] is the DEVICE address of plane p of frame i (a HOST array of batch*n_cam*3
+ * pointers; the V entries of NV12 are not read).  The library keeps a device copy of the table and uploads it again only
+ * when its contents change, as bevk_bev_run_frames does. */
+int bevk_bev_run_yuv_surfaces(bevk_ctx *ctx, const void *const *planes, const int64_t pitch[3], int batch, const void *d_car,
+                              int flags, void *d_out);
 /* Per-camera partial canvases for camera-sharded multi-GPU runs: rank r renders only
  * cameras [cam_lo, cam_hi) into d_out (zero elsewhere); the saturating sum of the
  * ranks' partials equals the full canvas (balance is not supported in this mode). */
