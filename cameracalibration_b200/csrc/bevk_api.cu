@@ -131,6 +131,7 @@ struct Undistorter {
   bool valid = false, fused = false;
   CamModel cm;
   DevBuf map1, map2;
+  DevBuf xs;                      // cm.xs of a fused fisheye slot
 };
 
 struct BevCam {
@@ -149,6 +150,7 @@ struct bevk_ctx {
   bool timed = false;
   long long launches = 0;
   DevBuf s_src, s_dst, s_m1, s_m2, s_o1, s_o2;   // scratch for the host-pointer entry points
+  DevBuf s_xs;                                   // cm.xs of bevk_undistort_map and bevk_bev_set_camera
   Undistorter und[8];
   // BEV engine
   int n_cam = 0, FW = 0, FH = 0, BW = 0, BH = 0;
@@ -237,6 +239,20 @@ struct bevk_ctx {
 static int use(bevk_ctx* c) {
   if (!c) return fail(BEVK_ERR_ARG, "null ctx");
   CU(cudaSetDevice(c->device));
+  return BEVK_OK;
+}
+
+// The fisheye model's table of OpenCV's running _x per column (bevk_device.cuh, xs_table_applies) into buf, with cm->xs
+// pointing at it; other models and P keep cm->xs null.  buf must outlive every kernel launched with *cm.
+static int attach_xs_table(bevk_ctx* c, DevBuf& buf, CamModel* cm) {
+  cm->xs = nullptr;
+  if (!xs_table_applies(*cm)) return BEVK_OK;
+  if (c->capturing) return fail(BEVK_ERR_ARG, "a camera model cannot be set up inside a graph capture");
+  std::vector<double> xs((size_t)cm->w);
+  fill_xs_table(*cm, xs.data());
+  RET(buf.ensure(xs.size() * sizeof(double)));
+  CU(cudaMemcpyAsync(buf.p, xs.data(), xs.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  cm->xs = buf.as<double>();
   return BEVK_OK;
 }
 #define LAUNCHED(c)                 \
@@ -354,6 +370,7 @@ int bevk_undistort_map(bevk_ctx* c, int model, const double K[9], const double* 
   if (!map1 || !map2) return fail(BEVK_ERR_ARG, "null output map");
   CamModel cm;
   RET(make_model(model, K, D, n_dist, P, w, h, &cm));
+  RET(attach_xs_table(c, c->s_xs, &cm));
   const size_t n = (size_t)w * h;
   RET(c->s_m1.ensure(n * 4));
   RET(c->s_m2.ensure(n * 2));
@@ -466,12 +483,17 @@ int bevk_undistorter_set(bevk_ctx* c, int slot, int model, const double K[9], co
   u.valid = false;
   RET(make_model(model, K, D, n_dist, P, dw, dh, &u.cm));
   u.fused = fused != 0;
-  if (!u.fused) {
+  if (u.fused) {   // the gathers evaluate the model per pixel: the slot keeps its column table
+    RET(attach_xs_table(c, u.xs, &u.cm));
+  } else {         // the table is read once, by the map build, from scratch
+    u.xs.release();
+    RET(attach_xs_table(c, c->s_xs, &u.cm));
     const size_t n = (size_t)dw * dh;
     RET(u.map1.ensure(n * 4));
     RET(u.map2.ensure(n * 2));
     k_undistort_map<<<grid2d(dw, dh), 256, 0, c->stream>>>(u.cm, u.map1.as<short2>(), u.map2.as<unsigned short>());
     LAUNCHED(c);
+    u.cm.xs = nullptr;
   }
   u.valid = true;
   return BEVK_OK;
@@ -661,6 +683,7 @@ int bevk_bev_set_camera(bevk_ctx* c, int cam, const double K[9], const double D[
   RET(need_cam(c, cam));
   WarpMapsArgs a{};
   RET(make_model(BEVK_MODEL_FISHEYE, K, D, 4, P, und_w, und_h, &a.cm));
+  RET(attach_xs_table(c, c->s_xs, &a.cm));
   RET(make_homog(H, &a.hm));
   BevCam& k = c->cam[cam];
   const size_t n = (size_t)c->BW * c->BH;

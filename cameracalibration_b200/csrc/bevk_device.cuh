@@ -34,6 +34,7 @@ struct CamModel {      // cv2.fisheye / cv2 initUndistortRectifyMap inputs, pre-
   double fx, fy, cx, cy;
   int model;           // BEVK_MODEL_*
   int w, h;            // size of the undistorted (destination) frame
+  const double* xs;    // fisheye with row-independent rays (xs_table_applies): OpenCV's running _x of column j; else null
 };
 
 struct Homog { double M[9]; };   // inv(H), as cv2.warpPerspective computes it
@@ -96,10 +97,30 @@ __host__ __device__ __forceinline__ int cv_round(double v) {
   return d2i_rn(v);
 }
 
+// A1: cv2.fisheye.initUndistortRectifyMap walks each row with running sums, _x = i*iR01 + iR02 followed by _x += iR00 per
+// column (and the same for _y, _w); j*iR00 + (i*iR01 + iR02) differs from that sum in the last bits, which moves cvRound
+// ties.  When iR has no skew and the last row (0, 0, *) -- every P of dst_camera_matrix -- the sums of _y and _w add
+// zeros (exact) and _x depends on the column only: the host tabulates it once per map (fill_xs_table), the kernels read
+// xs[j].  Any other P, and the pinhole model, keep the direct form.
+inline bool xs_table_applies(const CamModel& c) {
+  return c.model == 0 && c.iR[1] == 0. && c.iR[3] == 0. && c.iR[6] == 0. && c.iR[7] == 0.;
+}
+inline void fill_xs_table(const CamModel& c, double* xs) {
+  double x = c.iR[2];   // 0 * iR01 + iR02
+  for (int j = 0; j < c.w; ++j) {
+    xs[j] = x;
+    x = dadd(x, c.iR[0]);
+  }
+}
+
 // A1 / A11: source-image position (u,v) of undistorted pixel (j,i).
 __host__ __device__ __forceinline__ void undistort_point(const CamModel& c, int j, int i, double& u, double& v) {
   const double dj = (double)j, di = (double)i;
-  const double _x = dadd(dmul(dj, c.iR[0]), dadd(dmul(di, c.iR[1]), c.iR[2]));
+#ifdef __CUDA_ARCH__
+  const double _x = c.xs ? __ldg(c.xs + j) : dadd(dmul(dj, c.iR[0]), dadd(dmul(di, c.iR[1]), c.iR[2]));
+#else
+  const double _x = c.xs ? c.xs[j] : dadd(dmul(dj, c.iR[0]), dadd(dmul(di, c.iR[1]), c.iR[2]));
+#endif
   const double _y = dadd(dmul(dj, c.iR[3]), dadd(dmul(di, c.iR[4]), c.iR[5]));
   const double _w = dadd(dmul(dj, c.iR[6]), dadd(dmul(di, c.iR[7]), c.iR[8]));
   if (c.model == 0) {  // equidistant fisheye

@@ -360,7 +360,11 @@ int bevk_bev_frames_to_jpeg(bevk_ctx *ctx, const void *const *frames, int batch,
  * BevGenerator.__call__ (surroundBEV.py:312-325) for a fixed set of device buffers costs one graph launch per
  * frame-set instead of up to five kernel launches and two memsets (BALANCE), and a host that stalls between calls
  * cannot starve the GPU.  Run the same calls once before capturing: a call that has to allocate or build tables
- * inside a capture fails, and bevk_graph_end reports it.  Host-pointer entry points cannot be captured.       */
+ * inside a capture fails, and bevk_graph_end reports it.  Host-pointer entry points cannot be captured.
+ * A graph keeps the device buffers it was captured with: a map slot's maps and a fused fisheye slot's column table
+ * (bevk_undistorter_set), and the BEV LUT.  Setting that slot or camera up again after the capture changes what the
+ * graph reads (or frees it, if the buffer had to grow); capture again after bevk_undistorter_set /
+ * bevk_bev_set_camera.  Those set-up calls (and bevk_undistort_map) cannot themselves be captured.            */
 int bevk_graph_begin(bevk_ctx *ctx);
 int bevk_graph_end(bevk_ctx *ctx, int *graph_id);
 int bevk_graph_launch(bevk_ctx *ctx, int graph_id, int times);

@@ -56,6 +56,8 @@ static int mode_maps(int model, int w, int h, const char* path) {
   for (int i = 0; i < (model == 0 ? 4 : 5); ++i) cm.k[i] = D[i];
   cm.fx = K[0]; cm.fy = K[4]; cm.cx = K[2]; cm.cy = K[5];
   cm.model = model; cm.w = w; cm.h = h;
+  std::vector<double> xs(w);   // as bevk_api.cu attaches it (attach_xs_table)
+  if (xs_table_applies(cm)) { fill_xs_table(cm, xs.data()); cm.xs = xs.data(); }
   FILE* f = fopen(path, "wb");
   if (!f) return 4;
   short* m1 = (short*)malloc((size_t)w * h * 4);
@@ -132,6 +134,8 @@ static int mode_bevmaps(int uw, int uh, int bw, int bh, const char* path) {
   for (int i = 0; i < 4; ++i) a.cm.k[i] = D[i];
   a.cm.fx = K[0]; a.cm.fy = K[4]; a.cm.cx = K[2]; a.cm.cy = K[5];
   a.cm.model = 0; a.cm.w = uw; a.cm.h = uh;
+  std::vector<double> xs(uw);
+  if (xs_table_applies(a.cm)) { fill_xs_table(a.cm, xs.data()); a.cm.xs = xs.data(); }
   if (!inv3(H, a.hm.M)) memset(a.hm.M, 0, sizeof a.hm.M);
   a.sw = uw; a.sh = uh; a.dw = bw; a.dh = bh;
   const size_t n = (size_t)bw * bh;
@@ -464,6 +468,8 @@ static int mode_gather(int mode, int sw, int sh, int dw, int dh, const char* in_
     if (!read_doubles(H, 9)) return 2;
     if (!inv3(H, hm.M)) memset(hm.M, 0, sizeof hm.M);
   }
+  std::vector<double> xs(dw);
+  if (mode == 1 && xs_table_applies(cm)) { fill_xs_table(cm, xs.data()); cm.xs = xs.data(); }
   const size_t sbytes = (size_t)sw * sh * 3;
   std::vector<uint8_t> src(sbytes + 16, 0), dst((size_t)dw * dh * 3);   // slack: the library's buffers have it too
   FILE* f = fopen(in_path, "rb");

@@ -123,6 +123,7 @@ static int mode_run(const char* in_path, const char* out_path) {
     int64_t st[4];
     if (fread(st, 8, 4, fi) != 4) return 5;
     GatherArgs a{};
+    std::vector<double> xs;
     a.sw = sw; a.sh = sh; a.spitch = st[0]; a.sistride = st[1]; a.dw = dw; a.dh = dh; a.dpitch = st[2]; a.distride = st[3]; a.n = n;
     const size_t npx = (size_t)dw * dh;
     short2* m1 = static_cast<short2*>(alloc(npx * 4));
@@ -138,6 +139,11 @@ static int mode_run(const char* in_path, const char* out_path) {
       for (int i = 0; i < 5; ++i) a.cm.k[i] = D[i];
       a.cm.fx = K[0]; a.cm.fy = K[4]; a.cm.cx = K[2]; a.cm.cy = K[5];
       a.cm.model = (int)model; a.cm.w = dw; a.cm.h = dh;
+      if (xs_table_applies(a.cm)) {   // as bevk_api.cu attaches it (attach_xs_table)
+        xs.resize(dw);
+        fill_xs_table(a.cm, xs.data());
+        a.cm.xs = xs.data();
+      }
     }
     const size_t sbytes = (size_t)((n - 1) * st[1] + (sh - 1) * st[0] + (int64_t)sw * ch);
     const size_t dbytes = (size_t)((n - 1) * st[3] + (dh - 1) * st[2] + (int64_t)dw * ch);
