@@ -4,7 +4,8 @@
 //
 //   jpeg_enc <in.bin> <out.bin>
 //     in : records of int32 width, height, quality, then width*height*3 bytes (BGR, dense)
-//     out: per record uint64 stream size, uint64 bevk_jpeg_encode_bound, the stream
+//     out: per record uint64 stream size, uint64 bevk_jpeg_encode_bound, uint64 entropy-coded bits (without the pad),
+//          the stream
 // Built by tests/test_host_jpeg.py with nvcc; only host code runs.
 #include <cstdint>
 #include <cstdio>
@@ -16,7 +17,7 @@
 
 using namespace bevk::jpeg;
 
-static std::vector<uint8_t> encode(const uint8_t* img, int W, int H, int quality) {
+static std::vector<uint8_t> encode(const uint8_t* img, int W, int H, int quality, unsigned long long* bits) {
   Tables t;
   make_tables(quality, &t);
   const Geom g = geom(W, H);
@@ -58,6 +59,7 @@ static std::vector<uint8_t> encode(const uint8_t* img, int W, int H, int quality
     if (cnt.n > (unsigned)kMaxBlockBits) { fprintf(stderr, "block %lld: %u bits > bound\n", b, cnt.n); exit(3); }
     pred[comp] = dc;
   }
+  *bits = pos;
   const int pad = (int)((8 - (pos & 7)) & 7);
   if (pad) wr.put((1u << pad) - 1u, pad);
   wr.flush();
@@ -90,9 +92,10 @@ int main(int argc, char** argv) {
     const int W = hdr[0], H = hdr[1], q = hdr[2];
     std::vector<uint8_t> img((size_t)W * H * 3);
     if (fread(img.data(), 1, img.size(), fi) != img.size()) return 5;
-    const std::vector<uint8_t> s = encode(img.data(), W, H, q);
-    const uint64_t meta[2] = {s.size(), encode_bound(W, H)};
-    fwrite(meta, 8, 2, fo);
+    unsigned long long bits = 0;
+    const std::vector<uint8_t> s = encode(img.data(), W, H, q, &bits);
+    const uint64_t meta[3] = {s.size(), encode_bound(W, H), bits};
+    fwrite(meta, 8, 3, fo);
     fwrite(s.data(), 1, s.size(), fo);
   }
   fclose(fi);

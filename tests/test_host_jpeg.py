@@ -39,7 +39,8 @@ def _cv2(img, q):
 
 
 def _host_encode(exe, tmp_path, cases):
-    """cases: [(BGR image, quality or None)] -> [(stream, bound)] from the host build of the encoder."""
+    """cases: [(BGR image, quality or None)] -> [(stream, bound, entropy bits without the pad)] from the host build of
+    the encoder."""
     blob = [struct.pack("<3i", img.shape[1], img.shape[0], 95 if q is None else q) + np.ascontiguousarray(img).tobytes()
             for img, q in cases]
     (tmp_path / "jpeg_in.bin").write_bytes(b"".join(blob))
@@ -48,15 +49,15 @@ def _host_encode(exe, tmp_path, cases):
     assert r.returncode == 0, (r.returncode, r.stderr[-2000:])
     raw, p, out = (tmp_path / "jpeg_out.bin").read_bytes(), 0, []
     for _ in cases:
-        n, bound = struct.unpack_from("<2Q", raw, p)
-        out.append((raw[p + 16:p + 16 + n], bound))
-        p += 16 + n
+        n, bound, bits = struct.unpack_from("<3Q", raw, p)
+        out.append((raw[p + 24:p + 24 + n], bound, bits))
+        p += 24 + n
     assert p == len(raw)
     return out
 
 
 def _check(exe, tmp_path, cases):
-    for (img, q), (got, bound) in zip(cases, _host_encode(exe, tmp_path, cases)):
+    for (img, q), (got, bound, _bits) in zip(cases, _host_encode(exe, tmp_path, cases)):
         want = _cv2(img, q)
         first = next((i for i in range(min(len(got), len(want))) if got[i] != want[i]), None)
         assert got == want, (img.shape, q, len(got), len(want), first)
