@@ -301,7 +301,9 @@ class BevGenerator:
     def run_batch(self, frame_sets, car=None, out=None, pixel_format="bgr", out_format="bgr"):
         """frame_sets: iterable of (front, back, left, right) tuples -> uint8[n][BH][BW][3].  pixel_format "nv12" /
         "i420": the frames are YUV 4:2:0 buffers uint8[FH*3//2][FW] (cv2's layout), converted to BGR on the GPU exactly
-        as cv2.cvtColor does.  out_format "nv12" / "i420": the canvases come back as uint8[n][BH*3//2][BW], each
+        as cv2.cvtColor does.  pixel_format "yuyv" / "uyvy": packed YUV 4:2:2 camera frames uint8[FH][FW][2], as
+        cv2.cvtColor(frame, COLOR_YUV2BGR_YUY2 / _UYVY) makes them BGR.  out_format "nv12" / "i420": the canvases come
+        back as uint8[n][BH*3//2][BW], each
         cv2.cvtColor(canvas, COLOR_BGR2YUV_I420) (NV12: U and V interleaved), converted on the GPU."""
         return self.engine.run([list(fs) for fs in frame_sets], car, self.balance, out, pixel_format=pixel_format,
                                out_format=out_format)
@@ -309,7 +311,8 @@ class BevGenerator:
     def run_cuda(self, frames, car=None, out=None, stream=None, pixel_format="bgr", out_format="bgr"):
         """Frame-sets that are already on the GPU (uint8 CUDA array [n][4][FH][FW][3] in front/back/left/right
         order, or nested lists of per-frame CUDA arrays) -> CUDA array [n][BH][BW][3]; nothing crosses PCIe.
-        pixel_format "nv12" / "i420": one uint8 CUDA array [n][4][FH*3//2][FW] of YUV 4:2:0 frames.  out_format
+        pixel_format "nv12" / "i420": one uint8 CUDA array [n][4][FH*3//2][FW] of YUV 4:2:0 frames; "yuyv" / "uyvy":
+        one uint8 CUDA array [n][4][FH][FW][2] of packed 4:2:2 frames.  out_format
         "nv12" / "i420": the result is uint8[n][BH*3//2][BW] YUV 4:2:0 canvases (see run_batch)."""
         return self.engine.run_cuda(frames, car, self.balance, out, stream, pixel_format=pixel_format, out_format=out_format)
 
@@ -317,7 +320,7 @@ class BevGenerator:
         """run_cuda on YUV 4:2:0 frame-sets given plane by plane, as a video decoder leaves them on the GPU (pitched
         rows, each plane at its own address): y uint8 CUDA array [n][4][FH][FW], c [n][4][FH/2][FW] interleaved U,V
         ("nv12") or [n][4][FH/2][FW/2] U ("i420"), v the V plane ("i420"); or nested lists of per-frame plane tuples.
-        See BevEngine.run_cuda_planes."""
+        "yuyv" / "uyvy": y alone, the packed frames [n][4][FH][FW][2] with padded rows.  See BevEngine.run_cuda_planes."""
         return self.engine.run_cuda_planes(y, c, v, pixel_format, car, self.balance, out, stream, out_format=out_format)
 
     def jpeg(self, front, back, left, right, car=None, quality=95):

@@ -16,7 +16,9 @@ MAPS_UNDISTORT, MAPS_BEV = 0, 1
 MODEL_FISHEYE, MODEL_PINHOLE = 0, 1
 FLAG_BALANCE = 1
 FLAG_NV12, FLAG_I420 = 2, 4          # YUV 4:2:0 frames (cv2's single-buffer layout), bevk_bev_run / _run_stack only
-PIXEL_FORMATS = {"bgr": 0, "nv12": FLAG_NV12, "i420": FLAG_I420}
+FLAG_YUYV, FLAG_UYVY = 32, 64        # packed YUV 4:2:2 frames uint8[FH][FW][2] (cv2's COLOR_YUV2BGR_YUY2 / _UYVY input)
+PIXEL_FORMATS = {"bgr": 0, "nv12": FLAG_NV12, "i420": FLAG_I420, "yuyv": FLAG_YUYV, "uyvy": FLAG_UYVY}
+PACKED_FORMATS = (FLAG_YUYV, FLAG_UYVY)
 FLAG_OUT_NV12, FLAG_OUT_I420 = 8, 16  # YUV 4:2:0 canvases uint8[BH*3/2][BW] (cv2.cvtColor(COLOR_BGR2YUV_I420) layout)
 OUT_FORMATS = {"bgr": 0, "nv12": FLAG_OUT_NV12, "i420": FLAG_OUT_I420}
 SHARD_FRAMES, SHARD_CAMERAS = 0, 1

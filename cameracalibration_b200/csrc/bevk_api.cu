@@ -167,11 +167,12 @@ struct bevk_ctx {
   long long span_fetch_bytes = 0;           // bytes k_fetch_spans moves per frame-set
   long long last_h2d_bytes = 0;             // host->device bytes of the last bevk_bev_run call
   int cam_box[BEVK_MAX_CAMERAS][BEVK_MAX_BANDS][4] = {};   // per camera and band: sampled rows [y0,y1), bytes [bx0,bx1)
-  // YUV sources, per format (NV12, I420): page-locked ingest windows [camera][FH*3/2] and their bytes per frame-set, and
+  // YUV sources, per format (NV12, I420, YUYV, UYVY): page-locked ingest windows [camera][buffer rows: FH*3/2 for 4:2:0,
+  // FH for 4:2:2] and their bytes per frame-set, and
   // the DMA rectangles of pageable frames per camera
-  DevBuf d_yuv_win[2];
-  long long yuv_fetch_bytes[2] = {0, 0};
-  std::vector<int4> yuv_rects[2][BEVK_MAX_CAMERAS];
+  DevBuf d_yuv_win[4];
+  long long yuv_fetch_bytes[4] = {0, 0, 0, 0};
+  std::vector<int4> yuv_rects[4][BEVK_MAX_CAMERAS];
   DevBuf d_tiles, d_items, d_lut, d_hsv;
   int bev_grid[6] = {0, 0, 0, 0, 0, 0};   // resident CTAs of k_bev<BAL, NB>: index = 3*BAL + {NB=1:0, 4:1, 8:2}
   DevBuf d_frames, d_canvas, d_car, d_vsum, d_delta, d_csum;
@@ -856,19 +857,20 @@ int bevk_bev_finalize(bevk_ctx* c) {
   c->n_bands = 2;
   if (const char* env = getenv("BEVK_BANDS")) c->n_bands = std::max(1, std::min(BEVK_MAX_BANDS, atoi(env)));
   for (int k = 0; k < NC; ++k) plan_bands(spans.data() + (size_t)k * FH, FW, FH, c->n_bands, c->cam_box[k]);
-  if (FW % 2 == 0 && FH % 2 == 0) {   // YUV 4:2:0 ingest of the same spans (odd sizes: YUV calls are refused)
-    const int rows = FH * 3 / 2;
+  // YUV ingest of the same spans: 4:2:2 needs an even width, 4:2:0 an even size (other sizes: those calls are refused)
+  for (int fmt = YUV_NV12; fmt <= YUV_UYVY && FW % 2 == 0; ++fmt) {
+    const bool packed = fmt == YUV_YUYV || fmt == YUV_UYVY;
+    if (!packed && FH % 2) continue;
+    const int rows = packed ? FH : FH * 3 / 2;
     std::vector<int4> win((size_t)NC * rows);
-    for (int fmt = YUV_NV12; fmt <= YUV_I420; ++fmt) {
-      for (int k = 0; k < NC; ++k) {
-        yuv_windows(fmt, spans.data() + (size_t)k * FH, FW, FH, win.data() + (size_t)k * rows);
-        yuv_dma_rects(fmt, c->cam_box[k], c->n_bands, FW, FH, c->yuv_rects[fmt - 1][k]);
-      }
-      c->yuv_fetch_bytes[fmt - 1] = yuv_window_bytes(win.data(), NC * rows);
-      RET(c->d_yuv_win[fmt - 1].ensure(win.size() * sizeof(int4)));
-      CU(cudaMemcpyAsync(c->d_yuv_win[fmt - 1].p, win.data(), win.size() * sizeof(int4), cudaMemcpyHostToDevice, c->stream));
-      CU(cudaStreamSynchronize(c->stream));   // win is reused for the next format
+    for (int k = 0; k < NC; ++k) {
+      yuv_windows(fmt, spans.data() + (size_t)k * FH, FW, FH, win.data() + (size_t)k * rows);
+      yuv_dma_rects(fmt, c->cam_box[k], c->n_bands, FW, FH, c->yuv_rects[fmt - 1][k]);
     }
+    c->yuv_fetch_bytes[fmt - 1] = yuv_window_bytes(win.data(), NC * rows);
+    RET(c->d_yuv_win[fmt - 1].ensure(win.size() * sizeof(int4)));
+    CU(cudaMemcpyAsync(c->d_yuv_win[fmt - 1].p, win.data(), win.size() * sizeof(int4), cudaMemcpyHostToDevice, c->stream));
+    CU(cudaStreamSynchronize(c->stream));   // win goes out of scope before the next format
   }
   RET(ensure_hsv(c));
   CU(cudaStreamSynchronize(c->stream));
@@ -969,20 +971,35 @@ int bevk_bev_tma_plan_info(bevk_ctx* c, int64_t* n_items, int64_t* n_shapes, int
 
 int64_t bevk_bev_last_h2d_bytes(bevk_ctx* c) { return c ? c->last_h2d_bytes : 0; }
 
-// Source pixel format of a call from its flags: 0 = BGR, YUV_NV12, YUV_I420.  YUV needs even frame sizes, as cv2 does.
+// Source pixel format of a call from its flags: 0 = BGR, YUV_NV12, YUV_I420, YUV_YUYV, YUV_UYVY.  YUV 4:2:0 needs an even
+// frame size and 4:2:2 an even width, as cv2 does.
+constexpr int kInFlags = BEVK_FLAG_NV12 | BEVK_FLAG_I420 | BEVK_FLAG_YUYV | BEVK_FLAG_UYVY;
 static int pixel_format(bevk_ctx* c, int flags, int* fmt) {
-  const int yuv = flags & (BEVK_FLAG_NV12 | BEVK_FLAG_I420);
+  const int yuv = flags & kInFlags;
   *fmt = 0;
   if (!yuv) return BEVK_OK;
-  if (yuv == (BEVK_FLAG_NV12 | BEVK_FLAG_I420)) return fail(BEVK_ERR_ARG, "BEVK_FLAG_NV12 and BEVK_FLAG_I420 are exclusive");
+  if (yuv & (yuv - 1)) return fail(BEVK_ERR_ARG, "the input flags BEVK_FLAG_NV12, _I420, _YUYV and _UYVY are exclusive");
+  if (yuv & (BEVK_FLAG_YUYV | BEVK_FLAG_UYVY)) {
+    if (c->FW & 1) return fail(BEVK_ERR_UNSUPPORTED, "YUV 4:2:2 frames need an even width, not %d", c->FW);
+    *fmt = yuv == BEVK_FLAG_YUYV ? YUV_YUYV : YUV_UYVY;
+    return BEVK_OK;
+  }
   if ((c->FW | c->FH) & 1) return fail(BEVK_ERR_UNSUPPORTED, "YUV 4:2:0 frames need an even size, not %d x %d", c->FW, c->FH);
   *fmt = yuv == BEVK_FLAG_NV12 ? YUV_NV12 : YUV_I420;
   return BEVK_OK;
 }
 
+static bool packed_format(int fmt) { return fmt == YUV_YUYV || fmt == YUV_UYVY; }
+
+// Bytes of one dense frame of pixel format fmt (0 = BGR).
+static int64_t frame_bytes_of(const bevk_ctx* c, int fmt) {
+  const int64_t px = (int64_t)c->FW * c->FH;
+  return !fmt ? 3 * px : packed_format(fmt) ? 2 * px : 3 * px / 2;
+}
+
 // Entry points that read BGR frames only refuse the YUV flags rather than read a YUV buffer as BGR.
 static int bgr_only(int flags, const char* fn) {
-  if (flags & (BEVK_FLAG_NV12 | BEVK_FLAG_I420)) return fail(BEVK_ERR_UNSUPPORTED, "%s takes BGR frames only (no YUV flags)", fn);
+  if (flags & kInFlags) return fail(BEVK_ERR_UNSUPPORTED, "%s takes BGR frames only (no YUV flags)", fn);
   return BEVK_OK;
 }
 
@@ -1012,7 +1029,7 @@ int bevk_bev_host_copy_bytes(bevk_ctx* c, int flags, int64_t* h2d, int64_t* d2h)
   RET(out_format(c, flags, &ofmt));
   int64_t up = 0;
   for (int k = 0; k < c->n_cam; ++k) {
-    if (flags & BEVK_FLAG_BALANCE) { up += (int64_t)c->FW * c->FH * (fmt ? 3 : 6) / 2; continue; }
+    if (flags & BEVK_FLAG_BALANCE) { up += frame_bytes_of(c, fmt); continue; }
     if (fmt) {
       for (const int4& r : c->yuv_rects[fmt - 1][k]) up += (int64_t)r.y * r.w;
       continue;
@@ -1180,7 +1197,7 @@ static int yuv_prepass_fmt(bevk_ctx* c, Frames src, const YuvPlanes* planes, int
   const CamRange cr{0, c->n_cam, c->n_cam};
   const YuvPlanes in = planes ? *planes : yuv_dense_planes<FMT>(src.base, src.stride, c->FW, c->FH);
   if (bal) {
-    const int blocks = std::max(1, std::min(c->FH / 2, c->n_sm * 4 / std::max(1, std::min(nf, 64)) + 1));
+    const int blocks = std::max(1, std::min(yuv_chroma_rows_of<FMT>(c->FH), c->n_sm * 4 / std::max(1, std::min(nf, 64)) + 1));
     RET(lum_deltas(c, batch, nullptr, 1, [&](unsigned long long* vsum) {
       k_vsum_yuv<FMT><<<dim3(blocks, nf), 256, 0, c->stream>>>(in, c->FW, c->FH, vsum, cr);
     }));
@@ -1201,8 +1218,12 @@ static int yuv_prepass_fmt(bevk_ctx* c, Frames src, const YuvPlanes* planes, int
 
 // The frames are `planes` when given, else the dense stack src (cv2's single-buffer layout).
 static int yuv_prepass(bevk_ctx* c, int fmt, Frames src, const YuvPlanes* planes, int batch, bool bal, Frames* bgr_src) {
-  return fmt == YUV_NV12 ? yuv_prepass_fmt<YUV_NV12>(c, src, planes, batch, bal, bgr_src)
-                         : yuv_prepass_fmt<YUV_I420>(c, src, planes, batch, bal, bgr_src);
+  switch (fmt) {
+    case YUV_NV12: return yuv_prepass_fmt<YUV_NV12>(c, src, planes, batch, bal, bgr_src);
+    case YUV_I420: return yuv_prepass_fmt<YUV_I420>(c, src, planes, batch, bal, bgr_src);
+    case YUV_YUYV: return yuv_prepass_fmt<YUV_YUYV>(c, src, planes, batch, bal, bgr_src);
+    default: return yuv_prepass_fmt<YUV_UYVY>(c, src, planes, batch, bal, bgr_src);
+  }
 }
 
 // colour balance of `batch` full canvases from their channel sums, then the car (null: none), in place
@@ -1414,8 +1435,9 @@ int bevk_bev_run_stack(bevk_ctx* c, const void* d_frames, int64_t frame_stride, 
   RET(pixel_format(c, flags, &fmt));
   if (fmt) {   // YUV frames are read byte- or word-wise by k_vsum_yuv / k_yuv_spans only: any base and stride will do
     if (!d_frames) return fail(BEVK_ERR_ARG, "null frame stack");
-    if (frame_stride < (int64_t)c->FW * c->FH * 3 / 2)
-      return fail(BEVK_ERR_ARG, "frame_stride %lld smaller than a YUV 4:2:0 frame", (long long)frame_stride);
+    if (frame_stride < frame_bytes_of(c, fmt))
+      return fail(BEVK_ERR_ARG, "frame_stride %lld smaller than a YUV %s frame", (long long)frame_stride,
+                  packed_format(fmt) ? "4:2:2" : "4:2:0");
   } else {
     RET(check_stack(c, d_frames, frame_stride));
   }
@@ -1424,16 +1446,16 @@ int bevk_bev_run_stack(bevk_ctx* c, const void* d_frames, int64_t frame_stride, 
 }
 
 // The checks the two plane entry points share, before anything is enqueued: a YUV flag, batch, and pitches that cover
-// their planes' rows (plane 2 only for I420).
+// their planes' rows (plane 1 not for 4:2:2, plane 2 only for I420).
 static int check_yuv_planes(bevk_ctx* c, const int64_t* pitch, int batch, int flags, int* fmt, int* n_planes) {
   RET(need_plan(c));
   RET(pixel_format(c, flags, fmt));
-  if (!*fmt) return fail(BEVK_ERR_ARG, "YUV planes need BEVK_FLAG_NV12 or BEVK_FLAG_I420");
+  if (!*fmt) return fail(BEVK_ERR_ARG, "YUV planes need BEVK_FLAG_NV12, _I420, _YUYV or _UYVY");
   if (!pitch) return fail(BEVK_ERR_ARG, "null pitch array");
   if (batch < 1 || (long long)batch * c->n_cam > 65535)
     return fail(BEVK_ERR_ARG, "batch %d x %d cameras out of range [1,65535] frames", batch, c->n_cam);
-  *n_planes = *fmt == YUV_NV12 ? 2 : 3;
-  const int row[3] = {c->FW, *fmt == YUV_NV12 ? c->FW : c->FW / 2, c->FW / 2};
+  *n_planes = packed_format(*fmt) ? 1 : *fmt == YUV_NV12 ? 2 : 3;
+  const int row[3] = {packed_format(*fmt) ? 2 * c->FW : c->FW, *fmt == YUV_NV12 ? c->FW : c->FW / 2, c->FW / 2};
   for (int p = 0; p < *n_planes; ++p)
     if (pitch[p] < row[p]) return fail(BEVK_ERR_ARG, "pitch[%d] %lld smaller than the plane's %d-byte rows", p, (long long)pitch[p], row[p]);
   return BEVK_OK;
@@ -1447,7 +1469,7 @@ int bevk_bev_run_yuv_planes(bevk_ctx* c, const void* d_base, int64_t frame_strid
   if (!d_base || !offset) return fail(BEVK_ERR_ARG, "null surface pool or offset array");
   YuvPlanes planes;
   for (int p = 0; p < 3; ++p) {
-    const int q = p < np ? p : 1;   // NV12: plane 2 is never read
+    const int q = p < np ? p : np - 1;   // NV12: plane 2, 4:2:2: planes 1 and 2 are never read
     planes.f[p] = Frames(static_cast<const uint8_t*>(d_base) + offset[q], frame_stride);
     planes.pitch[p] = pitch[q];
   }
@@ -1468,7 +1490,8 @@ int bevk_bev_run_yuv_surfaces(bevk_ctx* c, const void* const* surfaces, const in
       if (!surfaces[3 * i + p]) return fail(BEVK_ERR_ARG, "plane %d of frame %zu is null", p, i);
       tab[p * n + i] = surfaces[3 * i + p];
     }
-  if (np == 2) std::copy(tab.begin() + n, tab.begin() + 2 * n, tab.begin() + 2 * n);   // NV12: plane 2 is never read
+  for (int p = np; p < 3; ++p)   // NV12: plane 2, 4:2:2: planes 1 and 2 are never read
+    std::copy(tab.begin() + (np - 1) * n, tab.begin() + np * n, tab.begin() + p * n);
   if (c->yuv_tab != tab) {
     RET(c->d_yuv_tab.ensure(tab.size() * sizeof(void*)));
     c->yuv_tab = tab;
@@ -1483,7 +1506,7 @@ int bevk_bev_run_yuv_surfaces(bevk_ctx* c, const void* const* surfaces, const in
   const void* const* d_tab = c->d_yuv_tab.as<const void*>();
   for (int p = 0; p < 3; ++p) {
     planes.f[p] = Frames(d_tab + p * n);
-    planes.pitch[p] = pitch[p < np ? p : 1];
+    planes.pitch[p] = pitch[p < np ? p : np - 1];
   }
   c->timed = true;
   return run_canvases(c, planes.f[0], batch, d_car, flags, d_out, &planes);
@@ -1527,7 +1550,7 @@ int bevk_sat_sum_device(bevk_ctx* c, const void* const* parts, int n, uint64_t b
 // call of bevk_bev_run / bevk_bev_run_to_jpeg shares between its chunks.
 struct HostIngest {
   size_t row = 0, fbytes = 0, fpad = 0, cbytes = 0;
-  int fmt = 0, rows = 0;                  // pixel format (0 = BGR) and buffer rows of a frame (FH; FH * 3 / 2 for YUV)
+  int fmt = 0, rows = 0;                  // pixel format (0 = BGR) and buffer rows of a frame (FH; FH * 3 / 2 for 4:2:0)
   int ofmt = 0;                           // canvas format (out_format), and the bytes of one canvas in it
   size_t obytes = 0;
   int chunk = 0;
@@ -1555,9 +1578,11 @@ static int ingest_setup(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_str
   int fmt = 0, ofmt = 0;
   RET(pixel_format(c, flags, &fmt));
   RET(out_format(c, flags, &ofmt));
-  // a YUV frame is uint8[FH * 3 / 2][FW] at the same row stride; it is staged as it is and converted on the device
-  const int rows = fmt ? c->FH * 3 / 2 : c->FH;
-  const size_t row = (size_t)c->FW * (fmt ? 1 : 3), fbytes = row * rows, fpad = pad256(fbytes);
+  // a YUV 4:2:0 frame is uint8[FH * 3 / 2][FW] and a 4:2:2 one uint8[FH][FW][2], rows at the same stride; it is staged as
+  // it is and converted on the device
+  const bool packed = packed_format(fmt);
+  const int rows = fmt && !packed ? c->FH * 3 / 2 : c->FH;
+  const size_t row = (size_t)c->FW * (!fmt ? 3 : packed ? 2 : 1), fbytes = row * rows, fpad = pad256(fbytes);
   if (src_stride < (int64_t)row) return fail(BEVK_ERR_ARG, "src_stride %lld < row bytes", (long long)src_stride);
   const size_t cbytes = (size_t)c->BW * c->BH * 3;
   h->row = row; h->fbytes = fbytes; h->fpad = fpad; h->cbytes = cbytes; h->fmt = fmt; h->rows = rows;

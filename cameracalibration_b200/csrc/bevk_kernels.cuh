@@ -584,10 +584,24 @@ __global__ void __launch_bounds__(128) k_lum_spans(Frames in, uint8_t* __restric
 // plane.  NV12: then FH/2 rows of interleaved U,V.  I420: then the U plane and the V plane, each FW/2 x FH/2 and packed,
 // so two chroma rows share a buffer row: chroma row k (U rows 0..FH/2-1, then the V rows) starts at buffer row FH + k/2,
 // column (k & 1) * FW/2 -- which is also where cv2 looks for it in a buffer with padded rows.
+// YUV 4:2:2 sources (YUYV, UYVY), FW even, FH any: one plane uint8[FH][FW][2] (cv2's input of COLOR_YUV2BGR_YUY2 /
+// _UYVY) whose rows hold pixel pairs of 4 bytes, YUYV: Y0 U0 Y1 V0, UYVY: U0 Y0 V0 Y1; both pixels of a pair take its U
+// and V, so pixel (x, y) has the chroma sample (x/2, y).  It reads through plane 0 of a YuvFrame like the others.
 // The colour conversion runs once per sampled source pixel into the same copy stack the BALANCE pre-pass fills; the
 // fused render then reads BGR from there as it always does.
 // ---------------------------------------------------------------------------------
-enum { YUV_NV12 = 1, YUV_I420 = 2 };
+enum { YUV_NV12 = 1, YUV_I420 = 2, YUV_YUYV = 3, YUV_UYVY = 4 };
+
+// Packed 4:2:2: byte positions within a pixel pair.  Y0 at yuv_y_byte, Y1 two bytes on; U at yuv_u_byte, V two bytes on.
+template <int FMT>
+__host__ __device__ __forceinline__ constexpr bool yuv_packed() { return FMT == YUV_YUYV || FMT == YUV_UYVY; }
+template <int FMT>
+__host__ __device__ __forceinline__ constexpr int yuv_y_byte() { return FMT == YUV_YUYV ? 0 : 1; }
+template <int FMT>
+__host__ __device__ __forceinline__ constexpr int yuv_u_byte() { return FMT == YUV_YUYV ? 1 : 0; }
+// Chroma rows of an FH-row frame: FH / 2 for 4:2:0, FH for 4:2:2.
+template <int FMT>
+__host__ __device__ __forceinline__ constexpr int yuv_chroma_rows_of(int FH) { return yuv_packed<FMT>() ? FH : FH / 2; }
 
 // cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420), OpenCV 4.x's fixed-point form (20 fraction bits), with U, V the chroma
 // samples of pixel (x/2, y/2).  One definition for the kernels and the CPU tests.
@@ -616,7 +630,8 @@ __host__ __device__ __forceinline__ constexpr int yuv_chroma_step() { return FMT
 
 // The planes of one YUV frame as the conversion reads them: row r of plane p starts at plane[p] + r * pitch[p].  Plane 0
 // is Y (FW bytes a row), plane 1 interleaved U,V (NV12, FW bytes) or U (I420, FW/2), plane 2 V (I420, FW/2; unused for
-// NV12).  Rows may be padded to any pitch and the planes may lie anywhere, as a video decoder's surfaces do.
+// NV12).  YUYV / UYVY: plane 0 is the packed frame (2 FW bytes a row); planes 1 and 2 are not read.  Rows may be padded
+// to any pitch and the planes may lie anywhere, as a video decoder's surfaces do.
 struct YuvFrame {
   const uint8_t* plane[3];
   long long pitch[3];
@@ -634,12 +649,15 @@ struct YuvPlanes {
 
 // cv2's single-buffer layout uint8[FH*3/2][FW] as planes: byte offsets and pitches of Y, UV / U and V in the buffer.
 // NV12: {0, FH*FW}, pitches {FW, FW}; I420: {0, FH*FW, FH*FW + FH*FW/4}, pitches {FW, FW/2, FW/2} (the packed U and V
-// planes, chroma row k of yuv_chroma_rows at FH*FW + k*FW/2).
+// planes, chroma row k of yuv_chroma_rows at FH*FW + k*FW/2).  YUYV / UYVY: the one plane uint8[FH][FW][2], pitch 2 FW.
 template <int FMT>
 __host__ __device__ __forceinline__ void yuv_dense_layout(int FW, int FH, long long (&off)[3], long long (&pitch)[3]) {
   const long long y = (long long)FW * FH;
   off[0] = 0; pitch[0] = FW;
-  if (FMT == YUV_NV12) {
+  if (yuv_packed<FMT>()) {
+    pitch[0] = 2LL * FW;
+    off[1] = off[2] = 0; pitch[1] = pitch[2] = 2LL * FW;   // unused
+  } else if (FMT == YUV_NV12) {
     off[1] = y; pitch[1] = FW;
     off[2] = y; pitch[2] = FW;   // unused
   } else {
@@ -688,6 +706,35 @@ __host__ __device__ __forceinline__ void span_groups(int2 sp, int& g0, int& g1) 
   g1 = sp.y > sp.x ? (sp.y + 3) >> 2 : g0;
 }
 
+// The Y, U and V samples of group g (pixels [4g, 4g + n)) of row y of a packed 4:2:2 frame: its n/2 pixel pairs, bytes
+// [8g, 8g + 2n) of the row.  One 8-byte load when they are a whole 8-aligned group, word loads when 4-aligned, bytes
+// otherwise (chosen per pointer).  Y[2k], Y[2k+1], U[k], V[k] come from pair k; a missing second pair reads as zero.
+template <int FMT>
+__host__ __device__ __forceinline__ void yuv_packed_group(const YuvFrame& fr, int y, int x0, int n, int (&Y)[4], int (&U)[2],
+                                                          int (&V)[2]) {
+  const uint8_t* p = fr.plane[0] + (long long)y * fr.pitch[0] + 2 * x0;
+  unsigned w[2] = {0u, 0u};
+#ifdef __CUDA_ARCH__
+  const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+  if (n == 4 && (a & 7) == 0) {
+    const uint2 q = __ldg(reinterpret_cast<const uint2*>(p));
+    w[0] = q.x; w[1] = q.y;
+  } else if ((a & 3) == 0) {
+    for (int k = 0; k < (n >> 1); ++k) w[k] = __ldg(reinterpret_cast<const unsigned*>(p) + k);
+  } else
+#endif
+  {
+    for (int k = 0; k < (n >> 1); ++k)
+      for (int j = 0; j < 4; ++j) w[k] |= (unsigned)ld_u8(p + 4 * k + j) << (8 * j);
+  }
+  constexpr int yb = 8 * yuv_y_byte<FMT>(), ub = 8 * yuv_u_byte<FMT>();
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    Y[2 * k] = (w[k] >> yb) & 255; Y[2 * k + 1] = (w[k] >> (yb + 16)) & 255;
+    U[k] = (w[k] >> ub) & 255; V[k] = (w[k] >> (ub + 16)) & 255;
+  }
+}
+
 // One work item of k_yuv_spans: group g of row y of frame fr, converted to BGR in c[3 * px + {0,1,2}] and, with BAL,
 // luminance-balanced by delta d (tab: the HSV division tables).  Returns the number of pixels (4 or 2).  The word loads
 // are chosen per pointer, so an odd base or pitch only costs byte loads.
@@ -695,6 +742,17 @@ template <int FMT, bool BAL>
 __host__ __device__ __forceinline__ int yuv_group(const YuvFrame& fr, int FW, int y, int g, int d, const int* __restrict__ tab,
                                                   int (&c)[12]) {
   const int x0 = 4 * g, n = min(4, FW - x0);
+  if constexpr (yuv_packed<FMT>()) {
+    int Y[4], U[2], V[2];
+    yuv_packed_group<FMT>(fr, y, x0, n, Y, U, V);
+    const bool rt = x0 >= FW - (FW % 32);   // luminance_balance's row tail (a multiple of 4: whole groups)
+#pragma unroll
+    for (int px = 0; px < 4; ++px) {
+      yuv_bgr(Y[px], U[px >> 1], V[px >> 1], c[3 * px], c[3 * px + 1], c[3 * px + 2]);
+      if (BAL) hsv_roundtrip(c[3 * px], c[3 * px + 1], c[3 * px + 2], d, rt, tab, tab + 256);
+    }
+    return n;
+  }
   const uint8_t *ur, *vr;
   yuv_chroma_ptrs<FMT>(fr, y >> 1, ur, vr);
   ur += yuv_chroma_step<FMT>() * (x0 >> 1);
@@ -737,7 +795,8 @@ __host__ __device__ __forceinline__ int yuv_group(const uint8_t* __restrict__ f,
 }
 
 // The YUV source pre-pass of a fused render: k_lum_spans' work decomposition (one CTA per LUM_ROWS source rows of one
-// frame, the rows' span groups as one flat list), reading Y row y and chroma row y/2 of the frame's planes and writing BGR
+// frame, the rows' span groups as one flat list), reading Y row y and chroma row y/2 of the frame's planes (4:2:2: row y
+// of the packed plane) and writing BGR
 // into the copy stack (frame f at out_base + f * out_stride, rows FW * 3 bytes); with BAL each pixel then takes
 // luminance_balance's HSV round trip with the frame's delta, so a balanced YUV render has no extra pass over the frames.
 template <int FMT, bool BAL>
@@ -814,17 +873,46 @@ __host__ __device__ __forceinline__ unsigned yuv_vsum_2x2(const uint8_t* __restr
   return yuv_vsum_2x2<FMT>(yuv_dense_frame<FMT>(f, FW, FH), cx, cy);
 }
 
+// V = max(B, G, R) summed over the pixel pair that shares chroma sample (cx, y) of a packed 4:2:2 frame fr.
+template <int FMT>
+__host__ __device__ __forceinline__ unsigned yuv_vsum_pair(const YuvFrame& fr, int cx, int y) {
+  const uint8_t* p = fr.plane[0] + (long long)y * fr.pitch[0] + 4 * cx;
+  const int U = ld_u8(p + yuv_u_byte<FMT>()), V = ld_u8(p + yuv_u_byte<FMT>() + 2);
+  const int Yv[2] = {ld_u8(p + yuv_y_byte<FMT>()), ld_u8(p + yuv_y_byte<FMT>() + 2)};
+  unsigned s = 0;
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    int b, g, r;
+    yuv_bgr(Yv[k], U, V, b, g, r);
+    s += (unsigned)max(b, max(g, r));
+  }
+  return s;
+}
+
+// The sum of V over the pixels of chroma sample (cx, cy): a 2 x 2 block (4:2:0) or a pixel pair (4:2:2).
+template <int FMT>
+__host__ __device__ __forceinline__ unsigned yuv_vsum_sample(const YuvFrame& fr, int cx, int cy) {
+  if constexpr (yuv_packed<FMT>()) return yuv_vsum_pair<FMT>(fr, cx, cy);
+  else return yuv_vsum_2x2<FMT>(fr, cx, cy);
+}
+
+// The same on a dense packed frame f (rows 2 FW bytes apart).
+template <int FMT>
+__host__ __device__ __forceinline__ unsigned yuv_vsum_pair(const uint8_t* __restrict__ f, int FW, int FH, int cx, int y) {
+  return yuv_vsum_pair<FMT>(yuv_dense_frame<FMT>(f, FW, FH), cx, y);
+}
+
 // k_vsum for YUV frames: vsum[frame] += the exact sum of V over the whole converted frame (what luminance_balance sees
-// after cvtColor).  grid = (blocks over chroma rows, frames of the range `cr`).
+// after cvtColor).  grid = (blocks over chroma rows (yuv_chroma_rows_of), frames of the range `cr`).
 template <int FMT>
 __global__ void __launch_bounds__(256, 8) k_vsum_yuv(YuvPlanes frames, int w, int h, unsigned long long* __restrict__ vsum,
                                                      CamRange cr) {
   const int fi = range_frame(cr, blockIdx.y);
   const YuvFrame f = frames.frame(fi);
   unsigned long long acc = 0;
-  for (int cy = blockIdx.x; cy < h / 2; cy += gridDim.x) {
+  for (int cy = blockIdx.x; cy < yuv_chroma_rows_of<FMT>(h); cy += gridDim.x) {
     unsigned s = 0;   // at most 4 * 255 per sample and FW/2 <= 16384 samples per row: fits 32 bits
-    for (int cx = threadIdx.x; cx < w / 2; cx += blockDim.x) s += yuv_vsum_2x2<FMT>(f, cx, cy);
+    for (int cx = threadIdx.x; cx < w / 2; cx += blockDim.x) s += yuv_vsum_sample<FMT>(f, cx, cy);
     acc += s;
   }
 #pragma unroll
@@ -1007,7 +1095,7 @@ __global__ void __launch_bounds__(128) k_fetch_spans(const uint8_t* const* __res
 // The same for page-locked YUV frames: buffer row y of the uint8[FH*3/2][FW] frame brings its one or two 16-byte
 // windows win[camera][y] = (x0, x1, x2, x3), bytes [x0, x1) and [x2, x3) (yuv_windows in bevk_plan.cuh: everything
 // k_yuv_spans reads of the row).  grid = (FH*3/2, n_frames); frame f goes to dev_frames + f * dev_stride, rows
-// row_bytes (= FW) apart.
+// row_bytes (= FW) apart.  Packed 4:2:2 frames uint8[FH][FW][2] take the same kernel with FH rows of 2 FW bytes.
 __global__ void __launch_bounds__(128) k_fetch_yuv(const uint8_t* const* __restrict__ host_frames, uint8_t* __restrict__ dev_frames,
                                                    long long dev_stride, const int4* __restrict__ win, int n_cam, int rows,
                                                    long long host_stride, int row_bytes) {

@@ -152,7 +152,14 @@ inline int4 yuv_window(int b0, int b1, int lo, int hi) {   // [b0, b1) widened t
   return make_int4(std::max(lo, b0) & ~15, std::min(hi, (b1 + 15) & ~15), 0, 0);
 }
 
+// Packed 4:2:2 (fmt 3 YUYV, 4 UYVY; frames uint8[FH][FW][2]): FH buffer rows, each the BGR rule in 2-byte pixels (span
+// +- 4 px) widened to 16-byte bounds inside [0, 2 FW); win: [FH] per camera.
 inline void yuv_windows(int fmt, const int2* spans /* [FH] of one camera */, int FW, int FH, int4* win) {
+  if (fmt >= 3) {
+    for (int y = 0; y < FH; ++y)
+      win[y] = spans[y].y > spans[y].x ? yuv_window(2 * (spans[y].x - 4), 2 * (spans[y].y + 4), 0, 2 * FW) : make_int4(0, 0, 0, 0);
+    return;
+  }
   auto uni = [&](int cy, int& x0, int& x1) {     // union of the spans of Y rows 2 cy, 2 cy + 1
     x0 = INT_MAX; x1 = -1;
     for (int y = 2 * cy; y < 2 * cy + 2; ++y)
@@ -189,13 +196,19 @@ inline long long yuv_window_bytes(const int4* win, int rows) {
 }
 
 // Pageable YUV frames: the DMA rectangles (buffer row, rows, byte column, bytes) of one camera's band boxes (plan_bands,
-// BGR byte columns): the Y rows of each band, and the chroma rows of those rows over the band's pixel columns.
+// BGR byte columns): the Y rows of each band, and the chroma rows of those rows over the band's pixel columns.  Packed
+// 4:2:2: one rectangle per band, its rows and pixel columns widened to whole pixel pairs, in bytes.
 inline void yuv_dma_rects(int fmt, const int (*box)[4], int n_bands, int FW, int FH, std::vector<int4>& rects) {
   rects.clear();
   for (int bnd = 0; bnd < n_bands; ++bnd) {
     const int* bx = box[bnd];
     if (bx[1] <= bx[0]) continue;
     const int y0 = bx[0], y1 = bx[1], x0 = bx[2] / 3, x1 = bx[3] / 3;
+    if (fmt >= 3) {
+      const int p0 = x0 & ~1, p1 = std::min(FW, (x1 + 1) & ~1);
+      rects.push_back(make_int4(y0, y1 - y0, 2 * p0, 2 * (p1 - p0)));
+      continue;
+    }
     rects.push_back(make_int4(y0, y1 - y0, x0, x1 - x0));
     const int c0 = y0 / 2, c1 = (y1 - 1) / 2 + 1;   // chroma rows of Y rows [y0, y1)
     if (fmt == 1) {

@@ -492,6 +492,10 @@ class BevEngine:
         padded); the canvases are those of cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / _I420) followed by the BGR call.
         The conversion runs on the GPU, and only the bytes the render samples (1.5 per pixel) cross PCIe.
 
+        pixel_format "yuyv" / "uyvy": every frame is a packed YUV 4:2:2 frame uint8[FH][FW][2] as UVC / V4L2 and GMSL
+        cameras deliver it (rows may be padded, pixels must be dense); the canvases are those of cv2.cvtColor(frame,
+        COLOR_YUV2BGR_YUY2 / _UYVY) followed by the BGR call, with 2 bytes per sampled pixel crossing PCIe.
+
         out_format "nv12" / "i420": the canvases are returned as YUV 4:2:0, uint8[batch][BH*3//2][BW], each
         cv2.cvtColor(bgr_canvas, COLOR_BGR2YUV_I420) (NV12: its U and V planes interleaved); the conversion runs on the
         GPU, so 1.5 bytes per canvas pixel come back instead of 3."""
@@ -526,21 +530,32 @@ class BevEngine:
         return (batch, self.BH * 3 // 2, self.BW) if ofmt else (batch, self.BH, self.BW, 3)
 
     def _pixel_format(self, pixel_format: str) -> int:
-        """Flag bits of a pixel_format argument ("bgr", "nv12", "i420"); YUV 4:2:0 needs an even frame size."""
+        """Flag bits of a pixel_format argument ("bgr", "nv12", "i420", "yuyv", "uyvy"); YUV 4:2:0 needs an even frame
+        size, packed 4:2:2 an even frame width."""
         fmt = L.PIXEL_FORMATS.get(str(pixel_format).lower())
         if fmt is None:
             raise L.BevkError(f"pixel_format must be one of {sorted(L.PIXEL_FORMATS)}, got {pixel_format!r}")
-        if fmt and (self.FW % 2 or self.FH % 2):
+        if fmt in L.PACKED_FORMATS:
+            if self.FW % 2:
+                raise L.BevkError(f"{pixel_format} frames need an even frame width, this engine's is {self.FW}")
+        elif fmt and (self.FW % 2 or self.FH % 2):
             raise L.BevkError(f"{pixel_format} frames need an even frame size, this engine's is {self.FW} x {self.FH}")
         return fmt
 
-    def _yuv_view(self, f):
-        """A host YUV 4:2:0 frame as bevk_bev_run reads it: uint8[FH*3//2][FW] with contiguous rows."""
-        shape = (self.FH * 3 // 2, self.FW)
+    def _yuv_shape(self, fmt: int):
+        """Shape of one YUV frame of input flag fmt: uint8[FH*3//2][FW] (4:2:0) or uint8[FH][FW][2] (packed 4:2:2)."""
+        return (self.FH, self.FW, 2) if fmt in L.PACKED_FORMATS else (self.FH * 3 // 2, self.FW)
+
+    def _yuv_view(self, f, fmt: int):
+        """A host YUV frame as bevk_bev_run reads it: _yuv_shape(fmt) with dense pixels (rows may be padded)."""
+        shape = self._yuv_shape(fmt)
         if not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.shape != shape:
             got = f"{f.dtype} {f.shape}" if isinstance(f, np.ndarray) else type(f).__name__
-            raise L.BevkError(f"YUV 4:2:0 frames must be uint8{list(shape)} arrays, got {got}")
-        if f.strides[1] != 1 or f.strides[0] < self.FW:
+            kind = "packed YUV 4:2:2" if fmt in L.PACKED_FORMATS else "YUV 4:2:0"
+            name = next(k for k, v in L.PIXEL_FORMATS.items() if v == fmt)
+            raise L.BevkError(f"{kind} frames (pixel_format {name!r}) must be uint8{list(shape)} arrays, got {got}")
+        row = self.FW * (2 if fmt in L.PACKED_FORMATS else 1)
+        if any(s != d for s, d in zip(f.strides[1:], np.empty(shape[1:], np.uint8).strides)) or f.strides[0] < row:
             f = np.ascontiguousarray(f)
         return f, f.strides[0]
 
@@ -555,7 +570,7 @@ class BevEngine:
                 raise L.BevkError(f"frame-set {b} has {len(fs)} frames, expected {self.n_cam}")
             for k, f in enumerate(fs):
                 if fmt:
-                    img, s = self._yuv_view(f)
+                    img, s = self._yuv_view(f, fmt)
                 else:
                     f = self._conform(f)
                     img, w, h, s, ch = L.image_view(f)
@@ -677,7 +692,8 @@ class BevEngine:
                   pixel_format: str = "bgr", out_format: str = "bgr"):
         """Frame stack on the device (frame i at d_frames_ptr + i * frame_stride, i = set * n_cam + camera): the
         TMA-staged kernel when base and stride are 16-byte aligned.  Only enqueues on the ctx stream.  pixel_format
-        "nv12" / "i420": dense uint8[FH*3//2][FW] YUV 4:2:0 frames at any base and stride.  out_format "nv12" / "i420":
+        "nv12" / "i420": dense uint8[FH*3//2][FW] YUV 4:2:0 frames at any base and stride; "yuyv" / "uyvy": dense
+        uint8[FH][FW][2] packed 4:2:2 frames at any base and stride (see run()).  out_format "nv12" / "i420":
         d_out_ptr receives uint8[batch][BH*3//2][BW] YUV 4:2:0 canvases (see run())."""
         if not self.finalized:
             self.finalize()
@@ -714,7 +730,9 @@ class BevEngine:
 
         pixel_format "nv12" / "i420": frames is one C-contiguous uint8 CUDA array [batch][n_cam][FH*3//2][FW] of YUV
         4:2:0 frames in cv2's layout (e.g. NVDEC NV12 surfaces); the result is that of cv2.cvtColor to BGR followed by
-        the BGR call, with the conversion done on the GPU.
+        the BGR call, with the conversion done on the GPU.  pixel_format "yuyv" / "uyvy": one C-contiguous uint8 CUDA
+        array [batch][n_cam][FH][FW][2] of packed 4:2:2 frames; the result is that of cv2.cvtColor(COLOR_YUV2BGR_YUY2 /
+        _UYVY) followed by the BGR call.
 
         out_format "nv12" / "i420": ``out`` is uint8[batch][BH*3//2][BW], YUV 4:2:0 canvases as run() describes them
         (e.g. for a hardware video encoder's NV12 input)."""
@@ -746,21 +764,23 @@ class BevEngine:
         return out, _cuda_ptr(out, shape)[0]
 
     def _run_cuda_yuv(self, frames, car, balance, out, stream, fmt, name, ofmt=0):
-        """run_cuda() on a YUV 4:2:0 frame stack: bevk_bev_run_stack with a YUV flag."""
+        """run_cuda() on a YUV frame stack: bevk_bev_run_stack with a YUV flag."""
+        want = (self.n_cam,) + self._yuv_shape(fmt)
+        dims = "".join(f"[{n}]" for n in want)
         if not hasattr(frames, "__cuda_array_interface__"):
-            raise L.BevkError(f"{name} frames must be one uint8 CUDA array [batch][{self.n_cam}][{self.FH * 3 // 2}][{self.FW}]")
+            raise L.BevkError(f"{name} frames must be one uint8 CUDA array [batch]{dims}")
         base, shape = _cuda_ptr(frames, None)
-        want = (self.n_cam, self.FH * 3 // 2, self.FW)
-        if len(shape) != 4 or tuple(shape[1:]) != want or shape[0] < 1:
-            raise L.BevkError(f"{name} frames must be uint8[batch][{self.n_cam}][{self.FH * 3 // 2}][{self.FW}], got {tuple(shape)}")
+        if len(shape) != len(want) + 1 or tuple(shape[1:]) != want or shape[0] < 1:
+            raise L.BevkError(f"{name} frames must be uint8[batch]{dims}, got {tuple(shape)}")
         batch = shape[0]
+        frame_bytes = int(np.prod(want[1:]))
         out, d_out = self._cuda_out(out, batch, ofmt)
         d_car = _cuda_ptr(car, (self.BH, self.BW, 3))[0] if car is not None else None
         if stream is None:
             from .sharding import _torch_current_stream
             stream = _torch_current_stream(self.ctx.device)
         with self.ctx.on_stream(stream):
-            L.check(self.ctx.lib.bevk_bev_run_stack(self.ctx.h, C.c_void_p(base), self.FW * self.FH * 3 // 2, batch,
+            L.check(self.ctx.lib.bevk_bev_run_stack(self.ctx.h, C.c_void_p(base), frame_bytes, batch,
                                                     C.c_void_p(d_car), (L.FLAG_BALANCE if balance else 0) | fmt | ofmt,
                                                     C.c_void_p(d_out)))
         return out
@@ -777,13 +797,17 @@ class BevEngine:
         (y, c) / (y, u, v) of 2-D CUDA arrays [rows][cols].  When every plane of every frame lies at one common frame
         stride (a surface pool) the call goes through bevk_bev_run_yuv_planes, otherwise through the plane table of
         bevk_bev_run_yuv_surfaces.  car, balance, out, stream and out_format as in run_cuda(); the result is that of
-        run_cuda() on the same frames in cv2's single-buffer layout.  Returns ``out``."""
+        run_cuda() on the same frames in cv2's single-buffer layout.  Returns ``out``.
+
+        pixel_format "yuyv" / "uyvy": y is the one packed plane, a strided uint8 CUDA array [batch][n_cam][FH][FW][2]
+        (rows padded to any pitch, pixels dense) or a list of lists of per-frame 1-tuples (y,) of [FH][FW][2] arrays; c
+        and v must be None.  The result is that of run_cuda() on the same frames packed densely."""
         if not self.finalized:
             self.finalize()
         fmt = self._pixel_format(pixel_format)
         ofmt = self._out_format(out_format)
         if not fmt:
-            raise L.BevkError(f"run_cuda_planes takes nv12 or i420 frames, not {pixel_format!r}")
+            raise L.BevkError(f"run_cuda_planes takes nv12, i420, yuyv or uyvy frames, not {pixel_format!r}")
         planes, pitch = self._yuv_planes(y, c, v, fmt, pixel_format)
         n = len(planes[0])
         batch = n // self.n_cam
@@ -815,8 +839,20 @@ class BevEngine:
         """([per plane: device address of the plane of every frame, frame-set major], [row pitch per plane]) of the
         frames run_cuda_planes takes."""
         FW, FH, nc = self.FW, self.FH, self.n_cam
-        shapes = [(FH, FW), (FH // 2, FW)] if fmt == L.FLAG_NV12 else [(FH, FW), (FH // 2, FW // 2), (FH // 2, FW // 2)]
-        what = ("y", "uv") if fmt == L.FLAG_NV12 else ("y", "u", "v")
+        packed = fmt in L.PACKED_FORMATS
+        if packed:
+            shapes, what = [(FH, FW, 2)], ("packed",)
+        elif fmt == L.FLAG_NV12:
+            shapes, what = [(FH, FW), (FH // 2, FW)], ("y", "uv")
+        else:
+            shapes, what = [(FH, FW), (FH // 2, FW // 2), (FH // 2, FW // 2)], ("y", "u", "v")
+
+        def plane(a, shape, k):
+            ptr, strides = _cuda_plane(a, shape, f"{name} plane {what[k]}")
+            if packed and strides[-1] != 2:
+                raise L.BevkError(f"{name} plane {what[k]}: the pixels of a row must be dense (2 bytes apart)")
+            return ptr, strides
+
         if isinstance(y, (list, tuple)):
             if c is not None or v is not None:
                 raise L.BevkError("with per-frame plane tuples, pass the list alone")
@@ -832,25 +868,31 @@ class BevEngine:
                 if len(f) != len(shapes):
                     raise L.BevkError(f"{name} frames are {len(shapes)} planes {what}, frame {i} has {len(f)}")
                 for k, a in enumerate(f):
-                    ptr, strides = _cuda_plane(a, shapes[k], f"{name} plane {what[k]}")
+                    ptr, strides = plane(a, shapes[k], k)
                     if pitch[k] is None:
                         pitch[k] = strides[0]
                     elif strides[0] != pitch[k]:
                         raise L.BevkError(f"every {what[k]} plane of a call must share one row pitch")
                     planes[k].append(ptr)
             return planes, pitch
-        arrs = [y, c] if fmt == L.FLAG_NV12 else [y, c, v]
+        if packed:
+            if c is not None or v is not None:
+                raise L.BevkError(f"{name} frames are one packed plane: pass y alone (c and v must be None)")
+            arrs = [y]
+        else:
+            arrs = [y, c] if fmt == L.FLAG_NV12 else [y, c, v]
         if any(a is None for a in arrs) or (fmt == L.FLAG_NV12 and v is not None):
             raise L.BevkError(f"{name} frames need the planes {', '.join(what)}")
         planes, pitch, batch = [], [], None
         for k, a in enumerate(arrs):
             iface = getattr(a, "__cuda_array_interface__", None)
             shape = tuple(iface["shape"]) if iface else ()
-            if len(shape) != 4 or shape[1:] != (nc,) + shapes[k] or shape[0] < 1 or (batch is not None and shape[0] != batch):
-                raise L.BevkError(f"{name} plane {what[k]} must be a uint8 CUDA array [batch][{nc}][{shapes[k][0]}]"
-                                  f"[{shapes[k][1]}], got {shape}")
+            if (len(shape) != 2 + len(shapes[k]) or shape[1:] != (nc,) + shapes[k] or shape[0] < 1 or
+                    (batch is not None and shape[0] != batch)):
+                raise L.BevkError(f"{name} plane {what[k]} must be a uint8 CUDA array [batch][{nc}]"
+                                  f"{''.join(f'[{n}]' for n in shapes[k])}, got {shape}")
             batch = shape[0]
-            ptr, strides = _cuda_plane(a, shape, f"{name} plane {what[k]}")
+            ptr, strides = plane(a, shape, k)
             planes.append([ptr + b * strides[0] + j * strides[1] for b in range(batch) for j in range(nc)])
             pitch.append(strides[2])
         return planes, pitch

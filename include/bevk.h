@@ -53,8 +53,16 @@ enum { BEVK_MODEL_FISHEYE = 0, BEVK_MODEL_PINHOLE = 1 };
  * cv2.cvtColor(bgr, COLOR_BGR2YUV_I420) of the BGR canvas `bgr` the same call writes without the flag (OUT_NV12: the
  * same Y plane, then the U and V planes interleaved).  The conversion runs on the device, so only 1.5 bytes per canvas
  * pixel leave it.  Accepted by bevk_bev_run, bevk_bev_run_device, bevk_bev_run_frames, bevk_bev_run_stack and
- * bevk_bev_host_copy_bytes; every other entry point with flags refuses them with BEVK_ERR_UNSUPPORTED. */
-enum { BEVK_FLAG_BALANCE = 1, BEVK_FLAG_NV12 = 2, BEVK_FLAG_I420 = 4, BEVK_FLAG_OUT_NV12 = 8, BEVK_FLAG_OUT_I420 = 16 };
+ * bevk_bev_host_copy_bytes; every other entry point with flags refuses them with BEVK_ERR_UNSUPPORTED.
+ * BEVK_FLAG_YUYV / BEVK_FLAG_UYVY say the frames are packed YUV 4:2:2 as UVC / V4L2 and GMSL cameras deliver them,
+ * uint8[frame_h][frame_w][2] (cv2's input shape for these codes; frame_w even, else BEVK_ERR_UNSUPPORTED; frame_h may be
+ * odd): each row holds pixel pairs of 4 bytes, YUYV: Y0 U0 Y1 V0, UYVY: U0 Y0 V0 Y1, and both pixels of a pair take its
+ * U and V.  The result is byte for byte cv2.cvtColor(frame, COLOR_YUV2BGR_YUY2 / COLOR_YUV2BGR_UYVY) followed by the BGR
+ * call.  They are accepted wherever the NV12 / I420 flags are and combine with the same flags; the plane entry points
+ * take one plane (offset[0] / plane 0, pitch[0] >= 2 * frame_w; entries 1 and 2 are not read).  Any two of the four input
+ * flags together are BEVK_ERR_ARG. */
+enum { BEVK_FLAG_BALANCE = 1, BEVK_FLAG_NV12 = 2, BEVK_FLAG_I420 = 4, BEVK_FLAG_OUT_NV12 = 8, BEVK_FLAG_OUT_I420 = 16,
+       BEVK_FLAG_YUYV = 32, BEVK_FLAG_UYVY = 64 };
 #define BEVK_MAX_CAMERAS 8
 
 int bevk_version(void);
@@ -162,7 +170,10 @@ int bevk_bev_finalize(bevk_ctx *ctx);
  * src_stride bytes apart.  Page-locked frames (frame_w and src_stride multiples of 16, no BALANCE) are read by the SMs
  * in the 16-byte windows around the sampled Y spans and the matching chroma bytes; pageable ones go up as the band
  * rectangles of the Y plane plus their chroma rows; with BALANCE whole frames.  On the device the sampled spans are
- * converted to BGR (and balanced) into a copy stack that the TMA-staged kernel renders from. */
+ * converted to BGR (and balanced) into a copy stack that the TMA-staged kernel renders from.
+ * With BEVK_FLAG_YUYV / _UYVY each frame is uint8[frame_h][frame_w][2], rows src_stride bytes apart: page-locked frames
+ * (2 * frame_w and src_stride multiples of 16, no BALANCE) bring the 16-byte windows around the sampled spans, pageable
+ * ones the band rectangles widened to whole pixel pairs, BALANCE whole frames (2 bytes per pixel). */
 int bevk_bev_run(bevk_ctx *ctx, const uint8_t *const *srcs, int64_t src_stride, int batch,
                  const uint8_t *car, int flags, uint8_t *out);
 /* Device-resident variant: d_srcs is a DEVICE array of batch*n_cam device pointers
@@ -187,7 +198,8 @@ int bevk_bev_run_frames(bevk_ctx *ctx, const void *const *frames, int batch, con
  * friendly BGR copy stack, so the TMA-staged kernel renders them whenever a TMA plan exists.  Still only enqueues, so
  * it can be captured into a graph (after one eager call of the same shape).  The same holds with BEVK_FLAG_OUT_NV12 /
  * _I420 (here and in bevk_bev_run_device / _frames): the BGR canvases are rendered into library scratch and converted
- * from there into d_out (any alignment).                                                                              */
+ * from there into d_out (any alignment).  With BEVK_FLAG_YUYV / _UYVY frame i is the dense uint8[frame_h][frame_w][2]
+ * packed frame at d_frames + i * frame_stride (any base and any stride >= frame_w * frame_h * 2).                     */
 int bevk_bev_run_stack(bevk_ctx *ctx, const void *d_frames, int64_t frame_stride, int batch, const void *d_car, int flags,
                        void *d_out);
 /* YUV 4:2:0 frames as a video decoder leaves them on the device (NVDEC / DeepStream surfaces, FFmpeg CUDA frames'
@@ -199,7 +211,9 @@ int bevk_bev_run_stack(bevk_ctx *ctx, const void *d_frames, int64_t frame_stride
  * with BALANCE, the car and BEVK_FLAG_OUT_*; the result is that of bevk_bev_run_stack on the same frames repacked
  * densely, with no repack: only the bytes the conversion samples are read (any base, offset, pitch or stride; odd ones
  * cost byte loads instead of word loads).  Refused with BEVK_ERR_ARG, nothing enqueued: no YUV flag or both, a pitch
- * below its plane's row bytes, a null plane, batch * n_cam > 65535.  Only enqueues on the ctx stream, so it can be
+ * below its plane's row bytes, a null plane, batch * n_cam > 65535.  With BEVK_FLAG_YUYV / _UYVY a frame is the one
+ * packed plane 0 (rows of 2 * frame_w bytes, pitch[0] >= that); offset / pitch / plane entries 1 and 2 are not read.
+ * Only enqueues on the ctx stream, so it can be
  * captured into a graph (after one eager call of the same shape).
  * Surface pool: plane p of frame i at d_base + i * frame_stride + offset[p] (a plane may lie before d_base's Y plane). */
 int bevk_bev_run_yuv_planes(bevk_ctx *ctx, const void *d_base, int64_t frame_stride, const int64_t offset[3],
@@ -234,7 +248,8 @@ int bevk_bev_plan_info(bevk_ctx *ctx, int64_t *n_tiles, int64_t *n_items, int64_
 /* Bytes bevk_bev_run moves over PCIe per frame-set for the given flags: host->device (without
  * BALANCE only the rectangle of each frame its camera's LUT can sample is uploaded; with BALANCE
  * the whole frames, because the V means cover them) and device->host (the canvas).  With a YUV
- * flag: the Y rectangles and their chroma rows (1.5 bytes per pixel), or whole YUV frames.  With an
+ * flag: the Y rectangles and their chroma rows (1.5 bytes per pixel; YUYV / UYVY: the rectangles at 2 bytes per
+ * pixel), or whole YUV frames.  With an
  * output flag the canvas is bev_w*bev_h*3/2 bytes. */
 int bevk_bev_host_copy_bytes(bevk_ctx *ctx, int flags, int64_t *h2d_per_frame_set, int64_t *d2h_per_frame_set);
 /* Host->device bytes the last bevk_bev_run call actually moved (page-locked frames are ingested span
