@@ -323,19 +323,19 @@ class BevGenerator:
         "yuyv" / "uyvy": y alone, the packed frames [n][4][FH][FW][2] with padded rows.  See BevEngine.run_cuda_planes."""
         return self.engine.run_cuda_planes(y, c, v, pixel_format, car, self.balance, out, stream, out_format=out_format)
 
-    def jpeg(self, front, back, left, right, car=None, quality=95):
-        """cv2.imencode('.jpg', self(front, back, left, right, car), [IMWRITE_JPEG_QUALITY, quality]) -- the bytes
-        main()'s cv2.imwrite('./surround.jpg', surround) writes (reference surroundBEV.py:340) -- encoded on the GPU:
-        only the JPEG stream crosses PCIe."""
-        return self.engine.run_to_jpeg([[front, back, left, right]], quality, car, self.balance)[0]
+    def jpeg(self, front, back, left, right, car=None, quality=95, params=None):
+        """cv2.imencode('.jpg', self(front, back, left, right, car), [IMWRITE_JPEG_QUALITY, quality] + params) -- the
+        bytes main()'s cv2.imwrite('./surround.jpg', surround) writes (reference surroundBEV.py:340) -- encoded on the
+        GPU: only the JPEG stream crosses PCIe.  params: cv2.imwrite's other JPEG pairs (see ops.jpeg_encode)."""
+        return self.engine.run_to_jpeg([[front, back, left, right]], quality, car, self.balance, params)[0]
 
-    def jpeg_batch(self, frame_sets, car=None, quality=95):
+    def jpeg_batch(self, frame_sets, car=None, quality=95, params=None):
         """frame_sets: iterable of (front, back, left, right) host tuples -> one JPEG ``bytes`` per frame-set."""
-        return self.engine.run_to_jpeg([list(fs) for fs in frame_sets], quality, car, self.balance)
+        return self.engine.run_to_jpeg([list(fs) for fs in frame_sets], quality, car, self.balance, params)
 
-    def jpeg_cuda(self, frames, car=None, quality=95):
+    def jpeg_cuda(self, frames, car=None, quality=95, params=None):
         """Frame-sets already on the GPU (as run_cuda takes them) -> one JPEG ``bytes`` per frame-set."""
-        return self.engine.cuda_to_jpeg(frames, quality, car, self.balance)
+        return self.engine.cuda_to_jpeg(frames, quality, car, self.balance, params)
 
 
 FRAME_WIDTH, FRAME_HEIGHT, BEV_WIDTH, BEV_HEIGHT = _geo.FW, _geo.FH, _geo.BW, _geo.BH

@@ -217,13 +217,17 @@ struct bevk_ctx {
   // nvJPEG ingest (bevk_jpeg_decode): library handle + decoder state, created on first use
   void* jpeg_handle = nullptr; void* jpeg_state = nullptr;
   DevBuf d_jpeg_frames, d_jpeg_canvas;
-  // JPEG encoder (bevk_jpeg_encode): header and tables of the last (width, height, quality), work buffers.  The
-  // compacted streams, their layout and their sizes are double-buffered (two slots), so that one batch can be encoded
-  // while the streams of the one before are still being copied out on out_stream.
+  // JPEG encoder (bevk_jpeg_encode): the cv2.imwrite parameters of bevk_jpeg_set_params, header and tables of the last
+  // (width, height, normalised options), work buffers.  The compacted streams, their layout and their sizes are
+  // double-buffered (two slots), so that one batch can be encoded while the streams of the one before are still being
+  // copied out on out_stream.
   struct JpegEnc {
-    int w = 0, h = 0, q = -1;
-    uint8_t header[jpeg::kHeaderBytes];
+    std::vector<int> params;
+    int w = 0, h = 0;
+    jpeg::Opts o{0, 0, -1, -1};
+    uint8_t header[jpeg::kMaxHeaderBytes] = {};
     DevBuf d_header, d_tabs, coef, bits, offs, dcdiff, words, ffcnt, ffscan, scan_tmp, out[2], meta[2];
+    DevBuf ilen, iofs, counts, huff, hdrs, hlen;   // restart intervals; optimised tables
     unsigned long long* h_sizes[2] = {nullptr, nullptr};   // page-locked copies of a slot's stream sizes
     size_t h_sizes_cap[2] = {0, 0};
     cudaStream_t out_stream = nullptr;                      // D2H of the streams
@@ -2313,6 +2317,37 @@ int bevk_jpeg_encode_bound(int width, int height, uint64_t* bytes) {
   return BEVK_OK;
 }
 
+// A bevk_jpeg_set_params list: keys 2..7 of cv2.IMWRITE_JPEG_*, normalised by jpeg::normalise.  The streams the device
+// encoder writes are baseline and one scan: PROGRESSIVE asks for another entropy coder and is refused, not ignored.
+static int jpeg_params_check(const int* params, int n, jpeg::Opts* o) {
+  if (n < 0 || (n & 1) || (n && !params)) return fail(BEVK_ERR_ARG, "JPEG params: %d ints, need (key, value) pairs", n);
+  for (int i = 0; i < n; i += 2)
+    if (params[i] < jpeg::kProgressive || params[i] > jpeg::kSamplingFactor)
+      return fail(BEVK_ERR_ARG, "JPEG params: key %d (IMWRITE_JPEG_QUALITY is the quality argument of each call; "
+                  "keys are 2..7)", params[i]);
+  jpeg::normalise(95, params, n, o);
+  if (o->progressive) return fail(BEVK_ERR_UNSUPPORTED, "JPEG params: IMWRITE_JPEG_PROGRESSIVE is not supported");
+  return BEVK_OK;
+}
+
+int bevk_jpeg_set_params(bevk_ctx* c, const int* params, int n) {
+  RET(use(c));
+  jpeg::Opts o;
+  RET(jpeg_params_check(params, n, &o));
+  c->enc.params.assign(params, params + n);
+  return BEVK_OK;
+}
+
+int bevk_jpeg_encode_bound_params(int width, int height, const int* params, int n, uint64_t* bytes) {
+  if (!bytes) return fail(BEVK_ERR_ARG, "null bytes");
+  if (width < 1 || height < 1 || width > jpeg::kMaxDim || height > jpeg::kMaxDim)
+    return fail(BEVK_ERR_ARG, "bad JPEG size %dx%d (1..%d)", width, height, jpeg::kMaxDim);
+  jpeg::Opts o;
+  RET(jpeg_params_check(params, n, &o));
+  *bytes = jpeg::encode_bound(jpeg::geom(width, height, o), o);
+  return BEVK_OK;
+}
+
 // What the encoder reads: n images at img + i * istride, rows pitch bytes apart.  With csum they are raw BEV canvases
 // under BALANCE (GainSrc): colour balance from their channel sums csum[3 * i ...] and the car (NULL or a dense canvas)
 // are applied as the blocks are loaded.
@@ -2330,23 +2365,25 @@ static int jpeg_enqueue(bevk_ctx* c, int s, const JpegIn& in, int n, int w, int 
   using namespace jpeg;
   auto& e = c->enc;
   if (!e.out_stream) RET(create_stream_set(&e.out_stream, {&e.ev_sizes[0], &e.ev_sizes[1], &e.ev_out_free[0], &e.ev_out_free[1]}));
-  const int q = clamp_quality(quality);
-  if (w != e.w || h != e.h || q != e.q) {   // header + tables depend on (w, h, quality) only
+  Opts o;
+  normalise(quality, e.params.data(), (int)e.params.size(), &o);   // bevk_jpeg_set_params checked the list
+  if (w != e.w || h != e.h || o != e.o) {   // header + tables depend on (w, h, options) only
     Tables t;
-    make_tables(q, &t);
-    make_header(w, h, q, e.header);
-    RET(e.d_header.ensure(kHeaderBytes));
+    make_tables(o, &t);
+    make_header(w, h, o, e.header);
+    RET(e.d_header.ensure(kMaxHeaderBytes));
     RET(e.d_tabs.ensure(sizeof(Tables)));
-    CU(cudaMemcpyAsync(e.d_header.p, e.header, kHeaderBytes, cudaMemcpyHostToDevice, c->stream));   // pageable: staged
+    CU(cudaMemcpyAsync(e.d_header.p, e.header, kMaxHeaderBytes, cudaMemcpyHostToDevice, c->stream));   // pageable: staged
     CU(cudaMemcpyAsync(e.d_tabs.p, &t, sizeof t, cudaMemcpyHostToDevice, c->stream));               // before returning
-    e.w = w; e.h = h; e.q = q;
+    e.w = w; e.h = h; e.o = o;
   }
-  const Geom g = geom(w, h);
+  const Geom g = geom(w, h, o);
   const long long nblk = blocks_per_image(g), nb = nblk * n;
-  const long long words_img = ((long long)((entropy_bound_bits(w, h) + 31) / 32) + 3) & ~3ll;   // 16-byte aligned regions
+  const long long nint = intervals(g, o), ni = nint * n;
+  const long long words_img = ((long long)((entropy_bound_bits(g, o) + 31) / 32) + 3) & ~3ll;   // 16-byte aligned regions
   const int chunks = (int)((words_img * 4 + kChunk - 1) / kChunk);
   const long long nch = (long long)n * chunks;
-  if (nb > INT_MAX || nch > INT_MAX) return fail(BEVK_ERR_ARG, "batch of %d %dx%d images is too large for one call", n, w, h);
+  if (nb > INT_MAX || nch > INT_MAX || ni > INT_MAX) return fail(BEVK_ERR_ARG, "batch of %d %dx%d images is too large for one call", n, w, h);
   RET(e.coef.ensure((size_t)nb * 128));
   RET(e.bits.ensure((size_t)nb * 8));
   RET(e.offs.ensure((size_t)nb * 8));
@@ -2356,7 +2393,17 @@ static int jpeg_enqueue(bevk_ctx* c, int s, const JpegIn& in, int n, int w, int 
   RET(e.ffcnt.ensure((size_t)nch * 4));
   if (e.ffcnt.cap != ffcap) CU(cudaMemsetAsync(e.ffcnt.p, 0, e.ffcnt.cap, c->stream));
   RET(e.ffscan.ensure((size_t)nch * 4));
-  RET(e.out[s].ensure((size_t)n * encode_bound(w, h)));
+  RET(e.out[s].ensure((size_t)n * encode_bound(g, o)));
+  if (o.rst) {
+    RET(e.ilen.ensure((size_t)ni * 8));
+    RET(e.iofs.ensure((size_t)ni * 8));
+  }
+  if (o.optimize) {
+    RET(e.counts.ensure((size_t)n * 1024 * 8));
+    RET(e.huff.ensure((size_t)n * sizeof(Huff)));
+    RET(e.hdrs.ensure((size_t)n * kMaxHeaderBytes));
+    RET(e.hlen.ensure((size_t)n * 4));
+  }
   RET(e.meta[s].ensure((size_t)n * 16));
   if (e.h_sizes_cap[s] < (size_t)n) {
     if (e.h_sizes[s]) CU(cudaFreeHost(e.h_sizes[s]));      // jpeg_collect waited for its last copy
@@ -2367,7 +2414,9 @@ static int jpeg_enqueue(bevk_ctx* c, int s, const JpegIn& in, int n, int w, int 
   size_t tmp1 = 0, tmp2 = 0;
   CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp1, e.bits.as<unsigned long long>(), e.offs.as<unsigned long long>(), (int)nb));
   CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp2, e.ffcnt.as<unsigned>(), e.ffscan.as<unsigned>(), (int)nch));
-  const size_t tmp = std::max(tmp1, tmp2);
+  size_t tmp3 = 0;
+  if (o.rst) CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp3, e.ilen.as<unsigned long long>(), e.iofs.as<unsigned long long>(), (int)ni));
+  const size_t tmp = std::max(std::max(tmp1, tmp2), tmp3);
   RET(e.scan_tmp.ensure(tmp));
 
   EncArgs a{};
@@ -2377,24 +2426,50 @@ static int jpeg_enqueue(bevk_ctx* c, int s, const JpegIn& in, int n, int w, int 
   a.chunks_img = chunks; a.ffcnt = e.ffcnt.as<unsigned>(); a.ffscan = e.ffscan.as<unsigned>(); a.header = e.d_header.as<uint8_t>();
   a.out = e.out[s].as<uint8_t>(); a.out_off = e.meta[s].as<unsigned long long>(); a.sizes = e.meta[s].as<unsigned long long>() + n;
   a.csum = in.csum; a.npix = (double)w * (double)h; a.car = in.car;
+  a.rst = o.rst; a.nint = nint; a.hlen0 = header_bytes(o);
+  if (o.rst) { a.ilen = e.ilen.as<unsigned long long>(); a.iofs = e.iofs.as<unsigned long long>(); }
+  if (o.optimize) {
+    a.counts = e.counts.as<unsigned long long>(); a.huff = e.huff.as<Huff>(); a.hdrs = e.hdrs.as<uint8_t>(); a.hlen = e.hlen.as<int>();
+  }
   const unsigned gb = (unsigned)((nb + kBlockThreads - 1) / kBlockThreads), gc = (unsigned)((nch + 255) / 256);
   CU(cudaStreamWaitEvent(c->stream, e.ev_out_free[s], 0));   // the slot's previous streams have been copied out
   CU(cudaEventRecord(c->ev0, c->stream));
-  if (in.csum) {
-    const size_t gsmem = (size_t)gain_images_per_cta(nblk, n) * 768;
-    CU(cudaFuncSetAttribute(k_jpeg_blocks<GainSrc>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gsmem));
-    k_jpeg_blocks<GainSrc><<<gb, kBlockThreads, gsmem, c->stream>>>(a);
-  } else {
-    k_jpeg_blocks<PlainSrc><<<gb, kBlockThreads, 0, c->stream>>>(a);
-  }
-  LAUNCHED(c);
-  k_jpeg_dc<<<gb, kBlockThreads, 0, c->stream>>>(a);
-  LAUNCHED(c);
-  CU(cub::DeviceScan::ExclusiveSum(e.scan_tmp.p, tmp1, a.bits, a.offs, (int)nb, c->stream));
-  k_jpeg_zero<<<c->n_sm * 4, 256, 0, c->stream>>>(a);
-  LAUNCHED(c);
-  k_jpeg_pack<<<gb, kBlockThreads, 0, c->stream>>>(a);
-  LAUNCHED(c);
+  RET(with_sampling(o.hy, o.vy, [&](auto hy, auto vy) -> int {
+    constexpr int HY = hy(), VY = vy();
+    if (in.csum) {
+      const size_t gsmem = (size_t)gain_images_per_cta(nblk, n) * 768;
+      CU(cudaFuncSetAttribute(k_jpeg_blocks<GainSrc, HY, VY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gsmem));
+      k_jpeg_blocks<GainSrc, HY, VY><<<gb, kBlockThreads, gsmem, c->stream>>>(a);
+    } else {
+      k_jpeg_blocks<PlainSrc, HY, VY><<<gb, kBlockThreads, 0, c->stream>>>(a);
+    }
+    LAUNCHED(c);
+    k_jpeg_dc<HY, VY><<<gb, kBlockThreads, 0, c->stream>>>(a);
+    LAUNCHED(c);
+    if (o.optimize) {   // per-image tables from the symbol counts, then every block's bits under them
+      CU(cudaMemsetAsync(a.counts, 0, (size_t)n * 1024 * 8, c->stream));
+      k_jpeg_count<HY, VY><<<gb, kBlockThreads, 0, c->stream>>>(a);
+      LAUNCHED(c);
+      k_jpeg_huff<<<(unsigned)((4ll * n + kHuffThreads - 1) / kHuffThreads), kHuffThreads, 0, c->stream>>>(a);
+      LAUNCHED(c);
+      k_jpeg_bits<HY, VY><<<gb, kBlockThreads, 0, c->stream>>>(a);
+      LAUNCHED(c);
+    }
+    CU(cub::DeviceScan::ExclusiveSum(e.scan_tmp.p, tmp1, a.bits, a.offs, (int)nb, c->stream));
+    if (o.rst) {        // byte-aligned intervals: their padded lengths and offsets
+      k_jpeg_intervals<<<(unsigned)((ni + 255) / 256), 256, 0, c->stream>>>(a);
+      LAUNCHED(c);
+      CU(cub::DeviceScan::ExclusiveSum(e.scan_tmp.p, tmp3, a.ilen, a.iofs, (int)ni, c->stream));
+    }
+    k_jpeg_zero<<<c->n_sm * 4, 256, 0, c->stream>>>(a);
+    LAUNCHED(c);
+    if (o.optimize && o.rst) k_jpeg_pack<HY, VY, true, true><<<gb, kBlockThreads, 0, c->stream>>>(a);
+    else if (o.optimize) k_jpeg_pack<HY, VY, true, false><<<gb, kBlockThreads, 0, c->stream>>>(a);
+    else if (o.rst) k_jpeg_pack<HY, VY, false, true><<<gb, kBlockThreads, 0, c->stream>>>(a);
+    else k_jpeg_pack<HY, VY, false, false><<<gb, kBlockThreads, 0, c->stream>>>(a);
+    LAUNCHED(c);
+    return BEVK_OK;
+  }));
   k_jpeg_ffcount<<<gc, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
   CU(cub::DeviceScan::ExclusiveSum(e.scan_tmp.p, tmp2, a.ffcnt, a.ffscan, (int)nch, c->stream));

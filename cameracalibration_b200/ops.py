@@ -117,10 +117,28 @@ def jpeg_decode(jpegs, width: int, height: int, out=None, ctx: L.Context | None 
     return out
 
 
-def jpeg_encode_bound(width: int, height: int) -> int:
-    """Largest JPEG stream bevk_jpeg_encode can produce for a width x height image."""
+def _jpeg_params(params):
+    """(ctypes int array, n) of a cv2.imwrite JPEG parameter list without the IMWRITE_JPEG_QUALITY pair; None is []."""
+    p = [] if params is None else [int(v) for v in params]
+    return (C.c_int * max(len(p), 1))(*p), len(p)
+
+
+def jpeg_set_params(ctx: L.Context, params=None):
+    """Apply cv2.imwrite's JPEG (key, value) pairs (keys 2..7, cv2.IMWRITE_JPEG_*) to ctx's encoding calls; None or []
+    restores cv2's defaults.  The wrappers below call it on every call, so no call inherits another's params."""
+    arr, n = _jpeg_params(params)
+    L.check(ctx.lib.bevk_jpeg_set_params(ctx.h, arr, n))
+
+
+def jpeg_encode_bound(width: int, height: int, params=None) -> int:
+    """Largest JPEG stream bevk_jpeg_encode can produce for a width x height image under params (cv2.imwrite's JPEG
+    pairs without IMWRITE_JPEG_QUALITY; None: cv2's defaults)."""
     n = C.c_uint64()
-    L.check(L.load().bevk_jpeg_encode_bound(int(width), int(height), C.byref(n)))
+    if params is None:
+        L.check(L.load().bevk_jpeg_encode_bound(int(width), int(height), C.byref(n)))
+    else:
+        arr, k = _jpeg_params(params)
+        L.check(L.load().bevk_jpeg_encode_bound_params(int(width), int(height), arr, k, C.byref(n)))
     return n.value
 
 
@@ -180,11 +198,14 @@ def _cuda_images(arr, what):
     return int(ptr), rank, n, h, w, ch, img, row
 
 
-def jpeg_encode(images, quality: int = 95, ctx: L.Context | None = None) -> list[bytes]:
-    """cv2.imencode('.jpg', img, [cv2.IMWRITE_JPEG_QUALITY, quality]) on the GPU, byte for byte, for one uint8[H][W][3]
-    BGR image or a batch uint8[N][H][W][3].  CUDA arrays (``__cuda_array_interface__``, e.g. the torch canvases of
-    BevEngine.run_cuda) are read in place, on torch's current stream; NumPy input is uploaded once.  Returns one
-    ``bytes`` per image -- what cv2.imwrite would write to a .jpg file."""
+def jpeg_encode(images, quality: int = 95, ctx: L.Context | None = None, params=None) -> list[bytes]:
+    """cv2.imencode('.jpg', img, [cv2.IMWRITE_JPEG_QUALITY, quality] + params) on the GPU, byte for byte, for one
+    uint8[H][W][3] BGR image or a batch uint8[N][H][W][3].  params: cv2.imwrite's other JPEG pairs
+    (IMWRITE_JPEG_SAMPLING_FACTOR, _LUMA_QUALITY, _CHROMA_QUALITY, _OPTIMIZE, _RST_INTERVAL; see bevk_jpeg_set_params),
+    None for cv2's defaults.
+    CUDA arrays (``__cuda_array_interface__``, e.g. the torch canvases of BevEngine.run_cuda) are read in place, on
+    torch's current stream; NumPy input is uploaded once.  Returns one ``bytes`` per image -- what cv2.imwrite would
+    write to a .jpg file."""
     ctx = ctx or L.default_context()
     from .sharding import _torch_current_stream
     keep = images
@@ -197,9 +218,10 @@ def jpeg_encode(images, quality: int = 95, ctx: L.Context | None = None) -> list
     ptr, n, h, w, img_stride, row_stride = _cuda_bgr_batch(keep)
     if n < 1:
         return []
-    cap = n * jpeg_encode_bound(w, h)
+    cap = n * jpeg_encode_bound(w, h, params)
     out = np.empty(cap, np.uint8)          # pages are only touched where streams land
     sizes = (C.c_uint64 * n)()
+    jpeg_set_params(ctx, params)
     with ctx.on_stream(_torch_current_stream(ctx.device)):
         L.check(ctx.lib.bevk_jpeg_encode(ctx.h, C.c_void_p(ptr), img_stride, row_stride, n, w, h, int(quality), L.vptr(out),
                                          cap, sizes))
@@ -361,15 +383,18 @@ class Undistorter:
                                             self.w * ch, _interp(interpolation)))
         return out
 
-    def jpeg(self, src: np.ndarray, quality: int = 95, interpolation: int = INTER_LINEAR) -> bytes:
-        """The undistorted image as the bytes cv2.imwrite(path, self(src), [IMWRITE_JPEG_QUALITY, quality]) writes to a .jpg
-        file; the image itself never leaves the GPU.  src: uint8[h][w][3] BGR."""
+    def jpeg(self, src: np.ndarray, quality: int = 95, interpolation: int = INTER_LINEAR, params=None) -> bytes:
+        """The undistorted image as the bytes cv2.imwrite(path, self(src), [IMWRITE_JPEG_QUALITY, quality] + params)
+        writes to a .jpg file; the image itself never leaves the GPU.  src: uint8[h][w][3] BGR.  params: cv2.imwrite's
+        other JPEG pairs (see jpeg_encode), None for cv2's defaults."""
         self._live()
         img, sw, sh, ss, ch = L.image_view(src)
         if ch != 3 or src.ndim != 3:
             raise L.BevkError("Undistorter.jpeg takes uint8[h][w][3] BGR images")
-        if getattr(self, "_jpeg_buf", None) is None:
-            self._jpeg_buf = np.empty(jpeg_encode_bound(self.w, self.h), np.uint8)
+        bound = jpeg_encode_bound(self.w, self.h, params)
+        if getattr(self, "_jpeg_buf", None) is None or self._jpeg_buf.size < bound:
+            self._jpeg_buf = np.empty(bound, np.uint8)
+        jpeg_set_params(self.ctx, params)
         size = C.c_uint64()
         L.check(self.ctx.lib.bevk_undistort_jpeg(self.ctx.h, self.slot, L.vptr(img), sw, sh, ss, _interp(interpolation),
                                                  int(quality), L.vptr(self._jpeg_buf), self._jpeg_buf.size, C.byref(size)))
@@ -400,17 +425,18 @@ class Undistorter:
                                                       C.c_void_p(optr), oimg, self.w, self.h, orow, _interp(interpolation)))
         return out
 
-    def cuda_to_jpeg(self, frames, quality: int = 95, interpolation: int = INTER_LINEAR) -> list[bytes]:
-        """cuda() followed by cv2.imencode('.jpg', img, [IMWRITE_JPEG_QUALITY, quality]) per frame, with the encoder on
-        the GPU: the undistorted images stay in library scratch and only the JPEG streams come back.  frames: a uint8
-        CUDA array [H][W][3] or [N][H][W][3] (BGR) laid out as cuda() takes it.  Runs on torch's current stream and
-        synchronises.  Returns one ``bytes`` per frame, byte-identical to cv2's."""
+    def cuda_to_jpeg(self, frames, quality: int = 95, interpolation: int = INTER_LINEAR, params=None) -> list[bytes]:
+        """cuda() followed by cv2.imencode('.jpg', img, [IMWRITE_JPEG_QUALITY, quality] + params) per frame, with the
+        encoder on the GPU: the undistorted images stay in library scratch and only the JPEG streams come back.  frames:
+        a uint8 CUDA array [H][W][3] or [N][H][W][3] (BGR) laid out as cuda() takes it.  params as in jpeg().  Runs on
+        torch's current stream and synchronises.  Returns one ``bytes`` per frame, byte-identical to cv2's."""
         self._live()
         ptr, rank, n, sh, sw, ch, simg, srow = _cuda_images(frames, "frames")
         if ch != 3 or rank == 2:
             raise L.BevkError("Undistorter.cuda_to_jpeg takes uint8[H][W][3] or uint8[N][H][W][3] BGR frames")
-        out = np.empty(max(n, 1) * jpeg_encode_bound(self.w, self.h), np.uint8)   # pages are only touched where streams land
+        out = np.empty(max(n, 1) * jpeg_encode_bound(self.w, self.h, params), np.uint8)   # pages are only touched where streams land
         sizes = (C.c_uint64 * max(n, 1))()
+        jpeg_set_params(self.ctx, params)
         from .sharding import _torch_current_stream
         with self.ctx.on_stream(_torch_current_stream(self.ctx.device)):
             L.check(self.ctx.lib.bevk_undistort_stack_jpeg(self.ctx.h, self.slot, C.c_void_p(ptr), simg, sw, sh, srow, n,
@@ -593,9 +619,11 @@ class BevEngine:
             raise L.BevkError("car must be uint8[bev_h][bev_w][3]")
         return car, L.vptr(car)
 
-    def _streams(self, batch):
-        """Host buffer for `batch` JPEG streams of a canvas (pages are only touched where streams land) and sizes[batch]."""
-        out = np.empty(batch * jpeg_encode_bound(self.BW, self.BH), np.uint8)
+    def _streams(self, batch, params=None):
+        """Host buffer for `batch` JPEG streams of a canvas under params (pages are only touched where streams land) and
+        sizes[batch]; params are set on the context for the encoding call that follows."""
+        out = np.empty(batch * jpeg_encode_bound(self.BW, self.BH, params), np.uint8)
+        jpeg_set_params(self.ctx, params)
         return out, (C.c_uint64 * batch)()
 
     @staticmethod
@@ -606,15 +634,16 @@ class BevEngine:
             off += s
         return res
 
-    def run_to_jpeg(self, frame_sets, quality: int = 95, car: np.ndarray | None = None, balance: bool = False) -> list[bytes]:
-        """run() followed by cv2.imencode('.jpg', canvas, [IMWRITE_JPEG_QUALITY, quality]) per frame-set, with the
-        encoder on the GPU: only the JPEG streams come back over PCIe.  frame_sets as in run().  Returns one ``bytes``
-        per frame-set, byte-identical to cv2's."""
+    def run_to_jpeg(self, frame_sets, quality: int = 95, car: np.ndarray | None = None, balance: bool = False,
+                    params=None) -> list[bytes]:
+        """run() followed by cv2.imencode('.jpg', canvas, [IMWRITE_JPEG_QUALITY, quality] + params) per frame-set, with
+        the encoder on the GPU: only the JPEG streams come back over PCIe.  frame_sets as in run(); params as in
+        ops.jpeg_encode.  Returns one ``bytes`` per frame-set, byte-identical to cv2's."""
         if not self.finalized:
             self.finalize()
         keep, ptrs, stride, batch = self._host_frames(frame_sets, "run_to_jpeg()")
         car, carp = self._host_car(car)
-        out, sizes = self._streams(batch)
+        out, sizes = self._streams(batch, params)
         L.check(self.ctx.lib.bevk_bev_run_to_jpeg(self.ctx.h, ptrs, stride, batch, carp, L.FLAG_BALANCE if balance else 0,
                                                   int(quality), L.vptr(out), out.size, sizes))
         return self._split(out, sizes)
@@ -897,16 +926,17 @@ class BevEngine:
             pitch.append(strides[2])
         return planes, pitch
 
-    def cuda_to_jpeg(self, frames, quality: int = 95, car=None, balance: bool = False) -> list[bytes]:
-        """run_cuda() followed by cv2.imencode('.jpg', canvas, [IMWRITE_JPEG_QUALITY, quality]) per frame-set: frames
-        (and car) as run_cuda takes them; the canvases stay in library scratch on the GPU and only the JPEG streams come
-        back.  Runs on torch's current stream and synchronises.  Returns one ``bytes`` per frame-set."""
+    def cuda_to_jpeg(self, frames, quality: int = 95, car=None, balance: bool = False, params=None) -> list[bytes]:
+        """run_cuda() followed by cv2.imencode('.jpg', canvas, [IMWRITE_JPEG_QUALITY, quality] + params) per frame-set:
+        frames (and car) as run_cuda takes them; params as in ops.jpeg_encode.  The canvases stay in library scratch on
+        the GPU and only the JPEG streams come back.  Runs on torch's current stream and synchronises.  Returns one
+        ``bytes`` per frame-set."""
         if not self.finalized:
             self.finalize()
         ptrs = self._cuda_frames(frames)
         batch = len(ptrs) // self.n_cam
         d_car = _cuda_ptr(car, (self.BH, self.BW, 3))[0] if car is not None else None
-        out, sizes = self._streams(batch)
+        out, sizes = self._streams(batch, params)
         from .sharding import _torch_current_stream
         table = (C.c_void_p * len(ptrs))(*ptrs)
         with self.ctx.on_stream(_torch_current_stream(self.ctx.device)):

@@ -332,10 +332,28 @@ int bevk_bev_run_jpeg(bevk_ctx *ctx, const uint8_t *const *jpegs, const uint64_t
 
 /* ---- JPEG encode on the device ------------------------------------------------------------------------------------
  * Replaces cv2.imwrite(path, img, [IMWRITE_JPEG_QUALITY, q]) at the end of the path (Tools/undistort.py:72-73,
- * surroundBEV.py:340): the streams are byte-identical to cv2's (libjpeg-turbo baseline: 4:2:0, islow DCT, Annex K
- * Huffman tables, JFIF 1.01 header, no restart markers), and only the compressed bytes cross PCIe.
- * bevk_jpeg_encode_bound: the largest stream a width x height image can produce (sizes the caller's buffer).          */
+ * surroundBEV.py:340): the streams are byte-identical to cv2's (libjpeg-turbo baseline: islow DCT, JFIF 1.01 header;
+ * by default 4:2:0, Annex K Huffman tables and no restart markers, otherwise as bevk_jpeg_set_params says), and only
+ * the compressed bytes cross PCIe.
+ * bevk_jpeg_encode_bound: the largest stream a width x height image can produce (sizes the caller's buffer) with no
+ * params set.  4:4:4, optimised and restart-marker streams can be larger: size buffers for params with
+ * bevk_jpeg_encode_bound_params.                                                                                     */
 int bevk_jpeg_encode_bound(int width, int height, uint64_t *bytes);
+/* cv2.imwrite's JPEG (key, value) pairs, n ints (n even), applied to every encoding call of this ctx (bevk_jpeg_encode,
+ * bevk_undistort_jpeg, bevk_undistort_stack_jpeg, bevk_bev_run_to_jpeg, bevk_bev_frames_to_jpeg) until the next call;
+ * n == 0 restores cv2's defaults.  Keys 2..7 as cv2.IMWRITE_JPEG_*, values normalised as cv2 does:
+ *   SAMPLING_FACTOR (7)  0x111111 4:4:4, 0x211111 4:2:2, 0x121111 4:4:0, 0x221111 4:2:0, 0x411111 4:1:1; else 4:2:0
+ *   LUMA_QUALITY (5)     >= 0: min(v, 100) replaces the call's quality (both tables unless CHROMA_QUALITY is given)
+ *   CHROMA_QUALITY (6)   >= 0 and LUMA_QUALITY given: the chroma table's quality; luma != chroma forces 4:4:4
+ *   OPTIMIZE (3)         != 0: per-image Huffman tables (libjpeg's jpeg_gen_optimal_table), built on the device
+ *   RST_INTERVAL (4)     clamped to [0, 65535] MCUs; > 0 writes DRI and an RSTn marker after every interval but the last
+ *   PROGRESSIVE (2)      0 as cv2's default; anything else is BEVK_ERR_UNSUPPORTED (a multi-scan coder)
+ * QUALITY (1) is refused (every encoding call takes quality itself), as are other keys and odd n (BEVK_ERR_ARG).  A
+ * refused list leaves the ctx's params as they were.  The streams are byte-identical to
+ * cv2.imencode('.jpg', img, [IMWRITE_JPEG_QUALITY, quality] + params).                                               */
+int bevk_jpeg_set_params(bevk_ctx *ctx, const int *params, int n);
+/* bevk_jpeg_encode_bound for streams made under `params` (same list and rules).                                       */
+int bevk_jpeg_encode_bound_params(int width, int height, const int *params, int n, uint64_t *bytes);
 /* n DEVICE images, 3-channel BGR, image i at d_images + i * image_stride, rows row_stride bytes apart (any pitch >= 3 *
  * width).  quality is clamped as cv2 does (to [0, 100]; 0 acts as 1; cv2's default is 95).  The streams are written
  * back to back into HOST memory at out, their sizes to sizes[n]; the call synchronises.  When they need more than
