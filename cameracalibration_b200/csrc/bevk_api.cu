@@ -25,8 +25,11 @@
 #include "bevk_plan_tma.cuh"
 #include "bevk_shard.cuh"
 #include "bevk_jpeg_enc.cuh"
+#include "bevk_png_enc.cuh"
 
 #include <cub/device/device_scan.cuh>
+#include <cub/iterator/counting_input_iterator.cuh>
+#include <cub/iterator/transform_input_iterator.cuh>
 
 #include <dlfcn.h>
 #include <nvtx3/nvToolsExt.h>   // header-only: ranges cost nothing unless a profiler injects itself
@@ -233,6 +236,12 @@ struct bevk_ctx {
     cudaStream_t out_stream = nullptr;                      // D2H of the streams
     cudaEvent_t ev_sizes[2] = {nullptr, nullptr}, ev_out_free[2] = {nullptr, nullptr};
   } enc;
+  // PNG encoder (bevk_png_encode): the cv2.imwrite parameters of bevk_png_set_params and the work buffers of one group
+  // of images (bevk_png_enc.cuh); every group's streams land compacted in `out`.
+  struct PngEnc {
+    std::vector<int> params;
+    DevBuf f, rowad, runs, symidx, syms, nsym, blk, codes, hdr, zw, zbytes, meta, out, scan_tmp;
+  } png;
   // CUDA graphs captured from the device-pointer entry points (bevk_graph_*)
   bool capturing = false;
   long long capture_launches0 = 0;
@@ -2674,6 +2683,141 @@ int bevk_undistort_stack_jpeg(bevk_ctx* c, int slot, const void* d_src, int64_t 
   });
 }
 
+// ------------------------------------------------------------------ PNG encode on the device (bevk_png_enc.cuh)
+// cv2.imwrite('x.png', img) writes through libpng + zlib on a host core.  Under cv2's default settings (SUB, level 1,
+// Z_RLE) and Z_HUFFMAN_ONLY zlib's parse has no history, so the device reproduces the stream byte for byte in parallel.
+static int png_params_check(const int* params, int n, png::Opts* o) {
+  const int r = png::normalise(params, n, o);
+  if (r == 1)
+    return fail(BEVK_ERR_ARG, "PNG params: %d ints; need (key, value) pairs with keys 16..20 (cv2.IMWRITE_PNG_*)", n);
+  if (r == 2)
+    return fail(BEVK_ERR_UNSUPPORTED, "PNG params: the device encoder writes zlib levels 1..9 under IMWRITE_PNG_STRATEGY_RLE "
+                "or _HUFFMAN_ONLY only (a compression level without a later strategy is zlib's hash-chain LZ77; level 0, "
+                "BILEVEL and ZLIBBUFFER_SIZE are refused too)");
+  return BEVK_OK;
+}
+
+static int png_size_check(int width, int height) {
+  if (width < 1 || height < 1 || png::image_bytes(width, height) > png::kMaxImageBytes)
+    return fail(BEVK_ERR_ARG, "bad PNG size %dx%d (at least 1x1, at most %lld filtered bytes)", width, height,
+                png::kMaxImageBytes);
+  return BEVK_OK;
+}
+
+int bevk_png_set_params(bevk_ctx* c, const int* params, int n) {
+  RET(use(c));
+  png::Opts o;
+  RET(png_params_check(params, n, &o));
+  c->png.params.assign(params, params + n);
+  return BEVK_OK;
+}
+
+int bevk_png_encode_bound(int width, int height, const int* params, int n, uint64_t* bytes) {
+  if (!bytes) return fail(BEVK_ERR_ARG, "null bytes");
+  RET(png_size_check(width, height));
+  png::Opts o;
+  RET(png_params_check(params, n, &o));
+  *bytes = (uint64_t)png::encode_bound(width, height);
+  return BEVK_OK;
+}
+
+// Filtered bytes per group: the group's scans, symbols and run starts take 11 bytes per filtered byte of scratch.
+constexpr long long kPngGroupBytes = 1ll << 27;
+
+int bevk_png_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, int64_t row_stride, int n, int width, int height,
+                    uint8_t* out, uint64_t capacity, uint64_t* sizes) {
+  NvtxRange nvtx_call("bevk_png_encode (device images -> host PNG streams)");
+  using namespace png;
+  RET(use(c));
+  if (!d_images || !out || !sizes || n < 1) return fail(BEVK_ERR_ARG, "bad argument");
+  if (c->capturing) return fail(BEVK_ERR_ARG, "bevk_png_encode synchronises and cannot be captured into a graph");
+  RET(png_size_check(width, height));
+  if (row_stride < (int64_t)width * 3) return fail(BEVK_ERR_ARG, "row stride %lld < %d bytes", (long long)row_stride, width * 3);
+  if (n > 1 && image_stride < (int64_t)(height - 1) * row_stride + width * 3)
+    return fail(BEVK_ERR_ARG, "image stride %lld is smaller than one image", (long long)image_stride);
+  auto& e = c->png;
+  Opts o;
+  normalise(e.params.data(), (int)e.params.size(), &o);   // bevk_png_set_params checked the list
+  const long long N = image_bytes(width, height), maxb = max_blocks(N), zb = zlib_bound(N);
+  const long long zwords = zb / 4 + 2, maxch = idat_chunks(zb), bound = encode_bound(width, height);
+  const int g = (int)std::max(1ll, std::min<long long>(n, kPngGroupBytes / N));
+  const long long gN = g * N;
+  RET(e.f.ensure((size_t)gN));
+  RET(e.rowad.ensure((size_t)g * height * sizeof(Adler)));
+  RET(e.syms.ensure((size_t)gN * 2));
+  RET(e.nsym.ensure((size_t)g * 4));
+  RET(e.blk.ensure((size_t)g * maxb * sizeof(Blk)));
+  RET(e.codes.ensure((size_t)g * maxb * (kLCodes + kDCodes) * 4));
+  RET(e.hdr.ensure((size_t)g * maxb * kHdrWords * 4));
+  RET(e.zw.ensure((size_t)g * zwords * 4));
+  RET(e.zbytes.ensure((size_t)g * 8));
+  RET(e.meta.ensure((size_t)(2ll * n + 1) * 8));   // sizes[n], offsets[n], running end
+  RET(e.out.ensure((size_t)(n * bound)));
+  using KeyIt = cub::TransformInputIterator<unsigned, RunStartKey, cub::CountingInputIterator<unsigned>>;
+  using FlagIt = cub::TransformInputIterator<unsigned, SymbolFlag, cub::CountingInputIterator<unsigned>>;
+  PngArgs a{};
+  a.istride = image_stride; a.pitch = row_stride; a.W = width; a.H = height; a.filters = o.filters; a.strategy = o.strategy;
+  a.N = N; a.maxb = maxb; a.zwords = zwords; a.maxchunks = maxch;
+  a.f = e.f.as<uint8_t>(); a.rowad = e.rowad.as<Adler>(); a.syms = e.syms.as<uint16_t>(); a.nsym = e.nsym.as<unsigned>();
+  a.blk = e.blk.as<Blk>(); a.codes = e.codes.as<uint32_t>(); a.hdr = e.hdr.as<uint32_t>(); a.zw = e.zw.as<uint32_t>();
+  a.zbytes = e.zbytes.as<unsigned long long>(); a.base = e.meta.as<unsigned long long>() + 2ll * n; a.out = e.out.as<uint8_t>();
+  size_t tmp1 = 0, tmp2 = 0;
+  if (o.strategy == kZRle) {   // run starts and symbol indices (Z_HUFFMAN_ONLY: every byte is a symbol at its position)
+    RET(e.runs.ensure((size_t)gN * 4));
+    RET(e.symidx.ensure((size_t)(gN + 1) * 4));
+    a.runs = e.runs.as<unsigned>(); a.symidx = e.symidx.as<unsigned>();
+    const cub::CountingInputIterator<unsigned> pos(0);
+    CU(cub::DeviceScan::InclusiveScan(nullptr, tmp1, KeyIt(pos, RunStartKey{a.f, N}), e.runs.as<unsigned>(), MaxOp(), (int)gN));
+    CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp2, FlagIt(pos, SymbolFlag{a, 0}), e.symidx.as<unsigned>(), (int)gN + 1));
+    RET(e.scan_tmp.ensure(std::max(tmp1, tmp2)));
+  }
+  CU(cudaMemsetAsync(a.base, 0, 8, c->stream));
+  CU(cudaEventRecord(c->ev0, c->stream));
+  for (int b0 = 0; b0 < n; b0 += g) {
+    const int gn = std::min(g, n - b0);
+    a.img = reinterpret_cast<const uint8_t*>(d_images) + b0 * image_stride;
+    a.n = gn;
+    a.sizes = e.meta.as<unsigned long long>() + b0;
+    a.out_off = e.meta.as<unsigned long long>() + n + b0;
+    const long long total = gn * N;
+    k_png_filter<<<(unsigned)(gn * height), kPngThreads, 0, c->stream>>>(a);
+    LAUNCHED(c);
+    if (o.strategy == kZRle) {
+      const cub::CountingInputIterator<unsigned> pos(0);
+      CU(cub::DeviceScan::InclusiveScan(e.scan_tmp.p, tmp1, KeyIt(pos, RunStartKey{a.f, N}), e.runs.as<unsigned>(), MaxOp(), (int)total,
+                                        c->stream));
+      CU(cub::DeviceScan::ExclusiveSum(e.scan_tmp.p, tmp2, FlagIt(pos, SymbolFlag{a, (unsigned)total}),
+                                       e.symidx.as<unsigned>(), (int)total + 1, c->stream));
+    }
+    k_png_setup<<<(unsigned)((gn + 127) / 128), 128, 0, c->stream>>>(a);
+    LAUNCHED(c);
+    k_png_compact<<<(unsigned)std::min<long long>((total + 255) / 256, (long long)c->n_sm * 16), 256, 0, c->stream>>>(a);
+    LAUNCHED(c);
+    k_png_tree<<<(unsigned)(gn * maxb), kPngThreads, 0, c->stream>>>(a);
+    LAUNCHED(c);
+    CU(cudaMemsetAsync(a.zw, 0, (size_t)gn * zwords * 4, c->stream));
+    k_png_layout<<<(unsigned)((gn + 127) / 128), 128, 0, c->stream>>>(a);
+    LAUNCHED(c);
+    k_png_offsets<<<1, 1, 0, c->stream>>>(a);
+    LAUNCHED(c);
+    k_png_pack<<<(unsigned)(gn * maxb), kPngThreads, 0, c->stream>>>(a);
+    LAUNCHED(c);
+    k_png_frame<<<(unsigned)((gn * maxch * 32 + kPngThreads - 1) / kPngThreads), kPngThreads, 0, c->stream>>>(a);
+    LAUNCHED(c);
+  }
+  CU(cudaEventRecord(c->ev1, c->stream));
+  c->timed = true;
+  CU(cudaMemcpyAsync(sizes, e.meta.p, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  unsigned long long all = 0;
+  for (int i = 0; i < n; ++i) all += sizes[i];
+  if (all > capacity)
+    return fail(BEVK_ERR_ARG, "the %d PNG streams take %llu bytes, capacity is %llu", n, all, (unsigned long long)capacity);
+  CU(cudaMemcpyAsync(out, e.out.p, all, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  return BEVK_OK;
+}
+
 // ------------------------------------------------------------------ CUDA graphs
 // Stream capture of whatever the device-pointer entry points enqueue between begin and end; replayed with one call.
 int bevk_graph_begin(bevk_ctx* c) {
@@ -2732,7 +2876,7 @@ int64_t bevk_launch_count(bevk_ctx* c) { return c ? c->launches : 0; }
 int bevk_last_kernel_ms(bevk_ctx* c, float* ms) {
   RET(use(c));
   if (!ms) return fail(BEVK_ERR_ARG, "null ms");
-  if (!c->timed) return fail(BEVK_ERR_ARG, "no timed bevk_bev_run_device call yet");
+  if (!c->timed) return fail(BEVK_ERR_ARG, "no timed bevk_bev_run_device, bevk_jpeg_encode or bevk_png_encode call yet");
   CU(cudaEventSynchronize(c->ev1));
   CU(cudaEventElapsedTime(ms, c->ev0, c->ev1));
   return BEVK_OK;

@@ -232,6 +232,53 @@ def jpeg_encode(images, quality: int = 95, ctx: L.Context | None = None, params=
     return res
 
 
+def png_set_params(ctx: L.Context, params=None):
+    """Apply cv2.imwrite's PNG (key, value) pairs (keys 16..20, cv2.IMWRITE_PNG_*) to ctx's PNG encoding; None or []
+    restores cv2's defaults.  png_encode calls it on every call, so no call inherits another's params."""
+    arr, n = _jpeg_params(params)
+    L.check(ctx.lib.bevk_png_set_params(ctx.h, arr, n))
+
+
+def png_encode_bound(width: int, height: int, params=None) -> int:
+    """Largest PNG stream bevk_png_encode can produce for a width x height image under params (cv2.imwrite's PNG
+    pairs; None: cv2's defaults)."""
+    n = C.c_uint64()
+    arr, k = _jpeg_params(params)
+    L.check(L.load().bevk_png_encode_bound(int(width), int(height), arr, k, C.byref(n)))
+    return n.value
+
+
+def png_encode(images, ctx: L.Context | None = None, params=None) -> list[bytes]:
+    """cv2.imencode('.png', img, params) on the GPU, byte for byte, for one uint8[H][W][3] BGR image or a batch
+    uint8[N][H][W][3].  params: cv2.imwrite's PNG pairs with the RLE or HUFFMAN_ONLY strategy (see bevk_png_set_params;
+    a list that ends at zlib's default strategy raises BevkError), None for cv2's defaults.
+    CUDA arrays (``__cuda_array_interface__``) are read in place, on torch's current stream; NumPy input is uploaded
+    once.  Returns one ``bytes`` per image -- what cv2.imwrite would write to a .png file."""
+    ctx = ctx or L.default_context()
+    from .sharding import _torch_current_stream
+    keep = images
+    if not hasattr(images, "__cuda_array_interface__"):
+        a = np.asarray(images)
+        if a.dtype != np.uint8 or a.ndim not in (3, 4) or a.shape[-1] != 3:
+            raise L.BevkError(f"png_encode takes uint8[H][W][3] or uint8[N][H][W][3] BGR images, got {a.dtype} {a.shape}")
+        import torch
+        keep = torch.from_numpy(np.ascontiguousarray(a)).to(torch.device("cuda", ctx.device))
+    ptr, n, h, w, img_stride, row_stride = _cuda_bgr_batch(keep)
+    if n < 1:
+        return []
+    cap = n * png_encode_bound(w, h, params)
+    out = np.empty(cap, np.uint8)          # pages are only touched where streams land
+    sizes = (C.c_uint64 * n)()
+    png_set_params(ctx, params)
+    with ctx.on_stream(_torch_current_stream(ctx.device)):
+        L.check(ctx.lib.bevk_png_encode(ctx.h, C.c_void_p(ptr), img_stride, row_stride, n, w, h, L.vptr(out), cap, sizes))
+    res, off = [], 0
+    for s in sizes:
+        res.append(out[off:off + s].tobytes())
+        off += s
+    return res
+
+
 def remap(src: np.ndarray, map1: np.ndarray, map2: np.ndarray | None, interpolation: int = INTER_LINEAR,
           ctx: L.Context | None = None, out: np.ndarray | None = None) -> np.ndarray:
     """cv2.remap with CV_16SC2 (+CV_16UC1) maps, BORDER_CONSTANT 0."""

@@ -387,6 +387,32 @@ int bevk_bev_run_to_jpeg(bevk_ctx *ctx, const uint8_t *const *srcs, int64_t src_
 int bevk_bev_frames_to_jpeg(bevk_ctx *ctx, const void *const *frames, int batch, const void *d_car, int flags, int quality,
                             uint8_t *out, uint64_t capacity, uint64_t *sizes);
 
+/* ---- PNG encode on the device -------------------------------------------------------------------------------------
+ * Replaces cv2.imwrite('x.png', img, params) / cv2.imencode('.png', ...) for 8-bit 3-channel BGR images: the streams are
+ * byte-identical to cv2's (libpng 1.6 + zlib 1.2.11: colour type 2, IDAT chunks of 8192 bytes) and only the compressed
+ * bytes cross PCIe.  cv2's defaults (SUB filter, zlib level 1, Z_RLE) and IMWRITE_PNG_STRATEGY_RLE / _HUFFMAN_ONLY are
+ * reproduced; zlib's hash-chain strategies are not.
+ * bevk_png_set_params: cv2.imwrite's PNG (key, value) pairs, n ints (n even), applied to bevk_png_encode on this ctx
+ * until the next call; n == 0 restores cv2's defaults.  Keys 16..20 as cv2.IMWRITE_PNG_*, read in order as cv2 4.13 does:
+ *   COMPRESSION (16)     clamped to [0, 9]; resets the strategy to DEFAULT and switches to adaptive filtering over all
+ *                        five filters (libpng's heuristic); a STRATEGY after it sets the strategy again
+ *   STRATEGY (17)        RLE (3) or HUFFMAN_ONLY (2); values outside 0..4 act as RLE
+ *   FILTER (19)          NONE 8, SUB 16, UP 32, AVG 64, PAETH 128, FAST 56, ALL 248 (others act as SUB); overrides the
+ *                        filters the level implies
+ *   BILEVEL (18)         0 only
+ * A list that ends at level 0, at the DEFAULT / FILTERED / FIXED strategy, or with BILEVEL != 0 or ZLIBBUFFER_SIZE (20)
+ * is BEVK_ERR_UNSUPPORTED; other keys and odd n are BEVK_ERR_ARG.  A refused list leaves the ctx's params as they were.
+ * bevk_png_encode_bound: the largest stream a width x height image can produce under `params` (every block at most its
+ * filtered bytes + 5, plus zlib header and trailer, signature, IHDR, IDAT framing and IEND).
+ * bevk_png_encode: n DEVICE images, image i at d_images + i * image_stride, rows row_stride bytes apart (any pitch >=
+ * 3 * width; filtered size (3 * width + 1) * height below 2^31 - 2^16).  The streams are written back to back into HOST
+ * memory at out, their sizes to sizes[n]; the call synchronises.  When they need more than capacity bytes the call fails
+ * with BEVK_ERR_ARG, still fills sizes[], and writes nothing to out.                                                   */
+int bevk_png_set_params(bevk_ctx *ctx, const int *params, int n);
+int bevk_png_encode_bound(int width, int height, const int *params, int n, uint64_t *bytes);
+int bevk_png_encode(bevk_ctx *ctx, const void *d_images, int64_t image_stride, int64_t row_stride, int n, int width, int height,
+                    uint8_t *out, uint64_t capacity, uint64_t *sizes);
+
 /* ---- CUDA graphs over the device-pointer entry points ------------------------------------------------
  * Everything the "_device" / "_stack" / "_frames" entry points enqueue on the ctx stream between begin and end is
  * captured (stream capture) instead of executed, instantiated once, and replayed `times` times by one call --
@@ -404,7 +430,7 @@ int bevk_graph_launch(bevk_ctx *ctx, int graph_id, int times);
 int bevk_graph_destroy(bevk_ctx *ctx, int graph_id);
 /* Kernel launches issued by this ctx since creation (bench "gpu_launches"). */
 int64_t bevk_launch_count(bevk_ctx *ctx);
-/* Milliseconds spent in the last bevk_bev_run_device or bevk_jpeg_encode call's kernels, measured with
+/* Milliseconds spent in the last bevk_bev_run_device, bevk_jpeg_encode or bevk_png_encode call's kernels, measured with
  * CUDA events on the ctx stream (synchronises). */
 int bevk_last_kernel_ms(bevk_ctx *ctx, float *ms);
 
