@@ -2,8 +2,9 @@
 
 The undistortion map is built once on the device and never leaves it.  With ``-dstformat jpg`` (the
 default) each image costs one upload, one gather kernel and the device JPEG encoder, and only the
-compressed stream comes back -- the same bytes cv2.imwrite writes; other formats download the image and
-encode it with cv2 as the reference does.  Decoding the source files stays on the host with cv2.  The
+compressed stream comes back -- the same bytes cv2.imwrite writes; so does ``-dstformat png`` at
+``-quality`` 4 and above (zlib levels 4..9; the default 100 is level 9) through the device PNG encoder.
+Other formats, and PNG at levels 0..3, download the image and encode it with cv2 as the reference does.  Decoding the source files stays on the host with cv2.  The
 command line accepts the reference's flags with the same defaults; boolean flags additionally understand
 0/1/true/false (the reference's ``type=bool`` turns every non-empty string into True), and ``-fused 1``
 evaluates the camera model inside the gather kernel instead of keeping a map in HBM; ``-workers N`` sizes
@@ -83,7 +84,8 @@ def run_directory(opts, undistorter, cv2):
     """Decode -> undistort -> encode over a directory, overlapped: a thread pool decodes the next files
     and writes finished ones (cv2 releases the GIL in imread/imwrite) while the GPU call for the current
     image runs on the calling thread.  For ``-dstformat jpg`` that call is ``undistorter.jpeg`` -- undistort
-    and encode on the device, the pool only writes the bytes; other formats are encoded by cv2 in the pool.
+    and encode on the device, the pool only writes the bytes (likewise ``undistorter.png`` for PNG at levels 4..9);
+    other formats are encoded by cv2 in the pool.
     Files are processed and numbered in ``os.listdir`` order exactly as the reference's serial loop does
     (:59-77); at most ``2 * workers`` decoded images are held at a time."""
     from collections import deque
@@ -94,6 +96,7 @@ def run_directory(opts, undistorter, cv2):
     workers = max(1, int(opts.workers))
     written, encodes = [], deque()
     device_jpeg = opts.dstformat == "jpg"
+    device_png = opts.dstformat == "png" and opts.quality >= 4   # cv2 clamps the level to 9
     with ThreadPoolExecutor(max_workers=workers) as pool:
         decodes, upcoming = deque(), iter(entries)
 
@@ -111,14 +114,17 @@ def run_directory(opts, undistorter, cv2):
             top_up()
             if device_jpeg:
                 result = undistorter.jpeg(pending.result(), opts.quality)
+            elif device_png:
+                result = undistorter.png(pending.result(), [cv2.IMWRITE_PNG_COMPRESSION, opts.quality])
             else:
                 result = undistorter(pending.result())
             if opts.name is not None:
                 entry = "{}_{:04d}.{}".format(opts.name, counter, opts.srcformat)
                 counter += 1
             stem = entry[:-4]
-            if device_jpeg:
-                encodes.append(pool.submit(_write_bytes, os.path.join(opts.path_save, stem) + ".jpg", result))
+            if device_jpeg or device_png:
+                ext = ".jpg" if device_jpeg else ".png"
+                encodes.append(pool.submit(_write_bytes, os.path.join(opts.path_save, stem) + ext, result))
             else:
                 encodes.append(pool.submit(_save, cv2, opts, os.path.join(opts.path_save, stem), stem, result))
             while len(encodes) > 2 * workers:

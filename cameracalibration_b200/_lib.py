@@ -96,6 +96,8 @@ SIGNATURES = {
     "bevk_png_encode_bound": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_uint64)]),
     "bevk_png_encode": (C.c_int, [_p, _p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int, _p, C.c_uint64,
                                   C.POINTER(C.c_uint64)]),
+    "bevk_png_encode_params": (C.c_int, [_p, C.POINTER(C.c_int), C.c_int, _p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int,
+                                         _p, C.c_uint64, C.POINTER(C.c_uint64)]),
     "bevk_jpeg_encode": (C.c_int, [_p, _p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, _p, C.c_uint64,
                                    C.POINTER(C.c_uint64)]),
     "bevk_undistort_jpeg": (C.c_int, [_p, C.c_int, _p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, _p, C.c_uint64,

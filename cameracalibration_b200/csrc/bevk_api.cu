@@ -241,6 +241,7 @@ struct bevk_ctx {
   struct PngEnc {
     std::vector<int> params;
     DevBuf f, rowad, runs, symidx, syms, nsym, blk, codes, hdr, zw, zbytes, meta, out, scan_tmp;
+    DevBuf nblk, keys, keys2, pos, pos2, prev, recs, jump, jump2, mark, cnt, dists;   // nblk; the hash-chain parse
   } png;
   // CUDA graphs captured from the device-pointer entry points (bevk_graph_*)
   bool capturing = false;
@@ -2686,14 +2687,18 @@ int bevk_undistort_stack_jpeg(bevk_ctx* c, int slot, const void* d_src, int64_t 
 // ------------------------------------------------------------------ PNG encode on the device (bevk_png_enc.cuh)
 // cv2.imwrite('x.png', img) writes through libpng + zlib on a host core.  Under cv2's default settings (SUB, level 1,
 // Z_RLE) and Z_HUFFMAN_ONLY zlib's parse has no history, so the device reproduces the stream byte for byte in parallel.
-static int png_params_check(const int* params, int n, png::Opts* o) {
-  const int r = png::normalise(params, n, o);
+static int png_params_check(const int* params, int n, png::Opts* o, bool hash_chain = false) {
+  const int r = png::normalise(params, n, o, hash_chain);
   if (r == 1)
     return fail(BEVK_ERR_ARG, "PNG params: %d ints; need (key, value) pairs with keys 16..20 (cv2.IMWRITE_PNG_*)", n);
+  if (r == 2 && hash_chain)
+    return fail(BEVK_ERR_UNSUPPORTED, "PNG params: the device encoder writes zlib levels 1..9 under IMWRITE_PNG_STRATEGY_RLE "
+                "or _HUFFMAN_ONLY, and levels 4..9 under the other strategies (levels 1..3 there are zlib's deflate_fast; "
+                "level 0, BILEVEL and ZLIBBUFFER_SIZE are refused too)");
   if (r == 2)
     return fail(BEVK_ERR_UNSUPPORTED, "PNG params: the device encoder writes zlib levels 1..9 under IMWRITE_PNG_STRATEGY_RLE "
-                "or _HUFFMAN_ONLY only (a compression level without a later strategy is zlib's hash-chain LZ77; level 0, "
-                "BILEVEL and ZLIBBUFFER_SIZE are refused too)");
+                "or _HUFFMAN_ONLY only (a compression level without a later strategy is zlib's hash-chain LZ77, which "
+                "bevk_png_encode_params takes at levels 4..9; level 0, BILEVEL and ZLIBBUFFER_SIZE are refused too)");
   return BEVK_OK;
 }
 
@@ -2721,28 +2726,33 @@ int bevk_png_encode_bound(int width, int height, const int* params, int n, uint6
   return BEVK_OK;
 }
 
-// Filtered bytes per group: the group's scans, symbols and run starts take 11 bytes per filtered byte of scratch.
-constexpr long long kPngGroupBytes = 1ll << 27;
+// Filtered bytes per group: the group's scans, symbols and run starts take 11 bytes per filtered byte of scratch.  The
+// hash-chain parse takes about 50 (sort keys and positions twice, prev, two match records, two jump arrays, marks,
+// counts, symbols and distances, the sort's scratch), so its groups are a quarter of the size; a single image larger
+// than a group still runs as one group of one, so a hash-chain image needs about 50 B of device memory per filtered
+// byte.  Its hash sort keys are (image in group << 15) | hash, 32 bits with the sentinel (group size << 15) of the
+// last 2 bytes: at most 2^16 images per group.
+constexpr long long kPngGroupBytes = 1ll << 27, kPngLazyGroupBytes = 1ll << 25, kPngLazyGroupImages = 1ll << 16;
 
-int bevk_png_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, int64_t row_stride, int n, int width, int height,
-                    uint8_t* out, uint64_t capacity, uint64_t* sizes) {
-  NvtxRange nvtx_call("bevk_png_encode (device images -> host PNG streams)");
+static int png_encode_opts(bevk_ctx* c, const png::Opts& o, const void* d_images, int64_t image_stride, int64_t row_stride,
+                           int n, int width, int height, uint8_t* out, uint64_t capacity, uint64_t* sizes) {
   using namespace png;
   RET(use(c));
   if (!d_images || !out || !sizes || n < 1) return fail(BEVK_ERR_ARG, "bad argument");
-  if (c->capturing) return fail(BEVK_ERR_ARG, "bevk_png_encode synchronises and cannot be captured into a graph");
+  if (c->capturing) return fail(BEVK_ERR_ARG, "PNG encoding synchronises and cannot be captured into a graph");
   RET(png_size_check(width, height));
   if (row_stride < (int64_t)width * 3) return fail(BEVK_ERR_ARG, "row stride %lld < %d bytes", (long long)row_stride, width * 3);
   if (n > 1 && image_stride < (int64_t)(height - 1) * row_stride + width * 3)
     return fail(BEVK_ERR_ARG, "image stride %lld is smaller than one image", (long long)image_stride);
   auto& e = c->png;
-  Opts o;
-  normalise(e.params.data(), (int)e.params.size(), &o);   // bevk_png_set_params checked the list
+  const bool lazy = lazy_parse(o);
   const long long N = image_bytes(width, height), maxb = max_blocks(N), zb = zlib_bound(N);
   const long long zwords = zb / 4 + 2, maxch = idat_chunks(zb), bound = encode_bound(width, height);
-  const int g = (int)std::max(1ll, std::min<long long>(n, kPngGroupBytes / N));
+  const int g = (int)std::max(1ll, std::min({(long long)n, (lazy ? kPngLazyGroupBytes : kPngGroupBytes) / N,
+                                               lazy ? kPngLazyGroupImages : (long long)n}));
   const long long gN = g * N;
-  RET(e.f.ensure((size_t)gN));
+  RET(e.f.ensure((size_t)gN + 8));   // common_len's word loads read up to 3 bytes past the last image
+  RET(e.nblk.ensure((size_t)g * 4));
   RET(e.rowad.ensure((size_t)g * height * sizeof(Adler)));
   RET(e.syms.ensure((size_t)gN * 2));
   RET(e.nsym.ensure((size_t)g * 4));
@@ -2761,7 +2771,23 @@ int bevk_png_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, int
   a.f = e.f.as<uint8_t>(); a.rowad = e.rowad.as<Adler>(); a.syms = e.syms.as<uint16_t>(); a.nsym = e.nsym.as<unsigned>();
   a.blk = e.blk.as<Blk>(); a.codes = e.codes.as<uint32_t>(); a.hdr = e.hdr.as<uint32_t>(); a.zw = e.zw.as<uint32_t>();
   a.zbytes = e.zbytes.as<unsigned long long>(); a.base = e.meta.as<unsigned long long>() + 2ll * n; a.out = e.out.as<uint8_t>();
+  a.nblk = e.nblk.as<unsigned>(); a.level = o.level; a.flevel = zlib_flevel(o);
   size_t tmp1 = 0, tmp2 = 0;
+  int key_bits = 15;
+  while ((1ll << key_bits) <= ((long long)g << 15)) ++key_bits;
+  if (lazy) {   // hash sort, prev, match records, jumps, marks, chain symbol counts and their scan, distances
+    RET(e.keys.ensure((size_t)gN * 4)); RET(e.keys2.ensure((size_t)gN * 4));
+    RET(e.pos.ensure((size_t)gN * 4)); RET(e.pos2.ensure((size_t)gN * 4));
+    RET(e.prev.ensure((size_t)gN * 4)); RET(e.recs.ensure((size_t)gN * sizeof(MatchRec)));
+    RET(e.jump.ensure((size_t)gN * 4)); RET(e.jump2.ensure((size_t)gN * 4)); RET(e.mark.ensure((size_t)gN));
+    RET(e.cnt.ensure((size_t)(gN + 1) * 4)); RET(e.symidx.ensure((size_t)(gN + 1) * 4)); RET(e.dists.ensure((size_t)gN * 2));
+    a.prev = e.prev.as<unsigned>(); a.recs = e.recs.as<MatchRec>(); a.mark = e.mark.as<uint8_t>();
+    a.cnt = e.cnt.as<unsigned>(); a.symidx = e.symidx.as<unsigned>(); a.dists = e.dists.as<uint16_t>();
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, tmp1, e.keys.as<unsigned>(), e.keys2.as<unsigned>(), e.pos.as<unsigned>(),
+                                       e.pos2.as<unsigned>(), (int)gN, 0, key_bits));
+    CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp2, e.cnt.as<unsigned>(), e.symidx.as<unsigned>(), (int)gN + 1));
+    RET(e.scan_tmp.ensure(std::max(tmp1, tmp2)));
+  }
   if (o.strategy == kZRle) {   // run starts and symbol indices (Z_HUFFMAN_ONLY: every byte is a symbol at its position)
     RET(e.runs.ensure((size_t)gN * 4));
     RET(e.symidx.ensure((size_t)(gN + 1) * 4));
@@ -2780,8 +2806,33 @@ int bevk_png_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, int
     a.sizes = e.meta.as<unsigned long long>() + b0;
     a.out_off = e.meta.as<unsigned long long>() + n + b0;
     const long long total = gn * N;
+    const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, (long long)c->n_sm * 16);
     k_png_filter<<<(unsigned)(gn * height), kPngThreads, 0, c->stream>>>(a);
     LAUNCHED(c);
+    if (lazy) {
+      k_png_keys<<<grid, 256, 0, c->stream>>>(HashKey{a.f, N, (unsigned)gn}, e.keys.as<unsigned>(), e.pos.as<unsigned>(),
+                                              (unsigned)total);
+      LAUNCHED(c);
+      CU(cub::DeviceRadixSort::SortPairs(e.scan_tmp.p, tmp1, e.keys.as<unsigned>(), e.keys2.as<unsigned>(), e.pos.as<unsigned>(),
+                                         e.pos2.as<unsigned>(), (int)total, 0, key_bits, c->stream));
+      k_png_prev<<<grid, 256, 0, c->stream>>>(e.keys2.as<unsigned>(), e.pos2.as<unsigned>(), e.prev.as<unsigned>(),
+                                               (unsigned)total, N);
+      LAUNCHED(c);
+      k_png_match<<<(unsigned)((total + 127) / 128), 128, 0, c->stream>>>(a);
+      LAUNCHED(c);
+      a.jump = e.jump.as<unsigned>(); a.jump2 = e.jump2.as<unsigned>();
+      k_png_next<<<grid, 256, 0, c->stream>>>(a);
+      LAUNCHED(c);
+      for (long long len = 1; len < N; len *= 2) {   // a parse has at most N positions
+        k_png_jump<<<grid, 256, 0, c->stream>>>(a.jump, a.jump2, a.mark, (unsigned)total);
+        LAUNCHED(c);
+        std::swap(a.jump, a.jump2);
+      }
+      k_png_count<<<grid, 256, 0, c->stream>>>(a);
+      LAUNCHED(c);
+      CU(cub::DeviceScan::ExclusiveSum(e.scan_tmp.p, tmp2, e.cnt.as<unsigned>(), e.symidx.as<unsigned>(), (int)total + 1,
+                                       c->stream));
+    }
     if (o.strategy == kZRle) {
       const cub::CountingInputIterator<unsigned> pos(0);
       CU(cub::DeviceScan::InclusiveScan(e.scan_tmp.p, tmp1, KeyIt(pos, RunStartKey{a.f, N}), e.runs.as<unsigned>(), MaxOp(), (int)total,
@@ -2791,7 +2842,8 @@ int bevk_png_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, int
     }
     k_png_setup<<<(unsigned)((gn + 127) / 128), 128, 0, c->stream>>>(a);
     LAUNCHED(c);
-    k_png_compact<<<(unsigned)std::min<long long>((total + 255) / 256, (long long)c->n_sm * 16), 256, 0, c->stream>>>(a);
+    if (lazy) k_png_lazy_compact<<<grid, 256, 0, c->stream>>>(a);
+    else k_png_compact<<<grid, 256, 0, c->stream>>>(a);
     LAUNCHED(c);
     k_png_tree<<<(unsigned)(gn * maxb), kPngThreads, 0, c->stream>>>(a);
     LAUNCHED(c);
@@ -2816,6 +2868,27 @@ int bevk_png_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, int
   CU(cudaMemcpyAsync(out, e.out.p, all, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaStreamSynchronize(c->stream));
   return BEVK_OK;
+}
+
+int bevk_png_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, int64_t row_stride, int n, int width, int height,
+                    uint8_t* out, uint64_t capacity, uint64_t* sizes) {
+  NvtxRange nvtx_call("bevk_png_encode (device images -> host PNG streams)");
+  RET(use(c));
+  png::Opts o;
+  png::normalise(c->png.params.data(), (int)c->png.params.size(), &o);   // bevk_png_set_params checked the list
+  return png_encode_opts(c, o, d_images, image_stride, row_stride, n, width, height, out, capacity, sizes);
+}
+
+// The parameter list per call, as cv2.imencode takes it; also zlib's hash-chain parse at levels 4..9 (deflate_slow,
+// bevk_png_enc.cuh).  The ctx's bevk_png_set_params list is neither read nor changed.
+int bevk_png_encode_params(bevk_ctx* c, const int* params, int n_params, const void* d_images, int64_t image_stride,
+                           int64_t row_stride, int n, int width, int height, uint8_t* out, uint64_t capacity,
+                           uint64_t* sizes) {
+  NvtxRange nvtx_call("bevk_png_encode_params (device images -> host PNG streams)");
+  RET(use(c));
+  png::Opts o;
+  RET(png_params_check(params, n_params, &o, true));
+  return png_encode_opts(c, o, d_images, image_stride, row_stride, n, width, height, out, capacity, sizes);
 }
 
 // ------------------------------------------------------------------ CUDA graphs

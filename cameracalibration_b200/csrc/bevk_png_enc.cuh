@@ -1,5 +1,6 @@
 // bevk_png_enc.cuh -- PNG encoder on the device (sm_90a), byte-identical to cv2.imwrite / cv2.imencode('.png') for
-// 8-bit BGR images under cv2's default settings and its Z_RLE / Z_HUFFMAN_ONLY strategies.
+// 8-bit BGR images under cv2's default settings and its Z_RLE / Z_HUFFMAN_ONLY strategies, and under zlib's hash-chain
+// parse at levels 4..9 (deflate_slow; the "parse (deflate_slow ...)" section and DESIGN.md section 2).
 //
 // cv2 writes PNG through libpng 1.6 and zlib 1.2.11.  With no parameters it asks for the SUB filter on every row,
 // zlib level 1 and strategy Z_RLE; IMWRITE_PNG_STRATEGY_HUFFMAN_ONLY asks for literals only.  Under those two strategies
@@ -31,6 +32,10 @@
 //   k_png_setup    symbols, blocks and block ranges per image
 //   k_png_compact  one thread per position: the symbol (u16: < 256 literal, 256 + len - 3 match) at its index, and the
 //                  raw start of every block
+//   (levels 4..9 instead of the two scans and k_png_compact: k_png_keys + a CUB radix sort by (image, hash) and
+//    k_png_prev -- each position's chain predecessor; k_png_match -- lazy_match per position; k_png_next -- every
+//    position's next canonical position; k_png_jump -- pointer doubling marking each image's parse; k_png_count + a CUB
+//    scan -- symbol indices; k_png_lazy_compact -- symbols, distances and block raw starts)
 //   k_png_tree     one CTA per block: histograms, then one thread builds the trees and picks the block type
 //   k_png_layout   one thread per image: block bit offsets in order (stored blocks byte-aligned), stream sizes,
 //                  zlib header and Adler-32 trailer; k_png_offsets: compacted output offsets
@@ -44,6 +49,7 @@
 
 #include <cub/block/block_reduce.cuh>
 #include <cub/block/block_scan.cuh>
+#include <cub/device/device_radix_sort.cuh>
 
 namespace bevk {
 namespace png {
@@ -77,7 +83,9 @@ struct Opts {
 // level 1; a level: every filter (libpng's default).  Returns 0, 1 for a list cv2 does not take (odd length, unknown
 // key) or 2 for one the encoder does not reproduce: level 0 (deflate_stored, whose blocks follow libpng's output
 // buffer), a hash-chain strategy (DEFAULT, FILTERED, FIXED), BILEVEL != 0 (not a 3-channel format) and ZLIBBUFFER_SIZE.
-inline int normalise(const int* p, int n, Opts* o) {
+// With hash_chain, a hash-chain strategy at levels 4..9 (zlib's deflate_slow) is taken too; levels 1..3 under those
+// strategies (deflate_fast, whose chains depend on its parse) stay refused.
+inline int normalise(const int* p, int n, Opts* o, bool hash_chain = false) {
   if (n < 0 || (n & 1) || (n && !p)) return 1;
   int level = -1, strategy = kZRle, filter = -1;
   bool bilevel = false, zbuf = false;
@@ -98,8 +106,29 @@ inline int normalise(const int* p, int n, Opts* o) {
   o->level = level < 0 ? 1 : level;
   o->strategy = strategy;
   o->filters = filter >= 0 ? filter : level < 0 ? kFilterSub : kFilterAll;
-  if (bilevel || zbuf || o->level == 0 || (strategy != kZRle && strategy != kZHuffmanOnly)) return 2;
+  if (bilevel || zbuf || o->level == 0) return 2;
+  if (strategy != kZRle && strategy != kZHuffmanOnly && !(hash_chain && o->level >= 4)) return 2;
   return 0;
+}
+__host__ __device__ inline bool lazy_parse(const Opts& o) { return o.strategy != kZRle && o.strategy != kZHuffmanOnly; }
+
+// zlib 1.2.11's configuration_table for deflate_slow (levels 4..9): good_length, max_lazy, nice_length, max_chain
+struct LazyCfg { int good, lazy, nice, chain; };
+__host__ __device__ inline LazyCfg lazy_cfg(int level) {
+  switch (level) {
+    case 4: return {4, 4, 16, 16};
+    case 5: return {8, 16, 32, 32};
+    case 6: return {8, 16, 128, 128};
+    case 7: return {8, 32, 128, 256};
+    case 8: return {32, 128, 258, 1024};
+    default: return {32, 258, 258, 4096};
+  }
+}
+// FLEVEL of the zlib header (deflate.c): 0 under Z_HUFFMAN_ONLY / Z_RLE / Z_FIXED or below level 2, 1 for levels 2..5,
+// 2 for level 6, 3 above
+__host__ __device__ inline int zlib_flevel(const Opts& o) {
+  if (o.strategy >= kZHuffmanOnly || o.level < 2) return 0;
+  return o.level < 6 ? 1 : o.level == 6 ? 2 : 3;
 }
 
 // ------------------------------------------------------------------ geometry and bounds
@@ -224,7 +253,7 @@ __host__ __device__ inline int window_bits(long long N) {
   }
   return wb < 9 ? 9 : wb;
 }
-__host__ __device__ inline void zlib_header(long long N, uint8_t out[2]) {
+__host__ __device__ inline void zlib_header(long long N, uint8_t out[2], int flevel = 0) {
   unsigned cinfo = (unsigned)window_bits(N) - 8;
   if (N <= 16384) {
     unsigned half = 1u << (cinfo + 7);
@@ -232,9 +261,9 @@ __host__ __device__ inline void zlib_header(long long N, uint8_t out[2]) {
       do { half >>= 1; --cinfo; } while (cinfo > 0 && (unsigned long long)N <= half);
     }
   }
-  const unsigned cmf = (cinfo << 4) | 8;
+  const unsigned cmf = (cinfo << 4) | 8, h = (cmf << 8) | ((unsigned)flevel << 6);
   out[0] = (uint8_t)cmf;
-  out[1] = (uint8_t)(31 - (cmf << 8) % 31);
+  out[1] = (uint8_t)((h & 0xff) + 31 - h % 31);
 }
 
 // ------------------------------------------------------------------ parse (Z_RLE / Z_HUFFMAN_ONLY)
@@ -254,6 +283,126 @@ __host__ __device__ inline int rle_symbol(const uint8_t* f, long long N, long lo
 }
 __host__ __device__ inline bool run_start(const uint8_t* f, long long p) { return p == 0 || f[p] != f[p - 1]; }
 
+// ------------------------------------------------------------------ parse (deflate_slow, levels 4..9; DESIGN.md section 2)
+// zlib's hash chains hold every earlier position with the same 3-byte hash (deflate_slow inserts the inside of its
+// matches too, and only skips the last 2 bytes of the stream, which nothing later can reach), so each position's
+// longest_match over the full chain and over a quarter of it (prev_length >= good_match) is a function of the
+// filtered bytes alone.  prev[p] is the nearest earlier position with p's hash (0: none; position 0 is zlib's NIL).
+constexpr int kTooFar = 4096, kMinLookahead = 262;
+constexpr uint32_t kKwHead = 1u << 31;   // see lazy_match
+__host__ __device__ inline unsigned hash3(const uint8_t* f, long long p) {
+  return (((unsigned)f[p] << 10) ^ ((unsigned)f[p + 1] << 5) ^ f[p + 2]) & 0x7fff;
+}
+// A match as deflate_slow weighs it: (len << 16) | dist, or 0 for none or for one zlib drops (Z_FILTERED: len <= 5;
+// TOO_FAR: len 3 farther than 4096).
+__host__ __device__ inline uint32_t match_rec(int len, long long dist, int strategy) {
+  if (len < 3 || (len <= 5 && (strategy == kZFiltered || (len == 3 && dist > kTooFar)))) return 0;
+  return ((uint32_t)len << 16) | (uint32_t)dist;
+}
+__host__ __device__ inline int rec_len(uint32_t m) { return (int)((m >> 16) & 0x1ff); }
+__host__ __device__ inline int rec_dist(uint32_t m) { return (int)(m & 0xffff); }
+// Common prefix of f[a..] and f[p..] (a < p), at most lim bytes.
+__host__ __device__ inline int common_len(const uint8_t* f, long long a, long long p, int lim) {
+#ifdef __CUDA_ARCH__
+  const uint8_t *x = f + a, *y = f + p;
+  int n = 0;
+  while (n + 4 <= lim) {   // 4 bytes at a time from aligned words
+    const uintptr_t ux = (uintptr_t)(x + n), uy = (uintptr_t)(y + n);
+    const uint32_t* wx = reinterpret_cast<const uint32_t*>(ux & ~(uintptr_t)3);
+    const uint32_t* wy = reinterpret_cast<const uint32_t*>(uy & ~(uintptr_t)3);
+    const uint32_t vx = __funnelshift_r(wx[0], (ux & 3) ? wx[1] : 0u, (unsigned)(ux & 3) * 8);
+    const uint32_t vy = __funnelshift_r(wy[0], (uy & 3) ? wy[1] : 0u, (unsigned)(uy & 3) * 8);
+    const uint32_t d = vx ^ vy;
+    if (d) return n + (__ffs(d) - 1) / 8;
+    n += 4;
+  }
+  while (n < lim && x[n] == y[n]) ++n;
+  return n;
+#else
+  int n = 0;
+  while (n < lim && f[a + n] == f[p + n]) ++n;
+  return n;
+#endif
+}
+struct MatchRec { uint32_t full, quarter; };
+// longest_match at position p of an N-byte stream under level / strategy, once with max_chain candidates (full) and
+// once with max_chain / 4 (quarter): the nearest candidate of the greatest length wins, the walk stops at nice_match
+// (at most the lookahead), lengths stop at 258 and at the end of the stream.  The head is taken at distance <=
+// MAX_DIST = w_size - 262, chain successors at < MAX_DIST.  Bytes past the end of the stream (zlib's window there holds
+// zeros or stale bytes) cannot change the winner: a candidate reaching the end is already >= nice_match, so the walk
+// stops at the first one.
+// One head needs the parse: at T = k w_size + MAX_DIST (k >= 1) a head at k w_size is zlib's NIL when the window
+// slides before T's search, which it does unless the window is full then -- that is, unless the input ends or the row
+// read last ends at (k + 1) w_size - 1 (then it is none here), or the last parse step before T lies at or below the
+// last row end before (k + 1) w_size minus 262 (lazy_chain checks that, flagged by kKwHead).
+__host__ __device__ inline MatchRec lazy_match(const uint8_t* f, long long N, const unsigned* prev, long long p, int level,
+                                               int strategy, long long rb) {
+  MatchRec r{0, 0};
+  const long long la = N - p;
+  if (la < 3) return r;
+  const long long head = prev[p], w = 1ll << window_bits(N), maxd = w - kMinLookahead;
+  if (head == 0 || p - head > maxd) return r;
+  uint32_t flag = 0;
+  if (p - head == maxd && head % w == 0) {
+    if (N < head + w || (head + w - 1) % rb == 0) return r;
+    flag = kKwHead;
+  }
+  const LazyCfg c = lazy_cfg(level);
+  const int lim = la < kMaxMatch ? (int)la : kMaxMatch, nice = c.nice < lim ? c.nice : lim, quarter = c.chain >> 2;
+  const long long limit = p > maxd ? p - maxd : 0;
+  int best = 2, seen = 0;
+  long long bestd = 0, cur = head;
+  bool have_q = false;
+  for (;;) {
+    if (f[cur + best] == f[p + best] && f[cur] == f[p] && f[cur + 1] == f[p + 1]) {   // longest_match's quick test
+      const int len = common_len(f, cur, p, lim);
+      if (len > best) {
+        best = len;
+        bestd = p - cur;
+        if (len >= nice) break;
+      }
+    }
+    if (++seen == quarter) { r.quarter = match_rec(best, bestd, strategy); have_q = true; }
+    if (seen == c.chain) break;
+    cur = prev[cur];
+    if (cur <= limit) break;
+  }
+  r.full = match_rec(best, bestd, strategy);
+  if (!have_q) r.quarter = r.full;
+  r.full |= flag;
+  r.quarter |= flag;
+  return r;
+}
+
+// From a canonical position s (no pending match, prev_length MIN_MATCH - 1) deflate_slow's lazy steps run to the next
+// canonical position: lits literals from s, then (m != 0) the match m at s + lits, then (extra) one literal at its end.
+// Each lazy replacement is strictly longer, so a chain takes at most 256 steps.  rec(p) gives lazy_match's MatchRec.
+struct Chain { unsigned lits; uint32_t m; bool extra; long long next; };
+template <class Rec>
+__host__ __device__ inline Chain lazy_chain(long long s, long long N, int level, long long rb, Rec rec) {
+  const LazyCfg c = lazy_cfg(level);
+  uint32_t m = rec(s).full & ~kKwHead;
+  if (!m) return Chain{1, 0, false, s + 1};
+  long long x = s;
+  for (;;) {
+    const int pl = rec_len(m);
+    if (pl >= c.lazy) break;
+    const MatchRec r = rec(x + 1);
+    const uint32_t m2 = (pl >= c.good ? r.quarter : r.full) & ~kKwHead;
+    if (rec_len(m2) <= pl) break;
+    m = m2;
+    ++x;
+  }
+  Chain ch{(unsigned)(x - s), m, false, x + rec_len(m)};
+  const long long t = ch.next;   // the match is emitted by the step at x + 1; the next step is t
+  if (t < N && (rec(t).full & kKwHead)) {
+    const long long row_end = (t + kMinLookahead - 1) / rb * rb;   // last row end before t + 262 = (k + 1) w_size
+    if (x + 1 <= row_end - kMinLookahead) { ch.extra = true; ch.next = t + 1; }   // the window slid: no search at t
+  }
+  return ch;
+}
+__host__ __device__ inline unsigned chain_symbols(const Chain& ch) { return ch.lits + (ch.m != 0) + ch.extra; }
+
 // ------------------------------------------------------------------ deflate tables
 // Length code (0..28) of a match length 3..258; zlib codes 258 as code 28 (285), not as 284 + 31.
 __host__ __device__ inline int length_code(int len) {
@@ -271,6 +420,16 @@ __host__ __device__ inline int length_base(int code) {   // base of lc = len - 3
   const int xb = length_extra(code);
   return (4 << xb) + ((code & 3) << xb);
 }
+// Distance code (0..29) of a distance 1..32768, its extra bits and the base of dist - 1 (zlib's d_code / base_dist)
+__host__ __device__ inline int dist_code(int dist) {
+  const unsigned d = (unsigned)dist - 1;
+  if (d < 4) return (int)d;
+  int nb = 31;
+  while (!(d >> nb)) --nb;
+  return 2 * nb + (int)((d >> (nb - 1)) & 1);
+}
+__host__ __device__ inline int dist_extra(int code) { return code < 4 ? 0 : (code - 2) >> 1; }
+__host__ __device__ inline int dist_base(int code) { return code < 4 ? code : (2 + (code & 1)) << dist_extra(code); }
 __host__ __device__ inline int static_llen(int n) { return n < 144 ? 8 : n < 256 ? 9 : n < 280 ? 7 : 8; }
 __host__ __device__ inline unsigned bit_reverse(unsigned code, int len) {
   unsigned r = 0;
@@ -466,7 +625,9 @@ struct BitSink {
 // block's raw length.  Builds the trees, fills w.lt / w.dt with the codes of the block type chosen (the static codes
 // for a static block) and returns the type; *hdr_bits: the bits after the 3-bit block header that precede the symbols
 // (dynamic tree description), written to hdr when non-NULL.
-__host__ __device__ inline int decide_block(TreeWork& w, unsigned long long stored_len, unsigned* hdr_bits, uint32_t* hdr) {
+// fixed (Z_FIXED): the static code unless the stored block is no larger (stored weighed against the static size).
+__host__ __device__ inline int decide_block(TreeWork& w, unsigned long long stored_len, unsigned* hdr_bits, uint32_t* hdr,
+                                            bool fixed = false) {
   w.opt_len = w.static_len = 0;
   w.lmax = build_tree(w, w.lt, kLCodes, 0);
   w.dmax = build_tree(w, w.dt, kDCodes, 1);
@@ -485,7 +646,7 @@ __host__ __device__ inline int decide_block(TreeWork& w, unsigned long long stor
   w.blmax = max_blindex;
   unsigned long long opt_lenb = (w.opt_len + 3 + 7) >> 3;
   const unsigned long long static_lenb = (w.static_len + 3 + 7) >> 3;
-  if (static_lenb <= opt_lenb) opt_lenb = static_lenb;
+  if (static_lenb <= opt_lenb || fixed) opt_lenb = static_lenb;
   int type;
   if (stored_len + 4 <= opt_lenb) type = kStored;
   else if (static_lenb == opt_lenb) type = kStatic;
@@ -531,6 +692,21 @@ __host__ __device__ inline int symbol_code(const Node* lt, const Node* dt, int s
   *v = val;
   return n + dt[0].dl;
 }
+// The same for a match at any distance: at most 15 + 5 + 15 + 13 = 48 bits.
+__host__ __device__ inline int symbol_code(const Node* lt, const Node* dt, int sym, int dist, uint64_t* v) {
+  if (sym < 256) { *v = lt[sym].fc; return lt[sym].dl; }
+  const int len = sym - 256 + 3, code = length_code(len), xb = length_extra(code);
+  const int ll = lt[257 + code].dl;
+  uint64_t val = lt[257 + code].fc;
+  int n = ll;
+  if (xb) { val |= (uint64_t)(len - 3 - length_base(code)) << n; n += xb; }
+  const int dc = dist_code(dist), dx = dist_extra(dc);
+  val |= (uint64_t)dt[dc].fc << n;
+  n += dt[dc].dl;
+  if (dx) { val |= (uint64_t)(dist - 1 - dist_base(dc)) << n; n += dx; }
+  *v = val;
+  return n;
+}
 
 
 // ------------------------------------------------------------------ device pipeline
@@ -562,8 +738,19 @@ struct PngArgs {
   unsigned long long* out_off;   // [n] offsets in out
   unsigned long long* base;      // running end of the compacted output (one value)
   uint8_t* out;
+  unsigned* nblk;                // [n] blocks per image
+  // hash-chain parse (levels 4..9); dists NULL under Z_RLE / Z_HUFFMAN_ONLY (every match at distance 1)
+  int level, flevel;
+  const unsigned* prev;          // [n * N] nearest earlier position of the same hash (image-relative, 0 none)
+  MatchRec* recs;                // [n * N] lazy_match per position
+  unsigned* jump;                // [n * N] next canonical position (group index, kEnd past the image), then doubled
+  unsigned* jump2;
+  uint8_t* mark;                 // [n * N] canonical position on the parse from the image start
+  unsigned* cnt;                 // [n * N + 1] symbols of each canonical position's chain
+  uint16_t* dists;               // [n][N] match distances beside syms
 };
 constexpr int kPngThreads = 256;
+constexpr unsigned kEnd = 0xffffffffu;
 
 __device__ inline void or_bits(uint32_t* words, unsigned long long pos, uint32_t v, int n) {
   if (!v || !n) return;
@@ -634,9 +821,106 @@ __global__ void __launch_bounds__(kPngThreads) k_png_filter(PngArgs a) {
 __global__ void k_png_setup(PngArgs a) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= a.n) return;
-  const unsigned ns = a.strategy == kZRle ? a.symidx[(i + 1) * a.N] - a.symidx[i * a.N] : (unsigned)a.N;
+  const unsigned ns = a.strategy == kZRle || a.dists ? a.symidx[(i + 1) * a.N] - a.symidx[i * a.N] : (unsigned)a.N;
   a.nsym[i] = ns;
-  if (ns % kBlockSyms == 0) a.blk[i * a.maxb + ns / kBlockSyms].raw0 = (unsigned)a.N;   // the empty final block
+  // deflate_slow tallies a literal left pending at the end without the block-full check: a last block of exactly 16383
+  // symbols ending in the literal of the last byte is not followed by an empty one
+  const bool tail_lit = a.dists && a.mark[(i + 1) * a.N - 1];
+  a.nblk[i] = ns / kBlockSyms + 1 - (ns && ns % kBlockSyms == 0 && tail_lit);
+  if (ns % kBlockSyms == 0 && !(ns && tail_lit)) a.blk[i * a.maxb + ns / kBlockSyms].raw0 = (unsigned)a.N;   // the empty final block
+}
+
+// ---- hash-chain parse: hash sort keys, prev[], lazy_match per position, canonical chains, their list ranking
+// Sort key of group position p: image and 3-byte hash, or past every image for the last 2 bytes (never inserted).
+struct HashKey {
+  const uint8_t* f;
+  long long N;
+  unsigned n;
+  __host__ __device__ unsigned operator()(unsigned p) const {
+    const unsigned i = (unsigned)(p / N);
+    const long long q = p - (long long)i * N;
+    return q + 3 <= N ? (i << 15) | hash3(f, p) : n << 15;
+  }
+};
+__global__ void k_png_keys(HashKey h, unsigned* key, unsigned* pos, unsigned total) {
+  for (unsigned p = blockIdx.x * blockDim.x + threadIdx.x; p < total; p += gridDim.x * blockDim.x) {
+    key[p] = h(p);
+    pos[p] = p;
+  }
+}
+__global__ void k_png_prev(const unsigned* key, const unsigned* pos, unsigned* prev, unsigned total, long long N) {
+  for (unsigned k = blockIdx.x * blockDim.x + threadIdx.x; k < total; k += gridDim.x * blockDim.x) {
+    const unsigned p = pos[k], base = (unsigned)(p / N * N);
+    prev[p] = k && key[k] == key[k - 1] ? pos[k - 1] - base : 0u;
+  }
+}
+__global__ void k_png_match(PngArgs a) {
+  const unsigned total = (unsigned)(a.n * a.N);
+  const long long rb = row_bytes(a.W);
+  for (unsigned p = blockIdx.x * blockDim.x + threadIdx.x; p < total; p += gridDim.x * blockDim.x) {
+    const unsigned i = (unsigned)(p / a.N), base = (unsigned)(i * a.N);
+    a.recs[p] = lazy_match(a.f + base, a.N, a.prev + base, p - base, a.level, a.strategy, rb);
+  }
+}
+struct RecAt {
+  const MatchRec* r;
+  __host__ __device__ MatchRec operator()(long long p) const { return r[p]; }
+};
+__device__ inline Chain group_chain(const PngArgs& a, unsigned p, unsigned* base) {
+  const unsigned i = (unsigned)(p / a.N);
+  *base = (unsigned)(i * a.N);
+  return lazy_chain(p - *base, a.N, a.level, row_bytes(a.W), RecAt{a.recs + *base});
+}
+// Every position's chain as if it were canonical: the next canonical position; image starts are on the parse.
+__global__ void k_png_next(PngArgs a) {
+  const unsigned total = (unsigned)(a.n * a.N);
+  for (unsigned p = blockIdx.x * blockDim.x + threadIdx.x; p < total; p += gridDim.x * blockDim.x) {
+    unsigned base;
+    const Chain ch = group_chain(a, p, &base);
+    a.jump[p] = ch.next < a.N ? base + (unsigned)ch.next : kEnd;
+    a.mark[p] = p == base;
+  }
+}
+// One doubling round: after round r, jump is next^(2^(r+1)) and the marks hold the first 2^(r+1) positions of every
+// image's parse (a mark set early in the round only adds a later position of the same parse).
+__global__ void k_png_jump(const unsigned* jump, unsigned* jump2, uint8_t* mark, unsigned total) {
+  for (unsigned p = blockIdx.x * blockDim.x + threadIdx.x; p < total; p += gridDim.x * blockDim.x) {
+    const unsigned j = jump[p];
+    if (j == kEnd) { jump2[p] = kEnd; continue; }
+    if (mark[p]) mark[j] = 1;
+    jump2[p] = jump[j];
+  }
+}
+__global__ void k_png_count(PngArgs a) {
+  const unsigned total = (unsigned)(a.n * a.N);
+  for (unsigned p = blockIdx.x * blockDim.x + threadIdx.x; p <= total; p += gridDim.x * blockDim.x) {
+    unsigned base, c = 0;
+    if (p < total && a.mark[p]) c = chain_symbols(group_chain(a, p, &base));
+    a.cnt[p] = c;
+  }
+}
+// Symbols of every canonical position's chain at their indices, and the raw start of every block.
+__global__ void k_png_lazy_compact(PngArgs a) {
+  const unsigned total = (unsigned)(a.n * a.N);
+  for (unsigned p = blockIdx.x * blockDim.x + threadIdx.x; p < total; p += gridDim.x * blockDim.x) {
+    if (!a.mark[p]) continue;
+    unsigned base;
+    const Chain ch = group_chain(a, p, &base);
+    const unsigned i = (unsigned)(p / a.N), q = p - base;
+    unsigned j = a.symidx[p] - a.symidx[base];
+    auto put = [&](unsigned at, int v, int d) {
+      a.syms[base + j] = (uint16_t)v;
+      a.dists[base + j] = (uint16_t)d;
+      if (j % kBlockSyms == 0) a.blk[i * a.maxb + j / kBlockSyms].raw0 = at;
+      ++j;
+    };
+    for (unsigned k = 0; k < ch.lits; ++k) put(q + k, a.f[p + k], 0);
+    if (ch.m) {
+      const int len = rec_len(ch.m);
+      put(q + ch.lits, 256 + len - 3, rec_dist(ch.m));
+      if (ch.extra) put(q + ch.lits + len, a.f[p + ch.lits + len], 0);
+    }
+  }
 }
 
 __global__ void k_png_compact(PngArgs a) {
@@ -653,7 +937,7 @@ __global__ void k_png_compact(PngArgs a) {
 
 __device__ inline bool block_range(const PngArgs& a, long long b, int* i, unsigned* s0, unsigned* cnt, bool* last) {
   *i = (int)(b / a.maxb);
-  const unsigned j = (unsigned)(b % a.maxb), ns = a.nsym[*i], nblk = ns / kBlockSyms + 1;
+  const unsigned j = (unsigned)(b % a.maxb), ns = a.nsym[*i], nblk = a.nblk[*i];
   if (j >= nblk) return false;
   *s0 = j * kBlockSyms;
   *cnt = min((unsigned)kBlockSyms, ns - *s0);
@@ -674,10 +958,11 @@ __global__ void __launch_bounds__(kPngThreads) k_png_tree(PngArgs a) {
   for (int k = threadIdx.x; k < 2 * kDCodes + 1; k += kPngThreads) w.dt[k].fc = 0;
   __syncthreads();
   const uint16_t* sy = a.syms + i * a.N + s0;
+  const uint16_t* dy = a.dists ? a.dists + i * a.N + s0 : nullptr;
   for (unsigned k = threadIdx.x; k < cnt; k += kPngThreads) {
     const int v = sy[k];
     if (v < 256) atomicAdd(&w.lt[v].fc, 1u);
-    else { atomicAdd(&w.lt[257 + length_code(v - 256 + 3)].fc, 1u); atomicAdd(&w.dt[0].fc, 1u); }
+    else { atomicAdd(&w.lt[257 + length_code(v - 256 + 3)].fc, 1u); atomicAdd(&w.dt[dy ? dist_code(dy[k]) : 0].fc, 1u); }
   }
   __syncthreads();
   __shared__ int s_type;
@@ -687,7 +972,7 @@ __global__ void __launch_bounds__(kPngThreads) k_png_tree(PngArgs a) {
     uint32_t* hdr = a.hdr + b * kHdrWords;
     for (int k = 0; k < kHdrWords; ++k) hdr[k] = 0;
     const unsigned raw0 = a.blk[b].raw0, raw1 = last ? (unsigned)a.N : a.blk[b + 1].raw0;
-    s_type = decide_block(w, raw1 - raw0, &s_hb, hdr);
+    s_type = decide_block(w, raw1 - raw0, &s_hb, hdr, a.strategy == kZFixed);
   }
   __syncthreads();
   if (s_type == kStored) {
@@ -699,8 +984,8 @@ __global__ void __launch_bounds__(kPngThreads) k_png_tree(PngArgs a) {
   for (int k = threadIdx.x; k < kDCodes; k += kPngThreads) codes[kLCodes + k] = ((uint32_t)w.dt[k].dl << 16) | w.dt[k].fc;
   unsigned long long bits = 0;
   for (unsigned k = threadIdx.x; k < cnt; k += kPngThreads) {
-    uint32_t v;
-    bits += symbol_code(w.lt, w.dt, sy[k], &v);
+    uint64_t v;
+    bits += symbol_code(w.lt, w.dt, sy[k], dy ? dy[k] : 1, &v);
   }
   bits = Reduce(tmp).Sum(bits);
   if (threadIdx.x == 0) {
@@ -713,7 +998,7 @@ __global__ void __launch_bounds__(kPngThreads) k_png_tree(PngArgs a) {
 __global__ void k_png_layout(PngArgs a) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= a.n) return;
-  const unsigned ns = a.nsym[i], nblk = ns / kBlockSyms + 1;
+  const unsigned nblk = a.nblk[i];
   unsigned long long pos = 16;
   for (unsigned j = 0; j < nblk; ++j) {
     Blk& bk = a.blk[i * a.maxb + j];
@@ -728,7 +1013,7 @@ __global__ void k_png_layout(PngArgs a) {
   pos = (pos + 7) & ~7ull;
   const unsigned long long zb = pos / 8 + 4;
   uint8_t* z = reinterpret_cast<uint8_t*>(a.zw + i * a.zwords);
-  zlib_header(a.N, z);
+  zlib_header(a.N, z, a.flevel);
   Adler ad{0, 0, 0};
   for (int y = 0; y < a.H; ++y) ad = adler_cat(ad, a.rowad[(long long)i * a.H + y]);
   const uint32_t v = adler_final(ad);
@@ -777,14 +1062,16 @@ __global__ void __launch_bounds__(kPngThreads) k_png_pack(PngArgs a) {
   if (threadIdx.x == 0) s_pos = bk.off + 3 + bk.hdr_bits;
   __syncthreads();
   const uint16_t* sy = a.syms + i * a.N + s0;
+  const uint16_t* dy = a.dists ? a.dists + i * a.N + s0 : nullptr;
   for (unsigned k0 = 0; k0 < cnt; k0 += kPngThreads) {
     const unsigned k = k0 + threadIdx.x;
-    uint32_t v = 0;
-    const unsigned n = k < cnt ? (unsigned)symbol_code(lt, dt, sy[k], &v) : 0u;
+    uint64_t v = 0;
+    const unsigned n = k < cnt ? (unsigned)symbol_code(lt, dt, sy[k], dy ? dy[k] : 1, &v) : 0u;
     unsigned off, tile;
     Scan(tmp).ExclusiveSum(n, off, tile);
     const unsigned long long p0 = s_pos;
-    or_bits(words, p0 + off, v, (int)n);
+    or_bits(words, p0 + off, (uint32_t)v, (int)min(n, 32u));
+    if (n > 32) or_bits(words, p0 + off + 32, (uint32_t)(v >> 32), (int)n - 32);
     __syncthreads();
     if (threadIdx.x == 0) s_pos = p0 + tile;
     __syncthreads();

@@ -234,7 +234,7 @@ def jpeg_encode(images, quality: int = 95, ctx: L.Context | None = None, params=
 
 def png_set_params(ctx: L.Context, params=None):
     """Apply cv2.imwrite's PNG (key, value) pairs (keys 16..20, cv2.IMWRITE_PNG_*) to ctx's PNG encoding; None or []
-    restores cv2's defaults.  png_encode calls it on every call, so no call inherits another's params."""
+    restores cv2's defaults.  The list applies to bevk_png_encode; png_encode takes its own list per call."""
     arr, n = _jpeg_params(params)
     L.check(ctx.lib.bevk_png_set_params(ctx.h, arr, n))
 
@@ -250,8 +250,10 @@ def png_encode_bound(width: int, height: int, params=None) -> int:
 
 def png_encode(images, ctx: L.Context | None = None, params=None) -> list[bytes]:
     """cv2.imencode('.png', img, params) on the GPU, byte for byte, for one uint8[H][W][3] BGR image or a batch
-    uint8[N][H][W][3].  params: cv2.imwrite's PNG pairs with the RLE or HUFFMAN_ONLY strategy (see bevk_png_set_params;
-    a list that ends at zlib's default strategy raises BevkError), None for cv2's defaults.
+    uint8[N][H][W][3].  params: cv2.imwrite's PNG pairs (see bevk_png_encode_params), None for cv2's defaults; the
+    RLE / HUFFMAN_ONLY strategies at any level and zlib's hash-chain parse at levels 4..9 (cv2.imwrite's
+    [IMWRITE_PNG_COMPRESSION, 9] among them).  Level 0, levels 1..3 under the hash-chain strategies, BILEVEL and
+    ZLIBBUFFER_SIZE raise BevkError.  The ctx's png_set_params list is left as it was.
     CUDA arrays (``__cuda_array_interface__``) are read in place, on torch's current stream; NumPy input is uploaded
     once.  Returns one ``bytes`` per image -- what cv2.imwrite would write to a .png file."""
     ctx = ctx or L.default_context()
@@ -266,12 +268,13 @@ def png_encode(images, ctx: L.Context | None = None, params=None) -> list[bytes]
     ptr, n, h, w, img_stride, row_stride = _cuda_bgr_batch(keep)
     if n < 1:
         return []
-    cap = n * png_encode_bound(w, h, params)
+    cap = n * png_encode_bound(w, h)       # the bound holds under every list
     out = np.empty(cap, np.uint8)          # pages are only touched where streams land
     sizes = (C.c_uint64 * n)()
-    png_set_params(ctx, params)
+    arr, k = _jpeg_params(params)
     with ctx.on_stream(_torch_current_stream(ctx.device)):
-        L.check(ctx.lib.bevk_png_encode(ctx.h, C.c_void_p(ptr), img_stride, row_stride, n, w, h, L.vptr(out), cap, sizes))
+        L.check(ctx.lib.bevk_png_encode_params(ctx.h, arr, k, C.c_void_p(ptr), img_stride, row_stride, n, w, h, L.vptr(out),
+                                               cap, sizes))
     res, off = [], 0
     for s in sizes:
         res.append(out[off:off + s].tobytes())
@@ -446,6 +449,18 @@ class Undistorter:
         L.check(self.ctx.lib.bevk_undistort_jpeg(self.ctx.h, self.slot, L.vptr(img), sw, sh, ss, _interp(interpolation),
                                                  int(quality), L.vptr(self._jpeg_buf), self._jpeg_buf.size, C.byref(size)))
         return self._jpeg_buf[:size.value].tobytes()
+
+    def png(self, src: np.ndarray, params=None, interpolation: int = INTER_LINEAR) -> bytes:
+        """The undistorted image as the bytes cv2.imwrite(path, self(src), params) writes to a .png file: undistorted
+        and encoded on the device (png_encode's params, e.g. [IMWRITE_PNG_COMPRESSION, 9]), only the stream comes back.
+        src: uint8[h][w][3] BGR."""
+        self._live()
+        a = np.asarray(src)
+        if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
+            raise L.BevkError("Undistorter.png takes uint8[h][w][3] BGR images")
+        import torch
+        d = torch.from_numpy(np.ascontiguousarray(a)).to(torch.device("cuda", self.ctx.device))
+        return png_encode(self.cuda(d, interpolation=interpolation), ctx=self.ctx, params=params)[0]
 
     def cuda(self, frames, out=None, interpolation: int = INTER_LINEAR, stream: int | None = None):
         """Undistort frames that already live on the GPU: no PCIe in the call.

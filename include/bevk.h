@@ -391,7 +391,8 @@ int bevk_bev_frames_to_jpeg(bevk_ctx *ctx, const void *const *frames, int batch,
  * Replaces cv2.imwrite('x.png', img, params) / cv2.imencode('.png', ...) for 8-bit 3-channel BGR images: the streams are
  * byte-identical to cv2's (libpng 1.6 + zlib 1.2.11: colour type 2, IDAT chunks of 8192 bytes) and only the compressed
  * bytes cross PCIe.  cv2's defaults (SUB filter, zlib level 1, Z_RLE) and IMWRITE_PNG_STRATEGY_RLE / _HUFFMAN_ONLY are
- * reproduced; zlib's hash-chain strategies are not.
+ * reproduced by every entry; bevk_png_encode_params also reproduces zlib's hash-chain parse (deflate_slow) at levels 4..9
+ * under the DEFAULT, FILTERED and FIXED strategies.
  * bevk_png_set_params: cv2.imwrite's PNG (key, value) pairs, n ints (n even), applied to bevk_png_encode on this ctx
  * until the next call; n == 0 restores cv2's defaults.  Keys 16..20 as cv2.IMWRITE_PNG_*, read in order as cv2 4.13 does:
  *   COMPRESSION (16)     clamped to [0, 9]; resets the strategy to DEFAULT and switches to adaptive filtering over all
@@ -412,6 +413,18 @@ int bevk_png_set_params(bevk_ctx *ctx, const int *params, int n);
 int bevk_png_encode_bound(int width, int height, const int *params, int n, uint64_t *bytes);
 int bevk_png_encode(bevk_ctx *ctx, const void *d_images, int64_t image_stride, int64_t row_stride, int n, int width, int height,
                     uint8_t *out, uint64_t capacity, uint64_t *sizes);
+/* bevk_png_encode_params: bevk_png_encode with the (key, value) list given per call, as cv2.imencode takes it, read as
+ * above except that a list ending at level 4..9 under the DEFAULT (0), FILTERED (1) or FIXED (4) strategy -- [16, 9],
+ * cv2.imwrite's level 9 -- is taken too.  Level 0, levels 1..3 under those strategies (a STRATEGY 0 / 1 / 4 without a
+ * COMPRESSION is level 1), BILEVEL != 0 and ZLIBBUFFER_SIZE are BEVK_ERR_UNSUPPORTED.  The same contract as
+ * bevk_png_encode (the call synchronises, sizes[] always filled, nothing written past capacity, bevk_last_kernel_ms
+ * covers it); the ctx's bevk_png_set_params list is neither read nor changed.  bevk_png_encode_bound(w, h, NULL, 0)
+ * bounds its streams too: the bound does not depend on the parameters.  The hash-chain parse keeps about 50 bytes of
+ * device memory per filtered byte of a group (up to 32 MB of filtered data, or one larger image) in the ctx until it
+ * is destroyed: an image of 1.5 G filtered bytes needs about 75 GB and fails with BEVK_ERR_OOM where that is not free. */
+int bevk_png_encode_params(bevk_ctx *ctx, const int *params, int n_params, const void *d_images, int64_t image_stride,
+                           int64_t row_stride, int n, int width, int height, uint8_t *out, uint64_t capacity,
+                           uint64_t *sizes);
 
 /* ---- CUDA graphs over the device-pointer entry points ------------------------------------------------
  * Everything the "_device" / "_stack" / "_frames" entry points enqueue on the ctx stream between begin and end is
