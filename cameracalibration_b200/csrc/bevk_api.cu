@@ -1249,8 +1249,8 @@ static int launch_gain(bevk_ctx* c, uint8_t* out, int batch, const unsigned long
   return BEVK_OK;
 }
 
-// run_device flag, not part of the ABI: with BALANCE, stop at the raw composed canvas and its channel sums (d_csum).  The
-// encoder's GainSrc applies the gains and the car, so k_gain does not run.  (Without BALANCE the write-out adds the car.)
+// run_device flag, not part of the ABI: with BALANCE, stop at the raw composed canvas and its channel sums (d_csum).
+// k_canvas_yuv<..., true> applies the gains and the car, so k_gain does not run.  (Without BALANCE the write-out adds the car.)
 constexpr int kFlagRawBalance = 1 << 30;
 
 // YUV frames (BEVK_FLAG_NV12 / _I420) are `planes` when given (src then only has to be non-null), else the dense stack src.
@@ -2358,14 +2358,10 @@ int bevk_jpeg_encode_bound_params(int width, int height, const int* params, int 
   return BEVK_OK;
 }
 
-// What the encoder reads: n images at img + i * istride, rows pitch bytes apart.  With csum they are raw BEV canvases
-// under BALANCE (GainSrc): colour balance from their channel sums csum[3 * i ...] and the car (NULL or a dense canvas)
-// are applied as the blocks are loaded.
+// What the encoder reads: n images at img + i * istride, rows pitch bytes apart.
 struct JpegIn {
   const void* img = nullptr;
   long long istride = 0, pitch = 0;
-  const unsigned long long* csum = nullptr;
-  const uint8_t* car = nullptr;
 };
 
 // Enqueue the encoder over n w x h images into slot s on the ctx stream: every kernel, then the D2H of the stream sizes
@@ -2435,7 +2431,6 @@ static int jpeg_enqueue(bevk_ctx* c, int s, const JpegIn& in, int n, int w, int 
   a.offs = e.offs.as<unsigned long long>(); a.dcdiff = e.dcdiff.as<int>(); a.words = e.words.as<uint32_t>(); a.words_img = words_img;
   a.chunks_img = chunks; a.ffcnt = e.ffcnt.as<unsigned>(); a.ffscan = e.ffscan.as<unsigned>(); a.header = e.d_header.as<uint8_t>();
   a.out = e.out[s].as<uint8_t>(); a.out_off = e.meta[s].as<unsigned long long>(); a.sizes = e.meta[s].as<unsigned long long>() + n;
-  a.csum = in.csum; a.npix = (double)w * (double)h; a.car = in.car;
   a.rst = o.rst; a.nint = nint; a.hlen0 = header_bytes(o);
   if (o.rst) { a.ilen = e.ilen.as<unsigned long long>(); a.iofs = e.iofs.as<unsigned long long>(); }
   if (o.optimize) {
@@ -2446,13 +2441,7 @@ static int jpeg_enqueue(bevk_ctx* c, int s, const JpegIn& in, int n, int w, int 
   CU(cudaEventRecord(c->ev0, c->stream));
   RET(with_sampling(o.hy, o.vy, [&](auto hy, auto vy) -> int {
     constexpr int HY = hy(), VY = vy();
-    if (in.csum) {
-      const size_t gsmem = (size_t)gain_images_per_cta(nblk, n) * 768;
-      CU(cudaFuncSetAttribute(k_jpeg_blocks<GainSrc, HY, VY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gsmem));
-      k_jpeg_blocks<GainSrc, HY, VY><<<gb, kBlockThreads, gsmem, c->stream>>>(a);
-    } else {
-      k_jpeg_blocks<PlainSrc, HY, VY><<<gb, kBlockThreads, 0, c->stream>>>(a);
-    }
+    k_jpeg_blocks<HY, VY><<<gb, kBlockThreads, 0, c->stream>>>(a);
     LAUNCHED(c);
     k_jpeg_dc<HY, VY><<<gb, kBlockThreads, 0, c->stream>>>(a);
     LAUNCHED(c);
@@ -2566,21 +2555,14 @@ static int jpeg_chunk(int n) {
 
 // ------------------------------------------------------------------ BEV canvases straight to JPEG (surroundBEV.py:340)
 // BevGenerator.__call__ then cv2.imencode: each chunk of frame-sets is rendered into ctx scratch and encoded there, and
-// only the streams come back.  Under BALANCE the canvases stay raw and the encoder applies colour balance and the car
-// (GainSrc), so k_gain does not run and the balanced canvas is never written.
+// only the streams come back.  Under BALANCE run_device's k_gain applies colour balance and the car to the chunk's
+// canvases before the encoder reads them.
 static int to_jpeg_check(bevk_ctx* c, uint8_t* out, uint64_t* sizes) {
   RET(need_plan(c));
   if (!out || !sizes) return fail(BEVK_ERR_ARG, "null host pointer");
   if (c->capturing) return fail(BEVK_ERR_ARG, "the BEV-to-JPEG calls synchronise and cannot be captured into a graph");
   uint64_t bound = 0;
   return bevk_jpeg_encode_bound(c->BW, c->BH, &bound);
-}
-
-static JpegIn canvas_in(bevk_ctx* c, const uint8_t* canvases, int flags, const void* d_car) {
-  JpegIn in;
-  in.img = canvases; in.pitch = (long long)c->BW * 3; in.istride = in.pitch * c->BH;
-  if (flags & BEVK_FLAG_BALANCE) { in.csum = c->d_csum.as<unsigned long long>(); in.car = reinterpret_cast<const uint8_t*>(d_car); }
-  return in;
 }
 
 int bevk_bev_run_to_jpeg(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, int batch, const uint8_t* car, int flags,
@@ -2595,8 +2577,8 @@ int bevk_bev_run_to_jpeg(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_st
   // the ingest chunks are the encoder's: staging half = canvas half = encoder slot
   return jpeg_chunks(c, batch, h.chunk, c->BW, c->BH, quality, false, out, capacity, sizes, [&](int b0, int nb, int half, JpegIn* in) -> int {
     uint8_t* dcanvas = nullptr;
-    RET(render_chunk(c, h, srcs, src_stride, flags | kFlagRawBalance, b0, nb, half, &dcanvas));
-    *in = canvas_in(c, dcanvas, flags, h.d_car);
+    RET(render_chunk(c, h, srcs, src_stride, flags, b0, nb, half, &dcanvas));
+    *in = JpegIn{dcanvas, (long long)h.cbytes, (long long)c->BW * 3};
     return BEVK_OK;
   });
 }
@@ -2620,8 +2602,8 @@ int bevk_bev_frames_to_jpeg(bevk_ctx* c, const void* const* frames, int batch, c
     if (part.table) part.table += (size_t)b0 * c->n_cam;
     else part.base += (long long)b0 * c->n_cam * part.stride;
     c->timed = false;
-    RET(run_device(c, part, nb, d_car, flags | kFlagRawBalance, dcanvas, 0, BEVK_MAX_CAMERAS));
-    *in = canvas_in(c, dcanvas, flags, d_car);
+    RET(run_device(c, part, nb, d_car, flags, dcanvas, 0, BEVK_MAX_CAMERAS));
+    *in = JpegIn{dcanvas, (long long)c->BW * c->BH * 3, (long long)c->BW * 3};
     return BEVK_OK;
   });
 }

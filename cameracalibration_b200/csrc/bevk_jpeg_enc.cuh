@@ -37,17 +37,15 @@
 // OPTIMIZE adds k_jpeg_count (symbol counts), k_jpeg_huff (tables, codes, per-image headers) and k_jpeg_bits (bits per
 // block under them) before the scan; RST_INTERVAL adds k_jpeg_intervals (padded bits per interval) and its scan after it.
 //
-// With GainSrc (bevk_bev_run_to_jpeg / bevk_bev_frames_to_jpeg under BALANCE) k_jpeg_blocks applies color_balance and
-// the car while it loads a block, so k_gain never runs.  Each CTA builds one gain table per image its blocks touch,
-// keyed by image, in dynamic shared memory (gain_images_per_cta; 768 B each, 2 for canvases of 128 blocks or more).
+// The encoder reads finished images only: BEV canvases under BALANCE (bevk_bev_run_to_jpeg / bevk_bev_frames_to_jpeg)
+// get colour balance and the car from k_gain before k_jpeg_blocks loads them.  Applying the gains in the load stage
+// instead was measured slower on H100 than k_gain followed by this encoder (DESIGN.md section 11).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
 
 #include <type_traits>
-
-#include "bevk_kernels.cuh"   // gain_table
 
 namespace bevk {
 namespace jpeg {
@@ -112,46 +110,22 @@ __host__ __device__ inline int ld8(const uint8_t* p) {
 #endif
 }
 
-// ------------------------------------------------------------------ pixel sources of the load stage
-// The load stage reads pixel (x, y) of the image being encoded through a source: src.bgr(x, y, b, g, r).
-// PlainSrc is the image as stored (bevk_jpeg_encode).
-struct PlainSrc {
-  const uint8_t* img;
-  long long pitch;
-  __host__ __device__ void bgr(int x, int y, int& b, int& g, int& r) const {
-    const uint8_t* p = img + y * pitch + 3ll * x;
-    b = ld8(p); g = ld8(p + 1); r = ld8(p + 2);
-  }
-};
-// GainSrc is a raw composed BEV canvas -- what k_bev<true> / k_bev_tma<true> leave with BALANCE -- as color_balance and
-// the car overlay turn it into the reference's result (surroundBEV.py:322-324): sat(tab[c][v] + car), where tab is
-// k_gain's 3 x 256 table (gray_world_gains + gain_entry of the canvas's channel sums).  The gained canvas never exists.
-struct GainSrc {
-  const uint8_t* img;
-  long long pitch;
-  const uint8_t* tab;     // [3][256]
-  const uint8_t* car;     // NULL, or uint8[H][W][3] at car_pitch
-  long long car_pitch;
-  __host__ __device__ void bgr(int x, int y, int& b, int& g, int& r) const {
-    const uint8_t* p = img + y * pitch + 3ll * x;
-    b = tab[ld8(p)]; g = tab[256 + ld8(p + 1)]; r = tab[512 + ld8(p + 2)];
-    if (car) {
-      const uint8_t* q = car + y * car_pitch + 3ll * x;
-      b += ld8(q); g += ld8(q + 1); r += ld8(q + 2);
-      b = b < 255 ? b : 255; g = g < 255 ? g : 255; r = r < 255 ? r : 255;
-    }
-  }
-};
+// pixel (x, y) of a BGR image with rows pitch bytes apart
+__host__ __device__ inline void bgr_at(const uint8_t* img, long long pitch, int x, int y, int& b, int& g, int& r) {
+  const uint8_t* p = img + y * pitch + 3ll * x;
+  b = ld8(p); g = ld8(p + 1); r = ld8(p + 2);
+}
+
 // Sample (r, c) of block k of MCU (mx, my): luma (k < HY*VY) or Cb (k == HY*VY) / Cr after HY x VY subsampling.
-template <int HY, int VY, class Src>
-__host__ __device__ inline int block_sample(const Src& src, const Geom& g, int mx, int my, int k, int r, int c) {
+template <int HY, int VY>
+__host__ __device__ inline int block_sample(const uint8_t* img, long long pitch, const Geom& g, int mx, int my, int k, int r, int c) {
   constexpr int NY = HY * VY;
   if (k < NY) {
     int x = (HY * mx + k % HY) * 8 + c, y = (VY * my + k / HY) * 8 + r;
     x = x < g.W ? x : g.W - 1;
     y = y < g.H ? y : g.H - 1;
     int b, gg, rr;
-    src.bgr(x, y, b, gg, rr);
+    bgr_at(img, pitch, x, y, b, gg, rr);
     return ycc_y(b, gg, rr);
   }
   const int last = (g.H + VY - 1) / VY - 1;              // chroma rows past ceil(H/VY) repeat the last one
@@ -164,7 +138,7 @@ __host__ __device__ inline int block_sample(const Src& src, const Geom& g, int m
     for (int j = 0; j < HY; ++j) {
       const int x = HY * cx + j < g.W ? HY * cx + j : g.W - 1;
       int b, gg, rr;
-      src.bgr(x, y, b, gg, rr);
+      bgr_at(img, pitch, x, y, b, gg, rr);
       s += k == NY ? ycc_cb(b, gg, rr) : ycc_cr(b, gg, rr);
     }
   }
@@ -186,17 +160,13 @@ inline auto with_sampling(int hy, int vy, F&& f) {
 }
 
 // The 64 samples of a block, level-shifted (sample - 128), natural order.
-template <int HY, int VY, class Src>
-__host__ __device__ inline void load_block_s(const Src& src, const Geom& g, int mx, int my, int k, int* d) {
+template <int HY, int VY>
+__host__ __device__ inline void load_block_s(const uint8_t* img, long long pitch, const Geom& g, int mx, int my, int k, int* d) {
   for (int r = 0; r < 8; ++r)
-    for (int c = 0; c < 8; ++c) d[r * 8 + c] = block_sample<HY, VY>(src, g, mx, my, k, r, c) - 128;
-}
-template <class Src>
-inline void load_block(const Src& src, const Geom& g, int mx, int my, int k, int* d) {
-  with_sampling(g.hy, g.vy, [&](auto hy, auto vy) { load_block_s<hy(), vy()>(src, g, mx, my, k, d); });
+    for (int c = 0; c < 8; ++c) d[r * 8 + c] = block_sample<HY, VY>(img, pitch, g, mx, my, k, r, c) - 128;
 }
 inline void load_block(const uint8_t* img, long long pitch, const Geom& g, int mx, int my, int k, int* d) {
-  load_block(PlainSrc{img, pitch}, g, mx, my, k, d);
+  with_sampling(g.hy, g.vy, [&](auto hy, auto vy) { load_block_s<hy(), vy()>(img, pitch, g, mx, my, k, d); });
 }
 
 // ------------------------------------------------------------------ forward DCT (jfdctint.c, islow) and quantisation
@@ -660,10 +630,6 @@ struct EncArgs {
   uint8_t* out;                  // compacted streams
   unsigned long long* out_off;   // [n]
   unsigned long long* sizes;     // [n]
-  // GainSrc only: channel sums of image i at csum + 3 * i, pixels per image, car (NULL or uint8[H][W][3], dense)
-  const unsigned long long* csum;
-  double npix;
-  const uint8_t* car;
   // restart intervals (rst > 0): nint per image; ilen / iofs [n * nint]: padded bits per interval and their exclusive
   // scan over the batch
   int rst;
@@ -700,26 +666,13 @@ __device__ inline unsigned long long image_bits(const EncArgs& a, int i) {
 }
 __device__ inline int header_len(const EncArgs& a, int i) { return a.hlen ? a.hlen[i] : a.hlen0; }
 
-// images whose blocks one CTA of k_jpeg_blocks can touch: the gain tables GainSrc needs per CTA
-__host__ __device__ inline int gain_images_per_cta(long long nblk, int n) {
-  const long long m = (kBlockThreads - 1) / nblk + 2;
-  return (int)(m < n ? m : n);
-}
-
-template <class Src, int HY, int VY>
+template <int HY, int VY>
 __global__ void __launch_bounds__(kBlockThreads) k_jpeg_blocks(EncArgs a) {
-  constexpr bool kGain = std::is_same<Src, GainSrc>::value;
   constexpr int NY = HY * VY, BPM = NY + 2;               // luma blocks and blocks per MCU
   __shared__ Tables st;
   __shared__ int sblk[kBlockThreads * kBlockPad];
-  extern __shared__ uint8_t sgain[];                      // GainSrc: [images this CTA touches][3][256]
   load_tables(&st, a.tabs);
   const long long b = (long long)blockIdx.x * kBlockThreads + threadIdx.x;
-  const int i0 = (int)((long long)blockIdx.x * kBlockThreads / a.nblk);
-  if constexpr (kGain) {
-    const long long last = min((long long)blockIdx.x * kBlockThreads + kBlockThreads, a.nblk * a.n) - 1;
-    for (int i = i0; i <= (int)(last / a.nblk); ++i) gain_table(a.csum + 3ll * i, a.npix, sgain + (i - i0) * 768);
-  }
   __syncthreads();
   if (b >= a.nblk * a.n) return;
   const int i = (int)(b / a.nblk);
@@ -735,8 +688,7 @@ __global__ void __launch_bounds__(kBlockThreads) k_jpeg_blocks(EncArgs a) {
     return;
   }
   int* d = sblk + threadIdx.x * kBlockPad;
-  if constexpr (kGain) load_block_s<HY, VY>(GainSrc{a.img + i * a.istride, a.pitch, sgain + (i - i0) * 768, a.car, 3ll * a.g.W}, a.g, mx, my, k, d);
-  else load_block_s<HY, VY>(PlainSrc{a.img + i * a.istride, a.pitch}, a.g, mx, my, k, d);
+  load_block_s<HY, VY>(a.img + i * a.istride, a.pitch, a.g, mx, my, k, d);
   fdct_islow(d);
   quantise(d, st.qdiv[t]);
   const uint8_t* zz = st.zz;

@@ -374,7 +374,7 @@ int bevk_undistort_stack_jpeg(bevk_ctx *ctx, int slot, const void *d_src, int64_
 /* ---- BEV canvases straight to JPEG ----------------------------------------------------------------------------------
  * BevGenerator.__call__ then cv2.imencode('.jpg', surround, [IMWRITE_JPEG_QUALITY, quality]) (surroundBEV.py:312-325,
  * :340): each canvas is rendered into library scratch and encoded on the device, and only the streams (byte-identical to
- * cv2's) cross PCIe.  With BEVK_FLAG_BALANCE the encoder applies colour balance and the car as it loads the raw canvas.
+ * cv2's) cross PCIe.  With BEVK_FLAG_BALANCE colour balance and the car are applied to the canvas before it is encoded.
  * Streams go back to back into host `out`, their sizes into sizes[batch], which is always filled for the whole batch.
  * Streams leave chunk by chunk, so when they need more than `capacity` bytes the call fails with BEVK_ERR_ARG after
  * `out` has received the whole streams of the leading frame-sets that fit; nothing is written at or past capacity.

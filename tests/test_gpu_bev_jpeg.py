@@ -2,7 +2,7 @@
 cuda_to_jpeg, BevGenerator.jpeg / jpeg_batch / jpeg_cuda): every stream must equal cv2.imencode of the oracle canvas
 byte for byte -- the reference's cv2 path on its own data, and the fuzz corpus of tests/bev_cases.py -- through the host
 chunk pipeline (chunk tails, pageable / page-locked / zero-copy frames, padded rows), device stacks and pointer tables,
-both fused kernels, BALANCE with colour balance and the car applied by the encoder, the capacity rule, quality clamping
+both fused kernels, BALANCE with colour balance and the car applied before the encoder, the capacity rule, quality clamping
 and the refusal inside a graph capture."""
 import ctypes
 import os
@@ -214,8 +214,9 @@ def test_cuda_to_jpeg_stack_table_and_gather(ops, torch):
                 want.check(e.cuda_to_jpeg(d, 95, car, balance), balance, True, 95, f"BEVK_JPEG_CHUNK {chunk}")
 
 
-def test_balance_encodes_without_k_gain(ops, torch):
-    """BALANCE to JPEG launches one kernel fewer than run_stack + ops.jpeg_encode (k_gain), with identical streams."""
+def test_balance_to_jpeg_launches_the_two_step_kernels(ops, torch):
+    """BALANCE to JPEG launches as many kernels as run_stack + ops.jpeg_encode (the render ending in k_gain, then the
+    encoder), with identical streams."""
     case = B.case_by_name("smooth4")
     e = _engine(ops, case)
     n, fb = 5, case.FW * case.FH * 3
@@ -233,11 +234,11 @@ def test_balance_encodes_without_k_gain(ops, torch):
     l0 = e.ctx.launches
     sep = two_calls()
     l1 = e.ctx.launches
-    fused = e.cuda_to_jpeg(d, 95, car, True)
+    one = e.cuda_to_jpeg(d, 95, car, True)
     l2 = e.ctx.launches
-    assert fused == sep
-    assert (l1 - l0) - (l2 - l1) == 1, (l1 - l0, l2 - l1)
-    Want(case).check(fused, True, True, 95, "fused gains")
+    assert one == sep
+    assert l1 - l0 == l2 - l1, (l1 - l0, l2 - l1)
+    Want(case).check(one, True, True, 95, "BALANCE to JPEG")
 
 
 @pytest.mark.parametrize("seed", range(B.N_CASES))

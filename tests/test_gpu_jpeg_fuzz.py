@@ -2,8 +2,8 @@
 cv2.imencode, byte for byte: the seeded corpus of tests/jpeg_cases.py through ops.jpeg_encode and bevk_jpeg_encode, one
 context reused across calls that change size, quality and batch, more than 2^32 entropy bits in one call,
 Undistorter.cuda_to_jpeg at every undistorted-width class mod 16 with the chunked pipeline at several chunk sizes, and
-BEV-to-JPEG with colour balance folded into the encoder (GainSrc) on canvases so small that one CTA's 128 blocks span
-up to 23 images.
+BEV-to-JPEG with colour balance (k_gain over the batch, then the encoder) on canvases so small that one CTA's 128
+blocks span up to 23 images.
 
 These run the device's decomposition of the work -- k_jpeg_dc's dummy-block DCs across MCUs, the batch-wide bit-offset
 scan, atomicOr on the words neighbouring blocks share, the pad written by each image's last block, 0xFF counts per
@@ -206,7 +206,7 @@ def test_undistorter_cuda_to_jpeg_chunks(torch, ops):
     print(f"{n_cmp} streams compared")
 
 
-# tiny canvases: 6, 12, 12 and 54 blocks, so that one CTA's 128 blocks touch up to 23 images (gain_images_per_cta)
+# tiny canvases: 6, 12, 12 and 54 blocks, so that one CTA's 128 blocks of k_jpeg_blocks touch up to 23 images
 _GAIN_CANVASES = (((16, 16), "local", 95), ((24, 16), "extreme", 100), ((17, 9), "local", 50), ((40, 40), "local", 75))
 
 
@@ -221,9 +221,10 @@ def _gain_case(i, BW, BH, kind, n_sets):
     return B.Case(f"gain{i}_{BW}x{BH}", kind, FW, FH, BW, BH, False, maps, masks, sets, car)
 
 
-def test_bev_to_jpeg_gain_source_tiny_canvases(torch, ops):
+def test_bev_to_jpeg_balance_tiny_canvases(torch, ops):
     """BALANCE, car on and off, batches 64 and 129, through BevEngine.cuda_to_jpeg (BEVK_JPEG_CHUNK 0 and the default
-    8) and run_to_jpeg: every stream equals cv2.imencode of the balanced canvas of the bev_cases oracle.  Frame-sets
+    8) and run_to_jpeg: k_gain over a batch of tiny canvases, then the encoder, whose CTAs span many of them.  Every
+    stream equals cv2.imencode of the balanced canvas of the bev_cases oracle.  Frame-sets
     whose balance is undefined (a zero channel mean) are skipped; most must be compared."""
     n_cmp = n_skip = 0
     for i, ((BW, BH), kind, q) in enumerate(_GAIN_CANVASES):

@@ -1,7 +1,7 @@
 """GPU test of the device JPEG encoder under cv2.imwrite's JPEG parameters (bevk_jpeg_set_params, params= of the Python
 wrappers): the seeded corpus of tests/jpeg_params_cases.py through ops.jpeg_encode (NumPy and CUDA input, padded and
 byte-offset layouts) and bevk_jpeg_encode, Undistorter.jpeg / cuda_to_jpeg with the chunked pipeline, and BevGenerator /
-BevEngine BEV-to-JPEG with and without BALANCE (GainSrc) and the car, under sampling factors, luma / chroma qualities,
+BevEngine BEV-to-JPEG with and without BALANCE (k_gain, then the encoder) and the car, under sampling factors, luma / chroma qualities,
 optimised tables and restart intervals -- every stream byte-identical to
 cv2.imencode(".jpg", img, [IMWRITE_JPEG_QUALITY, q] + params).  Also: the capacity error, params not leaking between
 wrapper calls on one context, and the refusals."""
@@ -219,11 +219,11 @@ def test_bevgenerator_jpeg_with_params(fx, balance):
     assert bev.jpeg(*F, car) == _cv2(canv["car"], 95)
 
 
-def test_gain_source_tiny_canvases_with_params(torch, ops):
+def test_balance_tiny_canvases_with_params(torch, ops):
     """BALANCE on 24x16 canvases (one CTA's 128 blocks span many images), batch 129, car on, through cuda_to_jpeg
     (BEVK_JPEG_CHUNK 0 and default) and run_to_jpeg, under 4:4:4, 4:1:1, luma / chroma qualities, and optimised tables
-    with and without one MCU per restart interval: GainSrc in the general MCU layouts, per-image tables over batches
-    of 129 images that each get their own."""
+    with and without one MCU per restart interval: k_gain over the tiny canvases, then the encoder in the general MCU
+    layouts, per-image tables over batches of 129 images that each get their own."""
     rng = np.random.default_rng(600)
     FW, FH, BW, BH = 64, 40, 24, 16
     maps = B._maps(rng, "extreme", 4, FW, FH, BW, BH)

@@ -10,7 +10,7 @@ balance), quality 95.  Per workload:
   device   frame-sets/s of BevEngine.cuda_to_jpeg on a device frame stack, in chunks of 8 canvases (the default: chunks
            that stay in the 50 MB L2) and the whole batch at once (BEVK_JPEG_CHUNK=0), against run_stack + ops.jpeg_encode
   d2h      bytes per frame-set that come back: the streams and their sizes, against the canvas
-  kernels  (balance only) kernel ms per step from torch.profiler: the fused-gain path against k_gain + the plain encoder
+  kernels  (balance only) kernel ms per step of cuda_to_jpeg from torch.profiler, and the kernels it launches
 Every stream is checked byte for byte against cv2.imencode of the canvas run() returns, and on the sample against the
 reference's cv2 path (``files_byte_identical``).
 
@@ -141,12 +141,7 @@ def _workload(name, w, iters, warmup, ref_sample, pool):
     res["h2d_bytes_per_frame_set"] = eng.host_copy_bytes(bal)[0]
 
     if bal:
-        fused_ms, fused_k = _kernel_ms(lambda: eng.cuda_to_jpeg(d, Q, car_d, True), 10)
-        sep_ms, sep_k = _kernel_ms(two_step, 10)
-        res["kernel_ms_per_step_fused_gain"] = fused_ms
-        res["kernel_ms_per_step_k_gain_plus_encoder"] = sep_ms
-        res["kernels_fused_gain"] = fused_k
-        res["kernels_k_gain_plus_encoder"] = sep_k
+        res["kernel_ms_per_step"], res["kernels"] = _kernel_ms(lambda: eng.cuda_to_jpeg(d, Q, car_d, True), 10)
     res["byte_identical_to_cv2"] = bool(identical)
     res["files_byte_identical"] = bool(files_identical)
     eng.ctx.close()
