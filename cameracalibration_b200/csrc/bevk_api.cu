@@ -25,6 +25,7 @@
 #include "bevk_plan_tma.cuh"
 #include "bevk_shard.cuh"
 #include "bevk_jpeg_enc.cuh"
+#include "bevk_jpeg_prog.cuh"
 #include "bevk_png_enc.cuh"
 
 #include <cub/device/device_scan.cuh>
@@ -236,6 +237,11 @@ struct bevk_ctx {
     cudaStream_t out_stream = nullptr;                      // D2H of the streams
     cudaEvent_t ev_sizes[2] = {nullptr, nullptr}, ev_out_free[2] = {nullptr, nullptr};
   } enc;
+  // progressive JPEG (bevk_jpeg_encode_params): work buffers of jpeg_prog_encode (bevk_jpeg_prog.cuh)
+  struct JpegProg {
+    DevBuf tabs, prefix, coef, desc, pe, pc, ph, jump, jump2, mark, rs, counts, codes, hdrs, hlen, bits, offs, ilen, iofs, ins,
+        insx, words, ffcnt, ffscan, out, meta, scan_tmp;
+  } prog;
   // PNG encoder (bevk_png_encode): the cv2.imwrite parameters of bevk_png_set_params and the work buffers of one group
   // of images (bevk_png_enc.cuh); every group's streams land compacted in `out`.
   struct PngEnc {
@@ -2328,7 +2334,8 @@ int bevk_jpeg_encode_bound(int width, int height, uint64_t* bytes) {
 }
 
 // A bevk_jpeg_set_params list: keys 2..7 of cv2.IMWRITE_JPEG_*, normalised by jpeg::normalise.  The streams the device
-// encoder writes are baseline and one scan: PROGRESSIVE asks for another entropy coder and is refused, not ignored.
+// encoder writes here are baseline and one scan: PROGRESSIVE asks for another entropy coder and is refused, not ignored
+// (the per-call bevk_jpeg_encode_params writes it).
 static int jpeg_params_check(const int* params, int n, jpeg::Opts* o) {
   if (n < 0 || (n & 1) || (n && !params)) return fail(BEVK_ERR_ARG, "JPEG params: %d ints, need (key, value) pairs", n);
   for (int i = 0; i < n; i += 2)
@@ -2621,6 +2628,204 @@ int bevk_jpeg_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, in
   JpegIn in;
   in.img = d_images; in.istride = image_stride; in.pitch = row_stride;
   return jpeg_encode_device(c, in, n, width, height, quality, out, capacity, sizes);
+}
+
+// ------------------------------------------------------------------ progressive JPEG and per-call JPEG params
+// A per-call list: keys 2..7, PROGRESSIVE and OPTIMIZE read as cv2 4.13 reads them (0 / 1), then jpeg::normalise.
+static int jpeg_call_params(const int* params, int n, std::vector<int>* list, jpeg::Opts* o) {
+  if (n < 0 || (n & 1) || (n && !params)) return fail(BEVK_ERR_ARG, "JPEG params: %d ints, need (key, value) pairs", n);
+  for (int i = 0; i < n; i += 2)
+    if (params[i] < jpeg::kProgressive || params[i] > jpeg::kSamplingFactor)
+      return fail(BEVK_ERR_ARG, "JPEG params: key %d (IMWRITE_JPEG_QUALITY is the quality argument of each call; "
+                  "keys are 2..7)", params[i]);
+  list->assign(params, params + n);
+  jpeg::prog::read_flags(list->data(), n);
+  jpeg::normalise(95, list->data(), n, o);
+  return BEVK_OK;
+}
+
+int bevk_jpeg_encode_params_bound(int width, int height, const int* params, int n, uint64_t* bytes) {
+  if (!bytes) return fail(BEVK_ERR_ARG, "null bytes");
+  if (width < 1 || height < 1 || width > jpeg::kMaxDim || height > jpeg::kMaxDim)
+    return fail(BEVK_ERR_ARG, "bad JPEG size %dx%d (1..%d)", width, height, jpeg::kMaxDim);
+  std::vector<int> list;
+  jpeg::Opts o;
+  RET(jpeg_call_params(params, n, &list, &o));
+  const jpeg::Geom g = jpeg::geom(width, height, o);
+  *bytes = o.progressive ? jpeg::prog::progressive_bound(g, o.rst) : jpeg::encode_bound(g, o);
+  return BEVK_OK;
+}
+
+// Progressive streams of n images: k_jpeg_blocks, then the k_jpeg_prog_* pipeline over every scan of every image at once
+// (bevk_jpeg_prog.cuh), then the streams to the host.  Synchronises.
+static int jpeg_prog_encode(bevk_ctx* c, const jpeg::Opts& o, const JpegIn& in, int n, int w, int h, uint8_t* out,
+                            uint64_t capacity, uint64_t* sizes) {
+  using namespace jpeg;
+  using namespace jpeg::prog;
+  auto& e = c->prog;
+  Tables t;
+  make_tables(o, &t);
+  uint8_t prefix[kPrefixBytes];
+  frame_prefix(w, h, o, prefix);
+  const Geom g = geom(w, h, o);
+  const Layout L = layout(g, o.rst);
+  const long long nblk = blocks_per_image(g), T = L.blk[kScans], S = L.seg[kScans];
+  const long long N = T * n, NS = S * n;
+  const long long words_img = ((long long)((prog::entropy_bound_bits(g, o.rst) + 31) / 32) + 3) & ~3ll;
+  const int chunks = (int)((words_img * 4 + kChunk - 1) / kChunk);
+  const long long nch = (long long)n * chunks;
+  if (N >= INT_MAX || NS >= INT_MAX || nch >= INT_MAX)
+    return fail(BEVK_ERR_ARG, "batch of %d %dx%d images is too large for one progressive call", n, w, h);
+  RET(e.tabs.ensure(sizeof(Tables)));
+  RET(e.prefix.ensure(kPrefixBytes));
+  RET(e.coef.ensure((size_t)(nblk * n) * 128));
+  RET(e.desc.ensure((size_t)N * 4));
+  RET(e.pe.ensure((size_t)N * 8));
+  RET(e.pc.ensure((size_t)N * 8));
+  RET(e.ph.ensure((size_t)N * 4));
+  RET(e.jump.ensure((size_t)(N + 1) * 4));
+  RET(e.jump2.ensure((size_t)(N + 1) * 4));
+  RET(e.mark.ensure((size_t)(N + 1)));
+  RET(e.rs.ensure((size_t)N * 4));
+  RET(e.counts.ensure((size_t)n * kTables * 256 * 4));
+  RET(e.codes.ensure((size_t)n * kTables * 256 * 4));
+  RET(e.hdrs.ensure((size_t)n * kScans * kHdrStride));
+  RET(e.hlen.ensure((size_t)n * kScans * 4));
+  RET(e.bits.ensure((size_t)N * 8));
+  RET(e.offs.ensure((size_t)N * 8));
+  RET(e.ilen.ensure((size_t)NS * 8));
+  RET(e.iofs.ensure((size_t)NS * 8));
+  RET(e.ins.ensure((size_t)NS * 4));
+  RET(e.insx.ensure((size_t)NS * 4));
+  RET(e.words.ensure((size_t)(n * words_img * 4)));
+  const size_t ffcap = e.ffcnt.cap;
+  RET(e.ffcnt.ensure((size_t)nch * 4));
+  if (e.ffcnt.cap != ffcap) CU(cudaMemsetAsync(e.ffcnt.p, 0, e.ffcnt.cap, c->stream));
+  RET(e.ffscan.ensure((size_t)nch * 4));
+  RET(e.out.ensure((size_t)n * progressive_bound(g, o.rst)));
+  RET(e.meta.ensure((size_t)n * 16));
+
+  ProgArgs a{};
+  a.n = n; a.rst = o.rst; a.g = g; a.nblk = nblk; a.L = L; a.T = T; a.S = S;
+  a.coef = e.coef.as<int16_t>(); a.desc = e.desc.as<uint32_t>(); a.pe = e.pe.as<unsigned long long>();
+  a.pc = e.pc.as<unsigned long long>(); a.ph = e.ph.as<unsigned>(); a.jump = e.jump.as<unsigned>(); a.jump2 = e.jump2.as<unsigned>();
+  a.mark = e.mark.as<uint8_t>(); a.rs = e.rs.as<unsigned>(); a.counts = e.counts.as<unsigned>(); a.codes = e.codes.as<uint32_t>();
+  a.hdrs = e.hdrs.as<uint8_t>(); a.hlen = e.hlen.as<int>(); a.bits = e.bits.as<unsigned long long>();
+  a.offs = e.offs.as<unsigned long long>(); a.ilen = e.ilen.as<unsigned long long>(); a.iofs = e.iofs.as<unsigned long long>();
+  a.ins = e.ins.as<unsigned>(); a.insx = e.insx.as<unsigned>(); a.words = e.words.as<uint32_t>(); a.words_img = words_img;
+  a.chunks_img = chunks; a.ffcnt = e.ffcnt.as<unsigned>(); a.ffscan = e.ffscan.as<unsigned>(); a.prefix = e.prefix.as<uint8_t>();
+  a.out = e.out.as<uint8_t>(); a.out_off = e.meta.as<unsigned long long>(); a.sizes = e.meta.as<unsigned long long>() + n;
+
+  using ItE = cub::TransformInputIterator<unsigned long long, DescE, const uint32_t*>;
+  using ItC = cub::TransformInputIterator<unsigned long long, DescC, const uint32_t*>;
+  using ItH = cub::TransformInputIterator<unsigned, DescH, const uint32_t*>;
+  using ItM = cub::TransformInputIterator<unsigned, MarkIndex, cub::CountingInputIterator<unsigned>>;
+  const ItM itm(cub::CountingInputIterator<unsigned>(0), MarkIndex{a.mark});
+  size_t tmp[8] = {};
+  CU(cub::DeviceScan::InclusiveSum(nullptr, tmp[0], ItE(a.desc, DescE()), a.pe, (int)N));
+  CU(cub::DeviceScan::InclusiveSum(nullptr, tmp[1], ItC(a.desc, DescC()), a.pc, (int)N));
+  CU(cub::DeviceScan::InclusiveSum(nullptr, tmp[2], ItH(a.desc, DescH()), a.ph, (int)N));
+  CU(cub::DeviceScan::InclusiveScan(nullptr, tmp[3], itm, a.rs, MaxU(), (int)N));
+  CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp[4], a.bits, a.offs, (int)N));
+  CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp[5], a.ilen, a.iofs, (int)NS));
+  CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp[6], a.ins, a.insx, (int)NS));
+  CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp[7], a.ffcnt, a.ffscan, (int)nch));
+  RET(e.scan_tmp.ensure(*std::max_element(tmp, tmp + 8)));
+  void* st = e.scan_tmp.p;
+
+  CU(cudaMemcpyAsync(e.tabs.p, &t, sizeof t, cudaMemcpyHostToDevice, c->stream));
+  CU(cudaMemcpyAsync(e.prefix.p, prefix, kPrefixBytes, cudaMemcpyHostToDevice, c->stream));
+  EncArgs b{};
+  b.img = reinterpret_cast<const uint8_t*>(in.img); b.istride = in.istride; b.pitch = in.pitch; b.n = n; b.g = g; b.nblk = nblk;
+  b.tabs = e.tabs.as<Tables>(); b.coef = e.coef.as<int16_t>(); b.bits = a.bits;   // k_jpeg_blocks' AC bit counts land in scratch
+  const unsigned gb = (unsigned)((nblk * n + kBlockThreads - 1) / kBlockThreads);
+  const unsigned gN = (unsigned)((N + 255) / 256), gN1 = (unsigned)((N + 1 + 255) / 256), gS = (unsigned)((NS + 255) / 256);
+  const unsigned gc = (unsigned)((nch + 255) / 256);
+  CU(cudaEventRecord(c->ev0, c->stream));
+  RET(with_sampling(o.hy, o.vy, [&](auto hy, auto vy) -> int {
+    k_jpeg_blocks<hy(), vy()><<<gb, kBlockThreads, 0, c->stream>>>(b);
+    LAUNCHED(c);
+    return BEVK_OK;
+  }));
+  k_jpeg_prog_desc<<<gN, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  k_jpeg_prog_hard<<<gN, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  CU(cub::DeviceScan::InclusiveSum(st, tmp[0], ItE(a.desc, DescE()), a.pe, (int)N, c->stream));
+  CU(cub::DeviceScan::InclusiveSum(st, tmp[1], ItC(a.desc, DescC()), a.pc, (int)N, c->stream));
+  CU(cub::DeviceScan::InclusiveSum(st, tmp[2], ItH(a.desc, DescH()), a.ph, (int)N, c->stream));
+  k_jpeg_prog_next<<<gN1, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  long long longest = 0;   // the longest scan bounds every chain of run starts
+  for (int s = 0; s < kScans; ++s) longest = std::max(longest, L.blk[s + 1] - L.blk[s]);
+  for (long long span = 1; span <= longest; span *= 2) {
+    k_jpeg_prog_jump<<<gN1, 256, 0, c->stream>>>(a.jump, a.jump2, a.mark, N);
+    LAUNCHED(c);
+    std::swap(a.jump, a.jump2);
+  }
+  CU(cub::DeviceScan::InclusiveScan(st, tmp[3], itm, a.rs, MaxU(), (int)N, c->stream));
+  CU(cudaMemsetAsync(a.counts, 0, (size_t)n * kTables * 256 * 4, c->stream));
+  k_jpeg_prog_count<<<gN, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  k_jpeg_prog_huff<<<(unsigned)((n + kProgHuffImages - 1) / kProgHuffImages), kProgHuffThreads, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  k_jpeg_prog_bits<<<gN, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  CU(cub::DeviceScan::ExclusiveSum(st, tmp[4], a.bits, a.offs, (int)N, c->stream));
+  k_jpeg_prog_segs<<<gS, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  CU(cub::DeviceScan::ExclusiveSum(st, tmp[5], a.ilen, a.iofs, (int)NS, c->stream));
+  CU(cub::DeviceScan::ExclusiveSum(st, tmp[6], a.ins, a.insx, (int)NS, c->stream));
+  k_jpeg_prog_zero<<<c->n_sm * 4, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  k_jpeg_prog_pack<<<gN, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  k_jpeg_prog_ffcount<<<gc, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  CU(cub::DeviceScan::ExclusiveSum(st, tmp[7], a.ffcnt, a.ffscan, (int)nch, c->stream));
+  k_jpeg_prog_layout<<<1, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  k_jpeg_prog_stuff<<<gc, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  CU(cudaEventRecord(c->ev1, c->stream));
+  c->timed = true;
+  std::vector<unsigned long long> hs((size_t)n);
+  CU(cudaMemcpyAsync(hs.data(), a.sizes, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  unsigned long long total = 0;
+  for (int i = 0; i < n; ++i) { sizes[i] = hs[(size_t)i]; total += hs[(size_t)i]; }
+  if (total > capacity) return capacity_error(n, sizes, capacity);
+  CU(cudaMemcpyAsync(out, a.out, total, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  return BEVK_OK;
+}
+
+int bevk_jpeg_encode_params(bevk_ctx* c, const int* params, int n_params, const void* d_images, int64_t image_stride,
+                            int64_t row_stride, int n, int width, int height, int quality, uint8_t* out, uint64_t capacity,
+                            uint64_t* sizes) {
+  NvtxRange nvtx_call("bevk_jpeg_encode_params (device images -> host JPEG streams)");
+  RET(use(c));
+  std::vector<int> list;
+  jpeg::Opts o;
+  RET(jpeg_call_params(params, n_params, &list, &o));
+  if (!d_images || !out || !sizes || n < 1) return fail(BEVK_ERR_ARG, "bad argument");
+  uint64_t bound = 0;
+  RET(bevk_jpeg_encode_bound(width, height, &bound));
+  if (row_stride < (int64_t)width * 3) return fail(BEVK_ERR_ARG, "row stride %lld < %d bytes", (long long)row_stride, width * 3);
+  if (n > 1 && image_stride < (int64_t)(height - 1) * row_stride + width * 3)
+    return fail(BEVK_ERR_ARG, "image stride %lld is smaller than one image", (long long)image_stride);
+  if (c->capturing) return fail(BEVK_ERR_ARG, "bevk_jpeg_encode_params synchronises and cannot be captured into a graph");
+  JpegIn in;
+  in.img = d_images; in.istride = image_stride; in.pitch = row_stride;
+  if (o.progressive) {
+    jpeg::normalise(quality, list.data(), n_params, &o);
+    return jpeg_prog_encode(c, o, in, n, width, height, out, capacity, sizes);
+  }
+  // baseline: the encoder of bevk_jpeg_encode under this list; the ctx's bevk_jpeg_set_params list is put back after
+  std::swap(c->enc.params, list);
+  const int r = jpeg_encode_device(c, in, n, width, height, quality, out, capacity, sizes);
+  std::swap(c->enc.params, list);
+  return r;
 }
 
 int bevk_undistort_jpeg(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int interp, int quality,

@@ -232,6 +232,45 @@ def jpeg_encode(images, quality: int = 95, ctx: L.Context | None = None, params=
     return res
 
 
+def jpeg_encode_params_bound(width: int, height: int, params=None) -> int:
+    """Largest JPEG stream jpeg_encode_params can produce for a width x height image under params."""
+    n = C.c_uint64()
+    arr, k = _jpeg_params(params)
+    L.check(L.load().bevk_jpeg_encode_params_bound(int(width), int(height), arr, k, C.byref(n)))
+    return n.value
+
+
+def jpeg_encode_params(images, params, quality: int = 95, ctx: L.Context | None = None) -> list[bytes]:
+    """cv2.imencode('.jpg', img, [cv2.IMWRITE_JPEG_QUALITY, quality] + params) on the GPU, byte for byte, with the
+    parameter list given per call (bevk_jpeg_encode_params): jpeg_encode's keys plus IMWRITE_JPEG_PROGRESSIVE, read as
+    cv2 4.13 reads it.  Takes the same images as jpeg_encode (NumPy, or CUDA arrays read in place on torch's current
+    stream); the ctx's jpeg_set_params list is left as it was.  Returns one ``bytes`` per image."""
+    ctx = ctx or L.default_context()
+    from .sharding import _torch_current_stream
+    keep = images
+    if not hasattr(images, "__cuda_array_interface__"):
+        a = np.asarray(images)
+        if a.dtype != np.uint8 or a.ndim not in (3, 4) or a.shape[-1] != 3:
+            raise L.BevkError(f"jpeg_encode_params takes uint8[H][W][3] or uint8[N][H][W][3] BGR images, got {a.dtype} {a.shape}")
+        import torch
+        keep = torch.from_numpy(np.ascontiguousarray(a)).to(torch.device("cuda", ctx.device))
+    ptr, n, h, w, img_stride, row_stride = _cuda_bgr_batch(keep)
+    if n < 1:
+        return []
+    cap = n * jpeg_encode_params_bound(w, h, params)
+    out = np.empty(cap, np.uint8)          # pages are only touched where streams land
+    sizes = (C.c_uint64 * n)()
+    arr, k = _jpeg_params(params)
+    with ctx.on_stream(_torch_current_stream(ctx.device)):
+        L.check(ctx.lib.bevk_jpeg_encode_params(ctx.h, arr, k, C.c_void_p(ptr), img_stride, row_stride, n, w, h, int(quality),
+                                                L.vptr(out), cap, sizes))
+    res, off = [], 0
+    for s in sizes:
+        res.append(out[off:off + s].tobytes())
+        off += s
+    return res
+
+
 def png_set_params(ctx: L.Context, params=None):
     """Apply cv2.imwrite's PNG (key, value) pairs (keys 16..20, cv2.IMWRITE_PNG_*) to ctx's PNG encoding; None or []
     restores cv2's defaults.  The list applies to bevk_png_encode; png_encode takes its own list per call."""

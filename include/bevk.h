@@ -347,7 +347,8 @@ int bevk_jpeg_encode_bound(int width, int height, uint64_t *bytes);
  *   CHROMA_QUALITY (6)   >= 0 and LUMA_QUALITY given: the chroma table's quality; luma != chroma forces 4:4:4
  *   OPTIMIZE (3)         != 0: per-image Huffman tables (libjpeg's jpeg_gen_optimal_table), built on the device
  *   RST_INTERVAL (4)     clamped to [0, 65535] MCUs; > 0 writes DRI and an RSTn marker after every interval but the last
- *   PROGRESSIVE (2)      0 as cv2's default; anything else is BEVK_ERR_UNSUPPORTED (a multi-scan coder)
+ *   PROGRESSIVE (2)      0 as cv2's default; anything else is BEVK_ERR_UNSUPPORTED here (a multi-scan coder: the
+ *                        per-call bevk_jpeg_encode_params below writes it)
  * QUALITY (1) is refused (every encoding call takes quality itself), as are other keys and odd n (BEVK_ERR_ARG).  A
  * refused list leaves the ctx's params as they were.  The streams are byte-identical to
  * cv2.imencode('.jpg', img, [IMWRITE_JPEG_QUALITY, quality] + params).                                               */
@@ -360,6 +361,21 @@ int bevk_jpeg_encode_bound_params(int width, int height, const int *params, int 
  * capacity bytes the call fails with BEVK_ERR_ARG, still fills sizes[], and writes nothing to out.                    */
 int bevk_jpeg_encode(bevk_ctx *ctx, const void *d_images, int64_t image_stride, int64_t row_stride, int n, int width, int height,
                      int quality, uint8_t *out, uint64_t capacity, uint64_t *sizes);
+/* bevk_jpeg_encode with the (key, value) list given per call, as cv2.imencode takes it: keys 2..7 as in
+ * bevk_jpeg_set_params (QUALITY stays the quality argument), with PROGRESSIVE and OPTIMIZE read as cv2 4.13 reads them
+ * (values below 0 act as 0, above 1 as 1).  PROGRESSIVE on writes libjpeg-turbo's progressive stream (SOF2, ten scans of
+ * spectral selection and successive approximation, Huffman tables optimised per scan; OPTIMIZE is implied) under the
+ * list's sampling, qualities and restart interval, byte-identical to cv2.imencode('.jpg', img,
+ * [IMWRITE_JPEG_QUALITY, quality] + params).  Other lists write what bevk_jpeg_encode writes under the same
+ * bevk_jpeg_set_params list.  The same contract as bevk_jpeg_encode (the call synchronises, sizes[] always filled,
+ * nothing written when the streams exceed capacity, not capturable, bevk_last_kernel_ms covers it); the ctx's
+ * bevk_jpeg_set_params list is neither read nor changed.  Progressive streams keep about 53 bytes of device scratch per
+ * block of each scan (about 5.3 scan blocks per 8x8 block at 4:2:0) besides 128 bytes per 8x8 block in the ctx.
+ * bevk_jpeg_encode_params_bound: the largest stream of a width x height image under `params` (the same list).         */
+int bevk_jpeg_encode_params(bevk_ctx *ctx, const int *params, int n_params, const void *d_images, int64_t image_stride,
+                            int64_t row_stride, int n, int width, int height, int quality, uint8_t *out, uint64_t capacity,
+                            uint64_t *sizes);
+int bevk_jpeg_encode_params_bound(int width, int height, const int *params, int n, uint64_t *bytes);
 /* bevk_undistort (3 channels) followed by the encoder: Tools/undistort.py:65-73 (imread'ed frame -> remap -> imwrite)
  * without the undistorted image ever leaving the device.  Works with map and fused slots; capacity as above.          */
 int bevk_undistort_jpeg(bevk_ctx *ctx, int slot, const uint8_t *src, int sw, int sh, int64_t sstride, int interp, int quality,
@@ -443,7 +459,7 @@ int bevk_graph_launch(bevk_ctx *ctx, int graph_id, int times);
 int bevk_graph_destroy(bevk_ctx *ctx, int graph_id);
 /* Kernel launches issued by this ctx since creation (bench "gpu_launches"). */
 int64_t bevk_launch_count(bevk_ctx *ctx);
-/* Milliseconds spent in the last bevk_bev_run_device, bevk_jpeg_encode or bevk_png_encode call's kernels, measured with
+/* Milliseconds spent in the last bevk_bev_run_device, bevk_jpeg_encode(_params) or bevk_png_encode call's kernels, measured with
  * CUDA events on the ctx stream (synchronises). */
 int bevk_last_kernel_ms(bevk_ctx *ctx, float *ms);
 
