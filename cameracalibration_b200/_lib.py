@@ -11,7 +11,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BEVK_LIB_PATH") or os.path.join(_HERE, "libbevk.so")   # BEVK_LIB_PATH: A/B builds
 
-INTER_NEAREST, INTER_LINEAR = 0, 1
+INTER_NEAREST, INTER_LINEAR, INTER_CUBIC, INTER_AREA, INTER_LANCZOS4 = 0, 1, 2, 3, 4   # cv2.INTER_*
 MAPS_UNDISTORT, MAPS_BEV = 0, 1
 MODEL_FISHEYE, MODEL_PINHOLE = 0, 1
 FLAG_BALANCE = 1
@@ -44,6 +44,8 @@ SIGNATURES = {
     "bevk_undistort": (C.c_int, [_p, C.c_int, _p, C.c_int, C.c_int, C.c_int64, C.c_int, _p, C.c_int, C.c_int, C.c_int64, C.c_int]),
     "bevk_undistort_stack": (C.c_int, [_p, C.c_int, _p, C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, _p, C.c_int64,
                                        C.c_int, C.c_int, C.c_int64, C.c_int]),
+    "bevk_undistort_stack_interp": (C.c_int, [_p, C.c_int, _p, C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, _p,
+                                              C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_int]),
     "bevk_undistort_last_path": (C.c_int, [_p]),
     "bevk_warp_perspective":(C.c_int, [_p, _p, C.c_int, C.c_int, C.c_int64, C.c_int, _dp, _p, C.c_int, C.c_int, C.c_int64, C.c_int]),
     "bevk_warp_maps": (C.c_int, [_p, _p, _p, C.c_int, C.c_int, _dp, C.c_int, C.c_int, _p, _p]),

@@ -155,6 +155,7 @@ struct bevk_ctx {
   long long launches = 0;
   DevBuf s_src, s_dst, s_m1, s_m2, s_o1, s_o2;   // scratch for the host-pointer entry points
   DevBuf s_xs;                                   // cm.xs of bevk_undistort_map and bevk_bev_set_camera
+  DevBuf d_wtab;                                 // INTER_CUBIC and INTER_LANCZOS4 weight tables (build_interp_tabs)
   Undistorter und[8];
   // BEV engine
   int n_cam = 0, FW = 0, FH = 0, BW = 0, BH = 0;
@@ -199,7 +200,8 @@ struct bevk_ctx {
   int tma_backoff_ns = 0;                   // BEVK_TMA_BACKOFF (read at finalize): producer poll interval when the ring is full
   int tma_grid[kMaxTmaConfigs][4] = {};                  // [config] resident CTAs of k_bev_tma<BAL, NB>: index = 2*BAL + {NB=1:0, 4:1}
   int last_path = 0;                        // 1: k_bev (global-offset gather), 2: k_bev_tma
-  int gather_path = 0;                      // stand-alone gathers: 4 = k_gather4 (word path), 1 = k_gather (byte path)
+  int gather_path = 0;                      // stand-alone gathers: 4 = k_gather4 (word path), 1 = k_gather (byte path),
+                                            // 2 = k_gather_taps (CUBIC / LANCZOS4)
   // multi-GPU sharding (bevk_shard_*): partition, slab geometry, NCCL communicator
   struct Shard {
     bool configured = false, geometry = false;
@@ -307,6 +309,23 @@ int bevk_ctx_create(int device, bevk_ctx** out) {
     return fail(BEVK_ERR_CUDA, "context setup: %s", cudaGetErrorString(e3));
   }
   c->stream = c->own;
+  // The weight tables of INTER_CUBIC / INTER_LANCZOS4 are uploaded here, so that the enqueue-only gathers
+  // (bevk_undistort_stack, also under graph capture) never allocate or copy.
+  static const std::vector<short> tabs = [] {
+    std::vector<short> t(INTERP_TAB_SHORTS);
+    build_interp_tabs(t.data());
+    return t;
+  }();
+  int r = c->d_wtab.ensure(tabs.size() * sizeof(short));
+  if (r == BEVK_OK) {
+    cudaError_t e4 = cudaMemcpyAsync(c->d_wtab.p, tabs.data(), tabs.size() * sizeof(short), cudaMemcpyHostToDevice, c->own);
+    if (e4 == cudaSuccess) e4 = cudaStreamSynchronize(c->own);
+    if (e4 != cudaSuccess) r = fail(BEVK_ERR_CUDA, "weight table upload: %s", cudaGetErrorString(e4));
+  }
+  if (r != BEVK_OK) {
+    delete c;
+    return r;
+  }
   *out = c;
   return BEVK_OK;
 }
@@ -414,6 +433,15 @@ static bool gather4_ok(const GatherArgs& a, int channels, int interp, int mode) 
          a.spitch < (1ll << 31) / std::max(1, a.sh) && (mode != 0 || a.map2 != nullptr);
 }
 
+// The interpolation flag of the image gathers: INTER_AREA is read as INTER_LINEAR, as cv2.remap and cv2.warpPerspective
+// read it; anything but NEAREST, LINEAR, CUBIC and LANCZOS4 is refused.
+static int gather_interp(int* interp) {
+  if (*interp == BEVK_INTER_AREA) *interp = BEVK_INTER_LINEAR;
+  if (*interp != BEVK_INTER_NEAREST && *interp != BEVK_INTER_LINEAR && *interp != BEVK_INTER_CUBIC && *interp != BEVK_INTER_LANCZOS4)
+    return fail(BEVK_ERR_UNSUPPORTED, "interp %d", *interp);
+  return BEVK_OK;
+}
+
 // Enqueue the gather of a.n >= 1 frames.  grid.z = frame groups of GATHER_NB, at most 65535 per launch; a single frame
 // takes k_gather4's single-frame form (NB = 1), which keeps the register count and speed of the one-frame kernel.
 template <int MODE>
@@ -436,15 +464,24 @@ static int launch_gather(bevk_ctx* c, const GatherArgs& a0, int channels, int in
     }
     const dim3 g((a.dw + 31) / 32, (a.dh + 7) / 8, gz);
 #define GO(C, L) k_gather<MODE, C, L><<<g, 256, 0, c->stream>>>(a)
-    if (interp == BEVK_INTER_LINEAR) {
+#define TAPS(C, KS) k_gather_taps<MODE, C, KS><<<g, 256, 0, c->stream>>>(a, wt)
+    if (interp == BEVK_INTER_CUBIC || interp == BEVK_INTER_LANCZOS4) {
+      const short* wt = c->d_wtab.as<short>() + (interp == BEVK_INTER_CUBIC ? 0 : INTERP_TAB_LANCZOS4);
+      if (interp == BEVK_INTER_CUBIC) {
+        if (channels == 1) TAPS(1, 4); else if (channels == 3) TAPS(3, 4); else TAPS(4, 4);
+      } else {
+        if (channels == 1) TAPS(1, 8); else if (channels == 3) TAPS(3, 8); else TAPS(4, 8);
+      }
+    } else if (interp == BEVK_INTER_LINEAR) {
       if (channels == 1) GO(1, 1); else if (channels == 3) GO(3, 1); else GO(4, 1);
     } else {
       if (channels == 1) GO(1, 0); else if (channels == 3) GO(3, 0); else GO(4, 0);
     }
 #undef GO
+#undef TAPS
     LAUNCHED(c);
   }
-  c->gather_path = words ? 4 : 1;
+  c->gather_path = words ? 4 : (interp == BEVK_INTER_CUBIC || interp == BEVK_INTER_LANCZOS4) ? 2 : 1;
   return BEVK_OK;
 }
 
@@ -477,8 +514,8 @@ int bevk_remap(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride,
   RET(check_image(src, sw, sh, sstride, channels, "src"));
   RET(check_image(dst, dw, dh, dstride, channels, "dst"));
   if (!map1) return fail(BEVK_ERR_ARG, "null map1");
-  if (interp == BEVK_INTER_LINEAR && !map2) return fail(BEVK_ERR_ARG, "INTER_LINEAR needs map2");
-  if (interp != BEVK_INTER_LINEAR && interp != BEVK_INTER_NEAREST) return fail(BEVK_ERR_UNSUPPORTED, "interp %d", interp);
+  RET(gather_interp(&interp));
+  if (interp != BEVK_INTER_NEAREST && !map2) return fail(BEVK_ERR_ARG, "interpolation %d needs map2", interp);
   const size_t n = (size_t)dw * dh;
   RET(upload_image(c, c->s_src, src, sw, sh, sstride, channels));
   RET(c->s_m1.ensure(n * 4));
@@ -552,7 +589,7 @@ static int undistort_to_scratch(bevk_ctx* c, int slot, const uint8_t* src, int s
   Undistorter& u = c->und[slot];
   const int dw = u.cm.w, dh = u.cm.h;
   RET(check_image(src, sw, sh, sstride, channels, "src"));
-  if (interp != BEVK_INTER_LINEAR && interp != BEVK_INTER_NEAREST) return fail(BEVK_ERR_UNSUPPORTED, "interp %d", interp);
+  RET(gather_interp(&interp));
   RET(upload_image(c, c->s_src, src, sw, sh, sstride, channels));
   RET(c->s_dst.ensure((size_t)dw * dh * channels));
   GatherArgs a{};
@@ -582,13 +619,13 @@ int bevk_undistort(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, in
 }
 
 // ------------------------------------------------------------------ undistortion of device frame batches
-// Checks the source side of the bevk_undistort_stack calls and fills a (slot's map or model, n frames of the source);
+// Checks the source side of the bevk_undistort_stack calls (and normalises *interp) and fills a (slot's map or model, n frames of the source);
 // the destination is left to the caller.  An image stride only matters when n > 1.
 static int stack_src_args(bevk_ctx* c, int slot, const void* d_src, int64_t sis, int sw, int sh, int64_t srs, int channels, int n,
-                          int interp, GatherArgs* a) {
+                          int* interp, GatherArgs* a) {
   RET(need_undistorter(c, slot));
   if (n < 1) return fail(BEVK_ERR_ARG, "n must be >= 1, got %d", n);
-  if (interp != BEVK_INTER_LINEAR && interp != BEVK_INTER_NEAREST) return fail(BEVK_ERR_UNSUPPORTED, "interp %d", interp);
+  RET(gather_interp(interp));
   RET(check_image(d_src, sw, sh, srs, channels, "src"));
   if (n > 1 && sis < (int64_t)(sh - 1) * srs + (int64_t)sw * channels)
     return fail(BEVK_ERR_ARG, "src image stride %lld is smaller than one image", (long long)sis);
@@ -606,12 +643,12 @@ static int launch_undistort(bevk_ctx* c, int slot, const GatherArgs& a, int chan
   return c->und[slot].fused ? launch_gather<1>(c, a, channels, interp) : launch_gather<0>(c, a, channels, interp);
 }
 
-int bevk_undistort_stack(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
-                         int channels, int n, void* d_dst, int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride,
-                         int interp) {
-  RET(use(c));
+// bevk_undistort_stack_interp: any interpolation gather_interp takes.
+static int undistort_stack(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
+                           int channels, int n, void* d_dst, int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride,
+                           int interp) {
   GatherArgs a;
-  RET(stack_src_args(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, interp, &a));
+  RET(stack_src_args(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, &interp, &a));
   if (dw != a.dw || dh != a.dh)   // the caller sized dst for another map: never write past it
     return fail(BEVK_ERR_ARG, "undistorter slot %d holds a %dx%d map, the caller expects %dx%d", slot, a.dw, a.dh, dw, dh);
   RET(check_image(d_dst, dw, dh, dst_row_stride, channels, "dst"));
@@ -627,6 +664,26 @@ int bevk_undistort_stack(bevk_ctx* c, int slot, const void* d_src, int64_t src_i
   return launch_undistort(c, slot, a, channels, interp);
 }
 
+int bevk_undistort_stack(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
+                         int channels, int n, void* d_dst, int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride,
+                         int interp) {
+  RET(use(c));
+  // this entry point's contract: INTER_NEAREST and INTER_LINEAR, every other value refused
+  if (interp != BEVK_INTER_LINEAR && interp != BEVK_INTER_NEAREST)
+    return fail(BEVK_ERR_UNSUPPORTED, "interp %d: bevk_undistort_stack takes INTER_NEAREST and INTER_LINEAR, "
+                "bevk_undistort_stack_interp every cv2 flag", interp);
+  return undistort_stack(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
+                         dst_row_stride, interp);
+}
+
+int bevk_undistort_stack_interp(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh,
+                                int64_t src_row_stride, int channels, int n, void* d_dst, int64_t dst_image_stride, int dw, int dh,
+                                int64_t dst_row_stride, int interp) {
+  RET(use(c));
+  return undistort_stack(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
+                         dst_row_stride, interp);
+}
+
 int bevk_undistort_last_path(bevk_ctx* c) { return c ? c->gather_path : 0; }
 
 // ------------------------------------------------------------------ K4 / K2
@@ -635,7 +692,7 @@ int bevk_warp_perspective(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64
   RET(use(c));
   RET(check_image(src, sw, sh, sstride, channels, "src"));
   RET(check_image(dst, dw, dh, dstride, channels, "dst"));
-  if (interp != BEVK_INTER_LINEAR && interp != BEVK_INTER_NEAREST) return fail(BEVK_ERR_UNSUPPORTED, "interp %d", interp);
+  RET(gather_interp(&interp));
   GatherArgs a{};
   a.n = 1;
   RET(make_homog(H, &a.hm));
@@ -2853,7 +2910,7 @@ int bevk_undistort_stack_jpeg(bevk_ctx* c, int slot, const void* d_src, int64_t 
   if (!out || !sizes) return fail(BEVK_ERR_ARG, "null host pointer");
   if (c->capturing) return fail(BEVK_ERR_ARG, "bevk_undistort_stack_jpeg synchronises and cannot be captured into a graph");
   GatherArgs a;
-  RET(stack_src_args(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, 3, n, interp, &a));
+  RET(stack_src_args(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, 3, n, &interp, &a));
   const int dw = a.dw, dh = a.dh;
   uint64_t bound = 0;
   RET(bevk_jpeg_encode_bound(dw, dh, &bound));

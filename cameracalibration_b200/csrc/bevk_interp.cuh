@@ -1,0 +1,135 @@
+// bevk_interp.cuh -- cv2.remap's INTER_CUBIC and INTER_LANCZOS4 for 8-bit images (OpenCV 4.13, CV_16SC2 + CV_16UC1
+// maps, BORDER_CONSTANT 0): the fixed-point weight tables and the per-pixel tap sum, shared by the device gathers
+// (k_gather_taps) and the host harness tests/host/remap_interp.cu.  DESIGN.md section 2 has the arithmetic.
+#pragma once
+#include <float.h>
+#include <math.h>
+#include <string.h>
+
+#include "bevk_device.cuh"
+
+namespace bevk {
+
+constexpr int INTER_TAB_SIZE2 = TAB * TAB;   // weight rows, indexed by map2 = fy * 32 + fx
+constexpr int COEF_BITS = 15;                // INTER_REMAP_COEF_BITS: the weights of a row sum to 1 << 15
+
+// ---- OpenCV's 1-D kernels (imgwarp.cpp interpolateCubic / interpolateLanczos4) at x = i / 32, i in 0..31.
+// OpenCV's baseline x86-64 unit has no FMA, so every float and double operation is rounded on its own: the host forms
+// of fmul / fadd / fsub / dmul / dadd / ddiv go through volatile stores, which no -ffp-contract or -march setting in
+// BEVK_NVCC_FLAGS can fuse.  sin / cos are the host libm's, the library cv2 itself calls (DESIGN.md section 2).
+inline void cubic_coeffs(float x, float* c) {
+  const float A = -0.75f;   // 5A, 8A, 4A, A + 2, A + 3 are exact
+  const float x1 = fadd(x, 1.f), xm = fsub(1.f, x);
+  c[0] = fsub(fmul(fadd(fmul(fsub(fmul(A, x1), 5 * A), x1), 8 * A), x1), 4 * A);
+  c[1] = fadd(fmul(fmul(fsub(fmul(A + 2, x), A + 3), x), x), 1.f);
+  c[2] = fadd(fmul(fmul(fsub(fmul(A + 2, xm), A + 3), xm), xm), 1.f);
+  c[3] = fsub(fsub(fsub(1.f, c[0]), c[1]), c[2]);
+}
+
+inline void lanczos4_coeffs(float x, float* c) {
+  if (x < FLT_EPSILON) {
+    for (int i = 0; i < 8; ++i) c[i] = 0.f;
+    c[3] = 1.f;
+    return;
+  }
+  const double s45 = 0.70710678118654752440084436210485, pi = 3.141592653589793238462643383279502884;
+  static const double cs[8][2] = {{1, 0}, {-s45, -s45}, {0, 1}, {s45, -s45}, {-1, 0}, {s45, s45}, {0, -1}, {-s45, s45}};
+  const double y0 = dmul(dmul((double)-fadd(x, 3.f), pi), 0.25), s0 = sin(y0), c0 = cos(y0);
+  float sum = 0.f;
+  for (int i = 0; i < 8; ++i) {
+    const double y = dmul(dmul((double)-fsub(fadd(x, 3.f), (float)i), pi), 0.25);
+    c[i] = (float)ddiv(dadd(dmul(cs[i][0], s0), dmul(cs[i][1], c0)), dmul(y, y));
+    sum = fadd(sum, c[i]);
+  }
+  volatile float inv = 1.f / sum;
+  for (int i = 0; i < 8; ++i) c[i] = fmul(c[i], inv);
+}
+
+// ---- initInterTab2D for 8-bit images: tab[(fy * 32 + fx) * KS * KS + k1 * KS + k2] = round(vy[k1] * vx[k2] * 2^15) as
+// int16, then each row forced to sum to 2^15.  OpenCV looks for the row's least and greatest weight in rows and columns
+// [KS/2, KS/2 + 2) -- not the central 2x2 -- starting from entry (KS/2, KS/2); a surplus comes off the least one, a
+// deficit goes onto the greatest.  KS = 4: cubic, 8: Lanczos4.
+template <int KS>
+inline void build_interp_tab(short* tab) {
+  float k1d[TAB][KS];
+  for (int i = 0; i < TAB; ++i) {
+    const float x = (float)i * (1.f / TAB);
+    if (KS == 4) cubic_coeffs(x, k1d[i]);
+    else lanczos4_coeffs(x, k1d[i]);
+  }
+  for (int fy = 0; fy < TAB; ++fy)
+    for (int fx = 0; fx < TAB; ++fx) {
+      short* t = tab + (fy * TAB + fx) * KS * KS;
+      int isum = 0;
+      for (int k1 = 0; k1 < KS; ++k1)
+        for (int k2 = 0; k2 < KS; ++k2) {
+          const float v = fmul(fmul(k1d[fy][k1], k1d[fx][k2]), (float)(1 << COEF_BITS));
+          isum += t[k1 * KS + k2] = (short)max(-32768, min(32767, f2i_rn(v)));
+        }
+      const int diff = isum - (1 << COEF_BITS);
+      if (diff == 0) continue;
+      const int h = KS / 2;
+      int mk1 = h, mk2 = h, Mk1 = h, Mk2 = h;
+      for (int k1 = h; k1 < h + 2; ++k1)
+        for (int k2 = h; k2 < h + 2; ++k2) {
+          if (t[k1 * KS + k2] < t[mk1 * KS + mk2]) mk1 = k1, mk2 = k2;
+          else if (t[k1 * KS + k2] > t[Mk1 * KS + Mk2]) Mk1 = k1, Mk2 = k2;
+        }
+      if (diff < 0) t[Mk1 * KS + Mk2] = (short)(t[Mk1 * KS + Mk2] - diff);
+      else t[mk1 * KS + mk2] = (short)(t[mk1 * KS + mk2] - diff);
+    }
+}
+
+// Both tables back to back, as the library uploads them: cubic (1024 rows of 16) at 0, Lanczos4 (1024 rows of 64) at
+// INTERP_TAB_LANCZOS4.
+constexpr int INTERP_TAB_LANCZOS4 = INTER_TAB_SIZE2 * 16;
+constexpr int INTERP_TAB_SHORTS = INTERP_TAB_LANCZOS4 + INTER_TAB_SIZE2 * 64;
+inline void build_interp_tabs(short* tabs) {
+  build_interp_tab<4>(tabs);
+  build_interp_tab<8>(tabs + INTERP_TAB_LANCZOS4);
+}
+
+__host__ __device__ __forceinline__ int tap8(const uint8_t* p) {
+#ifdef __CUDA_ARCH__
+  return __ldg(p);
+#else
+  return *p;
+#endif
+}
+
+// ---- one output pixel of a KS x KS kernel (remapBicubic / remapLanczos4).  (sx, sy): the window's top-left tap, map1 -
+// (KS/2 - 1) in int, so the int16 extremes do not wrap; w: the fraction class's row of weights, k1 * KS + k2.
+// A tap outside the source adds nothing (OpenCV's BORDER_CONSTANT sum is cval * 2^15 + sum (S - cval) w with cval 0, and
+// a window wholly outside is cval); windows wholly inside take OpenCV's fast-path test and read without checks.
+template <int KS, int C>
+__host__ __device__ __forceinline__ void taps_px(const uint8_t* __restrict__ src, long long spitch, int sw, int sh, int sx,
+                                                 int sy, const short (&w)[KS * KS], uint8_t* __restrict__ o) {
+  int sum[C];
+#pragma unroll
+  for (int c = 0; c < C; ++c) sum[c] = 0;
+  if ((unsigned)sx < (unsigned)max(sw - (KS - 1), 0) && (unsigned)sy < (unsigned)max(sh - (KS - 1), 0)) {
+    const uint8_t* q = src + (long long)sy * spitch + (long long)sx * C;
+#pragma unroll
+    for (int k1 = 0; k1 < KS; ++k1, q += spitch)
+#pragma unroll
+      for (int k2 = 0; k2 < KS; ++k2)
+#pragma unroll
+        for (int c = 0; c < C; ++c) sum[c] += tap8(q + k2 * C + c) * w[k1 * KS + k2];
+  } else if (sx < sw && sx + KS > 0 && sy < sh && sy + KS > 0) {
+#pragma unroll
+    for (int k1 = 0; k1 < KS; ++k1) {
+      if ((unsigned)(sy + k1) >= (unsigned)sh) continue;
+      const uint8_t* q = src + (long long)(sy + k1) * spitch;
+#pragma unroll
+      for (int k2 = 0; k2 < KS; ++k2) {
+        if ((unsigned)(sx + k2) >= (unsigned)sw) continue;
+#pragma unroll
+        for (int c = 0; c < C; ++c) sum[c] += tap8(q + (long long)(sx + k2) * C + c) * w[k1 * KS + k2];
+      }
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < C; ++c) o[c] = (uint8_t)max(0, min(255, (sum[c] + (1 << (COEF_BITS - 1))) >> COEF_BITS));
+}
+
+}  // namespace bevk

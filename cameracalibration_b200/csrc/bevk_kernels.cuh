@@ -2,6 +2,7 @@
 //
 //   k_undistort_map   K1  cv2.fisheye.initUndistortRectifyMap / cv2.initUndistortRectifyMap
 //   k_gather          K3/K4  cv2.remap, fused undistort (no map), cv2.warpPerspective on images
+//   k_gather_taps     K3/K4  the same with INTER_CUBIC / INTER_LANCZOS4
 //   k_warp_maps       K2  cv2.warpPerspective on the 16SC2/16UC1 map planes (BEV LUT build),
 //                         optionally fused with K1 so the full-size undistort map never exists
 //   k_blend_masks     K10 BlendMask.get_blend_mask
@@ -11,6 +12,7 @@
 //   k_sat_sum         multi-GPU compose of per-camera partial canvases
 #pragma once
 #include "bevk_device.cuh"
+#include "bevk_interp.cuh"
 
 namespace bevk {
 
@@ -136,6 +138,64 @@ __global__ void __launch_bounds__(256) k_gather(GatherArgs a) {
   const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= a.dw || y >= a.dh) return;
   gather_frames<MODE, C, LINEAR>(a, x, y, blockIdx.z * GATHER_NB);
+}
+
+// K3 / K4 with INTER_CUBIC (KS = 4) and INTER_LANCZOS4 (KS = 8): the source position is INTER_LINEAR's (map entry, camera
+// model, or warp_point at TAB scale), the map2 value picks a row of KS * KS int16 weights from wtab (bevk_interp.cuh,
+// 32 or 128 bytes read once per pixel through the read-only path), and the row and window serve up to GATHER_NB frames.
+// Host-capable, like gather_frames (tests/host/remap_interp.cu).
+template <int MODE, int C, int KS>
+__host__ __device__ __forceinline__ void gather_taps_frames(const GatherArgs& a, const short* __restrict__ wtab, int x, int y,
+                                                            int f0) {
+  int sx, sy;
+  unsigned fr;
+  if (MODE == 2) {
+    int X, Y;
+    warp_point(a.hm, x, y, (double)TAB, X, Y);
+    sx = sat_i16(X >> INTER_BITS); sy = sat_i16(Y >> INTER_BITS);
+    fr = (unsigned)((Y & (TAB - 1)) * TAB + (X & (TAB - 1)));
+  } else {
+    short mx, my;
+    unsigned short f;
+    if (MODE == 0) {
+      const size_t i = (size_t)y * a.dw + x;
+      const short2 m = a.map1[i];
+      mx = m.x; my = m.y;
+      f = a.map2[i];
+    } else {
+      double u, v;
+      undistort_point(a.cm, x, y, u, v);
+      quantise_uv(u, v, mx, my, f, pack_saturates(a.cm.model, x, a.cm.w));
+    }
+    sx = mx; sy = my;
+    fr = f & (INTER_TAB_SIZE2 - 1);
+  }
+  sx -= KS / 2 - 1; sy -= KS / 2 - 1;
+  short w[KS * KS];
+#ifdef __CUDA_ARCH__
+  const uint4* wr = reinterpret_cast<const uint4*>(wtab + fr * (KS * KS));
+#pragma unroll
+  for (int i = 0; i < KS * KS / 8; ++i) {
+    const uint4 q = __ldg(wr + i);
+    const unsigned u[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) { w[8 * i + 2 * k] = (short)(u[k] & 0xffffu); w[8 * i + 2 * k + 1] = (short)(u[k] >> 16); }
+  }
+#else
+  memcpy(w, wtab + fr * (KS * KS), sizeof w);
+#endif
+  const int nf = a.n - f0 < GATHER_NB ? a.n - f0 : GATHER_NB;
+  const uint8_t* s = a.src + (long long)f0 * a.sistride;
+  uint8_t* o = a.dst + (long long)f0 * a.distride + (long long)y * a.dpitch + (long long)x * C;
+  for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) taps_px<KS, C>(s, a.spitch, a.sw, a.sh, sx, sy, w, o);
+}
+
+template <int MODE, int C, int KS>
+__global__ void __launch_bounds__(256) k_gather_taps(GatherArgs a, const short* __restrict__ wtab) {
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31);
+  const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x >= a.dw || y >= a.dh) return;
+  gather_taps_frames<MODE, C, KS>(a, wtab, x, y, blockIdx.z * GATHER_NB);
 }
 
 // ---------------------------------------------------------------------------------

@@ -9,12 +9,15 @@ import numpy as np
 
 from . import _lib as L
 
-INTER_NEAREST, INTER_LINEAR = L.INTER_NEAREST, L.INTER_LINEAR
+INTER_NEAREST, INTER_LINEAR, INTER_CUBIC, INTER_AREA, INTER_LANCZOS4 = (
+    L.INTER_NEAREST, L.INTER_LINEAR, L.INTER_CUBIC, L.INTER_AREA, L.INTER_LANCZOS4)
+_INTERPOLATIONS = (INTER_NEAREST, INTER_LINEAR, INTER_CUBIC, INTER_AREA, INTER_LANCZOS4)
 
 
 def _interp(flag: int) -> int:
-    if flag not in (INTER_NEAREST, INTER_LINEAR):
-        raise L.BevkError(f"interpolation {flag} is not supported (INTER_NEAREST / INTER_LINEAR only)")
+    if flag not in _INTERPOLATIONS:
+        raise L.BevkError(f"interpolation {flag} is not supported (cv2's INTER_NEAREST, _LINEAR, _CUBIC, _AREA or "
+                          "_LANCZOS4)")
     return flag
 
 
@@ -323,7 +326,9 @@ def png_encode(images, ctx: L.Context | None = None, params=None) -> list[bytes]
 
 def remap(src: np.ndarray, map1: np.ndarray, map2: np.ndarray | None, interpolation: int = INTER_LINEAR,
           ctx: L.Context | None = None, out: np.ndarray | None = None) -> np.ndarray:
-    """cv2.remap with CV_16SC2 (+CV_16UC1) maps, BORDER_CONSTANT 0."""
+    """cv2.remap with CV_16SC2 (+CV_16UC1) maps, BORDER_CONSTANT 0.  interpolation: INTER_NEAREST, INTER_LINEAR,
+    INTER_CUBIC, INTER_AREA (read as INTER_LINEAR, as cv2.remap reads it) or INTER_LANCZOS4; all but NEAREST need map2.
+    The result is byte-identical to cv2.remap's."""
     ctx = ctx or L.default_context()
     img, sw, sh, ss, ch = L.image_view(src)
     m1 = np.ascontiguousarray(map1, np.int16)
@@ -341,7 +346,8 @@ def remap(src: np.ndarray, map1: np.ndarray, map2: np.ndarray | None, interpolat
 
 def warp_perspective(src: np.ndarray, H, dsize, flags: int = INTER_LINEAR, ctx: L.Context | None = None,
                      out: np.ndarray | None = None):
-    """cv2.warpPerspective(src, H, dsize, flags) for uint8 images, BORDER_CONSTANT 0."""
+    """cv2.warpPerspective(src, H, dsize, flags) for uint8 images, BORDER_CONSTANT 0.  flags: INTER_NEAREST,
+    INTER_LINEAR, INTER_CUBIC, INTER_AREA (read as INTER_LINEAR, as cv2 reads it) or INTER_LANCZOS4."""
     ctx = ctx or L.default_context()
     img, sw, sh, ss, ch = L.image_view(src)
     dw, dh = int(dsize[0]), int(dsize[1])
@@ -461,7 +467,7 @@ class Undistorter:
         return m1, m2
 
     def __call__(self, src: np.ndarray, interpolation: int = INTER_LINEAR, out: np.ndarray | None = None) -> np.ndarray:
-        """cv2.remap(src, map1, map2, interpolation).  A CUDA array (e.g. a torch tensor on the GPU) goes to cuda() and
+        """cv2.remap(src, map1, map2, interpolation), any of remap()'s interpolations.  A CUDA array (e.g. a torch tensor on the GPU) goes to cuda() and
         the result stays on the device; NumPy input is uploaded, undistorted and downloaded in one call."""
         if hasattr(src, "__cuda_array_interface__"):
             return self.cuda(src, out=out, interpolation=interpolation)
@@ -475,7 +481,7 @@ class Undistorter:
     def jpeg(self, src: np.ndarray, quality: int = 95, interpolation: int = INTER_LINEAR, params=None) -> bytes:
         """The undistorted image as the bytes cv2.imwrite(path, self(src), [IMWRITE_JPEG_QUALITY, quality] + params)
         writes to a .jpg file; the image itself never leaves the GPU.  src: uint8[h][w][3] BGR.  params: cv2.imwrite's
-        other JPEG pairs (see jpeg_encode), None for cv2's defaults."""
+        other JPEG pairs (see jpeg_encode), None for cv2's defaults.  interpolation: as for __call__."""
         self._live()
         img, sw, sh, ss, ch = L.image_view(src)
         if ch != 3 or src.ndim != 3:
@@ -492,7 +498,7 @@ class Undistorter:
     def png(self, src: np.ndarray, params=None, interpolation: int = INTER_LINEAR) -> bytes:
         """The undistorted image as the bytes cv2.imwrite(path, self(src), params) writes to a .png file: undistorted
         and encoded on the device (png_encode's params, e.g. [IMWRITE_PNG_COMPRESSION, 9]), only the stream comes back.
-        src: uint8[h][w][3] BGR."""
+        src: uint8[h][w][3] BGR.  interpolation: as for __call__."""
         self._live()
         a = np.asarray(src)
         if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
@@ -507,7 +513,8 @@ class Undistorter:
         frames: a uint8 CUDA array (``__cuda_array_interface__``) [H][W] (one grey image), [H][W][C] (one image) or
         [N][H][W][C] (a batch; a grey batch is [N][H][W][1]), C in 1, 3, 4.  Pixels must be dense; rows and images may
         be padded.  ``out``: a CUDA array of the matching shape (rows and images may be padded too), default a new torch
-        tensor.  Each output pixel's map entry (or camera model) is read once for several frames of the batch.  Runs on
+        tensor.  ``interpolation``: as for __call__.  Each output pixel's map entry (or camera model) and, for INTER_CUBIC /
+        INTER_LANCZOS4, its row of weights are read once for several frames of the batch.  Runs on
         ``stream`` (a raw CUDA stream handle), default torch's current stream, and only enqueues.  Returns ``out``."""
         self._live()
         ptr, rank, n, sh, sw, ch, simg, srow = _cuda_images(frames, "frames")
@@ -522,14 +529,14 @@ class Undistorter:
             from .sharding import _torch_current_stream
             stream = _torch_current_stream(self.ctx.device)
         with self.ctx.on_stream(stream):
-            L.check(self.ctx.lib.bevk_undistort_stack(self.ctx.h, self.slot, C.c_void_p(ptr), simg, sw, sh, srow, ch, n,
-                                                      C.c_void_p(optr), oimg, self.w, self.h, orow, _interp(interpolation)))
+            L.check(self.ctx.lib.bevk_undistort_stack_interp(self.ctx.h, self.slot, C.c_void_p(ptr), simg, sw, sh, srow, ch, n,
+                                                             C.c_void_p(optr), oimg, self.w, self.h, orow, _interp(interpolation)))
         return out
 
     def cuda_to_jpeg(self, frames, quality: int = 95, interpolation: int = INTER_LINEAR, params=None) -> list[bytes]:
         """cuda() followed by cv2.imencode('.jpg', img, [IMWRITE_JPEG_QUALITY, quality] + params) per frame, with the
         encoder on the GPU: the undistorted images stay in library scratch and only the JPEG streams come back.  frames:
-        a uint8 CUDA array [H][W][3] or [N][H][W][3] (BGR) laid out as cuda() takes it.  params as in jpeg().  Runs on
+        a uint8 CUDA array [H][W][3] or [N][H][W][3] (BGR) laid out as cuda() takes it.  params and interpolation as in jpeg().  Runs on
         torch's current stream and synchronises.  Returns one ``bytes`` per frame, byte-identical to cv2's."""
         self._live()
         ptr, rank, n, sh, sw, ch, simg, srow = _cuda_images(frames, "frames")
@@ -545,8 +552,9 @@ class Undistorter:
         return BevEngine._split(out, sizes)
 
     def last_path(self) -> str:
-        """Which gather the last call of this ctx launched: 'word' (k_gather4, 4 pixels per thread) or 'byte' (k_gather)."""
-        return {4: "word", 1: "byte"}.get(int(self.ctx.lib.bevk_undistort_last_path(self.ctx.h)), "none")
+        """Which gather the last call of this ctx launched: 'word' (k_gather4, 4 pixels per thread), 'byte' (k_gather) or
+        'taps' (k_gather_taps, INTER_CUBIC / INTER_LANCZOS4)."""
+        return {4: "word", 1: "byte", 2: "taps"}.get(int(self.ctx.lib.bevk_undistort_last_path(self.ctx.h)), "none")
 
 
 class BevEngine:

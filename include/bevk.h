@@ -37,7 +37,11 @@ typedef enum {
   BEVK_ERR_UNSUPPORTED = -4
 } bevk_status;
 
-enum { BEVK_INTER_NEAREST = 0, BEVK_INTER_LINEAR = 1 };          /* cv2.INTER_* values */
+/* cv2.INTER_* values.  The image gathers (bevk_remap, bevk_undistort, bevk_undistort_jpeg, bevk_undistort_stack_interp,
+ * bevk_undistort_stack_jpeg, bevk_warp_perspective) take all five and read
+ * INTER_AREA as INTER_LINEAR, as cv2.remap and cv2.warpPerspective do; CUBIC and LANCZOS4 need map2.  The BEV engine
+ * takes NEAREST and LINEAR only. */
+enum { BEVK_INTER_NEAREST = 0, BEVK_INTER_LINEAR = 1, BEVK_INTER_CUBIC = 2, BEVK_INTER_AREA = 3, BEVK_INTER_LANCZOS4 = 4 };
 enum { BEVK_MAPS_UNDISTORT = 0, BEVK_MAPS_BEV = 1 };
 enum { BEVK_MODEL_FISHEYE = 0, BEVK_MODEL_PINHOLE = 1 };
 /* bevk_bev_run flags.  BEVK_FLAG_NV12 / BEVK_FLAG_I420 (exclusive; they combine with BALANCE) say the frames are YUV
@@ -94,7 +98,7 @@ int bevk_undistort_map(bevk_ctx *ctx, int model, const double K[9], const double
 
 /* ---- K3: cv2.remap(src, map1, map2, interp), BORDER_CONSTANT 0 --------------
  *   surroundBEV.py:110-111,116-117; undistort.py:66; intrinsicCalib.py:193-195
- * channels in {1,3,4}; map2 may be NULL for NEAREST with integer maps.          */
+ * channels in {1,3,4}; map2 may be NULL for NEAREST with integer maps.  interp: any BEVK_INTER_* (see above).    */
 int bevk_remap(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t sstride, int channels,
                const int16_t *map1, const uint16_t *map2, int dw, int dh,
                uint8_t *dst, int64_t dstride, int interp);
@@ -121,8 +125,15 @@ int bevk_undistort(bevk_ctx *ctx, int slot, const uint8_t *src, int sw, int sh, 
 int bevk_undistort_stack(bevk_ctx *ctx, int slot, const void *d_src, int64_t src_image_stride, int sw, int sh,
                          int64_t src_row_stride, int channels, int n, void *d_dst, int64_t dst_image_stride,
                          int dw, int dh, int64_t dst_row_stride, int interp);
+/* bevk_undistort_stack takes INTER_NEAREST and INTER_LINEAR and refuses every other interp with BEVK_ERR_UNSUPPORTED.
+ * bevk_undistort_stack_interp is the same call for every cv2 flag (INTER_CUBIC, INTER_AREA and INTER_LANCZOS4 too, see
+ * BEVK_INTER_*).  It also only enqueues and can be graph-captured: the weight tables of CUBIC and LANCZOS4 are
+ * uploaded when the ctx is created. */
+int bevk_undistort_stack_interp(bevk_ctx *ctx, int slot, const void *d_src, int64_t src_image_stride, int sw, int sh,
+                                int64_t src_row_stride, int channels, int n, void *d_dst, int64_t dst_image_stride,
+                                int dw, int dh, int64_t dst_row_stride, int interp);
 /* Which gather the last undistort call (or bevk_remap / bevk_warp_perspective) launched: 4 = k_gather4 (word path),
- * 1 = k_gather (byte path), 0 = none yet. */
+ * 1 = k_gather (byte path), 2 = k_gather_taps (INTER_CUBIC / INTER_LANCZOS4), 0 = none yet. */
 int bevk_undistort_last_path(bevk_ctx *ctx);
 
 /* ---- K4: cv2.warpPerspective(src, H, (dw,dh), flags=interp), border 0 --------
