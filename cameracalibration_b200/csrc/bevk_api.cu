@@ -223,32 +223,33 @@ struct bevk_ctx {
   // nvJPEG ingest (bevk_jpeg_decode): library handle + decoder state, created on first use
   void* jpeg_handle = nullptr; void* jpeg_state = nullptr;
   DevBuf d_jpeg_frames, d_jpeg_canvas;
-  // JPEG encoder (bevk_jpeg_encode): the cv2.imwrite parameters of bevk_jpeg_set_params, header and tables of the last
-  // (width, height, normalised options), work buffers.  The compacted streams, their layout and their sizes are
-  // double-buffered (two slots), so that one batch can be encoded while the streams of the one before are still being
-  // copied out on out_stream.
+  // The streams of every encoder (JPEG, progressive JPEG, PNG) on their way to the host: two slots, so that one batch can
+  // be encoded while the streams of the one before are still being copied out on out_stream.  A slot's `out` holds the
+  // compacted streams and its `meta` their offsets [n], sizes [n] and running end [1].
+  struct EncOut {
+    DevBuf out[2], meta[2];
+    unsigned long long* h_sizes[2] = {nullptr, nullptr};   // page-locked copies of a slot's stream sizes
+    size_t h_sizes_cap[2] = {0, 0};
+    cudaStream_t out_stream = nullptr;                      // D2H of the streams
+    cudaEvent_t ev_sizes[2] = {nullptr, nullptr}, ev_out_free[2] = {nullptr, nullptr};
+  } enc_out;
+  // JPEG encoder (bevk_jpeg_encode, bevk_jpeg_encode_params): the cv2.imwrite parameters of bevk_jpeg_set_params, the
+  // header (baseline) or frame prefix (progressive) and tables of the last (width, height, normalised options), and the
+  // work buffers of both entropy coders.
   struct JpegEnc {
     std::vector<int> params;
     int w = 0, h = 0;
     jpeg::Opts o{0, 0, -1, -1};
     uint8_t header[jpeg::kMaxHeaderBytes] = {};
-    DevBuf d_header, d_tabs, coef, bits, offs, dcdiff, words, ffcnt, ffscan, scan_tmp, out[2], meta[2];
-    DevBuf ilen, iofs, counts, huff, hdrs, hlen;   // restart intervals; optimised tables
-    unsigned long long* h_sizes[2] = {nullptr, nullptr};   // page-locked copies of a slot's stream sizes
-    size_t h_sizes_cap[2] = {0, 0};
-    cudaStream_t out_stream = nullptr;                      // D2H of the streams
-    cudaEvent_t ev_sizes[2] = {nullptr, nullptr}, ev_out_free[2] = {nullptr, nullptr};
+    DevBuf d_header, d_tabs, coef, bits, offs, dcdiff, words, ffcnt, ffscan, scan_tmp;
+    DevBuf ilen, iofs, counts, huff, hdrs, hlen;   // restart intervals (segments); optimised tables
+    DevBuf desc, pe, pc, ph, jump, jump2, mark, rs, codes, ins, insx;   // progressive only (bevk_jpeg_prog.cuh)
   } enc;
-  // progressive JPEG (bevk_jpeg_encode_params): work buffers of jpeg_prog_encode (bevk_jpeg_prog.cuh)
-  struct JpegProg {
-    DevBuf tabs, prefix, coef, desc, pe, pc, ph, jump, jump2, mark, rs, counts, codes, hdrs, hlen, bits, offs, ilen, iofs, ins,
-        insx, words, ffcnt, ffscan, out, meta, scan_tmp;
-  } prog;
   // PNG encoder (bevk_png_encode): the cv2.imwrite parameters of bevk_png_set_params and the work buffers of one group
-  // of images (bevk_png_enc.cuh); every group's streams land compacted in `out`.
+  // of images (bevk_png_enc.cuh).
   struct PngEnc {
     std::vector<int> params;
-    DevBuf f, rowad, runs, symidx, syms, nsym, blk, codes, hdr, zw, zbytes, meta, out, scan_tmp;
+    DevBuf f, rowad, runs, symidx, syms, nsym, blk, codes, hdr, zw, zbytes, scan_tmp;
     DevBuf nblk, keys, keys2, pos, pos2, prev, recs, jump, jump2, mark, cnt, dists;   // nblk; the hash-chain parse
   } png;
   // CUDA graphs captured from the device-pointer entry points (bevk_graph_*)
@@ -337,12 +338,12 @@ bevk_ctx::~bevk_ctx() {
   shard_release(this);
   jpeg_release(this);
   for (auto& g : graphs) { if (g.x) cudaGraphExecDestroy(g.x); if (g.g) cudaGraphDestroy(g.g); }
-  for (cudaEvent_t e : {ev0, ev1, ev_switch, ev_in[0], ev_in[1], ev_free[0], ev_free[1], ev_hp[0], ev_hp[1], enc.ev_sizes[0],
-                        enc.ev_sizes[1], enc.ev_out_free[0], enc.ev_out_free[1]})
+  for (cudaEvent_t e : {ev0, ev1, ev_switch, ev_in[0], ev_in[1], ev_free[0], ev_free[1], ev_hp[0], ev_hp[1], enc_out.ev_sizes[0],
+                        enc_out.ev_sizes[1], enc_out.ev_out_free[0], enc_out.ev_out_free[1]})
     if (e) cudaEventDestroy(e);
-  for (cudaStream_t s : {copy_stream, enc.out_stream, own})
+  for (cudaStream_t s : {copy_stream, enc_out.out_stream, own})
     if (s) cudaStreamDestroy(s);
-  for (void* p : {(void*)h_hptrs, (void*)enc.h_sizes[0], (void*)enc.h_sizes[1]})
+  for (void* p : {(void*)h_hptrs, (void*)enc_out.h_sizes[0], (void*)enc_out.h_sizes[1]})
     if (p) cudaFreeHost(p);
 }
 
@@ -2379,74 +2380,207 @@ int bevk_bev_run_jpeg(bevk_ctx* c, const uint8_t* const* jpegs, const uint64_t* 
   return BEVK_OK;
 }
 
-// ------------------------------------------------------------------ JPEG encode on the device (bevk_jpeg_enc.cuh)
-// The reference writes its results with cv2.imwrite (Tools/undistort.py:72-73, surroundBEV.py:340): D2H of the whole
-// image, then libjpeg-turbo on a host core.  Here the encoder runs on the device and only the streams cross PCIe.
-int bevk_jpeg_encode_bound(int width, int height, uint64_t* bytes) {
-  if (!bytes) return fail(BEVK_ERR_ARG, "null bytes");
-  if (width < 1 || height < 1 || width > jpeg::kMaxDim || height > jpeg::kMaxDim)
-    return fail(BEVK_ERR_ARG, "bad JPEG size %dx%d (1..%d)", width, height, jpeg::kMaxDim);
-  *bytes = jpeg::encode_bound(width, height);
+// ------------------------------------------------------------------ encoders: one host path for JPEG and PNG
+// Every encoding call runs through enc_chunks: each chunk of images is encoded into one of the two slots of c->enc_out
+// (slot_open ... slot_close), and enc_collect copies that slot's streams to the host while the next chunk is encoded.
+
+// What an encoder reads: n images at img + i * istride, rows pitch bytes apart.
+struct EncIn {
+  const void* img = nullptr;
+  long long istride = 0, pitch = 0;
+};
+
+// n 3-channel device images of the bevk_*_encode calls, rows row_stride bytes apart, image_stride apart (n > 1)
+static int check_device_images(const void* d_images, int64_t image_stride, int64_t row_stride, int n, int w, int h) {
+  if (!d_images || n < 1) return fail(BEVK_ERR_ARG, "bad argument");
+  if (row_stride < (int64_t)w * 3) return fail(BEVK_ERR_ARG, "row stride %lld < %d bytes", (long long)row_stride, w * 3);
+  if (n > 1 && image_stride < (int64_t)(h - 1) * row_stride + (int64_t)w * 3)
+    return fail(BEVK_ERR_ARG, "image stride %lld is smaller than one image", (long long)image_stride);
   return BEVK_OK;
 }
 
-// A bevk_jpeg_set_params list: keys 2..7 of cv2.IMWRITE_JPEG_*, normalised by jpeg::normalise.  The streams the device
-// encoder writes here are baseline and one scan: PROGRESSIVE asks for another entropy coder and is refused, not ignored
-// (the per-call bevk_jpeg_encode_params writes it).
-static int jpeg_params_check(const int* params, int n, jpeg::Opts* o) {
+// The encoding calls write host memory and wait for the stream sizes, so they cannot be captured into a graph.
+static int enc_call_check(bevk_ctx* c, const uint8_t* out, const uint64_t* sizes) {
+  if (c->capturing) return fail(BEVK_ERR_ARG, "the encoding calls synchronise and cannot be captured into a graph");
+  if (!out || !sizes) return fail(BEVK_ERR_ARG, "null host pointer");
+  return BEVK_OK;
+}
+
+// Slot s for the streams of n images, `bytes` at most: its buffers, and the ctx stream ordered after the slot's previous
+// streams have been copied out.  An encoder calls it before its first write into the slot.
+static int slot_open(bevk_ctx* c, int s, int n, size_t bytes) {
+  auto& e = c->enc_out;
+  RET(e.out[s].ensure(bytes));
+  RET(e.meta[s].ensure((size_t)(2ll * n + 1) * 8));
+  if (e.h_sizes_cap[s] < (size_t)n) {
+    if (e.h_sizes[s]) CU(cudaFreeHost(e.h_sizes[s]));      // enc_collect waited for its last copy
+    e.h_sizes[s] = nullptr; e.h_sizes_cap[s] = 0;
+    CU(cudaHostAlloc(reinterpret_cast<void**>(&e.h_sizes[s]), (size_t)n * 8, cudaHostAllocDefault));
+    e.h_sizes_cap[s] = (size_t)n;
+  }
+  CU(cudaStreamWaitEvent(c->stream, e.ev_out_free[s], 0));
+  return BEVK_OK;
+}
+
+// After an encoder's last kernel into slot s: ev1 (bevk_last_kernel_ms covers the kernels only), then the D2H of the
+// stream sizes into page-locked memory and ev_sizes[s].  enc_collect(s) finishes the batch.
+static int slot_close(bevk_ctx* c, int s, int n) {
+  auto& e = c->enc_out;
+  CU(cudaEventRecord(c->ev1, c->stream));
+  c->timed = true;
+  CU(cudaMemcpyAsync(e.h_sizes[s], e.meta[s].as<unsigned long long>() + n, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaEventRecord(e.ev_sizes[s], c->stream));
+  return BEVK_OK;
+}
+
+// Finish slot s's batch of n: wait for its sizes, store them in sizes[n], and copy streams to the host at out + *used on
+// out_stream (not synchronised).  whole: all of the batch's streams or none; otherwise the leading streams that still fit
+// in capacity, none once *full (an earlier stream did not fit).  *used grows by the bytes copied.
+static int enc_collect(bevk_ctx* c, int s, int n, uint8_t* out, uint64_t capacity, bool whole, uint64_t* sizes, uint64_t* used,
+                       bool* full) {
+  auto& e = c->enc_out;
+  CU(cudaEventSynchronize(e.ev_sizes[s]));
+  unsigned long long fit = 0, all = 0;
+  for (int i = 0; i < n; ++i) {
+    sizes[i] = e.h_sizes[s][i];
+    all += sizes[i];
+    if (!*full && *used + fit + sizes[i] <= capacity) fit += sizes[i];
+    else *full = true;
+  }
+  if (whole && fit < all) fit = 0;
+  if (fit) {
+    CU(cudaStreamWaitEvent(e.out_stream, e.ev_sizes[s], 0));
+    CU(cudaMemcpyAsync(out + *used, e.out[s].p, fit, cudaMemcpyDeviceToHost, e.out_stream));
+    CU(cudaEventRecord(e.ev_out_free[s], e.out_stream));
+  }
+  *used += fit;
+  return BEVK_OK;
+}
+
+static int capacity_error(const char* fmt, int n, const uint64_t* sizes, uint64_t capacity) {
+  unsigned long long total = 0;
+  for (int i = 0; i < n; ++i) total += sizes[i];
+  return fail(BEVK_ERR_ARG, "the %d %s streams take %llu bytes, capacity is %llu", n, fmt, total, (unsigned long long)capacity);
+}
+
+// Encode n images (n >= 1) chunk by chunk through the two slots.  enqueue(b0, nb, s) enqueues what makes images
+// [b0, b0 + nb) and an encoder over them into slot s.  A chunk's streams are collected (wait for their sizes, D2H on
+// out_stream) after the next chunk has been enqueued into the other slot.  whole: all streams or none (a single chunk);
+// otherwise the leading streams that fit in capacity.  fmt names the format in the capacity error.
+template <class Enqueue>
+static int enc_chunks(bevk_ctx* c, const char* fmt, int n, int chunk, bool whole, uint8_t* out, uint64_t capacity,
+                      uint64_t* sizes, Enqueue enqueue) {
+  RET(enc_call_check(c, out, sizes));
+  auto& e = c->enc_out;
+  if (!e.out_stream) RET(create_stream_set(&e.out_stream, {&e.ev_sizes[0], &e.ev_sizes[1], &e.ev_out_free[0], &e.ev_out_free[1]}));
+  uint64_t used = 0;
+  bool full = false;
+  int s = 0, prev_b0 = -1, prev_nb = 0;
+  for (int b0 = 0; b0 < n; b0 += chunk, s ^= 1) {
+    const int nb = std::min(chunk, n - b0);
+    RET(enqueue(b0, nb, s));
+    if (prev_b0 >= 0) RET(enc_collect(c, s ^ 1, prev_nb, out, capacity, whole, sizes + prev_b0, &used, &full));
+    prev_b0 = b0; prev_nb = nb;
+  }
+  RET(enc_collect(c, s ^ 1, prev_nb, out, capacity, whole, sizes + prev_b0, &used, &full));
+  CU(cudaStreamSynchronize(e.out_stream));
+  return full ? capacity_error(fmt, n, sizes, capacity) : BEVK_OK;
+}
+
+// ------------------------------------------------------------------ JPEG encode on the device (bevk_jpeg_enc.cuh)
+// The reference writes its results with cv2.imwrite (Tools/undistort.py:72-73, surroundBEV.py:340): D2H of the whole
+// image, then libjpeg-turbo on a host core.  Here the encoder runs on the device and only the streams cross PCIe.
+static int jpeg_size_check(int width, int height) {
+  if (width < 1 || height < 1 || width > jpeg::kMaxDim || height > jpeg::kMaxDim)
+    return fail(BEVK_ERR_ARG, "bad JPEG size %dx%d (1..%d)", width, height, jpeg::kMaxDim);
+  return BEVK_OK;
+}
+
+// A JPEG list: keys 2..7 of cv2.IMWRITE_JPEG_*, normalised by jpeg::normalise under the call's quality.
+static int jpeg_params_check(const int* params, int n, int quality, jpeg::Opts* o) {
   if (n < 0 || (n & 1) || (n && !params)) return fail(BEVK_ERR_ARG, "JPEG params: %d ints, need (key, value) pairs", n);
   for (int i = 0; i < n; i += 2)
     if (params[i] < jpeg::kProgressive || params[i] > jpeg::kSamplingFactor)
       return fail(BEVK_ERR_ARG, "JPEG params: key %d (IMWRITE_JPEG_QUALITY is the quality argument of each call; "
                   "keys are 2..7)", params[i]);
-  jpeg::normalise(95, params, n, o);
+  jpeg::normalise(quality, params, n, o);
+  return BEVK_OK;
+}
+
+// A bevk_jpeg_set_params list.  The calls that read it write baseline streams: PROGRESSIVE asks for another entropy
+// coder and is refused, not ignored (the per-call bevk_jpeg_encode_params writes it).
+static int jpeg_ctx_params_check(const int* params, int n, jpeg::Opts* o) {
+  RET(jpeg_params_check(params, n, 95, o));
   if (o->progressive) return fail(BEVK_ERR_UNSUPPORTED, "JPEG params: IMWRITE_JPEG_PROGRESSIVE is not supported");
   return BEVK_OK;
+}
+
+// the ctx's list (bevk_jpeg_set_params checked it) under a call's quality
+static jpeg::Opts jpeg_ctx_opts(const bevk_ctx* c, int quality) {
+  jpeg::Opts o;
+  jpeg::normalise(quality, c->enc.params.data(), (int)c->enc.params.size(), &o);
+  return o;
+}
+
+static unsigned long long jpeg_bound(int w, int h, const jpeg::Opts& o) {
+  const jpeg::Geom g = jpeg::geom(w, h, o);
+  return o.progressive ? jpeg::prog::progressive_bound(g, o.rst) : jpeg::encode_bound(g, o);
+}
+
+int bevk_jpeg_encode_bound(int width, int height, uint64_t* bytes) {
+  return bevk_jpeg_encode_bound_params(width, height, nullptr, 0, bytes);
 }
 
 int bevk_jpeg_set_params(bevk_ctx* c, const int* params, int n) {
   RET(use(c));
   jpeg::Opts o;
-  RET(jpeg_params_check(params, n, &o));
+  RET(jpeg_ctx_params_check(params, n, &o));
   c->enc.params.assign(params, params + n);
   return BEVK_OK;
 }
 
 int bevk_jpeg_encode_bound_params(int width, int height, const int* params, int n, uint64_t* bytes) {
   if (!bytes) return fail(BEVK_ERR_ARG, "null bytes");
-  if (width < 1 || height < 1 || width > jpeg::kMaxDim || height > jpeg::kMaxDim)
-    return fail(BEVK_ERR_ARG, "bad JPEG size %dx%d (1..%d)", width, height, jpeg::kMaxDim);
+  RET(jpeg_size_check(width, height));
   jpeg::Opts o;
-  RET(jpeg_params_check(params, n, &o));
-  *bytes = jpeg::encode_bound(jpeg::geom(width, height, o), o);
+  RET(jpeg_ctx_params_check(params, n, &o));
+  *bytes = jpeg_bound(width, height, o);
   return BEVK_OK;
 }
 
-// What the encoder reads: n images at img + i * istride, rows pitch bytes apart.
-struct JpegIn {
-  const void* img = nullptr;
-  long long istride = 0, pitch = 0;
-};
+int bevk_jpeg_encode_params_bound(int width, int height, const int* params, int n, uint64_t* bytes) {
+  if (!bytes) return fail(BEVK_ERR_ARG, "null bytes");
+  RET(jpeg_size_check(width, height));
+  jpeg::Opts o;
+  RET(jpeg_params_check(params, n, 95, &o));
+  *bytes = jpeg_bound(width, height, o);
+  return BEVK_OK;
+}
 
-// Enqueue the encoder over n w x h images into slot s on the ctx stream: every kernel, then the D2H of the stream sizes
-// into page-locked memory and ev_sizes[s].  jpeg_collect(s) finishes the batch.  The per-block work buffers are single:
-// batches use them one after the other in stream order.
-static int jpeg_enqueue(bevk_ctx* c, int s, const JpegIn& in, int n, int w, int h, int quality) {
+// Header (baseline) or frame prefix (progressive) into d_header and the tables into d_tabs: they depend on
+// (w, h, options) only, so they are uploaded when one of these changes.
+static int jpeg_tables(bevk_ctx* c, int w, int h, const jpeg::Opts& o) {
   using namespace jpeg;
   auto& e = c->enc;
-  if (!e.out_stream) RET(create_stream_set(&e.out_stream, {&e.ev_sizes[0], &e.ev_sizes[1], &e.ev_out_free[0], &e.ev_out_free[1]}));
-  Opts o;
-  normalise(quality, e.params.data(), (int)e.params.size(), &o);   // bevk_jpeg_set_params checked the list
-  if (w != e.w || h != e.h || o != e.o) {   // header + tables depend on (w, h, options) only
-    Tables t;
-    make_tables(o, &t);
-    make_header(w, h, o, e.header);
-    RET(e.d_header.ensure(kMaxHeaderBytes));
-    RET(e.d_tabs.ensure(sizeof(Tables)));
-    CU(cudaMemcpyAsync(e.d_header.p, e.header, kMaxHeaderBytes, cudaMemcpyHostToDevice, c->stream));   // pageable: staged
-    CU(cudaMemcpyAsync(e.d_tabs.p, &t, sizeof t, cudaMemcpyHostToDevice, c->stream));               // before returning
-    e.w = w; e.h = h; e.o = o;
-  }
+  if (w == e.w && h == e.h && o == e.o) return BEVK_OK;
+  Tables t;
+  make_tables(o, &t);
+  if (o.progressive) prog::frame_prefix(w, h, o, e.header);
+  else make_header(w, h, o, e.header);
+  RET(e.d_header.ensure(kMaxHeaderBytes));
+  RET(e.d_tabs.ensure(sizeof(Tables)));
+  CU(cudaMemcpyAsync(e.d_header.p, e.header, kMaxHeaderBytes, cudaMemcpyHostToDevice, c->stream));   // pageable: staged
+  CU(cudaMemcpyAsync(e.d_tabs.p, &t, sizeof t, cudaMemcpyHostToDevice, c->stream));               // before returning
+  e.w = w; e.h = h; e.o = o;
+  return BEVK_OK;
+}
+
+// Enqueue the baseline encoder over n w x h images into slot s on the ctx stream.  The work buffers are single: batches
+// use them one after the other in stream order.
+static int jpeg_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int w, int h, const jpeg::Opts& o) {
+  using namespace jpeg;
+  auto& e = c->enc;
+  RET(jpeg_tables(c, w, h, o));
   const Geom g = geom(w, h, o);
   const long long nblk = blocks_per_image(g), nb = nblk * n;
   const long long nint = intervals(g, o), ni = nint * n;
@@ -2463,7 +2597,6 @@ static int jpeg_enqueue(bevk_ctx* c, int s, const JpegIn& in, int n, int w, int 
   RET(e.ffcnt.ensure((size_t)nch * 4));
   if (e.ffcnt.cap != ffcap) CU(cudaMemsetAsync(e.ffcnt.p, 0, e.ffcnt.cap, c->stream));
   RET(e.ffscan.ensure((size_t)nch * 4));
-  RET(e.out[s].ensure((size_t)n * encode_bound(g, o)));
   if (o.rst) {
     RET(e.ilen.ensure((size_t)ni * 8));
     RET(e.iofs.ensure((size_t)ni * 8));
@@ -2474,13 +2607,6 @@ static int jpeg_enqueue(bevk_ctx* c, int s, const JpegIn& in, int n, int w, int 
     RET(e.hdrs.ensure((size_t)n * kMaxHeaderBytes));
     RET(e.hlen.ensure((size_t)n * 4));
   }
-  RET(e.meta[s].ensure((size_t)n * 16));
-  if (e.h_sizes_cap[s] < (size_t)n) {
-    if (e.h_sizes[s]) CU(cudaFreeHost(e.h_sizes[s]));      // jpeg_collect waited for its last copy
-    e.h_sizes[s] = nullptr; e.h_sizes_cap[s] = 0;
-    CU(cudaHostAlloc(reinterpret_cast<void**>(&e.h_sizes[s]), (size_t)n * 8, cudaHostAllocDefault));
-    e.h_sizes_cap[s] = (size_t)n;
-  }
   size_t tmp1 = 0, tmp2 = 0;
   CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp1, e.bits.as<unsigned long long>(), e.offs.as<unsigned long long>(), (int)nb));
   CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp2, e.ffcnt.as<unsigned>(), e.ffscan.as<unsigned>(), (int)nch));
@@ -2488,20 +2614,20 @@ static int jpeg_enqueue(bevk_ctx* c, int s, const JpegIn& in, int n, int w, int 
   if (o.rst) CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp3, e.ilen.as<unsigned long long>(), e.iofs.as<unsigned long long>(), (int)ni));
   const size_t tmp = std::max(std::max(tmp1, tmp2), tmp3);
   RET(e.scan_tmp.ensure(tmp));
+  RET(slot_open(c, s, n, (size_t)n * encode_bound(g, o)));
 
   EncArgs a{};
   a.img = reinterpret_cast<const uint8_t*>(in.img); a.istride = in.istride; a.pitch = in.pitch; a.n = n; a.g = g; a.nblk = nblk;
   a.tabs = e.d_tabs.as<Tables>(); a.coef = e.coef.as<int16_t>(); a.bits = e.bits.as<unsigned long long>();
   a.offs = e.offs.as<unsigned long long>(); a.dcdiff = e.dcdiff.as<int>(); a.words = e.words.as<uint32_t>(); a.words_img = words_img;
   a.chunks_img = chunks; a.ffcnt = e.ffcnt.as<unsigned>(); a.ffscan = e.ffscan.as<unsigned>(); a.header = e.d_header.as<uint8_t>();
-  a.out = e.out[s].as<uint8_t>(); a.out_off = e.meta[s].as<unsigned long long>(); a.sizes = e.meta[s].as<unsigned long long>() + n;
+  a.out = c->enc_out.out[s].as<uint8_t>(); a.out_off = c->enc_out.meta[s].as<unsigned long long>(); a.sizes = a.out_off + n;
   a.rst = o.rst; a.nint = nint; a.hlen0 = header_bytes(o);
   if (o.rst) { a.ilen = e.ilen.as<unsigned long long>(); a.iofs = e.iofs.as<unsigned long long>(); }
   if (o.optimize) {
     a.counts = e.counts.as<unsigned long long>(); a.huff = e.huff.as<Huff>(); a.hdrs = e.hdrs.as<uint8_t>(); a.hlen = e.hlen.as<int>();
   }
   const unsigned gb = (unsigned)((nb + kBlockThreads - 1) / kBlockThreads), gc = (unsigned)((nch + 255) / 256);
-  CU(cudaStreamWaitEvent(c->stream, e.ev_out_free[s], 0));   // the slot's previous streams have been copied out
   CU(cudaEventRecord(c->ev0, c->stream));
   RET(with_sampling(o.hy, o.vy, [&](auto hy, auto vy) -> int {
     constexpr int HY = hy(), VY = vy();
@@ -2540,190 +2666,15 @@ static int jpeg_enqueue(bevk_ctx* c, int s, const JpegIn& in, int n, int w, int 
   LAUNCHED(c);
   k_jpeg_stuff<<<gc, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
-  CU(cudaEventRecord(c->ev1, c->stream));
-  c->timed = true;
-  CU(cudaMemcpyAsync(e.h_sizes[s], a.sizes, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaEventRecord(e.ev_sizes[s], c->stream));
-  return BEVK_OK;
+  return slot_close(c, s, n);
 }
 
-// Finish slot s's batch of n: wait for its sizes, store them in sizes[n], and copy streams to the host at out + *used on
-// out_stream (not synchronised).  whole: all of the batch's streams or none; otherwise the leading streams that still fit
-// in capacity, none once *full (an earlier stream did not fit).  *used grows by the bytes copied.
-static int jpeg_collect(bevk_ctx* c, int s, int n, uint8_t* out, uint64_t capacity, bool whole, uint64_t* sizes, uint64_t* used,
-                        bool* full) {
-  auto& e = c->enc;
-  CU(cudaEventSynchronize(e.ev_sizes[s]));
-  unsigned long long fit = 0, all = 0;
-  for (int i = 0; i < n; ++i) {
-    sizes[i] = e.h_sizes[s][i];
-    all += sizes[i];
-    if (!*full && *used + fit + sizes[i] <= capacity) fit += sizes[i];
-    else *full = true;
-  }
-  if (whole && fit < all) fit = 0;
-  if (fit) {
-    CU(cudaStreamWaitEvent(e.out_stream, e.ev_sizes[s], 0));
-    CU(cudaMemcpyAsync(out + *used, e.out[s].p, fit, cudaMemcpyDeviceToHost, e.out_stream));
-    CU(cudaEventRecord(e.ev_out_free[s], e.out_stream));
-  }
-  *used += fit;
-  return BEVK_OK;
-}
-
-static int capacity_error(int n, const uint64_t* sizes, uint64_t capacity) {
-  unsigned long long total = 0;
-  for (int i = 0; i < n; ++i) total += sizes[i];
-  return fail(BEVK_ERR_ARG, "the %d JPEG streams take %llu bytes, capacity is %llu", n, total, (unsigned long long)capacity);
-}
-
-// Encode n images chunk by chunk through the two slots.  enqueue(b0, nb, s, &in) enqueues what makes images
-// [b0, b0 + nb) and describes them in `in`; the encoder then runs on them in slot s.  A chunk's streams are collected
-// (wait for their sizes, D2H on out_stream) after the next chunk has been enqueued into the other slot.  whole: all
-// streams or none (a single chunk); otherwise the leading streams that fit in capacity.
-template <class Enqueue>
-static int jpeg_chunks(bevk_ctx* c, int n, int chunk, int w, int h, int quality, bool whole, uint8_t* out, uint64_t capacity,
-                       uint64_t* sizes, Enqueue enqueue) {
-  uint64_t used = 0;
-  bool full = false;
-  int s = 0, prev_b0 = -1, prev_nb = 0;
-  for (int b0 = 0; b0 < n; b0 += chunk, s ^= 1) {
-    const int nb = std::min(chunk, n - b0);
-    JpegIn in;
-    RET(enqueue(b0, nb, s, &in));
-    RET(jpeg_enqueue(c, s, in, nb, w, h, quality));
-    if (prev_b0 >= 0) RET(jpeg_collect(c, s ^ 1, prev_nb, out, capacity, whole, sizes + prev_b0, &used, &full));
-    prev_b0 = b0; prev_nb = nb;
-  }
-  RET(jpeg_collect(c, s ^ 1, prev_nb, out, capacity, whole, sizes + prev_b0, &used, &full));
-  CU(cudaStreamSynchronize(c->enc.out_stream));
-  return full ? capacity_error(n, sizes, capacity) : BEVK_OK;
-}
-
-static int jpeg_encode_device(bevk_ctx* c, const JpegIn& in, int n, int w, int h, int quality, uint8_t* out, uint64_t capacity,
-                              uint64_t* sizes) {
-  if (c->capturing) return fail(BEVK_ERR_ARG, "bevk_jpeg_encode synchronises and cannot be captured into a graph");
-  return jpeg_chunks(c, n, n, w, h, quality, true, out, capacity, sizes, [&](int, int, int, JpegIn* p) {
-    *p = in;
-    return BEVK_OK;
-  });
-}
-
-// Images per chunk of the chunked device-frame calls.  8 canvases (24 MB at 1000^2: they stay in the 50 MB L2) beat the
-// whole batch at once on H100 (DESIGN.md section 4); BEVK_JPEG_CHUNK=n sets another size, 0 the whole batch.
-static int jpeg_chunk(int n) {
-  int chunk = std::min(n, 8);
-  if (const char* env = getenv("BEVK_JPEG_CHUNK")) chunk = atoi(env) > 0 ? std::min(n, atoi(env)) : n;
-  return chunk;
-}
-
-// ------------------------------------------------------------------ BEV canvases straight to JPEG (surroundBEV.py:340)
-// BevGenerator.__call__ then cv2.imencode: each chunk of frame-sets is rendered into ctx scratch and encoded there, and
-// only the streams come back.  Under BALANCE run_device's k_gain applies colour balance and the car to the chunk's
-// canvases before the encoder reads them.
-static int to_jpeg_check(bevk_ctx* c, uint8_t* out, uint64_t* sizes) {
-  RET(need_plan(c));
-  if (!out || !sizes) return fail(BEVK_ERR_ARG, "null host pointer");
-  if (c->capturing) return fail(BEVK_ERR_ARG, "the BEV-to-JPEG calls synchronise and cannot be captured into a graph");
-  uint64_t bound = 0;
-  return bevk_jpeg_encode_bound(c->BW, c->BH, &bound);
-}
-
-int bevk_bev_run_to_jpeg(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, int batch, const uint8_t* car, int flags,
-                         int quality, uint8_t* out, uint64_t capacity, uint64_t* sizes) {
-  NvtxRange nvtx_call("bevk_bev_run_to_jpeg (host frames -> host JPEG streams)");
-  RET(use(c));
-  RET(bgr_only(flags, "bevk_bev_run_to_jpeg"));
-  RET(bgr_canvas_only(flags, "bevk_bev_run_to_jpeg"));
-  RET(to_jpeg_check(c, out, sizes));
-  HostIngest h;
-  RET(ingest_setup(c, srcs, src_stride, batch, car, flags, &h));
-  // the ingest chunks are the encoder's: staging half = canvas half = encoder slot
-  return jpeg_chunks(c, batch, h.chunk, c->BW, c->BH, quality, false, out, capacity, sizes, [&](int b0, int nb, int half, JpegIn* in) -> int {
-    uint8_t* dcanvas = nullptr;
-    RET(render_chunk(c, h, srcs, src_stride, flags, b0, nb, half, &dcanvas));
-    *in = JpegIn{dcanvas, (long long)h.cbytes, (long long)c->BW * 3};
-    return BEVK_OK;
-  });
-}
-
-int bevk_bev_frames_to_jpeg(bevk_ctx* c, const void* const* frames, int batch, const void* d_car, int flags, int quality,
-                            uint8_t* out, uint64_t capacity, uint64_t* sizes) {
-  NvtxRange nvtx_call("bevk_bev_frames_to_jpeg (device frames -> host JPEG streams)");
-  RET(use(c));
-  RET(bgr_only(flags, "bevk_bev_frames_to_jpeg"));
-  RET(bgr_canvas_only(flags, "bevk_bev_frames_to_jpeg"));
-  RET(to_jpeg_check(c, out, sizes));
-  if (!frames) return fail(BEVK_ERR_ARG, "null pointer");
-  Frames src;
-  RET(frames_src(c, frames, batch, &src));
-  // every chunk is rendered into the same canvas scratch: the next render is stream-ordered after the encoder read it
-  const int chunk = jpeg_chunk(batch);
-  RET(c->d_canvas.ensure((size_t)c->BW * c->BH * 3 * chunk));
-  uint8_t* dcanvas = c->d_canvas.as<uint8_t>();
-  return jpeg_chunks(c, batch, chunk, c->BW, c->BH, quality, false, out, capacity, sizes, [&](int b0, int nb, int, JpegIn* in) -> int {
-    Frames part = src;
-    if (part.table) part.table += (size_t)b0 * c->n_cam;
-    else part.base += (long long)b0 * c->n_cam * part.stride;
-    c->timed = false;
-    RET(run_device(c, part, nb, d_car, flags, dcanvas, 0, BEVK_MAX_CAMERAS));
-    *in = JpegIn{dcanvas, (long long)c->BW * c->BH * 3, (long long)c->BW * 3};
-    return BEVK_OK;
-  });
-}
-
-int bevk_jpeg_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, int64_t row_stride, int n, int width, int height,
-                     int quality, uint8_t* out, uint64_t capacity, uint64_t* sizes) {
-  NvtxRange nvtx_call("bevk_jpeg_encode (device images -> host JPEG streams)");
-  RET(use(c));
-  if (!d_images || !out || !sizes || n < 1) return fail(BEVK_ERR_ARG, "bad argument");
-  uint64_t bound = 0;
-  RET(bevk_jpeg_encode_bound(width, height, &bound));
-  if (row_stride < (int64_t)width * 3) return fail(BEVK_ERR_ARG, "row stride %lld < %d bytes", (long long)row_stride, width * 3);
-  if (n > 1 && image_stride < (int64_t)(height - 1) * row_stride + width * 3)
-    return fail(BEVK_ERR_ARG, "image stride %lld is smaller than one image", (long long)image_stride);
-  JpegIn in;
-  in.img = d_images; in.istride = image_stride; in.pitch = row_stride;
-  return jpeg_encode_device(c, in, n, width, height, quality, out, capacity, sizes);
-}
-
-// ------------------------------------------------------------------ progressive JPEG and per-call JPEG params
-// A per-call list: keys 2..7, PROGRESSIVE and OPTIMIZE read as cv2 4.13 reads them (0 / 1), then jpeg::normalise.
-static int jpeg_call_params(const int* params, int n, std::vector<int>* list, jpeg::Opts* o) {
-  if (n < 0 || (n & 1) || (n && !params)) return fail(BEVK_ERR_ARG, "JPEG params: %d ints, need (key, value) pairs", n);
-  for (int i = 0; i < n; i += 2)
-    if (params[i] < jpeg::kProgressive || params[i] > jpeg::kSamplingFactor)
-      return fail(BEVK_ERR_ARG, "JPEG params: key %d (IMWRITE_JPEG_QUALITY is the quality argument of each call; "
-                  "keys are 2..7)", params[i]);
-  list->assign(params, params + n);
-  jpeg::prog::read_flags(list->data(), n);
-  jpeg::normalise(95, list->data(), n, o);
-  return BEVK_OK;
-}
-
-int bevk_jpeg_encode_params_bound(int width, int height, const int* params, int n, uint64_t* bytes) {
-  if (!bytes) return fail(BEVK_ERR_ARG, "null bytes");
-  if (width < 1 || height < 1 || width > jpeg::kMaxDim || height > jpeg::kMaxDim)
-    return fail(BEVK_ERR_ARG, "bad JPEG size %dx%d (1..%d)", width, height, jpeg::kMaxDim);
-  std::vector<int> list;
-  jpeg::Opts o;
-  RET(jpeg_call_params(params, n, &list, &o));
-  const jpeg::Geom g = jpeg::geom(width, height, o);
-  *bytes = o.progressive ? jpeg::prog::progressive_bound(g, o.rst) : jpeg::encode_bound(g, o);
-  return BEVK_OK;
-}
-
-// Progressive streams of n images: k_jpeg_blocks, then the k_jpeg_prog_* pipeline over every scan of every image at once
-// (bevk_jpeg_prog.cuh), then the streams to the host.  Synchronises.
-static int jpeg_prog_encode(bevk_ctx* c, const jpeg::Opts& o, const JpegIn& in, int n, int w, int h, uint8_t* out,
-                            uint64_t capacity, uint64_t* sizes) {
+// Enqueue the progressive encoder over n w x h images into slot s: k_jpeg_blocks, then the k_jpeg_prog_* pipeline over
+// every scan of every image at once (bevk_jpeg_prog.cuh).
+static int jpeg_prog_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int w, int h, const jpeg::Opts& o) {
   using namespace jpeg;
   using namespace jpeg::prog;
-  auto& e = c->prog;
-  Tables t;
-  make_tables(o, &t);
-  uint8_t prefix[kPrefixBytes];
-  frame_prefix(w, h, o, prefix);
+  auto& e = c->enc;
   const Geom g = geom(w, h, o);
   const Layout L = layout(g, o.rst);
   const long long nblk = blocks_per_image(g), T = L.blk[kScans], S = L.seg[kScans];
@@ -2733,8 +2684,7 @@ static int jpeg_prog_encode(bevk_ctx* c, const jpeg::Opts& o, const JpegIn& in, 
   const long long nch = (long long)n * chunks;
   if (N >= INT_MAX || NS >= INT_MAX || nch >= INT_MAX)
     return fail(BEVK_ERR_ARG, "batch of %d %dx%d images is too large for one progressive call", n, w, h);
-  RET(e.tabs.ensure(sizeof(Tables)));
-  RET(e.prefix.ensure(kPrefixBytes));
+  RET(jpeg_tables(c, w, h, o));
   RET(e.coef.ensure((size_t)(nblk * n) * 128));
   RET(e.desc.ensure((size_t)N * 4));
   RET(e.pe.ensure((size_t)N * 8));
@@ -2759,8 +2709,7 @@ static int jpeg_prog_encode(bevk_ctx* c, const jpeg::Opts& o, const JpegIn& in, 
   RET(e.ffcnt.ensure((size_t)nch * 4));
   if (e.ffcnt.cap != ffcap) CU(cudaMemsetAsync(e.ffcnt.p, 0, e.ffcnt.cap, c->stream));
   RET(e.ffscan.ensure((size_t)nch * 4));
-  RET(e.out.ensure((size_t)n * progressive_bound(g, o.rst)));
-  RET(e.meta.ensure((size_t)n * 16));
+  RET(slot_open(c, s, n, (size_t)n * progressive_bound(g, o.rst)));
 
   ProgArgs a{};
   a.n = n; a.rst = o.rst; a.g = g; a.nblk = nblk; a.L = L; a.T = T; a.S = S;
@@ -2770,8 +2719,8 @@ static int jpeg_prog_encode(bevk_ctx* c, const jpeg::Opts& o, const JpegIn& in, 
   a.hdrs = e.hdrs.as<uint8_t>(); a.hlen = e.hlen.as<int>(); a.bits = e.bits.as<unsigned long long>();
   a.offs = e.offs.as<unsigned long long>(); a.ilen = e.ilen.as<unsigned long long>(); a.iofs = e.iofs.as<unsigned long long>();
   a.ins = e.ins.as<unsigned>(); a.insx = e.insx.as<unsigned>(); a.words = e.words.as<uint32_t>(); a.words_img = words_img;
-  a.chunks_img = chunks; a.ffcnt = e.ffcnt.as<unsigned>(); a.ffscan = e.ffscan.as<unsigned>(); a.prefix = e.prefix.as<uint8_t>();
-  a.out = e.out.as<uint8_t>(); a.out_off = e.meta.as<unsigned long long>(); a.sizes = e.meta.as<unsigned long long>() + n;
+  a.chunks_img = chunks; a.ffcnt = e.ffcnt.as<unsigned>(); a.ffscan = e.ffscan.as<unsigned>(); a.prefix = e.d_header.as<uint8_t>();
+  a.out = c->enc_out.out[s].as<uint8_t>(); a.out_off = c->enc_out.meta[s].as<unsigned long long>(); a.sizes = a.out_off + n;
 
   using ItE = cub::TransformInputIterator<unsigned long long, DescE, const uint32_t*>;
   using ItC = cub::TransformInputIterator<unsigned long long, DescC, const uint32_t*>;
@@ -2790,11 +2739,9 @@ static int jpeg_prog_encode(bevk_ctx* c, const jpeg::Opts& o, const JpegIn& in, 
   RET(e.scan_tmp.ensure(*std::max_element(tmp, tmp + 8)));
   void* st = e.scan_tmp.p;
 
-  CU(cudaMemcpyAsync(e.tabs.p, &t, sizeof t, cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemcpyAsync(e.prefix.p, prefix, kPrefixBytes, cudaMemcpyHostToDevice, c->stream));
   EncArgs b{};
   b.img = reinterpret_cast<const uint8_t*>(in.img); b.istride = in.istride; b.pitch = in.pitch; b.n = n; b.g = g; b.nblk = nblk;
-  b.tabs = e.tabs.as<Tables>(); b.coef = e.coef.as<int16_t>(); b.bits = a.bits;   // k_jpeg_blocks' AC bit counts land in scratch
+  b.tabs = e.d_tabs.as<Tables>(); b.coef = e.coef.as<int16_t>(); b.bits = a.bits;   // k_jpeg_blocks' AC bit counts land in scratch
   const unsigned gb = (unsigned)((nblk * n + kBlockThreads - 1) / kBlockThreads);
   const unsigned gN = (unsigned)((N + 255) / 256), gN1 = (unsigned)((N + 1 + 255) / 256), gS = (unsigned)((NS + 255) / 256);
   const unsigned gc = (unsigned)((nch + 255) / 256);
@@ -2814,7 +2761,7 @@ static int jpeg_prog_encode(bevk_ctx* c, const jpeg::Opts& o, const JpegIn& in, 
   k_jpeg_prog_next<<<gN1, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
   long long longest = 0;   // the longest scan bounds every chain of run starts
-  for (int s = 0; s < kScans; ++s) longest = std::max(longest, L.blk[s + 1] - L.blk[s]);
+  for (int k = 0; k < kScans; ++k) longest = std::max(longest, L.blk[k + 1] - L.blk[k]);
   for (long long span = 1; span <= longest; span *= 2) {
     k_jpeg_prog_jump<<<gN1, 256, 0, c->stream>>>(a.jump, a.jump2, a.mark, N);
     LAUNCHED(c);
@@ -2844,17 +2791,77 @@ static int jpeg_prog_encode(bevk_ctx* c, const jpeg::Opts& o, const JpegIn& in, 
   LAUNCHED(c);
   k_jpeg_prog_stuff<<<gc, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
-  CU(cudaEventRecord(c->ev1, c->stream));
-  c->timed = true;
-  std::vector<unsigned long long> hs((size_t)n);
-  CU(cudaMemcpyAsync(hs.data(), a.sizes, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  unsigned long long total = 0;
-  for (int i = 0; i < n; ++i) { sizes[i] = hs[(size_t)i]; total += hs[(size_t)i]; }
-  if (total > capacity) return capacity_error(n, sizes, capacity);
-  CU(cudaMemcpyAsync(out, a.out, total, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return BEVK_OK;
+  return slot_close(c, s, n);
+}
+
+// Images per chunk of the chunked device-frame calls.  8 canvases (24 MB at 1000^2: they stay in the 50 MB L2) beat the
+// whole batch at once on H100 (DESIGN.md section 4); BEVK_JPEG_CHUNK=n sets another size, 0 the whole batch.
+static int jpeg_chunk(int n) {
+  int chunk = std::min(n, 8);
+  if (const char* env = getenv("BEVK_JPEG_CHUNK")) chunk = atoi(env) > 0 ? std::min(n, atoi(env)) : n;
+  return chunk;
+}
+
+// ------------------------------------------------------------------ BEV canvases straight to JPEG (surroundBEV.py:340)
+// BevGenerator.__call__ then cv2.imencode: each chunk of frame-sets is rendered into ctx scratch and encoded there, and
+// only the streams come back.  Under BALANCE run_device's k_gain applies colour balance and the car to the chunk's
+// canvases before the encoder reads them.  The call is checked before the render set-up enqueues anything.
+static int to_jpeg_check(bevk_ctx* c, uint8_t* out, uint64_t* sizes) {
+  RET(need_plan(c));
+  RET(enc_call_check(c, out, sizes));
+  return jpeg_size_check(c->BW, c->BH);
+}
+
+int bevk_bev_run_to_jpeg(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, int batch, const uint8_t* car, int flags,
+                         int quality, uint8_t* out, uint64_t capacity, uint64_t* sizes) {
+  NvtxRange nvtx_call("bevk_bev_run_to_jpeg (host frames -> host JPEG streams)");
+  RET(use(c));
+  RET(bgr_only(flags, "bevk_bev_run_to_jpeg"));
+  RET(bgr_canvas_only(flags, "bevk_bev_run_to_jpeg"));
+  RET(to_jpeg_check(c, out, sizes));
+  const jpeg::Opts o = jpeg_ctx_opts(c, quality);
+  HostIngest h;
+  RET(ingest_setup(c, srcs, src_stride, batch, car, flags, &h));
+  // the ingest chunks are the encoder's: staging half = canvas half = encoder slot
+  return enc_chunks(c, "JPEG", batch, h.chunk, false, out, capacity, sizes, [&](int b0, int nb, int half) -> int {
+    uint8_t* dcanvas = nullptr;
+    RET(render_chunk(c, h, srcs, src_stride, flags, b0, nb, half, &dcanvas));
+    return jpeg_enqueue(c, half, EncIn{dcanvas, (long long)h.cbytes, (long long)c->BW * 3}, nb, c->BW, c->BH, o);
+  });
+}
+
+int bevk_bev_frames_to_jpeg(bevk_ctx* c, const void* const* frames, int batch, const void* d_car, int flags, int quality,
+                            uint8_t* out, uint64_t capacity, uint64_t* sizes) {
+  NvtxRange nvtx_call("bevk_bev_frames_to_jpeg (device frames -> host JPEG streams)");
+  RET(use(c));
+  RET(bgr_only(flags, "bevk_bev_frames_to_jpeg"));
+  RET(bgr_canvas_only(flags, "bevk_bev_frames_to_jpeg"));
+  RET(to_jpeg_check(c, out, sizes));
+  if (!frames) return fail(BEVK_ERR_ARG, "null pointer");
+  const jpeg::Opts o = jpeg_ctx_opts(c, quality);
+  Frames src;
+  RET(frames_src(c, frames, batch, &src));
+  // every chunk is rendered into the same canvas scratch: the next render is stream-ordered after the encoder read it
+  const int chunk = jpeg_chunk(batch);
+  RET(c->d_canvas.ensure((size_t)c->BW * c->BH * 3 * chunk));
+  uint8_t* dcanvas = c->d_canvas.as<uint8_t>();
+  return enc_chunks(c, "JPEG", batch, chunk, false, out, capacity, sizes, [&](int b0, int nb, int s) -> int {
+    Frames part = src;
+    if (part.table) part.table += (size_t)b0 * c->n_cam;
+    else part.base += (long long)b0 * c->n_cam * part.stride;
+    c->timed = false;
+    RET(run_device(c, part, nb, d_car, flags, dcanvas, 0, BEVK_MAX_CAMERAS));
+    return jpeg_enqueue(c, s, EncIn{dcanvas, (long long)c->BW * c->BH * 3, (long long)c->BW * 3}, nb, c->BW, c->BH, o);
+  });
+}
+
+// bevk_jpeg_encode is this call under the ctx's list, which bevk_jpeg_set_params checked as this call checks its own.
+int bevk_jpeg_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, int64_t row_stride, int n, int width, int height,
+                     int quality, uint8_t* out, uint64_t capacity, uint64_t* sizes) {
+  NvtxRange nvtx_call("bevk_jpeg_encode (device images -> host JPEG streams)");
+  RET(use(c));
+  return bevk_jpeg_encode_params(c, c->enc.params.data(), (int)c->enc.params.size(), d_images, image_stride, row_stride, n,
+                                 width, height, quality, out, capacity, sizes);
 }
 
 int bevk_jpeg_encode_params(bevk_ctx* c, const int* params, int n_params, const void* d_images, int64_t image_stride,
@@ -2862,27 +2869,14 @@ int bevk_jpeg_encode_params(bevk_ctx* c, const int* params, int n_params, const 
                             uint64_t* sizes) {
   NvtxRange nvtx_call("bevk_jpeg_encode_params (device images -> host JPEG streams)");
   RET(use(c));
-  std::vector<int> list;
   jpeg::Opts o;
-  RET(jpeg_call_params(params, n_params, &list, &o));
-  if (!d_images || !out || !sizes || n < 1) return fail(BEVK_ERR_ARG, "bad argument");
-  uint64_t bound = 0;
-  RET(bevk_jpeg_encode_bound(width, height, &bound));
-  if (row_stride < (int64_t)width * 3) return fail(BEVK_ERR_ARG, "row stride %lld < %d bytes", (long long)row_stride, width * 3);
-  if (n > 1 && image_stride < (int64_t)(height - 1) * row_stride + width * 3)
-    return fail(BEVK_ERR_ARG, "image stride %lld is smaller than one image", (long long)image_stride);
-  if (c->capturing) return fail(BEVK_ERR_ARG, "bevk_jpeg_encode_params synchronises and cannot be captured into a graph");
-  JpegIn in;
-  in.img = d_images; in.istride = image_stride; in.pitch = row_stride;
-  if (o.progressive) {
-    jpeg::normalise(quality, list.data(), n_params, &o);
-    return jpeg_prog_encode(c, o, in, n, width, height, out, capacity, sizes);
-  }
-  // baseline: the encoder of bevk_jpeg_encode under this list; the ctx's bevk_jpeg_set_params list is put back after
-  std::swap(c->enc.params, list);
-  const int r = jpeg_encode_device(c, in, n, width, height, quality, out, capacity, sizes);
-  std::swap(c->enc.params, list);
-  return r;
+  RET(jpeg_params_check(params, n_params, quality, &o));
+  RET(jpeg_size_check(width, height));
+  RET(check_device_images(d_images, image_stride, row_stride, n, width, height));
+  const EncIn in{d_images, image_stride, row_stride};
+  return enc_chunks(c, "JPEG", n, n, true, out, capacity, sizes, [&](int, int, int s) {
+    return o.progressive ? jpeg_prog_enqueue(c, s, in, n, width, height, o) : jpeg_enqueue(c, s, in, n, width, height, o);
+  });
 }
 
 int bevk_undistort_jpeg(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int interp, int quality,
@@ -2890,14 +2884,13 @@ int bevk_undistort_jpeg(bevk_ctx* c, int slot, const uint8_t* src, int sw, int s
   NvtxRange nvtx_call("bevk_undistort_jpeg (host frame -> undistorted JPEG)");
   RET(use(c));
   RET(need_undistorter(c, slot));
-  if (!out || !size) return fail(BEVK_ERR_ARG, "bad argument");
   const int dw = c->und[slot].cm.w, dh = c->und[slot].cm.h;
-  uint64_t bound = 0;
-  RET(bevk_jpeg_encode_bound(dw, dh, &bound));
-  RET(undistort_to_scratch(c, slot, src, sw, sh, sstride, 3, interp));
-  JpegIn in;
-  in.img = c->s_dst.p; in.pitch = (long long)dw * 3;
-  return jpeg_encode_device(c, in, 1, dw, dh, quality, out, capacity, size);
+  RET(jpeg_size_check(dw, dh));
+  const jpeg::Opts o = jpeg_ctx_opts(c, quality);
+  return enc_chunks(c, "JPEG", 1, 1, true, out, capacity, size, [&](int, int, int s) -> int {
+    RET(undistort_to_scratch(c, slot, src, sw, sh, sstride, 3, interp));
+    return jpeg_enqueue(c, s, EncIn{c->s_dst.p, 0, (long long)dw * 3}, 1, dw, dh, o);
+  });
 }
 
 // Device frames -> undistorted -> JPEG, chunk by chunk as bevk_bev_frames_to_jpeg: chunk i+1 is undistorted into the
@@ -2907,24 +2900,21 @@ int bevk_undistort_stack_jpeg(bevk_ctx* c, int slot, const void* d_src, int64_t 
                               uint64_t* sizes) {
   NvtxRange nvtx_call("bevk_undistort_stack_jpeg (device frames -> undistorted JPEG streams)");
   RET(use(c));
-  if (!out || !sizes) return fail(BEVK_ERR_ARG, "null host pointer");
-  if (c->capturing) return fail(BEVK_ERR_ARG, "bevk_undistort_stack_jpeg synchronises and cannot be captured into a graph");
   GatherArgs a;
   RET(stack_src_args(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, 3, n, &interp, &a));
   const int dw = a.dw, dh = a.dh;
-  uint64_t bound = 0;
-  RET(bevk_jpeg_encode_bound(dw, dh, &bound));
+  RET(jpeg_size_check(dw, dh));
+  const jpeg::Opts o = jpeg_ctx_opts(c, quality);
   const int chunk = jpeg_chunk(n);
   const long long ibytes = (long long)dw * dh * 3;
-  RET(c->s_dst.ensure((size_t)ibytes * chunk));
-  return jpeg_chunks(c, n, chunk, dw, dh, quality, false, out, capacity, sizes, [&](int b0, int nb, int, JpegIn* in) -> int {
+  return enc_chunks(c, "JPEG", n, chunk, false, out, capacity, sizes, [&](int b0, int nb, int s) -> int {
+    RET(c->s_dst.ensure((size_t)ibytes * chunk));
     GatherArgs part = a;
     part.src += (long long)b0 * a.sistride;
     part.n = nb;
     part.dst = c->s_dst.as<uint8_t>(); part.dpitch = (long long)dw * 3; part.distride = ibytes;
     RET(launch_undistort(c, slot, part, 3, interp));
-    in->img = c->s_dst.p; in->pitch = (long long)dw * 3; in->istride = ibytes;
-    return BEVK_OK;
+    return jpeg_enqueue(c, s, EncIn{c->s_dst.p, ibytes, (long long)dw * 3}, nb, dw, dh, o);
   });
 }
 
@@ -2978,16 +2968,10 @@ int bevk_png_encode_bound(int width, int height, const int* params, int n, uint6
 // last 2 bytes: at most 2^16 images per group.
 constexpr long long kPngGroupBytes = 1ll << 27, kPngLazyGroupBytes = 1ll << 25, kPngLazyGroupImages = 1ll << 16;
 
-static int png_encode_opts(bevk_ctx* c, const png::Opts& o, const void* d_images, int64_t image_stride, int64_t row_stride,
-                           int n, int width, int height, uint8_t* out, uint64_t capacity, uint64_t* sizes) {
+// Enqueue the PNG encoder over n width x height images into slot s, group by group; every group's streams land
+// compacted in the slot after the ones before (the running end at meta[2n]).
+static int png_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int width, int height, const png::Opts& o) {
   using namespace png;
-  RET(use(c));
-  if (!d_images || !out || !sizes || n < 1) return fail(BEVK_ERR_ARG, "bad argument");
-  if (c->capturing) return fail(BEVK_ERR_ARG, "PNG encoding synchronises and cannot be captured into a graph");
-  RET(png_size_check(width, height));
-  if (row_stride < (int64_t)width * 3) return fail(BEVK_ERR_ARG, "row stride %lld < %d bytes", (long long)row_stride, width * 3);
-  if (n > 1 && image_stride < (int64_t)(height - 1) * row_stride + width * 3)
-    return fail(BEVK_ERR_ARG, "image stride %lld is smaller than one image", (long long)image_stride);
   auto& e = c->png;
   const bool lazy = lazy_parse(o);
   const long long N = image_bytes(width, height), maxb = max_blocks(N), zb = zlib_bound(N);
@@ -3005,16 +2989,16 @@ static int png_encode_opts(bevk_ctx* c, const png::Opts& o, const void* d_images
   RET(e.hdr.ensure((size_t)g * maxb * kHdrWords * 4));
   RET(e.zw.ensure((size_t)g * zwords * 4));
   RET(e.zbytes.ensure((size_t)g * 8));
-  RET(e.meta.ensure((size_t)(2ll * n + 1) * 8));   // sizes[n], offsets[n], running end
-  RET(e.out.ensure((size_t)(n * bound)));
+  RET(slot_open(c, s, n, (size_t)(n * bound)));
+  unsigned long long* meta = c->enc_out.meta[s].as<unsigned long long>();
   using KeyIt = cub::TransformInputIterator<unsigned, RunStartKey, cub::CountingInputIterator<unsigned>>;
   using FlagIt = cub::TransformInputIterator<unsigned, SymbolFlag, cub::CountingInputIterator<unsigned>>;
   PngArgs a{};
-  a.istride = image_stride; a.pitch = row_stride; a.W = width; a.H = height; a.filters = o.filters; a.strategy = o.strategy;
+  a.istride = in.istride; a.pitch = in.pitch; a.W = width; a.H = height; a.filters = o.filters; a.strategy = o.strategy;
   a.N = N; a.maxb = maxb; a.zwords = zwords; a.maxchunks = maxch;
   a.f = e.f.as<uint8_t>(); a.rowad = e.rowad.as<Adler>(); a.syms = e.syms.as<uint16_t>(); a.nsym = e.nsym.as<unsigned>();
   a.blk = e.blk.as<Blk>(); a.codes = e.codes.as<uint32_t>(); a.hdr = e.hdr.as<uint32_t>(); a.zw = e.zw.as<uint32_t>();
-  a.zbytes = e.zbytes.as<unsigned long long>(); a.base = e.meta.as<unsigned long long>() + 2ll * n; a.out = e.out.as<uint8_t>();
+  a.zbytes = e.zbytes.as<unsigned long long>(); a.base = meta + 2ll * n; a.out = c->enc_out.out[s].as<uint8_t>();
   a.nblk = e.nblk.as<unsigned>(); a.level = o.level; a.flevel = zlib_flevel(o);
   size_t tmp1 = 0, tmp2 = 0;
   int key_bits = 15;
@@ -3045,10 +3029,10 @@ static int png_encode_opts(bevk_ctx* c, const png::Opts& o, const void* d_images
   CU(cudaEventRecord(c->ev0, c->stream));
   for (int b0 = 0; b0 < n; b0 += g) {
     const int gn = std::min(g, n - b0);
-    a.img = reinterpret_cast<const uint8_t*>(d_images) + b0 * image_stride;
+    a.img = reinterpret_cast<const uint8_t*>(in.img) + b0 * in.istride;
     a.n = gn;
-    a.sizes = e.meta.as<unsigned long long>() + b0;
-    a.out_off = e.meta.as<unsigned long long>() + n + b0;
+    a.out_off = meta + b0;
+    a.sizes = meta + n + b0;
     const long long total = gn * N;
     const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, (long long)c->n_sm * 16);
     k_png_filter<<<(unsigned)(gn * height), kPngThreads, 0, c->stream>>>(a);
@@ -3101,17 +3085,18 @@ static int png_encode_opts(bevk_ctx* c, const png::Opts& o, const void* d_images
     k_png_frame<<<(unsigned)((gn * maxch * 32 + kPngThreads - 1) / kPngThreads), kPngThreads, 0, c->stream>>>(a);
     LAUNCHED(c);
   }
-  CU(cudaEventRecord(c->ev1, c->stream));
-  c->timed = true;
-  CU(cudaMemcpyAsync(sizes, e.meta.p, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  unsigned long long all = 0;
-  for (int i = 0; i < n; ++i) all += sizes[i];
-  if (all > capacity)
-    return fail(BEVK_ERR_ARG, "the %d PNG streams take %llu bytes, capacity is %llu", n, all, (unsigned long long)capacity);
-  CU(cudaMemcpyAsync(out, e.out.p, all, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return BEVK_OK;
+  return slot_close(c, s, n);
+}
+
+// n device images through the PNG encoder under o, as one chunk: all streams or none
+static int png_encode_images(bevk_ctx* c, const png::Opts& o, const void* d_images, int64_t image_stride, int64_t row_stride,
+                             int n, int width, int height, uint8_t* out, uint64_t capacity, uint64_t* sizes) {
+  RET(png_size_check(width, height));
+  RET(check_device_images(d_images, image_stride, row_stride, n, width, height));
+  const EncIn in{d_images, image_stride, row_stride};
+  return enc_chunks(c, "PNG", n, n, true, out, capacity, sizes, [&](int, int, int s) {
+    return png_enqueue(c, s, in, n, width, height, o);
+  });
 }
 
 int bevk_png_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, int64_t row_stride, int n, int width, int height,
@@ -3120,7 +3105,7 @@ int bevk_png_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, int
   RET(use(c));
   png::Opts o;
   png::normalise(c->png.params.data(), (int)c->png.params.size(), &o);   // bevk_png_set_params checked the list
-  return png_encode_opts(c, o, d_images, image_stride, row_stride, n, width, height, out, capacity, sizes);
+  return png_encode_images(c, o, d_images, image_stride, row_stride, n, width, height, out, capacity, sizes);
 }
 
 // The parameter list per call, as cv2.imencode takes it; also zlib's hash-chain parse at levels 4..9 (deflate_slow,
@@ -3132,7 +3117,7 @@ int bevk_png_encode_params(bevk_ctx* c, const int* params, int n_params, const v
   RET(use(c));
   png::Opts o;
   RET(png_params_check(params, n_params, &o, true));
-  return png_encode_opts(c, o, d_images, image_stride, row_stride, n, width, height, out, capacity, sizes);
+  return png_encode_images(c, o, d_images, image_stride, row_stride, n, width, height, out, capacity, sizes);
 }
 
 // ------------------------------------------------------------------ CUDA graphs

@@ -24,7 +24,7 @@
 // The default (no parameters) is the 4:2:0 instance: geom(W, H), make_tables(q, ...), make_header(W, H, q, ...) and
 // encode_bound(W, H) are the general forms at Opts{2, 2, q, q}.
 //
-// Device pipeline for n equal-sized images (bevk_api.cu: jpeg_enqueue, then jpeg_collect copies the streams out):
+// Device pipeline for n equal-sized images (bevk_api.cu: jpeg_enqueue, then enc_collect copies the streams out):
 //   k_jpeg_blocks  one thread per 8x8 block: BGR -> samples with the edge rules, FDCT, quantise, int16 zigzag
 //                  coefficients (128 B per block) and the block's AC bit count
 //   (k_jpeg_blocks, k_jpeg_dc and k_jpeg_pack are instantiated per luma sampling HY x VY: the MCU layout is constant)
@@ -437,7 +437,7 @@ struct Opts {
 //   CHROMA_QUALITY   ignored below 0 or without LUMA_QUALITY; min(v, 100) otherwise.  Luma != chroma forces 4:4:4
 //   SAMPLING_FACTOR  0x111111 / 0x211111 / 0x121111 / 0x221111 / 0x411111 (Y h << 20 | v << 16); anything else 4:2:0
 //   RST_INTERVAL     clamped to [0, 65535]
-//   OPTIMIZE, PROGRESSIVE  on when non-zero
+//   OPTIMIZE, PROGRESSIVE  on above 0 (cv2 4.13 reads them as 0 / 1: values below 0 act as 0)
 inline bool normalise(int quality, const int* params, int n, Opts* o) {
   if (n < 0 || (n & 1) || (n && !params)) return false;
   int luma = -1, chroma = -1, sampling = 0;
@@ -447,8 +447,8 @@ inline bool normalise(int quality, const int* params, int n, Opts* o) {
     const int v = params[i + 1];
     switch (params[i]) {
       case kQuality: quality = v < 0 ? 0 : v > 100 ? 100 : v; break;
-      case kProgressive: r.progressive = v != 0; break;
-      case kOptimize: r.optimize = v != 0; break;
+      case kProgressive: r.progressive = v > 0; break;
+      case kOptimize: r.optimize = v > 0; break;
       case kRstInterval: r.rst = v < 0 ? 0 : v > 65535 ? 65535 : v; break;
       case kLumaQuality:
         if (v >= 0) {

@@ -81,8 +81,9 @@ __host__ __device__ inline Scan script(int s) {
 __host__ __device__ inline int ac_slot(int s) { return s < 6 ? s + 1 : s; }
 __host__ __device__ inline bool is_ac(int s) { return script(s).ss > 0; }
 
-// cv2 4.13 reads PROGRESSIVE and OPTIMIZE as 0 / 1 (values below 0 as 0, above 1 as 1); normalise() reads any non-zero
-// value as on, so the pairs of a list are mapped in place before it runs.
+// The pairs of a list with PROGRESSIVE and OPTIMIZE mapped in place to the 0 / 1 cv2 4.13 stores (values below 0 as 0,
+// above 1 as 1).  normalise() reads the flags the same way, so mapping first changes no Opts; the serial host encoder
+// (tests/host/jpeg_progressive.cu) maps its lists with it.
 inline void read_flags(int* params, int n) {
   for (int i = 0; i + 1 < n; i += 2)
     if (params[i] == kProgressive || params[i] == kOptimize) params[i + 1] = params[i + 1] > 0 ? 1 : 0;
@@ -353,7 +354,7 @@ inline unsigned long long progressive_bound(const Geom& g, int rst) {
 }
 
 
-// ------------------------------------------------------------------ device pipeline (bevk_api.cu: jpeg_prog_encode)
+// ------------------------------------------------------------------ device pipeline (bevk_api.cu: jpeg_prog_enqueue)
 // After k_jpeg_blocks, over the n * T blocks of all scans of all images (T = Layout.blk[10] per image, the "scan blocks";
 // global index J), and the n * S restart intervals ("segments", S = Layout.seg[10]):
 //   k_jpeg_prog_desc    per scan block: BlockRun (AC scans) -> desc bits; DC scans code a symbol or a bit per block

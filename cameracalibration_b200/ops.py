@@ -145,31 +145,6 @@ def jpeg_encode_bound(width: int, height: int, params=None) -> int:
     return n.value
 
 
-def _cuda_bgr_batch(arr):
-    """(device pointer, n, h, w, image stride, row stride) of a uint8 CUDA array [H][W][3] or [N][H][W][3] whose pixels
-    are dense (3-byte pixels, 1-byte channels); rows and images may be padded."""
-    iface = arr.__cuda_array_interface__
-    shape = tuple(iface["shape"])
-    if iface["typestr"] not in ("|u1", "<u1", "=u1"):
-        raise L.BevkError(f"CUDA array must be uint8, got typestr {iface['typestr']}")
-    if len(shape) not in (3, 4) or shape[-1] != 3:
-        raise L.BevkError(f"jpeg_encode takes uint8[H][W][3] or uint8[N][H][W][3] BGR images, got shape {shape}")
-    strides = iface.get("strides")
-    if strides is None:
-        strides = tuple(int(np.prod(shape[i + 1:])) for i in range(len(shape)))
-    if len(shape) == 3:
-        shape, strides = (1,) + shape, (0,) + tuple(strides)
-    n, h, w, _ = shape
-    if strides[3] != 1 or (w > 1 and strides[2] != 3):
-        raise L.BevkError("CUDA images must have dense BGR pixels (strides 3 and 1 along width and channels)")
-    ptr = iface["data"][0]
-    if not ptr:
-        raise L.BevkError("CUDA array has a null data pointer")
-    row = strides[1] if h > 1 else 3 * w
-    img = strides[0] if n > 1 else h * row
-    return int(ptr), n, h, w, int(img), int(row)
-
-
 def _cuda_images(arr, what):
     """(device pointer, rank, n, h, w, channels, image stride, row stride) of a uint8 CUDA array [H][W], [H][W][C] or
     [N][H][W][C] (C in 1, 3, 4) whose pixels are dense (C-byte pixels, 1-byte channels); rows and images may be padded."""
@@ -201,6 +176,41 @@ def _cuda_images(arr, what):
     return int(ptr), rank, n, h, w, ch, img, row
 
 
+def _split(out, sizes):
+    """The streams an encoding call wrote back to back into out, one ``bytes`` each."""
+    res, off = [], 0
+    for s in sizes:
+        res.append(out[off:off + s].tobytes())
+        off += s
+    return res
+
+
+def _encode(what, images, ctx, bound, call):
+    """The body of the encoding wrappers over uint8[H][W][3] or [N][H][W][3] BGR images: CUDA arrays
+    (``__cuda_array_interface__``) are read in place, NumPy input is uploaded once.  bound(w, h): the largest stream of one
+    image; call((ptr, image stride, row stride, n, w, h), out, capacity, sizes): the C call, run on torch's current
+    stream."""
+    from .sharding import _torch_current_stream
+    keep = images
+    if not hasattr(images, "__cuda_array_interface__"):
+        a = np.asarray(images)
+        if a.dtype != np.uint8 or a.ndim not in (3, 4) or a.shape[-1] != 3:
+            raise L.BevkError(f"{what} takes uint8[H][W][3] or uint8[N][H][W][3] BGR images, got {a.dtype} {a.shape}")
+        import torch
+        keep = torch.from_numpy(np.ascontiguousarray(a)).to(torch.device("cuda", ctx.device))
+    ptr, rank, n, h, w, ch, img_stride, row_stride = _cuda_images(keep, what)
+    if ch != 3 or rank == 2:
+        raise L.BevkError(f"{what} takes uint8[H][W][3] or uint8[N][H][W][3] BGR images")
+    if n < 1:
+        return []
+    cap = n * bound(w, h)
+    out = np.empty(cap, np.uint8)          # pages are only touched where streams land
+    sizes = (C.c_uint64 * n)()
+    with ctx.on_stream(_torch_current_stream(ctx.device)):
+        L.check(call((C.c_void_p(ptr), img_stride, row_stride, n, w, h), L.vptr(out), cap, sizes))
+    return _split(out, sizes)
+
+
 def jpeg_encode(images, quality: int = 95, ctx: L.Context | None = None, params=None) -> list[bytes]:
     """cv2.imencode('.jpg', img, [cv2.IMWRITE_JPEG_QUALITY, quality] + params) on the GPU, byte for byte, for one
     uint8[H][W][3] BGR image or a batch uint8[N][H][W][3].  params: cv2.imwrite's other JPEG pairs
@@ -210,29 +220,9 @@ def jpeg_encode(images, quality: int = 95, ctx: L.Context | None = None, params=
     torch's current stream; NumPy input is uploaded once.  Returns one ``bytes`` per image -- what cv2.imwrite would
     write to a .jpg file."""
     ctx = ctx or L.default_context()
-    from .sharding import _torch_current_stream
-    keep = images
-    if not hasattr(images, "__cuda_array_interface__"):
-        a = np.asarray(images)
-        if a.dtype != np.uint8 or a.ndim not in (3, 4) or a.shape[-1] != 3:
-            raise L.BevkError(f"jpeg_encode takes uint8[H][W][3] or uint8[N][H][W][3] BGR images, got {a.dtype} {a.shape}")
-        import torch
-        keep = torch.from_numpy(np.ascontiguousarray(a)).to(torch.device("cuda", ctx.device))
-    ptr, n, h, w, img_stride, row_stride = _cuda_bgr_batch(keep)
-    if n < 1:
-        return []
-    cap = n * jpeg_encode_bound(w, h, params)
-    out = np.empty(cap, np.uint8)          # pages are only touched where streams land
-    sizes = (C.c_uint64 * n)()
     jpeg_set_params(ctx, params)
-    with ctx.on_stream(_torch_current_stream(ctx.device)):
-        L.check(ctx.lib.bevk_jpeg_encode(ctx.h, C.c_void_p(ptr), img_stride, row_stride, n, w, h, int(quality), L.vptr(out),
-                                         cap, sizes))
-    res, off = [], 0
-    for s in sizes:
-        res.append(out[off:off + s].tobytes())
-        off += s
-    return res
+    return _encode("jpeg_encode", images, ctx, lambda w, h: jpeg_encode_bound(w, h, params),
+                   lambda img, out, cap, sizes: ctx.lib.bevk_jpeg_encode(ctx.h, *img, int(quality), out, cap, sizes))
 
 
 def jpeg_encode_params_bound(width: int, height: int, params=None) -> int:
@@ -249,29 +239,10 @@ def jpeg_encode_params(images, params, quality: int = 95, ctx: L.Context | None 
     cv2 4.13 reads it.  Takes the same images as jpeg_encode (NumPy, or CUDA arrays read in place on torch's current
     stream); the ctx's jpeg_set_params list is left as it was.  Returns one ``bytes`` per image."""
     ctx = ctx or L.default_context()
-    from .sharding import _torch_current_stream
-    keep = images
-    if not hasattr(images, "__cuda_array_interface__"):
-        a = np.asarray(images)
-        if a.dtype != np.uint8 or a.ndim not in (3, 4) or a.shape[-1] != 3:
-            raise L.BevkError(f"jpeg_encode_params takes uint8[H][W][3] or uint8[N][H][W][3] BGR images, got {a.dtype} {a.shape}")
-        import torch
-        keep = torch.from_numpy(np.ascontiguousarray(a)).to(torch.device("cuda", ctx.device))
-    ptr, n, h, w, img_stride, row_stride = _cuda_bgr_batch(keep)
-    if n < 1:
-        return []
-    cap = n * jpeg_encode_params_bound(w, h, params)
-    out = np.empty(cap, np.uint8)          # pages are only touched where streams land
-    sizes = (C.c_uint64 * n)()
     arr, k = _jpeg_params(params)
-    with ctx.on_stream(_torch_current_stream(ctx.device)):
-        L.check(ctx.lib.bevk_jpeg_encode_params(ctx.h, arr, k, C.c_void_p(ptr), img_stride, row_stride, n, w, h, int(quality),
-                                                L.vptr(out), cap, sizes))
-    res, off = [], 0
-    for s in sizes:
-        res.append(out[off:off + s].tobytes())
-        off += s
-    return res
+    return _encode("jpeg_encode_params", images, ctx, lambda w, h: jpeg_encode_params_bound(w, h, params),
+                   lambda img, out, cap, sizes: ctx.lib.bevk_jpeg_encode_params(ctx.h, arr, k, *img, int(quality), out, cap,
+                                                                                sizes))
 
 
 def png_set_params(ctx: L.Context, params=None):
@@ -299,29 +270,9 @@ def png_encode(images, ctx: L.Context | None = None, params=None) -> list[bytes]
     CUDA arrays (``__cuda_array_interface__``) are read in place, on torch's current stream; NumPy input is uploaded
     once.  Returns one ``bytes`` per image -- what cv2.imwrite would write to a .png file."""
     ctx = ctx or L.default_context()
-    from .sharding import _torch_current_stream
-    keep = images
-    if not hasattr(images, "__cuda_array_interface__"):
-        a = np.asarray(images)
-        if a.dtype != np.uint8 or a.ndim not in (3, 4) or a.shape[-1] != 3:
-            raise L.BevkError(f"png_encode takes uint8[H][W][3] or uint8[N][H][W][3] BGR images, got {a.dtype} {a.shape}")
-        import torch
-        keep = torch.from_numpy(np.ascontiguousarray(a)).to(torch.device("cuda", ctx.device))
-    ptr, n, h, w, img_stride, row_stride = _cuda_bgr_batch(keep)
-    if n < 1:
-        return []
-    cap = n * png_encode_bound(w, h)       # the bound holds under every list
-    out = np.empty(cap, np.uint8)          # pages are only touched where streams land
-    sizes = (C.c_uint64 * n)()
     arr, k = _jpeg_params(params)
-    with ctx.on_stream(_torch_current_stream(ctx.device)):
-        L.check(ctx.lib.bevk_png_encode_params(ctx.h, arr, k, C.c_void_p(ptr), img_stride, row_stride, n, w, h, L.vptr(out),
-                                               cap, sizes))
-    res, off = [], 0
-    for s in sizes:
-        res.append(out[off:off + s].tobytes())
-        off += s
-    return res
+    return _encode("png_encode", images, ctx, png_encode_bound,   # the bound holds under every list
+                   lambda img, out, cap, sizes: ctx.lib.bevk_png_encode_params(ctx.h, arr, k, *img, out, cap, sizes))
 
 
 def remap(src: np.ndarray, map1: np.ndarray, map2: np.ndarray | None, interpolation: int = INTER_LINEAR,
@@ -549,7 +500,7 @@ class Undistorter:
         with self.ctx.on_stream(_torch_current_stream(self.ctx.device)):
             L.check(self.ctx.lib.bevk_undistort_stack_jpeg(self.ctx.h, self.slot, C.c_void_p(ptr), simg, sw, sh, srow, n,
                                                            _interp(interpolation), int(quality), L.vptr(out), out.size, sizes))
-        return BevEngine._split(out, sizes)
+        return _split(out, sizes)
 
     def last_path(self) -> str:
         """Which gather the last call of this ctx launched: 'word' (k_gather4, 4 pixels per thread), 'byte' (k_gather) or
@@ -735,14 +686,6 @@ class BevEngine:
         jpeg_set_params(self.ctx, params)
         return out, (C.c_uint64 * batch)()
 
-    @staticmethod
-    def _split(out, sizes):
-        res, off = [], 0
-        for s in sizes:
-            res.append(out[off:off + s].tobytes())
-            off += s
-        return res
-
     def run_to_jpeg(self, frame_sets, quality: int = 95, car: np.ndarray | None = None, balance: bool = False,
                     params=None) -> list[bytes]:
         """run() followed by cv2.imencode('.jpg', canvas, [IMWRITE_JPEG_QUALITY, quality] + params) per frame-set, with
@@ -755,7 +698,7 @@ class BevEngine:
         out, sizes = self._streams(batch, params)
         L.check(self.ctx.lib.bevk_bev_run_to_jpeg(self.ctx.h, ptrs, stride, batch, carp, L.FLAG_BALANCE if balance else 0,
                                                   int(quality), L.vptr(out), out.size, sizes))
-        return self._split(out, sizes)
+        return _split(out, sizes)
 
     def run_jpeg(self, jpeg_sets, car: np.ndarray | None = None, balance: bool = False, out: np.ndarray | None = None):
         """jpeg_sets: list (batch) of lists (n_cam) of JPEG byte strings (the files cv2.imread would open).  The streams
@@ -1052,7 +995,7 @@ class BevEngine:
             L.check(self.ctx.lib.bevk_bev_frames_to_jpeg(self.ctx.h, table, batch, C.c_void_p(d_car),
                                                          L.FLAG_BALANCE if balance else 0, int(quality), L.vptr(out),
                                                          out.size, sizes))
-        return self._split(out, sizes)
+        return _split(out, sizes)
 
     def _cuda_frames(self, frames):
         """Device pointers (frame-set major) of the frames run_cuda takes."""

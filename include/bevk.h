@@ -356,9 +356,10 @@ int bevk_jpeg_encode_bound(int width, int height, uint64_t *bytes);
  *   SAMPLING_FACTOR (7)  0x111111 4:4:4, 0x211111 4:2:2, 0x121111 4:4:0, 0x221111 4:2:0, 0x411111 4:1:1; else 4:2:0
  *   LUMA_QUALITY (5)     >= 0: min(v, 100) replaces the call's quality (both tables unless CHROMA_QUALITY is given)
  *   CHROMA_QUALITY (6)   >= 0 and LUMA_QUALITY given: the chroma table's quality; luma != chroma forces 4:4:4
- *   OPTIMIZE (3)         != 0: per-image Huffman tables (libjpeg's jpeg_gen_optimal_table), built on the device
+ *   OPTIMIZE (3)         > 0: per-image Huffman tables (libjpeg's jpeg_gen_optimal_table), built on the device;
+ *                        <= 0 off (cv2 4.13 reads the flag as 0 / 1)
  *   RST_INTERVAL (4)     clamped to [0, 65535] MCUs; > 0 writes DRI and an RSTn marker after every interval but the last
- *   PROGRESSIVE (2)      0 as cv2's default; anything else is BEVK_ERR_UNSUPPORTED here (a multi-scan coder: the
+ *   PROGRESSIVE (2)      <= 0 off, as cv2 reads it; > 0 is BEVK_ERR_UNSUPPORTED here (a multi-scan coder: the
  *                        per-call bevk_jpeg_encode_params below writes it)
  * QUALITY (1) is refused (every encoding call takes quality itself), as are other keys and odd n (BEVK_ERR_ARG).  A
  * refused list leaves the ctx's params as they were.  The streams are byte-identical to

@@ -1,4 +1,4 @@
-"""GPU fuzz of the device JPEG encoder (bevk_jpeg_enc.cuh, jpeg_enqueue / jpeg_chunks in bevk_api.cu) against
+"""GPU fuzz of the device JPEG encoder (bevk_jpeg_enc.cuh, jpeg_enqueue / enc_chunks in bevk_api.cu) against
 cv2.imencode, byte for byte: the seeded corpus of tests/jpeg_cases.py through ops.jpeg_encode and bevk_jpeg_encode, one
 context reused across calls that change size, quality and batch, more than 2^32 entropy bits in one call,
 Undistorter.cuda_to_jpeg at every undistorted-width class mod 16 with the chunked pipeline at several chunk sizes, and

@@ -157,7 +157,7 @@ def test_refusals_and_capacity(torch, ops, L):
         arr, k = _ints(keep)
         assert ctx.lib.bevk_jpeg_set_params(ctx.h, arr, k) == 0
         for bad, rc in (([1, 90], -1), ([J.SAMPLING], -1), ([8, 1], -1), ([0, 0], -1), ([J.PROGRESSIVE, 1], -4),
-                        ([J.PROGRESSIVE, -3, J.OPTIMIZE, 1], -4), ([J.RST, 1, 1, 50], -1)):
+                        ([J.PROGRESSIVE, 3, J.OPTIMIZE, 1], -4), ([J.RST, 1, 1, 50], -1)):
             a, n = _ints(bad)
             assert ctx.lib.bevk_jpeg_set_params(ctx.h, a, n) == rc, bad
             b = ctypes.c_uint64()

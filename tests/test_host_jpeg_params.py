@@ -163,15 +163,20 @@ def test_normaliser_agrees_with_cv2(exe, tmp_path):
 
 
 def test_normaliser_flags_and_refusals(exe, tmp_path):
-    """Odd lists and unknown keys are refused; RST_INTERVAL is clamped to [0, 65535] and OPTIMIZE / PROGRESSIVE are on
-    for any non-zero value, as cv2 reads them (PROGRESSIVE streams are not written: no stream)."""
-    img = np.zeros((8, 8, 3), np.uint8)
-    recs = [(img, 95, p) for p in ([5], [8, 1], [0, 1], [4, 1], [4, 65536], [4, -1], [4, 70000], [3, 5], [3, -1], [2, 1],
-                                   [2, -2])]
+    """Odd lists and unknown keys are refused; RST_INTERVAL is clamped to [0, 65535].  OPTIMIZE and PROGRESSIVE are read
+    as cv2 reads them, on above 0 only: a PROGRESSIVE list is progressive exactly when cv2 writes SOF2 for it, and every
+    other list's stream equals cv2's (PROGRESSIVE streams are not written here: no stream)."""
+    img = np.random.default_rng(3).integers(0, 256, (24, 40, 3), dtype=np.uint8)
+    recs = [(img, 95, p) for p in ([5], [8, 1], [0, 1], [4, 1], [4, 65536], [4, -1], [4, 70000])]
     res = [o for o, *_ in host_run(exe, tmp_path, recs)]
-    assert [r["ok"] for r in res] == [0, 0, 0] + [1] * 8
+    assert [r["ok"] for r in res] == [0, 0, 0] + [1] * 4
     assert [r["rst"] for r in res[3:7]] == [1, 65535, 0, 65535]
-    assert [r["optimize"] for r in res[7:9]] == [1, 1] and [r["progressive"] for r in res[9:]] == [1, 1]
-    # cv2 writes a DRI for a positive interval and SOF2 for PROGRESSIVE (which the library refuses)
+    # cv2 writes a DRI for a positive interval
     assert header_opts(cv2_stream(img, 95, [4, 1]))[4]
-    assert any(m == 0xC2 for m, _ in segments(cv2_stream(img, 95, [2, 1])))
+    flags = [[3, -1], [3, 5], [2, -2], [2, 1]]
+    for p, (opts, got, _, _) in zip(flags, host_run(exe, tmp_path, [(img, 95, p) for p in flags])):
+        want = cv2_stream(img, 95, p)
+        assert opts["ok"] == 1, p
+        assert opts["progressive"] == any(m == 0xC2 for m, _ in segments(want)), (p, opts)
+        if not opts["progressive"]:
+            assert_same(got, want, p)
