@@ -1049,23 +1049,8 @@ int bevk_bev_tma_plan_info(bevk_ctx* c, int64_t* n_items, int64_t* n_shapes, int
 
 int64_t bevk_bev_last_h2d_bytes(bevk_ctx* c) { return c ? c->last_h2d_bytes : 0; }
 
-// Source pixel format of a call from its flags: 0 = BGR, YUV_NV12, YUV_I420, YUV_YUYV, YUV_UYVY.  YUV 4:2:0 needs an even
-// frame size and 4:2:2 an even width, as cv2 does.
 constexpr int kInFlags = BEVK_FLAG_NV12 | BEVK_FLAG_I420 | BEVK_FLAG_YUYV | BEVK_FLAG_UYVY;
-static int pixel_format(bevk_ctx* c, int flags, int* fmt) {
-  const int yuv = flags & kInFlags;
-  *fmt = 0;
-  if (!yuv) return BEVK_OK;
-  if (yuv & (yuv - 1)) return fail(BEVK_ERR_ARG, "the input flags BEVK_FLAG_NV12, _I420, _YUYV and _UYVY are exclusive");
-  if (yuv & (BEVK_FLAG_YUYV | BEVK_FLAG_UYVY)) {
-    if (c->FW & 1) return fail(BEVK_ERR_UNSUPPORTED, "YUV 4:2:2 frames need an even width, not %d", c->FW);
-    *fmt = yuv == BEVK_FLAG_YUYV ? YUV_YUYV : YUV_UYVY;
-    return BEVK_OK;
-  }
-  if ((c->FW | c->FH) & 1) return fail(BEVK_ERR_UNSUPPORTED, "YUV 4:2:0 frames need an even size, not %d x %d", c->FW, c->FH);
-  *fmt = yuv == BEVK_FLAG_NV12 ? YUV_NV12 : YUV_I420;
-  return BEVK_OK;
-}
+constexpr int kOutFlags = BEVK_FLAG_OUT_NV12 | BEVK_FLAG_OUT_I420;
 
 static bool packed_format(int fmt) { return fmt == YUV_YUYV || fmt == YUV_UYVY; }
 
@@ -1075,17 +1060,23 @@ static int64_t frame_bytes_of(const bevk_ctx* c, int fmt) {
   return !fmt ? 3 * px : packed_format(fmt) ? 2 * px : 3 * px / 2;
 }
 
-// Entry points that read BGR frames only refuse the YUV flags rather than read a YUV buffer as BGR.
-static int bgr_only(int flags, const char* fn) {
-  if (flags & kInFlags) return fail(BEVK_ERR_UNSUPPORTED, "%s takes BGR frames only (no YUV flags)", fn);
-  return BEVK_OK;
-}
-
-// Canvas format of a call from its flags: 0 = BGR, YUV_NV12, YUV_I420.  YUV needs an even canvas, as cv2 does.
-constexpr int kOutFlags = BEVK_FLAG_OUT_NV12 | BEVK_FLAG_OUT_I420;
-static int out_format(bevk_ctx* c, int flags, int* ofmt) {
-  const int o = flags & kOutFlags;
-  *ofmt = 0;
+// The source and canvas formats of a call from its flags: *fmt 0 = BGR, YUV_NV12, YUV_I420, YUV_YUYV, YUV_UYVY; *ofmt
+// 0 = BGR, YUV_NV12, YUV_I420.  `accepts` holds kInFlags if entry point fn reads YUV frames and kOutFlags if it writes
+// YUV canvases; the others are refused rather than read a YUV buffer as BGR or write BGR where YUV was asked for.  YUV
+// 4:2:0 needs an even frame or canvas size and 4:2:2 an even frame width, as cv2 does.
+static int read_flags(bevk_ctx* c, int flags, int accepts, const char* fn, int* fmt, int* ofmt) {
+  const int yuv = flags & kInFlags, o = flags & kOutFlags;
+  *fmt = *ofmt = 0;
+  if (yuv && !(accepts & kInFlags)) return fail(BEVK_ERR_UNSUPPORTED, "%s takes BGR frames only (no YUV flags)", fn);
+  if (yuv & (yuv - 1)) return fail(BEVK_ERR_ARG, "the input flags BEVK_FLAG_NV12, _I420, _YUYV and _UYVY are exclusive");
+  if (yuv & (BEVK_FLAG_YUYV | BEVK_FLAG_UYVY)) {
+    if (c->FW & 1) return fail(BEVK_ERR_UNSUPPORTED, "YUV 4:2:2 frames need an even width, not %d", c->FW);
+    *fmt = yuv == BEVK_FLAG_YUYV ? YUV_YUYV : YUV_UYVY;
+  } else if (yuv) {
+    if ((c->FW | c->FH) & 1) return fail(BEVK_ERR_UNSUPPORTED, "YUV 4:2:0 frames need an even size, not %d x %d", c->FW, c->FH);
+    *fmt = yuv == BEVK_FLAG_NV12 ? YUV_NV12 : YUV_I420;
+  }
+  if (o && !(accepts & kOutFlags)) return fail(BEVK_ERR_UNSUPPORTED, "%s writes BGR canvases only (no output flags)", fn);
   if (!o) return BEVK_OK;
   if (o == kOutFlags) return fail(BEVK_ERR_ARG, "BEVK_FLAG_OUT_NV12 and BEVK_FLAG_OUT_I420 are exclusive");
   if ((c->BW | c->BH) & 1) return fail(BEVK_ERR_UNSUPPORTED, "YUV 4:2:0 canvases need an even size, not %d x %d", c->BW, c->BH);
@@ -1093,18 +1084,11 @@ static int out_format(bevk_ctx* c, int flags, int* ofmt) {
   return BEVK_OK;
 }
 
-// Entry points that write BGR canvases only refuse the output flags rather than write BGR where YUV was asked for.
-static int bgr_canvas_only(int flags, const char* fn) {
-  if (flags & kOutFlags) return fail(BEVK_ERR_UNSUPPORTED, "%s writes BGR canvases only (no output flags)", fn);
-  return BEVK_OK;
-}
-
 int bevk_bev_host_copy_bytes(bevk_ctx* c, int flags, int64_t* h2d, int64_t* d2h) {
   RET(use(c));
   RET(need_plan(c));
   int fmt = 0, ofmt = 0;
-  RET(pixel_format(c, flags, &fmt));
-  RET(out_format(c, flags, &ofmt));
+  RET(read_flags(c, flags, kInFlags | kOutFlags, "bevk_bev_host_copy_bytes", &fmt, &ofmt));
   int64_t up = 0;
   for (int k = 0; k < c->n_cam; ++k) {
     if (flags & BEVK_FLAG_BALANCE) { up += frame_bytes_of(c, fmt); continue; }
@@ -1180,7 +1164,7 @@ static int launch_bev_tma(bevk_ctx* c, const TmaParams& P, int nbu, bool bal) {
   const TmaConfig cfg = kTmaConfigs[c->tma_cfg];
   const unsigned blocks = (unsigned)std::max<long long>(1, std::min<long long>(units, c->tma_grid[c->tma_cfg][variant]));
   const size_t smem = bev_tma_smem_bytes(nbu, cfg.fs, cfg.stages, cfg.eg);
-  const bool scatter = P.world != 0;   // peer-store output: only without BALANCE (run_device checks)
+  const bool scatter = P.world != 0;   // peer-store output: only without BALANCE (render runs windows without it)
 #ifdef BEVK_TRACE
   // slot timeline (tools/gpu/trace_slots.py): the 12th launch of the process records clock64 stamps of the first 8 CTAs
   // into BEVK_TRACE_FILE; a -DBEVK_TRACE build is for this measurement only
@@ -1313,79 +1297,30 @@ static int launch_gain(bevk_ctx* c, uint8_t* out, int batch, const unsigned long
   return BEVK_OK;
 }
 
-// run_device flag, not part of the ABI: with BALANCE, stop at the raw composed canvas and its channel sums (d_csum).
-// k_canvas_yuv<..., true> applies the gains and the car, so k_gain does not run.  (Without BALANCE the write-out adds the car.)
-constexpr int kFlagRawBalance = 1 << 30;
+// What every check and launch of one render reads.  The frames are `planes` when given (YUV only; src is then planes->f[0]),
+// else src: a frame stack or a device table of frame pointers, and dense YUV frames come as a stack.  Without a window
+// the render writes whole canvases of format ofmt to out: BGR straight there, YUV as BGR into `scratch` (dense, 4-byte
+// aligned, batch canvases) and converted from there by k_canvas_yuv.  A window (a shard's slab, or peer stores, where out
+// is null) renders the cameras [cam_lo, cam_hi) without car or colour balance: under BALANCE its caller has balanced
+// the frames of src already, and the balance of the canvases follows the compose.
+struct RenderReq {
+  Frames src; const YuvPlanes* planes = nullptr; int fmt = 0;   // the source and its pixel format
+  int batch = 0; bool bal = false; const void* car = nullptr;
+  void* out = nullptr; int ofmt = 0;                            // the canvases and their format
+  const OutWin* win = nullptr;
+  int cam_lo = 0, cam_hi = BEVK_MAX_CAMERAS;
+  uint8_t* scratch = nullptr;
+};
 
-// YUV frames (BEVK_FLAG_NV12 / _I420) are `planes` when given (src then only has to be non-null), else the dense stack src.
-static int run_device(bevk_ctx* c, Frames src, int batch, const void* d_car, int flags, void* d_out, int cam_lo, int cam_hi,
-                      const OutWin* win = nullptr, const YuvPlanes* planes = nullptr) {
-  NvtxRange nvtx_render("bevk render (fused BEV kernels)");
+// Every refusal of a render, before anything is enqueued.
+static int render_check(bevk_ctx* c, const RenderReq& q) {
   RET(need_plan(c));
-  if ((!src.table && !src.base) || (!d_out && !(win && win->world))) return fail(BEVK_ERR_ARG, "null device pointer");
-  if (batch < 1 || batch > 65535) return fail(BEVK_ERR_ARG, "batch %d out of range [1,65535]", batch);
-  const bool bal = (flags & BEVK_FLAG_BALANCE) != 0;
-  const int nf = batch * c->n_cam;
-  int fmt = 0;
-  RET(pixel_format(c, flags, &fmt));
-  if ((bal || fmt) && nf > 65535)
-    return fail(BEVK_ERR_ARG, "batch %d x %d cameras exceeds the 65535 frames of a BALANCE or YUV call", batch, c->n_cam);
-  if (fmt && (win || cam_lo != 0 || cam_hi < c->n_cam)) return fail(BEVK_ERR_UNSUPPORTED, "YUV frames render whole canvases only");
-  if (fmt && !planes && src.table) return fail(BEVK_ERR_UNSUPPORTED, "dense YUV frames come as a frame stack");
-  RenderParams R{};
-  R.n_cam = c->n_cam; R.FW = c->FW; R.FH = c->FH; R.pitch = (unsigned)c->FW * 3u;
-  R.out = reinterpret_cast<uint8_t*>(d_out); R.BW = c->BW; R.BH = c->BH;
-  R.canvas_bytes = (long long)c->BW * c->BH * 3;
-  R.out_pitch = c->BW * 3; R.ox = 0; R.oy = 0; R.ox1 = c->BW; R.oy1 = c->BH;
-  if (win) {
-    if (bal || d_car) return fail(BEVK_ERR_ARG, "balance and the car overlay need the full canvas");
-    R.canvas_bytes = win->stride; R.out_pitch = win->pitch; R.ox = win->ox; R.oy = win->oy; R.ox1 = win->ox1; R.oy1 = win->oy1;
-  }
-  R.car = reinterpret_cast<const uint8_t*>(d_car);
-  R.cam_lo = cam_lo; R.cam_hi = cam_hi;
-  R.n_tiles = (int)c->n_tiles; R.batch = batch;
-  // frame-sets per work unit: 4 amortises the LUT decode over a batch; 1 for single frames
-  int nbu = batch >= 4 ? 4 : 1;
-  if (c->nb_override) nbu = c->nb_override;
-  if (c->timed && !c->capturing) CU(cudaEventRecord(c->ev0, c->stream));
-  Frames gsrc = src;                           // what the fused gather reads
-  if (bal) {
-    RET(c->d_csum.ensure((size_t)batch * 24));
-    CU(cudaMemsetAsync(c->d_csum.p, 0, (size_t)batch * 24, c->stream));
-    if (!fmt) RET(balance_prepass(c, src, batch, 0, c->n_cam, nullptr, 1, &gsrc));
-    R.csum = c->d_csum.as<unsigned long long>();
-  }
-  if (fmt) RET(yuv_prepass(c, fmt, src, planes, batch, bal, &gsrc));   // BGR copies of the sampled spans (balanced with BALANCE)
-  // TMA-staged kernel for frame stacks (16-byte aligned base and stride); global-offset gather otherwise
-  const bool use_tma = c->tma_planned && !gsrc.table && (reinterpret_cast<uintptr_t>(gsrc.base) & 15) == 0 && (gsrc.stride & 15) == 0 &&
-                       gsrc.stride >= (long long)R.pitch * c->FH && (nbu == 1 || nbu == 4);
-  if (use_tma) {
-    TmaParams T{R};
-    T.tiles = c->d_ttiles.as<int4>(); T.items = c->d_titems.as<TmaItem>(); T.lut = c->d_tlut.as<uint4>();
-    RET(stack_maps(c, gsrc.base, gsrc.stride, nf, &T.maps));
-    T.base = gsrc.base; T.frame_stride = gsrc.stride;
-    T.backoff_ns = c->tma_backoff_ns;
-    if (win && win->world) { for (int r = 0; r < SHARD_MAX_RANKS; ++r) T.peer[r] = win->peer[r]; T.world = win->world; T.src_off = win->src_off; }
-    RET(c->d_unit_counter.ensure(256));
-    CU(cudaMemsetAsync(c->d_unit_counter.p, 0, 4, c->stream));
-    T.unit_counter = c->d_unit_counter.as<unsigned>();
-    RET(launch_bev_tma(c, T, nbu, bal));
-    c->last_path = 2;
-  } else {
-    if (win && win->world) return fail(BEVK_ERR_UNSUPPORTED, "peer-store output needs the TMA-staged kernel (a 16-byte friendly frame stack)");
-    BevParams P{R};
-    P.tiles = c->d_tiles.as<int4>(); P.items = c->d_items.as<BevItem>(); P.lut = c->d_lut.as<uint4>();
-    P.srcs = gsrc;
-    const long long units = c->n_tiles * ((batch + nbu - 1) / nbu);
-    const int variant = (bal ? 3 : 0) + (nbu == 8 ? 2 : (nbu == 4 ? 1 : 0));
-    const unsigned bev_blocks = (unsigned)std::max<long long>(1, std::min<long long>(units, c->bev_grid[variant]));
-    void* args[] = {&P};
-    CU(cudaLaunchKernel(kBevFns[variant], dim3(bev_blocks), dim3(256), args, bev_smem_bytes(bal, nbu), c->stream));
-    LAUNCHED(c);
-    c->last_path = 1;
-  }
-  if (bal && !(flags & kFlagRawBalance)) RET(launch_gain(c, R.out, batch, R.csum, R.car));
-  if (c->timed && !c->capturing) CU(cudaEventRecord(c->ev1, c->stream));
+  if ((!q.src.table && !q.src.base) || (!q.out && !(q.win && q.win->world))) return fail(BEVK_ERR_ARG, "null device pointer");
+  if (q.batch < 1 || q.batch > 65535) return fail(BEVK_ERR_ARG, "batch %d out of range [1,65535]", q.batch);
+  if ((q.bal || q.fmt) && (long long)q.batch * c->n_cam > 65535)
+    return fail(BEVK_ERR_ARG, "batch %d x %d cameras exceeds the 65535 frames of a BALANCE or YUV call", q.batch, c->n_cam);
+  if (q.fmt && (q.win || q.cam_lo != 0 || q.cam_hi < c->n_cam)) return fail(BEVK_ERR_UNSUPPORTED, "YUV frames render whole canvases only");
+  if (q.fmt && !q.planes && q.src.table) return fail(BEVK_ERR_UNSUPPORTED, "dense YUV frames come as a frame stack");
   return BEVK_OK;
 }
 
@@ -1409,46 +1344,106 @@ static int launch_canvas_yuv(bevk_ctx* c, int ofmt, const uint8_t* canvases, int
   return BEVK_OK;
 }
 
-// One whole-canvas render in canvas format ofmt (out_format): BGR canvases straight into d_out; YUV ones as BGR into
-// `scratch`, converted from there into d_out by k_canvas_yuv.  With BALANCE the render stops at the raw canvas and the
-// conversion applies colour balance and the car, so k_gain does not run.  The one conversion step of the host and the
-// device entry points.
-static int render_to(bevk_ctx* c, Frames src, int batch, const void* d_car, int flags, int ofmt, uint8_t* scratch, void* d_out,
-                     const YuvPlanes* planes = nullptr) {
-  if (!ofmt) return run_device(c, src, batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS, nullptr, planes);
-  RET(run_device(c, src, batch, d_car, (flags & ~kOutFlags) | kFlagRawBalance, scratch, 0, BEVK_MAX_CAMERAS, nullptr, planes));
-  return launch_canvas_yuv(c, ofmt, scratch, batch, (flags & BEVK_FLAG_BALANCE) ? c->d_csum.as<unsigned long long>() : nullptr,
-                           d_car, d_out);
+// One render that render_check passed: the BALANCE or YUV pre-pass, the fused kernel, then k_gain (BGR canvases under
+// BALANCE) or k_canvas_yuv (YUV canvases, which under BALANCE applies colour balance and the car itself).  Only enqueues.
+static int render(bevk_ctx* c, const RenderReq& q) {
+  NvtxRange nvtx_render("bevk render (fused BEV kernels)");
+  const bool bal = q.bal && !q.win;
+  const int nf = q.batch * c->n_cam;
+  RenderParams R{};
+  R.n_cam = c->n_cam; R.FW = c->FW; R.FH = c->FH; R.pitch = (unsigned)c->FW * 3u;
+  R.out = reinterpret_cast<uint8_t*>(q.ofmt ? q.scratch : q.out); R.BW = c->BW; R.BH = c->BH;
+  R.canvas_bytes = (long long)c->BW * c->BH * 3;
+  R.out_pitch = c->BW * 3; R.ox = 0; R.oy = 0; R.ox1 = c->BW; R.oy1 = c->BH;
+  const OutWin* w = q.win;   // null: the whole canvas
+  if (w) { R.canvas_bytes = w->stride; R.out_pitch = w->pitch; R.ox = w->ox; R.oy = w->oy; R.ox1 = w->ox1; R.oy1 = w->oy1; }
+  R.car = reinterpret_cast<const uint8_t*>(q.car);
+  R.cam_lo = q.cam_lo; R.cam_hi = q.cam_hi;
+  R.n_tiles = (int)c->n_tiles; R.batch = q.batch;
+  // frame-sets per work unit: 4 amortises the LUT decode over a batch; 1 for single frames
+  int nbu = q.batch >= 4 ? 4 : 1;
+  if (c->nb_override) nbu = c->nb_override;
+  Frames gsrc = q.src;                         // what the fused gather reads
+  if (bal) {
+    RET(c->d_csum.ensure((size_t)q.batch * 24));
+    CU(cudaMemsetAsync(c->d_csum.p, 0, (size_t)q.batch * 24, c->stream));
+    if (!q.fmt) RET(balance_prepass(c, q.src, q.batch, 0, c->n_cam, nullptr, 1, &gsrc));
+    R.csum = c->d_csum.as<unsigned long long>();
+  }
+  if (q.fmt) RET(yuv_prepass(c, q.fmt, q.src, q.planes, q.batch, bal, &gsrc));   // BGR copies of the sampled spans (balanced with BALANCE)
+  // TMA-staged kernel for frame stacks (16-byte aligned base and stride); global-offset gather otherwise
+  const bool use_tma = c->tma_planned && !gsrc.table && (reinterpret_cast<uintptr_t>(gsrc.base) & 15) == 0 && (gsrc.stride & 15) == 0 &&
+                       gsrc.stride >= (long long)R.pitch * c->FH && (nbu == 1 || nbu == 4);
+  if (use_tma) {
+    TmaParams T{R};
+    T.tiles = c->d_ttiles.as<int4>(); T.items = c->d_titems.as<TmaItem>(); T.lut = c->d_tlut.as<uint4>();
+    RET(stack_maps(c, gsrc.base, gsrc.stride, nf, &T.maps));
+    T.base = gsrc.base; T.frame_stride = gsrc.stride;
+    T.backoff_ns = c->tma_backoff_ns;
+    if (w && w->world) { for (int r = 0; r < SHARD_MAX_RANKS; ++r) T.peer[r] = w->peer[r]; T.world = w->world; T.src_off = w->src_off; }
+    RET(c->d_unit_counter.ensure(256));
+    CU(cudaMemsetAsync(c->d_unit_counter.p, 0, 4, c->stream));
+    T.unit_counter = c->d_unit_counter.as<unsigned>();
+    RET(launch_bev_tma(c, T, nbu, bal));
+    c->last_path = 2;
+  } else {
+    if (w && w->world) return fail(BEVK_ERR_UNSUPPORTED, "peer-store output needs the TMA-staged kernel (a 16-byte friendly frame stack)");
+    BevParams P{R};
+    P.tiles = c->d_tiles.as<int4>(); P.items = c->d_items.as<BevItem>(); P.lut = c->d_lut.as<uint4>();
+    P.srcs = gsrc;
+    const long long units = c->n_tiles * ((q.batch + nbu - 1) / nbu);
+    const int variant = (bal ? 3 : 0) + (nbu == 8 ? 2 : (nbu == 4 ? 1 : 0));
+    const unsigned bev_blocks = (unsigned)std::max<long long>(1, std::min<long long>(units, c->bev_grid[variant]));
+    void* args[] = {&P};
+    CU(cudaLaunchKernel(kBevFns[variant], dim3(bev_blocks), dim3(256), args, bev_smem_bytes(bal, nbu), c->stream));
+    LAUNCHED(c);
+    c->last_path = 1;
+  }
+  if (q.ofmt) return launch_canvas_yuv(c, q.ofmt, q.scratch, q.batch, R.csum, q.car, q.out);
+  if (bal) RET(launch_gain(c, R.out, q.batch, R.csum, R.car));
+  return BEVK_OK;
 }
 
-// The device entry points' render: run_device for BGR canvases; for YUV ones render_to over the whole batch through
-// d_out_bgr.  Rendering in chunks of 8 frame-sets, so that the conversion reads canvases still in L2, was slower: the
-// fused kernels lose more on the smaller batches than the conversion gains (DESIGN.md section 4).  Only enqueues;
-// bevk_last_kernel_ms covers the render and the conversion.
-static int run_canvases(bevk_ctx* c, Frames src, int batch, const void* d_car, int flags, void* d_out,
-                        const YuvPlanes* planes = nullptr) {
-  int ofmt = 0;
-  RET(need_plan(c));
-  RET(out_format(c, flags, &ofmt));
-  if (!ofmt) return run_device(c, src, batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS, nullptr, planes);
-  if (!d_out) return fail(BEVK_ERR_ARG, "null device pointer");
-  if (batch < 1 || batch > 65535) return fail(BEVK_ERR_ARG, "batch %d out of range [1,65535]", batch);
-  RET(c->d_out_bgr.ensure((size_t)c->BW * c->BH * 3 * batch));
-  const bool timed = c->timed;
-  if (timed && !c->capturing) CU(cudaEventRecord(c->ev0, c->stream));
-  c->timed = false;   // the render records no events of its own
-  const int rc = render_to(c, src, batch, d_car, flags, ofmt, c->d_out_bgr.as<uint8_t>(), d_out, planes);
-  c->timed = timed;
-  RET(rc);
-  if (timed && !c->capturing) CU(cudaEventRecord(c->ev1, c->stream));
+// bevk_last_kernel_ms reads the window between ev0 and ev1 that a timed call records around its kernels (not inside a
+// graph capture); c->timed says that they hold the last timed call's window, and untimed calls clear it.
+static int time_begin(bevk_ctx* c) {
+  if (!c->capturing) CU(cudaEventRecord(c->ev0, c->stream));
+  return BEVK_OK;
+}
+
+static int time_end(bevk_ctx* c) {
+  if (!c->capturing) CU(cudaEventRecord(c->ev1, c->stream));
+  c->timed = true;
+  return BEVK_OK;
+}
+
+// The device entry points: one checked, timed render.  YUV canvases are rendered through d_out_bgr over the whole batch.
+// Rendering in chunks of 8 frame-sets, so that the conversion reads canvases still in L2, was slower: the fused kernels
+// lose more on the smaller batches than the conversion gains (DESIGN.md section 4).
+static int render_timed(bevk_ctx* c, RenderReq q) {
+  RET(render_check(c, q));
+  if (q.ofmt) {
+    RET(c->d_out_bgr.ensure((size_t)c->BW * c->BH * 3 * q.batch));
+    q.scratch = c->d_out_bgr.as<uint8_t>();
+  }
+  RET(time_begin(c));
+  RET(render(c, q));
+  return time_end(c);
+}
+
+// A whole-canvas render request of the entry point fn with the given flags (`accepts`: see read_flags).
+static int canvas_req(bevk_ctx* c, const char* fn, int flags, int accepts, Frames src, int batch, const void* d_car, void* d_out,
+                      RenderReq* q) {
+  RET(read_flags(c, flags, accepts, fn, &q->fmt, &q->ofmt));
+  q->src = src; q->batch = batch; q->bal = (flags & BEVK_FLAG_BALANCE) != 0; q->car = d_car; q->out = d_out;
   return BEVK_OK;
 }
 
 int bevk_bev_run_device(bevk_ctx* c, const void* d_srcs, int batch, const void* d_car, int flags, void* d_out) {
   RET(use(c));
-  RET(bgr_only(flags, "bevk_bev_run_device"));
-  c->timed = true;
-  return run_canvases(c, Frames(d_srcs), batch, d_car, flags, d_out);
+  RenderReq q;
+  RET(canvas_req(c, "bevk_bev_run_device", flags, kOutFlags, Frames(d_srcs), batch, d_car, d_out, &q));
+  return render_timed(c, q);
 }
 
 // frames[i] == frames[0] + i * stride with a 16-byte friendly stride?  (a frame stack: the TMA-staged kernel applies)
@@ -1463,8 +1458,23 @@ static bool affine_table(const void* const* frames, size_t n, long long* stride)
   return true;
 }
 
-// The frames of a host table of device pointers as run_device reads them: a frame stack when the table describes one
-// (no table upload at all), else the ctx's device copy of the table, uploaded only when its contents change.
+// The host table tab in the device buffer d, whose contents `cached` remembers: uploaded only when they change.  The
+// source is pageable, so the driver stages it before returning, and stream order protects launches still reading the
+// old table.  A failed upload leaves nothing cached, so that the next call uploads again.
+static int upload_table(bevk_ctx* c, const void* const* tab, size_t n, DevBuf& d, std::vector<const void*>& cached, const char* what) {
+  if (cached.size() == n && memcmp(cached.data(), tab, n * sizeof(void*)) == 0) return BEVK_OK;
+  RET(d.ensure(n * sizeof(void*)));
+  cached.assign(tab, tab + n);
+  const cudaError_t e = cudaMemcpyAsync(d.p, cached.data(), n * sizeof(void*), cudaMemcpyHostToDevice, c->stream);
+  if (e != cudaSuccess) {
+    cached.clear();
+    return fail(BEVK_ERR_CUDA, "%s upload: %s", what, cudaGetErrorString(e));
+  }
+  return BEVK_OK;
+}
+
+// The frames of a host table of device pointers as render reads them: a frame stack when the table describes one
+// (no table upload at all), else the ctx's device copy of the table.
 static int frames_src(bevk_ctx* c, const void* const* frames, int batch, Frames* src) {
   if (batch < 1) return fail(BEVK_ERR_ARG, "batch must be >= 1");
   const size_t n = (size_t)batch * c->n_cam;
@@ -1475,16 +1485,7 @@ static int frames_src(bevk_ctx* c, const void* const* frames, int batch, Frames*
     *src = Frames(frames[0], stride);
     return BEVK_OK;
   }
-  if (c->user_tab.size() != n || memcmp(c->user_tab.data(), frames, n * sizeof(void*)) != 0) {
-    RET(c->d_user_ptrs.ensure(n * sizeof(void*)));
-    c->user_tab.assign(frames, frames + n);
-    // pageable source: the driver stages it before returning, and stream order protects launches still reading the old table
-    const cudaError_t e = cudaMemcpyAsync(c->d_user_ptrs.p, c->user_tab.data(), n * sizeof(void*), cudaMemcpyHostToDevice, c->stream);
-    if (e != cudaSuccess) {
-      c->user_tab.clear();   // nothing cached: the next call uploads again
-      return fail(BEVK_ERR_CUDA, "frame table upload: %s", cudaGetErrorString(e));
-    }
-  }
+  RET(upload_table(c, frames, n, c->d_user_ptrs, c->user_tab, "frame table"));
   *src = Frames(c->d_user_ptrs.p);
   return BEVK_OK;
 }
@@ -1493,15 +1494,22 @@ int bevk_bev_run_frames(bevk_ctx* c, const void* const* frames, int batch, const
   RET(use(c));
   RET(need_plan(c));
   if (!frames || !d_out) return fail(BEVK_ERR_ARG, "null pointer");
-  RET(bgr_only(flags, "bevk_bev_run_frames"));
-  Frames src;
-  RET(frames_src(c, frames, batch, &src));
-  c->timed = true;
-  return run_canvases(c, src, batch, d_car, flags, d_out);
+  RenderReq q;
+  RET(canvas_req(c, "bevk_bev_run_frames", flags, kOutFlags, Frames(), batch, d_car, d_out, &q));
+  RET(frames_src(c, frames, batch, &q.src));
+  return render_timed(c, q);
 }
 
-static int check_stack(bevk_ctx* c, const void* d_frames, int64_t frame_stride) {
+// A frame stack of pixel format fmt.  BGR frames need 4-byte alignment; YUV frames are read byte- or word-wise by
+// k_vsum_yuv / k_yuv_spans only, so any base and stride will do.
+static int check_stack(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int fmt = 0) {
   if (!d_frames) return fail(BEVK_ERR_ARG, "null frame stack");
+  if (fmt) {
+    if (frame_stride < frame_bytes_of(c, fmt))
+      return fail(BEVK_ERR_ARG, "frame_stride %lld smaller than a YUV %s frame", (long long)frame_stride,
+                  packed_format(fmt) ? "4:2:2" : "4:2:0");
+    return BEVK_OK;
+  }
   if (reinterpret_cast<uintptr_t>(d_frames) & 3) return fail(BEVK_ERR_ARG, "frame stack not 4-byte aligned");
   if (frame_stride < (int64_t)c->FW * c->FH * 3 || (frame_stride & 3)) return fail(BEVK_ERR_ARG, "frame_stride %lld smaller than a frame or not a multiple of 4", (long long)frame_stride);
   return BEVK_OK;
@@ -1509,31 +1517,23 @@ static int check_stack(bevk_ctx* c, const void* d_frames, int64_t frame_stride) 
 
 int bevk_bev_run_stack(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, const void* d_car, int flags, void* d_out) {
   RET(use(c));
-  int fmt = 0;
-  RET(pixel_format(c, flags, &fmt));
-  if (fmt) {   // YUV frames are read byte- or word-wise by k_vsum_yuv / k_yuv_spans only: any base and stride will do
-    if (!d_frames) return fail(BEVK_ERR_ARG, "null frame stack");
-    if (frame_stride < frame_bytes_of(c, fmt))
-      return fail(BEVK_ERR_ARG, "frame_stride %lld smaller than a YUV %s frame", (long long)frame_stride,
-                  packed_format(fmt) ? "4:2:2" : "4:2:0");
-  } else {
-    RET(check_stack(c, d_frames, frame_stride));
-  }
-  c->timed = true;
-  return run_canvases(c, Frames(d_frames, frame_stride), batch, d_car, flags, d_out);
+  RenderReq q;
+  RET(canvas_req(c, "bevk_bev_run_stack", flags, kInFlags | kOutFlags, Frames(d_frames, frame_stride), batch, d_car, d_out, &q));
+  RET(check_stack(c, d_frames, frame_stride, q.fmt));
+  return render_timed(c, q);
 }
 
-// The checks the two plane entry points share, before anything is enqueued: a YUV flag, batch, and pitches that cover
-// their planes' rows (plane 1 not for 4:2:2, plane 2 only for I420).
-static int check_yuv_planes(bevk_ctx* c, const int64_t* pitch, int batch, int flags, int* fmt, int* n_planes) {
+// The request of the two plane entry points, before anything is enqueued: a YUV flag and pitches that cover their
+// planes' rows (plane 1 not for 4:2:2, plane 2 only for I420).
+static int yuv_planes_req(bevk_ctx* c, const char* fn, const int64_t* pitch, int batch, const void* d_car, int flags, void* d_out,
+                          RenderReq* q, int* n_planes) {
   RET(need_plan(c));
-  RET(pixel_format(c, flags, fmt));
-  if (!*fmt) return fail(BEVK_ERR_ARG, "YUV planes need BEVK_FLAG_NV12, _I420, _YUYV or _UYVY");
+  RET(canvas_req(c, fn, flags, kInFlags | kOutFlags, Frames(), batch, d_car, d_out, q));
+  const int fmt = q->fmt;
+  if (!fmt) return fail(BEVK_ERR_ARG, "YUV planes need BEVK_FLAG_NV12, _I420, _YUYV or _UYVY");
   if (!pitch) return fail(BEVK_ERR_ARG, "null pitch array");
-  if (batch < 1 || (long long)batch * c->n_cam > 65535)
-    return fail(BEVK_ERR_ARG, "batch %d x %d cameras out of range [1,65535] frames", batch, c->n_cam);
-  *n_planes = packed_format(*fmt) ? 1 : *fmt == YUV_NV12 ? 2 : 3;
-  const int row[3] = {packed_format(*fmt) ? 2 * c->FW : c->FW, *fmt == YUV_NV12 ? c->FW : c->FW / 2, c->FW / 2};
+  *n_planes = packed_format(fmt) ? 1 : fmt == YUV_NV12 ? 2 : 3;
+  const int row[3] = {packed_format(fmt) ? 2 * c->FW : c->FW, fmt == YUV_NV12 ? c->FW : c->FW / 2, c->FW / 2};
   for (int p = 0; p < *n_planes; ++p)
     if (pitch[p] < row[p]) return fail(BEVK_ERR_ARG, "pitch[%d] %lld smaller than the plane's %d-byte rows", p, (long long)pitch[p], row[p]);
   return BEVK_OK;
@@ -1542,25 +1542,30 @@ static int check_yuv_planes(bevk_ctx* c, const int64_t* pitch, int batch, int fl
 int bevk_bev_run_yuv_planes(bevk_ctx* c, const void* d_base, int64_t frame_stride, const int64_t offset[3], const int64_t pitch[3],
                             int batch, const void* d_car, int flags, void* d_out) {
   RET(use(c));
-  int fmt = 0, np = 0;
-  RET(check_yuv_planes(c, pitch, batch, flags, &fmt, &np));
+  RenderReq q;
+  int np = 0;
+  RET(yuv_planes_req(c, "bevk_bev_run_yuv_planes", pitch, batch, d_car, flags, d_out, &q, &np));
   if (!d_base || !offset) return fail(BEVK_ERR_ARG, "null surface pool or offset array");
   YuvPlanes planes;
   for (int p = 0; p < 3; ++p) {
-    const int q = p < np ? p : np - 1;   // NV12: plane 2, 4:2:2: planes 1 and 2 are never read
-    planes.f[p] = Frames(static_cast<const uint8_t*>(d_base) + offset[q], frame_stride);
-    planes.pitch[p] = pitch[q];
+    const int k = p < np ? p : np - 1;   // NV12: plane 2, 4:2:2: planes 1 and 2 are never read
+    planes.f[p] = Frames(static_cast<const uint8_t*>(d_base) + offset[k], frame_stride);
+    planes.pitch[p] = pitch[k];
   }
-  c->timed = true;
-  return run_canvases(c, planes.f[0], batch, d_car, flags, d_out, &planes);
+  q.src = planes.f[0]; q.planes = &planes;
+  return render_timed(c, q);
 }
 
 int bevk_bev_run_yuv_surfaces(bevk_ctx* c, const void* const* surfaces, const int64_t pitch[3], int batch, const void* d_car,
                               int flags, void* d_out) {
   RET(use(c));
-  int fmt = 0, np = 0;
-  RET(check_yuv_planes(c, pitch, batch, flags, &fmt, &np));
+  RenderReq q;
+  int np = 0;
+  RET(yuv_planes_req(c, "bevk_bev_run_yuv_surfaces", pitch, batch, d_car, flags, d_out, &q, &np));
   if (!surfaces) return fail(BEVK_ERR_ARG, "null plane table");
+  YuvPlanes planes;
+  q.src = Frames(surfaces); q.planes = &planes;   // checked before the table is read; the render reads the planes
+  RET(render_check(c, q));
   const size_t n = (size_t)batch * c->n_cam;
   std::vector<const void*> tab(3 * n, nullptr);   // plane-major: plane p of frame i at [p * n + i]
   for (size_t i = 0; i < n; ++i)
@@ -1570,41 +1575,35 @@ int bevk_bev_run_yuv_surfaces(bevk_ctx* c, const void* const* surfaces, const in
     }
   for (int p = np; p < 3; ++p)   // NV12: plane 2, 4:2:2: planes 1 and 2 are never read
     std::copy(tab.begin() + (np - 1) * n, tab.begin() + np * n, tab.begin() + p * n);
-  if (c->yuv_tab != tab) {
-    RET(c->d_yuv_tab.ensure(tab.size() * sizeof(void*)));
-    c->yuv_tab = tab;
-    // pageable source: the driver stages it before returning, and stream order protects launches still reading the old table
-    const cudaError_t e = cudaMemcpyAsync(c->d_yuv_tab.p, c->yuv_tab.data(), tab.size() * sizeof(void*), cudaMemcpyHostToDevice, c->stream);
-    if (e != cudaSuccess) {
-      c->yuv_tab.clear();   // nothing cached: the next call uploads again
-      return fail(BEVK_ERR_CUDA, "plane table upload: %s", cudaGetErrorString(e));
-    }
-  }
-  YuvPlanes planes;
+  RET(upload_table(c, tab.data(), tab.size(), c->d_yuv_tab, c->yuv_tab, "plane table"));
   const void* const* d_tab = c->d_yuv_tab.as<const void*>();
   for (int p = 0; p < 3; ++p) {
     planes.f[p] = Frames(d_tab + p * n);
     planes.pitch[p] = pitch[p < np ? p : np - 1];
   }
-  c->timed = true;
-  return run_canvases(c, planes.f[0], batch, d_car, flags, d_out, &planes);
+  q.src = planes.f[0];
+  return render_timed(c, q);
+}
+
+// The cameras [cam_lo, cam_hi) of src into whole BGR canvases, without car or colour balance.
+static int render_cams(bevk_ctx* c, Frames src, int batch, int cam_lo, int cam_hi, void* d_out) {
+  if (cam_lo < 0 || cam_hi > c->n_cam || cam_lo > cam_hi) return fail(BEVK_ERR_ARG, "bad camera range [%d,%d)", cam_lo, cam_hi);
+  RenderReq q;
+  q.src = src; q.batch = batch; q.out = d_out; q.cam_lo = cam_lo; q.cam_hi = cam_hi;
+  return render_timed(c, q);
 }
 
 int bevk_bev_run_stack_cams(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, int cam_lo, int cam_hi, void* d_out) {
   RET(use(c));
   RET(check_stack(c, d_frames, frame_stride));
-  if (cam_lo < 0 || cam_hi > c->n_cam || cam_lo > cam_hi) return fail(BEVK_ERR_ARG, "bad camera range [%d,%d)", cam_lo, cam_hi);
-  c->timed = true;
-  return run_device(c, Frames(d_frames, frame_stride), batch, nullptr, 0, d_out, cam_lo, cam_hi);
+  return render_cams(c, Frames(d_frames, frame_stride), batch, cam_lo, cam_hi, d_out);
 }
 
 int bevk_bev_last_path(bevk_ctx* c) { return c ? c->last_path : 0; }
 
 int bevk_bev_run_device_cams(bevk_ctx* c, const void* d_srcs, int batch, int cam_lo, int cam_hi, void* d_out) {
   RET(use(c));
-  if (cam_lo < 0 || cam_hi > c->n_cam || cam_lo > cam_hi) return fail(BEVK_ERR_ARG, "bad camera range [%d,%d)", cam_lo, cam_hi);
-  c->timed = true;
-  return run_device(c, Frames(d_srcs), batch, nullptr, 0, d_out, cam_lo, cam_hi);
+  return render_cams(c, Frames(d_srcs), batch, cam_lo, cam_hi, d_out);
 }
 
 int bevk_sat_sum_device(bevk_ctx* c, const void* const* parts, int n, uint64_t bytes, const void* d_car, void* d_out) {
@@ -1629,7 +1628,7 @@ int bevk_sat_sum_device(bevk_ctx* c, const void* const* parts, int n, uint64_t b
 struct HostIngest {
   size_t row = 0, fbytes = 0, fpad = 0, cbytes = 0;
   int fmt = 0, rows = 0;                  // pixel format (0 = BGR) and buffer rows of a frame (FH; FH * 3 / 2 for 4:2:0)
-  int ofmt = 0;                           // canvas format (out_format), and the bytes of one canvas in it
+  int ofmt = 0;                           // canvas format, and the bytes of one canvas in it
   size_t obytes = 0;
   int chunk = 0;
   bool zero_copy = false;
@@ -1648,14 +1647,13 @@ static int upload_car(bevk_ctx* c, const uint8_t* car, const void** d_car) {
   return BEVK_OK;
 }
 
+// h->fmt and h->ofmt come from read_flags.
 static int ingest_setup(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, int batch, const uint8_t* car, int flags,
                         HostIngest* h) {
   RET(need_plan(c));
   if (!srcs) return fail(BEVK_ERR_ARG, "null host pointer");
   if (batch < 1) return fail(BEVK_ERR_ARG, "batch must be >= 1");
-  int fmt = 0, ofmt = 0;
-  RET(pixel_format(c, flags, &fmt));
-  RET(out_format(c, flags, &ofmt));
+  const int fmt = h->fmt, ofmt = h->ofmt;
   // a YUV 4:2:0 frame is uint8[FH * 3 / 2][FW] and a 4:2:2 one uint8[FH][FW][2], rows at the same stride; it is staged as
   // it is and converted on the device
   const bool packed = packed_format(fmt);
@@ -1663,8 +1661,8 @@ static int ingest_setup(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_str
   const size_t row = (size_t)c->FW * (!fmt ? 3 : packed ? 2 : 1), fbytes = row * rows, fpad = pad256(fbytes);
   if (src_stride < (int64_t)row) return fail(BEVK_ERR_ARG, "src_stride %lld < row bytes", (long long)src_stride);
   const size_t cbytes = (size_t)c->BW * c->BH * 3;
-  h->row = row; h->fbytes = fbytes; h->fpad = fpad; h->cbytes = cbytes; h->fmt = fmt; h->rows = rows;
-  h->ofmt = ofmt; h->obytes = ofmt ? cbytes / 2 : cbytes;
+  h->row = row; h->fbytes = fbytes; h->fpad = fpad; h->cbytes = cbytes; h->rows = rows;
+  h->obytes = ofmt ? cbytes / 2 : cbytes;
   // Two-deep pipeline over chunks of frame-sets: the H2D copies of chunk i+1 run on the copy
   // stream while chunk i is rendered and its canvases go back on the main stream, so the two
   // PCIe directions overlap and the kernel hides under the copies.
@@ -1708,7 +1706,7 @@ static int ingest_setup(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_str
 }
 
 // Frame-sets [b0, b0 + nb) into staging half `half` on the copy stream, and the main stream made to wait for them.  *fsrc:
-// the staged frames as run_device reads them (a frame stack, so the TMA-staged kernel serves them too).
+// the staged frames as render reads them (a frame stack, so the TMA-staged kernel serves them too).
 static int ingest_chunk(bevk_ctx* c, const HostIngest& h, const uint8_t* const* srcs, int64_t src_stride, int flags, int b0, int nb,
                         int half, Frames* fsrc) {
   const size_t set_frames = (size_t)c->n_cam, row = h.row, fbytes = h.fbytes, fpad = h.fpad;
@@ -1772,12 +1770,13 @@ static int ingest_chunk(bevk_ctx* c, const HostIngest& h, const uint8_t* const* 
 // canvases in d_canvas are converted into half `half` of d_out_yuv, and *dcanvas points there.
 static int render_chunk(bevk_ctx* c, const HostIngest& h, const uint8_t* const* srcs, int64_t src_stride, int flags, int b0, int nb,
                         int half, uint8_t** dcanvas) {
-  Frames fsrc;
-  RET(ingest_chunk(c, h, srcs, src_stride, flags, b0, nb, half, &fsrc));
-  c->timed = false;
-  uint8_t* bgr = c->d_canvas.as<uint8_t>() + (size_t)half * h.chunk * h.cbytes;
-  *dcanvas = h.ofmt ? c->d_out_yuv.as<uint8_t>() + (size_t)half * h.chunk * h.obytes : bgr;
-  RET(render_to(c, fsrc, nb, h.d_car, flags, h.ofmt, bgr, *dcanvas));
+  RenderReq q;
+  RET(ingest_chunk(c, h, srcs, src_stride, flags, b0, nb, half, &q.src));
+  q.scratch = c->d_canvas.as<uint8_t>() + (size_t)half * h.chunk * h.cbytes;
+  *dcanvas = h.ofmt ? c->d_out_yuv.as<uint8_t>() + (size_t)half * h.chunk * h.obytes : q.scratch;
+  q.fmt = h.fmt; q.batch = nb; q.bal = (flags & BEVK_FLAG_BALANCE) != 0; q.car = h.d_car; q.out = *dcanvas; q.ofmt = h.ofmt;
+  RET(render_check(c, q));
+  RET(render(c, q));
   CU(cudaEventRecord(c->ev_free[half], c->stream));
   return BEVK_OK;
 }
@@ -1789,7 +1788,9 @@ int bevk_bev_run(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_stride, in
   RET(need_plan(c));
   if (!srcs || !out) return fail(BEVK_ERR_ARG, "null host pointer");
   HostIngest h;
+  RET(read_flags(c, flags, kInFlags | kOutFlags, "bevk_bev_run", &h.fmt, &h.ofmt));
   RET(ingest_setup(c, srcs, src_stride, batch, car, flags, &h));
+  c->timed = false;
   for (int b0 = 0, half = 0; b0 < batch; b0 += h.chunk, half ^= 1) {
     const int nb = std::min(h.chunk, batch - b0);
     uint8_t* dcanvas = nullptr;
@@ -2016,13 +2017,26 @@ int bevk_shard_info(bevk_ctx* c, int rank, int* cam_lo, int* cam_hi, int32_t rec
   return BEVK_OK;
 }
 
-// rank `as_rank`'s slabs of `batch` frame-sets into d_slabs[as_rank][batch][slab_bytes]
-static int shard_render(bevk_ctx* c, Frames src, int batch, int as_rank, void* d_slabs) {
-  bevk_ctx::Shard& s = c->shard;
-  uint8_t* dst = reinterpret_cast<uint8_t*>(d_slabs) + (size_t)as_rank * batch * s.slab_bytes;
-  if (!has_slab(s, as_rank)) return BEVK_OK;
-  const OutWin w = slab_win(s, as_rank);
-  return run_device(c, src, batch, nullptr, 0, dst, s.cam_lo[as_rank], s.cam_hi[as_rank], &w);
+// The render of rank r's slabs of `batch` frame-sets into d_slabs[r][batch][slab_bytes], through *w.  Under BALANCE
+// slab_prepass points q.src at the balanced copies first.
+static RenderReq slab_req(bevk_ctx* c, Frames src, int batch, int r, bool bal, void* d_slabs, OutWin* w) {
+  const bevk_ctx::Shard& s = c->shard;
+  *w = slab_win(s, r);
+  RenderReq q;
+  q.src = src; q.batch = batch; q.bal = bal; q.win = w; q.cam_lo = s.cam_lo[r]; q.cam_hi = s.cam_hi[r];
+  q.out = reinterpret_cast<uint8_t*>(d_slabs) + (size_t)r * batch * s.slab_bytes;
+  return q;
+}
+
+// rank r's slabs; a rank without one renders nothing
+static int shard_render(bevk_ctx* c, const RenderReq& q, int r) { return has_slab(c->shard, r) ? render(c, q) : BEVK_OK; }
+
+// BALANCE of rank r's slabs: luminance balance of its own cameras from the exchanged V sums [world][batch][n_cam] into
+// balanced copies, which q->src then reads
+static int slab_prepass(bevk_ctx* c, RenderReq* q, int r, const unsigned long long* d_vsums) {
+  const bevk_ctx::Shard& s = c->shard;
+  if (!has_slab(s, r)) return BEVK_OK;
+  return balance_prepass(c, q->src, q->batch, s.cam_lo[r], s.cam_hi[r], d_vsums, s.world, &q->src);
 }
 
 // bal: colour balance after the compose -- k_compose_slabs<.., true> writes the raw canvases and their channel sums,
@@ -2056,13 +2070,6 @@ static int shard_compose(bevk_ctx* c, const void* d_slabs, int batch, const void
   return launch_gain(c, a.out, batch, a.csum, reinterpret_cast<const uint8_t*>(d_car));
 }
 
-// BALANCE limits of a camera-sharded call, checked before anything is enqueued (those of run_device)
-static int shard_balance_limits(bevk_ctx* c, int batch) {
-  if (batch < 1 || batch > 65535) return fail(BEVK_ERR_ARG, "batch %d out of range [1,65535]", batch);
-  if ((long long)batch * c->n_cam > 65535) return fail(BEVK_ERR_ARG, "batch %d x %d cameras exceeds the 65535 frames of a BALANCE call", batch, c->n_cam);
-  return BEVK_OK;
-}
-
 // the V sums of rank `as_rank`'s own cameras into block as_rank of d_vsums[world][batch][n_cam], zero in the other
 // columns; other cameras' frames are never read
 static int shard_vsum(bevk_ctx* c, Frames src, int batch, int as_rank, unsigned long long* d_vsums) {
@@ -2076,56 +2083,52 @@ static int shard_vsum(bevk_ctx* c, Frames src, int batch, int as_rank, unsigned 
   return BEVK_OK;
 }
 
-// rank `as_rank`'s slabs under BALANCE: luminance balance of its own cameras from the exchanged V sums, then the
-// ordinary windowed render of the balanced copies
-static int shard_render_balanced(bevk_ctx* c, Frames src, int batch, int as_rank, const unsigned long long* d_vsums, void* d_slabs) {
-  bevk_ctx::Shard& s = c->shard;
-  if (!has_slab(s, as_rank)) return BEVK_OK;
-  Frames bal;
-  RET(balance_prepass(c, src, batch, s.cam_lo[as_rank], s.cam_hi[as_rank], d_vsums, s.world, &bal));
-  return shard_render(c, bal, batch, as_rank, d_slabs);
-}
-
 int bevk_shard_vsum(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, int as_rank, uint64_t* d_vsums) {
   RET(use(c));
   RET(shard_geometry(c));
   RET(check_stack(c, d_frames, frame_stride));
-  RET(shard_balance_limits(c, batch));
   RET(check_rank(c, as_rank));
   RET(check_dev_buf(d_vsums, 8, "V-sum buffer"));
-  return shard_vsum(c, Frames(d_frames, frame_stride), batch, as_rank, reinterpret_cast<unsigned long long*>(d_vsums));
+  const Frames src(d_frames, frame_stride);
+  OutWin w;
+  RET(render_check(c, slab_req(c, src, batch, as_rank, true, d_vsums, &w)));   // the limits of the render these sums balance
+  return shard_vsum(c, src, batch, as_rank, reinterpret_cast<unsigned long long*>(d_vsums));
+}
+
+// bevk_shard_render, and with V sums bevk_shard_render_balanced, whose window starts after its balance pre-pass
+static int shard_render_call(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, int as_rank, bool bal,
+                             const uint64_t* d_vsums, void* d_slabs) {
+  RET(use(c));
+  RET(shard_geometry(c));
+  RET(check_stack(c, d_frames, frame_stride));
+  RET(check_rank(c, as_rank));
+  if (bal) RET(check_dev_buf(d_vsums, 8, "V-sum buffer"));
+  RET(check_dev_buf(d_slabs, 16, "slab buffer"));
+  OutWin w;
+  RenderReq q = slab_req(c, Frames(d_frames, frame_stride), batch, as_rank, bal, d_slabs, &w);
+  RET(render_check(c, q));
+  if (bal) RET(slab_prepass(c, &q, as_rank, reinterpret_cast<const unsigned long long*>(d_vsums)));
+  RET(time_begin(c));
+  RET(shard_render(c, q, as_rank));
+  return time_end(c);
 }
 
 int bevk_shard_render_balanced(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, int as_rank, const uint64_t* d_vsums,
                                void* d_slabs) {
-  RET(use(c));
-  RET(shard_geometry(c));
-  RET(check_stack(c, d_frames, frame_stride));
-  RET(shard_balance_limits(c, batch));
-  RET(check_rank(c, as_rank));
-  RET(check_dev_buf(d_vsums, 8, "V-sum buffer"));
-  RET(check_dev_buf(d_slabs, 16, "slab buffer"));
-  c->timed = true;
-  return shard_render_balanced(c, Frames(d_frames, frame_stride), batch, as_rank,
-                               reinterpret_cast<const unsigned long long*>(d_vsums), d_slabs);
+  return shard_render_call(c, d_frames, frame_stride, batch, as_rank, true, d_vsums, d_slabs);
 }
 
 int bevk_shard_compose_balanced(bevk_ctx* c, const void* d_slabs, int batch, const void* d_car, void* d_out) {
   RET(use(c));
   RET(shard_geometry(c));
-  if (!d_slabs || !d_out) return fail(BEVK_ERR_ARG, "null device pointer");
-  RET(shard_balance_limits(c, batch));
+  RenderReq q;   // the limits of the canvases the compose balances
+  q.src = Frames(d_slabs, 0); q.batch = batch; q.bal = true; q.car = d_car; q.out = d_out;
+  RET(render_check(c, q));
   return shard_compose(c, d_slabs, batch, d_car, d_out, 0, true);
 }
 
 int bevk_shard_render(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, int as_rank, void* d_slabs) {
-  RET(use(c));
-  RET(shard_geometry(c));
-  RET(check_stack(c, d_frames, frame_stride));
-  RET(check_rank(c, as_rank));
-  RET(check_dev_buf(d_slabs, 16, "slab buffer"));
-  c->timed = true;
-  return shard_render(c, Frames(d_frames, frame_stride), batch, as_rank, d_slabs);
+  return shard_render_call(c, d_frames, frame_stride, batch, as_rank, false, nullptr, d_slabs);
 }
 
 int bevk_shard_compose(bevk_ctx* c, const void* d_slabs, int batch, const void* d_car, void* d_out) {
@@ -2153,37 +2156,33 @@ static int shard_exchange_vsums(bevk_ctx* c, Frames src, int batch, long long* r
 int bevk_bev_run_sharded(bevk_ctx* c, const void* d_frames, int64_t frame_stride, int batch, const void* d_car, int flags, void* d_out) {
   NvtxRange nvtx_call("bevk_bev_run_sharded (render slabs, all-gather, compose)");
   RET(use(c));
-  RET(bgr_only(flags, "bevk_bev_run_sharded"));
-  RET(bgr_canvas_only(flags, "bevk_bev_run_sharded"));
+  RenderReq q;
+  RET(canvas_req(c, "bevk_bev_run_sharded", flags, 0, Frames(d_frames, frame_stride), batch, d_car, d_out, &q));
   if (!c->shard.configured) return fail(BEVK_ERR_ARG, "bevk_shard_configure not called");
   RET(check_stack(c, d_frames, frame_stride));
   bevk_ctx::Shard& s = c->shard;
   s.last_link_bytes = 0;
-  if (s.policy == BEVK_SHARD_FRAMES || s.world == 1) {   // every rank renders its own frame-sets: no exchange
-    c->timed = true;
-    return run_device(c, Frames(d_frames, frame_stride), batch, d_car, flags, d_out, 0, BEVK_MAX_CAMERAS);
-  }
-  const bool bal = (flags & BEVK_FLAG_BALANCE) != 0;
-  if (bal) RET(shard_balance_limits(c, batch));
+  if (s.policy == BEVK_SHARD_FRAMES || s.world == 1) return render_timed(c, q);   // every rank renders its own frame-sets
+  RET(render_check(c, q));   // the canvases the compose writes
   if (!s.comm) return fail(BEVK_ERR_ARG, "bevk_shard_connect not called");
   RET(shard_geometry(c));
-  const Frames src = Frames(d_frames, frame_stride);
   const size_t per_rank = (size_t)batch * s.slab_bytes;
   RET(s.d_slabs.ensure(per_rank * s.world));
   c->timed = false;
+  OutWin w;
+  RenderReq sq = slab_req(c, q.src, batch, s.rank, q.bal, s.d_slabs.p, &w);
   long long vsum_bytes = 0;
-  if (bal) {
+  if (q.bal) {
     // luminance_balance needs every camera's V mean: ONE all-gather of the ranks' V-sum blocks before the render
-    RET(shard_exchange_vsums(c, src, batch, &vsum_bytes));
-    RET(shard_render_balanced(c, src, batch, s.rank, s.d_vsums.as<unsigned long long>(), s.d_slabs.p));
-  } else {
-    RET(shard_render(c, src, batch, s.rank, s.d_slabs.p));
+    RET(shard_exchange_vsums(c, q.src, batch, &vsum_bytes));
+    RET(slab_prepass(c, &sq, s.rank, s.d_vsums.as<unsigned long long>()));
   }
+  RET(shard_render(c, sq, s.rank));
   // ONE all-gather of the slabs (in place: this rank's block is already where it belongs)
   const int r = nccl().AllGather(s.d_slabs.as<uint8_t>() + per_rank * s.rank, s.d_slabs.p, per_rank, kNcclUint8, s.comm, c->stream);
   if (r != 0) return fail(BEVK_ERR_CUDA, "ncclAllGather: %s", nccl().GetErrorString(r));
   s.last_link_bytes = (long long)per_rank * (s.world - 1) + vsum_bytes;
-  return shard_compose(c, s.d_slabs.p, batch, d_car, d_out, 0, bal);
+  return shard_compose(c, s.d_slabs.p, batch, d_car, d_out, 0, q.bal);
 }
 
 // ---- camera sharding with peer stores: compute and exchange in one kernel ----------------------------------------
@@ -2241,13 +2240,11 @@ int bevk_bev_run_scattered(bevk_ctx* c, const void* d_frames, int64_t frame_stri
                            void* d_out_own, int* n_own) {
   NvtxRange nvtx_call("bevk_bev_run_scattered (render with peer stores, barrier, compose own)");
   RET(use(c));
-  RET(bgr_only(flags, "bevk_bev_run_scattered"));
-  RET(bgr_canvas_only(flags, "bevk_bev_run_scattered"));
+  RenderReq q;
+  RET(canvas_req(c, "bevk_bev_run_scattered", flags, 0, Frames(d_frames, frame_stride), batch, d_car, d_out_own, &q));
   bevk_ctx::Shard& s = c->shard;
   if (!s.configured || s.policy != BEVK_SHARD_CAMERAS) return fail(BEVK_ERR_ARG, "bevk_shard_configure(CAMERAS) not called");
   RET(check_stack(c, d_frames, frame_stride));
-  const bool bal = (flags & BEVK_FLAG_BALANCE) != 0;
-  if (bal) RET(shard_balance_limits(c, batch));
   RET(shard_geometry(c));
   if (!s.comm && s.world > 1) return fail(BEVK_ERR_ARG, "bevk_shard_connect not called");
   if (!s.attached || batch > s.prepared_batch || (batch + s.world - 1) / s.world != s.own_max)
@@ -2256,19 +2253,21 @@ int bevk_bev_run_scattered(bevk_ctx* c, const void* d_frames, int64_t frame_stri
   if (n_own) *n_own = mine;
   if (mine > 0 && !d_out_own) return fail(BEVK_ERR_ARG, "null output");
   const size_t half = (size_t)s.world * s.own_max * s.slab_bytes, rank_stride = (size_t)s.own_max * s.slab_bytes;
-  const Frames src = Frames(d_frames, frame_stride);
+  const unsigned par = s.step & 1u;     // double buffer: a peer may already store step n+1 while this rank composes step n
+  OutWin w;
+  RenderReq sq = slab_req(c, q.src, batch, s.rank, q.bal, nullptr, &w);
+  sq.out = nullptr;
+  w.world = s.world; w.src_off = (long long)(par * half + (size_t)s.rank * rank_stride);
+  for (int r = 0; r < s.world; ++r) w.peer[r] = reinterpret_cast<uint8_t*>(s.peer_recv[r]);
+  RET(render_check(c, sq));
+  s.step++;
   s.last_link_bytes = 0;
   c->timed = false;
   long long vsum_bytes = 0;
-  if (bal) RET(shard_exchange_vsums(c, src, batch, &vsum_bytes));
-  const unsigned par = s.step++ & 1u;     // double buffer: a peer may already store step n+1 while this rank composes step n
+  if (q.bal) RET(shard_exchange_vsums(c, q.src, batch, &vsum_bytes));
   if (has_slab(s, s.rank)) {
-    OutWin w = slab_win(s, s.rank);
-    w.world = s.world; w.src_off = (long long)(par * half + (size_t)s.rank * rank_stride);
-    for (int r = 0; r < s.world; ++r) w.peer[r] = reinterpret_cast<uint8_t*>(s.peer_recv[r]);
-    Frames rsrc = src;   // BALANCE: the peer-store render reads this rank's balanced copies
-    if (bal) RET(balance_prepass(c, src, batch, s.cam_lo[s.rank], s.cam_hi[s.rank], s.d_vsums.as<unsigned long long>(), s.world, &rsrc));
-    RET(run_device(c, rsrc, batch, nullptr, 0, nullptr, s.cam_lo[s.rank], s.cam_hi[s.rank], &w));
+    if (q.bal) RET(slab_prepass(c, &sq, s.rank, s.d_vsums.as<unsigned long long>()));   // the peer-store render reads them
+    RET(render(c, sq));
     s.last_link_bytes = (long long)(batch - mine) * s.slab_bytes;   // what this rank stored into its peers
   }
   s.last_link_bytes += vsum_bytes;
@@ -2277,7 +2276,7 @@ int bevk_bev_run_scattered(bevk_ctx* c, const void* d_frames, int64_t frame_stri
     const int r = nccl().AllGather(f + SHARD_MAX_RANKS, f, 4, kNcclUint8, s.comm, c->stream);
     if (r != 0) return fail(BEVK_ERR_CUDA, "ncclAllGather (step barrier): %s", nccl().GetErrorString(r));
   }
-  if (mine > 0) RET(shard_compose(c, reinterpret_cast<const uint8_t*>(s.recv) + par * half, mine, d_car, d_out_own, (long long)rank_stride, bal));
+  if (mine > 0) RET(shard_compose(c, reinterpret_cast<const uint8_t*>(s.recv) + par * half, mine, d_car, d_out_own, (long long)rank_stride, q.bal));
   return BEVK_OK;
 }
 
@@ -2362,19 +2361,20 @@ int bevk_bev_run_jpeg(bevk_ctx* c, const uint8_t* const* jpegs, const uint64_t* 
                       uint8_t* out) {
   NvtxRange nvtx_call("bevk_bev_run_jpeg (JPEG streams -> host canvases)");
   RET(use(c));
-  RET(bgr_only(flags, "bevk_bev_run_jpeg"));
-  RET(bgr_canvas_only(flags, "bevk_bev_run_jpeg"));
+  RenderReq q;
+  RET(canvas_req(c, "bevk_bev_run_jpeg", flags, 0, Frames(), batch, nullptr, nullptr, &q));
   RET(need_plan(c));
   if (!jpegs || !sizes || !out || batch < 1) return fail(BEVK_ERR_ARG, "bad argument");
   const size_t fpad = pad256((size_t)c->FW * c->FH * 3), cbytes = (size_t)c->BW * c->BH * 3;
   const int nf = batch * c->n_cam;
   RET(c->d_jpeg_frames.ensure(fpad * nf));
   RET(c->d_jpeg_canvas.ensure(cbytes * batch));
+  q.src = Frames(c->d_jpeg_frames.p, (long long)fpad); q.out = c->d_jpeg_canvas.p;
+  RET(render_check(c, q));
   RET(bevk_jpeg_decode(c, jpegs, sizes, nf, c->FW, c->FH, c->d_jpeg_frames.p, (int64_t)fpad));
-  const void* d_car = nullptr;
-  RET(upload_car(c, car, &d_car));
+  RET(upload_car(c, car, &q.car));
   c->timed = false;
-  RET(run_device(c, Frames(c->d_jpeg_frames.p, (long long)fpad), batch, d_car, flags, c->d_jpeg_canvas.p, 0, BEVK_MAX_CAMERAS));
+  RET(render(c, q));
   CU(cudaMemcpyAsync(out, c->d_jpeg_canvas.p, cbytes * batch, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaStreamSynchronize(c->stream));
   return BEVK_OK;
@@ -2426,8 +2426,7 @@ static int slot_open(bevk_ctx* c, int s, int n, size_t bytes) {
 // stream sizes into page-locked memory and ev_sizes[s].  enc_collect(s) finishes the batch.
 static int slot_close(bevk_ctx* c, int s, int n) {
   auto& e = c->enc_out;
-  CU(cudaEventRecord(c->ev1, c->stream));
-  c->timed = true;
+  RET(time_end(c));
   CU(cudaMemcpyAsync(e.h_sizes[s], e.meta[s].as<unsigned long long>() + n, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaEventRecord(e.ev_sizes[s], c->stream));
   return BEVK_OK;
@@ -2804,7 +2803,7 @@ static int jpeg_chunk(int n) {
 
 // ------------------------------------------------------------------ BEV canvases straight to JPEG (surroundBEV.py:340)
 // BevGenerator.__call__ then cv2.imencode: each chunk of frame-sets is rendered into ctx scratch and encoded there, and
-// only the streams come back.  Under BALANCE run_device's k_gain applies colour balance and the car to the chunk's
+// only the streams come back.  Under BALANCE the render's k_gain applies colour balance and the car to the chunk's
 // canvases before the encoder reads them.  The call is checked before the render set-up enqueues anything.
 static int to_jpeg_check(bevk_ctx* c, uint8_t* out, uint64_t* sizes) {
   RET(need_plan(c));
@@ -2816,11 +2815,10 @@ int bevk_bev_run_to_jpeg(bevk_ctx* c, const uint8_t* const* srcs, int64_t src_st
                          int quality, uint8_t* out, uint64_t capacity, uint64_t* sizes) {
   NvtxRange nvtx_call("bevk_bev_run_to_jpeg (host frames -> host JPEG streams)");
   RET(use(c));
-  RET(bgr_only(flags, "bevk_bev_run_to_jpeg"));
-  RET(bgr_canvas_only(flags, "bevk_bev_run_to_jpeg"));
+  HostIngest h;
+  RET(read_flags(c, flags, 0, "bevk_bev_run_to_jpeg", &h.fmt, &h.ofmt));
   RET(to_jpeg_check(c, out, sizes));
   const jpeg::Opts o = jpeg_ctx_opts(c, quality);
-  HostIngest h;
   RET(ingest_setup(c, srcs, src_stride, batch, car, flags, &h));
   // the ingest chunks are the encoder's: staging half = canvas half = encoder slot
   return enc_chunks(c, "JPEG", batch, h.chunk, false, out, capacity, sizes, [&](int b0, int nb, int half) -> int {
@@ -2834,8 +2832,8 @@ int bevk_bev_frames_to_jpeg(bevk_ctx* c, const void* const* frames, int batch, c
                             uint8_t* out, uint64_t capacity, uint64_t* sizes) {
   NvtxRange nvtx_call("bevk_bev_frames_to_jpeg (device frames -> host JPEG streams)");
   RET(use(c));
-  RET(bgr_only(flags, "bevk_bev_frames_to_jpeg"));
-  RET(bgr_canvas_only(flags, "bevk_bev_frames_to_jpeg"));
+  RenderReq q;
+  RET(canvas_req(c, "bevk_bev_frames_to_jpeg", flags, 0, Frames(), batch, d_car, nullptr, &q));
   RET(to_jpeg_check(c, out, sizes));
   if (!frames) return fail(BEVK_ERR_ARG, "null pointer");
   const jpeg::Opts o = jpeg_ctx_opts(c, quality);
@@ -2846,11 +2844,12 @@ int bevk_bev_frames_to_jpeg(bevk_ctx* c, const void* const* frames, int batch, c
   RET(c->d_canvas.ensure((size_t)c->BW * c->BH * 3 * chunk));
   uint8_t* dcanvas = c->d_canvas.as<uint8_t>();
   return enc_chunks(c, "JPEG", batch, chunk, false, out, capacity, sizes, [&](int b0, int nb, int s) -> int {
-    Frames part = src;
-    if (part.table) part.table += (size_t)b0 * c->n_cam;
-    else part.base += (long long)b0 * c->n_cam * part.stride;
-    c->timed = false;
-    RET(run_device(c, part, nb, d_car, flags, dcanvas, 0, BEVK_MAX_CAMERAS));
+    q.src = src;
+    if (src.table) q.src.table += (size_t)b0 * c->n_cam;
+    else q.src.base += (long long)b0 * c->n_cam * src.stride;
+    q.batch = nb; q.out = dcanvas;
+    RET(render_check(c, q));
+    RET(render(c, q));
     return jpeg_enqueue(c, s, EncIn{dcanvas, (long long)c->BW * c->BH * 3, (long long)c->BW * 3}, nb, c->BW, c->BH, o);
   });
 }

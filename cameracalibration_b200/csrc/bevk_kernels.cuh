@@ -1114,7 +1114,7 @@ __host__ __device__ __forceinline__ void canvas_yuv_item(const CanvasYuvArgs& a,
 
 // The conversion pass: grid = (blocks, batch); the items (4-pixel groups of row pairs) of canvas blockIdx.y, row pair
 // major, are strided over its blocks, so that a warp reads 32 consecutive groups of two rows and writes 32 consecutive Y
-// words per row.  GAIN: the canvases are raw BALANCE renders (run_device's kFlagRawBalance) and each CTA builds the
+// words per row.  GAIN: the canvases are raw BALANCE renders (render of a YUV canvas) and each CTA builds the
 // canvas's gain table in shared memory, so k_gain does not run and the balanced BGR canvas is never written.
 template <int FMT, bool GAIN>
 __global__ void __launch_bounds__(256) k_canvas_yuv(CanvasYuvArgs a) {

@@ -216,7 +216,7 @@ static int mode_balance() {
 // One frame-set through the product's plan compiler (bevk_plan.cuh, the code bevk_bev_finalize runs) and a plain-loop
 // interpreter of that plan that uses the kernels' own per-entry arithmetic (interp_fast, sample_slow_core, sat_add_bgr,
 // hsv_roundtrip, lum_deltas, gray_world_gains / gain_entry).  It mirrors k_bev's work decomposition -- tile, item,
-// entry index -> accumulator position by orientation, first-camera store vs saturating add -- and run_device's
+// entry index -> accumulator position by orientation, first-camera store vs saturating add -- and render's
 // BALANCE sequence (V sums, offsets, balanced row spans, gather, channel sums, gains, car), without threads.
 // in.bin : int32 NC FW FH BW BH nearest balance has_car; per camera map1 int16[BH*BW*2], map2 uint16[BH*BW],
 //          mask u8[BH*BW]; NC frames u8[FH*FW*3]; car u8[BH*BW*3] if has_car.   out.bin: canvas u8[BH*BW*3]

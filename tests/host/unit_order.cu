@@ -28,7 +28,7 @@ int main(int argc, char** argv) {
     if (t < 0 || t >= n_tiles || seen_tile[t]++) { printf("tile %d repeated or out of range\n", t); return 1; }
   }
   if ((int)order.size() != n_tiles) { printf("tile list has %zu of %d tiles\n", order.size(), n_tiles); return 1; }
-  // the kernel's frame-sets per unit: 4 for batches of at least 4, else 1 (bevk_api.cu run_device)
+  // the kernel's frame-sets per unit: 4 for batches of at least 4, else 1 (bevk_api.cu render)
   const int NB = batch >= 4 ? 4 : 1, groups = (batch + NB - 1) / NB;
   const long long n_units = (long long)n_tiles * groups;
   std::vector<int> seen(n_units, 0);
