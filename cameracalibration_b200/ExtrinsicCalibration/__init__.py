@@ -1,1 +1,1 @@
-from .extrinsicCalib import ExCalibrator  # noqa: F401
+from .extrinsicCalib import CenterImage, ExCalibrator, ScaleImage  # noqa: F401

@@ -12,6 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BEVK_LIB_PATH") or os.path.join(_HERE, "libbevk.so")   # BEVK_LIB_PATH: A/B builds
 
 INTER_NEAREST, INTER_LINEAR, INTER_CUBIC, INTER_AREA, INTER_LANCZOS4 = 0, 1, 2, 3, 4   # cv2.INTER_*
+INTER_LINEAR_EXACT, INTER_NEAREST_EXACT, WARP_INVERSE_MAP = 5, 6, 16                   # refused by every call; warp_affine's flag
 MAPS_UNDISTORT, MAPS_BEV = 0, 1
 MODEL_FISHEYE, MODEL_PINHOLE = 0, 1
 FLAG_BALANCE = 1
@@ -49,6 +50,13 @@ SIGNATURES = {
     "bevk_undistort_last_path": (C.c_int, [_p]),
     "bevk_warp_perspective":(C.c_int, [_p, _p, C.c_int, C.c_int, C.c_int64, C.c_int, _dp, _p, C.c_int, C.c_int, C.c_int64, C.c_int]),
     "bevk_warp_maps": (C.c_int, [_p, _p, _p, C.c_int, C.c_int, _dp, C.c_int, C.c_int, _p, _p]),
+    "bevk_warp_affine": (C.c_int, [_p, _p, C.c_int, C.c_int, C.c_int64, C.c_int, _dp, _p, C.c_int, C.c_int, C.c_int64, C.c_int]),
+    "bevk_warp_affine_stack": (C.c_int, [_p, _p, C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, _dp, _p, C.c_int64,
+                                         C.c_int, C.c_int, C.c_int64, C.c_int]),
+    "bevk_resize": (C.c_int, [_p, _p, C.c_int, C.c_int, C.c_int64, C.c_int, _p, C.c_int, C.c_int, C.c_int64, C.c_double,
+                              C.c_double, C.c_int]),
+    "bevk_resize_stack": (C.c_int, [_p, _p, C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, _p, C.c_int64, C.c_int,
+                                    C.c_int, C.c_int64, C.c_double, C.c_double, C.c_int]),
     "bevk_bev_configure": (C.c_int, [_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "bevk_bev_set_camera": (C.c_int, [_p, C.c_int, _dp, _dp, _dp, C.c_int, C.c_int, _dp]),
     "bevk_bev_set_maps": (C.c_int, [_p, C.c_int, _p, _p]),

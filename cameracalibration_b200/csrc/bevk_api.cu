@@ -27,6 +27,7 @@
 #include "bevk_jpeg_enc.cuh"
 #include "bevk_jpeg_prog.cuh"
 #include "bevk_png_enc.cuh"
+#include "bevk_resize.cuh"
 
 #include <cub/device/device_scan.cuh>
 #include <cub/iterator/counting_input_iterator.cuh>
@@ -620,16 +621,22 @@ int bevk_undistort(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, in
 }
 
 // ------------------------------------------------------------------ undistortion of device frame batches
+// The source side of the device-batch calls: a frame, n >= 1, and an image stride that covers an image when n > 1.
+static int check_stack_src(const void* d_src, int64_t sis, int sw, int sh, int64_t srs, int channels, int n) {
+  if (n < 1) return fail(BEVK_ERR_ARG, "n must be >= 1, got %d", n);
+  RET(check_image(d_src, sw, sh, srs, channels, "src"));
+  if (n > 1 && sis < (int64_t)(sh - 1) * srs + (int64_t)sw * channels)
+    return fail(BEVK_ERR_ARG, "src image stride %lld is smaller than one image", (long long)sis);
+  return BEVK_OK;
+}
+
 // Checks the source side of the bevk_undistort_stack calls (and normalises *interp) and fills a (slot's map or model, n frames of the source);
 // the destination is left to the caller.  An image stride only matters when n > 1.
 static int stack_src_args(bevk_ctx* c, int slot, const void* d_src, int64_t sis, int sw, int sh, int64_t srs, int channels, int n,
                           int* interp, GatherArgs* a) {
   RET(need_undistorter(c, slot));
-  if (n < 1) return fail(BEVK_ERR_ARG, "n must be >= 1, got %d", n);
   RET(gather_interp(interp));
-  RET(check_image(d_src, sw, sh, srs, channels, "src"));
-  if (n > 1 && sis < (int64_t)(sh - 1) * srs + (int64_t)sw * channels)
-    return fail(BEVK_ERR_ARG, "src image stride %lld is smaller than one image", (long long)sis);
+  RET(check_stack_src(d_src, sis, sw, sh, srs, channels, n));
   const Undistorter& u = c->und[slot];
   *a = GatherArgs{};
   a->src = reinterpret_cast<const uint8_t*>(d_src); a->sw = sw; a->sh = sh; a->spitch = srs;
@@ -644,6 +651,21 @@ static int launch_undistort(bevk_ctx* c, int slot, const GatherArgs& a, int chan
   return c->und[slot].fused ? launch_gather<1>(c, a, channels, interp) : launch_gather<0>(c, a, channels, interp);
 }
 
+// The destination side of the device-batch calls, given a checked source: rows, an image stride that covers an image
+// (n > 1), and byte ranges [first, last] of the whole batch on each side that do not overlap -- an output that overwrites
+// frames still to be read is refused.
+static int check_stack_dst(const void* d_src, int64_t sis, int sw, int sh, int64_t srs, int channels, int n, const void* d_dst,
+                           int64_t dis, int dw, int dh, int64_t drs) {
+  RET(check_image(d_dst, dw, dh, drs, channels, "dst"));
+  const int64_t dimg = (int64_t)(dh - 1) * drs + (int64_t)dw * channels;
+  if (n > 1 && dis < dimg) return fail(BEVK_ERR_ARG, "dst image stride %lld is smaller than one image", (long long)dis);
+  const uintptr_t s0 = reinterpret_cast<uintptr_t>(d_src), d0 = reinterpret_cast<uintptr_t>(d_dst);
+  const uintptr_t s1 = s0 + (uintptr_t)(n > 1 ? (n - 1) * sis : 0) + (uintptr_t)((int64_t)(sh - 1) * srs + (int64_t)sw * channels);
+  const uintptr_t d1 = d0 + (uintptr_t)(n > 1 ? (n - 1) * dis : 0) + (uintptr_t)dimg;
+  if (s0 < d1 && d0 < s1) return fail(BEVK_ERR_ARG, "the destination range overlaps the source frames");
+  return BEVK_OK;
+}
+
 // bevk_undistort_stack_interp: any interpolation gather_interp takes.
 static int undistort_stack(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
                            int channels, int n, void* d_dst, int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride,
@@ -652,15 +674,8 @@ static int undistort_stack(bevk_ctx* c, int slot, const void* d_src, int64_t src
   RET(stack_src_args(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, &interp, &a));
   if (dw != a.dw || dh != a.dh)   // the caller sized dst for another map: never write past it
     return fail(BEVK_ERR_ARG, "undistorter slot %d holds a %dx%d map, the caller expects %dx%d", slot, a.dw, a.dh, dw, dh);
-  RET(check_image(d_dst, dw, dh, dst_row_stride, channels, "dst"));
-  const int64_t dimg = (int64_t)(dh - 1) * dst_row_stride + (int64_t)dw * channels;
-  if (n > 1 && dst_image_stride < dimg)
-    return fail(BEVK_ERR_ARG, "dst image stride %lld is smaller than one image", (long long)dst_image_stride);
-  // byte ranges [first, last] of the whole batch on each side: an output that overwrites frames still to be read is refused
-  const uintptr_t s0 = reinterpret_cast<uintptr_t>(d_src), d0 = reinterpret_cast<uintptr_t>(d_dst);
-  const uintptr_t s1 = s0 + (uintptr_t)(n > 1 ? (n - 1) * src_image_stride : 0) + (uintptr_t)((int64_t)(sh - 1) * src_row_stride + (int64_t)sw * channels);
-  const uintptr_t d1 = d0 + (uintptr_t)(n > 1 ? (n - 1) * dst_image_stride : 0) + (uintptr_t)dimg;
-  if (s0 < d1 && d0 < s1) return fail(BEVK_ERR_ARG, "the destination range overlaps the source frames");
+  RET(check_stack_dst(d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
+                      dst_row_stride));
   a.dst = reinterpret_cast<uint8_t*>(d_dst); a.dpitch = dst_row_stride; a.distride = n > 1 ? dst_image_stride : 0;
   return launch_undistort(c, slot, a, channels, interp);
 }
@@ -703,6 +718,140 @@ int bevk_warp_perspective(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64
   a.dst = c->s_dst.as<uint8_t>(); a.dw = dw; a.dh = dh; a.dpitch = (long long)dw * channels;
   RET(launch_gather<2>(c, a, channels, interp));
   return download_image(c, c->s_dst, dst, dw, dh, dstride, channels);
+}
+
+// ------------------------------------------------------------------ cv2.warpAffine
+// flags -> interpolation (gather_interp's) and the inverse map in a->hm.M[0..5].
+static int affine_args(const double* M, int flags, int* interp, GatherArgs* a) {
+  if (!M) return fail(BEVK_ERR_ARG, "null M");
+  if (flags & ~(7 | BEVK_WARP_INVERSE_MAP)) return fail(BEVK_ERR_UNSUPPORTED, "warpAffine flags %d", flags);
+  *interp = flags & 7;
+  RET(gather_interp(interp));
+  if (flags & BEVK_WARP_INVERSE_MAP) memcpy(a->hm.M, M, 6 * sizeof(double));
+  else inv_affine(M, a->hm.M);
+  return BEVK_OK;
+}
+
+int bevk_warp_affine(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, const double M[6],
+                     uint8_t* dst, int dw, int dh, int64_t dstride, int flags) {
+  RET(use(c));
+  RET(check_image(src, sw, sh, sstride, channels, "src"));
+  RET(check_image(dst, dw, dh, dstride, channels, "dst"));
+  GatherArgs a{};
+  int interp;
+  RET(affine_args(M, flags, &interp, &a));
+  a.n = 1;
+  RET(upload_image(c, c->s_src, src, sw, sh, sstride, channels));
+  RET(c->s_dst.ensure((size_t)dw * dh * channels));
+  a.src = c->s_src.as<uint8_t>(); a.sw = sw; a.sh = sh; a.spitch = (long long)sw * channels;
+  a.dst = c->s_dst.as<uint8_t>(); a.dw = dw; a.dh = dh; a.dpitch = (long long)dw * channels;
+  RET(launch_gather<3>(c, a, channels, interp));
+  return download_image(c, c->s_dst, dst, dw, dh, dstride, channels);
+}
+
+int bevk_warp_affine_stack(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
+                           int channels, int n, const double M[6], void* d_dst, int64_t dst_image_stride, int dw, int dh,
+                           int64_t dst_row_stride, int flags) {
+  RET(use(c));
+  GatherArgs a{};
+  int interp;
+  RET(affine_args(M, flags, &interp, &a));
+  RET(check_stack_src(d_src, src_image_stride, sw, sh, src_row_stride, channels, n));
+  RET(check_stack_dst(d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
+                      dst_row_stride));
+  a.src = reinterpret_cast<const uint8_t*>(d_src); a.sw = sw; a.sh = sh; a.spitch = src_row_stride;
+  a.dst = reinterpret_cast<uint8_t*>(d_dst); a.dw = dw; a.dh = dh; a.dpitch = dst_row_stride;
+  a.n = n; a.sistride = n > 1 ? src_image_stride : 0; a.distride = n > 1 ? dst_image_stride : 0;
+  return launch_gather<3>(c, a, channels, interp);
+}
+
+// ------------------------------------------------------------------ cv2.resize
+// Checks interp and cv2's size rule (resize_geometry) and fills a's scales; returns the body in *kind.
+static int resize_args(int sw, int sh, int dw, int dh, double fx, double fy, int interp, ResizeArgs* a, int* kind) {
+  if (interp != BEVK_INTER_NEAREST && interp != BEVK_INTER_LINEAR && interp != BEVK_INTER_AREA)
+    return fail(BEVK_ERR_UNSUPPORTED, "resize interp %d: INTER_NEAREST, INTER_LINEAR and INTER_AREA only", interp);
+  if (sw <= 0 || sh <= 0 || dw <= 0 || dh <= 0) return fail(BEVK_ERR_ARG, "bad size %dx%d -> %dx%d", sw, sh, dw, dh);
+  *a = ResizeArgs{};
+  if (fx == 0. && fy == 0.) {
+    a->inv_x = (double)dw / sw; a->inv_y = (double)dh / sh;
+  } else {
+    int w = 0, h = 0;
+    a->inv_x = fx; a->inv_y = fy;
+    if (!resize_geometry(sw, sh, &w, &h, &a->inv_x, &a->inv_y))
+      return fail(BEVK_ERR_ARG, "fx %g, fy %g give no image from %dx%d", fx, fy, sw, sh);
+    if (w != dw || h != dh) return fail(BEVK_ERR_ARG, "fx %g, fy %g make %dx%d images, the caller expects %dx%d", fx, fy, w, h, dw, dh);
+  }
+  *kind = resize_kind(interp, *a);
+  a->sw = sw; a->sh = sh; a->dw = dw; a->dh = dh;
+  return BEVK_OK;
+}
+
+template <int C, int KIND>
+static void launch_resize_c(bevk_ctx* c, const ResizeArgs& a, dim3 g, bool batch) {
+  if (batch) k_resize<C, KIND, GATHER_NB><<<g, 256, 0, c->stream>>>(a);
+  else k_resize<C, KIND, 1><<<g, 256, 0, c->stream>>>(a);
+}
+template <int C>
+static void launch_resize_k(bevk_ctx* c, const ResizeArgs& a, int kind, dim3 g, bool batch) {
+  switch (kind) {
+    case RZ_NEAREST: launch_resize_c<C, RZ_NEAREST>(c, a, g, batch); break;
+    case RZ_LINEAR: launch_resize_c<C, RZ_LINEAR>(c, a, g, batch); break;
+    case RZ_AREA_LINEAR: launch_resize_c<C, RZ_AREA_LINEAR>(c, a, g, batch); break;
+    case RZ_AREA_FAST: launch_resize_c<C, RZ_AREA_FAST>(c, a, g, batch); break;
+    default: launch_resize_c<C, RZ_AREA>(c, a, g, batch);
+  }
+}
+
+// Enqueue k_resize over a.n >= 1 frames: grid.z = frame groups of GATHER_NB (one frame: NB = 1), 65535 groups a launch.
+static int launch_resize(bevk_ctx* c, const ResizeArgs& a0, int channels, int kind) {
+  const int per_launch = 65535 * GATHER_NB;
+  for (int f0 = 0; f0 < a0.n; f0 += per_launch) {
+    ResizeArgs a = a0;
+    a.n = std::min(per_launch, a0.n - f0);
+    a.src += (long long)f0 * a0.sistride;
+    a.dst += (long long)f0 * a0.distride;
+    const bool batch = a.n > 1;
+    const dim3 g((a.dw + 31) / 32, (a.dh + 7) / 8, batch ? (unsigned)((a.n + GATHER_NB - 1) / GATHER_NB) : 1u);
+    if (channels == 1) launch_resize_k<1>(c, a, kind, g, batch);
+    else if (channels == 3) launch_resize_k<3>(c, a, kind, g, batch);
+    else launch_resize_k<4>(c, a, kind, g, batch);
+    LAUNCHED(c);
+  }
+  c->gather_path = 3;
+  return BEVK_OK;
+}
+
+int bevk_resize(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, uint8_t* dst, int dw, int dh,
+                int64_t dstride, double fx, double fy, int interp) {
+  RET(use(c));
+  RET(check_image(src, sw, sh, sstride, channels, "src"));
+  RET(check_image(dst, dw, dh, dstride, channels, "dst"));
+  ResizeArgs a;
+  int kind;
+  RET(resize_args(sw, sh, dw, dh, fx, fy, interp, &a, &kind));
+  RET(upload_image(c, c->s_src, src, sw, sh, sstride, channels));
+  RET(c->s_dst.ensure((size_t)dw * dh * channels));
+  a.n = 1;
+  a.src = c->s_src.as<uint8_t>(); a.spitch = (long long)sw * channels;
+  a.dst = c->s_dst.as<uint8_t>(); a.dpitch = (long long)dw * channels;
+  RET(launch_resize(c, a, channels, kind));
+  return download_image(c, c->s_dst, dst, dw, dh, dstride, channels);
+}
+
+int bevk_resize_stack(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
+                      int channels, int n, void* d_dst, int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride,
+                      double fx, double fy, int interp) {
+  RET(use(c));
+  ResizeArgs a;
+  int kind;
+  RET(resize_args(sw, sh, dw, dh, fx, fy, interp, &a, &kind));
+  RET(check_stack_src(d_src, src_image_stride, sw, sh, src_row_stride, channels, n));
+  RET(check_stack_dst(d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
+                      dst_row_stride));
+  a.src = reinterpret_cast<const uint8_t*>(d_src); a.spitch = src_row_stride;
+  a.dst = reinterpret_cast<uint8_t*>(d_dst); a.dpitch = dst_row_stride;
+  a.n = n; a.sistride = n > 1 ? src_image_stride : 0; a.distride = n > 1 ? dst_image_stride : 0;
+  return launch_resize(c, a, channels, kind);
 }
 
 int bevk_warp_maps(bevk_ctx* c, const int16_t* map1, const uint16_t* map2, int sw, int sh, const double H[9], int dw,

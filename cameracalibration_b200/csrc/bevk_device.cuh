@@ -185,6 +185,30 @@ __host__ __device__ __forceinline__ void warp_point(const Homog& hm, int x, int 
   Y = cv_round(fY);
 }
 
+// A3': cv2.warpAffine.  Unless WARP_INVERSE_MAP is set, cv2 inverts M with invertAffineTransform's closed form (a
+// singular M gives D = 0 and the zero matrix's translation part); the inverse lives in Homog::M[0..5].
+inline void inv_affine(const double* S, double* T) {
+  double D = S[0] * S[4] - S[1] * S[3];
+  D = D != 0. ? 1. / D : 0.;
+  const double A11 = S[4] * D, A22 = S[0] * D, A12 = S[1] * -D, A21 = S[3] * -D;
+  T[0] = A11; T[1] = A12; T[3] = A21; T[4] = A22;
+  T[2] = -T[0] * S[2] - T[1] * S[5];
+  T[5] = -T[3] * S[2] - T[4] * S[5];
+}
+
+// Fixed-point pre-image of destination pixel (x,y) under cv2.warpAffine (AB_BITS = 10): X = (X0(y) + adelta(x)) >> 5
+// at TAB scale (every flag but NEAREST), >> 10 in whole pixels for NEAREST.  The int sum wraps as cv2's SIMD add does;
+// the consumers saturate X >> 5 to int16 as cv2's pack does.
+__host__ __device__ __forceinline__ void affine_point(const Homog& hm, int x, int y, bool nearest, int& X, int& Y) {
+  const double* M = hm.M;
+  const int round_delta = nearest ? 512 : 16, shift = nearest ? 10 : 10 - INTER_BITS;
+  const double dy = (double)y, dx = (double)x;
+  const unsigned X0 = (unsigned)cv_round(dmul(dadd(dmul(M[1], dy), M[2]), 1024.)) + round_delta;
+  const unsigned Y0 = (unsigned)cv_round(dmul(dadd(dmul(M[4], dy), M[5]), 1024.)) + round_delta;
+  X = (int)(X0 + (unsigned)cv_round(dmul(dmul(M[0], dx), 1024.))) >> shift;
+  Y = (int)(Y0 + (unsigned)cv_round(dmul(dmul(M[3], dx), 1024.))) >> shift;
+}
+
 __host__ __device__ __forceinline__ int sat_i16(int v) { return max(-32768, min(32767, v)); }
 
 // ---- byte-lane primitives with a host form ------------------------------------

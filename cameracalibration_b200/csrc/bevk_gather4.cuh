@@ -1,7 +1,8 @@
 // bevk_gather4.cuh -- 4-pixels-per-thread form of the stand-alone gathers for 3-channel INTER_LINEAR:
 // cv2.remap with resident maps (MODE 0; Camera.undistort / InCalibrator.undistort / Tools/undistort.py,
 // surroundBEV.py:110-111, intrinsicCalib.py:193-195, undistort.py:66), the same with the camera model
-// evaluated in-kernel (MODE 1) and cv2.warpPerspective (MODE 2; extrinsicCalib.py:166-169).
+// evaluated in-kernel (MODE 1), cv2.warpPerspective (MODE 2; extrinsicCalib.py:166-169) and cv2.warpAffine
+// (MODE 3; extrinsicCalib.py:58).
 // Same tap machinery as the fused BEV kernel (aligned 32-bit words, funnel shift, PRMT, DP2A);
 // each thread produces 12 output bytes per frame and stores them as three 32-bit words.  Over a
 // batch it resolves its 4 pixels' taps once and gathers them from NB = GATHER_NB frames (see k_gather).
@@ -80,9 +81,9 @@ __host__ __device__ __forceinline__ void gather4_frames(const GatherArgs& a, int
   unsigned fx[4], fy[4], px[4];
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
-    if (MODE == 2) {
+    if (MODE >= 2) {
       int X, Y;
-      warp_point(a.hm, x4 + q, y, (double)TAB, X, Y);
+      warp_xy<MODE>(a.hm, x4 + q, y, false, X, Y);
       sx[q] = sat_i16(X >> INTER_BITS); sy[q] = sat_i16(Y >> INTER_BITS);
       fx[q] = X & (TAB - 1); fy[q] = Y & (TAB - 1);
     } else {

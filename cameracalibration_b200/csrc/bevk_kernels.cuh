@@ -1,7 +1,7 @@
 // bevk_kernels.cuh -- the sm_90a kernels behind libbevk.so.
 //
 //   k_undistort_map   K1  cv2.fisheye.initUndistortRectifyMap / cv2.initUndistortRectifyMap
-//   k_gather          K3/K4  cv2.remap, fused undistort (no map), cv2.warpPerspective on images
+//   k_gather          K3/K4  cv2.remap, fused undistort (no map), cv2.warpPerspective / cv2.warpAffine on images
 //   k_gather_taps     K3/K4  the same with INTER_CUBIC / INTER_LANCZOS4
 //   k_warp_maps       K2  cv2.warpPerspective on the 16SC2/16UC1 map planes (BEV LUT build),
 //                         optionally fused with K1 so the full-size undistort map never exists
@@ -38,7 +38,7 @@ __global__ void __launch_bounds__(256) k_undistort_map(CamModel cm, short2* __re
 
 // ---------------------------------------------------------------------------------
 // K3 / K4: generic gather.  MODE 0: maps in HBM, 1: camera model evaluated in-kernel
-// (fused undistort), 2: homography (warpPerspective).
+// (fused undistort), 2: homography (warpPerspective), 3: affine matrix (warpAffine, inverse in hm.M[0..5]).
 // Over a batch of n frames: the taps of an output pixel depend on the pixel only, so a thread
 // resolves them once (map load or camera model) and gathers them from GATHER_NB frames of its
 // grid-z slice.  Frame f is read at src + f * sistride and written at dst + f * distride.
@@ -57,6 +57,13 @@ struct GatherArgs {
 #define BEVK_GATHER_NB 8
 #endif
 constexpr int GATHER_NB = BEVK_GATHER_NB;
+
+// MODE 2 / 3: the fixed-point source position of destination pixel (x, y), at TAB scale or (nearest) in whole pixels.
+template <int MODE>
+__host__ __device__ __forceinline__ void warp_xy(const Homog& hm, int x, int y, bool nearest, int& X, int& Y) {
+  if (MODE == 3) affine_point(hm, x, y, nearest, X, Y);
+  else warp_point(hm, x, y, nearest ? 1.0 : (double)TAB, X, Y);
+}
 
 template <int C>
 __host__ __device__ __forceinline__ void load_px(const uint8_t* __restrict__ src, long long spitch, int sw, int sh,
@@ -80,14 +87,13 @@ __host__ __device__ __forceinline__ void load_px(const uint8_t* __restrict__ src
 template <int MODE, int C, int LINEAR>
 __host__ __device__ __forceinline__ void gather_frames(const GatherArgs& a, int x, int y, int f0) {
   int sx, sy, fx = 0, fy = 0;
-  if (MODE == 2) {
+  if (MODE >= 2) {
     int X, Y;
+    warp_xy<MODE>(a.hm, x, y, !LINEAR, X, Y);
     if (LINEAR) {
-      warp_point(a.hm, x, y, (double)TAB, X, Y);
       sx = sat_i16(X >> INTER_BITS); sy = sat_i16(Y >> INTER_BITS);
       fx = X & (TAB - 1); fy = Y & (TAB - 1);
     } else {
-      warp_point(a.hm, x, y, 1.0, X, Y);
       sx = sat_i16(X); sy = sat_i16(Y);
     }
   } else {
@@ -149,9 +155,9 @@ __host__ __device__ __forceinline__ void gather_taps_frames(const GatherArgs& a,
                                                             int f0) {
   int sx, sy;
   unsigned fr;
-  if (MODE == 2) {
+  if (MODE >= 2) {
     int X, Y;
-    warp_point(a.hm, x, y, (double)TAB, X, Y);
+    warp_xy<MODE>(a.hm, x, y, false, X, Y);
     sx = sat_i16(X >> INTER_BITS); sy = sat_i16(Y >> INTER_BITS);
     fr = (unsigned)((Y & (TAB - 1)) * TAB + (X & (TAB - 1)));
   } else {

@@ -308,6 +308,96 @@ def warp_perspective(src: np.ndarray, H, dsize, flags: int = INTER_LINEAR, ctx: 
     return out
 
 
+INTER_LINEAR_EXACT, INTER_NEAREST_EXACT, WARP_INVERSE_MAP = L.INTER_LINEAR_EXACT, L.INTER_NEAREST_EXACT, L.WARP_INVERSE_MAP
+BORDER_CONSTANT = 0
+
+
+def _device_images(src, dw, dh, out, ctx, what, call):
+    """The body of the device forms of resize / warp_affine: src a uint8 CUDA array [H][W], [H][W][C] or [N][H][W][C]
+    read in place; out (default a new torch tensor) of the same rank with dh x dw images; call(src, out) with the
+    (pointer, image stride, ...) layouts is run on torch's current stream and only enqueues."""
+    from .sharding import _torch_current_stream
+    ptr, rank, n, sh, sw, ch, simg, srow = _cuda_images(src, what)
+    shape = {2: (dh, dw), 3: (dh, dw, ch), 4: (n, dh, dw, ch)}[rank]
+    if out is None:
+        import torch
+        out = torch.empty(shape, dtype=torch.uint8, device=torch.device("cuda", ctx.device))
+    optr, orank, on, oh, ow, och, oimg, orow = _cuda_images(out, "out")
+    if orank != rank or (on, oh, ow, och) != (n, dh, dw, ch):
+        raise L.BevkError(f"out must be a uint8 CUDA array of shape {shape}")
+    with ctx.on_stream(_torch_current_stream(ctx.device)):
+        L.check(call((C.c_void_p(ptr), simg, sw, sh, srow, ch, n), (C.c_void_p(optr), oimg, dw, dh, orow)))
+    return out
+
+
+def _src_size(src):
+    """(width, height) of a NumPy image or a CUDA array [H][W], [H][W][C] or [N][H][W][C]."""
+    if hasattr(src, "__cuda_array_interface__"):
+        shape = tuple(src.__cuda_array_interface__["shape"])
+        return (shape[1], shape[0]) if len(shape) < 4 else (shape[2], shape[1])
+    return src.shape[1], src.shape[0]
+
+
+def resize_size(ssize, dsize, fx: float = 0, fy: float = 0):
+    """cv2.resize's output size: dsize, or when dsize is (0, 0) / None, (round(sw * fx), round(sh * fy))."""
+    if dsize is not None and tuple(int(v) for v in dsize) != (0, 0):
+        return int(dsize[0]), int(dsize[1])
+    if not (fx > 0 and fy > 0):
+        raise L.BevkError("resize: dsize (0, 0) needs fx > 0 and fy > 0")
+    dw, dh = int(np.rint(ssize[0] * float(fx))), int(np.rint(ssize[1] * float(fy)))   # saturate_cast: half to even
+    if dw <= 0 or dh <= 0:
+        raise L.BevkError(f"resize: fx {fx}, fy {fy} make an empty image from {ssize}")
+    return dw, dh
+
+
+def resize(src, dsize, fx: float = 0, fy: float = 0, interpolation: int = INTER_LINEAR, ctx: L.Context | None = None,
+           out=None):
+    """cv2.resize(src, dsize, fx=fx, fy=fy, interpolation=interpolation) for uint8 images, byte for byte: INTER_NEAREST,
+    INTER_LINEAR and INTER_AREA (others raise BevkError).  As in cv2, a dsize of (0, 0) takes the size from fx, fy and uses
+    them as the scales, which gives other pixels than the dsize form of the same size.
+    NumPy input ([H][W] or [H][W][C]) is uploaded, resized and downloaded; a CUDA array ([H][W], [H][W][C] or a batch
+    [N][H][W][C], rows and images may be padded) is read in place on torch's current stream and the result stays on the
+    device (``out``, default a new torch tensor)."""
+    ctx = ctx or L.default_context()
+    dw, dh = resize_size(_src_size(src), dsize, fx, fy)
+    sx, sy = (float(fx), float(fy)) if dsize is None or tuple(int(v) for v in dsize) == (0, 0) else (0.0, 0.0)
+    if hasattr(src, "__cuda_array_interface__"):
+        return _device_images(src, dw, dh, out, ctx, "resize",
+                              lambda s, d: ctx.lib.bevk_resize_stack(ctx.h, *s, *d, sx, sy, int(interpolation)))
+    img, sw, sh, ss, ch = L.image_view(src)
+    out = _out((dh, dw) if src.ndim == 2 else (dh, dw, ch), out)
+    L.check(ctx.lib.bevk_resize(ctx.h, L.vptr(img), sw, sh, ss, ch, L.vptr(out), dw, dh, dw * ch, sx, sy, int(interpolation)))
+    return out
+
+
+def warp_affine(src, M, dsize, flags: int = INTER_LINEAR, borderMode: int = BORDER_CONSTANT, borderValue=0,
+                ctx: L.Context | None = None, out=None):
+    """cv2.warpAffine(src, M, dsize, flags=flags) for uint8 images with a zero constant border, byte for byte.  M: 2x3.
+    flags: any interpolation warp_perspective takes, optionally | WARP_INVERSE_MAP.  Other borders raise BevkError.
+    Takes NumPy images and CUDA arrays as resize() does."""
+    if borderMode != BORDER_CONSTANT or np.any(np.asarray(borderValue) != 0):
+        raise L.BevkError("warp_affine supports BORDER_CONSTANT with value 0 only")
+    ctx = ctx or L.default_context()
+    m = np.asarray(M, np.float64)
+    if m.shape != (2, 3):
+        raise L.BevkError(f"M must be 2x3, got shape {m.shape}")
+    dw, dh = int(dsize[0]), int(dsize[1])
+    if hasattr(src, "__cuda_array_interface__"):
+        return _device_images(src, dw, dh, out, ctx, "warp_affine",
+                              lambda s, d: ctx.lib.bevk_warp_affine_stack(ctx.h, *s, L.dptr(m), *d, int(flags)))
+    img, sw, sh, ss, ch = L.image_view(src)
+    out = _out((dh, dw) if src.ndim == 2 else (dh, dw, ch), out)
+    L.check(ctx.lib.bevk_warp_affine(ctx.h, L.vptr(img), sw, sh, ss, ch, L.dptr(m), L.vptr(out), dw, dh, dw * ch, int(flags)))
+    return out
+
+
+def last_path(ctx: L.Context | None = None) -> str:
+    """Which kernel the last gather or resize call of ctx launched: 'word' (k_gather4), 'byte' (k_gather), 'taps'
+    (k_gather_taps) or 'resize' (k_resize)."""
+    ctx = ctx or L.default_context()
+    return {4: "word", 1: "byte", 2: "taps", 3: "resize"}.get(int(ctx.lib.bevk_undistort_last_path(ctx.h)), "none")
+
+
 def warp_perspective_maps(map1, map2, H, dsize, ctx: L.Context | None = None):
     """cv2.warpPerspective applied to a CV_16SC2 / CV_16UC1 map pair (Camera.get_bev_maps)."""
     ctx = ctx or L.default_context()

@@ -42,6 +42,9 @@ typedef enum {
  * INTER_AREA as INTER_LINEAR, as cv2.remap and cv2.warpPerspective do; CUBIC and LANCZOS4 need map2.  The BEV engine
  * takes NEAREST and LINEAR only. */
 enum { BEVK_INTER_NEAREST = 0, BEVK_INTER_LINEAR = 1, BEVK_INTER_CUBIC = 2, BEVK_INTER_AREA = 3, BEVK_INTER_LANCZOS4 = 4 };
+/* cv2.INTER_LINEAR_EXACT / INTER_NEAREST_EXACT (refused by every call: BEVK_ERR_UNSUPPORTED) and cv2.WARP_INVERSE_MAP
+ * (bevk_warp_affine's flags: M already maps destination to source). */
+enum { BEVK_INTER_LINEAR_EXACT = 5, BEVK_INTER_NEAREST_EXACT = 6, BEVK_WARP_INVERSE_MAP = 16 };
 enum { BEVK_MAPS_UNDISTORT = 0, BEVK_MAPS_BEV = 1 };
 enum { BEVK_MODEL_FISHEYE = 0, BEVK_MODEL_PINHOLE = 1 };
 /* bevk_bev_run flags.  BEVK_FLAG_NV12 / BEVK_FLAG_I420 (exclusive; they combine with BALANCE) say the frames are YUV
@@ -132,14 +135,44 @@ int bevk_undistort_stack(bevk_ctx *ctx, int slot, const void *d_src, int64_t src
 int bevk_undistort_stack_interp(bevk_ctx *ctx, int slot, const void *d_src, int64_t src_image_stride, int sw, int sh,
                                 int64_t src_row_stride, int channels, int n, void *d_dst, int64_t dst_image_stride,
                                 int dw, int dh, int64_t dst_row_stride, int interp);
-/* Which gather the last undistort call (or bevk_remap / bevk_warp_perspective) launched: 4 = k_gather4 (word path),
- * 1 = k_gather (byte path), 2 = k_gather_taps (INTER_CUBIC / INTER_LANCZOS4), 0 = none yet. */
+/* Which gather the last undistort call (or bevk_remap / bevk_warp_perspective / bevk_warp_affine(_stack) /
+ * bevk_resize(_stack)) launched: 4 = k_gather4 (word path), 1 = k_gather (byte path), 2 = k_gather_taps (INTER_CUBIC /
+ * INTER_LANCZOS4), 3 = k_resize, 0 = none yet. */
 int bevk_undistort_last_path(bevk_ctx *ctx);
 
 /* ---- K4: cv2.warpPerspective(src, H, (dw,dh), flags=interp), border 0 --------
  *   ExtrinsicCalibration/extrinsicCalib.py:166-169, surroundBEV.py:113-114      */
 int bevk_warp_perspective(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t sstride, int channels,
                           const double H[9], uint8_t *dst, int dw, int dh, int64_t dstride, int interp);
+/* ---- cv2.warpAffine(src, M, (dw,dh), flags), BORDER_CONSTANT 0 ------------------
+ *   ExtrinsicCalibration/extrinsicCalib.py:58 (CenterImage.translate)
+ * M: the 2x3 matrix, row-major.  flags: a BEVK_INTER_* (INTER_AREA read as INTER_LINEAR, as cv2 reads it), optionally
+ * | BEVK_WARP_INVERSE_MAP; anything else is BEVK_ERR_UNSUPPORTED.  The same gathers as bevk_warp_perspective, with the
+ * source position of cv2's fixed-point affine walk. */
+int bevk_warp_affine(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t sstride, int channels,
+                     const double M[6], uint8_t *dst, int dw, int dh, int64_t dstride, int flags);
+/* The same for n DEVICE frames, laid out as bevk_undistort_stack lays them out (image and row strides on both sides,
+ * strides smaller than one image and a destination overlapping the source refused with BEVK_ERR_ARG); word and byte
+ * paths as there (bevk_undistort_last_path).  Only enqueues on the ctx stream; can be graph-captured. */
+int bevk_warp_affine_stack(bevk_ctx *ctx, const void *d_src, int64_t src_image_stride, int sw, int sh,
+                           int64_t src_row_stride, int channels, int n, const double M[6], void *d_dst,
+                           int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride, int flags);
+
+/* ---- cv2.resize(src, (dw,dh), fx=fx, fy=fy, interpolation=interp) -----------------
+ *   IntrinsicCalibration/intrinsicCalib.py:236, ExtrinsicCalibration/extrinsicCalib.py:125 (ScaleImage)
+ * dw x dh is the destination the caller allocated.  fx = fy = 0: cv2's dsize form (scales dw / sw, dh / sh); fx, fy
+ * > 0: cv2's dsize = (0, 0) form, whose scales are fx and fy themselves (other pixels than the dsize form of the same
+ * size), and dw, dh must be cv2's size for them, round(sw * fx) x round(sh * fy) (BEVK_ERR_ARG otherwise).
+ * interp: BEVK_INTER_NEAREST, _LINEAR or _AREA; CUBIC, LANCZOS4, LINEAR_EXACT and NEAREST_EXACT are
+ * BEVK_ERR_UNSUPPORTED.  Kernel k_resize (bevk_undistort_last_path reports 3). */
+int bevk_resize(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t sstride, int channels, uint8_t *dst, int dw,
+                int dh, int64_t dstride, double fx, double fy, int interp);
+/* The same for n DEVICE frames, laid out and checked as bevk_warp_affine_stack's.  Only enqueues; can be
+ * graph-captured. */
+int bevk_resize_stack(bevk_ctx *ctx, const void *d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
+                      int channels, int n, void *d_dst, int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride,
+                      double fx, double fy, int interp);
+
 /* The same call applied to a 16SC2 / 16UC1 map pair (Camera.get_bev_maps,
  * surroundBEV.py:105-108): float-table bilinear, rounded, saturated.            */
 int bevk_warp_maps(bevk_ctx *ctx, const int16_t *map1, const uint16_t *map2, int sw, int sh,
