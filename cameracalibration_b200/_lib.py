@@ -111,6 +111,12 @@ SIGNATURES = {
     "bevk_jpeg_encode_params": (C.c_int, [_p, C.POINTER(C.c_int), C.c_int, _p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int,
                                           C.c_int, _p, C.c_uint64, C.POINTER(C.c_uint64)]),
     "bevk_jpeg_encode_params_bound": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_uint64)]),
+    "bevk_jpeg_encode_channels": (C.c_int, [_p, C.POINTER(C.c_int), C.c_int, _p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int,
+                                            C.c_int, C.c_int, _p, C.c_uint64, C.POINTER(C.c_uint64)]),
+    "bevk_png_encode_channels": (C.c_int, [_p, C.POINTER(C.c_int), C.c_int, _p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int,
+                                           C.c_int, _p, C.c_uint64, C.POINTER(C.c_uint64)]),
+    "bevk_jpeg_encode_channels_bound": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_uint64)]),
+    "bevk_png_encode_channels_bound": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint64)]),
     "bevk_jpeg_encode": (C.c_int, [_p, _p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, _p, C.c_uint64,
                                    C.POINTER(C.c_uint64)]),
     "bevk_undistort_jpeg": (C.c_int, [_p, C.c_int, _p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, _p, C.c_uint64,

@@ -2539,11 +2539,20 @@ struct EncIn {
   long long istride = 0, pitch = 0;
 };
 
-// n 3-channel device images of the bevk_*_encode calls, rows row_stride bytes apart, image_stride apart (n > 1)
-static int check_device_images(const void* d_images, int64_t image_stride, int64_t row_stride, int n, int w, int h) {
+// The channel counts the encoders take: grey, BGR, BGRA
+static int check_enc_channels(int channels) {
+  if (channels != 1 && channels != 3 && channels != 4)
+    return fail(BEVK_ERR_UNSUPPORTED, "%d channels: the encoders take 1 (grey), 3 (BGR) or 4 (BGRA)", channels);
+  return BEVK_OK;
+}
+
+// n device images of `channels` channels of the bevk_*_encode calls, rows row_stride bytes apart, image_stride apart
+// (n > 1)
+static int check_device_images(const void* d_images, int64_t image_stride, int64_t row_stride, int channels, int n, int w, int h) {
   if (!d_images || n < 1) return fail(BEVK_ERR_ARG, "bad argument");
-  if (row_stride < (int64_t)w * 3) return fail(BEVK_ERR_ARG, "row stride %lld < %d bytes", (long long)row_stride, w * 3);
-  if (n > 1 && image_stride < (int64_t)(h - 1) * row_stride + (int64_t)w * 3)
+  const int64_t rb = (int64_t)w * channels;
+  if (row_stride < rb) return fail(BEVK_ERR_ARG, "row stride %lld < %lld bytes", (long long)row_stride, (long long)rb);
+  if (n > 1 && image_stride < (int64_t)(h - 1) * row_stride + rb)
     return fail(BEVK_ERR_ARG, "image stride %lld is smaller than one image", (long long)image_stride);
   return BEVK_OK;
 }
@@ -2697,12 +2706,33 @@ int bevk_jpeg_encode_bound_params(int width, int height, const int* params, int 
 }
 
 int bevk_jpeg_encode_params_bound(int width, int height, const int* params, int n, uint64_t* bytes) {
+  return bevk_jpeg_encode_channels_bound(width, height, 3, params, n, bytes);
+}
+
+int bevk_jpeg_encode_channels_bound(int width, int height, int channels, const int* params, int n, uint64_t* bytes) {
   if (!bytes) return fail(BEVK_ERR_ARG, "null bytes");
+  RET(check_enc_channels(channels));
   RET(jpeg_size_check(width, height));
   jpeg::Opts o;
   RET(jpeg_params_check(params, n, 95, &o));
-  *bytes = jpeg_bound(width, height, o);
+  *bytes = jpeg_bound(width, height, jpeg::channel_opts(o, channels));
   return BEVK_OK;
+}
+
+// Launch shapes of the baseline kernels: f(HY, VY, NC) as integral constants, for the layout of o (grey: 1, 1, 1)
+template <class F>
+static int with_layout(const jpeg::Opts& o, F&& f) {
+  using std::integral_constant;
+  if (o.nc == 1) return f(integral_constant<int, 1>{}, integral_constant<int, 1>{}, integral_constant<int, 1>{});
+  return jpeg::with_sampling(o.hy, o.vy, [&](auto hy, auto vy) { return f(hy, vy, integral_constant<int, 3>{}); });
+}
+// k_jpeg_blocks of layout (HY, VY, NC) over images of C bytes per pixel
+template <int HY, int VY, int NC>
+static void launch_blocks(int C, unsigned grid, cudaStream_t st, const jpeg::EncArgs& a) {
+  using namespace jpeg;
+  if constexpr (NC == 1) k_jpeg_blocks<1, 1, 1><<<grid, kBlockThreads, 0, st>>>(a);
+  else if (C == 4) k_jpeg_blocks<HY, VY, 4><<<grid, kBlockThreads, 0, st>>>(a);
+  else k_jpeg_blocks<HY, VY><<<grid, kBlockThreads, 0, st>>>(a);
 }
 
 // Header (baseline) or frame prefix (progressive) into d_header and the tables into d_tabs: they depend on
@@ -2723,9 +2753,9 @@ static int jpeg_tables(bevk_ctx* c, int w, int h, const jpeg::Opts& o) {
   return BEVK_OK;
 }
 
-// Enqueue the baseline encoder over n w x h images into slot s on the ctx stream.  The work buffers are single: batches
-// use them one after the other in stream order.
-static int jpeg_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int w, int h, const jpeg::Opts& o) {
+// Enqueue the baseline encoder over n w x h images of C channels (o = channel_opts(..., C)) into slot s on the ctx
+// stream.  The work buffers are single: batches use them one after the other in stream order.
+static int jpeg_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int w, int h, const jpeg::Opts& o, int C = 3) {
   using namespace jpeg;
   auto& e = c->enc;
   RET(jpeg_tables(c, w, h, o));
@@ -2777,19 +2807,19 @@ static int jpeg_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int w, int h
   }
   const unsigned gb = (unsigned)((nb + kBlockThreads - 1) / kBlockThreads), gc = (unsigned)((nch + 255) / 256);
   CU(cudaEventRecord(c->ev0, c->stream));
-  RET(with_sampling(o.hy, o.vy, [&](auto hy, auto vy) -> int {
-    constexpr int HY = hy(), VY = vy();
-    k_jpeg_blocks<HY, VY><<<gb, kBlockThreads, 0, c->stream>>>(a);
+  RET(with_layout(o, [&](auto hy, auto vy, auto nc) -> int {
+    constexpr int HY = hy(), VY = vy(), NC = nc();
+    launch_blocks<HY, VY, NC>(C, gb, c->stream, a);
     LAUNCHED(c);
-    k_jpeg_dc<HY, VY><<<gb, kBlockThreads, 0, c->stream>>>(a);
+    k_jpeg_dc<HY, VY, NC><<<gb, kBlockThreads, 0, c->stream>>>(a);
     LAUNCHED(c);
     if (o.optimize) {   // per-image tables from the symbol counts, then every block's bits under them
       CU(cudaMemsetAsync(a.counts, 0, (size_t)n * 1024 * 8, c->stream));
-      k_jpeg_count<HY, VY><<<gb, kBlockThreads, 0, c->stream>>>(a);
+      k_jpeg_count<HY, VY, NC><<<gb, kBlockThreads, 0, c->stream>>>(a);
       LAUNCHED(c);
-      k_jpeg_huff<<<(unsigned)((4ll * n + kHuffThreads - 1) / kHuffThreads), kHuffThreads, 0, c->stream>>>(a);
+      k_jpeg_huff<NC><<<(unsigned)((4ll * n + kHuffThreads - 1) / kHuffThreads), kHuffThreads, 0, c->stream>>>(a);
       LAUNCHED(c);
-      k_jpeg_bits<HY, VY><<<gb, kBlockThreads, 0, c->stream>>>(a);
+      k_jpeg_bits<HY, VY, NC><<<gb, kBlockThreads, 0, c->stream>>>(a);
       LAUNCHED(c);
     }
     CU(cub::DeviceScan::ExclusiveSum(e.scan_tmp.p, tmp1, a.bits, a.offs, (int)nb, c->stream));
@@ -2800,10 +2830,10 @@ static int jpeg_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int w, int h
     }
     k_jpeg_zero<<<c->n_sm * 4, 256, 0, c->stream>>>(a);
     LAUNCHED(c);
-    if (o.optimize && o.rst) k_jpeg_pack<HY, VY, true, true><<<gb, kBlockThreads, 0, c->stream>>>(a);
-    else if (o.optimize) k_jpeg_pack<HY, VY, true, false><<<gb, kBlockThreads, 0, c->stream>>>(a);
-    else if (o.rst) k_jpeg_pack<HY, VY, false, true><<<gb, kBlockThreads, 0, c->stream>>>(a);
-    else k_jpeg_pack<HY, VY, false, false><<<gb, kBlockThreads, 0, c->stream>>>(a);
+    if (o.optimize && o.rst) k_jpeg_pack<HY, VY, true, true, NC><<<gb, kBlockThreads, 0, c->stream>>>(a);
+    else if (o.optimize) k_jpeg_pack<HY, VY, true, false, NC><<<gb, kBlockThreads, 0, c->stream>>>(a);
+    else if (o.rst) k_jpeg_pack<HY, VY, false, true, NC><<<gb, kBlockThreads, 0, c->stream>>>(a);
+    else k_jpeg_pack<HY, VY, false, false, NC><<<gb, kBlockThreads, 0, c->stream>>>(a);
     LAUNCHED(c);
     return BEVK_OK;
   }));
@@ -2818,8 +2848,10 @@ static int jpeg_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int w, int h
 }
 
 // Enqueue the progressive encoder over n w x h images into slot s: k_jpeg_blocks, then the k_jpeg_prog_* pipeline over
-// every scan of every image at once (bevk_jpeg_prog.cuh).
-static int jpeg_prog_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int w, int h, const jpeg::Opts& o) {
+// every scan of every image at once (bevk_jpeg_prog.cuh).  The k_jpeg_prog_* kernels are instantiated per component
+// count (NC = o.nc): grey images run the six-scan script.
+template <int NC>
+static int jpeg_prog_run(bevk_ctx* c, int s, const EncIn& in, int n, int w, int h, const jpeg::Opts& o, int C) {
   using namespace jpeg;
   using namespace jpeg::prog;
   auto& e = c->enc;
@@ -2894,19 +2926,19 @@ static int jpeg_prog_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int w, 
   const unsigned gN = (unsigned)((N + 255) / 256), gN1 = (unsigned)((N + 1 + 255) / 256), gS = (unsigned)((NS + 255) / 256);
   const unsigned gc = (unsigned)((nch + 255) / 256);
   CU(cudaEventRecord(c->ev0, c->stream));
-  RET(with_sampling(o.hy, o.vy, [&](auto hy, auto vy) -> int {
-    k_jpeg_blocks<hy(), vy()><<<gb, kBlockThreads, 0, c->stream>>>(b);
+  RET(with_layout(o, [&](auto hy, auto vy, auto nc) -> int {
+    launch_blocks<hy(), vy(), nc()>(C, gb, c->stream, b);
     LAUNCHED(c);
     return BEVK_OK;
   }));
-  k_jpeg_prog_desc<<<gN, 256, 0, c->stream>>>(a);
+  k_jpeg_prog_desc<NC><<<gN, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
-  k_jpeg_prog_hard<<<gN, 256, 0, c->stream>>>(a);
+  k_jpeg_prog_hard<NC><<<gN, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
   CU(cub::DeviceScan::InclusiveSum(st, tmp[0], ItE(a.desc, DescE()), a.pe, (int)N, c->stream));
   CU(cub::DeviceScan::InclusiveSum(st, tmp[1], ItC(a.desc, DescC()), a.pc, (int)N, c->stream));
   CU(cub::DeviceScan::InclusiveSum(st, tmp[2], ItH(a.desc, DescH()), a.ph, (int)N, c->stream));
-  k_jpeg_prog_next<<<gN1, 256, 0, c->stream>>>(a);
+  k_jpeg_prog_next<NC><<<gN1, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
   long long longest = 0;   // the longest scan bounds every chain of run starts
   for (int k = 0; k < kScans; ++k) longest = std::max(longest, L.blk[k + 1] - L.blk[k]);
@@ -2917,29 +2949,32 @@ static int jpeg_prog_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int w, 
   }
   CU(cub::DeviceScan::InclusiveScan(st, tmp[3], itm, a.rs, MaxU(), (int)N, c->stream));
   CU(cudaMemsetAsync(a.counts, 0, (size_t)n * kTables * 256 * 4, c->stream));
-  k_jpeg_prog_count<<<gN, 256, 0, c->stream>>>(a);
+  k_jpeg_prog_count<NC><<<gN, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
-  k_jpeg_prog_huff<<<(unsigned)((n + kProgHuffImages - 1) / kProgHuffImages), kProgHuffThreads, 0, c->stream>>>(a);
+  k_jpeg_prog_huff<NC><<<(unsigned)((n + kProgHuffImages - 1) / kProgHuffImages), kProgHuffThreads, 0, c->stream>>>(a);
   LAUNCHED(c);
-  k_jpeg_prog_bits<<<gN, 256, 0, c->stream>>>(a);
+  k_jpeg_prog_bits<NC><<<gN, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
   CU(cub::DeviceScan::ExclusiveSum(st, tmp[4], a.bits, a.offs, (int)N, c->stream));
-  k_jpeg_prog_segs<<<gS, 256, 0, c->stream>>>(a);
+  k_jpeg_prog_segs<NC><<<gS, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
   CU(cub::DeviceScan::ExclusiveSum(st, tmp[5], a.ilen, a.iofs, (int)NS, c->stream));
   CU(cub::DeviceScan::ExclusiveSum(st, tmp[6], a.ins, a.insx, (int)NS, c->stream));
   k_jpeg_prog_zero<<<c->n_sm * 4, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
-  k_jpeg_prog_pack<<<gN, 256, 0, c->stream>>>(a);
+  k_jpeg_prog_pack<NC><<<gN, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
   k_jpeg_prog_ffcount<<<gc, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
   CU(cub::DeviceScan::ExclusiveSum(st, tmp[7], a.ffcnt, a.ffscan, (int)nch, c->stream));
-  k_jpeg_prog_layout<<<1, 256, 0, c->stream>>>(a);
+  k_jpeg_prog_layout<NC><<<1, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
-  k_jpeg_prog_stuff<<<gc, 256, 0, c->stream>>>(a);
+  k_jpeg_prog_stuff<NC><<<gc, 256, 0, c->stream>>>(a);
   LAUNCHED(c);
   return slot_close(c, s, n);
+}
+static int jpeg_prog_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int w, int h, const jpeg::Opts& o, int C = 3) {
+  return o.nc == 1 ? jpeg_prog_run<1>(c, s, in, n, w, h, o, C) : jpeg_prog_run<3>(c, s, in, n, w, h, o, C);
 }
 
 // Images per chunk of the chunked device-frame calls.  8 canvases (24 MB at 1000^2: they stay in the 50 MB L2) beat the
@@ -3012,19 +3047,38 @@ int bevk_jpeg_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, in
                                  width, height, quality, out, capacity, sizes);
 }
 
+// n device images of `channels` channels under a per-call list, as one chunk: all streams or none
+static int jpeg_encode_images(bevk_ctx* c, const int* params, int n_params, const void* d_images, int64_t image_stride,
+                              int64_t row_stride, int channels, int n, int width, int height, int quality, uint8_t* out,
+                              uint64_t capacity, uint64_t* sizes) {
+  RET(use(c));
+  RET(check_enc_channels(channels));
+  jpeg::Opts o;
+  RET(jpeg_params_check(params, n_params, quality, &o));
+  o = jpeg::channel_opts(o, channels);
+  RET(jpeg_size_check(width, height));
+  RET(check_device_images(d_images, image_stride, row_stride, channels, n, width, height));
+  const EncIn in{d_images, image_stride, row_stride};
+  return enc_chunks(c, "JPEG", n, n, true, out, capacity, sizes, [&](int, int, int s) {
+    return o.progressive ? jpeg_prog_enqueue(c, s, in, n, width, height, o, channels)
+                         : jpeg_enqueue(c, s, in, n, width, height, o, channels);
+  });
+}
+
 int bevk_jpeg_encode_params(bevk_ctx* c, const int* params, int n_params, const void* d_images, int64_t image_stride,
                             int64_t row_stride, int n, int width, int height, int quality, uint8_t* out, uint64_t capacity,
                             uint64_t* sizes) {
   NvtxRange nvtx_call("bevk_jpeg_encode_params (device images -> host JPEG streams)");
-  RET(use(c));
-  jpeg::Opts o;
-  RET(jpeg_params_check(params, n_params, quality, &o));
-  RET(jpeg_size_check(width, height));
-  RET(check_device_images(d_images, image_stride, row_stride, n, width, height));
-  const EncIn in{d_images, image_stride, row_stride};
-  return enc_chunks(c, "JPEG", n, n, true, out, capacity, sizes, [&](int, int, int s) {
-    return o.progressive ? jpeg_prog_enqueue(c, s, in, n, width, height, o) : jpeg_enqueue(c, s, in, n, width, height, o);
-  });
+  return jpeg_encode_images(c, params, n_params, d_images, image_stride, row_stride, 3, n, width, height, quality, out,
+                            capacity, sizes);
+}
+
+int bevk_jpeg_encode_channels(bevk_ctx* c, const int* params, int n_params, const void* d_images, int64_t image_stride,
+                              int64_t row_stride, int channels, int n, int width, int height, int quality, uint8_t* out,
+                              uint64_t capacity, uint64_t* sizes) {
+  NvtxRange nvtx_call("bevk_jpeg_encode_channels (device images -> host JPEG streams)");
+  return jpeg_encode_images(c, params, n_params, d_images, image_stride, row_stride, channels, n, width, height, quality,
+                            out, capacity, sizes);
 }
 
 int bevk_undistort_jpeg(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int interp, int quality,
@@ -3084,8 +3138,8 @@ static int png_params_check(const int* params, int n, png::Opts* o, bool hash_ch
   return BEVK_OK;
 }
 
-static int png_size_check(int width, int height) {
-  if (width < 1 || height < 1 || png::image_bytes(width, height) > png::kMaxImageBytes)
+static int png_size_check(int width, int height, int channels = 3) {
+  if (width < 1 || height < 1 || png::image_bytes(width, height, channels) > png::kMaxImageBytes)
     return fail(BEVK_ERR_ARG, "bad PNG size %dx%d (at least 1x1, at most %lld filtered bytes)", width, height,
                 png::kMaxImageBytes);
   return BEVK_OK;
@@ -3108,6 +3162,14 @@ int bevk_png_encode_bound(int width, int height, const int* params, int n, uint6
   return BEVK_OK;
 }
 
+int bevk_png_encode_channels_bound(int width, int height, int channels, uint64_t* bytes) {
+  if (!bytes) return fail(BEVK_ERR_ARG, "null bytes");
+  RET(check_enc_channels(channels));
+  RET(png_size_check(width, height, channels));
+  *bytes = (uint64_t)png::encode_bound(width, height, channels);
+  return BEVK_OK;
+}
+
 // Filtered bytes per group: the group's scans, symbols and run starts take 11 bytes per filtered byte of scratch.  The
 // hash-chain parse takes about 50 (sort keys and positions twice, prev, two match records, two jump arrays, marks,
 // counts, symbols and distances, the sort's scratch), so its groups are a quarter of the size; a single image larger
@@ -3116,14 +3178,14 @@ int bevk_png_encode_bound(int width, int height, const int* params, int n, uint6
 // last 2 bytes: at most 2^16 images per group.
 constexpr long long kPngGroupBytes = 1ll << 27, kPngLazyGroupBytes = 1ll << 25, kPngLazyGroupImages = 1ll << 16;
 
-// Enqueue the PNG encoder over n width x height images into slot s, group by group; every group's streams land
-// compacted in the slot after the ones before (the running end at meta[2n]).
-static int png_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int width, int height, const png::Opts& o) {
+// Enqueue the PNG encoder over n width x height images of C channels into slot s, group by group; every group's streams
+// land compacted in the slot after the ones before (the running end at meta[2n]).
+static int png_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int width, int height, const png::Opts& o, int C = 3) {
   using namespace png;
   auto& e = c->png;
   const bool lazy = lazy_parse(o);
-  const long long N = image_bytes(width, height), maxb = max_blocks(N), zb = zlib_bound(N);
-  const long long zwords = zb / 4 + 2, maxch = idat_chunks(zb), bound = encode_bound(width, height);
+  const long long N = image_bytes(width, height, C), maxb = max_blocks(N), zb = zlib_bound(N);
+  const long long zwords = zb / 4 + 2, maxch = idat_chunks(zb), bound = encode_bound(width, height, C);
   const int g = (int)std::max(1ll, std::min({(long long)n, (lazy ? kPngLazyGroupBytes : kPngGroupBytes) / N,
                                                lazy ? kPngLazyGroupImages : (long long)n}));
   const long long gN = g * N;
@@ -3143,6 +3205,7 @@ static int png_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int width, in
   using FlagIt = cub::TransformInputIterator<unsigned, SymbolFlag, cub::CountingInputIterator<unsigned>>;
   PngArgs a{};
   a.istride = in.istride; a.pitch = in.pitch; a.W = width; a.H = height; a.filters = o.filters; a.strategy = o.strategy;
+  a.colour = colour_type(C); a.rb = row_bytes(width, C);
   a.N = N; a.maxb = maxb; a.zwords = zwords; a.maxchunks = maxch;
   a.f = e.f.as<uint8_t>(); a.rowad = e.rowad.as<Adler>(); a.syms = e.syms.as<uint16_t>(); a.nsym = e.nsym.as<unsigned>();
   a.blk = e.blk.as<Blk>(); a.codes = e.codes.as<uint32_t>(); a.hdr = e.hdr.as<uint32_t>(); a.zw = e.zw.as<uint32_t>();
@@ -3183,7 +3246,10 @@ static int png_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int width, in
     a.sizes = meta + n + b0;
     const long long total = gn * N;
     const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, (long long)c->n_sm * 16);
-    k_png_filter<<<(unsigned)(gn * height), kPngThreads, 0, c->stream>>>(a);
+    const unsigned gf = (unsigned)(gn * height);
+    if (C == 1) k_png_filter<1><<<gf, kPngThreads, 0, c->stream>>>(a);
+    else if (C == 4) k_png_filter<4><<<gf, kPngThreads, 0, c->stream>>>(a);
+    else k_png_filter<<<gf, kPngThreads, 0, c->stream>>>(a);
     LAUNCHED(c);
     if (lazy) {
       k_png_keys<<<grid, 256, 0, c->stream>>>(HashKey{a.f, N, (unsigned)gn}, e.keys.as<unsigned>(), e.pos.as<unsigned>(),
@@ -3236,14 +3302,15 @@ static int png_enqueue(bevk_ctx* c, int s, const EncIn& in, int n, int width, in
   return slot_close(c, s, n);
 }
 
-// n device images through the PNG encoder under o, as one chunk: all streams or none
+// n device images of `channels` channels through the PNG encoder under o, as one chunk: all streams or none
 static int png_encode_images(bevk_ctx* c, const png::Opts& o, const void* d_images, int64_t image_stride, int64_t row_stride,
-                             int n, int width, int height, uint8_t* out, uint64_t capacity, uint64_t* sizes) {
-  RET(png_size_check(width, height));
-  RET(check_device_images(d_images, image_stride, row_stride, n, width, height));
+                             int channels, int n, int width, int height, uint8_t* out, uint64_t capacity, uint64_t* sizes) {
+  RET(check_enc_channels(channels));
+  RET(png_size_check(width, height, channels));
+  RET(check_device_images(d_images, image_stride, row_stride, channels, n, width, height));
   const EncIn in{d_images, image_stride, row_stride};
   return enc_chunks(c, "PNG", n, n, true, out, capacity, sizes, [&](int, int, int s) {
-    return png_enqueue(c, s, in, n, width, height, o);
+    return png_enqueue(c, s, in, n, width, height, o, channels);
   });
 }
 
@@ -3253,7 +3320,7 @@ int bevk_png_encode(bevk_ctx* c, const void* d_images, int64_t image_stride, int
   RET(use(c));
   png::Opts o;
   png::normalise(c->png.params.data(), (int)c->png.params.size(), &o);   // bevk_png_set_params checked the list
-  return png_encode_images(c, o, d_images, image_stride, row_stride, n, width, height, out, capacity, sizes);
+  return png_encode_images(c, o, d_images, image_stride, row_stride, 3, n, width, height, out, capacity, sizes);
 }
 
 // The parameter list per call, as cv2.imencode takes it; also zlib's hash-chain parse at levels 4..9 (deflate_slow,
@@ -3262,10 +3329,18 @@ int bevk_png_encode_params(bevk_ctx* c, const int* params, int n_params, const v
                            int64_t row_stride, int n, int width, int height, uint8_t* out, uint64_t capacity,
                            uint64_t* sizes) {
   NvtxRange nvtx_call("bevk_png_encode_params (device images -> host PNG streams)");
+  return bevk_png_encode_channels(c, params, n_params, d_images, image_stride, row_stride, 3, n, width, height, out,
+                                  capacity, sizes);
+}
+
+int bevk_png_encode_channels(bevk_ctx* c, const int* params, int n_params, const void* d_images, int64_t image_stride,
+                             int64_t row_stride, int channels, int n, int width, int height, uint8_t* out, uint64_t capacity,
+                             uint64_t* sizes) {
+  NvtxRange nvtx_call("bevk_png_encode_channels (device images -> host PNG streams)");
   RET(use(c));
   png::Opts o;
   RET(png_params_check(params, n_params, &o, true));
-  return png_encode_images(c, o, d_images, image_stride, row_stride, n, width, height, out, capacity, sizes);
+  return png_encode_images(c, o, d_images, image_stride, row_stride, channels, n, width, height, out, capacity, sizes);
 }
 
 // ------------------------------------------------------------------ CUDA graphs

@@ -21,13 +21,21 @@
 // Everything per block is __host__ __device__: tests/host/jpeg_enc.cu runs the same functions serially over a whole
 // image and compares the stream with live cv2.imencode.
 //
+// Grey and BGRA images (cv2.imencode of [H][W] / [H][W][1] and [H][W][4]):
+//   grey       one component (JCS_GRAYSCALE): an MCU is one 8x8 block, ceil(W/8) x ceil(H/8) blocks in raster order,
+//              edges replicated, the sample is the byte itself (libjpeg's grayscale pass-through); only quantisation
+//              table 0 at the luma quality and DHT DC0 / AC0; SAMPLING_FACTOR does not reach the stream (a one-component
+//              scan is non-interleaved); the restart interval counts blocks.  Header: kGreyHeaderBytes
+//   BGRA       cv2 drops alpha: the colour samples are read with a 4-byte pixel stride and the stream is the BGR one
+//
 // The default (no parameters) is the 4:2:0 instance: geom(W, H), make_tables(q, ...), make_header(W, H, q, ...) and
 // encode_bound(W, H) are the general forms at Opts{2, 2, q, q}.
 //
 // Device pipeline for n equal-sized images (bevk_api.cu: jpeg_enqueue, then enc_collect copies the streams out):
 //   k_jpeg_blocks  one thread per 8x8 block: BGR -> samples with the edge rules, FDCT, quantise, int16 zigzag
 //                  coefficients (128 B per block) and the block's AC bit count
-//   (k_jpeg_blocks, k_jpeg_dc and k_jpeg_pack are instantiated per luma sampling HY x VY: the MCU layout is constant)
+//   (k_jpeg_blocks, k_jpeg_dc and k_jpeg_pack are instantiated per luma sampling HY x VY: the MCU layout is constant;
+//    grey images take the NC = 1 instances, one block per MCU, and k_jpeg_blocks loads C = 1, 3 or 4 bytes per pixel)
 //   k_jpeg_dc      DC differences (dummy blocks resolved), bits per block
 //   scan           exclusive sum of bits per block (CUB): every block's bit offset in its image's stream
 //   k_jpeg_zero    clears the used words of each image's bit buffer
@@ -59,6 +67,9 @@ constexpr int kDriBytes = 6;                  // DRI segment, written when resta
 constexpr int kMaxHeaderBytes = kHeaderBytes + kDriBytes;   // optimal DHTs are never longer than Annex K's
 constexpr int kChunk = 128;                   // bytes per thread of the stuffing pass
 constexpr int kMaxDim = 65500;                // JPEG_MAX_DIMENSION of libjpeg
+constexpr int kGreyHeaderPrefix = 102;        // grey: SOI + APP0 + DQT 0 + SOF0 with one component
+constexpr int kGreyAnnexKDhtBytes = 216;      // grey: DHT DC0 + AC0
+constexpr int kGreyHeaderBytes = 328;         // grey: prefix + DHT DC0 AC0 + SOS with one component
 
 // Per-quality tables the kernels read (built on the host, copied into shared memory per CTA).
 struct Tables {
@@ -72,6 +83,7 @@ struct Tables {
 struct Geom {
   int W, H, mcux, mcuy, wb, hb;   // MCUs across / down, luma blocks across / down that hold image samples
   int hy, vy;                     // luma blocks per MCU across / down
+  int nc;                         // components: 3 (YCbCr) or 1 (grey: hy = vy = 1)
 };
 __host__ __device__ inline Geom geom(int W, int H, int hy, int vy) {
   Geom g;
@@ -79,11 +91,14 @@ __host__ __device__ inline Geom geom(int W, int H, int hy, int vy) {
   g.mcux = (W + 8 * hy - 1) / (8 * hy); g.mcuy = (H + 8 * vy - 1) / (8 * vy);
   g.wb = (W + 7) / 8; g.hb = (H + 7) / 8;
   g.hy = hy; g.vy = vy;
+  g.nc = 3;
   return g;
 }
 __host__ __device__ inline Geom geom(int W, int H) { return geom(W, H, 2, 2); }
+// blocks per MCU: the hy*vy luma blocks, then Cb and Cr (none for grey)
+__host__ __device__ inline int mcu_blocks(const Geom& g) { return g.hy * g.vy + (g.nc == 1 ? 0 : 2); }
 // blocks of one image in scan order: MCU raster, per MCU the hy*vy luma blocks row-major, Cb, Cr
-__host__ __device__ inline long long blocks_per_image(const Geom& g) { return (long long)g.mcux * g.mcuy * (g.hy * g.vy + 2); }
+__host__ __device__ inline long long blocks_per_image(const Geom& g) { return (long long)g.mcux * g.mcuy * mcu_blocks(g); }
 
 // luma block k (0..HY*VY-1) of MCU (mx, my) lies outside the image's blocks: a dummy (AC 0, DC of the block before it)
 template <int HY, int VY>
@@ -110,22 +125,25 @@ __host__ __device__ inline int ld8(const uint8_t* p) {
 #endif
 }
 
-// pixel (x, y) of a BGR image with rows pitch bytes apart
+// pixel (x, y) of a BGR (C 3) or BGRA (C 4) image with rows pitch bytes apart
+template <int C = 3>
 __host__ __device__ inline void bgr_at(const uint8_t* img, long long pitch, int x, int y, int& b, int& g, int& r) {
-  const uint8_t* p = img + y * pitch + 3ll * x;
+  const uint8_t* p = img + y * pitch + (long long)C * x;
   b = ld8(p); g = ld8(p + 1); r = ld8(p + 2);
 }
 
-// Sample (r, c) of block k of MCU (mx, my): luma (k < HY*VY) or Cb (k == HY*VY) / Cr after HY x VY subsampling.
-template <int HY, int VY>
+// Sample (r, c) of block k of MCU (mx, my): luma (k < HY*VY) or Cb (k == HY*VY) / Cr after HY x VY subsampling, of an
+// image of C channels (1 grey: the byte itself, HY = VY = 1; 3 BGR; 4 BGRA, alpha unread).
+template <int HY, int VY, int C = 3>
 __host__ __device__ inline int block_sample(const uint8_t* img, long long pitch, const Geom& g, int mx, int my, int k, int r, int c) {
   constexpr int NY = HY * VY;
   if (k < NY) {
     int x = (HY * mx + k % HY) * 8 + c, y = (VY * my + k / HY) * 8 + r;
     x = x < g.W ? x : g.W - 1;
     y = y < g.H ? y : g.H - 1;
+    if constexpr (C == 1) return ld8(img + y * pitch + x);
     int b, gg, rr;
-    bgr_at(img, pitch, x, y, b, gg, rr);
+    bgr_at<C>(img, pitch, x, y, b, gg, rr);
     return ycc_y(b, gg, rr);
   }
   const int last = (g.H + VY - 1) / VY - 1;              // chroma rows past ceil(H/VY) repeat the last one
@@ -138,7 +156,7 @@ __host__ __device__ inline int block_sample(const uint8_t* img, long long pitch,
     for (int j = 0; j < HY; ++j) {
       const int x = HY * cx + j < g.W ? HY * cx + j : g.W - 1;
       int b, gg, rr;
-      bgr_at(img, pitch, x, y, b, gg, rr);
+      bgr_at<C>(img, pitch, x, y, b, gg, rr);
       s += k == NY ? ycc_cb(b, gg, rr) : ycc_cr(b, gg, rr);
     }
   }
@@ -160,13 +178,19 @@ inline auto with_sampling(int hy, int vy, F&& f) {
 }
 
 // The 64 samples of a block, level-shifted (sample - 128), natural order.
-template <int HY, int VY>
+template <int HY, int VY, int C = 3>
 __host__ __device__ inline void load_block_s(const uint8_t* img, long long pitch, const Geom& g, int mx, int my, int k, int* d) {
   for (int r = 0; r < 8; ++r)
-    for (int c = 0; c < 8; ++c) d[r * 8 + c] = block_sample<HY, VY>(img, pitch, g, mx, my, k, r, c) - 128;
+    for (int c = 0; c < 8; ++c) d[r * 8 + c] = block_sample<HY, VY, C>(img, pitch, g, mx, my, k, r, c) - 128;
 }
 inline void load_block(const uint8_t* img, long long pitch, const Geom& g, int mx, int my, int k, int* d) {
   with_sampling(g.hy, g.vy, [&](auto hy, auto vy) { load_block_s<hy(), vy()>(img, pitch, g, mx, my, k, d); });
+}
+// the same for an image of `channels` (1, 3 or 4) channels
+inline void load_block(const uint8_t* img, long long pitch, const Geom& g, int channels, int mx, int my, int k, int* d) {
+  if (channels == 1) return load_block_s<1, 1, 1>(img, pitch, g, mx, my, k, d);
+  if (channels == 3) return load_block(img, pitch, g, mx, my, k, d);
+  with_sampling(g.hy, g.vy, [&](auto hy, auto vy) { load_block_s<hy(), vy(), 4>(img, pitch, g, mx, my, k, d); });
 }
 
 // ------------------------------------------------------------------ forward DCT (jfdctint.c, islow) and quantisation
@@ -395,12 +419,14 @@ __host__ __device__ inline int gen_optimal_table(long long* freq, uint8_t* bits1
 }
 
 // A stream's header with optimised tables: the common header's prefix (SOI .. SOF0), DHT DC0 AC0 DC1 AC1 from bits[t]
-// / vals[t] (t = 2 * table + class), then the common header's tail (DRI, SOS).  Returns the header's length.
+// / vals[t] (t = 2 * table + class; DC0 AC0 only for grey, nc 1), then the common header's tail (DRI, SOS).  Returns
+// the header's length.
 __host__ __device__ inline int optimal_header(const uint8_t* common, int common_len, const uint8_t (*bits)[16],
-                                              const uint8_t (*vals)[256], uint8_t* out) {
+                                              const uint8_t (*vals)[256], uint8_t* out, int nc = 3) {
+  const int prefix = nc == 1 ? kGreyHeaderPrefix : kHeaderPrefix, dhts = nc == 1 ? kGreyAnnexKDhtBytes : kAnnexKDhtBytes;
   int o = 0;
-  for (int k = 0; k < kHeaderPrefix; ++k) out[o++] = common[k];
-  for (int t = 0; t < 4; ++t) {
+  for (int k = 0; k < prefix; ++k) out[o++] = common[k];
+  for (int t = 0; t < (nc == 1 ? 2 : 4); ++t) {
     int n = 0;
     for (int l = 0; l < 16; ++l) n += bits[t][l];
     const int len = 2 + 1 + 16 + n;
@@ -409,7 +435,7 @@ __host__ __device__ inline int optimal_header(const uint8_t* common, int common_
     for (int l = 0; l < 16; ++l) out[o++] = bits[t][l];
     for (int k = 0; k < n; ++k) out[o++] = vals[t][k];
   }
-  for (int k = kHeaderPrefix + kAnnexKDhtBytes; k < common_len; ++k) out[o++] = common[k];
+  for (int k = prefix + dhts; k < common_len; ++k) out[o++] = common[k];
   return o;
 }
 
@@ -423,9 +449,10 @@ struct Opts {
   int qy = 95, qc = 95;     // quality of the luma / chroma quantisation table, 1..100
   int rst = 0;              // restart interval in MCUs, 0..65535
   int optimize = 0, progressive = 0;
+  int nc = 3;               // components: 3 (BGR / BGRA images) or 1 (grey)
   bool operator==(const Opts& o) const {
     return hy == o.hy && vy == o.vy && qy == o.qy && qc == o.qc && rst == o.rst && optimize == o.optimize &&
-           progressive == o.progressive;
+           progressive == o.progressive && nc == o.nc;
   }
   bool operator!=(const Opts& o) const { return !(*this == o); }
 };
@@ -481,7 +508,17 @@ inline Opts default_opts(int quality) {
   normalise(quality, nullptr, 0, &o);
   return o;
 }
-inline Geom geom(int W, int H, const Opts& o) { return geom(W, H, o.hy, o.vy); }
+// The options for an image of `channels` channels: grey has one component in 1x1 MCUs (cv2's SAMPLING_FACTOR and the
+// chroma quality do not reach its stream; the luma quality is table 0's); BGRA is BGR.
+inline Opts channel_opts(Opts o, int channels) {
+  if (channels == 1) { o.nc = 1; o.hy = o.vy = 1; }
+  return o;
+}
+inline Geom geom(int W, int H, const Opts& o) {
+  Geom g = geom(W, H, o.hy, o.vy);
+  g.nc = o.nc;
+  return g;
+}
 
 // Restart intervals of one image (1 without restart markers): each is byte-aligned with a 1-bit pad and followed by
 // RSTn except the last, so each adds up to 7 pad bits and a 2-byte marker.
@@ -492,7 +529,7 @@ inline long long intervals(const Geom& g, const Opts& o) {
 inline unsigned long long entropy_bound_bits(const Geom& g, const Opts& o) {
   return (unsigned long long)blocks_per_image(g) * (o.optimize ? kMaxBlockBitsOpt : kMaxBlockBits) + 7ull * intervals(g, o);
 }
-inline int header_bytes(const Opts& o) { return kHeaderBytes + (o.rst ? kDriBytes : 0); }
+inline int header_bytes(const Opts& o) { return (o.nc == 1 ? kGreyHeaderBytes : kHeaderBytes) + (o.rst ? kDriBytes : 0); }
 // The params bound: header, entropy bits with every interval's pad, doubled by stuffing, markers, EOI.  With no params
 // this is encode_bound(W, H).
 inline unsigned long long encode_bound(const Geom& g, const Opts& o) {
@@ -570,8 +607,10 @@ inline void make_tables(const Opts& o, Tables* t) {
 inline void make_tables(int quality, Tables* t) { make_tables(default_opts(quality), t); }
 
 // SOI, APP0 (JFIF 1.01, no units, 1x1), DQT 0 (qy) and DQT 1 (qc), SOF0 (Y hy x vy table 0, Cb/Cr 1x1 table 1),
-// DHT DC0 AC0 DC1 AC1, SOS (Y 0/0, Cb 1/1, Cr 1/1, Ss 0 Se 63 Ah/Al 0): kHeaderBytes bytes
+// DHT DC0 AC0 DC1 AC1, SOS (Y 0/0, Cb 1/1, Cr 1/1, Ss 0 Se 63 Ah/Al 0): kHeaderBytes bytes.  Grey (o.nc 1): DQT 0,
+// SOF0 with one component (1x1, table 0), DHT DC0 AC0, SOS with one component: kGreyHeaderBytes.
 inline void make_header(int W, int H, const Opts& o, uint8_t* out) {
+  const int nt = o.nc == 1 ? 1 : 2;   // quantisation and Huffman table pairs
   uint8_t* p = out;
   auto b = [&](int v) { *p++ = (uint8_t)v; };
   auto w16 = [&](int v) { b(v >> 8); b(v & 255); };
@@ -579,17 +618,19 @@ inline void make_header(int W, int H, const Opts& o, uint8_t* out) {
   b(0xff); b(0xe0); w16(16);
   for (const char ch : {'J', 'F', 'I', 'F', '\0'}) b(ch);
   b(1); b(1); b(0); w16(1); w16(1); b(0); b(0);
-  for (int t = 0; t < 2; ++t) {
+  for (int t = 0; t < nt; ++t) {
     int q[64];
     quant_steps(t ? o.qc : o.qy, t, q);
     b(0xff); b(0xdb); w16(67); b(t);
     for (int k = 0; k < 64; ++k) b(q[annex_k::kZigzag[k]]);
   }
-  b(0xff); b(0xc0); w16(17); b(8); w16(H); w16(W); b(3);
+  b(0xff); b(0xc0); w16(8 + 3 * o.nc); b(8); w16(H); w16(W); b(o.nc);
   b(1); b((o.hy << 4) | o.vy); b(0);
-  b(2); b(0x11); b(1);
-  b(3); b(0x11); b(1);
-  for (int t = 0; t < 2; ++t) {
+  if (o.nc == 3) {
+    b(2); b(0x11); b(1);
+    b(3); b(0x11); b(1);
+  }
+  for (int t = 0; t < nt; ++t) {
     for (int cls = 0; cls < 2; ++cls) {
       const uint8_t* bits = cls ? annex_k::kAcBits[t] : annex_k::kDcBits[t];
       const uint8_t* vals = cls ? annex_k::kAcVals[t] : annex_k::kDcVals;
@@ -601,10 +642,12 @@ inline void make_header(int W, int H, const Opts& o, uint8_t* out) {
     }
   }
   if (o.rst) { b(0xff); b(0xdd); w16(4); w16(o.rst); }   // DRI
-  b(0xff); b(0xda); w16(12); b(3);
+  b(0xff); b(0xda); w16(6 + 2 * o.nc); b(o.nc);
   b(1); b(0x00);
-  b(2); b(0x11);
-  b(3); b(0x11);
+  if (o.nc == 3) {
+    b(2); b(0x11);
+    b(3); b(0x11);
+  }
   b(0); b(63); b(0);
 }
 inline void make_header(int W, int H, int quality, uint8_t* out) { make_header(W, H, default_opts(quality), out); }
@@ -666,9 +709,13 @@ __device__ inline unsigned long long image_bits(const EncArgs& a, int i) {
 }
 __device__ inline int header_len(const EncArgs& a, int i) { return a.hlen ? a.hlen[i] : a.hlen0; }
 
-template <int HY, int VY>
+// blocks per MCU of an NC-component layout
+template <int HY, int VY, int NC>
+constexpr int kBpm = HY * VY + (NC == 1 ? 0 : 2);
+
+template <int HY, int VY, int C = 3>
 __global__ void __launch_bounds__(kBlockThreads) k_jpeg_blocks(EncArgs a) {
-  constexpr int NY = HY * VY, BPM = NY + 2;               // luma blocks and blocks per MCU
+  constexpr int NY = HY * VY, BPM = kBpm<HY, VY, C == 1 ? 1 : 3>;   // luma blocks and blocks per MCU
   __shared__ Tables st;
   __shared__ int sblk[kBlockThreads * kBlockPad];
   load_tables(&st, a.tabs);
@@ -688,7 +735,7 @@ __global__ void __launch_bounds__(kBlockThreads) k_jpeg_blocks(EncArgs a) {
     return;
   }
   int* d = sblk + threadIdx.x * kBlockPad;
-  load_block_s<HY, VY>(a.img + i * a.istride, a.pitch, a.g, mx, my, k, d);
+  load_block_s<HY, VY, C>(a.img + i * a.istride, a.pitch, a.g, mx, my, k, d);
   fdct_islow(d);
   quantise(d, st.qdiv[t]);
   const uint8_t* zz = st.zz;
@@ -708,9 +755,9 @@ __device__ inline int resolved_dc(const EncArgs& a, long long mcu_base, int mx, 
   return a.coef[(mcu_base + k) * 64];
 }
 
-template <int HY, int VY>
+template <int HY, int VY, int NC = 3>
 __global__ void k_jpeg_dc(EncArgs a) {
-  constexpr int NY = HY * VY, BPM = NY + 2;
+  constexpr int NY = HY * VY, BPM = kBpm<HY, VY, NC>;
   const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= a.nblk * a.n) return;
   const int i = (int)(b / a.nblk);
@@ -742,9 +789,9 @@ __global__ void k_jpeg_zero(EncArgs a) {
 }
 
 // kOpt: the image's own codes (k_jpeg_huff) instead of the shared Annex K tables; kRst: byte-aligned restart intervals
-template <int HY, int VY, bool kOpt, bool kRst>
+template <int HY, int VY, bool kOpt, bool kRst, int NC = 3>
 __global__ void __launch_bounds__(kBlockThreads) k_jpeg_pack(EncArgs a) {
-  constexpr int NY = HY * VY, BPM = NY + 2;
+  constexpr int NY = HY * VY, BPM = kBpm<HY, VY, NC>;
   __shared__ Tables st;
   if constexpr (!kOpt) load_tables(&st, a.tabs);
   __syncthreads();
@@ -783,7 +830,7 @@ __global__ void __launch_bounds__(kBlockThreads) k_jpeg_pack(EncArgs a) {
 __global__ void k_jpeg_intervals(EncArgs a) {
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= a.n * a.nint) return;
-  const int bpm = a.g.hy * a.g.vy + 2;
+  const int bpm = mcu_blocks(a.g);
   const long long i = t / a.nint, j = t - i * a.nint, mcus = (long long)a.g.mcux * a.g.mcuy;
   const long long mend = (j + 1) * a.rst < mcus ? (j + 1) * a.rst : mcus;
   const long long first = i * a.nblk + j * a.rst * bpm, last = i * a.nblk + mend * bpm - 1;
@@ -792,9 +839,9 @@ __global__ void k_jpeg_intervals(EncArgs a) {
 
 // optimised tables, pass 1: symbol counts per image and table.  Each CTA gathers the first two images its blocks
 // touch in shared memory and adds those counts once; blocks of further images (small images) add theirs directly.
-template <int HY, int VY>
+template <int HY, int VY, int NC = 3>
 __global__ void __launch_bounds__(kBlockThreads) k_jpeg_count(EncArgs a) {
-  constexpr int NY = HY * VY, BPM = NY + 2;
+  constexpr int NY = HY * VY, BPM = kBpm<HY, VY, NC>;
   __shared__ unsigned sc[2][4 * 256];
   for (int e = threadIdx.x; e < 2 * 4 * 256; e += blockDim.x) (&sc[0][0])[e] = 0;
   __syncthreads();
@@ -820,14 +867,15 @@ __global__ void __launch_bounds__(kBlockThreads) k_jpeg_count(EncArgs a) {
 }
 
 // optimised tables, pass 2: one thread per (image, table) runs jpeg_gen_optimal_table and writes the codes; then one
-// thread per image writes its header (the common prefix, its four DHTs, the common DRI / SOS)
+// thread per image writes its header (the common prefix, its four DHTs -- two for grey, NC 1 -- the common DRI / SOS)
 constexpr int kHuffThreads = 128;
+template <int NC = 3>
 __global__ void __launch_bounds__(kHuffThreads) k_jpeg_huff(EncArgs a) {
   __shared__ uint8_t sbits[kHuffThreads][16];
   __shared__ uint8_t svals[kHuffThreads][256];
   const long long t = (long long)blockIdx.x * kHuffThreads + threadIdx.x;
   const int i = (int)(t >> 2), tb = (int)(t & 3);
-  if (i < a.n) {
+  if (i < a.n && (NC == 3 || tb < 2)) {
     long long freq[257];
     for (int k = 0; k < 256; ++k) freq[k] = (long long)a.counts[(size_t)i * 1024 + tb * 256 + k];
     gen_optimal_table(freq, sbits[threadIdx.x], svals[threadIdx.x]);
@@ -838,14 +886,14 @@ __global__ void __launch_bounds__(kHuffThreads) k_jpeg_huff(EncArgs a) {
   __syncthreads();
   if (i < a.n && tb == 0) {
     const int q = threadIdx.x;   // this image's four tables are threads q .. q + 3
-    a.hlen[i] = optimal_header(a.header, a.hlen0, &sbits[q], &svals[q], a.hdrs + (size_t)i * kMaxHeaderBytes);
+    a.hlen[i] = optimal_header(a.header, a.hlen0, &sbits[q], &svals[q], a.hdrs + (size_t)i * kMaxHeaderBytes, NC);
   }
 }
 
 // optimised tables, pass 3: each block's bits under its image's codes
-template <int HY, int VY>
+template <int HY, int VY, int NC = 3>
 __global__ void __launch_bounds__(kBlockThreads) k_jpeg_bits(EncArgs a) {
-  constexpr int NY = HY * VY, BPM = NY + 2;
+  constexpr int NY = HY * VY, BPM = kBpm<HY, VY, NC>;
   const long long b = (long long)blockIdx.x * kBlockThreads + threadIdx.x;
   if (b >= a.nblk * a.n) return;
   const int i = (int)(b / a.nblk);

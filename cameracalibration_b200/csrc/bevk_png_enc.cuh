@@ -22,11 +22,15 @@
 //              Adler-32 of the filtered stream, big-endian
 //   PNG        signature, IHDR (colour type 2, depth 8), the zlib stream in IDAT chunks of 8192 bytes (the last one
 //              shorter), IEND; every chunk with its CRC-32
+// Grey and BGRA images (cv2.imencode of [H][W] / [H][W][1] and [H][W][4]): IHDR colour type 0 / 6, the filters run with
+// bpp 1 / 4 (BGRA swapped to RGBA first, libpng's png_set_bgr), rows of C*W + 1 bytes; everything after the filter
+// stage sees only filtered bytes and is the same.
 // Everything per row, per position and per block is __host__ __device__: tests/host/png_enc.cu runs the same functions
 // serially over whole images and compares the stream with live cv2.imencode.
 //
 // Device pipeline for a group of equal-sized images (bevk_api.cu: png_group):
-//   k_png_filter   one CTA per row: BGR -> RGB, the filter choice, the filtered row, the row's Adler-32 sums
+//   k_png_filter   one CTA per row: BGR -> RGB (BGRA -> RGBA), the filter choice, the filtered row, the row's Adler-32
+//                  sums; instantiated per bytes per pixel C (1, 3, 4)
 //   scan           inclusive max-scan (CUB) of run starts: every position's run start
 //   scan           exclusive sum (CUB) of "a symbol starts here": every symbol's index
 //   k_png_setup    symbols, blocks and block ranges per image
@@ -82,7 +86,7 @@ struct Opts {
 // {NONE, SUB, UP, AVG, PAETH, FAST, ALL} becomes SUB and replaces whatever filters the level implies.  No level: SUB and
 // level 1; a level: every filter (libpng's default).  Returns 0, 1 for a list cv2 does not take (odd length, unknown
 // key) or 2 for one the encoder does not reproduce: level 0 (deflate_stored, whose blocks follow libpng's output
-// buffer), a hash-chain strategy (DEFAULT, FILTERED, FIXED), BILEVEL != 0 (not a 3-channel format) and ZLIBBUFFER_SIZE.
+// buffer), a hash-chain strategy (DEFAULT, FILTERED, FIXED), BILEVEL != 0 (1-bit output) and ZLIBBUFFER_SIZE.
 // With hash_chain, a hash-chain strategy at levels 4..9 (zlib's deflate_slow) is taken too; levels 1..3 under those
 // strategies (deflate_fast, whose chains depend on its parse) stay refused.
 inline int normalise(const int* p, int n, Opts* o, bool hash_chain = false) {
@@ -132,8 +136,11 @@ __host__ __device__ inline int zlib_flevel(const Opts& o) {
 }
 
 // ------------------------------------------------------------------ geometry and bounds
-__host__ __device__ inline long long row_bytes(int W) { return 3ll * W + 1; }
-__host__ __device__ inline long long image_bytes(int W, int H) { return row_bytes(W) * H; }
+// C: bytes per pixel of the image and of the PNG (1 grey, 3 BGR -> RGB, 4 BGRA -> RGBA)
+__host__ __device__ inline long long row_bytes(int W, int C = 3) { return (long long)C * W + 1; }
+__host__ __device__ inline long long image_bytes(int W, int H, int C = 3) { return row_bytes(W, C) * H; }
+// IHDR colour type of C channels: grey 0, truecolour 2, truecolour with alpha 6
+__host__ __device__ inline int colour_type(int C) { return C == 1 ? 0 : C == 4 ? 6 : 2; }
 // Blocks of an image of N filtered bytes: nsym / 16383 + 1 (a full last block is followed by an empty one), nsym <= N.
 __host__ __device__ inline long long max_blocks(long long N) { return N / kBlockSyms + 1; }
 // Every block costs at most its raw bytes + 5: a stored block is 3 bits, a pad to the byte, LEN, NLEN and the bytes,
@@ -141,7 +148,7 @@ __host__ __device__ inline long long max_blocks(long long N) { return N / kBlock
 __host__ __device__ inline long long zlib_bound(long long N) { return 2 + N + 5 * max_blocks(N) + 4; }
 __host__ __device__ inline long long idat_chunks(long long zbytes) { return (zbytes + kIdatBytes - 1) / kIdatBytes; }
 __host__ __device__ inline long long png_bytes(long long zbytes) { return kPngHead + zbytes + 12 * idat_chunks(zbytes) + kPngTail; }
-__host__ __device__ inline long long encode_bound(int W, int H) { return png_bytes(zlib_bound(image_bytes(W, H))); }
+__host__ __device__ inline long long encode_bound(int W, int H, int C = 3) { return png_bytes(zlib_bound(image_bytes(W, H, C))); }
 
 // Filters libpng tries on a W x H image (png_write_start_row).
 __host__ __device__ inline int row_filters(int filters, int W, int H) {
@@ -153,17 +160,25 @@ __host__ __device__ inline int row_filters(int filters, int W, int H) {
 // ------------------------------------------------------------------ filters
 // Byte i of a row in RGB order read from a BGR row.
 __host__ __device__ inline int rgb_at(const uint8_t* row, long long i) { return row[i - 2 * (i % 3) + 2]; }
+// Byte i of a row in PNG order read from a C-channel row: grey as is, BGR -> RGB, BGRA -> RGBA
+template <int C>
+__host__ __device__ inline int png_at(const uint8_t* row, long long i) {
+  if constexpr (C == 1) return row[i];
+  else if constexpr (C == 3) return rgb_at(row, i);
+  else return row[(i & 1) ? i : i ^ 2];
+}
 __host__ __device__ inline int paeth(int a, int b, int c) {
   const int p = b - c, q = a - c;
   const int pa = p < 0 ? -p : p, pb = q < 0 ? -q : q, pc = p + q < 0 ? -(p + q) : p + q;
   return (pa <= pb && pa <= pc) ? a : pb <= pc ? b : c;
 }
-// Filtered byte i (0 .. 3W-1) of filter type t (0 NONE .. 4 PAETH); prev NULL is a row of zeros.
+// Filtered byte i (0 .. C*W-1) of filter type t (0 NONE .. 4 PAETH) with bpp C; prev NULL is a row of zeros.
+template <int C = 3>
 __host__ __device__ inline uint8_t filter_byte(int t, const uint8_t* cur, const uint8_t* prev, long long i) {
-  const int x = rgb_at(cur, i);
-  const int a = i >= 3 ? rgb_at(cur, i - 3) : 0;
-  const int b = prev ? rgb_at(prev, i) : 0;
-  const int c = prev && i >= 3 ? rgb_at(prev, i - 3) : 0;
+  const int x = png_at<C>(cur, i);
+  const int a = i >= C ? png_at<C>(cur, i - C) : 0;
+  const int b = prev ? png_at<C>(prev, i) : 0;
+  const int c = prev && i >= C ? png_at<C>(prev, i - C) : 0;
   int pred = 0;
   switch (t) {
     case 1: pred = a; break;
@@ -722,6 +737,8 @@ struct PngArgs {
   const uint8_t* img;
   long long istride, pitch;
   int W, H, n, filters, strategy;
+  int colour;                    // IHDR colour type
+  long long rb;                  // filtered bytes per row, C * W + 1: the rows libpng hands to zlib
   long long N, maxb, zwords, maxchunks;
   uint8_t* f;                    // [n][N] filtered rows
   Adler* rowad;                  // [n][H] Adler-32 sums per row
@@ -779,6 +796,7 @@ struct MaxOp {
   __device__ unsigned operator()(unsigned x, unsigned y) const { return x > y ? x : y; }
 };
 
+template <int C = 3>
 __global__ void __launch_bounds__(kPngThreads) k_png_filter(PngArgs a) {
   using Reduce = cub::BlockReduce<unsigned long long, kPngThreads>;
   __shared__ typename Reduce::TempStorage tmp;
@@ -786,14 +804,14 @@ __global__ void __launch_bounds__(kPngThreads) k_png_filter(PngArgs a) {
   const int r = blockIdx.x, i = r / a.H, y = r % a.H;
   const uint8_t* cur = a.img + i * a.istride + y * a.pitch;
   const uint8_t* prev = y ? cur - a.pitch : nullptr;
-  const long long pitch = 3ll * a.W, rb = pitch + 1;
+  const long long pitch = (long long)C * a.W, rb = pitch + 1;
   const int filters = row_filters(a.filters, a.W, a.H);
   if (filters & (filters - 1)) {
     unsigned long long sum[5];
     for (int t = 0; t < 5; ++t) {
       unsigned long long v = 0;
       if (filters & (kFilterNone << t))
-        for (long long k = threadIdx.x; k < pitch; k += kPngThreads) v += filter_cost(filter_byte(t, cur, prev, k));
+        for (long long k = threadIdx.x; k < pitch; k += kPngThreads) v += filter_cost(filter_byte<C>(t, cur, prev, k));
       sum[t] = Reduce(tmp).Sum(v);
       __syncthreads();
     }
@@ -807,7 +825,7 @@ __global__ void __launch_bounds__(kPngThreads) k_png_filter(PngArgs a) {
   uint8_t* dst = a.f + i * a.N + y * rb;
   unsigned long long s1 = 0, s2 = 0;
   for (long long k = threadIdx.x; k < rb; k += kPngThreads) {
-    const uint8_t v = k ? filter_byte(t, cur, prev, k - 1) : (uint8_t)t;
+    const uint8_t v = k ? filter_byte<C>(t, cur, prev, k - 1) : (uint8_t)t;
     dst[k] = v;
     s1 += v;
     s2 += (unsigned long long)(rb - k) * v;
@@ -856,7 +874,7 @@ __global__ void k_png_prev(const unsigned* key, const unsigned* pos, unsigned* p
 }
 __global__ void k_png_match(PngArgs a) {
   const unsigned total = (unsigned)(a.n * a.N);
-  const long long rb = row_bytes(a.W);
+  const long long rb = a.rb;
   for (unsigned p = blockIdx.x * blockDim.x + threadIdx.x; p < total; p += gridDim.x * blockDim.x) {
     const unsigned i = (unsigned)(p / a.N), base = (unsigned)(i * a.N);
     a.recs[p] = lazy_match(a.f + base, a.N, a.prev + base, p - base, a.level, a.strategy, rb);
@@ -869,7 +887,7 @@ struct RecAt {
 __device__ inline Chain group_chain(const PngArgs& a, unsigned p, unsigned* base) {
   const unsigned i = (unsigned)(p / a.N);
   *base = (unsigned)(i * a.N);
-  return lazy_chain(p - *base, a.N, a.level, row_bytes(a.W), RecAt{a.recs + *base});
+  return lazy_chain(p - *base, a.N, a.level, a.rb, RecAt{a.recs + *base});
 }
 // Every position's chain as if it were canonical: the next canonical position; image starts are on the parse.
 __global__ void k_png_next(PngArgs a) {
@@ -1112,7 +1130,7 @@ __global__ void __launch_bounds__(kPngThreads) k_png_frame(PngArgs a) {
                        (uint8_t)(a.W >> 24), (uint8_t)(a.W >> 16), (uint8_t)(a.W >> 8), (uint8_t)a.W,
                        (uint8_t)(a.H >> 24), (uint8_t)(a.H >> 16), (uint8_t)(a.H >> 8), (uint8_t)a.H, 8};
       for (int k = 0; k < 17; ++k) o[8 + k] = h[k];
-      const uint8_t rest[4] = {2, 0, 0, 0};
+      const uint8_t rest[4] = {(uint8_t)a.colour, 0, 0, 0};
       for (int k = 0; k < 4; ++k) o[25 + k] = rest[k];
       const uint32_t hc = crc32(o + 12, 17);
       for (int k = 0; k < 4; ++k) o[29 + k] = (uint8_t)(hc >> (24 - 8 * k));

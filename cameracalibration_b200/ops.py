@@ -185,29 +185,35 @@ def _split(out, sizes):
     return res
 
 
-def _encode(what, images, ctx, bound, call):
+def _encode(what, images, ctx, bound, call, channels=False):
     """The body of the encoding wrappers over uint8[H][W][3] or [N][H][W][3] BGR images: CUDA arrays
     (``__cuda_array_interface__``) are read in place, NumPy input is uploaded once.  bound(w, h): the largest stream of one
     image; call((ptr, image stride, row stride, n, w, h), out, capacity, sizes): the C call, run on torch's current
-    stream."""
+    stream.  channels: take [H][W] and [H][W][C] / [N][H][W][C] with C in 1, 3, 4 instead, with bound(w, h, C) and
+    call((ptr, image stride, row stride, C, n, w, h), ...)."""
     from .sharding import _torch_current_stream
     keep = images
     if not hasattr(images, "__cuda_array_interface__"):
         a = np.asarray(images)
-        if a.dtype != np.uint8 or a.ndim not in (3, 4) or a.shape[-1] != 3:
+        if channels:
+            if a.dtype != np.uint8 or a.ndim not in (2, 3, 4) or (a.ndim > 2 and a.shape[-1] not in (1, 3, 4)):
+                raise L.BevkError(f"{what} takes uint8[H][W], [H][W][C] or [N][H][W][C] images with C in 1, 3, 4, "
+                                  f"got {a.dtype} {a.shape}")
+        elif a.dtype != np.uint8 or a.ndim not in (3, 4) or a.shape[-1] != 3:
             raise L.BevkError(f"{what} takes uint8[H][W][3] or uint8[N][H][W][3] BGR images, got {a.dtype} {a.shape}")
         import torch
         keep = torch.from_numpy(np.ascontiguousarray(a)).to(torch.device("cuda", ctx.device))
     ptr, rank, n, h, w, ch, img_stride, row_stride = _cuda_images(keep, what)
-    if ch != 3 or rank == 2:
+    if not channels and (ch != 3 or rank == 2):
         raise L.BevkError(f"{what} takes uint8[H][W][3] or uint8[N][H][W][3] BGR images")
     if n < 1:
         return []
-    cap = n * bound(w, h)
+    cap = n * (bound(w, h, ch) if channels else bound(w, h))
     out = np.empty(cap, np.uint8)          # pages are only touched where streams land
     sizes = (C.c_uint64 * n)()
+    img = (C.c_void_p(ptr), img_stride, row_stride) + ((ch,) if channels else ()) + (n, w, h)
     with ctx.on_stream(_torch_current_stream(ctx.device)):
-        L.check(call((C.c_void_p(ptr), img_stride, row_stride, n, w, h), L.vptr(out), cap, sizes))
+        L.check(call(img, L.vptr(out), cap, sizes))
     return _split(out, sizes)
 
 
@@ -273,6 +279,63 @@ def png_encode(images, ctx: L.Context | None = None, params=None) -> list[bytes]
     arr, k = _jpeg_params(params)
     return _encode("png_encode", images, ctx, png_encode_bound,   # the bound holds under every list
                    lambda img, out, cap, sizes: ctx.lib.bevk_png_encode_params(ctx.h, arr, k, *img, out, cap, sizes))
+
+
+JPEG_EXTS = (".jpg", ".jpeg", ".jpe")
+
+
+def imencode_bound(ext: str, width: int, height: int, channels: int = 3, params=None) -> int:
+    """Largest stream imencode can produce for one width x height image of `channels` channels under params."""
+    ext = str(ext).lower()
+    n = C.c_uint64()
+    if ext in JPEG_EXTS:
+        _, arr, k = _imencode_jpeg_params(params)
+        L.check(L.load().bevk_jpeg_encode_channels_bound(int(width), int(height), int(channels), arr, k, C.byref(n)))
+    elif ext == ".png":
+        L.check(L.load().bevk_png_encode_channels_bound(int(width), int(height), int(channels), C.byref(n)))
+    else:
+        raise L.BevkError(f"imencode: extension {ext!r} is not one the device encoders write (.jpg, .jpeg, .jpe, .png)")
+    return n.value
+
+
+def _imencode_jpeg_params(params):
+    """(quality, ctypes array, n) of a whole cv2 JPEG list: IMWRITE_JPEG_QUALITY pairs become the quality (the last one
+    wins, as in cv2; 95 without one), the other pairs stay in order."""
+    p = [] if params is None else [int(v) for v in params]
+    if len(p) % 2:
+        raise L.BevkError(f"imencode: params must be (key, value) pairs, got {len(p)} ints")
+    quality, rest = 95, []
+    for key, value in zip(p[::2], p[1::2]):
+        if key == 1:   # cv2.IMWRITE_JPEG_QUALITY
+            quality = value
+        else:
+            rest += [key, value]
+    arr, k = _jpeg_params(rest)
+    return quality, arr, k
+
+
+def imencode(ext: str, images, params=None, ctx: L.Context | None = None) -> list[bytes]:
+    """cv2.imencode(ext, img, params) on the GPU, byte for byte, for grey, BGR and BGRA images: one stream per image.
+    ext: ".jpg", ".jpeg", ".jpe" or ".png" (others raise BevkError).  images: uint8[H][W], [H][W][C] or [N][H][W][C] with
+    C in 1 (grey), 3 (BGR), 4 (BGRA; JPEG drops alpha as cv2 does, PNG stores RGBA); a grey batch is [N][H][W][1].
+    CUDA arrays (``__cuda_array_interface__``, e.g. the output of Undistorter.cuda) are read in place on torch's current
+    stream; NumPy input is uploaded once.  params: cv2's whole list for the format, read as cv2 4.13 reads it --
+    IMWRITE_JPEG_QUALITY (default 95) with the other IMWRITE_JPEG_* keys, PROGRESSIVE included, or the IMWRITE_PNG_*
+    keys with png_encode's refusals (level 0, levels 1..3 under the hash-chain strategies, BILEVEL, ZLIBBUFFER_SIZE)."""
+    ctx = ctx or L.default_context()
+    ext = str(ext).lower()
+    if ext in JPEG_EXTS:
+        quality, arr, k = _imencode_jpeg_params(params)
+        return _encode("imencode", images, ctx, lambda w, h, ch: imencode_bound(ext, w, h, ch, params),
+                       lambda img, out, cap, sizes: ctx.lib.bevk_jpeg_encode_channels(ctx.h, arr, k, *img, int(quality),
+                                                                                      out, cap, sizes),
+                       channels=True)
+    if ext == ".png":
+        arr, k = _jpeg_params(params)
+        return _encode("imencode", images, ctx, lambda w, h, ch: imencode_bound(ext, w, h, ch),
+                       lambda img, out, cap, sizes: ctx.lib.bevk_png_encode_channels(ctx.h, arr, k, *img, out, cap, sizes),
+                       channels=True)
+    raise L.BevkError(f"imencode: extension {ext!r} is not one the device encoders write (.jpg, .jpeg, .jpe, .png)")
 
 
 def remap(src: np.ndarray, map1: np.ndarray, map2: np.ndarray | None, interpolation: int = INTER_LINEAR,

@@ -487,6 +487,29 @@ int bevk_png_encode_params(bevk_ctx *ctx, const int *params, int n_params, const
                            int64_t row_stride, int n, int width, int height, uint8_t *out, uint64_t capacity,
                            uint64_t *sizes);
 
+/* ---- grey, BGR and BGRA images to JPEG and PNG -------------------------------------------------------------------
+ * bevk_jpeg_encode_params and bevk_png_encode_params for images of `channels` channels: 1 (grey), 3 (BGR) or 4 (BGRA);
+ * any other count is BEVK_ERR_UNSUPPORTED.  Pixels are `channels` bytes apart, rows row_stride bytes apart (any pitch >=
+ * channels * width), images image_stride apart.  The streams are byte-identical to cv2.imencode of the same array:
+ *   grey JPEG    a one-component JFIF stream (DQT 0 at the luma quality, SOF with one 1x1 component, DHT DC0 / AC0,
+ *                SOS with one component; SAMPLING_FACTOR and CHROMA_QUALITY do not reach it); PROGRESSIVE writes
+ *                libjpeg's six-scan script for one component
+ *   BGRA JPEG    alpha is dropped: the stream of the BGR image
+ *   grey PNG     colour type 0, filters with one byte per pixel
+ *   BGRA PNG     colour type 6, bytes stored RGBA, filters with four bytes per pixel
+ * The same parameter lists, refusals and contract as the 3-channel calls (the call synchronises, sizes[] always filled,
+ * nothing written past capacity, not capturable, bevk_last_kernel_ms covers it); with channels = 3 they are those calls.
+ * The _bound calls give the largest stream of a width x height image of `channels` channels (JPEG: under `params`; PNG:
+ * under any list; its filtered size (channels * width + 1) * height must stay below 2^31 - 2^16).                     */
+int bevk_jpeg_encode_channels(bevk_ctx *ctx, const int *params, int n_params, const void *d_images, int64_t image_stride,
+                              int64_t row_stride, int channels, int n, int width, int height, int quality, uint8_t *out,
+                              uint64_t capacity, uint64_t *sizes);
+int bevk_png_encode_channels(bevk_ctx *ctx, const int *params, int n_params, const void *d_images, int64_t image_stride,
+                             int64_t row_stride, int channels, int n, int width, int height, uint8_t *out, uint64_t capacity,
+                             uint64_t *sizes);
+int bevk_jpeg_encode_channels_bound(int width, int height, int channels, const int *params, int n, uint64_t *bytes);
+int bevk_png_encode_channels_bound(int width, int height, int channels, uint64_t *bytes);
+
 /* ---- CUDA graphs over the device-pointer entry points ------------------------------------------------
  * Everything the "_device" / "_stack" / "_frames" entry points enqueue on the ctx stream between begin and end is
  * captured (stream capture) instead of executed, instantiated once, and replayed `times` times by one call --
