@@ -406,6 +406,24 @@ int bevk_host_free(void* p) {
 }
 
 // ------------------------------------------------------------------ K1
+// k_undistort_map of cm into the pair (m1, m2): cm.w x cm.h entries
+static int build_map(bevk_ctx* c, const CamModel& cm, DevBuf& m1, DevBuf& m2) {
+  const size_t n = (size_t)cm.w * cm.h;
+  RET(m1.ensure(n * 4));
+  RET(m2.ensure(n * 2));
+  k_undistort_map<<<grid2d(cm.w, cm.h), 256, 0, c->stream>>>(cm, m1.as<short2>(), m2.as<unsigned short>());
+  LAUNCHED(c);
+  return BEVK_OK;
+}
+
+// n entries of the device map pair (m1, m2) to the caller's host maps, then wait for them
+static int download_maps(bevk_ctx* c, const void* m1, const void* m2, size_t n, int16_t* map1, uint16_t* map2) {
+  CU(cudaMemcpyAsync(map1, m1, n * 4, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaMemcpyAsync(map2, m2, n * 2, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  return BEVK_OK;
+}
+
 int bevk_undistort_map(bevk_ctx* c, int model, const double K[9], const double* D, int n_dist, const double P[9], int w,
                        int h, int16_t* map1, uint16_t* map2) {
   RET(use(c));
@@ -413,18 +431,15 @@ int bevk_undistort_map(bevk_ctx* c, int model, const double K[9], const double* 
   CamModel cm;
   RET(make_model(model, K, D, n_dist, P, w, h, &cm));
   RET(attach_xs_table(c, c->s_xs, &cm));
-  const size_t n = (size_t)w * h;
-  RET(c->s_m1.ensure(n * 4));
-  RET(c->s_m2.ensure(n * 2));
-  k_undistort_map<<<grid2d(w, h), 256, 0, c->stream>>>(cm, c->s_m1.as<short2>(), c->s_m2.as<unsigned short>());
-  LAUNCHED(c);
-  CU(cudaMemcpyAsync(map1, c->s_m1.p, n * 4, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaMemcpyAsync(map2, c->s_m2.p, n * 2, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return BEVK_OK;
+  RET(build_map(c, cm, c->s_m1, c->s_m2));
+  return download_maps(c, c->s_m1.p, c->s_m2.p, (size_t)w * h, map1, map2);
 }
 
-// ------------------------------------------------------------------ gather dispatch
+// ------------------------------------------------------------------ image operations
+// remap, undistort, warpPerspective, warpAffine and resize are each an ImageOp (what the operation adds to the frames,
+// checked by its builder, which enqueues nothing) run over an ImageBatch (the frames it reads and writes) by launch().
+// The host forms run it over dense scratch (host_image), the device forms over the caller's frames (device_image).
+
 // k_gather4's word path: 32-bit tap loads need every source row to start on a 4-byte boundary (base, row pitch and, over
 // a batch, image stride), and its 32-bit stores the same of the destination (padded rows are fine).  Anything else,
 // e.g. caller memory at an odd address, takes k_gather's byte path.
@@ -444,46 +459,183 @@ static int gather_interp(int* interp) {
   return BEVK_OK;
 }
 
-// Enqueue the gather of a.n >= 1 frames.  grid.z = frame groups of GATHER_NB, at most 65535 per launch; a single frame
-// takes k_gather4's single-frame form (NB = 1), which keeps the register count and speed of the one-frame kernel.
+// n >= 1 frames: source and destination images, rows `pitch` bytes apart and images `istride` bytes apart (0 when n = 1)
+struct ImageBatch {
+  const uint8_t* src; int sw, sh; long long spitch, sistride;
+  uint8_t* dst; int dw, dh; long long dpitch, distride;
+  int n;
+};
+
+constexpr int OP_RESIZE = 4;   // ImageOp::mode after the gathers' MODE 0..3
+
+struct ImageOp {
+  int mode = 0;                     // the gathers' MODE (0 maps, 1 camera model, 2 homography, 3 affine) or OP_RESIZE
+  int interp = 0;                   // a gather's interpolation after gather_interp; a resize's body (resize_kind)
+  GatherArgs g{};                   // a gather's maps, camera model or inverse matrix
+  ResizeArgs r{};                   // a resize's scales
+  int slot = -1, dw = 0, dh = 0;    // an undistorter slot and the size of the images it writes
+  const int16_t* hmap1 = nullptr;   // bevk_remap: the caller's host maps, uploaded once every check has passed
+  const uint16_t* hmap2 = nullptr;
+};
+
+// a (GatherArgs or ResizeArgs) with its frame fields taken from b
+template <class Args>
+static Args with_frames(Args a, const ImageBatch& b) {
+  a.src = b.src; a.sw = b.sw; a.sh = b.sh; a.spitch = b.spitch; a.sistride = b.sistride;
+  a.dst = b.dst; a.dw = b.dw; a.dh = b.dh; a.dpitch = b.dpitch; a.distride = b.distride;
+  a.n = b.n;
+  return a;
+}
+
 template <int MODE>
-static int launch_gather(bevk_ctx* c, const GatherArgs& a0, int channels, int interp) {
-  const bool words = gather4_ok(a0, channels, interp, MODE);
-  const int per_launch = 65535 * GATHER_NB;
-  for (int f0 = 0; f0 < a0.n; f0 += per_launch) {
-    GatherArgs a = a0;
-    a.n = std::min(per_launch, a0.n - f0);
-    a.src += (long long)f0 * a0.sistride;
-    a.dst += (long long)f0 * a0.distride;
-    const unsigned gz = (unsigned)((a.n + GATHER_NB - 1) / GATHER_NB);
-    if (words) {
-      // 4 output pixels per thread, 32-bit tap loads and 12-byte stores
-      const dim3 g4((a.dw / 4 + 31) / 32, (a.dh + 7) / 8, gz);
-      if (a.n == 1) k_gather4<MODE, 1><<<g4, 256, 0, c->stream>>>(a);
-      else k_gather4<MODE, GATHER_NB><<<g4, 256, 0, c->stream>>>(a);
-      LAUNCHED(c);
-      continue;
-    }
-    const dim3 g((a.dw + 31) / 32, (a.dh + 7) / 8, gz);
+static void gather(bevk_ctx* c, const GatherArgs& a, int channels, int interp, bool words, unsigned gz) {
+  if (words) {
+    // 4 output pixels per thread, 32-bit tap loads and 12-byte stores
+    const dim3 g4((a.dw / 4 + 31) / 32, (a.dh + 7) / 8, gz);
+    if (a.n == 1) k_gather4<MODE, 1><<<g4, 256, 0, c->stream>>>(a);
+    else k_gather4<MODE, GATHER_NB><<<g4, 256, 0, c->stream>>>(a);
+    return;
+  }
+  const dim3 g((a.dw + 31) / 32, (a.dh + 7) / 8, gz);
 #define GO(C, L) k_gather<MODE, C, L><<<g, 256, 0, c->stream>>>(a)
 #define TAPS(C, KS) k_gather_taps<MODE, C, KS><<<g, 256, 0, c->stream>>>(a, wt)
-    if (interp == BEVK_INTER_CUBIC || interp == BEVK_INTER_LANCZOS4) {
-      const short* wt = c->d_wtab.as<short>() + (interp == BEVK_INTER_CUBIC ? 0 : INTERP_TAB_LANCZOS4);
-      if (interp == BEVK_INTER_CUBIC) {
-        if (channels == 1) TAPS(1, 4); else if (channels == 3) TAPS(3, 4); else TAPS(4, 4);
-      } else {
-        if (channels == 1) TAPS(1, 8); else if (channels == 3) TAPS(3, 8); else TAPS(4, 8);
-      }
-    } else if (interp == BEVK_INTER_LINEAR) {
-      if (channels == 1) GO(1, 1); else if (channels == 3) GO(3, 1); else GO(4, 1);
+  if (interp == BEVK_INTER_CUBIC || interp == BEVK_INTER_LANCZOS4) {
+    const short* wt = c->d_wtab.as<short>() + (interp == BEVK_INTER_CUBIC ? 0 : INTERP_TAB_LANCZOS4);
+    if (interp == BEVK_INTER_CUBIC) {
+      if (channels == 1) TAPS(1, 4); else if (channels == 3) TAPS(3, 4); else TAPS(4, 4);
     } else {
-      if (channels == 1) GO(1, 0); else if (channels == 3) GO(3, 0); else GO(4, 0);
+      if (channels == 1) TAPS(1, 8); else if (channels == 3) TAPS(3, 8); else TAPS(4, 8);
     }
+  } else if (interp == BEVK_INTER_LINEAR) {
+    if (channels == 1) GO(1, 1); else if (channels == 3) GO(3, 1); else GO(4, 1);
+  } else {
+    if (channels == 1) GO(1, 0); else if (channels == 3) GO(3, 0); else GO(4, 0);
+  }
 #undef GO
 #undef TAPS
+}
+
+template <int C, int KIND>
+static void resize_c(bevk_ctx* c, const ResizeArgs& a, dim3 g) {
+  if (a.n > 1) k_resize<C, KIND, GATHER_NB><<<g, 256, 0, c->stream>>>(a);
+  else k_resize<C, KIND, 1><<<g, 256, 0, c->stream>>>(a);
+}
+template <int C>
+static void resize_k(bevk_ctx* c, const ResizeArgs& a, int kind, dim3 g) {
+  switch (kind) {
+    case RZ_NEAREST: resize_c<C, RZ_NEAREST>(c, a, g); break;
+    case RZ_LINEAR: resize_c<C, RZ_LINEAR>(c, a, g); break;
+    case RZ_AREA_LINEAR: resize_c<C, RZ_AREA_LINEAR>(c, a, g); break;
+    case RZ_AREA_FAST: resize_c<C, RZ_AREA_FAST>(c, a, g); break;
+    default: resize_c<C, RZ_AREA>(c, a, g);
+  }
+}
+
+// Enqueue op over b.n >= 1 frames.  grid.z = frame groups of GATHER_NB, at most 65535 per launch; a single frame takes
+// the kernels' single-frame form (NB = 1), which keeps the register count and speed of the one-frame kernel.
+static int launch(bevk_ctx* c, const ImageOp& op, const ImageBatch& b, int channels) {
+  const bool words = op.mode != OP_RESIZE && gather4_ok(with_frames(op.g, b), channels, op.interp, op.mode);
+  const int per_launch = 65535 * GATHER_NB;
+  for (int f0 = 0; f0 < b.n; f0 += per_launch) {
+    ImageBatch p = b;
+    p.n = std::min(per_launch, b.n - f0);
+    p.src += (long long)f0 * b.sistride;
+    p.dst += (long long)f0 * b.distride;
+    const unsigned gz = (unsigned)((p.n + GATHER_NB - 1) / GATHER_NB);
+    if (op.mode != OP_RESIZE) {
+      const GatherArgs a = with_frames(op.g, p);
+      switch (op.mode) {
+        case 0: gather<0>(c, a, channels, op.interp, words, gz); break;
+        case 1: gather<1>(c, a, channels, op.interp, words, gz); break;
+        case 2: gather<2>(c, a, channels, op.interp, words, gz); break;
+        default: gather<3>(c, a, channels, op.interp, words, gz);
+      }
+    } else {
+      const ResizeArgs a = with_frames(op.r, p);
+      const dim3 g((a.dw + 31) / 32, (a.dh + 7) / 8, gz);
+      if (channels == 1) resize_k<1>(c, a, op.interp, g);
+      else if (channels == 3) resize_k<3>(c, a, op.interp, g);
+      else resize_k<4>(c, a, op.interp, g);
+    }
     LAUNCHED(c);
   }
-  c->gather_path = words ? 4 : (interp == BEVK_INTER_CUBIC || interp == BEVK_INTER_LANCZOS4) ? 2 : 1;
+  const bool taps = op.interp == BEVK_INTER_CUBIC || op.interp == BEVK_INTER_LANCZOS4;
+  c->gather_path = op.mode == OP_RESIZE ? 3 : words ? 4 : taps ? 2 : 1;
+  return BEVK_OK;
+}
+
+// ---- the operations' builders: each makes the refusals of its operation's own arguments and fills a default op
+static int remap_op(const int16_t* map1, const uint16_t* map2, int interp, ImageOp* op) {
+  if (!map1) return fail(BEVK_ERR_ARG, "null map1");
+  RET(gather_interp(&interp));
+  if (interp != BEVK_INTER_NEAREST && !map2) return fail(BEVK_ERR_ARG, "interpolation %d needs map2", interp);
+  op->interp = interp;
+  op->hmap1 = map1; op->hmap2 = map2;
+  return BEVK_OK;
+}
+
+static int need_undistorter(bevk_ctx* c, int slot) {
+  if (slot < 0 || slot >= 8 || !c->und[slot].valid) return fail(BEVK_ERR_ARG, "undistorter slot %d not set", slot);
+  return BEVK_OK;
+}
+
+// a slot's resident map (MODE 0) or, fused, its camera model (MODE 1); the images it writes are the map's size
+static int undistort_op(bevk_ctx* c, int slot, int interp, ImageOp* op) {
+  RET(need_undistorter(c, slot));
+  RET(gather_interp(&interp));
+  const Undistorter& u = c->und[slot];
+  op->mode = u.fused ? 1 : 0;
+  op->interp = interp;
+  if (u.fused) op->g.cm = u.cm;
+  else { op->g.map1 = u.map1.as<short2>(); op->g.map2 = u.map2.as<unsigned short>(); }
+  op->slot = slot; op->dw = u.cm.w; op->dh = u.cm.h;
+  return BEVK_OK;
+}
+
+static int perspective_op(const double* H, int interp, ImageOp* op) {
+  RET(gather_interp(&interp));
+  op->mode = 2;
+  op->interp = interp;
+  return make_homog(H, &op->g.hm);
+}
+
+// flags -> interpolation (gather_interp's) and the inverse map in hm.M[0..5]
+static int affine_op(const double* M, int flags, ImageOp* op) {
+  if (!M) return fail(BEVK_ERR_ARG, "null M");
+  if (flags & ~(7 | BEVK_WARP_INVERSE_MAP)) return fail(BEVK_ERR_UNSUPPORTED, "warpAffine flags %d", flags);
+  int interp = flags & 7;
+  RET(gather_interp(&interp));
+  op->mode = 3;
+  op->interp = interp;
+  if (flags & BEVK_WARP_INVERSE_MAP) memcpy(op->g.hm.M, M, 6 * sizeof(double));
+  else inv_affine(M, op->g.hm.M);
+  return BEVK_OK;
+}
+
+// interp and cv2's size rule (resize_geometry): the scales and the body
+static int resize_op(int sw, int sh, int dw, int dh, double fx, double fy, int interp, ImageOp* op) {
+  if (interp != BEVK_INTER_NEAREST && interp != BEVK_INTER_LINEAR && interp != BEVK_INTER_AREA)
+    return fail(BEVK_ERR_UNSUPPORTED, "resize interp %d: INTER_NEAREST, INTER_LINEAR and INTER_AREA only", interp);
+  if (sw <= 0 || sh <= 0 || dw <= 0 || dh <= 0) return fail(BEVK_ERR_ARG, "bad size %dx%d -> %dx%d", sw, sh, dw, dh);
+  op->mode = OP_RESIZE;
+  ResizeArgs& a = op->r;
+  if (fx == 0. && fy == 0.) {
+    a.inv_x = (double)dw / sw; a.inv_y = (double)dh / sh;
+  } else {
+    int w = 0, h = 0;
+    a.inv_x = fx; a.inv_y = fy;
+    if (!resize_geometry(sw, sh, &w, &h, &a.inv_x, &a.inv_y))
+      return fail(BEVK_ERR_ARG, "fx %g, fy %g give no image from %dx%d", fx, fy, sw, sh);
+    if (w != dw || h != dh) return fail(BEVK_ERR_ARG, "fx %g, fy %g make %dx%d images, the caller expects %dx%d", fx, fy, w, h, dw, dh);
+  }
+  op->interp = resize_kind(interp, a);
+  return BEVK_OK;
+}
+
+// ---- the two paths: the source is checked, then the destination (an undistorter slot's size first)
+static int check_op_size(const ImageOp& op, int dw, int dh) {
+  if (op.slot >= 0 && (dw != op.dw || dh != op.dh))   // the caller sized dst for another map: never write past it
+    return fail(BEVK_ERR_ARG, "undistorter slot %d holds a %dx%d map, the caller expects %dx%d", op.slot, op.dw, op.dh, dw, dh);
   return BEVK_OK;
 }
 
@@ -510,117 +662,35 @@ static int download_image(bevk_ctx* c, const DevBuf& buf, uint8_t* dst, int w, i
   return BEVK_OK;
 }
 
-int bevk_remap(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, const int16_t* map1,
-               const uint16_t* map2, int dw, int dh, uint8_t* dst, int64_t dstride, int interp) {
-  RET(use(c));
-  RET(check_image(src, sw, sh, sstride, channels, "src"));
-  RET(check_image(dst, dw, dh, dstride, channels, "dst"));
-  if (!map1) return fail(BEVK_ERR_ARG, "null map1");
-  RET(gather_interp(&interp));
-  if (interp != BEVK_INTER_NEAREST && !map2) return fail(BEVK_ERR_ARG, "interpolation %d needs map2", interp);
-  const size_t n = (size_t)dw * dh;
-  RET(upload_image(c, c->s_src, src, sw, sh, sstride, channels));
-  RET(c->s_m1.ensure(n * 4));
-  RET(c->s_m2.ensure(n * 2));
-  RET(c->s_dst.ensure(n * channels));
-  CU(cudaMemcpyAsync(c->s_m1.p, map1, n * 4, cudaMemcpyHostToDevice, c->stream));
-  if (map2) CU(cudaMemcpyAsync(c->s_m2.p, map2, n * 2, cudaMemcpyHostToDevice, c->stream));
-  GatherArgs a{};
-  a.n = 1;
-  a.src = c->s_src.as<uint8_t>(); a.sw = sw; a.sh = sh; a.spitch = (long long)sw * channels;
-  a.dst = c->s_dst.as<uint8_t>(); a.dw = dw; a.dh = dh; a.dpitch = (long long)dw * channels;
-  a.map1 = c->s_m1.as<short2>(); a.map2 = map2 ? c->s_m2.as<unsigned short>() : nullptr;
-  RET(launch_gather<0>(c, a, channels, interp));
-  return download_image(c, c->s_dst, dst, dw, dh, dstride, channels);
-}
-
-// ------------------------------------------------------------------ cached-map undistortion
-int bevk_undistorter_set(bevk_ctx* c, int slot, int model, const double K[9], const double* D, int n_dist,
-                         const double P[9], int dw, int dh, int fused) {
-  RET(use(c));
-  if (slot < 0 || slot >= 8) return fail(BEVK_ERR_ARG, "slot %d out of range", slot);
-  Undistorter& u = c->und[slot];
-  u.valid = false;
-  RET(make_model(model, K, D, n_dist, P, dw, dh, &u.cm));
-  u.fused = fused != 0;
-  if (u.fused) {   // the gathers evaluate the model per pixel: the slot keeps its column table
-    RET(attach_xs_table(c, u.xs, &u.cm));
-  } else {         // the table is read once, by the map build, from scratch
-    u.xs.release();
-    RET(attach_xs_table(c, c->s_xs, &u.cm));
-    const size_t n = (size_t)dw * dh;
-    RET(u.map1.ensure(n * 4));
-    RET(u.map2.ensure(n * 2));
-    k_undistort_map<<<grid2d(dw, dh), 256, 0, c->stream>>>(u.cm, u.map1.as<short2>(), u.map2.as<unsigned short>());
-    LAUNCHED(c);
-    u.cm.xs = nullptr;
-  }
-  u.valid = true;
-  return BEVK_OK;
-}
-
-static int need_undistorter(bevk_ctx* c, int slot) {
-  if (slot < 0 || slot >= 8 || !c->und[slot].valid) return fail(BEVK_ERR_ARG, "undistorter slot %d not set", slot);
-  return BEVK_OK;
-}
-
-int bevk_undistorter_maps(bevk_ctx* c, int slot, int16_t* map1, uint16_t* map2) {
-  RET(use(c));
-  RET(need_undistorter(c, slot));
-  if (!map1 || !map2) return fail(BEVK_ERR_ARG, "null output map");
-  Undistorter& u = c->und[slot];
-  const size_t n = (size_t)u.cm.w * u.cm.h;
-  const short2* m1 = u.map1.as<short2>();
-  const unsigned short* m2 = u.map2.as<unsigned short>();
-  if (u.fused) {   // no resident map: evaluate into scratch
-    RET(c->s_m1.ensure(n * 4));
-    RET(c->s_m2.ensure(n * 2));
-    k_undistort_map<<<grid2d(u.cm.w, u.cm.h), 256, 0, c->stream>>>(u.cm, c->s_m1.as<short2>(), c->s_m2.as<unsigned short>());
-    LAUNCHED(c);
-    m1 = c->s_m1.as<short2>(); m2 = c->s_m2.as<unsigned short>();
-  }
-  CU(cudaMemcpyAsync(map1, m1, n * 4, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaMemcpyAsync(map2, m2, n * 2, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return BEVK_OK;
-}
-
-// Upload a host frame and gather the slot's undistorted image into c->s_dst (dense, row pitch dw * channels).
-static int undistort_to_scratch(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
-                                int interp) {
-  Undistorter& u = c->und[slot];
-  const int dw = u.cm.w, dh = u.cm.h;
-  RET(check_image(src, sw, sh, sstride, channels, "src"));
-  RET(gather_interp(&interp));
+// Host path, without the read-back: a checked host frame uploaded to c->s_src and op run into c->s_dst.  Both are dense
+// (row pitch w * channels), so k_gather4's word-path choice sees the same pitches whatever the caller's strides.
+static int host_launch(bevk_ctx* c, ImageOp op, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, int dw,
+                       int dh) {
   RET(upload_image(c, c->s_src, src, sw, sh, sstride, channels));
   RET(c->s_dst.ensure((size_t)dw * dh * channels));
-  GatherArgs a{};
-  a.n = 1;
-  a.src = c->s_src.as<uint8_t>(); a.sw = sw; a.sh = sh; a.spitch = (long long)sw * channels;
-  a.dst = c->s_dst.as<uint8_t>(); a.dw = dw; a.dh = dh; a.dpitch = (long long)dw * channels;
-  if (u.fused) {
-    a.cm = u.cm;
-    RET(launch_gather<1>(c, a, channels, interp));
-  } else {
-    a.map1 = u.map1.as<short2>(); a.map2 = u.map2.as<unsigned short>();
-    RET(launch_gather<0>(c, a, channels, interp));
+  if (op.hmap1) {
+    const size_t n = (size_t)dw * dh;
+    RET(c->s_m1.ensure(n * 4));
+    RET(c->s_m2.ensure(n * 2));
+    CU(cudaMemcpyAsync(c->s_m1.p, op.hmap1, n * 4, cudaMemcpyHostToDevice, c->stream));
+    if (op.hmap2) CU(cudaMemcpyAsync(c->s_m2.p, op.hmap2, n * 2, cudaMemcpyHostToDevice, c->stream));
+    op.g.map1 = c->s_m1.as<short2>(); op.g.map2 = op.hmap2 ? c->s_m2.as<unsigned short>() : nullptr;
   }
-  return BEVK_OK;
+  const ImageBatch b{c->s_src.as<uint8_t>(), sw, sh, (long long)sw * channels, 0,
+                     c->s_dst.as<uint8_t>(), dw, dh, (long long)dw * channels, 0, 1};
+  return launch(c, op, b, channels);
 }
 
-int bevk_undistort(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
-                   uint8_t* dst, int dw, int dh, int64_t dstride, int interp) {
-  RET(use(c));
-  RET(need_undistorter(c, slot));
-  Undistorter& u = c->und[slot];
-  if (dw != u.cm.w || dh != u.cm.h)   // the caller sized dst for another map: never write past it
-    return fail(BEVK_ERR_ARG, "undistorter slot %d holds a %dx%d map, the caller expects %dx%d", slot, u.cm.w, u.cm.h, dw, dh);
+// Host path: one host image through op into another, which the call has written when it returns.
+static int host_image(bevk_ctx* c, const ImageOp& op, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
+                      uint8_t* dst, int dw, int dh, int64_t dstride) {
+  RET(check_image(src, sw, sh, sstride, channels, "src"));
+  RET(check_op_size(op, dw, dh));
   RET(check_image(dst, dw, dh, dstride, channels, "dst"));
-  RET(undistort_to_scratch(c, slot, src, sw, sh, sstride, channels, interp));
+  RET(host_launch(c, op, src, sw, sh, sstride, channels, dw, dh));
   return download_image(c, c->s_dst, dst, dw, dh, dstride, channels);
 }
 
-// ------------------------------------------------------------------ undistortion of device frame batches
 // The source side of the device-batch calls: a frame, n >= 1, and an image stride that covers an image when n > 1.
 static int check_stack_src(const void* d_src, int64_t sis, int sw, int sh, int64_t srs, int channels, int n) {
   if (n < 1) return fail(BEVK_ERR_ARG, "n must be >= 1, got %d", n);
@@ -628,27 +698,6 @@ static int check_stack_src(const void* d_src, int64_t sis, int sw, int sh, int64
   if (n > 1 && sis < (int64_t)(sh - 1) * srs + (int64_t)sw * channels)
     return fail(BEVK_ERR_ARG, "src image stride %lld is smaller than one image", (long long)sis);
   return BEVK_OK;
-}
-
-// Checks the source side of the bevk_undistort_stack calls (and normalises *interp) and fills a (slot's map or model, n frames of the source);
-// the destination is left to the caller.  An image stride only matters when n > 1.
-static int stack_src_args(bevk_ctx* c, int slot, const void* d_src, int64_t sis, int sw, int sh, int64_t srs, int channels, int n,
-                          int* interp, GatherArgs* a) {
-  RET(need_undistorter(c, slot));
-  RET(gather_interp(interp));
-  RET(check_stack_src(d_src, sis, sw, sh, srs, channels, n));
-  const Undistorter& u = c->und[slot];
-  *a = GatherArgs{};
-  a->src = reinterpret_cast<const uint8_t*>(d_src); a->sw = sw; a->sh = sh; a->spitch = srs;
-  a->n = n; a->sistride = n > 1 ? sis : 0;
-  a->dw = u.cm.w; a->dh = u.cm.h;
-  if (u.fused) a->cm = u.cm;
-  else { a->map1 = u.map1.as<short2>(); a->map2 = u.map2.as<unsigned short>(); }
-  return BEVK_OK;
-}
-
-static int launch_undistort(bevk_ctx* c, int slot, const GatherArgs& a, int channels, int interp) {
-  return c->und[slot].fused ? launch_gather<1>(c, a, channels, interp) : launch_gather<0>(c, a, channels, interp);
 }
 
 // The destination side of the device-batch calls, given a checked source: rows, an image stride that covers an image
@@ -666,20 +715,71 @@ static int check_stack_dst(const void* d_src, int64_t sis, int sw, int sh, int64
   return BEVK_OK;
 }
 
-// bevk_undistort_stack_interp: any interpolation gather_interp takes.
-static int undistort_stack(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
-                           int channels, int n, void* d_dst, int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride,
-                           int interp) {
-  GatherArgs a;
-  RET(stack_src_args(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, &interp, &a));
-  if (dw != a.dw || dh != a.dh)   // the caller sized dst for another map: never write past it
-    return fail(BEVK_ERR_ARG, "undistorter slot %d holds a %dx%d map, the caller expects %dx%d", slot, a.dw, a.dh, dw, dh);
-  RET(check_stack_dst(d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
-                      dst_row_stride));
-  a.dst = reinterpret_cast<uint8_t*>(d_dst); a.dpitch = dst_row_stride; a.distride = n > 1 ? dst_image_stride : 0;
-  return launch_undistort(c, slot, a, channels, interp);
+// the caller's n device frames; an image stride only matters when n > 1
+static ImageBatch device_batch(const void* d_src, int64_t sis, int sw, int sh, int64_t srs, int n, void* d_dst, int64_t dis,
+                               int dw, int dh, int64_t drs) {
+  return ImageBatch{reinterpret_cast<const uint8_t*>(d_src), sw, sh, srs, n > 1 ? sis : 0,
+                    reinterpret_cast<uint8_t*>(d_dst), dw, dh, drs, n > 1 ? dis : 0, n};
 }
 
+// Device path: n device frames through op, enqueued only.  It allocates and copies nothing, so a graph can capture it.
+static int device_image(bevk_ctx* c, const ImageOp& op, const void* d_src, int64_t sis, int sw, int sh, int64_t srs, int channels,
+                        int n, void* d_dst, int64_t dis, int dw, int dh, int64_t drs) {
+  RET(check_stack_src(d_src, sis, sw, sh, srs, channels, n));
+  RET(check_op_size(op, dw, dh));
+  RET(check_stack_dst(d_src, sis, sw, sh, srs, channels, n, d_dst, dis, dw, dh, drs));
+  return launch(c, op, device_batch(d_src, sis, sw, sh, srs, n, d_dst, dis, dw, dh, drs), channels);
+}
+
+// ---- the entry points
+int bevk_remap(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, const int16_t* map1,
+               const uint16_t* map2, int dw, int dh, uint8_t* dst, int64_t dstride, int interp) {
+  RET(use(c));
+  ImageOp op;
+  RET(remap_op(map1, map2, interp, &op));
+  return host_image(c, op, src, sw, sh, sstride, channels, dst, dw, dh, dstride);
+}
+
+// ------------------------------------------------------------------ cached-map undistortion
+int bevk_undistorter_set(bevk_ctx* c, int slot, int model, const double K[9], const double* D, int n_dist,
+                         const double P[9], int dw, int dh, int fused) {
+  RET(use(c));
+  if (slot < 0 || slot >= 8) return fail(BEVK_ERR_ARG, "slot %d out of range", slot);
+  Undistorter& u = c->und[slot];
+  u.valid = false;
+  RET(make_model(model, K, D, n_dist, P, dw, dh, &u.cm));
+  u.fused = fused != 0;
+  if (u.fused) {   // the gathers evaluate the model per pixel: the slot keeps its column table
+    RET(attach_xs_table(c, u.xs, &u.cm));
+  } else {         // the table is read once, by the map build, from scratch
+    u.xs.release();
+    RET(attach_xs_table(c, c->s_xs, &u.cm));
+    RET(build_map(c, u.cm, u.map1, u.map2));
+    u.cm.xs = nullptr;
+  }
+  u.valid = true;
+  return BEVK_OK;
+}
+
+int bevk_undistorter_maps(bevk_ctx* c, int slot, int16_t* map1, uint16_t* map2) {
+  RET(use(c));
+  RET(need_undistorter(c, slot));
+  if (!map1 || !map2) return fail(BEVK_ERR_ARG, "null output map");
+  Undistorter& u = c->und[slot];
+  const bool resident = !u.fused;   // a fused slot has no resident map: evaluate into scratch
+  if (!resident) RET(build_map(c, u.cm, c->s_m1, c->s_m2));
+  return download_maps(c, resident ? u.map1.p : c->s_m1.p, resident ? u.map2.p : c->s_m2.p, (size_t)u.cm.w * u.cm.h, map1, map2);
+}
+
+int bevk_undistort(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
+                   uint8_t* dst, int dw, int dh, int64_t dstride, int interp) {
+  RET(use(c));
+  ImageOp op;
+  RET(undistort_op(c, slot, interp, &op));
+  return host_image(c, op, src, sw, sh, sstride, channels, dst, dw, dh, dstride);
+}
+
+// ------------------------------------------------------------------ undistortion of device frame batches
 int bevk_undistort_stack(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
                          int channels, int n, void* d_dst, int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride,
                          int interp) {
@@ -688,16 +788,18 @@ int bevk_undistort_stack(bevk_ctx* c, int slot, const void* d_src, int64_t src_i
   if (interp != BEVK_INTER_LINEAR && interp != BEVK_INTER_NEAREST)
     return fail(BEVK_ERR_UNSUPPORTED, "interp %d: bevk_undistort_stack takes INTER_NEAREST and INTER_LINEAR, "
                 "bevk_undistort_stack_interp every cv2 flag", interp);
-  return undistort_stack(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
-                         dst_row_stride, interp);
+  return bevk_undistort_stack_interp(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst,
+                                     dst_image_stride, dw, dh, dst_row_stride, interp);
 }
 
 int bevk_undistort_stack_interp(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh,
                                 int64_t src_row_stride, int channels, int n, void* d_dst, int64_t dst_image_stride, int dw, int dh,
                                 int64_t dst_row_stride, int interp) {
   RET(use(c));
-  return undistort_stack(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
-                         dst_row_stride, interp);
+  ImageOp op;
+  RET(undistort_op(c, slot, interp, &op));
+  return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
+                      dst_row_stride);
 }
 
 int bevk_undistort_last_path(bevk_ctx* c) { return c ? c->gather_path : 0; }
@@ -706,152 +808,47 @@ int bevk_undistort_last_path(bevk_ctx* c) { return c ? c->gather_path : 0; }
 int bevk_warp_perspective(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
                           const double H[9], uint8_t* dst, int dw, int dh, int64_t dstride, int interp) {
   RET(use(c));
-  RET(check_image(src, sw, sh, sstride, channels, "src"));
-  RET(check_image(dst, dw, dh, dstride, channels, "dst"));
-  RET(gather_interp(&interp));
-  GatherArgs a{};
-  a.n = 1;
-  RET(make_homog(H, &a.hm));
-  RET(upload_image(c, c->s_src, src, sw, sh, sstride, channels));
-  RET(c->s_dst.ensure((size_t)dw * dh * channels));
-  a.src = c->s_src.as<uint8_t>(); a.sw = sw; a.sh = sh; a.spitch = (long long)sw * channels;
-  a.dst = c->s_dst.as<uint8_t>(); a.dw = dw; a.dh = dh; a.dpitch = (long long)dw * channels;
-  RET(launch_gather<2>(c, a, channels, interp));
-  return download_image(c, c->s_dst, dst, dw, dh, dstride, channels);
+  ImageOp op;
+  RET(perspective_op(H, interp, &op));
+  return host_image(c, op, src, sw, sh, sstride, channels, dst, dw, dh, dstride);
 }
 
 // ------------------------------------------------------------------ cv2.warpAffine
-// flags -> interpolation (gather_interp's) and the inverse map in a->hm.M[0..5].
-static int affine_args(const double* M, int flags, int* interp, GatherArgs* a) {
-  if (!M) return fail(BEVK_ERR_ARG, "null M");
-  if (flags & ~(7 | BEVK_WARP_INVERSE_MAP)) return fail(BEVK_ERR_UNSUPPORTED, "warpAffine flags %d", flags);
-  *interp = flags & 7;
-  RET(gather_interp(interp));
-  if (flags & BEVK_WARP_INVERSE_MAP) memcpy(a->hm.M, M, 6 * sizeof(double));
-  else inv_affine(M, a->hm.M);
-  return BEVK_OK;
-}
-
 int bevk_warp_affine(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, const double M[6],
                      uint8_t* dst, int dw, int dh, int64_t dstride, int flags) {
   RET(use(c));
-  RET(check_image(src, sw, sh, sstride, channels, "src"));
-  RET(check_image(dst, dw, dh, dstride, channels, "dst"));
-  GatherArgs a{};
-  int interp;
-  RET(affine_args(M, flags, &interp, &a));
-  a.n = 1;
-  RET(upload_image(c, c->s_src, src, sw, sh, sstride, channels));
-  RET(c->s_dst.ensure((size_t)dw * dh * channels));
-  a.src = c->s_src.as<uint8_t>(); a.sw = sw; a.sh = sh; a.spitch = (long long)sw * channels;
-  a.dst = c->s_dst.as<uint8_t>(); a.dw = dw; a.dh = dh; a.dpitch = (long long)dw * channels;
-  RET(launch_gather<3>(c, a, channels, interp));
-  return download_image(c, c->s_dst, dst, dw, dh, dstride, channels);
+  ImageOp op;
+  RET(affine_op(M, flags, &op));
+  return host_image(c, op, src, sw, sh, sstride, channels, dst, dw, dh, dstride);
 }
 
 int bevk_warp_affine_stack(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
                            int channels, int n, const double M[6], void* d_dst, int64_t dst_image_stride, int dw, int dh,
                            int64_t dst_row_stride, int flags) {
   RET(use(c));
-  GatherArgs a{};
-  int interp;
-  RET(affine_args(M, flags, &interp, &a));
-  RET(check_stack_src(d_src, src_image_stride, sw, sh, src_row_stride, channels, n));
-  RET(check_stack_dst(d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
-                      dst_row_stride));
-  a.src = reinterpret_cast<const uint8_t*>(d_src); a.sw = sw; a.sh = sh; a.spitch = src_row_stride;
-  a.dst = reinterpret_cast<uint8_t*>(d_dst); a.dw = dw; a.dh = dh; a.dpitch = dst_row_stride;
-  a.n = n; a.sistride = n > 1 ? src_image_stride : 0; a.distride = n > 1 ? dst_image_stride : 0;
-  return launch_gather<3>(c, a, channels, interp);
+  ImageOp op;
+  RET(affine_op(M, flags, &op));
+  return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
+                      dst_row_stride);
 }
 
 // ------------------------------------------------------------------ cv2.resize
-// Checks interp and cv2's size rule (resize_geometry) and fills a's scales; returns the body in *kind.
-static int resize_args(int sw, int sh, int dw, int dh, double fx, double fy, int interp, ResizeArgs* a, int* kind) {
-  if (interp != BEVK_INTER_NEAREST && interp != BEVK_INTER_LINEAR && interp != BEVK_INTER_AREA)
-    return fail(BEVK_ERR_UNSUPPORTED, "resize interp %d: INTER_NEAREST, INTER_LINEAR and INTER_AREA only", interp);
-  if (sw <= 0 || sh <= 0 || dw <= 0 || dh <= 0) return fail(BEVK_ERR_ARG, "bad size %dx%d -> %dx%d", sw, sh, dw, dh);
-  *a = ResizeArgs{};
-  if (fx == 0. && fy == 0.) {
-    a->inv_x = (double)dw / sw; a->inv_y = (double)dh / sh;
-  } else {
-    int w = 0, h = 0;
-    a->inv_x = fx; a->inv_y = fy;
-    if (!resize_geometry(sw, sh, &w, &h, &a->inv_x, &a->inv_y))
-      return fail(BEVK_ERR_ARG, "fx %g, fy %g give no image from %dx%d", fx, fy, sw, sh);
-    if (w != dw || h != dh) return fail(BEVK_ERR_ARG, "fx %g, fy %g make %dx%d images, the caller expects %dx%d", fx, fy, w, h, dw, dh);
-  }
-  *kind = resize_kind(interp, *a);
-  a->sw = sw; a->sh = sh; a->dw = dw; a->dh = dh;
-  return BEVK_OK;
-}
-
-template <int C, int KIND>
-static void launch_resize_c(bevk_ctx* c, const ResizeArgs& a, dim3 g, bool batch) {
-  if (batch) k_resize<C, KIND, GATHER_NB><<<g, 256, 0, c->stream>>>(a);
-  else k_resize<C, KIND, 1><<<g, 256, 0, c->stream>>>(a);
-}
-template <int C>
-static void launch_resize_k(bevk_ctx* c, const ResizeArgs& a, int kind, dim3 g, bool batch) {
-  switch (kind) {
-    case RZ_NEAREST: launch_resize_c<C, RZ_NEAREST>(c, a, g, batch); break;
-    case RZ_LINEAR: launch_resize_c<C, RZ_LINEAR>(c, a, g, batch); break;
-    case RZ_AREA_LINEAR: launch_resize_c<C, RZ_AREA_LINEAR>(c, a, g, batch); break;
-    case RZ_AREA_FAST: launch_resize_c<C, RZ_AREA_FAST>(c, a, g, batch); break;
-    default: launch_resize_c<C, RZ_AREA>(c, a, g, batch);
-  }
-}
-
-// Enqueue k_resize over a.n >= 1 frames: grid.z = frame groups of GATHER_NB (one frame: NB = 1), 65535 groups a launch.
-static int launch_resize(bevk_ctx* c, const ResizeArgs& a0, int channels, int kind) {
-  const int per_launch = 65535 * GATHER_NB;
-  for (int f0 = 0; f0 < a0.n; f0 += per_launch) {
-    ResizeArgs a = a0;
-    a.n = std::min(per_launch, a0.n - f0);
-    a.src += (long long)f0 * a0.sistride;
-    a.dst += (long long)f0 * a0.distride;
-    const bool batch = a.n > 1;
-    const dim3 g((a.dw + 31) / 32, (a.dh + 7) / 8, batch ? (unsigned)((a.n + GATHER_NB - 1) / GATHER_NB) : 1u);
-    if (channels == 1) launch_resize_k<1>(c, a, kind, g, batch);
-    else if (channels == 3) launch_resize_k<3>(c, a, kind, g, batch);
-    else launch_resize_k<4>(c, a, kind, g, batch);
-    LAUNCHED(c);
-  }
-  c->gather_path = 3;
-  return BEVK_OK;
-}
-
 int bevk_resize(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, uint8_t* dst, int dw, int dh,
                 int64_t dstride, double fx, double fy, int interp) {
   RET(use(c));
-  RET(check_image(src, sw, sh, sstride, channels, "src"));
-  RET(check_image(dst, dw, dh, dstride, channels, "dst"));
-  ResizeArgs a;
-  int kind;
-  RET(resize_args(sw, sh, dw, dh, fx, fy, interp, &a, &kind));
-  RET(upload_image(c, c->s_src, src, sw, sh, sstride, channels));
-  RET(c->s_dst.ensure((size_t)dw * dh * channels));
-  a.n = 1;
-  a.src = c->s_src.as<uint8_t>(); a.spitch = (long long)sw * channels;
-  a.dst = c->s_dst.as<uint8_t>(); a.dpitch = (long long)dw * channels;
-  RET(launch_resize(c, a, channels, kind));
-  return download_image(c, c->s_dst, dst, dw, dh, dstride, channels);
+  ImageOp op;
+  RET(resize_op(sw, sh, dw, dh, fx, fy, interp, &op));
+  return host_image(c, op, src, sw, sh, sstride, channels, dst, dw, dh, dstride);
 }
 
 int bevk_resize_stack(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
                       int channels, int n, void* d_dst, int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride,
                       double fx, double fy, int interp) {
   RET(use(c));
-  ResizeArgs a;
-  int kind;
-  RET(resize_args(sw, sh, dw, dh, fx, fy, interp, &a, &kind));
-  RET(check_stack_src(d_src, src_image_stride, sw, sh, src_row_stride, channels, n));
-  RET(check_stack_dst(d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
-                      dst_row_stride));
-  a.src = reinterpret_cast<const uint8_t*>(d_src); a.spitch = src_row_stride;
-  a.dst = reinterpret_cast<uint8_t*>(d_dst); a.dpitch = dst_row_stride;
-  a.n = n; a.sistride = n > 1 ? src_image_stride : 0; a.distride = n > 1 ? dst_image_stride : 0;
-  return launch_resize(c, a, channels, kind);
+  ImageOp op;
+  RET(resize_op(sw, sh, dw, dh, fx, fy, interp, &op));
+  return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
+                      dst_row_stride);
 }
 
 int bevk_warp_maps(bevk_ctx* c, const int16_t* map1, const uint16_t* map2, int sw, int sh, const double H[9], int dw,
@@ -872,10 +869,7 @@ int bevk_warp_maps(bevk_ctx* c, const int16_t* map1, const uint16_t* map2, int s
   a.out1 = c->s_o1.as<short2>(); a.out2 = c->s_o2.as<unsigned short>(); a.dw = dw; a.dh = dh;
   k_warp_maps<0><<<grid2d(dw, dh), 256, 0, c->stream>>>(a);
   LAUNCHED(c);
-  CU(cudaMemcpyAsync(out1, c->s_o1.p, nd * 4, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaMemcpyAsync(out2, c->s_o2.p, nd * 2, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return BEVK_OK;
+  return download_maps(c, c->s_o1.p, c->s_o2.p, nd, out1, out2);
 }
 
 // ------------------------------------------------------------------ BEV engine: setup
@@ -3085,13 +3079,14 @@ int bevk_undistort_jpeg(bevk_ctx* c, int slot, const uint8_t* src, int sw, int s
                         uint8_t* out, uint64_t capacity, uint64_t* size) {
   NvtxRange nvtx_call("bevk_undistort_jpeg (host frame -> undistorted JPEG)");
   RET(use(c));
-  RET(need_undistorter(c, slot));
-  const int dw = c->und[slot].cm.w, dh = c->und[slot].cm.h;
-  RET(jpeg_size_check(dw, dh));
+  ImageOp op;
+  RET(undistort_op(c, slot, interp, &op));
+  RET(check_image(src, sw, sh, sstride, 3, "src"));
+  RET(jpeg_size_check(op.dw, op.dh));
   const jpeg::Opts o = jpeg_ctx_opts(c, quality);
   return enc_chunks(c, "JPEG", 1, 1, true, out, capacity, size, [&](int, int, int s) -> int {
-    RET(undistort_to_scratch(c, slot, src, sw, sh, sstride, 3, interp));
-    return jpeg_enqueue(c, s, EncIn{c->s_dst.p, 0, (long long)dw * 3}, 1, dw, dh, o);
+    RET(host_launch(c, op, src, sw, sh, sstride, 3, op.dw, op.dh));
+    return jpeg_enqueue(c, s, EncIn{c->s_dst.p, 0, (long long)op.dw * 3}, 1, op.dw, op.dh, o);
   });
 }
 
@@ -3102,20 +3097,22 @@ int bevk_undistort_stack_jpeg(bevk_ctx* c, int slot, const void* d_src, int64_t 
                               uint64_t* sizes) {
   NvtxRange nvtx_call("bevk_undistort_stack_jpeg (device frames -> undistorted JPEG streams)");
   RET(use(c));
-  GatherArgs a;
-  RET(stack_src_args(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, 3, n, &interp, &a));
-  const int dw = a.dw, dh = a.dh;
+  ImageOp op;
+  RET(undistort_op(c, slot, interp, &op));
+  RET(check_stack_src(d_src, src_image_stride, sw, sh, src_row_stride, 3, n));
+  const int dw = op.dw, dh = op.dh;
   RET(jpeg_size_check(dw, dh));
   const jpeg::Opts o = jpeg_ctx_opts(c, quality);
   const int chunk = jpeg_chunk(n);
   const long long ibytes = (long long)dw * dh * 3;
+  const ImageBatch b = device_batch(d_src, src_image_stride, sw, sh, src_row_stride, n, nullptr, ibytes, dw, dh, (long long)dw * 3);
   return enc_chunks(c, "JPEG", n, chunk, false, out, capacity, sizes, [&](int b0, int nb, int s) -> int {
     RET(c->s_dst.ensure((size_t)ibytes * chunk));
-    GatherArgs part = a;
-    part.src += (long long)b0 * a.sistride;
+    ImageBatch part = b;   // frames [b0, b0 + nb) into the dense scratch
+    part.src += (long long)b0 * b.sistride;
     part.n = nb;
-    part.dst = c->s_dst.as<uint8_t>(); part.dpitch = (long long)dw * 3; part.distride = ibytes;
-    RET(launch_undistort(c, slot, part, 3, interp));
+    part.dst = c->s_dst.as<uint8_t>(); part.distride = ibytes;
+    RET(launch(c, op, part, 3));
     return jpeg_enqueue(c, s, EncIn{c->s_dst.p, ibytes, (long long)dw * 3}, nb, dw, dh, o);
   });
 }

@@ -344,7 +344,6 @@ def remap(src: np.ndarray, map1: np.ndarray, map2: np.ndarray | None, interpolat
     INTER_CUBIC, INTER_AREA (read as INTER_LINEAR, as cv2.remap reads it) or INTER_LANCZOS4; all but NEAREST need map2.
     The result is byte-identical to cv2.remap's."""
     ctx = ctx or L.default_context()
-    img, sw, sh, ss, ch = L.image_view(src)
     m1 = np.ascontiguousarray(map1, np.int16)
     if m1.ndim != 3 or m1.shape[2] != 2:
         raise L.BevkError("map1 must be int16[h][w][2] (CV_16SC2)")
@@ -352,10 +351,8 @@ def remap(src: np.ndarray, map1: np.ndarray, map2: np.ndarray | None, interpolat
     m2 = None if map2 is None else np.ascontiguousarray(map2, np.uint16)
     if m2 is not None and m2.shape != (dh, dw):
         raise L.BevkError("map2 must be uint16[h][w] (CV_16UC1)")
-    out = _out((dh, dw) if src.ndim == 2 else (dh, dw, ch), out)
-    L.check(ctx.lib.bevk_remap(ctx.h, L.vptr(img), sw, sh, ss, ch, L.vptr(m1), None if m2 is None else L.vptr(m2),
-                               dw, dh, L.vptr(out), dw * ch, _interp(interpolation)))
-    return out
+    return _host_image(src, dw, dh, out, lambda s, d, dstride: ctx.lib.bevk_remap(
+        ctx.h, *s, L.vptr(m1), None if m2 is None else L.vptr(m2), dw, dh, d, dstride, _interp(interpolation)))
 
 
 def warp_perspective(src: np.ndarray, H, dsize, flags: int = INTER_LINEAR, ctx: L.Context | None = None,
@@ -363,23 +360,28 @@ def warp_perspective(src: np.ndarray, H, dsize, flags: int = INTER_LINEAR, ctx: 
     """cv2.warpPerspective(src, H, dsize, flags) for uint8 images, BORDER_CONSTANT 0.  flags: INTER_NEAREST,
     INTER_LINEAR, INTER_CUBIC, INTER_AREA (read as INTER_LINEAR, as cv2 reads it) or INTER_LANCZOS4."""
     ctx = ctx or L.default_context()
-    img, sw, sh, ss, ch = L.image_view(src)
     dw, dh = int(dsize[0]), int(dsize[1])
-    out = _out((dh, dw) if src.ndim == 2 else (dh, dw, ch), out)
-    L.check(ctx.lib.bevk_warp_perspective(ctx.h, L.vptr(img), sw, sh, ss, ch, L.dptr(H), L.vptr(out), dw, dh,
-                                          dw * ch, _interp(flags)))
-    return out
+    return _host_image(src, dw, dh, out, lambda s, d, dstride: ctx.lib.bevk_warp_perspective(
+        ctx.h, *s, L.dptr(H), d, dw, dh, dstride, _interp(flags)))
 
 
 INTER_LINEAR_EXACT, INTER_NEAREST_EXACT, WARP_INVERSE_MAP = L.INTER_LINEAR_EXACT, L.INTER_NEAREST_EXACT, L.WARP_INVERSE_MAP
 BORDER_CONSTANT = 0
 
 
-def _device_images(src, dw, dh, out, ctx, what, call):
-    """The body of the device forms of resize / warp_affine: src a uint8 CUDA array [H][W], [H][W][C] or [N][H][W][C]
-    read in place; out (default a new torch tensor) of the same rank with dh x dw images; call(src, out) with the
-    (pointer, image stride, ...) layouts is run on torch's current stream and only enqueues."""
-    from .sharding import _torch_current_stream
+def _host_image(src, dw, dh, out, call):
+    """The body of the host forms: src a NumPy image [H][W] or [H][W][C]; out (default a new array) [dh][dw] of the same
+    rank; call(src, dst, dst_stride) with src's (pointer, width, height, stride, channels) and dst's pointer."""
+    img, sw, sh, ss, ch = L.image_view(src)
+    out = _out((dh, dw) if src.ndim == 2 else (dh, dw, ch), out)
+    L.check(call((L.vptr(img), sw, sh, ss, ch), L.vptr(out), dw * ch))
+    return out
+
+
+def _device_images(src, dw, dh, out, ctx, what, call, stream=None):
+    """The body of the device forms: src a uint8 CUDA array [H][W], [H][W][C] or [N][H][W][C] read in place; out
+    (default a new torch tensor) of the same rank with dh x dw images; call(src, out) with the (pointer, image stride,
+    ...) layouts is run on ``stream`` (default torch's current stream) and only enqueues."""
     ptr, rank, n, sh, sw, ch, simg, srow = _cuda_images(src, what)
     shape = {2: (dh, dw), 3: (dh, dw, ch), 4: (n, dh, dw, ch)}[rank]
     if out is None:
@@ -388,9 +390,20 @@ def _device_images(src, dw, dh, out, ctx, what, call):
     optr, orank, on, oh, ow, och, oimg, orow = _cuda_images(out, "out")
     if orank != rank or (on, oh, ow, och) != (n, dh, dw, ch):
         raise L.BevkError(f"out must be a uint8 CUDA array of shape {shape}")
-    with ctx.on_stream(_torch_current_stream(ctx.device)):
+    if stream is None:
+        from .sharding import _torch_current_stream
+        stream = _torch_current_stream(ctx.device)
+    with ctx.on_stream(stream):
         L.check(call((C.c_void_p(ptr), simg, sw, sh, srow, ch, n), (C.c_void_p(optr), oimg, dw, dh, orow)))
     return out
+
+
+def _image_call(src, dw, dh, out, ctx, what, host, device):
+    """A CUDA array goes to the device form (_device_images, with ``device``), anything else to the host form
+    (_host_image, with ``host``)."""
+    if hasattr(src, "__cuda_array_interface__"):
+        return _device_images(src, dw, dh, out, ctx, what, device)
+    return _host_image(src, dw, dh, out, host)
 
 
 def _src_size(src):
@@ -424,13 +437,9 @@ def resize(src, dsize, fx: float = 0, fy: float = 0, interpolation: int = INTER_
     ctx = ctx or L.default_context()
     dw, dh = resize_size(_src_size(src), dsize, fx, fy)
     sx, sy = (float(fx), float(fy)) if dsize is None or tuple(int(v) for v in dsize) == (0, 0) else (0.0, 0.0)
-    if hasattr(src, "__cuda_array_interface__"):
-        return _device_images(src, dw, dh, out, ctx, "resize",
-                              lambda s, d: ctx.lib.bevk_resize_stack(ctx.h, *s, *d, sx, sy, int(interpolation)))
-    img, sw, sh, ss, ch = L.image_view(src)
-    out = _out((dh, dw) if src.ndim == 2 else (dh, dw, ch), out)
-    L.check(ctx.lib.bevk_resize(ctx.h, L.vptr(img), sw, sh, ss, ch, L.vptr(out), dw, dh, dw * ch, sx, sy, int(interpolation)))
-    return out
+    return _image_call(src, dw, dh, out, ctx, "resize",
+                       lambda s, d, ds: ctx.lib.bevk_resize(ctx.h, *s, d, dw, dh, ds, sx, sy, int(interpolation)),
+                       lambda s, d: ctx.lib.bevk_resize_stack(ctx.h, *s, *d, sx, sy, int(interpolation)))
 
 
 def warp_affine(src, M, dsize, flags: int = INTER_LINEAR, borderMode: int = BORDER_CONSTANT, borderValue=0,
@@ -445,20 +454,19 @@ def warp_affine(src, M, dsize, flags: int = INTER_LINEAR, borderMode: int = BORD
     if m.shape != (2, 3):
         raise L.BevkError(f"M must be 2x3, got shape {m.shape}")
     dw, dh = int(dsize[0]), int(dsize[1])
-    if hasattr(src, "__cuda_array_interface__"):
-        return _device_images(src, dw, dh, out, ctx, "warp_affine",
-                              lambda s, d: ctx.lib.bevk_warp_affine_stack(ctx.h, *s, L.dptr(m), *d, int(flags)))
-    img, sw, sh, ss, ch = L.image_view(src)
-    out = _out((dh, dw) if src.ndim == 2 else (dh, dw, ch), out)
-    L.check(ctx.lib.bevk_warp_affine(ctx.h, L.vptr(img), sw, sh, ss, ch, L.dptr(m), L.vptr(out), dw, dh, dw * ch, int(flags)))
-    return out
+    return _image_call(src, dw, dh, out, ctx, "warp_affine",
+                       lambda s, d, ds: ctx.lib.bevk_warp_affine(ctx.h, *s, L.dptr(m), d, dw, dh, ds, int(flags)),
+                       lambda s, d: ctx.lib.bevk_warp_affine_stack(ctx.h, *s, L.dptr(m), *d, int(flags)))
+
+
+_GATHER_PATHS = {4: "word", 1: "byte", 2: "taps", 3: "resize"}
 
 
 def last_path(ctx: L.Context | None = None) -> str:
     """Which kernel the last gather or resize call of ctx launched: 'word' (k_gather4), 'byte' (k_gather), 'taps'
     (k_gather_taps) or 'resize' (k_resize)."""
     ctx = ctx or L.default_context()
-    return {4: "word", 1: "byte", 2: "taps", 3: "resize"}.get(int(ctx.lib.bevk_undistort_last_path(ctx.h)), "none")
+    return _GATHER_PATHS.get(int(ctx.lib.bevk_undistort_last_path(ctx.h)), "none")
 
 
 def warp_perspective_maps(map1, map2, H, dsize, ctx: L.Context | None = None):
@@ -573,14 +581,11 @@ class Undistorter:
     def __call__(self, src: np.ndarray, interpolation: int = INTER_LINEAR, out: np.ndarray | None = None) -> np.ndarray:
         """cv2.remap(src, map1, map2, interpolation), any of remap()'s interpolations.  A CUDA array (e.g. a torch tensor on the GPU) goes to cuda() and
         the result stays on the device; NumPy input is uploaded, undistorted and downloaded in one call."""
-        if hasattr(src, "__cuda_array_interface__"):
-            return self.cuda(src, out=out, interpolation=interpolation)
         self._live()
-        img, sw, sh, ss, ch = L.image_view(src)
-        out = _out((self.h, self.w) if src.ndim == 2 else (self.h, self.w, ch), out)
-        L.check(self.ctx.lib.bevk_undistort(self.ctx.h, self.slot, L.vptr(img), sw, sh, ss, ch, L.vptr(out), self.w, self.h,
-                                            self.w * ch, _interp(interpolation)))
-        return out
+        lib, h = self.ctx.lib, self.ctx.h
+        return _image_call(src, self.w, self.h, out, self.ctx, "frames",
+                           lambda s, d, ds: lib.bevk_undistort(h, self.slot, *s, d, self.w, self.h, ds, _interp(interpolation)),
+                           lambda s, d: lib.bevk_undistort_stack_interp(h, self.slot, *s, *d, _interp(interpolation)))
 
     def jpeg(self, src: np.ndarray, quality: int = 95, interpolation: int = INTER_LINEAR, params=None) -> bytes:
         """The undistorted image as the bytes cv2.imwrite(path, self(src), [IMWRITE_JPEG_QUALITY, quality] + params)
@@ -621,21 +626,8 @@ class Undistorter:
         INTER_LANCZOS4, its row of weights are read once for several frames of the batch.  Runs on
         ``stream`` (a raw CUDA stream handle), default torch's current stream, and only enqueues.  Returns ``out``."""
         self._live()
-        ptr, rank, n, sh, sw, ch, simg, srow = _cuda_images(frames, "frames")
-        shape = {2: (self.h, self.w), 3: (self.h, self.w, ch), 4: (n, self.h, self.w, ch)}[rank]
-        if out is None:
-            import torch
-            out = torch.empty(shape, dtype=torch.uint8, device=torch.device("cuda", self.ctx.device))
-        optr, orank, on, oh, ow, och, oimg, orow = _cuda_images(out, "out")
-        if orank != rank or (on, oh, ow, och) != (n, self.h, self.w, ch):
-            raise L.BevkError(f"out must be a uint8 CUDA array of shape {shape}")
-        if stream is None:
-            from .sharding import _torch_current_stream
-            stream = _torch_current_stream(self.ctx.device)
-        with self.ctx.on_stream(stream):
-            L.check(self.ctx.lib.bevk_undistort_stack_interp(self.ctx.h, self.slot, C.c_void_p(ptr), simg, sw, sh, srow, ch, n,
-                                                             C.c_void_p(optr), oimg, self.w, self.h, orow, _interp(interpolation)))
-        return out
+        return _device_images(frames, self.w, self.h, out, self.ctx, "frames", lambda s, d: self.ctx.lib.bevk_undistort_stack_interp(
+            self.ctx.h, self.slot, *s, *d, _interp(interpolation)), stream)
 
     def cuda_to_jpeg(self, frames, quality: int = 95, interpolation: int = INTER_LINEAR, params=None) -> list[bytes]:
         """cuda() followed by cv2.imencode('.jpg', img, [IMWRITE_JPEG_QUALITY, quality] + params) per frame, with the
@@ -658,7 +650,7 @@ class Undistorter:
     def last_path(self) -> str:
         """Which gather the last call of this ctx launched: 'word' (k_gather4, 4 pixels per thread), 'byte' (k_gather) or
         'taps' (k_gather_taps, INTER_CUBIC / INTER_LANCZOS4)."""
-        return {4: "word", 1: "byte", 2: "taps"}.get(int(self.ctx.lib.bevk_undistort_last_path(self.ctx.h)), "none")
+        return last_path(self.ctx)
 
 
 class BevEngine:
