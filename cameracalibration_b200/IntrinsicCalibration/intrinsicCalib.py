@@ -110,6 +110,7 @@ class InCalibrator:
         return args
 
     def set_calibration(self, camera_mat, dist_coeff):
+        """K and D as cv2 calibrated them: a fisheye D of 4 coefficients, a "normal" (pinhole) D of 4, 5, 8, 12 or 14."""
         d = self.camera.data
         d.camera_mat = np.asarray(camera_mat, np.float64)
         d.dist_coeff = np.asarray(dist_coeff, np.float64)

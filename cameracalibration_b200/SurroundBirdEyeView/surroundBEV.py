@@ -14,6 +14,8 @@ Differences from the reference that are deliberate:
     ``get_args()`` returns the same mutable namespace with the same attribute names.
   * K/D/H are read from ``args.DATA_DIR`` (default ``<this dir>/data``, the reference's
     layout ``{name}/camera_{name}_{K,D,H}.npy``) or passed as ``calib={name: (K, D, H)}``.
+    ``calib={name: (K, D, H, "pinhole")}`` takes a pinhole camera instead of a fisheye, with D of
+    4, 5, 8, 12 or 14 coefficients as cv2.initUndistortRectifyMap takes it.
   * ``BevGenerator.run_batch`` renders many frame-sets per call (the reference has no
     batch API); ``BevGenerator(..., interpolation=cv2.INTER_NEAREST)`` selects nearest-neighbour
     sampling with cv2.remap's exact fixed-point-map semantics (the reference always uses bilinear).
@@ -92,7 +94,8 @@ def luminance_balance(images):
 
 # ----------------------------------------------------------------------------------------
 class Camera:
-    """One fisheye camera: K, D, H, destination matrix, undistort maps, BEV maps."""
+    """One camera: K, D, H, destination matrix, undistort maps, BEV maps.  A fisheye, or a pinhole when calib has a
+    fourth element "pinhole"."""
 
     def __init__(self, name, calib=None, geo: _Geo | None = None):
         self.name = name
@@ -100,7 +103,10 @@ class Camera:
         if calib is None:
             base = os.path.join(args.DATA_DIR, name, "camera_" + name + "_")
             calib = tuple(np.load(base + s + ".npy") for s in "KDH")
-        self.camera_mat, self.dist_coeff, self.homography = (np.asarray(m, np.float64) for m in calib)
+        self.model = calib[3] if len(calib) > 3 else "fisheye"
+        if self.model not in ("fisheye", "pinhole"):
+            raise L.BevkError(f'camera {name}: model must be "fisheye" or "pinhole", got {self.model!r}')
+        self.camera_mat, self.dist_coeff, self.homography = (np.asarray(m, np.float64) for m in calib[:3])
         self.camera_mat_dst = self.get_camera_mat_dst()
         self._und = None
         self._und_maps = None
@@ -119,7 +125,8 @@ class Camera:
     # maps live on the device; the numpy views are materialised only if somebody asks
     def _undistorter(self):
         if self._und is None:
-            self._und = ops.Undistorter(self.camera_mat, self.dist_coeff, self.camera_mat_dst, self._g.und_size)
+            self._und = ops.Undistorter(self.camera_mat, self.dist_coeff, self.camera_mat_dst, self._g.und_size,
+                                        model=self.model)
         return self._und
 
     def get_undistort_maps(self):
@@ -145,7 +152,7 @@ class Camera:
         if self._bev1 is None:
             g = self._g
             e = ops.BevEngine(1, (g.FW, g.FH), (g.BW, g.BH))
-            e.set_camera(0, self.camera_mat, self.dist_coeff, self.camera_mat_dst, g.und_size, self.homography)
+            e.set_camera(0, self.camera_mat, self.dist_coeff, self.camera_mat_dst, g.und_size, self.homography, self.model)
             e.set_mask(0, np.full((g.BH, g.BW), 255, np.uint8))
             e.finalize()
             self._bev1 = e
@@ -281,7 +288,8 @@ class BevGenerator:
         if interpolation is not None:   # extension: cv2.INTER_NEAREST (0) / cv2.INTER_LINEAR (1, the reference)
             self.engine.set_interpolation(interpolation)
         for i, (cam, mk) in enumerate(zip(self.cameras, self.masks)):
-            self.engine.set_camera(i, cam.camera_mat, cam.dist_coeff, cam.camera_mat_dst, g.und_size, cam.homography)
+            self.engine.set_camera(i, cam.camera_mat, cam.dist_coeff, cam.camera_mat_dst, g.und_size, cam.homography,
+                                   cam.model)
             self.engine.set_mask(i, mk.mask)
         self.engine.finalize()
 

@@ -39,8 +39,10 @@ SIGNATURES = {
     "bevk_host_alloc": (C.c_int, [C.c_uint64, C.POINTER(_p)]),
     "bevk_host_free": (C.c_int, [_p]),
     "bevk_undistort_map": (C.c_int, [_p, C.c_int, _dp, _dp, C.c_int, _dp, C.c_int, C.c_int, _p, _p]),
+    "bevk_undistort_rectify_map": (C.c_int, [_p, C.c_int, _dp, _dp, C.c_int, _dp, _dp, C.c_int, C.c_int, _p, _p]),
     "bevk_remap": (C.c_int, [_p, _p, C.c_int, C.c_int, C.c_int64, C.c_int, _p, _p, C.c_int, C.c_int, _p, C.c_int64, C.c_int]),
     "bevk_undistorter_set": (C.c_int, [_p, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, C.c_int, C.c_int, C.c_int]),
+    "bevk_undistorter_set_rectify": (C.c_int, [_p, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, _dp, C.c_int, C.c_int, C.c_int]),
     "bevk_undistorter_maps": (C.c_int, [_p, C.c_int, _p, _p]),
     "bevk_undistort": (C.c_int, [_p, C.c_int, _p, C.c_int, C.c_int, C.c_int64, C.c_int, _p, C.c_int, C.c_int, C.c_int64, C.c_int]),
     "bevk_undistort_stack": (C.c_int, [_p, C.c_int, _p, C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, _p, C.c_int64,
@@ -59,6 +61,7 @@ SIGNATURES = {
                                     C.c_int, C.c_int64, C.c_double, C.c_double, C.c_int]),
     "bevk_bev_configure": (C.c_int, [_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "bevk_bev_set_camera": (C.c_int, [_p, C.c_int, _dp, _dp, _dp, C.c_int, C.c_int, _dp]),
+    "bevk_bev_set_camera_model": (C.c_int, [_p, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, C.c_int, C.c_int, _dp]),
     "bevk_bev_set_maps": (C.c_int, [_p, C.c_int, _p, _p]),
     "bevk_bev_get_maps": (C.c_int, [_p, C.c_int, _p, _p]),
     "bevk_bev_set_interpolation": (C.c_int, [_p, C.c_int]),

@@ -109,19 +109,42 @@ struct DevBuf {
   template <class T> T* as() const { return reinterpret_cast<T*>(p); }
 };
 
-static int make_model(int model, const double* K, const double* D, int n_dist, const double* P, int w, int h,
-                      CamModel* cm) {
+// A camera of either model (K, D, R, P) as the kernels take it (lens_model): CamModel, LensExt and whether it needs the
+// LENS = 1 instances.  D lengths cv2 refuses are refused.
+struct Lens {
+  CamModel cm;
+  LensExt lx;
+  bool full = false;
+};
+
+static int make_model(int model, const double* K, const double* D, int n_dist, const double* R, const double* P, int w, int h,
+                      Lens* L) {
   if (!K || !P || (n_dist > 0 && !D)) return fail(BEVK_ERR_ARG, "null K/D/P");
   if (model != BEVK_MODEL_FISHEYE && model != BEVK_MODEL_PINHOLE) return fail(BEVK_ERR_ARG, "bad camera model %d", model);
   if (w <= 0 || h <= 0) return fail(BEVK_ERR_ARG, "bad map size %dx%d", w, h);
-  memset(cm, 0, sizeof *cm);
-  if (!inv3(P, cm->iR)) return fail(BEVK_ERR_ARG, "P is singular");
-  const int want = model == BEVK_MODEL_FISHEYE ? 4 : 5;
-  for (int i = 0; i < want && i < n_dist; ++i) cm->k[i] = D[i];
-  cm->fx = K[0]; cm->fy = K[4]; cm->cx = K[2]; cm->cy = K[5];
-  cm->model = model; cm->w = w; cm->h = h;
+  switch (lens_model(model, K, D, n_dist, R, P, w, h, &L->cm, &L->lx, &L->full)) {
+    case LENS_BAD_COUNT:
+      return fail(BEVK_ERR_ARG, model == BEVK_MODEL_FISHEYE ? "fisheye D has %d coefficients, cv2 takes 4 (or 0)"
+                                                           : "pinhole D has %d coefficients, cv2 takes 0, 4, 5, 8, 12 or 14", n_dist);
+    case LENS_SINGULAR: return fail(BEVK_ERR_ARG, R ? "P * R is singular" : "P is singular");
+  }
   return BEVK_OK;
 }
+
+// The D of the entry points that take no R (bevk_undistort_map, bevk_undistorter_set, bevk_bev_set_camera), as they have
+// always read it: a pinhole D of 8, 12 or 14 coefficients in full, the first 5 (zero-padded) of any other count; a
+// fisheye D's first 4.
+struct LegacyDist {
+  double d[14] = {};
+  const double* D;
+  int n;
+  LegacyDist(int model, const double* src, int n_dist) : D(src), n(n_dist) {
+    if (dist_count_ok(model, n_dist) || (n_dist > 0 && !src)) return;   // a count cv2 takes, or a null D: as given
+    n = model == BEVK_MODEL_FISHEYE ? 4 : 5;
+    if (n_dist > 0) memcpy(d, src, sizeof(double) * std::min(n, n_dist));
+    D = d;
+  }
+};
 
 static int make_homog(const double* H, Homog* hm) {
   if (!H) return fail(BEVK_ERR_ARG, "null H");
@@ -134,7 +157,7 @@ static dim3 grid2d(int w, int h) { return dim3((w + 31) / 32, (h + 7) / 8); }
 // ------------------------------------------------------------------ context
 struct Undistorter {
   bool valid = false, fused = false;
-  CamModel cm;
+  Lens lens;
   DevBuf map1, map2;
   DevBuf xs;                      // cm.xs of a fused fisheye slot
 };
@@ -156,6 +179,7 @@ struct bevk_ctx {
   long long launches = 0;
   DevBuf s_src, s_dst, s_m1, s_m2, s_o1, s_o2;   // scratch for the host-pointer entry points
   DevBuf s_xs;                                   // cm.xs of bevk_undistort_map and bevk_bev_set_camera
+  DevBuf s_rays;                                 // lx.rays of a map build whose fisheye rays depend on the row
   DevBuf d_wtab;                                 // INTER_CUBIC and INTER_LANCZOS4 weight tables (build_interp_tabs)
   Undistorter und[8];
   // BEV engine
@@ -406,13 +430,28 @@ int bevk_host_free(void* p) {
 }
 
 // ------------------------------------------------------------------ K1
-// k_undistort_map of cm into the pair (m1, m2): cm.w x cm.h entries
-static int build_map(bevk_ctx* c, const CamModel& cm, DevBuf& m1, DevBuf& m2) {
+// k_undistort_map of L into the pair (m1, m2): cm.w x cm.h entries.  A fisheye whose rays depend on the row walks them into
+// scratch first (k_walk_rays), as cv2 walks each row: 24 bytes per map entry (126 MB at 2560 x 2048), freed again once the
+// map is built, so that a ctx does not hold it between set-ups.
+static int build_map(bevk_ctx* c, Lens L, DevBuf& m1, DevBuf& m2) {
+  const CamModel& cm = L.cm;
   const size_t n = (size_t)cm.w * cm.h;
   RET(m1.ensure(n * 4));
   RET(m2.ensure(n * 2));
-  k_undistort_map<<<grid2d(cm.w, cm.h), 256, 0, c->stream>>>(cm, m1.as<short2>(), m2.as<unsigned short>());
+  if (fisheye_walks(cm, L.full)) {
+    if (c->capturing) return fail(BEVK_ERR_ARG, "a camera model cannot be set up inside a graph capture");
+    RET(c->s_rays.ensure(n * 3 * sizeof(double)));
+    k_walk_rays<<<(cm.h + 127) / 128, 128, 0, c->stream>>>(cm, c->s_rays.as<double>());
+    LAUNCHED(c);
+    L.lx.rays = c->s_rays.as<double>();
+  }
+  if (L.full) k_undistort_map<1><<<grid2d(cm.w, cm.h), 256, 0, c->stream>>>(cm, L.lx, m1.as<short2>(), m2.as<unsigned short>());
+  else k_undistort_map<0><<<grid2d(cm.w, cm.h), 256, 0, c->stream>>>(cm, L.lx, m1.as<short2>(), m2.as<unsigned short>());
   LAUNCHED(c);
+  if (L.lx.rays) {   // the map kernel reads the rays: wait for it before the scratch goes
+    CU(cudaStreamSynchronize(c->stream));
+    c->s_rays.release();
+  }
   return BEVK_OK;
 }
 
@@ -424,15 +463,21 @@ static int download_maps(bevk_ctx* c, const void* m1, const void* m2, size_t n, 
   return BEVK_OK;
 }
 
-int bevk_undistort_map(bevk_ctx* c, int model, const double K[9], const double* D, int n_dist, const double P[9], int w,
-                       int h, int16_t* map1, uint16_t* map2) {
+int bevk_undistort_rectify_map(bevk_ctx* c, int model, const double K[9], const double* D, int n_dist, const double* R,
+                               const double P[9], int w, int h, int16_t* map1, uint16_t* map2) {
   RET(use(c));
   if (!map1 || !map2) return fail(BEVK_ERR_ARG, "null output map");
-  CamModel cm;
-  RET(make_model(model, K, D, n_dist, P, w, h, &cm));
-  RET(attach_xs_table(c, c->s_xs, &cm));
-  RET(build_map(c, cm, c->s_m1, c->s_m2));
+  Lens L;
+  RET(make_model(model, K, D, n_dist, R, P, w, h, &L));
+  RET(attach_xs_table(c, c->s_xs, &L.cm));
+  RET(build_map(c, L, c->s_m1, c->s_m2));
   return download_maps(c, c->s_m1.p, c->s_m2.p, (size_t)w * h, map1, map2);
+}
+
+int bevk_undistort_map(bevk_ctx* c, int model, const double K[9], const double* D, int n_dist, const double P[9], int w,
+                       int h, int16_t* map1, uint16_t* map2) {
+  const LegacyDist d(model, D, n_dist);
+  return bevk_undistort_rectify_map(c, model, K, d.D, d.n, nullptr, P, w, h, map1, map2);
 }
 
 // ------------------------------------------------------------------ image operations
@@ -470,6 +515,7 @@ constexpr int OP_RESIZE = 4;   // ImageOp::mode after the gathers' MODE 0..3
 
 struct ImageOp {
   int mode = 0;                     // the gathers' MODE (0 maps, 1 camera model, 2 homography, 3 affine) or OP_RESIZE
+  bool lens = false;                // MODE 1: the camera needs the LENS = 1 instances (lens_model)
   int interp = 0;                   // a gather's interpolation after gather_interp; a resize's body (resize_kind)
   GatherArgs g{};                   // a gather's maps, camera model or inverse matrix
   ResizeArgs r{};                   // a resize's scales
@@ -487,18 +533,18 @@ static Args with_frames(Args a, const ImageBatch& b) {
   return a;
 }
 
-template <int MODE>
+template <int MODE, int LENS>
 static void gather(bevk_ctx* c, const GatherArgs& a, int channels, int interp, bool words, unsigned gz) {
   if (words) {
     // 4 output pixels per thread, 32-bit tap loads and 12-byte stores
     const dim3 g4((a.dw / 4 + 31) / 32, (a.dh + 7) / 8, gz);
-    if (a.n == 1) k_gather4<MODE, 1><<<g4, 256, 0, c->stream>>>(a);
-    else k_gather4<MODE, GATHER_NB><<<g4, 256, 0, c->stream>>>(a);
+    if (a.n == 1) k_gather4<MODE, 1, LENS><<<g4, 256, 0, c->stream>>>(a);
+    else k_gather4<MODE, GATHER_NB, LENS><<<g4, 256, 0, c->stream>>>(a);
     return;
   }
   const dim3 g((a.dw + 31) / 32, (a.dh + 7) / 8, gz);
-#define GO(C, L) k_gather<MODE, C, L><<<g, 256, 0, c->stream>>>(a)
-#define TAPS(C, KS) k_gather_taps<MODE, C, KS><<<g, 256, 0, c->stream>>>(a, wt)
+#define GO(C, L) k_gather<MODE, C, L, LENS><<<g, 256, 0, c->stream>>>(a)
+#define TAPS(C, KS) k_gather_taps<MODE, C, KS, LENS><<<g, 256, 0, c->stream>>>(a, wt)
   if (interp == BEVK_INTER_CUBIC || interp == BEVK_INTER_LANCZOS4) {
     const short* wt = c->d_wtab.as<short>() + (interp == BEVK_INTER_CUBIC ? 0 : INTERP_TAB_LANCZOS4);
     if (interp == BEVK_INTER_CUBIC) {
@@ -545,10 +591,13 @@ static int launch(bevk_ctx* c, const ImageOp& op, const ImageBatch& b, int chann
     if (op.mode != OP_RESIZE) {
       const GatherArgs a = with_frames(op.g, p);
       switch (op.mode) {
-        case 0: gather<0>(c, a, channels, op.interp, words, gz); break;
-        case 1: gather<1>(c, a, channels, op.interp, words, gz); break;
-        case 2: gather<2>(c, a, channels, op.interp, words, gz); break;
-        default: gather<3>(c, a, channels, op.interp, words, gz);
+        case 0: gather<0, 0>(c, a, channels, op.interp, words, gz); break;
+        case 1:
+          if (op.lens) gather<1, 1>(c, a, channels, op.interp, words, gz);
+          else gather<1, 0>(c, a, channels, op.interp, words, gz);
+          break;
+        case 2: gather<2, 0>(c, a, channels, op.interp, words, gz); break;
+        default: gather<3, 0>(c, a, channels, op.interp, words, gz);
       }
     } else {
       const ResizeArgs a = with_frames(op.r, p);
@@ -586,9 +635,9 @@ static int undistort_op(bevk_ctx* c, int slot, int interp, ImageOp* op) {
   const Undistorter& u = c->und[slot];
   op->mode = u.fused ? 1 : 0;
   op->interp = interp;
-  if (u.fused) op->g.cm = u.cm;
+  if (u.fused) { op->g.cm = u.lens.cm; op->g.lx = u.lens.lx; op->lens = u.lens.full; }
   else { op->g.map1 = u.map1.as<short2>(); op->g.map2 = u.map2.as<unsigned short>(); }
-  op->slot = slot; op->dw = u.cm.w; op->dh = u.cm.h;
+  op->slot = slot; op->dw = u.lens.cm.w; op->dh = u.lens.cm.h;
   return BEVK_OK;
 }
 
@@ -741,24 +790,34 @@ int bevk_remap(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride,
 }
 
 // ------------------------------------------------------------------ cached-map undistortion
-int bevk_undistorter_set(bevk_ctx* c, int slot, int model, const double K[9], const double* D, int n_dist,
-                         const double P[9], int dw, int dh, int fused) {
+int bevk_undistorter_set_rectify(bevk_ctx* c, int slot, int model, const double K[9], const double* D, int n_dist,
+                                 const double* R, const double P[9], int dw, int dh, int fused) {
   RET(use(c));
   if (slot < 0 || slot >= 8) return fail(BEVK_ERR_ARG, "slot %d out of range", slot);
   Undistorter& u = c->und[slot];
   u.valid = false;
-  RET(make_model(model, K, D, n_dist, P, dw, dh, &u.cm));
+  Lens& L = u.lens;
+  RET(make_model(model, K, D, n_dist, R, P, dw, dh, &L));
   u.fused = fused != 0;
+  if (u.fused && fisheye_walks(L.cm, L.full))
+    return fail(BEVK_ERR_UNSUPPORTED, "a fused fisheye slot cannot follow cv2's running ray sums when R makes the rays depend "
+                "on the row; set up a map-resident slot (fused = 0) for this camera");
   if (u.fused) {   // the gathers evaluate the model per pixel: the slot keeps its column table
-    RET(attach_xs_table(c, u.xs, &u.cm));
-  } else {         // the table is read once, by the map build, from scratch
+    RET(attach_xs_table(c, u.xs, &L.cm));
+  } else {         // the table (and walked rays) are read once, by the map build, from scratch
     u.xs.release();
-    RET(attach_xs_table(c, c->s_xs, &u.cm));
-    RET(build_map(c, u.cm, u.map1, u.map2));
-    u.cm.xs = nullptr;
+    RET(attach_xs_table(c, c->s_xs, &L.cm));
+    RET(build_map(c, L, u.map1, u.map2));
+    L.cm.xs = nullptr;
   }
   u.valid = true;
   return BEVK_OK;
+}
+
+int bevk_undistorter_set(bevk_ctx* c, int slot, int model, const double K[9], const double* D, int n_dist,
+                         const double P[9], int dw, int dh, int fused) {
+  const LegacyDist d(model, D, n_dist);
+  return bevk_undistorter_set_rectify(c, slot, model, K, d.D, d.n, nullptr, P, dw, dh, fused);
 }
 
 int bevk_undistorter_maps(bevk_ctx* c, int slot, int16_t* map1, uint16_t* map2) {
@@ -767,8 +826,9 @@ int bevk_undistorter_maps(bevk_ctx* c, int slot, int16_t* map1, uint16_t* map2) 
   if (!map1 || !map2) return fail(BEVK_ERR_ARG, "null output map");
   Undistorter& u = c->und[slot];
   const bool resident = !u.fused;   // a fused slot has no resident map: evaluate into scratch
-  if (!resident) RET(build_map(c, u.cm, c->s_m1, c->s_m2));
-  return download_maps(c, resident ? u.map1.p : c->s_m1.p, resident ? u.map2.p : c->s_m2.p, (size_t)u.cm.w * u.cm.h, map1, map2);
+  if (!resident) RET(build_map(c, u.lens, c->s_m1, c->s_m2));
+  return download_maps(c, resident ? u.map1.p : c->s_m1.p, resident ? u.map2.p : c->s_m2.p, (size_t)u.lens.cm.w * u.lens.cm.h,
+                       map1, map2);
 }
 
 int bevk_undistort(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
@@ -867,7 +927,7 @@ int bevk_warp_maps(bevk_ctx* c, const int16_t* map1, const uint16_t* map2, int s
   CU(cudaMemcpyAsync(c->s_m2.p, map2, ns * 2, cudaMemcpyHostToDevice, c->stream));
   a.in1 = c->s_m1.as<short2>(); a.in2 = c->s_m2.as<unsigned short>(); a.sw = sw; a.sh = sh;
   a.out1 = c->s_o1.as<short2>(); a.out2 = c->s_o2.as<unsigned short>(); a.dw = dw; a.dh = dh;
-  k_warp_maps<0><<<grid2d(dw, dh), 256, 0, c->stream>>>(a);
+  k_warp_maps<0, 0><<<grid2d(dw, dh), 256, 0, c->stream>>>(a);
   LAUNCHED(c);
   return download_maps(c, c->s_o1.p, c->s_o2.p, nd, out1, out2);
 }
@@ -899,12 +959,14 @@ static int need_plan(bevk_ctx* c) {
   return c->planned ? BEVK_OK : fail(BEVK_ERR_ARG, "bevk_bev_finalize not called");
 }
 
-int bevk_bev_set_camera(bevk_ctx* c, int cam, const double K[9], const double D[4], const double P[9], int und_w,
-                        int und_h, const double H[9]) {
+int bevk_bev_set_camera_model(bevk_ctx* c, int cam, int model, const double K[9], const double* D, int n_dist,
+                              const double P[9], int und_w, int und_h, const double H[9]) {
   RET(use(c));
   RET(need_cam(c, cam));
   WarpMapsArgs a{};
-  RET(make_model(BEVK_MODEL_FISHEYE, K, D, 4, P, und_w, und_h, &a.cm));
+  Lens L;
+  RET(make_model(model, K, D, n_dist, nullptr, P, und_w, und_h, &L));
+  a.cm = L.cm; a.lx = L.lx;
   RET(attach_xs_table(c, c->s_xs, &a.cm));
   RET(make_homog(H, &a.hm));
   BevCam& k = c->cam[cam];
@@ -913,11 +975,17 @@ int bevk_bev_set_camera(bevk_ctx* c, int cam, const double K[9], const double D[
   RET(k.map2.ensure(n * 2));
   a.sw = und_w; a.sh = und_h;
   a.out1 = k.map1.as<short2>(); a.out2 = k.map2.as<unsigned short>(); a.dw = c->BW; a.dh = c->BH;
-  k_warp_maps<1><<<grid2d(c->BW, c->BH), 256, 0, c->stream>>>(a);
+  if (L.full) k_warp_maps<1, 1><<<grid2d(c->BW, c->BH), 256, 0, c->stream>>>(a);
+  else k_warp_maps<1, 0><<<grid2d(c->BW, c->BH), 256, 0, c->stream>>>(a);
   LAUNCHED(c);
   k.has_maps = true;
   c->planned = false;
   return BEVK_OK;
+}
+
+int bevk_bev_set_camera(bevk_ctx* c, int cam, const double K[9], const double D[4], const double P[9], int und_w,
+                        int und_h, const double H[9]) {
+  return bevk_bev_set_camera_model(c, cam, BEVK_MODEL_FISHEYE, K, D, 4, P, und_w, und_h, H);
 }
 
 int bevk_bev_set_maps(bevk_ctx* c, int cam, const int16_t* map1, const uint16_t* map2) {

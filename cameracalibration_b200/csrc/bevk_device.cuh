@@ -7,7 +7,9 @@
 // bilinear), A3 (warpPerspective coordinates), A9 (8-bit HSV round trip).
 #pragma once
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
+#include <string.h>
 
 namespace bevk {
 
@@ -29,12 +31,20 @@ struct Frames {
 };
 
 struct CamModel {      // cv2.fisheye / cv2 initUndistortRectifyMap inputs, pre-digested on the host
-  double iR[9];        // inv(P * R), R = I
+  double iR[9];        // inv(P * R)
   double k[5];         // fisheye: k1..k4 ; pinhole: k1,k2,p1,p2,k3
   double fx, fy, cx, cy;
   int model;           // BEVK_MODEL_*
   int w, h;            // size of the undistorted (destination) frame
   const double* xs;    // fisheye with row-independent rays (xs_table_applies): OpenCV's running _x of column j; else null
+};
+
+// What cv2's full lens models add to CamModel.  Only the LENS = 1 instances of the kernels receive it (lens_model), so
+// that the 4-coefficient fisheye and the 5-coefficient pinhole keep the instances they always ran.
+struct LensExt {
+  double k[7];          // pinhole: k4 k5 k6 (rational), s1 s2 s3 s4 (thin prism); zeros when D has fewer coefficients
+  double T[9];          // pinhole: computeTiltProjectionMatrix(tauX, tauY); the identity without tilt
+  const double* rays;   // fisheye map builds whose rays depend on the row: cv2's running _x, _y, _w ([3][h][w], walk_rays)
 };
 
 struct Homog { double M[9]; };   // inv(H), as cv2.warpPerspective computes it
@@ -113,16 +123,51 @@ inline void fill_xs_table(const CamModel& c, double* xs) {
   }
 }
 
-// A1 / A11: source-image position (u,v) of undistorted pixel (j,i).
-__host__ __device__ __forceinline__ void undistort_point(const CamModel& c, int j, int i, double& u, double& v) {
+// A1 with a general R: cv2.fisheye.initUndistortRectifyMap's rays of row i, _x = i*iR01 + iR02 then _x += iR00 per
+// column (and the same for _y, _w), into the planes of rays ([3][h][w]).  The sums are serial along the row, so the map
+// builds of a camera whose rays depend on the row run this once per row first (k_walk_rays) and read the planes.
+__host__ __device__ __forceinline__ void walk_rays(const CamModel& c, int i, double* rays) {
+  const size_t n = (size_t)c.w * c.h, q = (size_t)i * c.w;
+  const double di = (double)i;
+  double _x = dadd(dmul(di, c.iR[1]), c.iR[2]), _y = dadd(dmul(di, c.iR[4]), c.iR[5]), _w = dadd(dmul(di, c.iR[7]), c.iR[8]);
+  for (int j = 0; j < c.w; ++j) {
+    rays[q + j] = _x; rays[n + q + j] = _y; rays[2 * n + q + j] = _w;
+    _x = dadd(_x, c.iR[0]); _y = dadd(_y, c.iR[3]); _w = dadd(_w, c.iR[6]);
+  }
+}
+
+// The ray (_x, _y, _w) of undistorted pixel (j,i) that undistort_point<LENS> projects: the walked rays of lx when it
+// has them (LENS = 1), else the column table's _x or the direct form.  tests/host/lens_models.cu reads it.
+template <int LENS>
+__host__ __device__ __forceinline__ void camera_ray(const CamModel& c, const LensExt& lx, int j, int i, double& _x, double& _y,
+                                                    double& _w) {
   const double dj = (double)j, di = (double)i;
+  if (LENS && lx.rays) {
+    const size_t n = (size_t)c.w * c.h, q = (size_t)i * c.w + j;
 #ifdef __CUDA_ARCH__
-  const double _x = c.xs ? __ldg(c.xs + j) : dadd(dmul(dj, c.iR[0]), dadd(dmul(di, c.iR[1]), c.iR[2]));
+    _x = __ldg(lx.rays + q); _y = __ldg(lx.rays + n + q); _w = __ldg(lx.rays + 2 * n + q);
 #else
-  const double _x = c.xs ? c.xs[j] : dadd(dmul(dj, c.iR[0]), dadd(dmul(di, c.iR[1]), c.iR[2]));
+    _x = lx.rays[q]; _y = lx.rays[n + q]; _w = lx.rays[2 * n + q];
 #endif
-  const double _y = dadd(dmul(dj, c.iR[3]), dadd(dmul(di, c.iR[4]), c.iR[5]));
-  const double _w = dadd(dmul(dj, c.iR[6]), dadd(dmul(di, c.iR[7]), c.iR[8]));
+  } else {
+#ifdef __CUDA_ARCH__
+    _x = c.xs ? __ldg(c.xs + j) : dadd(dmul(dj, c.iR[0]), dadd(dmul(di, c.iR[1]), c.iR[2]));
+#else
+    _x = c.xs ? c.xs[j] : dadd(dmul(dj, c.iR[0]), dadd(dmul(di, c.iR[1]), c.iR[2]));
+#endif
+    _y = dadd(dmul(dj, c.iR[3]), dadd(dmul(di, c.iR[4]), c.iR[5]));
+    _w = dadd(dmul(dj, c.iR[6]), dadd(dmul(di, c.iR[7]), c.iR[8]));
+  }
+}
+
+// A1 / A11: source-image position (u,v) of undistorted pixel (j,i).  LENS = 0 is the 4-coefficient fisheye and the
+// 5-coefficient pinhole; LENS = 1 adds what lx holds: cv2's rational denominator, thin-prism terms and tilt, and the
+// fisheye's walked rays.  With lx's coefficients zero, T the identity and no rays, LENS = 1 computes LENS = 0's values
+// (a division by 1, adds of 0, a multiply by 1).
+template <int LENS>
+__host__ __device__ __forceinline__ void undistort_point(const CamModel& c, const LensExt& lx, int j, int i, double& u, double& v) {
+  double _x, _y, _w;
+  camera_ray<LENS>(c, lx, j, i, _x, _y, _w);
   if (c.model == 0) {  // equidistant fisheye
     if (_w <= 0) {
       const double inf = dinf();
@@ -139,18 +184,97 @@ __host__ __device__ __forceinline__ void undistort_point(const CamModel& c, int 
     const double s = (r == 0) ? 1.0 : ddiv(thd, r);
     u = dadd(dmul(dmul(c.fx, x), s), c.cx);
     v = dadd(dmul(dmul(c.fy, y), s), c.cy);
-  } else {             // pinhole, k1 k2 p1 p2 k3
+  } else {             // pinhole, k1 k2 p1 p2 k3 (LENS: k4 k5 k6 s1 s2 s3 s4 tauX tauY)
     const double w = ddiv(1.0, _w), x = dmul(_x, w), y = dmul(_y, w);
     const double x2 = dmul(x, x), y2 = dmul(y, y);
     const double r2 = dadd(x2, y2), _2xy = dmul(dmul(2.0, x), y);
     const double k1 = c.k[0], k2 = c.k[1], p1 = c.k[2], p2 = c.k[3], k3 = c.k[4];
-    const double kr = dadd(1.0, dmul(dadd(dmul(dadd(dmul(k3, r2), k2), r2), k1), r2));
-    const double xd = dadd(dadd(dmul(x, kr), dmul(p1, _2xy)), dmul(p2, dadd(r2, dmul(2.0, x2))));
-    const double yd = dadd(dadd(dmul(y, kr), dmul(p1, dadd(r2, dmul(2.0, y2)))), dmul(p2, _2xy));
-    u = dadd(dmul(c.fx, xd), c.cx);
-    v = dadd(dmul(c.fy, yd), c.cy);
+    double kr = dadd(1.0, dmul(dadd(dmul(dadd(dmul(k3, r2), k2), r2), k1), r2));
+    if (LENS) kr = ddiv(kr, dadd(1.0, dmul(dadd(dmul(dadd(dmul(lx.k[2], r2), lx.k[1]), r2), lx.k[0]), r2)));
+    double xd = dadd(dadd(dmul(x, kr), dmul(p1, _2xy)), dmul(p2, dadd(r2, dmul(2.0, x2))));
+    double yd = dadd(dadd(dmul(y, kr), dmul(p1, dadd(r2, dmul(2.0, y2)))), dmul(p2, _2xy));
+    if (LENS) {
+      xd = dadd(dadd(xd, dmul(lx.k[3], r2)), dmul(dmul(lx.k[4], r2), r2));
+      yd = dadd(dadd(yd, dmul(lx.k[5], r2)), dmul(dmul(lx.k[6], r2), r2));
+      const double* T = lx.T;   // cv2: vecTilt = matTilt * (xd, yd, 1), invProj = vecTilt(2) ? 1 / vecTilt(2) : 1
+      const double vx = dadd(dadd(dmul(T[0], xd), dmul(T[1], yd)), T[2]);
+      const double vy = dadd(dadd(dmul(T[3], xd), dmul(T[4], yd)), T[5]);
+      const double vz = dadd(dadd(dmul(T[6], xd), dmul(T[7], yd)), T[8]);
+      const double ip = vz != 0. ? ddiv(1.0, vz) : 1.0;
+      u = dadd(dmul(dmul(c.fx, ip), vx), c.cx);
+      v = dadd(dmul(dmul(c.fy, ip), vy), c.cy);
+    } else {
+      u = dadd(dmul(c.fx, xd), c.cx);
+      v = dadd(dmul(c.fy, yd), c.cy);
+    }
   }
 }
+
+__host__ __device__ __forceinline__ void undistort_point(const CamModel& c, int j, int i, double& u, double& v) {
+  const LensExt none{};
+  undistort_point<0>(c, none, j, i, u, v);
+}
+
+// ---- the camera set-up of every entry point (host only; tests/host/lens_models.cu runs it against cv2)
+// A 3x3 product as cv::Matx forms P * R and the tilt matrix: entry (r, c) = (a_r0 b_0c + a_r1 b_1c) + a_r2 b_2c.
+inline void mul3(const double* A, const double* B, double* C) {
+  for (int r = 0; r < 3; ++r)
+    for (int k = 0; k < 3; ++k)
+      C[r * 3 + k] = dadd(dadd(dmul(A[r * 3], B[k]), dmul(A[r * 3 + 1], B[3 + k])), dmul(A[r * 3 + 2], B[6 + k]));
+}
+inline bool is_identity3(const double* M) {
+  for (int i = 0; i < 9; ++i)
+    if (M[i] != (i % 4 == 0 ? 1. : 0.)) return false;
+  return true;
+}
+// cv::detail::computeTiltProjectionMatrix(tauX, tauY): projZ(Ry * Rx) * (Ry * Rx)
+inline void tilt_matrix(double tx, double ty, double* T) {
+  const double ctx = cos(tx), stx = sin(tx), cty = cos(ty), sty = sin(ty);
+  const double Rx[9] = {1, 0, 0, 0, ctx, stx, 0, -stx, ctx}, Ry[9] = {cty, 0, -sty, 0, 1, 0, sty, 0, cty};
+  double Rxy[9];
+  mul3(Ry, Rx, Rxy);
+  const double Pz[9] = {Rxy[8], 0, -Rxy[2], 0, Rxy[8], -Rxy[5], 0, 0, 1};
+  mul3(Pz, Rxy, T);
+}
+
+// D lengths cv2.initUndistortRectifyMap (pinhole) and cv2.fisheye.initUndistortRectifyMap accept (an empty D is zeros)
+inline bool dist_count_ok(int model, int n) {
+  return model == 0 ? (n == 0 || n == 4) : (n == 0 || n == 4 || n == 5 || n == 8 || n == 12 || n == 14);
+}
+
+enum { LENS_OK = 0, LENS_BAD_COUNT = 1, LENS_SINGULAR = 2 };
+
+// cv2.initUndistortRectifyMap / cv2.fisheye.initUndistortRectifyMap's (K, D, R, P) as the kernels take them: iR =
+// inv(P * R) (R == null: inv(P)), k1..k5 in cm, the rest of a 8-, 12- or 14-coefficient D and the tilt matrix in lx.
+// *lens says whether the camera needs the LENS = 1 instances: a pinhole with any of k4..k6, s1..s4, tauX, tauY non-zero,
+// or a fisheye whose rotated rays depend on the row (fisheye_walks).  Any other camera, R included, computes the same
+// bytes in the LENS = 0 instances.  The caller attaches cm.xs and lx.rays.
+inline int lens_model(int model, const double* K, const double* D, int n_dist, const double* R, const double* P, int w, int h,
+                      CamModel* cm, LensExt* lx, bool* lens) {
+  memset(cm, 0, sizeof *cm);
+  memset(lx, 0, sizeof *lx);
+  if (!dist_count_ok(model, n_dist)) return LENS_BAD_COUNT;
+  const bool rotated = R && !is_identity3(R);
+  double PR[9];
+  if (rotated) mul3(P, R, PR);
+  if (!inv3(rotated ? PR : P, cm->iR)) return LENS_SINGULAR;
+  for (int i = 0; i < n_dist && i < (model == 0 ? 4 : 5); ++i) cm->k[i] = D[i];
+  for (int i = 5; i < n_dist && i < 12; ++i) lx->k[i - 5] = D[i];
+  tilt_matrix(n_dist == 14 ? D[12] : 0., n_dist == 14 ? D[13] : 0., lx->T);
+  cm->fx = K[0]; cm->fy = K[4]; cm->cx = K[2]; cm->cy = K[5];
+  cm->model = model; cm->w = w; cm->h = h;
+  if (model == 0) {
+    *lens = rotated && !xs_table_applies(*cm);
+  } else {
+    bool extra = !is_identity3(lx->T);
+    for (double k : lx->k) extra = extra || k != 0.;
+    *lens = extra;
+  }
+  return LENS_OK;
+}
+
+// A LENS = 1 fisheye: its map builds read walked rays, and a fused gather cannot walk them per pixel.
+inline bool fisheye_walks(const CamModel& cm, bool lens) { return lens && cm.model == 0; }
 
 // CV_16SC2 + CV_16UC1 quantisation of (u,v): map1 = (iu>>5, iv>>5) as int16 (wrapping
 // cast), map2 = (iv&31)*32 + (iu&31).

@@ -62,7 +62,7 @@ __host__ __device__ __forceinline__ unsigned gather_px(const uint8_t* __restrict
 // (tests/host/undistort_stack.cu).  Requirements checked by the host (gather4_ok in bevk_api.cu): channels == 3,
 // INTER_LINEAR, dw % 4 == 0; src, dst, both row pitches and (n > 1) both image strides multiples of 4; spitch * sh < 2^31
 // (gather_px's 32-bit offsets within a frame).
-template <int MODE, int NB, class LD = Ldg>
+template <int MODE, int NB, class LD = Ldg, int LENS = 0>
 __host__ __device__ __forceinline__ void gather4_frames(const GatherArgs& a, int x4, int y, int f0) {
   short mx[4], my[4];
   unsigned short fr[4];
@@ -89,7 +89,7 @@ __host__ __device__ __forceinline__ void gather4_frames(const GatherArgs& a, int
     } else {
       if (MODE == 1) {
         double u, v;
-        undistort_point(a.cm, x4 + q, y, u, v);
+        undistort_point<LENS>(a.cm, a.lx, x4 + q, y, u, v);
         quantise_uv(u, v, mx[q], my[q], fr[q], pack_saturates(a.cm.model, x4 + q, a.cm.w));
       }
       sx[q] = mx[q]; sy[q] = my[q];
@@ -117,12 +117,12 @@ __host__ __device__ __forceinline__ void gather4_frames(const GatherArgs& a, int
 
 // NB = frames per thread: GATHER_NB over a batch, 1 for a single frame (n = 1 then compiles to the single-frame body
 // and keeps its register count and occupancy; the batch form needs about twice the registers).
-template <int MODE, int NB>
+template <int MODE, int NB, int LENS>
 __global__ void __launch_bounds__(256) k_gather4(GatherArgs a) {
   const int x4 = (blockIdx.x * 32 + (threadIdx.x & 31)) * 4;
   const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x4 >= a.dw || y >= a.dh) return;
-  gather4_frames<MODE, NB>(a, x4, y, blockIdx.z * NB);
+  gather4_frames<MODE, NB, Ldg, LENS>(a, x4, y, blockIdx.z * NB);
 }
 
 }  // namespace bevk

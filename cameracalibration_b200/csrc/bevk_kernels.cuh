@@ -21,19 +21,26 @@ constexpr int BEVK_MAX_CAMERAS_K = 8;   // == BEVK_MAX_CAMERAS in include/bevk.h
 // ---------------------------------------------------------------------------------
 // K1
 // ---------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_undistort_map(CamModel cm, short2* __restrict__ map1,
+template <int LENS>
+__global__ void __launch_bounds__(256) k_undistort_map(CamModel cm, LensExt lx, short2* __restrict__ map1,
                                                        unsigned short* __restrict__ map2) {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31);
   const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= cm.w || y >= cm.h) return;
   double u, v;
-  undistort_point(cm, x, y, u, v);
+  undistort_point<LENS>(cm, lx, x, y, u, v);
   short mx, my;
   unsigned short fr;
   quantise_uv(u, v, mx, my, fr, pack_saturates(cm.model, x, cm.w));
   const size_t i = (size_t)y * cm.w + x;
   map1[i] = make_short2(mx, my);
   map2[i] = fr;
+}
+
+// K1 set-up of a fisheye whose rays depend on the row (LensExt::rays): one thread walks one row.
+__global__ void __launch_bounds__(128) k_walk_rays(CamModel cm, double* __restrict__ rays) {
+  const int i = blockIdx.x * 128 + threadIdx.x;
+  if (i < cm.h) walk_rays(cm, i, rays);
 }
 
 // ---------------------------------------------------------------------------------
@@ -48,6 +55,7 @@ struct GatherArgs {
   uint8_t* dst; int dw, dh; long long dpitch;
   const short2* map1; const unsigned short* map2;
   CamModel cm;
+  LensExt lx;                            // MODE 1 with LENS = 1 only
   Homog hm;
   int n; long long sistride, distride;   // frames, and the 64-bit image strides of source and destination
 };
@@ -84,7 +92,8 @@ __host__ __device__ __forceinline__ void load_px(const uint8_t* __restrict__ src
 
 // One thread of k_gather: output pixel (x, y) of frames [f0, min(n, f0 + GATHER_NB)).  Host-capable, so that
 // tests/host/undistort_stack.cu runs the same frame loop and addressing on a CPU.
-template <int MODE, int C, int LINEAR>
+// LENS (MODE 1): the camera model's instance, undistort_point<LENS>.
+template <int MODE, int C, int LINEAR, int LENS = 0>
 __host__ __device__ __forceinline__ void gather_frames(const GatherArgs& a, int x, int y, int f0) {
   int sx, sy, fx = 0, fy = 0;
   if (MODE >= 2) {
@@ -108,7 +117,7 @@ __host__ __device__ __forceinline__ void gather_frames(const GatherArgs& a, int 
       fr = have_frac ? a.map2[i] : 0;
     } else {
       double u, v;
-      undistort_point(a.cm, x, y, u, v);
+      undistort_point<LENS>(a.cm, a.lx, x, y, u, v);
       quantise_uv(u, v, mx, my, fr, pack_saturates(a.cm.model, x, a.cm.w));
     }
     sx = mx; sy = my;
@@ -138,19 +147,19 @@ __host__ __device__ __forceinline__ void gather_frames(const GatherArgs& a, int 
   }
 }
 
-template <int MODE, int C, int LINEAR>
+template <int MODE, int C, int LINEAR, int LENS>
 __global__ void __launch_bounds__(256) k_gather(GatherArgs a) {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31);
   const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= a.dw || y >= a.dh) return;
-  gather_frames<MODE, C, LINEAR>(a, x, y, blockIdx.z * GATHER_NB);
+  gather_frames<MODE, C, LINEAR, LENS>(a, x, y, blockIdx.z * GATHER_NB);
 }
 
 // K3 / K4 with INTER_CUBIC (KS = 4) and INTER_LANCZOS4 (KS = 8): the source position is INTER_LINEAR's (map entry, camera
 // model, or warp_point at TAB scale), the map2 value picks a row of KS * KS int16 weights from wtab (bevk_interp.cuh,
 // 32 or 128 bytes read once per pixel through the read-only path), and the row and window serve up to GATHER_NB frames.
 // Host-capable, like gather_frames (tests/host/remap_interp.cu).
-template <int MODE, int C, int KS>
+template <int MODE, int C, int KS, int LENS = 0>
 __host__ __device__ __forceinline__ void gather_taps_frames(const GatherArgs& a, const short* __restrict__ wtab, int x, int y,
                                                             int f0) {
   int sx, sy;
@@ -170,7 +179,7 @@ __host__ __device__ __forceinline__ void gather_taps_frames(const GatherArgs& a,
       f = a.map2[i];
     } else {
       double u, v;
-      undistort_point(a.cm, x, y, u, v);
+      undistort_point<LENS>(a.cm, a.lx, x, y, u, v);
       quantise_uv(u, v, mx, my, f, pack_saturates(a.cm.model, x, a.cm.w));
     }
     sx = mx; sy = my;
@@ -196,12 +205,12 @@ __host__ __device__ __forceinline__ void gather_taps_frames(const GatherArgs& a,
   for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) taps_px<KS, C>(s, a.spitch, a.sw, a.sh, sx, sy, w, o);
 }
 
-template <int MODE, int C, int KS>
+template <int MODE, int C, int KS, int LENS>
 __global__ void __launch_bounds__(256) k_gather_taps(GatherArgs a, const short* __restrict__ wtab) {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31);
   const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= a.dw || y >= a.dh) return;
-  gather_taps_frames<MODE, C, KS>(a, wtab, x, y, blockIdx.z * GATHER_NB);
+  gather_taps_frames<MODE, C, KS, LENS>(a, wtab, x, y, blockIdx.z * GATHER_NB);
 }
 
 // ---------------------------------------------------------------------------------
@@ -211,12 +220,13 @@ __global__ void __launch_bounds__(256) k_gather_taps(GatherArgs a, const short* 
 struct WarpMapsArgs {
   const short2* in1; const unsigned short* in2; int sw, sh;   // FROM_MODEL=0
   CamModel cm;                                                // FROM_MODEL=1 (sw,sh = cm.w,cm.h)
+  LensExt lx;                                                 // FROM_MODEL=1 with LENS = 1 only
   Homog hm;
   short2* out1; unsigned short* out2; int dw, dh;
 };
 
 // One destination pixel of that warp (host-capable: tests/host/kernel_math.cu runs it on a CPU against cv2).
-template <int FROM_MODEL>
+template <int FROM_MODEL, int LENS = 0>
 __host__ __device__ __forceinline__ void warp_maps_pixel(const WarpMapsArgs& a, int x, int y, short& ox, short& oy,
                                                          unsigned short& of) {
   int X, Y;
@@ -235,7 +245,7 @@ __host__ __device__ __forceinline__ void warp_maps_pixel(const WarpMapsArgs& a, 
       unsigned short fr;
       if (FROM_MODEL) {
         double u, v;
-        undistort_point(a.cm, tx, ty, u, v);
+        undistort_point<LENS>(a.cm, a.lx, tx, ty, u, v);
         quantise_uv(u, v, mx, my, fr, pack_saturates(a.cm.model, tx, a.cm.w));
       } else {
         const size_t i = (size_t)ty * a.sw + tx;
@@ -258,14 +268,14 @@ __host__ __device__ __forceinline__ void warp_maps_pixel(const WarpMapsArgs& a, 
   of = (unsigned short)(fi < 0 ? 0 : (fi > 65535 ? 65535 : fi));
 }
 
-template <int FROM_MODEL>
+template <int FROM_MODEL, int LENS>
 __global__ void __launch_bounds__(256) k_warp_maps(WarpMapsArgs a) {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31);
   const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= a.dw || y >= a.dh) return;
   short ox, oy;
   unsigned short of;
-  warp_maps_pixel<FROM_MODEL>(a, x, y, ox, oy, of);
+  warp_maps_pixel<FROM_MODEL, LENS>(a, x, y, ox, oy, of);
   const size_t o = (size_t)y * a.dw + x;
   a.out1[o] = make_short2(ox, oy);
   a.out2[o] = of;

@@ -21,24 +21,39 @@ def _interp(flag: int) -> int:
     return flag
 
 
-def fisheye_init_undistort_rectify_map(K, D, P, size, ctx: L.Context | None = None):
-    """cv2.fisheye.initUndistortRectifyMap(K, D, eye(3), P, size, CV_16SC2)."""
-    return _undistort_map(L.MODEL_FISHEYE, K, D, P, size, ctx)
+def fisheye_init_undistort_rectify_map(K, D, P, size, ctx: L.Context | None = None, R=None):
+    """cv2.fisheye.initUndistortRectifyMap(K, D, R, P, size, CV_16SC2); R=None is eye(3)."""
+    return _undistort_map(L.MODEL_FISHEYE, K, D, P, size, ctx, R)
 
 
-def init_undistort_rectify_map(K, D, P, size, ctx: L.Context | None = None):
-    """cv2.initUndistortRectifyMap(K, D(k1,k2,p1,p2,k3), eye(3), P, size, CV_16SC2)."""
-    return _undistort_map(L.MODEL_PINHOLE, K, D, P, size, ctx)
+def init_undistort_rectify_map(K, D, P, size, ctx: L.Context | None = None, R=None):
+    """cv2.initUndistortRectifyMap(K, D, R, P, size, CV_16SC2) with D of 4, 5, 8, 12 or 14 coefficients (rational,
+    thin-prism and tilted models); R=None is eye(3)."""
+    return _undistort_map(L.MODEL_PINHOLE, K, D, P, size, ctx, R)
 
 
-def _undistort_map(model, K, D, P, size, ctx):
+def _rotation(R):
+    """double* of a 3x3 rectification rotation, or None (NULL: the identity)."""
+    if R is None:
+        return None
+    r = np.asarray(R, np.float64)
+    if r.shape != (3, 3):
+        raise L.BevkError(f"R must be a 3x3 matrix, got shape {r.shape}")
+    return L.dptr(r)
+
+
+def _undistort_map(model, K, D, P, size, ctx, R=None):
     ctx = ctx or L.default_context()
     w, h = int(size[0]), int(size[1])
     d = np.asarray(D, np.float64).reshape(-1)
     m1 = np.empty((h, w, 2), np.int16)
     m2 = np.empty((h, w), np.uint16)
-    L.check(ctx.lib.bevk_undistort_map(ctx.h, model, L.dptr(K), L.dptr(d), int(d.size), L.dptr(P), w, h,
-                                       L.vptr(m1), L.vptr(m2)))
+    if R is None:
+        L.check(ctx.lib.bevk_undistort_map(ctx.h, model, L.dptr(K), L.dptr(d), int(d.size), L.dptr(P), w, h,
+                                           L.vptr(m1), L.vptr(m2)))
+    else:
+        L.check(ctx.lib.bevk_undistort_rectify_map(ctx.h, model, L.dptr(K), L.dptr(d), int(d.size), _rotation(R), L.dptr(P),
+                                                   w, h, L.vptr(m1), L.vptr(m2)))
     return m1, m2
 
 
@@ -524,12 +539,16 @@ def luminance_balance(images, ctx: L.Context | None = None):
 class Undistorter:
     """Device-resident undistortion map (or fused camera model) + per-frame gather.
 
+    D: 4 fisheye coefficients, or 4, 5, 8, 12 or 14 pinhole ones (cv2's rational, thin-prism and tilted models).  R: a
+    rectification rotation (cv2.stereoRectify's R1 / R2), None for eye(3).  A fused fisheye whose rotated rays depend on
+    the row is refused (BevkError): cv2 walks those rays with running row sums, which only a map-resident slot follows.
+
     A bevk_ctx has 8 undistorter slots.  Each live Undistorter owns one slot of its ctx; the slot returns to the
     pool on close() / garbage collection, and a 9th live object on one ctx raises instead of silently taking over a
     slot another object still uses."""
 
     def __init__(self, K, D, P, size, model: str = "fisheye", fused: bool = False, ctx: L.Context | None = None,
-                 slot: int | None = None):
+                 slot: int | None = None, R=None):
         self.ctx = ctx or L.default_context()
         self.slot = None
         live = self.ctx.__dict__.setdefault("_und_slots", set())
@@ -551,8 +570,12 @@ class Undistorter:
         self.w, self.h = int(size[0]), int(size[1])
         d = np.asarray(D, np.float64).reshape(-1)
         m = L.MODEL_FISHEYE if model == "fisheye" else L.MODEL_PINHOLE
-        L.check(self.ctx.lib.bevk_undistorter_set(self.ctx.h, slot, m, L.dptr(K), L.dptr(d), int(d.size), L.dptr(P),
-                                                  self.w, self.h, int(fused)))
+        if R is None:
+            L.check(self.ctx.lib.bevk_undistorter_set(self.ctx.h, slot, m, L.dptr(K), L.dptr(d), int(d.size), L.dptr(P),
+                                                      self.w, self.h, int(fused)))
+        else:
+            L.check(self.ctx.lib.bevk_undistorter_set_rectify(self.ctx.h, slot, m, L.dptr(K), L.dptr(d), int(d.size),
+                                                              _rotation(R), L.dptr(P), self.w, self.h, int(fused)))
         self.slot = int(slot)
         live.add(self.slot)
 
@@ -664,12 +687,20 @@ class BevEngine:
         L.check(self.ctx.lib.bevk_bev_configure(self.ctx.h, n_cam, self.FW, self.FH, self.BW, self.BH))
         self.finalized = False
 
-    def set_camera(self, cam: int, K, D, P, und_size, H):
-        d = np.zeros(4)
+    def set_camera(self, cam: int, K, D, P, und_size, H, model: str = "fisheye"):
+        """Camera `cam`'s LUT: cv2.warpPerspective by H of cv2's undistortion maps of (K, D, P) at und_size.  model
+        "fisheye" (D: the first 4 coefficients) or "pinhole" (D: 0, 4, 5, 8, 12 or 14 coefficients, as cv2 takes them)."""
         dd = np.asarray(D, np.float64).reshape(-1)
-        d[:min(4, dd.size)] = dd[:4]
-        L.check(self.ctx.lib.bevk_bev_set_camera(self.ctx.h, cam, L.dptr(K), L.dptr(d), L.dptr(P),
-                                                 int(und_size[0]), int(und_size[1]), L.dptr(H)))
+        if model == "fisheye":
+            d = np.zeros(4)
+            d[:min(4, dd.size)] = dd[:4]
+            L.check(self.ctx.lib.bevk_bev_set_camera(self.ctx.h, cam, L.dptr(K), L.dptr(d), L.dptr(P),
+                                                     int(und_size[0]), int(und_size[1]), L.dptr(H)))
+        elif model == "pinhole":
+            L.check(self.ctx.lib.bevk_bev_set_camera_model(self.ctx.h, cam, L.MODEL_PINHOLE, L.dptr(K), L.dptr(dd), int(dd.size),
+                                                           L.dptr(P), int(und_size[0]), int(und_size[1]), L.dptr(H)))
+        else:
+            raise L.BevkError(f'camera model must be "fisheye" or "pinhole", got {model!r}')
         self.finalized = False
 
     def set_maps(self, cam: int, map1, map2):

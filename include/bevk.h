@@ -98,6 +98,19 @@ int bevk_host_free(void *p);
  * map1: int16[h][w][2] (x,y integer part), map2: uint16[h][w] (fy*32+fx).        */
 int bevk_undistort_map(bevk_ctx *ctx, int model, const double K[9], const double *D, int n_dist,
                        const double P[9], int w, int h, int16_t *map1, uint16_t *map2);
+/* cv2.initUndistortRectifyMap(K, D, R, P, (w,h), CV_16SC2) / cv2.fisheye.initUndistortRectifyMap(K, D, R, P, ...):
+ * the same maps with a rectification rotation R (row-major 3x3; NULL means the identity), e.g. from
+ * cv2.stereoRectify / cv2.fisheye.stereoRectify, and every lens model cv2 calibrates.  n_dist: a pinhole D of 0, 4,
+ * 5, 8 (k1 k2 p1 p2 k3 k4 k5 k6, CALIB_RATIONAL_MODEL), 12 (+ s1 s2 s3 s4, CALIB_THIN_PRISM_MODEL) or 14 (+ tauX tauY,
+ * CALIB_TILTED_MODEL) coefficients, a fisheye D of 4 (or 0: zeros); other lengths, which cv2 refuses too, are
+ * BEVK_ERR_ARG.
+ * A fisheye whose rotated rays depend on the row is walked row by row on the device first, as cv2 walks it: the walk
+ * needs 24 bytes of device scratch per map entry (126 MB at 2560x2048) for the duration of the call.
+ * bevk_undistort_map is this call with R = NULL.  There, a pinhole n_dist of 8, 12 or 14 applies every coefficient
+ * (before this call existed it read the first 5); any other n_dist keeps its old reading: the first 5 (pinhole) or 4
+ * (fisheye) coefficients, zero-padded. */
+int bevk_undistort_rectify_map(bevk_ctx *ctx, int model, const double K[9], const double *D, int n_dist, const double *R,
+                               const double P[9], int w, int h, int16_t *map1, uint16_t *map2);
 
 /* ---- K3: cv2.remap(src, map1, map2, interp), BORDER_CONSTANT 0 --------------
  *   surroundBEV.py:110-111,116-117; undistort.py:66; intrinsicCalib.py:193-195
@@ -113,6 +126,11 @@ int bevk_remap(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t sstrid
  * the gather kernel (no 6 B/px map traffic; same results).                      */
 int bevk_undistorter_set(bevk_ctx *ctx, int slot, int model, const double K[9], const double *D, int n_dist,
                          const double P[9], int dw, int dh, int fused);
+/* bevk_undistorter_set with R and D as bevk_undistort_rectify_map takes them (bevk_undistorter_set is this call with
+ * R = NULL and D read as bevk_undistort_map reads it).  A fused fisheye slot whose rotated rays depend on the row
+ * cannot follow cv2's running row sums per pixel: BEVK_ERR_UNSUPPORTED; a map-resident slot (fused = 0) takes it. */
+int bevk_undistorter_set_rectify(bevk_ctx *ctx, int slot, int model, const double K[9], const double *D, int n_dist,
+                                 const double *R, const double P[9], int dw, int dh, int fused);
 int bevk_undistorter_maps(bevk_ctx *ctx, int slot, int16_t *map1, uint16_t *map2);   /* D2H, for parity tests */
 /* dw x dh: the destination size the caller allocated; must equal the slot's map size (checked, so a stale handle to
  * a slot that was re-set can never make the library write past dst). */
@@ -187,6 +205,11 @@ int bevk_bev_configure(bevk_ctx *ctx, int n_cam, int frame_w, int frame_h, int b
  * without materialising the und_w x und_h intermediate map.                      */
 int bevk_bev_set_camera(bevk_ctx *ctx, int cam, const double K[9], const double D[4], const double P[9],
                         int und_w, int und_h, const double H[9]);
+/* bevk_bev_set_camera for a camera of either model: its LUT is cv2.warpPerspective of cv2's own undistortion maps for
+ * (model, K, D, P), D as bevk_undistort_rectify_map takes it.  bevk_bev_set_camera is this call with BEVK_MODEL_FISHEYE
+ * and 4 coefficients. */
+int bevk_bev_set_camera_model(bevk_ctx *ctx, int cam, int model, const double K[9], const double *D, int n_dist,
+                              const double P[9], int und_w, int und_h, const double H[9]);
 /* Inject / read back a camera's BEV maps (int16[bev_h][bev_w][2], uint16[bev_h][bev_w]). */
 int bevk_bev_set_maps(bevk_ctx *ctx, int cam, const int16_t *map1, const uint16_t *map2);
 int bevk_bev_get_maps(bevk_ctx *ctx, int cam, int16_t *map1, uint16_t *map2);
@@ -520,7 +543,8 @@ int bevk_png_encode_channels_bound(int width, int height, int channels, uint64_t
  * A graph keeps the device buffers it was captured with: a map slot's maps and a fused fisheye slot's column table
  * (bevk_undistorter_set), and the BEV LUT.  Setting that slot or camera up again after the capture changes what the
  * graph reads (or frees it, if the buffer had to grow); capture again after bevk_undistorter_set /
- * bevk_bev_set_camera.  Those set-up calls (and bevk_undistort_map) cannot themselves be captured.            */
+ * bevk_bev_set_camera.  Those set-up calls (and bevk_undistort_map) cannot themselves be captured.  A fused pinhole
+ * slot with more than 5 coefficients carries them in the captured launch itself.                                  */
 int bevk_graph_begin(bevk_ctx *ctx);
 int bevk_graph_end(bevk_ctx *ctx, int *graph_id);
 int bevk_graph_launch(bevk_ctx *ctx, int graph_id, int times);
