@@ -115,6 +115,7 @@ struct Lens {
   CamModel cm;
   LensExt lx;
   bool full = false;
+  bool walks = false;   // R makes the rays depend on the row (rays_walk): they are walked first (k_walk_rays)
 };
 
 static int make_model(int model, const double* K, const double* D, int n_dist, const double* R, const double* P, int w, int h,
@@ -128,6 +129,8 @@ static int make_model(int model, const double* K, const double* D, int n_dist, c
                                                            : "pinhole D has %d coefficients, cv2 takes 0, 4, 5, 8, 12 or 14", n_dist);
     case LENS_SINGULAR: return fail(BEVK_ERR_ARG, R ? "P * R is singular" : "P is singular");
   }
+  L->walks = rays_walk(L->cm, R);
+  L->full = L->full || L->walks;
   return BEVK_OK;
 }
 
@@ -159,7 +162,8 @@ struct Undistorter {
   bool valid = false, fused = false;
   Lens lens;
   DevBuf map1, map2;
-  DevBuf xs;                      // cm.xs of a fused fisheye slot
+  DevBuf xs;                      // cm.xs of a fused slot
+  DevBuf rays;                    // lx.rays of a fused pinhole slot whose rays walk: its block starts (walk_rays)
 };
 
 struct BevCam {
@@ -179,7 +183,7 @@ struct bevk_ctx {
   long long launches = 0;
   DevBuf s_src, s_dst, s_m1, s_m2, s_o1, s_o2;   // scratch for the host-pointer entry points
   DevBuf s_xs;                                   // cm.xs of bevk_undistort_map and bevk_bev_set_camera
-  DevBuf s_rays;                                 // lx.rays of a map build whose fisheye rays depend on the row
+  DevBuf s_rays;                                 // lx.rays of a map build whose rays depend on the row
   DevBuf d_wtab;                                 // INTER_CUBIC and INTER_LANCZOS4 weight tables (build_interp_tabs)
   Undistorter und[8];
   // BEV engine
@@ -291,8 +295,8 @@ static int use(bevk_ctx* c) {
   return BEVK_OK;
 }
 
-// The fisheye model's table of OpenCV's running _x per column (bevk_device.cuh, xs_table_applies) into buf, with cm->xs
-// pointing at it; other models and P keep cm->xs null.  buf must outlive every kernel launched with *cm.
+// The table of OpenCV's running _x per column (bevk_device.cuh, xs_table_applies) into buf, with cm->xs pointing at it;
+// rays that depend on the row keep cm->xs null.  buf must outlive every kernel launched with *cm.
 static int attach_xs_table(bevk_ctx* c, DevBuf& buf, CamModel* cm) {
   cm->xs = nullptr;
   if (!xs_table_applies(*cm)) return BEVK_OK;
@@ -430,25 +434,33 @@ int bevk_host_free(void* p) {
 }
 
 // ------------------------------------------------------------------ K1
-// k_undistort_map of L into the pair (m1, m2): cm.w x cm.h entries.  A fisheye whose rays depend on the row walks them into
-// scratch first (k_walk_rays), as cv2 walks each row: 24 bytes per map entry (126 MB at 2560 x 2048), freed again once the
-// map is built, so that a ctx does not hold it between set-ups.
+// The walked rays of L (walk_rays, k_walk_rays) into buf, with L->lx.rays pointing at them: 24 bytes per map entry for the
+// fisheye (126 MB at 2560 x 2048), 3 for the pinhole's block starts.
+static int walk_into(bevk_ctx* c, DevBuf& buf, Lens* L) {
+  const CamModel& cm = L->cm;
+  if (c->capturing) return fail(BEVK_ERR_ARG, "a camera model cannot be set up inside a graph capture");
+  RET(buf.ensure((size_t)ray_row_len(cm) * cm.h * 3 * sizeof(double)));
+  if (cm.model == BEVK_MODEL_PINHOLE) k_walk_rays<1><<<(cm.h + 127) / 128, 128, 0, c->stream>>>(cm, buf.as<double>());
+  else k_walk_rays<0><<<(cm.h + 127) / 128, 128, 0, c->stream>>>(cm, buf.as<double>());
+  LAUNCHED(c);
+  L->lx.rays = buf.as<double>();
+  return BEVK_OK;
+}
+
+// k_undistort_map of L into the pair (m1, m2): cm.w x cm.h entries.  A camera whose rays depend on the row walks them into
+// scratch first (walk_into), as cv2 walks each row, unless L already carries them (a fused slot's); the scratch is freed
+// again once the map is built, so that a ctx does not hold it between set-ups.
 static int build_map(bevk_ctx* c, Lens L, DevBuf& m1, DevBuf& m2) {
   const CamModel& cm = L.cm;
   const size_t n = (size_t)cm.w * cm.h;
   RET(m1.ensure(n * 4));
   RET(m2.ensure(n * 2));
-  if (fisheye_walks(cm, L.full)) {
-    if (c->capturing) return fail(BEVK_ERR_ARG, "a camera model cannot be set up inside a graph capture");
-    RET(c->s_rays.ensure(n * 3 * sizeof(double)));
-    k_walk_rays<<<(cm.h + 127) / 128, 128, 0, c->stream>>>(cm, c->s_rays.as<double>());
-    LAUNCHED(c);
-    L.lx.rays = c->s_rays.as<double>();
-  }
+  const bool scratch = L.walks && !L.lx.rays;
+  if (scratch) RET(walk_into(c, c->s_rays, &L));
   if (L.full) k_undistort_map<1><<<grid2d(cm.w, cm.h), 256, 0, c->stream>>>(cm, L.lx, m1.as<short2>(), m2.as<unsigned short>());
   else k_undistort_map<0><<<grid2d(cm.w, cm.h), 256, 0, c->stream>>>(cm, L.lx, m1.as<short2>(), m2.as<unsigned short>());
   LAUNCHED(c);
-  if (L.lx.rays) {   // the map kernel reads the rays: wait for it before the scratch goes
+  if (scratch) {   // the map kernel reads the rays: wait for it before the scratch goes
     CU(cudaStreamSynchronize(c->stream));
     c->s_rays.release();
   }
@@ -799,13 +811,16 @@ int bevk_undistorter_set_rectify(bevk_ctx* c, int slot, int model, const double 
   Lens& L = u.lens;
   RET(make_model(model, K, D, n_dist, R, P, dw, dh, &L));
   u.fused = fused != 0;
-  if (u.fused && fisheye_walks(L.cm, L.full))
+  if (u.fused && L.walks && model == BEVK_MODEL_FISHEYE)
     return fail(BEVK_ERR_UNSUPPORTED, "a fused fisheye slot cannot follow cv2's running ray sums when R makes the rays depend "
                 "on the row; set up a map-resident slot (fused = 0) for this camera");
-  if (u.fused) {   // the gathers evaluate the model per pixel: the slot keeps its column table
+  if (u.fused) {   // the gathers evaluate the model per pixel: the slot keeps its column table or its block starts
     RET(attach_xs_table(c, u.xs, &L.cm));
+    if (L.walks) RET(walk_into(c, u.rays, &L));
+    else u.rays.release();
   } else {         // the table (and walked rays) are read once, by the map build, from scratch
     u.xs.release();
+    u.rays.release();
     RET(attach_xs_table(c, c->s_xs, &L.cm));
     RET(build_map(c, L, u.map1, u.map2));
     L.cm.xs = nullptr;

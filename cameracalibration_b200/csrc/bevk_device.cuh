@@ -36,7 +36,7 @@ struct CamModel {      // cv2.fisheye / cv2 initUndistortRectifyMap inputs, pre-
   double fx, fy, cx, cy;
   int model;           // BEVK_MODEL_*
   int w, h;            // size of the undistorted (destination) frame
-  const double* xs;    // fisheye with row-independent rays (xs_table_applies): OpenCV's running _x of column j; else null
+  const double* xs;    // rays independent of the row (xs_table_applies): OpenCV's running _x of column j; else null
 };
 
 // What cv2's full lens models add to CamModel.  Only the LENS = 1 instances of the kernels receive it (lens_model), so
@@ -44,7 +44,7 @@ struct CamModel {      // cv2.fisheye / cv2 initUndistortRectifyMap inputs, pre-
 struct LensExt {
   double k[7];          // pinhole: k4 k5 k6 (rational), s1 s2 s3 s4 (thin prism); zeros when D has fewer coefficients
   double T[9];          // pinhole: computeTiltProjectionMatrix(tauX, tauY); the identity without tilt
-  const double* rays;   // fisheye map builds whose rays depend on the row: cv2's running _x, _y, _w ([3][h][w], walk_rays)
+  const double* rays;   // rays that depend on the row: cv2's running _x, _y, _w (walk_rays), or null
 };
 
 struct Homog { double M[9]; };   // inv(H), as cv2.warpPerspective computes it
@@ -107,54 +107,95 @@ __host__ __device__ __forceinline__ int cv_round(double v) {
   return d2i_rn(v);
 }
 
-// A1: cv2.fisheye.initUndistortRectifyMap walks each row with running sums, _x = i*iR01 + iR02 followed by _x += iR00 per
-// column (and the same for _y, _w); j*iR00 + (i*iR01 + iR02) differs from that sum in the last bits, which moves cvRound
-// ties.  When iR has no skew and the last row (0, 0, *) -- every P of dst_camera_matrix -- the sums of _y and _w add
-// zeros (exact) and _x depends on the column only: the host tabulates it once per map (fill_xs_table), the kernels read
-// xs[j].  Any other P, and the pinhole model, keep the direct form.
-inline bool xs_table_applies(const CamModel& c) {
-  return c.model == 0 && c.iR[1] == 0. && c.iR[3] == 0. && c.iR[6] == 0. && c.iR[7] == 0.;
-}
-inline void fill_xs_table(const CamModel& c, double* xs) {
-  double x = c.iR[2];   // 0 * iR01 + iR02
-  for (int j = 0; j < c.w; ++j) {
-    xs[j] = x;
-    x = dadd(x, c.iR[0]);
-  }
+// A1 / A11: cv2 builds the rays of a map row from running sums that start at _x = i*iR01 + iR02 (the same for _y, _w).
+// cv2.fisheye.initUndistortRectifyMap adds iR00 column by column.  cv2.initUndistortRectifyMap (pinhole) adds 8*iR00 per
+// 8-column block of its vector body and offsets column k of a block by k*iR00; its scalar tail (the last W % 8 columns)
+// adds iR00 column by column from where the blocks end.  The 8 is the AVX2 build's, as in pack_saturates.
+// j*iR00 + (i*iR01 + iR02) differs from those sums in the last bits, which moves cvRound ties and, where _w is near 0,
+// decides between _w == 0 and a tiny _w.  row_sums writes the sums of one row and one ray component from x0 by step.
+template <int MODEL>
+__host__ __device__ __forceinline__ void row_sums(double x0, double step, int w, double* out) {
+  int j = 0;
+  if (MODEL == 1)
+    for (; j < w - w % 8; j += 8, x0 = dadd(x0, dmul(8.0, step)))
+      for (int k = 0; k < 8; ++k) out[j + k] = dadd(x0, dmul((double)k, step));
+  for (; j < w; ++j, x0 = dadd(x0, step)) out[j] = x0;
 }
 
-// A1 with a general R: cv2.fisheye.initUndistortRectifyMap's rays of row i, _x = i*iR01 + iR02 then _x += iR00 per
-// column (and the same for _y, _w), into the planes of rays ([3][h][w]).  The sums are serial along the row, so the map
-// builds of a camera whose rays depend on the row run this once per row first (k_walk_rays) and read the planes.
+// When iR has no skew and the last row (0, 0, *) -- every P of dst_camera_matrix, R = I, R = diag(-1, -1, 1) -- the
+// sums of _y and _w add zeros (exact) and _x depends on the column only: the host tabulates it once per map
+// (fill_xs_table), the kernels read xs[j].  Any other P without R keeps the direct form.
+inline bool xs_table_applies(const CamModel& c) {
+  return c.iR[1] == 0. && c.iR[3] == 0. && c.iR[6] == 0. && c.iR[7] == 0.;
+}
+inline void fill_xs_table(const CamModel& c, double* xs) {   // x0 = 0 * iR01 + iR02
+  if (c.model == 1) row_sums<1>(c.iR[2], c.iR[0], c.w, xs);
+  else row_sums<0>(c.iR[2], c.iR[0], c.w, xs);
+}
+
+// A1 / A11 with a general R, for a camera whose rays depend on the row (rays_walk): what camera_ray<1> reads of lx.rays,
+// walked once per row first (k_walk_rays), since the sums are serial along the row.
+//   fisheye: cv2's rays of every pixel, [3][h][w] (24 bytes per map entry);
+//   pinhole: the block starts of every row, [3][h][w / 8 + 1] (3 bytes per map entry): entry b of row i is the sum at
+//            column 8b, the last one where the scalar tail starts.  A pixel needs its block start and k*iR00 (or, in the
+//            tail, at most 7 running adds), so a fused pinhole slot can keep the table and evaluate per pixel.
+inline int ray_row_len(const CamModel& c) { return c.model == 1 ? c.w / 8 + 1 : c.w; }
+
+template <int MODEL>
 __host__ __device__ __forceinline__ void walk_rays(const CamModel& c, int i, double* rays) {
-  const size_t n = (size_t)c.w * c.h, q = (size_t)i * c.w;
   const double di = (double)i;
+  if (MODEL == 1) {
+    const int nb = c.w / 8;
+    const size_t n = (size_t)(nb + 1) * c.h, q = (size_t)i * (nb + 1);
+    for (int k = 0; k < 3; ++k) {
+      double x = dadd(dmul(di, c.iR[3 * k + 1]), c.iR[3 * k + 2]);
+      const double step8 = dmul(8.0, c.iR[3 * k]);
+      for (int b = 0; b <= nb; ++b, x = dadd(x, step8)) rays[k * n + q + b] = x;
+    }
+    return;
+  }
+  const size_t n = (size_t)c.w * c.h, q = (size_t)i * c.w;
   double _x = dadd(dmul(di, c.iR[1]), c.iR[2]), _y = dadd(dmul(di, c.iR[4]), c.iR[5]), _w = dadd(dmul(di, c.iR[7]), c.iR[8]);
   for (int j = 0; j < c.w; ++j) {
     rays[q + j] = _x; rays[n + q + j] = _y; rays[2 * n + q + j] = _w;
     _x = dadd(_x, c.iR[0]); _y = dadd(_y, c.iR[3]); _w = dadd(_w, c.iR[6]);
   }
 }
+__host__ __device__ __forceinline__ void walk_rays(const CamModel& c, int i, double* rays) {
+  if (c.model == 1) walk_rays<1>(c, i, rays);
+  else walk_rays<0>(c, i, rays);
+}
 
-// The ray (_x, _y, _w) of undistorted pixel (j,i) that undistort_point<LENS> projects: the walked rays of lx when it
+__host__ __device__ __forceinline__ double ldd(const double* p) {
+#ifdef __CUDA_ARCH__
+  return __ldg(p);
+#else
+  return *p;
+#endif
+}
+
+// The ray (_x, _y, _w) of undistorted pixel (j,i) that undistort_point<LENS> projects: from the walked rays of lx when it
 // has them (LENS = 1), else the column table's _x or the direct form.  tests/host/lens_models.cu reads it.
 template <int LENS>
 __host__ __device__ __forceinline__ void camera_ray(const CamModel& c, const LensExt& lx, int j, int i, double& _x, double& _y,
                                                     double& _w) {
   const double dj = (double)j, di = (double)i;
-  if (LENS && lx.rays) {
+  if (LENS && lx.rays && c.model == 1) {   // block start, then row_sums' in-block offset or tail sum
+    const int nb1 = c.w / 8 + 1, b = j >> 3, k = j & 7;
+    const size_t n = (size_t)nb1 * c.h, q = (size_t)i * nb1 + b;
+    double r[3];
+    for (int p = 0; p < 3; ++p) {
+      double x = ldd(lx.rays + p * n + q);
+      if (b < nb1 - 1) x = dadd(x, dmul((double)k, c.iR[3 * p]));
+      else for (int t = 0; t < k; ++t) x = dadd(x, c.iR[3 * p]);
+      r[p] = x;
+    }
+    _x = r[0]; _y = r[1]; _w = r[2];
+  } else if (LENS && lx.rays) {
     const size_t n = (size_t)c.w * c.h, q = (size_t)i * c.w + j;
-#ifdef __CUDA_ARCH__
-    _x = __ldg(lx.rays + q); _y = __ldg(lx.rays + n + q); _w = __ldg(lx.rays + 2 * n + q);
-#else
-    _x = lx.rays[q]; _y = lx.rays[n + q]; _w = lx.rays[2 * n + q];
-#endif
+    _x = ldd(lx.rays + q); _y = ldd(lx.rays + n + q); _w = ldd(lx.rays + 2 * n + q);
   } else {
-#ifdef __CUDA_ARCH__
-    _x = c.xs ? __ldg(c.xs + j) : dadd(dmul(dj, c.iR[0]), dadd(dmul(di, c.iR[1]), c.iR[2]));
-#else
-    _x = c.xs ? c.xs[j] : dadd(dmul(dj, c.iR[0]), dadd(dmul(di, c.iR[1]), c.iR[2]));
-#endif
+    _x = c.xs ? ldd(c.xs + j) : dadd(dmul(dj, c.iR[0]), dadd(dmul(di, c.iR[1]), c.iR[2]));
     _y = dadd(dmul(dj, c.iR[3]), dadd(dmul(di, c.iR[4]), c.iR[5]));
     _w = dadd(dmul(dj, c.iR[6]), dadd(dmul(di, c.iR[7]), c.iR[8]));
   }
@@ -162,7 +203,7 @@ __host__ __device__ __forceinline__ void camera_ray(const CamModel& c, const Len
 
 // A1 / A11: source-image position (u,v) of undistorted pixel (j,i).  LENS = 0 is the 4-coefficient fisheye and the
 // 5-coefficient pinhole; LENS = 1 adds what lx holds: cv2's rational denominator, thin-prism terms and tilt, and the
-// fisheye's walked rays.  With lx's coefficients zero, T the identity and no rays, LENS = 1 computes LENS = 0's values
+// walked rays.  With lx's coefficients zero, T the identity and no rays, LENS = 1 computes LENS = 0's values
 // (a division by 1, adds of 0, a multiply by 1).
 template <int LENS>
 __host__ __device__ __forceinline__ void undistort_point(const CamModel& c, const LensExt& lx, int j, int i, double& u, double& v) {
@@ -246,9 +287,10 @@ enum { LENS_OK = 0, LENS_BAD_COUNT = 1, LENS_SINGULAR = 2 };
 
 // cv2.initUndistortRectifyMap / cv2.fisheye.initUndistortRectifyMap's (K, D, R, P) as the kernels take them: iR =
 // inv(P * R) (R == null: inv(P)), k1..k5 in cm, the rest of a 8-, 12- or 14-coefficient D and the tilt matrix in lx.
-// *lens says whether the camera needs the LENS = 1 instances: a pinhole with any of k4..k6, s1..s4, tauX, tauY non-zero,
-// or a fisheye whose rotated rays depend on the row (fisheye_walks).  Any other camera, R included, computes the same
-// bytes in the LENS = 0 instances.  The caller attaches cm.xs and lx.rays.
+// *lens says whether the camera's lens needs the LENS = 1 instances: a pinhole with any of k4..k6, s1..s4, tauX, tauY
+// non-zero, or a fisheye whose rotated rays depend on the row (fisheye_walks).  A camera whose rays walk (rays_walk)
+// needs them too.  Any other camera, R included, computes the same bytes in the LENS = 0 instances.  The caller attaches
+// cm.xs and lx.rays.
 inline int lens_model(int model, const double* K, const double* D, int n_dist, const double* R, const double* P, int w, int h,
                       CamModel* cm, LensExt* lx, bool* lens) {
   memset(cm, 0, sizeof *cm);
@@ -273,7 +315,11 @@ inline int lens_model(int model, const double* K, const double* D, int n_dist, c
   return LENS_OK;
 }
 
-// A LENS = 1 fisheye: its map builds read walked rays, and a fused gather cannot walk them per pixel.
+// Does R make the rays of cm depend on the row, so that the map builds walk them (walk_rays) and the LENS = 1 instances
+// read them?  Without R (or with R = I) the rays keep the column table or the direct form.
+inline bool rays_walk(const CamModel& cm, const double* R) { return R && !is_identity3(R) && !xs_table_applies(cm); }
+
+// A fisheye whose rays walk: a fused gather cannot walk its per-pixel rays, so only a map-resident slot takes it.
 inline bool fisheye_walks(const CamModel& cm, bool lens) { return lens && cm.model == 0; }
 
 // CV_16SC2 + CV_16UC1 quantisation of (u,v): map1 = (iu>>5, iv>>5) as int16 (wrapping

@@ -37,10 +37,11 @@ __global__ void __launch_bounds__(256) k_undistort_map(CamModel cm, LensExt lx, 
   map2[i] = fr;
 }
 
-// K1 set-up of a fisheye whose rays depend on the row (LensExt::rays): one thread walks one row.
+// K1 set-up of a camera whose rays depend on the row (LensExt::rays): one thread walks one row.
+template <int MODEL>
 __global__ void __launch_bounds__(128) k_walk_rays(CamModel cm, double* __restrict__ rays) {
   const int i = blockIdx.x * 128 + threadIdx.x;
-  if (i < cm.h) walk_rays(cm, i, rays);
+  if (i < cm.h) walk_rays<MODEL>(cm, i, rays);
 }
 
 // ---------------------------------------------------------------------------------

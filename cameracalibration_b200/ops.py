@@ -542,6 +542,7 @@ class Undistorter:
     D: 4 fisheye coefficients, or 4, 5, 8, 12 or 14 pinhole ones (cv2's rational, thin-prism and tilted models).  R: a
     rectification rotation (cv2.stereoRectify's R1 / R2), None for eye(3).  A fused fisheye whose rotated rays depend on
     the row is refused (BevkError): cv2 walks those rays with running row sums, which only a map-resident slot follows.
+    A fused pinhole slot of such a camera keeps the block starts of cv2's sums (3 bytes per pixel of device memory).
 
     A bevk_ctx has 8 undistorter slots.  Each live Undistorter owns one slot of its ctx; the slot returns to the
     pool on close() / garbage collection, and a 9th live object on one ctx raises instead of silently taking over a

@@ -104,8 +104,9 @@ int bevk_undistort_map(bevk_ctx *ctx, int model, const double K[9], const double
  * 5, 8 (k1 k2 p1 p2 k3 k4 k5 k6, CALIB_RATIONAL_MODEL), 12 (+ s1 s2 s3 s4, CALIB_THIN_PRISM_MODEL) or 14 (+ tauX tauY,
  * CALIB_TILTED_MODEL) coefficients, a fisheye D of 4 (or 0: zeros); other lengths, which cv2 refuses too, are
  * BEVK_ERR_ARG.
- * A fisheye whose rotated rays depend on the row is walked row by row on the device first, as cv2 walks it: the walk
- * needs 24 bytes of device scratch per map entry (126 MB at 2560x2048) for the duration of the call.
+ * A camera whose rotated rays depend on the row is walked row by row on the device first, as cv2 walks it: the walk
+ * needs device scratch for the duration of the call, 24 bytes per map entry for the fisheye (126 MB at 2560x2048), 3 for
+ * the pinhole (its block starts).
  * bevk_undistort_map is this call with R = NULL.  There, a pinhole n_dist of 8, 12 or 14 applies every coefficient
  * (before this call existed it read the first 5); any other n_dist keeps its old reading: the first 5 (pinhole) or 4
  * (fisheye) coefficients, zero-padded. */
@@ -540,7 +541,7 @@ int bevk_png_encode_channels_bound(int width, int height, int channels, uint64_t
  * frame-set instead of up to five kernel launches and two memsets (BALANCE), and a host that stalls between calls
  * cannot starve the GPU.  Run the same calls once before capturing: a call that has to allocate or build tables
  * inside a capture fails, and bevk_graph_end reports it.  Host-pointer entry points cannot be captured.
- * A graph keeps the device buffers it was captured with: a map slot's maps and a fused fisheye slot's column table
+ * A graph keeps the device buffers it was captured with: a map slot's maps and a fused slot's column table or block starts
  * (bevk_undistorter_set), and the BEV LUT.  Setting that slot or camera up again after the capture changes what the
  * graph reads (or frees it, if the buffer had to grow); capture again after bevk_undistorter_set /
  * bevk_bev_set_camera.  Those set-up calls (and bevk_undistort_map) cannot themselves be captured.  A fused pinhole

@@ -2,8 +2,8 @@
 // lens_model (P * R, the tilt matrix, the D counts cv2 takes), walk_rays, undistort_point<LENS>, warp_maps_pixel<1, LENS>.
 // Built and run by tests/test_host_lens_models.py with nvcc (host code only is executed), compared there with live cv2.
 //   lens_models maps <model> <w> <h> <n_dist> <has_R> <instance: -1 as the library picks, 0, 1> <out.bin>
-//       stdin: K[9] D[n_dist] R[9 if has_R] P[9] as C99 hex floats; prints "lens <0|1>" (the instance the library picks)
-//       and exits 5 for a D length lens_model refuses
+//       stdin: K[9] D[n_dist] R[9 if has_R] P[9] as C99 hex floats; prints "lens <0|1> walks <0|1>" (the instance the
+//       library picks, and whether it walks the rays) and exits 5 for a D length lens_model refuses
 //   lens_models bevmaps <model> <w> <h> <n_dist> <bw> <bh> <out.bin>   stdin: K[9] D[n_dist] P[9] H[9]
 //   lens_models rays <model> <w> <h> <n_dist> <has_R> <out.bin>   stdin as for maps; the rays camera_ray<LENS> hands to the
 //       projection in the instance the library picks, as double[3][h][w] (_x, _y, _w planes)
@@ -34,20 +34,22 @@ static int write_planes(const char* path, const short* m1, const unsigned short*
   return 0;
 }
 
-// As bevk_api.cu sets a camera up: lens_model, then the column table (xs_table_applies) and, for a walking fisheye, the
+// As bevk_api.cu sets a camera up: lens_model, then the column table (xs_table_applies) and, for a camera that walks, the
 // rays of every row.
 struct Camera {
   CamModel cm;
   LensExt lx;
-  bool lens = false;
+  bool lens = false, walks = false;
   std::vector<double> xs, rays;
   int setup(int model, const double* K, const double* D, int n, const double* R, const double* P, int w, int h) {
     const int r = lens_model(model, K, D, n, R, P, w, h, &cm, &lx, &lens);
     if (r != LENS_OK) return r;
+    walks = rays_walk(cm, R);
+    lens = lens || walks;
     xs.resize(w);
     if (xs_table_applies(cm)) { fill_xs_table(cm, xs.data()); cm.xs = xs.data(); }
-    if (fisheye_walks(cm, lens)) {
-      rays.resize((size_t)w * h * 3);
+    if (walks) {   // k_walk_rays
+      rays.resize((size_t)ray_row_len(cm) * h * 3);
       for (int i = 0; i < h; ++i) walk_rays(cm, i, rays.data());
       lx.rays = rays.data();
     }
@@ -63,7 +65,7 @@ static int mode_maps(int model, int w, int h, int n, int has_r, int instance, co
   const int r = cam.setup(model, K, D, n, has_r ? R : nullptr, P, w, h);
   if (r == LENS_BAD_COUNT) { printf("refused\n"); return 5; }
   if (r != LENS_OK) return 3;
-  printf("lens %d\n", (int)cam.lens);
+  printf("lens %d walks %d\n", (int)cam.lens, (int)cam.walks);
   const bool full = instance < 0 ? cam.lens : instance == 1;
   const size_t N = (size_t)w * h;
   std::vector<short> m1(2 * N);

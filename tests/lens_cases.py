@@ -157,8 +157,18 @@ def outside_only(c: LensCase, got, want) -> bool:
 def xs_table_form(c: LensCase) -> bool:
     """Are the fisheye rays of c independent of the row (bevk_device.cuh xs_table_applies: inv(P * R) without skew and
     with last row (0, 0, *))?  Otherwise cv2's running row sums have to be walked row by row."""
+    return bool(c.fisheye and _row_free(c))
+
+
+def _row_free(c) -> bool:
     iR = _iR(c)
-    return bool(c.fisheye and iR[0, 1] == 0 and iR[1, 0] == 0 and iR[2, 0] == 0 and iR[2, 1] == 0)
+    return bool(iR[0, 1] == 0 and iR[1, 0] == 0 and iR[2, 0] == 0 and iR[2, 1] == 0)
+
+
+def walks(c) -> bool:
+    """Does the library walk the rays of c row by row (lens_model's walks: an R other than the identity whose inv(P * R)
+    makes the rays depend on the row), for either model?"""
+    return bool(c.R is not None and not (c.R == np.eye(3)).all() and not _row_free(c))
 
 
 def _inv3(S):

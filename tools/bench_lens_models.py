@@ -4,7 +4,8 @@ tilted-14 cameras (the reference's front camera K; seeded mild D), map-resident 
 1280x1024 and -> 2560x2048, batches 1 and 128, 3 channels, INTER_LINEAR.  Per frame from CUDA events around repeated
 Undistorter.cuda calls (about 0.2 s per point after a warm-up); plus the map build (bevk_undistorter_set_rectify of a
 map-resident slot) and bevk_bev_set_camera_model, host clock around the call and a device synchronise; and the map build
-of the fisheye rotated by a stereo-rectification-sized R (0.05 rad), whose rays are walked row by row first (k_walk_rays).
+of the fisheye and of the rational-8 pinhole rotated by a stereo-rectification-sized R (0.05 rad), whose rays are walked
+row by row first (k_walk_rays).
 One JSON line, with the card's name and power limit read in the same run.
 
     python tools/bench_lens_models.py [--batches 1,128] [--sizes 1280x1024,2560x2048]
@@ -108,9 +109,10 @@ def main():
             H = np.array([[0.5, 0, 10], [0, 0.5, 10], [0, 1e-4, 1.0]])
             res["bev_set_camera_ms"][f"{cam}/{dst[0]}x{dst[1]}"] = round(_setup_ms(
                 ctx, lambda: eng.set_camera(0, K, D, P, dst, H, model=model)), 3)
-        model, K, D, P = _camera("fisheye4", dst)
-        res["walked_map_build_ms"][f"fisheye4/{dst[0]}x{dst[1]}"] = round(_setup_ms(
-            ctx, lambda: ops.Undistorter(K, D, P, dst, model=model, ctx=ctx, slot=7, R=R).close()), 3)
+        for cam in ("fisheye4", "rational8"):
+            model, K, D, P = _camera(cam, dst)
+            res["walked_map_build_ms"][f"{cam}/{dst[0]}x{dst[1]}"] = round(_setup_ms(
+                ctx, lambda: ops.Undistorter(K, D, P, dst, model=model, ctx=ctx, slot=7, R=R).close()), 3)
         del out
     print(json.dumps(res))
 
