@@ -15,6 +15,7 @@ INTER_NEAREST, INTER_LINEAR, INTER_CUBIC, INTER_AREA, INTER_LANCZOS4 = 0, 1, 2, 
 INTER_LINEAR_EXACT, INTER_NEAREST_EXACT, WARP_INVERSE_MAP = 5, 6, 16                   # refused by every call; warp_affine's flag
 MAPS_UNDISTORT, MAPS_BEV = 0, 1
 MODEL_FISHEYE, MODEL_PINHOLE = 0, 1
+CV_32FC1, CV_16SC2, CV_32FC2 = 5, 11, 13                                               # cv2 map types (m1type)
 FLAG_BALANCE = 1
 FLAG_NV12, FLAG_I420 = 2, 4          # YUV 4:2:0 frames (cv2's single-buffer layout), bevk_bev_run / _run_stack only
 FLAG_YUYV, FLAG_UYVY = 32, 64        # packed YUV 4:2:2 frames uint8[FH][FW][2] (cv2's COLOR_YUV2BGR_YUY2 / _UYVY input)
@@ -40,10 +41,18 @@ SIGNATURES = {
     "bevk_host_free": (C.c_int, [_p]),
     "bevk_undistort_map": (C.c_int, [_p, C.c_int, _dp, _dp, C.c_int, _dp, C.c_int, C.c_int, _p, _p]),
     "bevk_undistort_rectify_map": (C.c_int, [_p, C.c_int, _dp, _dp, C.c_int, _dp, _dp, C.c_int, C.c_int, _p, _p]),
+    "bevk_undistort_rectify_map_f32": (C.c_int, [_p, C.c_int, _dp, _dp, C.c_int, _dp, _dp, C.c_int, C.c_int, C.c_int, _p, _p]),
     "bevk_remap": (C.c_int, [_p, _p, C.c_int, C.c_int, C.c_int64, C.c_int, _p, _p, C.c_int, C.c_int, _p, C.c_int64, C.c_int]),
+    "bevk_remap_f32": (C.c_int, [_p, _p, C.c_int, C.c_int, C.c_int64, C.c_int, _p, _p, C.c_int, C.c_int, _p, C.c_int64, C.c_int]),
+    "bevk_remap_f32_stack": (C.c_int, [_p, _p, C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, _p, _p, _p, C.c_int64,
+                                       C.c_int, C.c_int, C.c_int64, C.c_int]),
+    "bevk_convert_maps": (C.c_int, [_p, _p, _p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _p, _p, C.c_int]),
     "bevk_undistorter_set": (C.c_int, [_p, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, C.c_int, C.c_int, C.c_int]),
     "bevk_undistorter_set_rectify": (C.c_int, [_p, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, _dp, C.c_int, C.c_int, C.c_int]),
     "bevk_undistorter_maps": (C.c_int, [_p, C.c_int, _p, _p]),
+    "bevk_undistorter_set_f32": (C.c_int, [_p, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, _dp, C.c_int, C.c_int, C.c_int,
+                                           C.c_int]),
+    "bevk_undistorter_maps_f32": (C.c_int, [_p, C.c_int, _p, _p]),
     "bevk_undistort": (C.c_int, [_p, C.c_int, _p, C.c_int, C.c_int, C.c_int64, C.c_int, _p, C.c_int, C.c_int, C.c_int64, C.c_int]),
     "bevk_undistort_stack": (C.c_int, [_p, C.c_int, _p, C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, _p, C.c_int64,
                                        C.c_int, C.c_int, C.c_int64, C.c_int]),

@@ -160,8 +160,9 @@ static dim3 grid2d(int w, int h) { return dim3((w + 31) / 32, (h + 7) / 8); }
 // ------------------------------------------------------------------ context
 struct Undistorter {
   bool valid = false, fused = false;
+  int m1type = MAP_16SC2;         // the maps the slot follows: CV_16SC2 + CV_16UC1, CV_32FC1 or CV_32FC2
   Lens lens;
-  DevBuf map1, map2;
+  DevBuf map1, map2;              // resident: CV_16SC2 + CV_16UC1, CV_32FC1's x and y planes, or CV_32FC2 in map1
   DevBuf xs;                      // cm.xs of a fused slot
   DevBuf rays;                    // lx.rays of a fused pinhole slot whose rays walk: its block starts (walk_rays)
 };
@@ -447,18 +448,34 @@ static int walk_into(bevk_ctx* c, DevBuf& buf, Lens* L) {
   return BEVK_OK;
 }
 
-// k_undistort_map of L into the pair (m1, m2): cm.w x cm.h entries.  A camera whose rays depend on the row walks them into
-// scratch first (walk_into), as cv2 walks each row, unless L already carries them (a fused slot's); the scratch is freed
-// again once the map is built, so that a ctx does not hold it between set-ups.
-static int build_map(bevk_ctx* c, Lens L, DevBuf& m1, DevBuf& m2) {
+// Bytes per entry of a map pair of type m1type: map1 and map2 (0: none, as for CV_32FC2).
+static void map_entry_bytes(int m1type, size_t* b1, size_t* b2) {
+  *b1 = m1type == MAP_32FC2 ? 8 : 4;
+  *b2 = m1type == MAP_16SC2 ? 2 : m1type == MAP_32FC1 ? 4 : 0;
+}
+
+// k_undistort_map (CV_16SC2 + CV_16UC1) or k_undistort_map_f32 (CV_32FC1, CV_32FC2) of L into the pair (m1, m2): cm.w x
+// cm.h entries.  A camera whose rays depend on the row walks them into scratch first (walk_into), as cv2 walks each row,
+// unless L already carries them (a fused slot's); the scratch is freed again once the map is built, so that a ctx does
+// not hold it between set-ups.
+static int build_map(bevk_ctx* c, Lens L, DevBuf& m1, DevBuf& m2, int m1type = MAP_16SC2) {
   const CamModel& cm = L.cm;
   const size_t n = (size_t)cm.w * cm.h;
-  RET(m1.ensure(n * 4));
-  RET(m2.ensure(n * 2));
+  size_t b1, b2;
+  map_entry_bytes(m1type, &b1, &b2);
+  RET(m1.ensure(n * b1));
+  if (b2) RET(m2.ensure(n * b2));
   const bool scratch = L.walks && !L.lx.rays;
   if (scratch) RET(walk_into(c, c->s_rays, &L));
-  if (L.full) k_undistort_map<1><<<grid2d(cm.w, cm.h), 256, 0, c->stream>>>(cm, L.lx, m1.as<short2>(), m2.as<unsigned short>());
-  else k_undistort_map<0><<<grid2d(cm.w, cm.h), 256, 0, c->stream>>>(cm, L.lx, m1.as<short2>(), m2.as<unsigned short>());
+  if (m1type != MAP_16SC2) {
+    float* y = m1type == MAP_32FC1 ? m2.as<float>() : nullptr;
+    if (L.full) k_undistort_map_f32<1><<<grid2d(cm.w, cm.h), 256, 0, c->stream>>>(cm, L.lx, m1.as<float>(), y);
+    else k_undistort_map_f32<0><<<grid2d(cm.w, cm.h), 256, 0, c->stream>>>(cm, L.lx, m1.as<float>(), y);
+  } else if (L.full) {
+    k_undistort_map<1><<<grid2d(cm.w, cm.h), 256, 0, c->stream>>>(cm, L.lx, m1.as<short2>(), m2.as<unsigned short>());
+  } else {
+    k_undistort_map<0><<<grid2d(cm.w, cm.h), 256, 0, c->stream>>>(cm, L.lx, m1.as<short2>(), m2.as<unsigned short>());
+  }
   LAUNCHED(c);
   if (scratch) {   // the map kernel reads the rays: wait for it before the scratch goes
     CU(cudaStreamSynchronize(c->stream));
@@ -486,6 +503,43 @@ int bevk_undistort_rectify_map(bevk_ctx* c, int model, const double K[9], const 
   return download_maps(c, c->s_m1.p, c->s_m2.p, (size_t)w * h, map1, map2);
 }
 
+// n entries of a device float map pair of type m1type (CV_32FC1 / CV_32FC2) to the caller's host maps, then wait
+static int download_maps_f32(bevk_ctx* c, const void* m1, const void* m2, size_t n, int m1type, float* map1, float* map2) {
+  size_t b1, b2;
+  map_entry_bytes(m1type, &b1, &b2);
+  CU(cudaMemcpyAsync(map1, m1, n * b1, cudaMemcpyDeviceToHost, c->stream));
+  if (b2) CU(cudaMemcpyAsync(map2, m2, n * b2, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  return BEVK_OK;
+}
+
+// The float map types a camera can be built into: CV_32FC1 for both models, CV_32FC2 for the pinhole only, as
+// cv2.fisheye.initUndistortRectifyMap asserts on CV_32FC2.
+static int check_f32_type(int model, int m1type) {
+  if (m1type != MAP_32FC1 && m1type != MAP_32FC2)
+    return fail(BEVK_ERR_ARG, "m1type %d: float maps are CV_32FC1 (%d) or CV_32FC2 (%d)", m1type, MAP_32FC1, MAP_32FC2);
+  if (model == BEVK_MODEL_FISHEYE && m1type == MAP_32FC2)
+    return fail(BEVK_ERR_ARG, "cv2.fisheye.initUndistortRectifyMap builds CV_16SC2 or CV_32FC1 maps, not CV_32FC2");
+  return BEVK_OK;
+}
+// ... and the host maps such a build writes: CV_32FC1 needs both planes
+static int check_f32_maps(int model, int m1type, const void* map1, const void* map2) {
+  RET(check_f32_type(model, m1type));
+  if (!map1 || (m1type == MAP_32FC1 && !map2)) return fail(BEVK_ERR_ARG, "null output map");
+  return BEVK_OK;
+}
+
+int bevk_undistort_rectify_map_f32(bevk_ctx* c, int model, const double K[9], const double* D, int n_dist, const double* R,
+                                   const double P[9], int w, int h, int m1type, float* map1, float* map2) {
+  RET(use(c));
+  RET(check_f32_maps(model, m1type, map1, map2));
+  Lens L;
+  RET(make_model(model, K, D, n_dist, R, P, w, h, &L));
+  RET(attach_xs_table(c, c->s_xs, &L.cm));
+  RET(build_map(c, L, c->s_m1, c->s_m2, m1type));
+  return download_maps_f32(c, c->s_m1.p, c->s_m2.p, (size_t)w * h, m1type, map1, map2);
+}
+
 int bevk_undistort_map(bevk_ctx* c, int model, const double K[9], const double* D, int n_dist, const double P[9], int w,
                        int h, int16_t* map1, uint16_t* map2) {
   const LegacyDist d(model, D, n_dist);
@@ -504,7 +558,8 @@ static bool gather4_ok(const GatherArgs& a, int channels, int interp, int mode) 
   const uintptr_t al = reinterpret_cast<uintptr_t>(a.src) | reinterpret_cast<uintptr_t>(a.dst) | (uintptr_t)a.spitch |
                        (uintptr_t)a.dpitch | (a.n > 1 ? (uintptr_t)(a.sistride | a.distride) : 0);
   return channels == 3 && interp == BEVK_INTER_LINEAR && (a.dw % 4) == 0 && (al & 3) == 0 &&
-         a.spitch < (1ll << 31) / std::max(1, a.sh) && (mode != 0 || a.map2 != nullptr);
+         a.spitch < (1ll << 31) / std::max(1, a.sh) && (mode != 0 || a.map2 != nullptr) &&
+         (mode != 4 || ((reinterpret_cast<uintptr_t>(a.fmap1) | reinterpret_cast<uintptr_t>(a.fmap2)) & 15) == 0);   // float4 loads
 }
 
 // The interpolation flag of the image gathers: INTER_AREA is read as INTER_LINEAR, as cv2.remap and cv2.warpPerspective
@@ -523,17 +578,20 @@ struct ImageBatch {
   int n;
 };
 
-constexpr int OP_RESIZE = 4;   // ImageOp::mode after the gathers' MODE 0..3
+constexpr int OP_RESIZE = 6;   // ImageOp::mode after the gathers' MODE 0..5
 
 struct ImageOp {
-  int mode = 0;                     // the gathers' MODE (0 maps, 1 camera model, 2 homography, 3 affine) or OP_RESIZE
-  bool lens = false;                // MODE 1: the camera needs the LENS = 1 instances (lens_model)
+  int mode = 0;                     // the gathers' MODE (0 maps, 1 camera model, 2 homography, 3 affine, 4 float maps,
+                                    // 5 camera model through float maps) or OP_RESIZE
+  bool lens = false;                // MODE 1 / 5: the camera needs the LENS = 1 instances (lens_model)
   int interp = 0;                   // a gather's interpolation after gather_interp; a resize's body (resize_kind)
   GatherArgs g{};                   // a gather's maps, camera model or inverse matrix
   ResizeArgs r{};                   // a resize's scales
   int slot = -1, dw = 0, dh = 0;    // an undistorter slot and the size of the images it writes
   const int16_t* hmap1 = nullptr;   // bevk_remap: the caller's host maps, uploaded once every check has passed
   const uint16_t* hmap2 = nullptr;
+  const float* hfmap1 = nullptr;    // bevk_remap_f32: the same for the caller's float maps (hfmap2 null: CV_32FC2)
+  const float* hfmap2 = nullptr;
 };
 
 // a (GatherArgs or ResizeArgs) with its frame fields taken from b
@@ -609,7 +667,11 @@ static int launch(bevk_ctx* c, const ImageOp& op, const ImageBatch& b, int chann
           else gather<1, 0>(c, a, channels, op.interp, words, gz);
           break;
         case 2: gather<2, 0>(c, a, channels, op.interp, words, gz); break;
-        default: gather<3, 0>(c, a, channels, op.interp, words, gz);
+        case 3: gather<3, 0>(c, a, channels, op.interp, words, gz); break;
+        case 4: gather<4, 0>(c, a, channels, op.interp, words, gz); break;
+        default:
+          if (op.lens) gather<5, 1>(c, a, channels, op.interp, words, gz);
+          else gather<5, 0>(c, a, channels, op.interp, words, gz);
       }
     } else {
       const ResizeArgs a = with_frames(op.r, p);
@@ -635,19 +697,33 @@ static int remap_op(const int16_t* map1, const uint16_t* map2, int interp, Image
   return BEVK_OK;
 }
 
+// float maps: map2 null means map1 is CV_32FC2; host maps are uploaded by host_launch, device maps read in place
+static int remap_f32_op(const float* map1, const float* map2, int interp, bool host, ImageOp* op) {
+  if (!map1) return fail(BEVK_ERR_ARG, "null map1");
+  RET(gather_interp(&interp));
+  op->mode = 4;
+  op->interp = interp;
+  if (host) { op->hfmap1 = map1; op->hfmap2 = map2; }
+  else { op->g.fmap1 = map1; op->g.fmap2 = map2; }
+  return BEVK_OK;
+}
+
 static int need_undistorter(bevk_ctx* c, int slot) {
   if (slot < 0 || slot >= 8 || !c->und[slot].valid) return fail(BEVK_ERR_ARG, "undistorter slot %d not set", slot);
   return BEVK_OK;
 }
 
-// a slot's resident map (MODE 0) or, fused, its camera model (MODE 1); the images it writes are the map's size
+// a slot's resident map (MODE 0, float: 4) or, fused, its camera model (MODE 1, float: 5); the images it writes are the
+// map's size
 static int undistort_op(bevk_ctx* c, int slot, int interp, ImageOp* op) {
   RET(need_undistorter(c, slot));
   RET(gather_interp(&interp));
   const Undistorter& u = c->und[slot];
-  op->mode = u.fused ? 1 : 0;
+  const bool f32 = u.m1type != MAP_16SC2;
+  op->mode = u.fused ? (f32 ? 5 : 1) : (f32 ? 4 : 0);
   op->interp = interp;
   if (u.fused) { op->g.cm = u.lens.cm; op->g.lx = u.lens.lx; op->lens = u.lens.full; }
+  else if (f32) { op->g.fmap1 = u.map1.as<float>(); op->g.fmap2 = u.m1type == MAP_32FC1 ? u.map2.as<float>() : nullptr; }
   else { op->g.map1 = u.map1.as<short2>(); op->g.map2 = u.map2.as<unsigned short>(); }
   op->slot = slot; op->dw = u.lens.cm.w; op->dh = u.lens.cm.h;
   return BEVK_OK;
@@ -737,6 +813,14 @@ static int host_launch(bevk_ctx* c, ImageOp op, const uint8_t* src, int sw, int 
     if (op.hmap2) CU(cudaMemcpyAsync(c->s_m2.p, op.hmap2, n * 2, cudaMemcpyHostToDevice, c->stream));
     op.g.map1 = c->s_m1.as<short2>(); op.g.map2 = op.hmap2 ? c->s_m2.as<unsigned short>() : nullptr;
   }
+  if (op.hfmap1) {
+    const size_t n = (size_t)dw * dh, b1 = op.hfmap2 ? n * 4 : n * 8;
+    RET(c->s_m1.ensure(b1));
+    if (op.hfmap2) RET(c->s_m2.ensure(n * 4));
+    CU(cudaMemcpyAsync(c->s_m1.p, op.hfmap1, b1, cudaMemcpyHostToDevice, c->stream));
+    if (op.hfmap2) CU(cudaMemcpyAsync(c->s_m2.p, op.hfmap2, n * 4, cudaMemcpyHostToDevice, c->stream));
+    op.g.fmap1 = c->s_m1.as<float>(); op.g.fmap2 = op.hfmap2 ? c->s_m2.as<float>() : nullptr;
+  }
   const ImageBatch b{c->s_src.as<uint8_t>(), sw, sh, (long long)sw * channels, 0,
                      c->s_dst.as<uint8_t>(), dw, dh, (long long)dw * channels, 0, 1};
   return launch(c, op, b, channels);
@@ -789,6 +873,14 @@ static int device_image(bevk_ctx* c, const ImageOp& op, const void* d_src, int64
   RET(check_stack_src(d_src, sis, sw, sh, srs, channels, n));
   RET(check_op_size(op, dw, dh));
   RET(check_stack_dst(d_src, sis, sw, sh, srs, channels, n, d_dst, dis, dw, dh, drs));
+  if (op.mode == 4 && op.slot < 0) {   // the caller's float maps: the images written must not overwrite them
+    const uintptr_t d0 = reinterpret_cast<uintptr_t>(d_dst);
+    const uintptr_t d1 = d0 + (uintptr_t)(n > 1 ? (n - 1) * dis : 0) + (uintptr_t)((int64_t)(dh - 1) * drs + (int64_t)dw * channels);
+    const size_t np = (size_t)dw * dh;
+    const uintptr_t x0 = reinterpret_cast<uintptr_t>(op.g.fmap1), x1 = x0 + np * (op.g.fmap2 ? 4 : 8);
+    const uintptr_t y0 = reinterpret_cast<uintptr_t>(op.g.fmap2), y1 = op.g.fmap2 ? y0 + np * 4 : y0;
+    if ((x0 < d1 && d0 < x1) || (y0 < d1 && d0 < y1)) return fail(BEVK_ERR_ARG, "the destination range overlaps the maps");
+  }
   return launch(c, op, device_batch(d_src, sis, sw, sh, srs, n, d_dst, dis, dw, dh, drs), channels);
 }
 
@@ -801,9 +893,29 @@ int bevk_remap(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride,
   return host_image(c, op, src, sw, sh, sstride, channels, dst, dw, dh, dstride);
 }
 
+int bevk_remap_f32(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, const float* map1,
+                   const float* map2, int dw, int dh, uint8_t* dst, int64_t dstride, int interp) {
+  RET(use(c));
+  ImageOp op;
+  RET(remap_f32_op(map1, map2, interp, true, &op));
+  return host_image(c, op, src, sw, sh, sstride, channels, dst, dw, dh, dstride);
+}
+
+int bevk_remap_f32_stack(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
+                         int channels, int n, const float* d_map1, const float* d_map2, void* d_dst, int64_t dst_image_stride,
+                         int dw, int dh, int64_t dst_row_stride, int interp) {
+  RET(use(c));
+  ImageOp op;
+  RET(remap_f32_op(d_map1, d_map2, interp, false, &op));
+  return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
+                      dst_row_stride);
+}
+
 // ------------------------------------------------------------------ cached-map undistortion
-int bevk_undistorter_set_rectify(bevk_ctx* c, int slot, int model, const double K[9], const double* D, int n_dist,
-                                 const double* R, const double P[9], int dw, int dh, int fused) {
+// A slot following maps of type m1type: CV_16SC2 + CV_16UC1 (bevk_undistorter_set_rectify), CV_32FC1 or CV_32FC2
+// (bevk_undistorter_set_f32).
+static int set_undistorter(bevk_ctx* c, int slot, int model, const double K[9], const double* D, int n_dist, const double* R,
+                           const double P[9], int dw, int dh, int fused, int m1type) {
   RET(use(c));
   if (slot < 0 || slot >= 8) return fail(BEVK_ERR_ARG, "slot %d out of range", slot);
   Undistorter& u = c->und[slot];
@@ -811,6 +923,7 @@ int bevk_undistorter_set_rectify(bevk_ctx* c, int slot, int model, const double 
   Lens& L = u.lens;
   RET(make_model(model, K, D, n_dist, R, P, dw, dh, &L));
   u.fused = fused != 0;
+  u.m1type = m1type;
   if (u.fused && L.walks && model == BEVK_MODEL_FISHEYE)
     return fail(BEVK_ERR_UNSUPPORTED, "a fused fisheye slot cannot follow cv2's running ray sums when R makes the rays depend "
                 "on the row; set up a map-resident slot (fused = 0) for this camera");
@@ -822,11 +935,22 @@ int bevk_undistorter_set_rectify(bevk_ctx* c, int slot, int model, const double 
     u.xs.release();
     u.rays.release();
     RET(attach_xs_table(c, c->s_xs, &L.cm));
-    RET(build_map(c, L, u.map1, u.map2));
+    RET(build_map(c, L, u.map1, u.map2, m1type));
     L.cm.xs = nullptr;
   }
   u.valid = true;
   return BEVK_OK;
+}
+
+int bevk_undistorter_set_rectify(bevk_ctx* c, int slot, int model, const double K[9], const double* D, int n_dist,
+                                 const double* R, const double P[9], int dw, int dh, int fused) {
+  return set_undistorter(c, slot, model, K, D, n_dist, R, P, dw, dh, fused, MAP_16SC2);
+}
+
+int bevk_undistorter_set_f32(bevk_ctx* c, int slot, int model, const double K[9], const double* D, int n_dist,
+                             const double* R, const double P[9], int dw, int dh, int fused, int m1type) {
+  RET(check_f32_type(model, m1type));
+  return set_undistorter(c, slot, model, K, D, n_dist, R, P, dw, dh, fused, m1type);
 }
 
 int bevk_undistorter_set(bevk_ctx* c, int slot, int model, const double K[9], const double* D, int n_dist,
@@ -840,10 +964,69 @@ int bevk_undistorter_maps(bevk_ctx* c, int slot, int16_t* map1, uint16_t* map2) 
   RET(need_undistorter(c, slot));
   if (!map1 || !map2) return fail(BEVK_ERR_ARG, "null output map");
   Undistorter& u = c->und[slot];
+  if (u.m1type != MAP_16SC2)
+    return fail(BEVK_ERR_ARG, "undistorter slot %d follows CV_32F maps (type %d): read them with bevk_undistorter_maps_f32",
+                slot, u.m1type);
   const bool resident = !u.fused;   // a fused slot has no resident map: evaluate into scratch
   if (!resident) RET(build_map(c, u.lens, c->s_m1, c->s_m2));
   return download_maps(c, resident ? u.map1.p : c->s_m1.p, resident ? u.map2.p : c->s_m2.p, (size_t)u.lens.cm.w * u.lens.cm.h,
                        map1, map2);
+}
+
+int bevk_undistorter_maps_f32(bevk_ctx* c, int slot, float* map1, float* map2) {
+  RET(use(c));
+  RET(need_undistorter(c, slot));
+  Undistorter& u = c->und[slot];
+  if (u.m1type == MAP_16SC2)
+    return fail(BEVK_ERR_ARG, "undistorter slot %d follows CV_16SC2 maps: read them with bevk_undistorter_maps", slot);
+  RET(check_f32_maps(u.lens.cm.model, u.m1type, map1, map2));
+  const bool resident = !u.fused;
+  if (!resident) RET(build_map(c, u.lens, c->s_m1, c->s_m2, u.m1type));
+  return download_maps_f32(c, resident ? u.map1.p : c->s_m1.p, resident ? u.map2.p : c->s_m2.p,
+                           (size_t)u.lens.cm.w * u.lens.cm.h, u.m1type, map1, map2);
+}
+
+// ------------------------------------------------------------------ cv2.convertMaps
+int bevk_convert_maps(bevk_ctx* c, const void* map1, const void* map2, int m1type, int w, int h, int dstm1type,
+                      int nninterpolation, void* dst1, void* dst2, int on_device) {
+  RET(use(c));
+  const auto known = [](int t) { return t == MAP_16SC2 || t == MAP_32FC1 || t == MAP_32FC2; };
+  if (!known(m1type) || !known(dstm1type))
+    return fail(BEVK_ERR_ARG, "map types %d -> %d: cv2.convertMaps converts between CV_16SC2 (%d), CV_32FC1 (%d) and "
+                "CV_32FC2 (%d)", m1type, dstm1type, MAP_16SC2, MAP_32FC1, MAP_32FC2);
+  if (m1type == dstm1type) return fail(BEVK_ERR_ARG, "map type %d -> %d: nothing to convert", m1type, dstm1type);
+  if (w <= 0 || h <= 0) return fail(BEVK_ERR_ARG, "bad map size %dx%d", w, h);
+  const bool nn = nninterpolation != 0 && dstm1type == MAP_16SC2;
+  if (!map1 || (m1type == MAP_32FC1 && !map2)) return fail(BEVK_ERR_ARG, "null source map");
+  if (!dst1 || ((dstm1type == MAP_32FC1 || (dstm1type == MAP_16SC2 && !nn)) && !dst2))
+    return fail(BEVK_ERR_ARG, "null destination map");
+  const long long n = (long long)w * h;
+  size_t i1, i2, o1, o2;
+  map_entry_bytes(m1type, &i1, &i2);
+  map_entry_bytes(dstm1type, &o1, &o2);
+  if (m1type != MAP_32FC1 && !map2) i2 = 0;   // CV_16SC2 without map2
+  if (nn) o2 = 0;
+  ConvertMapsArgs a{map1, i2 ? map2 : nullptr, m1type, dst1, o2 ? dst2 : nullptr, dstm1type, nn, n};
+  if (!on_device) {   // host maps: through scratch, then wait
+    if (c->capturing) return fail(BEVK_ERR_ARG, "host maps cannot be converted inside a graph capture");
+    RET(c->s_m1.ensure(n * i1));
+    if (i2) RET(c->s_m2.ensure(n * i2));
+    RET(c->s_o1.ensure(n * o1));
+    if (o2) RET(c->s_o2.ensure(n * o2));
+    CU(cudaMemcpyAsync(c->s_m1.p, map1, n * i1, cudaMemcpyHostToDevice, c->stream));
+    if (i2) CU(cudaMemcpyAsync(c->s_m2.p, map2, n * i2, cudaMemcpyHostToDevice, c->stream));
+    a.in1 = c->s_m1.p; a.in2 = i2 ? c->s_m2.p : nullptr;
+    a.out1 = c->s_o1.p; a.out2 = o2 ? c->s_o2.p : nullptr;
+  }
+  const long long blocks = std::min<long long>((n + 255) / 256, (long long)c->n_sm * 16);
+  k_convert_maps<<<(unsigned)blocks, 256, 0, c->stream>>>(a);
+  LAUNCHED(c);
+  if (!on_device) {
+    CU(cudaMemcpyAsync(dst1, c->s_o1.p, n * o1, cudaMemcpyDeviceToHost, c->stream));
+    if (o2) CU(cudaMemcpyAsync(dst2, c->s_o2.p, n * o2, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+  }
+  return BEVK_OK;
 }
 
 int bevk_undistort(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,

@@ -381,6 +381,47 @@ __host__ __device__ __forceinline__ void affine_point(const Homog& hm, int x, in
 
 __host__ __device__ __forceinline__ int sat_i16(int v) { return max(-32768, min(32767, v)); }
 
+// ---- CV_32FC1 / CV_32FC2 maps ------------------------------------------------
+// cv2 stores a float map entry as (float)u of the double the CV_16SC2 build quantises.
+__host__ __device__ __forceinline__ float d2f(double v) {
+#ifdef __CUDA_ARCH__
+  return __double2float_rn(v);
+#else
+  return (float)v;
+#endif
+}
+
+// cvRound(float) / saturate_cast<int>(float) on x86 (cvtss2si): INT_MIN for NaN, +-inf and anything outside the int
+// range.  PTX cvt.rni.s32.f32 saturates instead and gives 0 for NaN.
+__host__ __device__ __forceinline__ int x86_round(float v) {
+  if (!(fabsf(v) < 2147483648.f)) return INT_MIN;
+  return f2i_rn(v);
+}
+
+// cv2.convertMaps(x, y, CV_16SC2, nninterpolation), which is what cv2.remap does to float maps before its integer
+// remap.  Non-NEAREST: ix = cvRound(x * 32.f) in float, map1 = saturate_cast<short>(ix >> 5), frac = (iy & 31) * 32 +
+// (ix & 31).  NEAREST: map1 = saturate_cast<short>(cvRound(x)), rounding half to even on the float itself, and no frac
+// (so no NNDeltaTab rule either).
+__host__ __device__ __forceinline__ void quantise_xy(float x, float y, bool nearest, short& mx, short& my, unsigned short& frac) {
+  if (nearest) {
+    mx = (short)sat_i16(x86_round(x));
+    my = (short)sat_i16(x86_round(y));
+    frac = 0;
+    return;
+  }
+  const int ix = x86_round(fmul(x, (float)TAB)), iy = x86_round(fmul(y, (float)TAB));
+  mx = (short)sat_i16(ix >> INTER_BITS);
+  my = (short)sat_i16(iy >> INTER_BITS);
+  frac = (unsigned short)((iy & (TAB - 1)) * TAB + (ix & (TAB - 1)));
+}
+
+// cv2.convertMaps(CV_16SC2 [+ CV_16UC1] -> CV_32F): x + (frac & 31) / 32, exact in float.  No map2 is frac 0.
+__host__ __device__ __forceinline__ void unquantise_xy(short mx, short my, unsigned frac, float& x, float& y) {
+  frac &= TAB * TAB - 1;
+  x = fadd((float)mx, fmul((float)(frac & (TAB - 1)), 1.f / TAB));
+  y = fadd((float)my, fmul((float)(frac >> INTER_BITS), 1.f / TAB));
+}
+
 // ---- byte-lane primitives with a host form ------------------------------------
 // The packed integer arithmetic of the gathers (interp_fast, sat_add_bgr, the tile write-out) is built from
 // these; on the device they are single SASS instructions (PRMT, SHF, IDP.2A, VADDUS4-style), on the host plain

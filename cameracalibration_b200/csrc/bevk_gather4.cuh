@@ -2,7 +2,7 @@
 // cv2.remap with resident maps (MODE 0; Camera.undistort / InCalibrator.undistort / Tools/undistort.py,
 // surroundBEV.py:110-111, intrinsicCalib.py:193-195, undistort.py:66), the same with the camera model
 // evaluated in-kernel (MODE 1), cv2.warpPerspective (MODE 2; extrinsicCalib.py:166-169) and cv2.warpAffine
-// (MODE 3; extrinsicCalib.py:58).
+// (MODE 3; extrinsicCalib.py:58), and cv2.remap / undistortion with float maps (MODE 4 and 5).
 // Same tap machinery as the fused BEV kernel (aligned 32-bit words, funnel shift, PRMT, DP2A);
 // each thread produces 12 output bytes per frame and stores them as three 32-bit words.  Over a
 // batch it resolves its 4 pixels' taps once and gathers them from NB = GATHER_NB frames (see k_gather).
@@ -76,12 +76,26 @@ __host__ __device__ __forceinline__ void gather4_frames(const GatherArgs& a, int
     mx[3] = (short)(m.w & 0xffff); my[3] = (short)(m.w >> 16);
     fr[0] = (unsigned short)(f.x & 0xffffu); fr[1] = (unsigned short)(f.x >> 16);
     fr[2] = (unsigned short)(f.y & 0xffffu); fr[3] = (unsigned short)(f.y >> 16);
+  } else if (MODE == 4) {   // 16-byte map loads: the host checks the maps' alignment (gather4_ok)
+    const size_t i = (size_t)y * a.dw + x4;
+    float X[4], Y[4];
+    if (a.fmap2) {
+      const float4 p = *reinterpret_cast<const float4*>(a.fmap1 + i), q = *reinterpret_cast<const float4*>(a.fmap2 + i);
+      X[0] = p.x; X[1] = p.y; X[2] = p.z; X[3] = p.w;
+      Y[0] = q.x; Y[1] = q.y; Y[2] = q.z; Y[3] = q.w;
+    } else {
+      const float4 p = *reinterpret_cast<const float4*>(a.fmap1 + 2 * i), q = *reinterpret_cast<const float4*>(a.fmap1 + 2 * i + 4);
+      X[0] = p.x; Y[0] = p.y; X[1] = p.z; Y[1] = p.w;
+      X[2] = q.x; Y[2] = q.y; X[3] = q.z; Y[3] = q.w;
+    }
+#pragma unroll
+    for (int q = 0; q < 4; ++q) quantise_xy(X[q], Y[q], false, mx[q], my[q], fr[q]);
   }
   int sx[4], sy[4];
   unsigned fx[4], fy[4], px[4];
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
-    if (MODE >= 2) {
+    if (MODE == 2 || MODE == 3) {
       int X, Y;
       warp_xy<MODE>(a.hm, x4 + q, y, false, X, Y);
       sx[q] = sat_i16(X >> INTER_BITS); sy[q] = sat_i16(Y >> INTER_BITS);
@@ -91,6 +105,8 @@ __host__ __device__ __forceinline__ void gather4_frames(const GatherArgs& a, int
         double u, v;
         undistort_point<LENS>(a.cm, a.lx, x4 + q, y, u, v);
         quantise_uv(u, v, mx[q], my[q], fr[q], pack_saturates(a.cm.model, x4 + q, a.cm.w));
+      } else if (MODE == 5) {
+        float_taps<MODE, LENS>(a, x4 + q, y, false, mx[q], my[q], fr[q]);
       }
       sx[q] = mx[q]; sy[q] = my[q];
       fx[q] = fr[q] & (TAB - 1); fy[q] = (fr[q] >> INTER_BITS) & (TAB - 1);

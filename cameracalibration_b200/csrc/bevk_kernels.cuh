@@ -37,6 +37,64 @@ __global__ void __launch_bounds__(256) k_undistort_map(CamModel cm, LensExt lx, 
   map2[i] = fr;
 }
 
+// K1 into CV_32FC1 (map2 = the y plane) or CV_32FC2 (map2 null, map1 interleaved): cv2 stores (float)u, (float)v of the
+// very (u, v) the CV_16SC2 build quantises.
+template <int LENS>
+__host__ __device__ __forceinline__ void undistort_map_f32_px(const CamModel& cm, const LensExt& lx, int x, int y,
+                                                             float* __restrict__ map1, float* __restrict__ map2) {
+  double u, v;
+  undistort_point<LENS>(cm, lx, x, y, u, v);
+  const size_t i = (size_t)y * cm.w + x;
+  if (map2) { map1[i] = d2f(u); map2[i] = d2f(v); }
+  else { map1[2 * i] = d2f(u); map1[2 * i + 1] = d2f(v); }
+}
+
+template <int LENS>
+__global__ void __launch_bounds__(256) k_undistort_map_f32(CamModel cm, LensExt lx, float* __restrict__ map1,
+                                                           float* __restrict__ map2) {
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31);
+  const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x >= cm.w || y >= cm.h) return;
+  undistort_map_f32_px<LENS>(cm, lx, x, y, map1, map2);
+}
+
+// cv2.convertMaps between CV_16SC2 (+ CV_16UC1), CV_32FC1 and CV_32FC2, one map entry per thread.  Map types are cv2's
+// values (BEVK_CV_*); a float source is read as (x, y), a CV_16SC2 one as its exact float value (unquantise_xy).
+constexpr int MAP_16SC2 = 11, MAP_32FC1 = 5, MAP_32FC2 = 13;
+struct ConvertMapsArgs {
+  const void* in1; const void* in2; int intype;   // in2: CV_16UC1 (may be null) or the y plane of CV_32FC1
+  void* out1; void* out2; int outtype;            // out2: CV_16UC1 (null with nn) or the y plane of CV_32FC1
+  bool nn;                                        // nninterpolation: CV_16SC2 without map2, rounded to whole pixels
+  long long n;
+};
+
+__host__ __device__ __forceinline__ void convert_map_px(const ConvertMapsArgs& a, long long i) {
+  float x, y;
+  if (a.intype == MAP_16SC2) {
+    const short2 m = static_cast<const short2*>(a.in1)[i];
+    unquantise_xy(m.x, m.y, a.in2 ? static_cast<const unsigned short*>(a.in2)[i] : 0u, x, y);
+  } else if (a.intype == MAP_32FC2) {
+    x = static_cast<const float*>(a.in1)[2 * i]; y = static_cast<const float*>(a.in1)[2 * i + 1];
+  } else {
+    x = static_cast<const float*>(a.in1)[i]; y = static_cast<const float*>(a.in2)[i];
+  }
+  if (a.outtype == MAP_16SC2) {
+    short mx, my;
+    unsigned short fr;
+    quantise_xy(x, y, a.nn, mx, my, fr);
+    static_cast<short2*>(a.out1)[i] = make_short2(mx, my);
+    if (!a.nn) static_cast<unsigned short*>(a.out2)[i] = fr;
+  } else if (a.outtype == MAP_32FC2) {
+    static_cast<float*>(a.out1)[2 * i] = x; static_cast<float*>(a.out1)[2 * i + 1] = y;
+  } else {
+    static_cast<float*>(a.out1)[i] = x; static_cast<float*>(a.out2)[i] = y;
+  }
+}
+
+__global__ void __launch_bounds__(256) k_convert_maps(ConvertMapsArgs a) {
+  for (long long i = blockIdx.x * 256ll + threadIdx.x; i < a.n; i += (long long)gridDim.x * 256) convert_map_px(a, i);
+}
+
 // K1 set-up of a camera whose rays depend on the row (LensExt::rays): one thread walks one row.
 template <int MODEL>
 __global__ void __launch_bounds__(128) k_walk_rays(CamModel cm, double* __restrict__ rays) {
@@ -46,7 +104,9 @@ __global__ void __launch_bounds__(128) k_walk_rays(CamModel cm, double* __restri
 
 // ---------------------------------------------------------------------------------
 // K3 / K4: generic gather.  MODE 0: maps in HBM, 1: camera model evaluated in-kernel
-// (fused undistort), 2: homography (warpPerspective), 3: affine matrix (warpAffine, inverse in hm.M[0..5]).
+// (fused undistort), 2: homography (warpPerspective), 3: affine matrix (warpAffine, inverse in hm.M[0..5]),
+// 4: CV_32FC1 / CV_32FC2 maps in HBM, 5: camera model rounded to float as a float map holds it.  MODE 4 and 5 resolve
+// their taps as cv2.remap converts float maps (quantise_xy).
 // Over a batch of n frames: the taps of an output pixel depend on the pixel only, so a thread
 // resolves them once (map load or camera model) and gathers them from GATHER_NB frames of its
 // grid-z slice.  Frame f is read at src + f * sistride and written at dst + f * distride.
@@ -54,12 +114,33 @@ __global__ void __launch_bounds__(128) k_walk_rays(CamModel cm, double* __restri
 struct GatherArgs {
   const uint8_t* src; int sw, sh; long long spitch;
   uint8_t* dst; int dw, dh; long long dpitch;
-  const short2* map1; const unsigned short* map2;
+  // MODE 0: CV_16SC2 + CV_16UC1 (map2 may be null for NEAREST); MODE 4: x and y planes (CV_32FC1), or fmap2 null and
+  // (x, y) pairs in fmap1 (CV_32FC2).  Unions, so that the arguments of every other MODE keep their offsets.
+  union { const short2* map1; const float* fmap1; };
+  union { const unsigned short* map2; const float* fmap2; };
   CamModel cm;
   LensExt lx;                            // MODE 1 with LENS = 1 only
   Homog hm;
   int n; long long sistride, distride;   // frames, and the 64-bit image strides of source and destination
 };
+
+// MODE 4 / 5: the integer map entry of output pixel (x, y): the float map's (x, y), or the camera model's (u, v) rounded
+// to float, through quantise_xy.
+template <int MODE, int LENS>
+__host__ __device__ __forceinline__ void float_taps(const GatherArgs& a, int x, int y, bool nearest, short& mx, short& my,
+                                                    unsigned short& fr) {
+  float fx, fy;
+  if (MODE == 4) {
+    const size_t i = (size_t)y * a.dw + x;
+    if (a.fmap2) { fx = a.fmap1[i]; fy = a.fmap2[i]; }
+    else { fx = a.fmap1[2 * i]; fy = a.fmap1[2 * i + 1]; }
+  } else {
+    double u, v;
+    undistort_point<LENS>(a.cm, a.lx, x, y, u, v);
+    fx = d2f(u); fy = d2f(v);
+  }
+  quantise_xy(fx, fy, nearest, mx, my, fr);
+}
 
 // Frames per thread (grid.z = ceil(n / GATHER_NB)); DESIGN.md section 4 has the measurement that chose it.
 #ifndef BEVK_GATHER_NB
@@ -97,7 +178,7 @@ __host__ __device__ __forceinline__ void load_px(const uint8_t* __restrict__ src
 template <int MODE, int C, int LINEAR, int LENS = 0>
 __host__ __device__ __forceinline__ void gather_frames(const GatherArgs& a, int x, int y, int f0) {
   int sx, sy, fx = 0, fy = 0;
-  if (MODE >= 2) {
+  if (MODE == 2 || MODE == 3) {
     int X, Y;
     warp_xy<MODE>(a.hm, x, y, !LINEAR, X, Y);
     if (LINEAR) {
@@ -116,10 +197,13 @@ __host__ __device__ __forceinline__ void gather_frames(const GatherArgs& a, int 
       mx = m.x; my = m.y;
       have_frac = (a.map2 != nullptr);
       fr = have_frac ? a.map2[i] : 0;
-    } else {
+    } else if (MODE == 1) {
       double u, v;
       undistort_point<LENS>(a.cm, a.lx, x, y, u, v);
       quantise_uv(u, v, mx, my, fr, pack_saturates(a.cm.model, x, a.cm.w));
+    } else {
+      float_taps<MODE, LENS>(a, x, y, !LINEAR, mx, my, fr);
+      have_frac = LINEAR;
     }
     sx = mx; sy = my;
     fx = fr & (TAB - 1); fy = (fr >> INTER_BITS) & (TAB - 1);
@@ -165,7 +249,7 @@ __host__ __device__ __forceinline__ void gather_taps_frames(const GatherArgs& a,
                                                             int f0) {
   int sx, sy;
   unsigned fr;
-  if (MODE >= 2) {
+  if (MODE == 2 || MODE == 3) {
     int X, Y;
     warp_xy<MODE>(a.hm, x, y, false, X, Y);
     sx = sat_i16(X >> INTER_BITS); sy = sat_i16(Y >> INTER_BITS);
@@ -178,10 +262,12 @@ __host__ __device__ __forceinline__ void gather_taps_frames(const GatherArgs& a,
       const short2 m = a.map1[i];
       mx = m.x; my = m.y;
       f = a.map2[i];
-    } else {
+    } else if (MODE == 1) {
       double u, v;
       undistort_point<LENS>(a.cm, a.lx, x, y, u, v);
       quantise_uv(u, v, mx, my, f, pack_saturates(a.cm.model, x, a.cm.w));
+    } else {
+      float_taps<MODE, LENS>(a, x, y, false, mx, my, f);
     }
     sx = mx; sy = my;
     fr = f & (INTER_TAB_SIZE2 - 1);

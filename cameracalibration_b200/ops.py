@@ -12,6 +12,8 @@ from . import _lib as L
 INTER_NEAREST, INTER_LINEAR, INTER_CUBIC, INTER_AREA, INTER_LANCZOS4 = (
     L.INTER_NEAREST, L.INTER_LINEAR, L.INTER_CUBIC, L.INTER_AREA, L.INTER_LANCZOS4)
 _INTERPOLATIONS = (INTER_NEAREST, INTER_LINEAR, INTER_CUBIC, INTER_AREA, INTER_LANCZOS4)
+CV_16SC2, CV_32FC1, CV_32FC2 = L.CV_16SC2, L.CV_32FC1, L.CV_32FC2
+_MAP_TYPES = (CV_16SC2, CV_32FC1, CV_32FC2)
 
 
 def _interp(flag: int) -> int:
@@ -21,15 +23,17 @@ def _interp(flag: int) -> int:
     return flag
 
 
-def fisheye_init_undistort_rectify_map(K, D, P, size, ctx: L.Context | None = None, R=None):
-    """cv2.fisheye.initUndistortRectifyMap(K, D, R, P, size, CV_16SC2); R=None is eye(3)."""
-    return _undistort_map(L.MODEL_FISHEYE, K, D, P, size, ctx, R)
+def fisheye_init_undistort_rectify_map(K, D, P, size, ctx: L.Context | None = None, R=None, m1type: int = CV_16SC2):
+    """cv2.fisheye.initUndistortRectifyMap(K, D, R, P, size, m1type); R=None is eye(3).  m1type: CV_16SC2 (int16[h][w][2]
+    and uint16[h][w]) or CV_32FC1 (float32[h][w] x and y planes); cv2 refuses CV_32FC2 for the fisheye, and so does this."""
+    return _undistort_map(L.MODEL_FISHEYE, K, D, P, size, ctx, R, m1type)
 
 
-def init_undistort_rectify_map(K, D, P, size, ctx: L.Context | None = None, R=None):
-    """cv2.initUndistortRectifyMap(K, D, R, P, size, CV_16SC2) with D of 4, 5, 8, 12 or 14 coefficients (rational,
-    thin-prism and tilted models); R=None is eye(3)."""
-    return _undistort_map(L.MODEL_PINHOLE, K, D, P, size, ctx, R)
+def init_undistort_rectify_map(K, D, P, size, ctx: L.Context | None = None, R=None, m1type: int = CV_16SC2):
+    """cv2.initUndistortRectifyMap(K, D, R, P, size, m1type) with D of 4, 5, 8, 12 or 14 coefficients (rational,
+    thin-prism and tilted models); R=None is eye(3).  m1type: CV_16SC2, CV_32FC1 (float32 x and y planes) or CV_32FC2
+    (float32[h][w][2] and None)."""
+    return _undistort_map(L.MODEL_PINHOLE, K, D, P, size, ctx, R, m1type)
 
 
 def _rotation(R):
@@ -42,10 +46,29 @@ def _rotation(R):
     return L.dptr(r)
 
 
-def _undistort_map(model, K, D, P, size, ctx, R=None):
+def _map_type(m1type):
+    if m1type not in _MAP_TYPES:
+        raise L.BevkError(f"m1type {m1type} is not a map type (cv2's CV_16SC2, CV_32FC1 or CV_32FC2)")
+    return int(m1type)
+
+
+def _float_maps(m1type, h, w):
+    """Empty host maps of a float type: CV_32FC1's two planes, or CV_32FC2's pairs and None."""
+    if m1type == CV_32FC2:
+        return np.empty((h, w, 2), np.float32), None
+    return np.empty((h, w), np.float32), np.empty((h, w), np.float32)
+
+
+def _undistort_map(model, K, D, P, size, ctx, R=None, m1type=CV_16SC2):
     ctx = ctx or L.default_context()
     w, h = int(size[0]), int(size[1])
     d = np.asarray(D, np.float64).reshape(-1)
+    if _map_type(m1type) != CV_16SC2:
+        m1, m2 = _float_maps(m1type, h, w)
+        L.check(ctx.lib.bevk_undistort_rectify_map_f32(ctx.h, model, L.dptr(K), L.dptr(d), int(d.size), _rotation(R),
+                                                       L.dptr(P), w, h, int(m1type), L.vptr(m1),
+                                                       None if m2 is None else L.vptr(m2)))
+        return m1, m2
     m1 = np.empty((h, w, 2), np.int16)
     m2 = np.empty((h, w), np.uint16)
     if R is None:
@@ -357,8 +380,15 @@ def remap(src: np.ndarray, map1: np.ndarray, map2: np.ndarray | None, interpolat
           ctx: L.Context | None = None, out: np.ndarray | None = None) -> np.ndarray:
     """cv2.remap with CV_16SC2 (+CV_16UC1) maps, BORDER_CONSTANT 0.  interpolation: INTER_NEAREST, INTER_LINEAR,
     INTER_CUBIC, INTER_AREA (read as INTER_LINEAR, as cv2.remap reads it) or INTER_LANCZOS4; all but NEAREST need map2.
-    The result is byte-identical to cv2.remap's."""
+    The result is byte-identical to cv2.remap's.
+
+    float32 maps (CV_32FC1: map1, map2 float32[h][w]; CV_32FC2: map1 float32[h][w][2], map2 None) give cv2.remap's bytes
+    for float maps.  With them src may also be a CUDA array ([H][W], [H][W][C] or a batch [N][H][W][C], rows and images
+    may be padded), read in place on torch's current stream, with the maps NumPy or CUDA arrays; the result then stays
+    on the device (``out``, default a new torch tensor)."""
     ctx = ctx or L.default_context()
+    if _is_float32(map1):
+        return _remap_f32(src, map1, map2, interpolation, ctx, out)
     m1 = np.ascontiguousarray(map1, np.int16)
     if m1.ndim != 3 or m1.shape[2] != 2:
         raise L.BevkError("map1 must be int16[h][w][2] (CV_16SC2)")
@@ -368,6 +398,118 @@ def remap(src: np.ndarray, map1: np.ndarray, map2: np.ndarray | None, interpolat
         raise L.BevkError("map2 must be uint16[h][w] (CV_16UC1)")
     return _host_image(src, dw, dh, out, lambda s, d, dstride: ctx.lib.bevk_remap(
         ctx.h, *s, L.vptr(m1), None if m2 is None else L.vptr(m2), dw, dh, d, dstride, _interp(interpolation)))
+
+
+def _is_float32(a) -> bool:
+    iface = getattr(a, "__cuda_array_interface__", None)
+    if iface is not None:
+        return iface["typestr"] == "<f4"
+    return getattr(a, "dtype", None) == np.float32
+
+
+def _float_map_shapes(map1, map2):
+    """(dh, dw) of a float map pair: CV_32FC1 planes [h][w] + [h][w], or CV_32FC2 [h][w][2] + None."""
+    s1 = _shape(map1)
+    if map2 is None:
+        if len(s1) != 3 or s1[2] != 2:
+            raise L.BevkError(f"a float map1 without map2 must be float32[h][w][2] (CV_32FC2), got shape {s1}")
+    elif len(s1) != 2 or _shape(map2) != s1 or not _is_float32(map2):
+        raise L.BevkError(f"float maps must be float32[h][w] planes (CV_32FC1) or float32[h][w][2] and None (CV_32FC2); "
+                          f"got shapes {s1} and {_shape(map2)}")
+    return s1[0], s1[1]
+
+
+def _shape(a):
+    iface = getattr(a, "__cuda_array_interface__", None)
+    return tuple(iface["shape"]) if iface is not None else np.shape(a)
+
+
+def _cuda_dense(arr, typestr, what):
+    """Device pointer of a C-contiguous CUDA array of the given typestr."""
+    iface = arr.__cuda_array_interface__
+    if iface["typestr"] != typestr:
+        raise L.BevkError(f"{what} must have typestr {typestr}, got {iface['typestr']}")
+    shape, strides = tuple(iface["shape"]), iface.get("strides")
+    if strides is not None:
+        step = np.dtype(typestr).itemsize
+        for n, st in zip(reversed(shape), reversed(strides)):
+            if n > 1 and st != step:
+                raise L.BevkError(f"{what} must be C-contiguous")
+            step *= n
+    if not iface["data"][0]:
+        raise L.BevkError(f"{what} has a null data pointer")
+    return C.c_void_p(int(iface["data"][0]))
+
+
+def _device_maps(maps, dtypes, ctx):
+    """Device pointers of maps (None stays None) given as CUDA arrays of the given dtypes, or as NumPy arrays, which are
+    uploaded on torch's current stream and returned with the pointers so that they outlive the call that reads them."""
+    import torch
+    ptrs, keep = [], []
+    for m, dt in zip(maps, dtypes):
+        if m is None:
+            ptrs.append(None)
+            continue
+        if not hasattr(m, "__cuda_array_interface__"):
+            m = torch.from_numpy(np.ascontiguousarray(m, dt)).to(torch.device("cuda", ctx.device))
+            keep.append(m)
+        ptrs.append(_cuda_dense(m, np.dtype(dt).str, "map"))
+    return ptrs, keep
+
+
+def _remap_f32(src, map1, map2, interpolation, ctx, out):
+    dh, dw = _float_map_shapes(map1, map2)
+    if hasattr(src, "__cuda_array_interface__"):
+        (m1, m2), keep = _device_maps((map1, map2), (np.float32, np.float32), ctx)
+        return _device_images(src, dw, dh, out, ctx, "remap", lambda s, d: ctx.lib.bevk_remap_f32_stack(
+            ctx.h, *s, m1, m2, *d, _interp(interpolation)))
+    if hasattr(map1, "__cuda_array_interface__") or hasattr(map2, "__cuda_array_interface__"):
+        raise L.BevkError("remap: CUDA maps need a CUDA source image")
+    m1 = np.ascontiguousarray(map1, np.float32)
+    m2 = None if map2 is None else np.ascontiguousarray(map2, np.float32)
+    return _host_image(src, dw, dh, out, lambda s, d, dstride: ctx.lib.bevk_remap_f32(
+        ctx.h, *s, L.vptr(m1), None if m2 is None else L.vptr(m2), dw, dh, d, dstride, _interp(interpolation)))
+
+
+def convert_maps(map1, map2, dstmap1type: int, nninterpolation: bool = False, ctx: L.Context | None = None):
+    """cv2.convertMaps(map1, map2, dstmap1type, nninterpolation=...) between CV_16SC2 (int16[h][w][2] with a uint16[h][w]
+    map2 or None), CV_32FC1 (float32[h][w] planes) and CV_32FC2 (float32[h][w][2], map2 None), bit for bit.  Returns
+    (map1, map2) with map2 None for CV_32FC2 and for CV_16SC2 with nninterpolation.  NumPy maps come back as NumPy
+    arrays; CUDA arrays are converted in place on torch's current stream into new torch tensors.  Converting a type
+    to itself raises BevkError."""
+    ctx = ctx or L.default_context()
+    dst = _map_type(dstmap1type)
+    s1 = _shape(map1)
+    if len(s1) == 3 and s1[2] == 2 and not _is_float32(map1):
+        src = CV_16SC2
+        if map2 is not None and _shape(map2) != s1[:2]:
+            raise L.BevkError(f"map2 of a CV_16SC2 map1 must be uint16{list(s1[:2])} or None")
+    else:
+        src = CV_32FC2 if map2 is None else CV_32FC1
+        _float_map_shapes(map1, map2)
+    h, w = s1[0], s1[1]
+    nn = bool(nninterpolation) and dst == CV_16SC2
+    shapes = {CV_16SC2: [((h, w, 2), np.int16), None if nn else ((h, w), np.uint16)],
+              CV_32FC1: [((h, w), np.float32), ((h, w), np.float32)],
+              CV_32FC2: [((h, w, 2), np.float32), None]}[dst]
+    want = {CV_16SC2: (np.int16, np.uint16), CV_32FC1: (np.float32, np.float32), CV_32FC2: (np.float32, None)}[src]
+    if hasattr(map1, "__cuda_array_interface__"):
+        import torch
+        dev = torch.device("cuda", ctx.device)
+        outs = [None if sd is None else torch.empty(sd[0], dtype=getattr(torch, np.dtype(sd[1]).name), device=dev)
+                for sd in shapes]
+        (p1, p2), keep = _device_maps((map1, map2), want, ctx)
+        from .sharding import _torch_current_stream
+        with ctx.on_stream(_torch_current_stream(ctx.device)):
+            L.check(ctx.lib.bevk_convert_maps(ctx.h, p1, p2, src, w, h, dst, int(nn),
+                                              *[None if o is None else C.c_void_p(o.data_ptr()) for o in outs], 1))
+        return outs[0], outs[1]
+    m1 = np.ascontiguousarray(map1, want[0])
+    m2 = None if map2 is None else np.ascontiguousarray(map2, want[1])
+    outs = [None if sd is None else np.empty(*sd) for sd in shapes]
+    L.check(ctx.lib.bevk_convert_maps(ctx.h, L.vptr(m1), None if m2 is None else L.vptr(m2), src, w, h, dst, int(nn),
+                                      *[None if o is None else L.vptr(o) for o in outs], 0))
+    return outs[0], outs[1]
 
 
 def warp_perspective(src: np.ndarray, H, dsize, flags: int = INTER_LINEAR, ctx: L.Context | None = None,
@@ -543,13 +685,15 @@ class Undistorter:
     rectification rotation (cv2.stereoRectify's R1 / R2), None for eye(3).  A fused fisheye whose rotated rays depend on
     the row is refused (BevkError): cv2 walks those rays with running row sums, which only a map-resident slot follows.
     A fused pinhole slot of such a camera keeps the block starts of cv2's sums (3 bytes per pixel of device memory).
+    m1type: the maps whose cv2.remap bytes every call gives: CV_16SC2 (default), CV_32FC1 or CV_32FC2 (pinhole only, as
+    in cv2).  A map-resident float slot keeps 8 bytes per pixel; a fused one rounds the model's (u, v) to float per pixel.
 
     A bevk_ctx has 8 undistorter slots.  Each live Undistorter owns one slot of its ctx; the slot returns to the
     pool on close() / garbage collection, and a 9th live object on one ctx raises instead of silently taking over a
     slot another object still uses."""
 
     def __init__(self, K, D, P, size, model: str = "fisheye", fused: bool = False, ctx: L.Context | None = None,
-                 slot: int | None = None, R=None):
+                 slot: int | None = None, R=None, m1type: int = CV_16SC2):
         self.ctx = ctx or L.default_context()
         self.slot = None
         live = self.ctx.__dict__.setdefault("_und_slots", set())
@@ -571,7 +715,11 @@ class Undistorter:
         self.w, self.h = int(size[0]), int(size[1])
         d = np.asarray(D, np.float64).reshape(-1)
         m = L.MODEL_FISHEYE if model == "fisheye" else L.MODEL_PINHOLE
-        if R is None:
+        self.m1type = _map_type(m1type)
+        if self.m1type != CV_16SC2:
+            L.check(self.ctx.lib.bevk_undistorter_set_f32(self.ctx.h, slot, m, L.dptr(K), L.dptr(d), int(d.size),
+                                                          _rotation(R), L.dptr(P), self.w, self.h, int(fused), self.m1type))
+        elif R is None:
             L.check(self.ctx.lib.bevk_undistorter_set(self.ctx.h, slot, m, L.dptr(K), L.dptr(d), int(d.size), L.dptr(P),
                                                       self.w, self.h, int(fused)))
         else:
@@ -596,7 +744,12 @@ class Undistorter:
             raise L.BevkError("this Undistorter was closed")
 
     def maps(self):
+        """The maps the slot follows, as cv2.initUndistortRectifyMap builds them with the slot's m1type."""
         self._live()
+        if self.m1type != CV_16SC2:
+            m1, m2 = _float_maps(self.m1type, self.h, self.w)
+            L.check(self.ctx.lib.bevk_undistorter_maps_f32(self.ctx.h, self.slot, L.vptr(m1), None if m2 is None else L.vptr(m2)))
+            return m1, m2
         m1 = np.empty((self.h, self.w, 2), np.int16)
         m2 = np.empty((self.h, self.w), np.uint16)
         L.check(self.ctx.lib.bevk_undistorter_maps(self.ctx.h, self.slot, L.vptr(m1), L.vptr(m2)))

@@ -47,6 +47,9 @@ enum { BEVK_INTER_NEAREST = 0, BEVK_INTER_LINEAR = 1, BEVK_INTER_CUBIC = 2, BEVK
 enum { BEVK_INTER_LINEAR_EXACT = 5, BEVK_INTER_NEAREST_EXACT = 6, BEVK_WARP_INVERSE_MAP = 16 };
 enum { BEVK_MAPS_UNDISTORT = 0, BEVK_MAPS_BEV = 1 };
 enum { BEVK_MODEL_FISHEYE = 0, BEVK_MODEL_PINHOLE = 1 };
+/* cv2's map types (m1type / dstmap1type values): CV_16SC2 (+ a CV_16UC1 map2), CV_32FC1 (map1 = x, map2 = y planes)
+ * and CV_32FC2 (map1 = interleaved x, y; no map2). */
+enum { BEVK_CV_32FC1 = 5, BEVK_CV_16SC2 = 11, BEVK_CV_32FC2 = 13 };
 /* bevk_bev_run flags.  BEVK_FLAG_NV12 / BEVK_FLAG_I420 (exclusive; they combine with BALANCE) say the frames are YUV
  * 4:2:0 in cv2's single-buffer layout, uint8[frame_h*3/2][frame_w] (frame_w, frame_h even, else BEVK_ERR_UNSUPPORTED):
  * the Y plane, then NV12: interleaved U,V rows; I420: the U plane, then the V plane, each frame_w/2 x frame_h/2 and
@@ -112,6 +115,11 @@ int bevk_undistort_map(bevk_ctx *ctx, int model, const double K[9], const double
  * (fisheye) coefficients, zero-padded. */
 int bevk_undistort_rectify_map(bevk_ctx *ctx, int model, const double K[9], const double *D, int n_dist, const double *R,
                                const double P[9], int w, int h, int16_t *map1, uint16_t *map2);
+/* The same maps as cv2 builds them with m1type BEVK_CV_32FC1 (map1, map2: float[h][w], x and y) or BEVK_CV_32FC2
+ * (map1: float[h][w][2], map2 unused): (float)u, (float)v of the very (u, v) the CV_16SC2 build quantises.  A fisheye
+ * ray behind the camera gives +-inf.  The fisheye CV_32FC2, which cv2 refuses, is BEVK_ERR_ARG. */
+int bevk_undistort_rectify_map_f32(bevk_ctx *ctx, int model, const double K[9], const double *D, int n_dist,
+                                   const double *R, const double P[9], int w, int h, int m1type, float *map1, float *map2);
 
 /* ---- K3: cv2.remap(src, map1, map2, interp), BORDER_CONSTANT 0 --------------
  *   surroundBEV.py:110-111,116-117; undistort.py:66; intrinsicCalib.py:193-195
@@ -119,6 +127,24 @@ int bevk_undistort_rectify_map(bevk_ctx *ctx, int model, const double K[9], cons
 int bevk_remap(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t sstride, int channels,
                const int16_t *map1, const uint16_t *map2, int dw, int dh,
                uint8_t *dst, int64_t dstride, int interp);
+/* cv2.remap with float maps: map1, map2 float[dh][dw] (CV_32FC1), or map2 NULL and map1 float[dh][dw][2] (CV_32FC2).
+ * Byte for byte cv2.convertMaps(map1, map2, CV_16SC2, nninterpolation = (interp == NEAREST)) followed by the integer
+ * remap, which is what cv2.remap does: cvRound(x * 32.f) (NEAREST: cvRound(x), half to even, without the integer maps'
+ * nearest-neighbour rule), saturated to int16; NaN, +-inf and values beyond the int range become -32768. */
+int bevk_remap_f32(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t sstride, int channels,
+                   const float *map1, const float *map2, int dw, int dh, uint8_t *dst, int64_t dstride, int interp);
+/* The same for n DEVICE frames through DEVICE maps (dense, as above), with the strides, checks and word path of
+ * bevk_undistort_stack (the maps need 16-byte alignment for the word path); a destination range that overlaps the
+ * source frames or the maps is refused.  Only enqueues; can be graph-captured. */
+int bevk_remap_f32_stack(bevk_ctx *ctx, const void *d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
+                         int channels, int n, const float *d_map1, const float *d_map2, void *d_dst, int64_t dst_image_stride,
+                         int dw, int dh, int64_t dst_row_stride, int interp);
+/* cv2.convertMaps(map1, map2, dstmap1type, nninterpolation) for w x h maps between BEVK_CV_16SC2 (map2: uint16[h][w] or
+ * NULL), BEVK_CV_32FC1 and BEVK_CV_32FC2.  To CV_16SC2 as bevk_remap_f32 converts (dst2 unused with nninterpolation);
+ * from CV_16SC2 as x + (map2 & 31) / 32, exactly.  The same type on both sides is BEVK_ERR_ARG.  on_device = 0: host
+ * maps, converted when the call returns; 1: device maps, only enqueued (graph-capturable). */
+int bevk_convert_maps(bevk_ctx *ctx, const void *map1, const void *map2, int m1type, int w, int h, int dstm1type,
+                      int nninterpolation, void *dst1, void *dst2, int on_device);
 
 /* ---- cached-map undistortion (the per-frame call of InCalibrator.undistort /
  * Camera.undistort / Tools/undistort.py's loop).  The map is built on the device
@@ -133,6 +159,14 @@ int bevk_undistorter_set(bevk_ctx *ctx, int slot, int model, const double K[9], 
 int bevk_undistorter_set_rectify(bevk_ctx *ctx, int slot, int model, const double K[9], const double *D, int n_dist,
                                  const double *R, const double P[9], int dw, int dh, int fused);
 int bevk_undistorter_maps(bevk_ctx *ctx, int slot, int16_t *map1, uint16_t *map2);   /* D2H, for parity tests */
+/* A slot that follows cv2's float maps (m1type BEVK_CV_32FC1 or BEVK_CV_32FC2; the fisheye CV_32FC2 is BEVK_ERR_ARG):
+ * every call on it gives the bytes of cv2.remap with the maps bevk_undistort_rectify_map_f32 builds.  A map-resident
+ * slot keeps those maps (8 bytes per pixel); a fused one rounds the model's (u, v) to float per pixel.  Fused slots are
+ * refused as bevk_undistorter_set_rectify refuses them.  bevk_undistorter_maps_f32 reads such a slot's maps back
+ * (map2 unused for CV_32FC2); bevk_undistorter_maps refuses it, and bevk_undistorter_maps_f32 a CV_16SC2 slot. */
+int bevk_undistorter_set_f32(bevk_ctx *ctx, int slot, int model, const double K[9], const double *D, int n_dist,
+                             const double *R, const double P[9], int dw, int dh, int fused, int m1type);
+int bevk_undistorter_maps_f32(bevk_ctx *ctx, int slot, float *map1, float *map2);
 /* dw x dh: the destination size the caller allocated; must equal the slot's map size (checked, so a stale handle to
  * a slot that was re-set can never make the library write past dst). */
 int bevk_undistort(bevk_ctx *ctx, int slot, const uint8_t *src, int sw, int sh, int64_t sstride, int channels,
