@@ -145,6 +145,10 @@ SIGNATURES = {
     "bevk_launch_count": (C.c_int64, [_p]),
     "bevk_last_kernel_ms": (C.c_int, [_p, C.POINTER(C.c_float)]),
 }
+# the _typed siblings of the image gathers: the same arguments with a cv2 type code in place of the channel count
+SIGNATURES.update({n + "_typed": SIGNATURES[n] for n in (
+    "bevk_remap", "bevk_remap_f32", "bevk_remap_f32_stack", "bevk_undistort", "bevk_undistort_stack_interp",
+    "bevk_warp_perspective", "bevk_warp_affine", "bevk_warp_affine_stack")})
 
 _lib = None
 
@@ -186,11 +190,12 @@ def vptr(a: np.ndarray) -> _p:
     return C.c_void_p(a.ctypes.data)
 
 
-def image_view(img: np.ndarray):
-    """(array to pass, w, h, row stride, channels) for a uint8 HxW or HxWxC image.  Rows
-    must be internally contiguous; otherwise a contiguous copy is made."""
-    if img.dtype != np.uint8:
-        raise BevkError("images must be uint8")
+def image_view(img: np.ndarray, dtypes=(np.uint8,)):
+    """(array to pass, w, h, row stride, channels) for a uint8 HxW or HxWxC image (the image gathers also take the other
+    dtypes they list).  Rows must be internally contiguous; otherwise a contiguous copy is made."""
+    if img.dtype not in dtypes:
+        raise BevkError("images must be uint8" if len(dtypes) == 1 else
+                        f"images must be {', '.join(np.dtype(d).name for d in dtypes)}, got {img.dtype}")
     if img.ndim == 2:
         ch = 1
     elif img.ndim == 3 and img.shape[2] in (1, 3, 4):
@@ -198,7 +203,9 @@ def image_view(img: np.ndarray):
     else:
         raise BevkError(f"unsupported image shape {img.shape}")
     h, w = img.shape[:2]
-    ok = img.strides[1] == ch and (img.ndim == 2 or img.strides[2] == 1) and img.strides[0] >= w * ch
+    es = img.itemsize
+    ok = (img.strides[1] == ch * es and (img.ndim == 2 or img.strides[2] == es) and img.strides[0] >= w * ch * es and
+          img.strides[0] % es == 0)
     if not ok:
         img = np.ascontiguousarray(img)
     return img, w, h, img.strides[0], ch

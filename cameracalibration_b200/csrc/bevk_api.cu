@@ -185,7 +185,8 @@ struct bevk_ctx {
   DevBuf s_src, s_dst, s_m1, s_m2, s_o1, s_o2;   // scratch for the host-pointer entry points
   DevBuf s_xs;                                   // cm.xs of bevk_undistort_map and bevk_bev_set_camera
   DevBuf s_rays;                                 // lx.rays of a map build whose rays depend on the row
-  DevBuf d_wtab;                                 // INTER_CUBIC and INTER_LANCZOS4 weight tables (build_interp_tabs)
+  DevBuf d_wtab;                                 // INTER_CUBIC and INTER_LANCZOS4 weight tables (build_interp_tabs), then
+                                                 // their float 1-D rows for 16U / 16S / 32F sources (build_interp_rows)
   Undistorter und[8];
   // BEV engine
   int n_cam = 0, FW = 0, FH = 0, BW = 0, BH = 0;
@@ -343,8 +344,11 @@ int bevk_ctx_create(int device, bevk_ctx** out) {
   // The weight tables of INTER_CUBIC / INTER_LANCZOS4 are uploaded here, so that the enqueue-only gathers
   // (bevk_undistort_stack, also under graph capture) never allocate or copy.
   static const std::vector<short> tabs = [] {
-    std::vector<short> t(INTERP_TAB_SHORTS);
+    std::vector<short> t(INTERP_TAB_SHORTS + INTERP_ROWS_FLOATS * 2);
     build_interp_tabs(t.data());
+    float rows[INTERP_ROWS_FLOATS];
+    build_interp_rows(rows);
+    memcpy(t.data() + INTERP_TAB_SHORTS, rows, sizeof rows);
     return t;
   }();
   int r = c->d_wtab.ensure(tabs.size() * sizeof(short));
@@ -554,7 +558,28 @@ int bevk_undistort_map(bevk_ctx* c, int model, const double K[9], const double* 
 // k_gather4's word path: 32-bit tap loads need every source row to start on a 4-byte boundary (base, row pitch and, over
 // a batch, image stride), and its 32-bit stores the same of the destination (padded rows are fine).  Anything else,
 // e.g. caller memory at an odd address, takes k_gather's byte path.
-static bool gather4_ok(const GatherArgs& a, int channels, int interp, int mode) {
+// An image's cv2 type (CV_8UC1 .. CV_32FC4): the depth (CV_8U 0, CV_16U 2, CV_16S 3, CV_32F 5), the channels and the bytes
+// of one element.  Rows, images and base pointers of a wider depth are element-aligned (check_image).
+struct PixType {
+  int depth, channels, esize;
+  long long px() const { return (long long)channels * esize; }   // bytes per pixel
+};
+static PixType u8(int channels) { return PixType{0, channels, 1}; }
+
+// a cv2 type code of the image gathers: 8U, 16U, 16S and 32F; 8S and 16F, which cv2.remap refuses, and 64F are refused
+static int pix_type(int type, PixType* t) {
+  if (type < 0 || type >= (512 << 3)) return fail(BEVK_ERR_ARG, "image type %d is not a cv2 type code", type);
+  const int depth = type & 7;
+  static const int esize[8] = {1, 0, 2, 2, 0, 4, 0, 0};
+  if (!esize[depth])
+    return fail(BEVK_ERR_UNSUPPORTED, "image type %d: depth %d; the gathers take CV_8U, CV_16U, CV_16S and CV_32F images",
+                type, depth);
+  *t = PixType{depth, (type >> 3) + 1, esize[depth]};
+  return BEVK_OK;
+}
+
+static bool gather4_ok(const GatherArgs& a, PixType t, int interp, int mode) {
+  const int channels = t.esize == 1 ? t.channels : 0;   // the word path is 8-bit only
   const uintptr_t al = reinterpret_cast<uintptr_t>(a.src) | reinterpret_cast<uintptr_t>(a.dst) | (uintptr_t)a.spitch |
                        (uintptr_t)a.dpitch | (a.n > 1 ? (uintptr_t)(a.sistride | a.distride) : 0);
   return channels == 3 && interp == BEVK_INTER_LINEAR && (a.dw % 4) == 0 && (al & 3) == 0 &&
@@ -603,20 +628,16 @@ static Args with_frames(Args a, const ImageBatch& b) {
   return a;
 }
 
-template <int MODE, int LENS>
-static void gather(bevk_ctx* c, const GatherArgs& a, int channels, int interp, bool words, unsigned gz) {
-  if (words) {
-    // 4 output pixels per thread, 32-bit tap loads and 12-byte stores
-    const dim3 g4((a.dw / 4 + 31) / 32, (a.dh + 7) / 8, gz);
-    if (a.n == 1) k_gather4<MODE, 1, LENS><<<g4, 256, 0, c->stream>>>(a);
-    else k_gather4<MODE, GATHER_NB, LENS><<<g4, 256, 0, c->stream>>>(a);
-    return;
-  }
+template <int MODE, int LENS, class T>
+static void gather_t(bevk_ctx* c, const GatherArgs& a, int channels, int interp, unsigned gz) {
   const dim3 g((a.dw + 31) / 32, (a.dh + 7) / 8, gz);
-#define GO(C, L) k_gather<MODE, C, L, LENS><<<g, 256, 0, c->stream>>>(a)
-#define TAPS(C, KS) k_gather_taps<MODE, C, KS, LENS><<<g, 256, 0, c->stream>>>(a, wt)
+#define GO(C, L) k_gather<MODE, C, L, LENS, T><<<g, 256, 0, c->stream>>>(a)
+#define TAPS(C, KS) k_gather_taps<MODE, C, KS, LENS, T><<<g, 256, 0, c->stream>>>(a, wt)
   if (interp == BEVK_INTER_CUBIC || interp == BEVK_INTER_LANCZOS4) {
-    const short* wt = c->d_wtab.as<short>() + (interp == BEVK_INTER_CUBIC ? 0 : INTERP_TAB_LANCZOS4);
+    const TapWeights<T>* wt;
+    if constexpr (sizeof(T) == 1) wt = c->d_wtab.as<short>() + (interp == BEVK_INTER_CUBIC ? 0 : INTERP_TAB_LANCZOS4);
+    else wt = reinterpret_cast<const float*>(c->d_wtab.as<short>() + INTERP_TAB_SHORTS) +
+              (interp == BEVK_INTER_CUBIC ? 0 : INTERP_ROWS_LANCZOS4);
     if (interp == BEVK_INTER_CUBIC) {
       if (channels == 1) TAPS(1, 4); else if (channels == 3) TAPS(3, 4); else TAPS(4, 4);
     } else {
@@ -629,6 +650,23 @@ static void gather(bevk_ctx* c, const GatherArgs& a, int channels, int interp, b
   }
 #undef GO
 #undef TAPS
+}
+
+template <int MODE, int LENS>
+static void gather(bevk_ctx* c, const GatherArgs& a, PixType t, int interp, bool words, unsigned gz) {
+  if (words) {
+    // 4 output pixels per thread, 32-bit tap loads and 12-byte stores
+    const dim3 g4((a.dw / 4 + 31) / 32, (a.dh + 7) / 8, gz);
+    if (a.n == 1) k_gather4<MODE, 1, LENS><<<g4, 256, 0, c->stream>>>(a);
+    else k_gather4<MODE, GATHER_NB, LENS><<<g4, 256, 0, c->stream>>>(a);
+    return;
+  }
+  switch (t.depth) {
+    case 0: gather_t<MODE, LENS, uint8_t>(c, a, t.channels, interp, gz); break;
+    case 2: gather_t<MODE, LENS, uint16_t>(c, a, t.channels, interp, gz); break;
+    case 3: gather_t<MODE, LENS, int16_t>(c, a, t.channels, interp, gz); break;
+    default: gather_t<MODE, LENS, float>(c, a, t.channels, interp, gz);
+  }
 }
 
 template <int C, int KIND>
@@ -649,8 +687,9 @@ static void resize_k(bevk_ctx* c, const ResizeArgs& a, int kind, dim3 g) {
 
 // Enqueue op over b.n >= 1 frames.  grid.z = frame groups of GATHER_NB, at most 65535 per launch; a single frame takes
 // the kernels' single-frame form (NB = 1), which keeps the register count and speed of the one-frame kernel.
-static int launch(bevk_ctx* c, const ImageOp& op, const ImageBatch& b, int channels) {
-  const bool words = op.mode != OP_RESIZE && gather4_ok(with_frames(op.g, b), channels, op.interp, op.mode);
+static int launch(bevk_ctx* c, const ImageOp& op, const ImageBatch& b, PixType t) {
+  const bool words = op.mode != OP_RESIZE && gather4_ok(with_frames(op.g, b), t, op.interp, op.mode);
+  const int channels = t.channels;
   const int per_launch = 65535 * GATHER_NB;
   for (int f0 = 0; f0 < b.n; f0 += per_launch) {
     ImageBatch p = b;
@@ -661,17 +700,17 @@ static int launch(bevk_ctx* c, const ImageOp& op, const ImageBatch& b, int chann
     if (op.mode != OP_RESIZE) {
       const GatherArgs a = with_frames(op.g, p);
       switch (op.mode) {
-        case 0: gather<0, 0>(c, a, channels, op.interp, words, gz); break;
+        case 0: gather<0, 0>(c, a, t, op.interp, words, gz); break;
         case 1:
-          if (op.lens) gather<1, 1>(c, a, channels, op.interp, words, gz);
-          else gather<1, 0>(c, a, channels, op.interp, words, gz);
+          if (op.lens) gather<1, 1>(c, a, t, op.interp, words, gz);
+          else gather<1, 0>(c, a, t, op.interp, words, gz);
           break;
-        case 2: gather<2, 0>(c, a, channels, op.interp, words, gz); break;
-        case 3: gather<3, 0>(c, a, channels, op.interp, words, gz); break;
-        case 4: gather<4, 0>(c, a, channels, op.interp, words, gz); break;
+        case 2: gather<2, 0>(c, a, t, op.interp, words, gz); break;
+        case 3: gather<3, 0>(c, a, t, op.interp, words, gz); break;
+        case 4: gather<4, 0>(c, a, t, op.interp, words, gz); break;
         default:
-          if (op.lens) gather<5, 1>(c, a, channels, op.interp, words, gz);
-          else gather<5, 0>(c, a, channels, op.interp, words, gz);
+          if (op.lens) gather<5, 1>(c, a, t, op.interp, words, gz);
+          else gather<5, 0>(c, a, t, op.interp, words, gz);
       }
     } else {
       const ResizeArgs a = with_frames(op.r, p);
@@ -776,23 +815,26 @@ static int check_op_size(const ImageOp& op, int dw, int dh) {
   return BEVK_OK;
 }
 
-static int check_image(const void* p, int w, int h, int64_t stride, int channels, const char* what) {
+static int check_image(const void* p, int w, int h, int64_t stride, PixType t, const char* what) {
   if (!p) return fail(BEVK_ERR_ARG, "null %s", what);
   if (w <= 0 || h <= 0) return fail(BEVK_ERR_ARG, "bad %s size %dx%d", what, w, h);
-  if (channels != 1 && channels != 3 && channels != 4) return fail(BEVK_ERR_UNSUPPORTED, "channels must be 1, 3 or 4");
-  if (stride < (int64_t)w * channels) return fail(BEVK_ERR_ARG, "%s stride %lld < row bytes", what, (long long)stride);
+  if (t.channels != 1 && t.channels != 3 && t.channels != 4) return fail(BEVK_ERR_UNSUPPORTED, "channels must be 1, 3 or 4");
+  if (stride < (int64_t)w * t.px()) return fail(BEVK_ERR_ARG, "%s stride %lld < row bytes", what, (long long)stride);
+  if ((reinterpret_cast<uintptr_t>(p) | (uintptr_t)stride) % t.esize)
+    return fail(BEVK_ERR_ARG, "%s base %p and row stride %lld must be multiples of the %d-byte element", what, p,
+                (long long)stride, t.esize);
   return BEVK_OK;
 }
 
-static int upload_image(bevk_ctx* c, DevBuf& buf, const uint8_t* src, int w, int h, int64_t stride, int channels) {
-  const size_t row = (size_t)w * channels;
+static int upload_image(bevk_ctx* c, DevBuf& buf, const void* src, int w, int h, int64_t stride, PixType t) {
+  const size_t row = (size_t)(w * t.px());
   RET(buf.ensure(row * h));
   if ((size_t)stride == row) CU(cudaMemcpyAsync(buf.p, src, row * h, cudaMemcpyHostToDevice, c->stream));   // dense: one DMA
   else CU(cudaMemcpy2DAsync(buf.p, row, src, (size_t)stride, row, h, cudaMemcpyHostToDevice, c->stream));
   return BEVK_OK;
 }
-static int download_image(bevk_ctx* c, const DevBuf& buf, uint8_t* dst, int w, int h, int64_t stride, int channels) {
-  const size_t row = (size_t)w * channels;
+static int download_image(bevk_ctx* c, const DevBuf& buf, void* dst, int w, int h, int64_t stride, PixType t) {
+  const size_t row = (size_t)(w * t.px());
   if ((size_t)stride == row) CU(cudaMemcpyAsync(dst, buf.p, row * h, cudaMemcpyDeviceToHost, c->stream));
   else CU(cudaMemcpy2DAsync(dst, (size_t)stride, buf.p, row, row, h, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaStreamSynchronize(c->stream));
@@ -800,11 +842,10 @@ static int download_image(bevk_ctx* c, const DevBuf& buf, uint8_t* dst, int w, i
 }
 
 // Host path, without the read-back: a checked host frame uploaded to c->s_src and op run into c->s_dst.  Both are dense
-// (row pitch w * channels), so k_gather4's word-path choice sees the same pitches whatever the caller's strides.
-static int host_launch(bevk_ctx* c, ImageOp op, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, int dw,
-                       int dh) {
-  RET(upload_image(c, c->s_src, src, sw, sh, sstride, channels));
-  RET(c->s_dst.ensure((size_t)dw * dh * channels));
+// (row pitch w times the pixel bytes), so k_gather4's word-path choice sees the same pitches whatever the caller's strides.
+static int host_launch(bevk_ctx* c, ImageOp op, const void* src, int sw, int sh, int64_t sstride, PixType t, int dw, int dh) {
+  RET(upload_image(c, c->s_src, src, sw, sh, sstride, t));
+  RET(c->s_dst.ensure((size_t)dw * dh * t.px()));
   if (op.hmap1) {
     const size_t n = (size_t)dw * dh;
     RET(c->s_m1.ensure(n * 4));
@@ -821,40 +862,43 @@ static int host_launch(bevk_ctx* c, ImageOp op, const uint8_t* src, int sw, int 
     if (op.hfmap2) CU(cudaMemcpyAsync(c->s_m2.p, op.hfmap2, n * 4, cudaMemcpyHostToDevice, c->stream));
     op.g.fmap1 = c->s_m1.as<float>(); op.g.fmap2 = op.hfmap2 ? c->s_m2.as<float>() : nullptr;
   }
-  const ImageBatch b{c->s_src.as<uint8_t>(), sw, sh, (long long)sw * channels, 0,
-                     c->s_dst.as<uint8_t>(), dw, dh, (long long)dw * channels, 0, 1};
-  return launch(c, op, b, channels);
+  const ImageBatch b{c->s_src.as<uint8_t>(), sw, sh, sw * t.px(), 0, c->s_dst.as<uint8_t>(), dw, dh, dw * t.px(), 0, 1};
+  return launch(c, op, b, t);
 }
 
 // Host path: one host image through op into another, which the call has written when it returns.
-static int host_image(bevk_ctx* c, const ImageOp& op, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
-                      uint8_t* dst, int dw, int dh, int64_t dstride) {
-  RET(check_image(src, sw, sh, sstride, channels, "src"));
+static int host_image(bevk_ctx* c, const ImageOp& op, const void* src, int sw, int sh, int64_t sstride, PixType t, void* dst,
+                      int dw, int dh, int64_t dstride) {
+  RET(check_image(src, sw, sh, sstride, t, "src"));
   RET(check_op_size(op, dw, dh));
-  RET(check_image(dst, dw, dh, dstride, channels, "dst"));
-  RET(host_launch(c, op, src, sw, sh, sstride, channels, dw, dh));
-  return download_image(c, c->s_dst, dst, dw, dh, dstride, channels);
+  RET(check_image(dst, dw, dh, dstride, t, "dst"));
+  RET(host_launch(c, op, src, sw, sh, sstride, t, dw, dh));
+  return download_image(c, c->s_dst, dst, dw, dh, dstride, t);
 }
 
 // The source side of the device-batch calls: a frame, n >= 1, and an image stride that covers an image when n > 1.
-static int check_stack_src(const void* d_src, int64_t sis, int sw, int sh, int64_t srs, int channels, int n) {
+static int check_stack_src(const void* d_src, int64_t sis, int sw, int sh, int64_t srs, PixType t, int n) {
   if (n < 1) return fail(BEVK_ERR_ARG, "n must be >= 1, got %d", n);
-  RET(check_image(d_src, sw, sh, srs, channels, "src"));
-  if (n > 1 && sis < (int64_t)(sh - 1) * srs + (int64_t)sw * channels)
+  RET(check_image(d_src, sw, sh, srs, t, "src"));
+  if (n > 1 && sis < (int64_t)(sh - 1) * srs + sw * t.px())
     return fail(BEVK_ERR_ARG, "src image stride %lld is smaller than one image", (long long)sis);
+  if (n > 1 && sis % t.esize)
+    return fail(BEVK_ERR_ARG, "src image stride %lld must be a multiple of the %d-byte element", (long long)sis, t.esize);
   return BEVK_OK;
 }
 
 // The destination side of the device-batch calls, given a checked source: rows, an image stride that covers an image
 // (n > 1), and byte ranges [first, last] of the whole batch on each side that do not overlap -- an output that overwrites
 // frames still to be read is refused.
-static int check_stack_dst(const void* d_src, int64_t sis, int sw, int sh, int64_t srs, int channels, int n, const void* d_dst,
+static int check_stack_dst(const void* d_src, int64_t sis, int sw, int sh, int64_t srs, PixType t, int n, const void* d_dst,
                            int64_t dis, int dw, int dh, int64_t drs) {
-  RET(check_image(d_dst, dw, dh, drs, channels, "dst"));
-  const int64_t dimg = (int64_t)(dh - 1) * drs + (int64_t)dw * channels;
+  RET(check_image(d_dst, dw, dh, drs, t, "dst"));
+  const int64_t dimg = (int64_t)(dh - 1) * drs + dw * t.px();
   if (n > 1 && dis < dimg) return fail(BEVK_ERR_ARG, "dst image stride %lld is smaller than one image", (long long)dis);
+  if (n > 1 && dis % t.esize)
+    return fail(BEVK_ERR_ARG, "dst image stride %lld must be a multiple of the %d-byte element", (long long)dis, t.esize);
   const uintptr_t s0 = reinterpret_cast<uintptr_t>(d_src), d0 = reinterpret_cast<uintptr_t>(d_dst);
-  const uintptr_t s1 = s0 + (uintptr_t)(n > 1 ? (n - 1) * sis : 0) + (uintptr_t)((int64_t)(sh - 1) * srs + (int64_t)sw * channels);
+  const uintptr_t s1 = s0 + (uintptr_t)(n > 1 ? (n - 1) * sis : 0) + (uintptr_t)((int64_t)(sh - 1) * srs + sw * t.px());
   const uintptr_t d1 = d0 + (uintptr_t)(n > 1 ? (n - 1) * dis : 0) + (uintptr_t)dimg;
   if (s0 < d1 && d0 < s1) return fail(BEVK_ERR_ARG, "the destination range overlaps the source frames");
   return BEVK_OK;
@@ -868,47 +912,85 @@ static ImageBatch device_batch(const void* d_src, int64_t sis, int sw, int sh, i
 }
 
 // Device path: n device frames through op, enqueued only.  It allocates and copies nothing, so a graph can capture it.
-static int device_image(bevk_ctx* c, const ImageOp& op, const void* d_src, int64_t sis, int sw, int sh, int64_t srs, int channels,
+static int device_image(bevk_ctx* c, const ImageOp& op, const void* d_src, int64_t sis, int sw, int sh, int64_t srs, PixType t,
                         int n, void* d_dst, int64_t dis, int dw, int dh, int64_t drs) {
-  RET(check_stack_src(d_src, sis, sw, sh, srs, channels, n));
+  RET(check_stack_src(d_src, sis, sw, sh, srs, t, n));
   RET(check_op_size(op, dw, dh));
-  RET(check_stack_dst(d_src, sis, sw, sh, srs, channels, n, d_dst, dis, dw, dh, drs));
+  RET(check_stack_dst(d_src, sis, sw, sh, srs, t, n, d_dst, dis, dw, dh, drs));
   if (op.mode == 4 && op.slot < 0) {   // the caller's float maps: the images written must not overwrite them
     const uintptr_t d0 = reinterpret_cast<uintptr_t>(d_dst);
-    const uintptr_t d1 = d0 + (uintptr_t)(n > 1 ? (n - 1) * dis : 0) + (uintptr_t)((int64_t)(dh - 1) * drs + (int64_t)dw * channels);
+    const uintptr_t d1 = d0 + (uintptr_t)(n > 1 ? (n - 1) * dis : 0) + (uintptr_t)((int64_t)(dh - 1) * drs + dw * t.px());
     const size_t np = (size_t)dw * dh;
     const uintptr_t x0 = reinterpret_cast<uintptr_t>(op.g.fmap1), x1 = x0 + np * (op.g.fmap2 ? 4 : 8);
     const uintptr_t y0 = reinterpret_cast<uintptr_t>(op.g.fmap2), y1 = op.g.fmap2 ? y0 + np * 4 : y0;
     if ((x0 < d1 && d0 < x1) || (y0 < d1 && d0 < y1)) return fail(BEVK_ERR_ARG, "the destination range overlaps the maps");
   }
-  return launch(c, op, device_batch(d_src, sis, sw, sh, srs, n, d_dst, dis, dw, dh, drs), channels);
+  return launch(c, op, device_batch(d_src, sis, sw, sh, srs, n, d_dst, dis, dw, dh, drs), t);
 }
 
 // ---- the entry points
+// Each uint8 entry point is its _typed sibling at CV_8UC(channels); the sibling reads a cv2 type code (pix_type) first.
+static int remap_image(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, PixType t, const int16_t* map1,
+                       const uint16_t* map2, int dw, int dh, void* dst, int64_t dstride, int interp) {
+  ImageOp op;
+  RET(remap_op(map1, map2, interp, &op));
+  return host_image(c, op, src, sw, sh, sstride, t, dst, dw, dh, dstride);
+}
 int bevk_remap(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, const int16_t* map1,
                const uint16_t* map2, int dw, int dh, uint8_t* dst, int64_t dstride, int interp) {
   RET(use(c));
-  ImageOp op;
-  RET(remap_op(map1, map2, interp, &op));
-  return host_image(c, op, src, sw, sh, sstride, channels, dst, dw, dh, dstride);
+  return remap_image(c, src, sw, sh, sstride, u8(channels), map1, map2, dw, dh, dst, dstride, interp);
+}
+int bevk_remap_typed(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, int type, const int16_t* map1,
+                     const uint16_t* map2, int dw, int dh, void* dst, int64_t dstride, int interp) {
+  RET(use(c));
+  PixType t;
+  RET(pix_type(type, &t));
+  return remap_image(c, src, sw, sh, sstride, t, map1, map2, dw, dh, dst, dstride, interp);
 }
 
+static int remap_f32_image(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, PixType t, const float* map1,
+                           const float* map2, int dw, int dh, void* dst, int64_t dstride, int interp) {
+  ImageOp op;
+  RET(remap_f32_op(map1, map2, interp, true, &op));
+  return host_image(c, op, src, sw, sh, sstride, t, dst, dw, dh, dstride);
+}
 int bevk_remap_f32(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, const float* map1,
                    const float* map2, int dw, int dh, uint8_t* dst, int64_t dstride, int interp) {
   RET(use(c));
-  ImageOp op;
-  RET(remap_f32_op(map1, map2, interp, true, &op));
-  return host_image(c, op, src, sw, sh, sstride, channels, dst, dw, dh, dstride);
+  return remap_f32_image(c, src, sw, sh, sstride, u8(channels), map1, map2, dw, dh, dst, dstride, interp);
+}
+int bevk_remap_f32_typed(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, int type, const float* map1,
+                         const float* map2, int dw, int dh, void* dst, int64_t dstride, int interp) {
+  RET(use(c));
+  PixType t;
+  RET(pix_type(type, &t));
+  return remap_f32_image(c, src, sw, sh, sstride, t, map1, map2, dw, dh, dst, dstride, interp);
 }
 
+static int remap_f32_frames(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
+                            PixType t, int n, const float* d_map1, const float* d_map2, void* d_dst, int64_t dst_image_stride,
+                            int dw, int dh, int64_t dst_row_stride, int interp) {
+  ImageOp op;
+  RET(remap_f32_op(d_map1, d_map2, interp, false, &op));
+  return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, t, n, d_dst, dst_image_stride, dw, dh,
+                      dst_row_stride);
+}
 int bevk_remap_f32_stack(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
                          int channels, int n, const float* d_map1, const float* d_map2, void* d_dst, int64_t dst_image_stride,
                          int dw, int dh, int64_t dst_row_stride, int interp) {
   RET(use(c));
-  ImageOp op;
-  RET(remap_f32_op(d_map1, d_map2, interp, false, &op));
-  return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
-                      dst_row_stride);
+  return remap_f32_frames(c, d_src, src_image_stride, sw, sh, src_row_stride, u8(channels), n, d_map1, d_map2, d_dst,
+                          dst_image_stride, dw, dh, dst_row_stride, interp);
+}
+int bevk_remap_f32_stack_typed(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
+                               int type, int n, const float* d_map1, const float* d_map2, void* d_dst, int64_t dst_image_stride,
+                               int dw, int dh, int64_t dst_row_stride, int interp) {
+  RET(use(c));
+  PixType t;
+  RET(pix_type(type, &t));
+  return remap_f32_frames(c, d_src, src_image_stride, sw, sh, src_row_stride, t, n, d_map1, d_map2, d_dst, dst_image_stride,
+                          dw, dh, dst_row_stride, interp);
 }
 
 // ------------------------------------------------------------------ cached-map undistortion
@@ -1029,12 +1111,23 @@ int bevk_convert_maps(bevk_ctx* c, const void* map1, const void* map2, int m1typ
   return BEVK_OK;
 }
 
+static int undistort_image(bevk_ctx* c, int slot, const void* src, int sw, int sh, int64_t sstride, PixType t, void* dst, int dw,
+                           int dh, int64_t dstride, int interp) {
+  ImageOp op;
+  RET(undistort_op(c, slot, interp, &op));
+  return host_image(c, op, src, sw, sh, sstride, t, dst, dw, dh, dstride);
+}
 int bevk_undistort(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
                    uint8_t* dst, int dw, int dh, int64_t dstride, int interp) {
   RET(use(c));
-  ImageOp op;
-  RET(undistort_op(c, slot, interp, &op));
-  return host_image(c, op, src, sw, sh, sstride, channels, dst, dw, dh, dstride);
+  return undistort_image(c, slot, src, sw, sh, sstride, u8(channels), dst, dw, dh, dstride, interp);
+}
+int bevk_undistort_typed(bevk_ctx* c, int slot, const void* src, int sw, int sh, int64_t sstride, int type, void* dst, int dw,
+                         int dh, int64_t dstride, int interp) {
+  RET(use(c));
+  PixType t;
+  RET(pix_type(type, &t));
+  return undistort_image(c, slot, src, sw, sh, sstride, t, dst, dw, dh, dstride, interp);
 }
 
 // ------------------------------------------------------------------ undistortion of device frame batches
@@ -1050,44 +1143,114 @@ int bevk_undistort_stack(bevk_ctx* c, int slot, const void* d_src, int64_t src_i
                                      dst_image_stride, dw, dh, dst_row_stride, interp);
 }
 
+static int undistort_frames(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh,
+                            int64_t src_row_stride, PixType t, int n, void* d_dst, int64_t dst_image_stride, int dw, int dh,
+                            int64_t dst_row_stride, int interp) {
+  ImageOp op;
+  RET(undistort_op(c, slot, interp, &op));
+  return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, t, n, d_dst, dst_image_stride, dw, dh,
+                      dst_row_stride);
+}
 int bevk_undistort_stack_interp(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh,
                                 int64_t src_row_stride, int channels, int n, void* d_dst, int64_t dst_image_stride, int dw, int dh,
                                 int64_t dst_row_stride, int interp) {
   RET(use(c));
-  ImageOp op;
-  RET(undistort_op(c, slot, interp, &op));
-  return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
-                      dst_row_stride);
+  return undistort_frames(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, u8(channels), n, d_dst, dst_image_stride,
+                          dw, dh, dst_row_stride, interp);
+}
+int bevk_undistort_stack_interp_typed(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh,
+                                      int64_t src_row_stride, int type, int n, void* d_dst, int64_t dst_image_stride, int dw,
+                                      int dh, int64_t dst_row_stride, int interp) {
+  RET(use(c));
+  PixType t;
+  RET(pix_type(type, &t));
+  return undistort_frames(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, t, n, d_dst, dst_image_stride, dw, dh,
+                          dst_row_stride, interp);
 }
 
 int bevk_undistort_last_path(bevk_ctx* c) { return c ? c->gather_path : 0; }
 
 // ------------------------------------------------------------------ K4 / K2
+// cv2 4.13's warpPerspective and warpAffine compute a few wider-source cases with warp-specific bodies whose pixels
+// differ from cv2.remap through the same 1/32-px positions, which is what the gathers compute: warpPerspective LINEAR
+// (and AREA, read as LINEAR) at 16UC3 / 16UC4 and NEAREST at 32FC1 / 32FC4; warpAffine NEAREST at 16UC4 and at 16S with
+// any channel count, with or without WARP_INVERSE_MAP.  Exactly those are refused rather than given other pixels than
+// cv2's; every other depth, channel count and interpolation follows remap (DESIGN.md section 2).
+static int check_warp_depth(const ImageOp& op, PixType t) {
+  const bool nearest = op.interp == BEVK_INTER_NEAREST, linear = op.interp == BEVK_INTER_LINEAR;
+  const bool leaves = op.mode == 2 ? (t.depth == 2 && linear && t.channels != 1) || (t.depth == 5 && nearest && t.channels != 3)
+                                   : nearest && (t.depth == 3 || (t.depth == 2 && t.channels == 4));
+  if (leaves)
+    return fail(BEVK_ERR_UNSUPPORTED, "%s with interp %d at depth %d, %d channels: cv2 computes it with another body than "
+                "cv2.remap's", op.mode == 2 ? "warpPerspective" : "warpAffine", op.interp, t.depth, t.channels);
+  return BEVK_OK;
+}
+
+static int perspective_image(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, PixType t, const double H[9],
+                             void* dst, int dw, int dh, int64_t dstride, int interp) {
+  ImageOp op;
+  RET(perspective_op(H, interp, &op));
+  RET(check_warp_depth(op, t));
+  return host_image(c, op, src, sw, sh, sstride, t, dst, dw, dh, dstride);
+}
 int bevk_warp_perspective(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
                           const double H[9], uint8_t* dst, int dw, int dh, int64_t dstride, int interp) {
   RET(use(c));
-  ImageOp op;
-  RET(perspective_op(H, interp, &op));
-  return host_image(c, op, src, sw, sh, sstride, channels, dst, dw, dh, dstride);
+  return perspective_image(c, src, sw, sh, sstride, u8(channels), H, dst, dw, dh, dstride, interp);
+}
+int bevk_warp_perspective_typed(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, int type, const double H[9],
+                                void* dst, int dw, int dh, int64_t dstride, int interp) {
+  RET(use(c));
+  PixType t;
+  RET(pix_type(type, &t));
+  return perspective_image(c, src, sw, sh, sstride, t, H, dst, dw, dh, dstride, interp);
 }
 
 // ------------------------------------------------------------------ cv2.warpAffine
+static int affine_image(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, PixType t, const double M[6], void* dst,
+                        int dw, int dh, int64_t dstride, int flags) {
+  ImageOp op;
+  RET(affine_op(M, flags, &op));
+  RET(check_warp_depth(op, t));
+  return host_image(c, op, src, sw, sh, sstride, t, dst, dw, dh, dstride);
+}
 int bevk_warp_affine(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, const double M[6],
                      uint8_t* dst, int dw, int dh, int64_t dstride, int flags) {
   RET(use(c));
-  ImageOp op;
-  RET(affine_op(M, flags, &op));
-  return host_image(c, op, src, sw, sh, sstride, channels, dst, dw, dh, dstride);
+  return affine_image(c, src, sw, sh, sstride, u8(channels), M, dst, dw, dh, dstride, flags);
+}
+int bevk_warp_affine_typed(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, int type, const double M[6], void* dst,
+                           int dw, int dh, int64_t dstride, int flags) {
+  RET(use(c));
+  PixType t;
+  RET(pix_type(type, &t));
+  return affine_image(c, src, sw, sh, sstride, t, M, dst, dw, dh, dstride, flags);
 }
 
+static int affine_frames(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
+                         PixType t, int n, const double M[6], void* d_dst, int64_t dst_image_stride, int dw, int dh,
+                         int64_t dst_row_stride, int flags) {
+  ImageOp op;
+  RET(affine_op(M, flags, &op));
+  RET(check_warp_depth(op, t));
+  return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, t, n, d_dst, dst_image_stride, dw, dh,
+                      dst_row_stride);
+}
 int bevk_warp_affine_stack(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
                            int channels, int n, const double M[6], void* d_dst, int64_t dst_image_stride, int dw, int dh,
                            int64_t dst_row_stride, int flags) {
   RET(use(c));
-  ImageOp op;
-  RET(affine_op(M, flags, &op));
-  return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
-                      dst_row_stride);
+  return affine_frames(c, d_src, src_image_stride, sw, sh, src_row_stride, u8(channels), n, M, d_dst, dst_image_stride, dw, dh,
+                       dst_row_stride, flags);
+}
+int bevk_warp_affine_stack_typed(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
+                                 int type, int n, const double M[6], void* d_dst, int64_t dst_image_stride, int dw, int dh,
+                                 int64_t dst_row_stride, int flags) {
+  RET(use(c));
+  PixType t;
+  RET(pix_type(type, &t));
+  return affine_frames(c, d_src, src_image_stride, sw, sh, src_row_stride, t, n, M, d_dst, dst_image_stride, dw, dh,
+                       dst_row_stride, flags);
 }
 
 // ------------------------------------------------------------------ cv2.resize
@@ -1096,7 +1259,7 @@ int bevk_resize(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride
   RET(use(c));
   ImageOp op;
   RET(resize_op(sw, sh, dw, dh, fx, fy, interp, &op));
-  return host_image(c, op, src, sw, sh, sstride, channels, dst, dw, dh, dstride);
+  return host_image(c, op, src, sw, sh, sstride, u8(channels), dst, dw, dh, dstride);
 }
 
 int bevk_resize_stack(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
@@ -1105,7 +1268,7 @@ int bevk_resize_stack(bevk_ctx* c, const void* d_src, int64_t src_image_stride, 
   RET(use(c));
   ImageOp op;
   RET(resize_op(sw, sh, dw, dh, fx, fy, interp, &op));
-  return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, channels, n, d_dst, dst_image_stride, dw, dh,
+  return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, u8(channels), n, d_dst, dst_image_stride, dw, dh,
                       dst_row_stride);
 }
 
@@ -3347,11 +3510,11 @@ int bevk_undistort_jpeg(bevk_ctx* c, int slot, const uint8_t* src, int sw, int s
   RET(use(c));
   ImageOp op;
   RET(undistort_op(c, slot, interp, &op));
-  RET(check_image(src, sw, sh, sstride, 3, "src"));
+  RET(check_image(src, sw, sh, sstride, u8(3), "src"));
   RET(jpeg_size_check(op.dw, op.dh));
   const jpeg::Opts o = jpeg_ctx_opts(c, quality);
   return enc_chunks(c, "JPEG", 1, 1, true, out, capacity, size, [&](int, int, int s) -> int {
-    RET(host_launch(c, op, src, sw, sh, sstride, 3, op.dw, op.dh));
+    RET(host_launch(c, op, src, sw, sh, sstride, u8(3), op.dw, op.dh));
     return jpeg_enqueue(c, s, EncIn{c->s_dst.p, 0, (long long)op.dw * 3}, 1, op.dw, op.dh, o);
   });
 }
@@ -3365,7 +3528,7 @@ int bevk_undistort_stack_jpeg(bevk_ctx* c, int slot, const void* d_src, int64_t 
   RET(use(c));
   ImageOp op;
   RET(undistort_op(c, slot, interp, &op));
-  RET(check_stack_src(d_src, src_image_stride, sw, sh, src_row_stride, 3, n));
+  RET(check_stack_src(d_src, src_image_stride, sw, sh, src_row_stride, u8(3), n));
   const int dw = op.dw, dh = op.dh;
   RET(jpeg_size_check(dw, dh));
   const jpeg::Opts o = jpeg_ctx_opts(c, quality);
@@ -3378,7 +3541,7 @@ int bevk_undistort_stack_jpeg(bevk_ctx* c, int slot, const void* d_src, int64_t 
     part.src += (long long)b0 * b.sistride;
     part.n = nb;
     part.dst = c->s_dst.as<uint8_t>(); part.distride = ibytes;
-    RET(launch(c, op, part, 3));
+    RET(launch(c, op, part, u8(3)));
     return jpeg_enqueue(c, s, EncIn{c->s_dst.p, ibytes, (long long)dw * 3}, nb, dw, dh, o);
   });
 }

@@ -97,6 +97,45 @@ __host__ __device__ __forceinline__ int tap8(const uint8_t* p) {
 #endif
 }
 
+// ---- The 16U, 16S and 32F sources: cv2 takes its float tables there (initInterTab2D without the fixed-point form),
+// whose 2-D entry is vy[k1] * vx[k2] rounded to float, with no fix-up.  The 1-D rows are all the gathers keep: cubic
+// (32 rows of 4) at 0, Lanczos4 (32 rows of 8) at INTERP_ROWS_LANCZOS4; each pixel forms its products from two of them.
+constexpr int INTERP_ROWS_LANCZOS4 = TAB * 4;
+constexpr int INTERP_ROWS_FLOATS = INTERP_ROWS_LANCZOS4 + TAB * 8;
+inline void build_interp_rows(float* rows) {
+  for (int i = 0; i < TAB; ++i) {
+    const float x = (float)i * (1.f / TAB);
+    cubic_coeffs(x, rows + i * 4);
+    lanczos4_coeffs(x, rows + INTERP_ROWS_LANCZOS4 + i * 8);
+  }
+}
+
+// One element of type T at byte address p (16U, 16S, 32F: element-aligned), and a float sum stored as cv2's
+// Cast<float, T> stores it: cvRound (half to even) and saturation for the integer depths, the float itself for 32F.
+template <class T>
+__host__ __device__ __forceinline__ T ld_elem(const uint8_t* p) {
+#ifdef __CUDA_ARCH__
+  return __ldg(reinterpret_cast<const T*>(p));
+#else
+  T v;
+  memcpy(&v, p, sizeof v);
+  return v;
+#endif
+}
+
+template <class T>
+__host__ __device__ __forceinline__ void st_sum(uint8_t* p, float v) {
+  T r;
+  if constexpr (sizeof(T) == 4) r = v;
+  else if constexpr ((T)-1 > 0) r = (T)max(0, min(65535, f2i_rn(v)));
+  else r = (T)max(-32768, min(32767, f2i_rn(v)));
+#ifdef __CUDA_ARCH__
+  *reinterpret_cast<T*>(p) = r;
+#else
+  memcpy(p, &r, sizeof r);
+#endif
+}
+
 // ---- one output pixel of a KS x KS kernel (remapBicubic / remapLanczos4).  (sx, sy): the window's top-left tap, map1 -
 // (KS/2 - 1) in int, so the int16 extremes do not wrap; w: the fraction class's row of weights, k1 * KS + k2.
 // A tap outside the source adds nothing (OpenCV's BORDER_CONSTANT sum is cval * 2^15 + sum (S - cval) w with cval 0, and
@@ -130,6 +169,53 @@ __host__ __device__ __forceinline__ void taps_px(const uint8_t* __restrict__ src
   }
 #pragma unroll
   for (int c = 0; c < C; ++c) o[c] = (uint8_t)max(0, min(255, (sum[c] + (1 << (COEF_BITS - 1))) >> COEF_BITS));
+}
+
+// The same pixel from a 16U, 16S or 32F source, in cv2's float arithmetic: weight vy[k1] * vx[k2], each tap times its
+// weight rounded on its own, no contraction.  Inside the frame (the same fast-path test) a row's KS products are summed
+// left to right; cubic then adds rows 1..3 onto row 0, Lanczos4 adds rows 0..7 onto +0 (so an all -0.0 window gives -0.0
+// with cubic and +0.0 with Lanczos4).  Across an edge the sum starts at +0 and takes the in-frame taps one by one in
+// row-major order; a window wholly outside is +0.  A NaN or inf tap inside the frame poisons the sum whatever its weight.
+template <int KS, int C, class T>
+__host__ __device__ __forceinline__ void taps_px_f(const uint8_t* __restrict__ src, long long spitch, int sw, int sh, int sx,
+                                                   int sy, const float (&vy)[KS], const float (&vx)[KS], uint8_t* __restrict__ o) {
+  constexpr int E = (int)sizeof(T);
+  float sum[C];
+#pragma unroll
+  for (int c = 0; c < C; ++c) sum[c] = 0.f;
+  if ((unsigned)sx < (unsigned)max(sw - (KS - 1), 0) && (unsigned)sy < (unsigned)max(sh - (KS - 1), 0)) {
+    const uint8_t* q = src + (long long)sy * spitch + (long long)sx * (C * E);
+#pragma unroll
+    for (int k1 = 0; k1 < KS; ++k1, q += spitch) {
+      float r[C];
+#pragma unroll
+      for (int k2 = 0; k2 < KS; ++k2) {
+        const float w = fmul(vy[k1], vx[k2]);
+#pragma unroll
+        for (int c = 0; c < C; ++c) {
+          const float t = fmul((float)ld_elem<T>(q + (k2 * C + c) * E), w);
+          r[c] = k2 ? fadd(r[c], t) : t;
+        }
+      }
+#pragma unroll
+      for (int c = 0; c < C; ++c) sum[c] = (KS == 4 && k1 == 0) ? r[c] : fadd(sum[c], r[c]);
+    }
+  } else if (sx < sw && sx + KS > 0 && sy < sh && sy + KS > 0) {
+#pragma unroll
+    for (int k1 = 0; k1 < KS; ++k1) {
+      if ((unsigned)(sy + k1) >= (unsigned)sh) continue;
+      const uint8_t* q = src + (long long)(sy + k1) * spitch;
+#pragma unroll
+      for (int k2 = 0; k2 < KS; ++k2) {
+        if ((unsigned)(sx + k2) >= (unsigned)sw) continue;
+        const float w = fmul(vy[k1], vx[k2]);
+#pragma unroll
+        for (int c = 0; c < C; ++c) sum[c] = fadd(sum[c], fmul((float)ld_elem<T>(q + ((long long)(sx + k2) * C + c) * E), w));
+      }
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < C; ++c) st_sum<T>(o + c * E, sum[c]);
 }
 
 }  // namespace bevk

@@ -14,6 +14,8 @@
 #include "bevk_device.cuh"
 #include "bevk_interp.cuh"
 
+#include <type_traits>
+
 namespace bevk {
 
 constexpr int BEVK_MAX_CAMERAS_K = 8;   // == BEVK_MAX_CAMERAS in include/bevk.h
@@ -172,10 +174,22 @@ __host__ __device__ __forceinline__ void load_px(const uint8_t* __restrict__ src
   }
 }
 
+// load_px of a 16U, 16S or 32F pixel, as float; a tap outside the frame is +0 (cv2's BORDER_CONSTANT value)
+template <int C, class T>
+__host__ __device__ __forceinline__ void load_px_f(const uint8_t* __restrict__ src, long long spitch, int sw, int sh,
+                                                   int x, int y, float (&p)[C]) {
+  const bool in = (unsigned)x < (unsigned)sw && (unsigned)y < (unsigned)sh;
+  const uint8_t* q = src + (long long)y * spitch + (long long)x * (C * (int)sizeof(T));
+#pragma unroll
+  for (int c = 0; c < C; ++c) p[c] = in ? (float)ld_elem<T>(q + c * sizeof(T)) : 0.f;
+}
+
 // One thread of k_gather: output pixel (x, y) of frames [f0, min(n, f0 + GATHER_NB)).  Host-capable, so that
 // tests/host/undistort_stack.cu runs the same frame loop and addressing on a CPU.
-// LENS (MODE 1): the camera model's instance, undistort_point<LENS>.
-template <int MODE, int C, int LINEAR, int LENS = 0>
+// LENS (MODE 1): the camera model's instance, undistort_point<LENS>.  T: the source and destination element, uint8_t or
+// (tests/host/remap_depth.cu) uint16_t, int16_t, float.  The taps are T-independent: cv2 quantises to 1/32 px at every
+// depth.  8-bit LINEAR is the Q10 sum; the wider depths take cv2's float bilinear (gather_px_f).
+template <int MODE, int C, int LINEAR, int LENS = 0, class T = uint8_t>
 __host__ __device__ __forceinline__ void gather_frames(const GatherArgs& a, int x, int y, int f0) {
   int sx, sy, fx = 0, fy = 0;
   if (MODE == 2 || MODE == 3) {
@@ -211,42 +225,82 @@ __host__ __device__ __forceinline__ void gather_frames(const GatherArgs& a, int 
       sx += (fx < 16); sy += (fy < 16);
     }
   }
+  constexpr int PX = C * (int)sizeof(T);   // bytes per pixel
   const int nf = a.n - f0 < GATHER_NB ? a.n - f0 : GATHER_NB;
   const uint8_t* s = a.src + (long long)f0 * a.sistride;
-  uint8_t* o = a.dst + (long long)f0 * a.distride + (long long)y * a.dpitch + (long long)x * C;
-  for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) {
-    if (LINEAR) {
-      int p00[C], p01[C], p10[C], p11[C];
-      load_px<C>(s, a.spitch, a.sw, a.sh, sx, sy, p00);
-      load_px<C>(s, a.spitch, a.sw, a.sh, sx + 1, sy, p01);
-      load_px<C>(s, a.spitch, a.sw, a.sh, sx, sy + 1, p10);
-      load_px<C>(s, a.spitch, a.sw, a.sh, sx + 1, sy + 1, p11);
+  uint8_t* o = a.dst + (long long)f0 * a.distride + (long long)y * a.dpitch + (long long)x * PX;
+  if constexpr (sizeof(T) == 1) {
+    for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) {
+      if (LINEAR) {
+        int p00[C], p01[C], p10[C], p11[C];
+        load_px<C>(s, a.spitch, a.sw, a.sh, sx, sy, p00);
+        load_px<C>(s, a.spitch, a.sw, a.sh, sx + 1, sy, p01);
+        load_px<C>(s, a.spitch, a.sw, a.sh, sx, sy + 1, p10);
+        load_px<C>(s, a.spitch, a.sw, a.sh, sx + 1, sy + 1, p11);
 #pragma unroll
-      for (int c = 0; c < C; ++c) o[c] = (uint8_t)bilerp_q10(p00[c], p01[c], p10[c], p11[c], fx, fy);
-    } else {
-      int p[C];
-      load_px<C>(s, a.spitch, a.sw, a.sh, sx, sy, p);
+        for (int c = 0; c < C; ++c) o[c] = (uint8_t)bilerp_q10(p00[c], p01[c], p10[c], p11[c], fx, fy);
+      } else {
+        int p[C];
+        load_px<C>(s, a.spitch, a.sw, a.sh, sx, sy, p);
 #pragma unroll
-      for (int c = 0; c < C; ++c) o[c] = (uint8_t)p[c];
+        for (int c = 0; c < C; ++c) o[c] = (uint8_t)p[c];
+      }
+    }
+  } else if constexpr (LINEAR) {
+    // cv2's float table: w = vy * vx with vx = {1 - fx / 32, fx / 32}, each product rounded to float
+    const float ax = fmul((float)fx, 1.f / TAB), ay = fmul((float)fy, 1.f / TAB);
+    const float bx = fsub(1.f, ax), by = fsub(1.f, ay);
+    const float w00 = fmul(by, bx), w01 = fmul(by, ax), w10 = fmul(ay, bx), w11 = fmul(ay, ax);
+    for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) {
+      float p00[C], p01[C], p10[C], p11[C];
+      load_px_f<C, T>(s, a.spitch, a.sw, a.sh, sx, sy, p00);
+      load_px_f<C, T>(s, a.spitch, a.sw, a.sh, sx + 1, sy, p01);
+      load_px_f<C, T>(s, a.spitch, a.sw, a.sh, sx, sy + 1, p10);
+      load_px_f<C, T>(s, a.spitch, a.sw, a.sh, sx + 1, sy + 1, p11);
+#pragma unroll
+      for (int c = 0; c < C; ++c)   // ((t00 w00 + t01 w01) + t10 w10) + t11 w11, taps outside the frame 0
+        st_sum<T>(o + c * sizeof(T), fadd(fadd(fadd(fmul(p00[c], w00), fmul(p01[c], w01)), fmul(p10[c], w10)), fmul(p11[c], w11)));
+    }
+  } else {
+    // NEAREST moves the element's bits: a float NaN keeps its payload, -0.0 its sign; outside the frame 0
+    for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) {
+      const bool in = (unsigned)sx < (unsigned)a.sw && (unsigned)sy < (unsigned)a.sh;
+      const uint8_t* q = s + (long long)sy * a.spitch + (long long)sx * PX;
+#pragma unroll
+      for (int c = 0; c < C; ++c) {
+        const T v = in ? ld_elem<T>(q + c * sizeof(T)) : (T)0;
+#ifdef __CUDA_ARCH__
+        reinterpret_cast<T*>(o)[c] = v;
+#else
+        memcpy(o + c * sizeof(T), &v, sizeof v);
+#endif
+      }
     }
   }
 }
 
-template <int MODE, int C, int LINEAR, int LENS>
+template <int MODE, int C, int LINEAR, int LENS, class T>
 __global__ void __launch_bounds__(256) k_gather(GatherArgs a) {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31);
   const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= a.dw || y >= a.dh) return;
-  gather_frames<MODE, C, LINEAR, LENS>(a, x, y, blockIdx.z * GATHER_NB);
+  gather_frames<MODE, C, LINEAR, LENS, T>(a, x, y, blockIdx.z * GATHER_NB);
 }
+
+// The weights k_gather_taps reads: 8-bit sources the int16 2-D rows of build_interp_tabs, wider ones the float 1-D rows
+// of build_interp_rows.
+template <class T>
+using TapWeights = typename std::conditional<sizeof(T) == 1, short, float>::type;
 
 // K3 / K4 with INTER_CUBIC (KS = 4) and INTER_LANCZOS4 (KS = 8): the source position is INTER_LINEAR's (map entry, camera
 // model, or warp_point at TAB scale), the map2 value picks a row of KS * KS int16 weights from wtab (bevk_interp.cuh,
 // 32 or 128 bytes read once per pixel through the read-only path), and the row and window serve up to GATHER_NB frames.
-// Host-capable, like gather_frames (tests/host/remap_interp.cu).
-template <int MODE, int C, int KS, int LENS = 0>
-__host__ __device__ __forceinline__ void gather_taps_frames(const GatherArgs& a, const short* __restrict__ wtab, int x, int y,
-                                                            int f0) {
+// A 16U, 16S or 32F source instead reads the fraction's two 1-D float rows (2 * KS floats) and forms each 2-D weight as
+// cv2's float table holds it (taps_px_f): 2 * KS registers rather than KS * KS.
+// Host-capable, like gather_frames (tests/host/remap_interp.cu, tests/host/remap_depth.cu).
+template <int MODE, int C, int KS, int LENS = 0, class T = uint8_t>
+__host__ __device__ __forceinline__ void gather_taps_frames(const GatherArgs& a, const TapWeights<T>* __restrict__ wtab, int x,
+                                                            int y, int f0) {
   int sx, sy;
   unsigned fr;
   if (MODE == 2 || MODE == 3) {
@@ -273,31 +327,52 @@ __host__ __device__ __forceinline__ void gather_taps_frames(const GatherArgs& a,
     fr = f & (INTER_TAB_SIZE2 - 1);
   }
   sx -= KS / 2 - 1; sy -= KS / 2 - 1;
-  short w[KS * KS];
+  if constexpr (sizeof(T) == 1) {
+    short w[KS * KS];
 #ifdef __CUDA_ARCH__
-  const uint4* wr = reinterpret_cast<const uint4*>(wtab + fr * (KS * KS));
+    const uint4* wr = reinterpret_cast<const uint4*>(wtab + fr * (KS * KS));
 #pragma unroll
-  for (int i = 0; i < KS * KS / 8; ++i) {
-    const uint4 q = __ldg(wr + i);
-    const unsigned u[4] = {q.x, q.y, q.z, q.w};
+    for (int i = 0; i < KS * KS / 8; ++i) {
+      const uint4 q = __ldg(wr + i);
+      const unsigned u[4] = {q.x, q.y, q.z, q.w};
 #pragma unroll
-    for (int k = 0; k < 4; ++k) { w[8 * i + 2 * k] = (short)(u[k] & 0xffffu); w[8 * i + 2 * k + 1] = (short)(u[k] >> 16); }
-  }
+      for (int k = 0; k < 4; ++k) { w[8 * i + 2 * k] = (short)(u[k] & 0xffffu); w[8 * i + 2 * k + 1] = (short)(u[k] >> 16); }
+    }
 #else
-  memcpy(w, wtab + fr * (KS * KS), sizeof w);
+    memcpy(w, wtab + fr * (KS * KS), sizeof w);
 #endif
-  const int nf = a.n - f0 < GATHER_NB ? a.n - f0 : GATHER_NB;
-  const uint8_t* s = a.src + (long long)f0 * a.sistride;
-  uint8_t* o = a.dst + (long long)f0 * a.distride + (long long)y * a.dpitch + (long long)x * C;
-  for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) taps_px<KS, C>(s, a.spitch, a.sw, a.sh, sx, sy, w, o);
+    const int nf = a.n - f0 < GATHER_NB ? a.n - f0 : GATHER_NB;
+    const uint8_t* s = a.src + (long long)f0 * a.sistride;
+    uint8_t* o = a.dst + (long long)f0 * a.distride + (long long)y * a.dpitch + (long long)x * C;
+    for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) taps_px<KS, C>(s, a.spitch, a.sw, a.sh, sx, sy, w, o);
+  } else {
+    float vy[KS], vx[KS];
+    const float* ry = wtab + (fr >> INTER_BITS) * KS;
+    const float* rx = wtab + (fr & (TAB - 1)) * KS;
+#ifdef __CUDA_ARCH__
+#pragma unroll
+    for (int i = 0; i < KS / 4; ++i) {
+      const float4 qy = __ldg(reinterpret_cast<const float4*>(ry) + i), qx = __ldg(reinterpret_cast<const float4*>(rx) + i);
+      vy[4 * i] = qy.x; vy[4 * i + 1] = qy.y; vy[4 * i + 2] = qy.z; vy[4 * i + 3] = qy.w;
+      vx[4 * i] = qx.x; vx[4 * i + 1] = qx.y; vx[4 * i + 2] = qx.z; vx[4 * i + 3] = qx.w;
+    }
+#else
+    memcpy(vy, ry, sizeof vy);
+    memcpy(vx, rx, sizeof vx);
+#endif
+    const int nf = a.n - f0 < GATHER_NB ? a.n - f0 : GATHER_NB;
+    const uint8_t* s = a.src + (long long)f0 * a.sistride;
+    uint8_t* o = a.dst + (long long)f0 * a.distride + (long long)y * a.dpitch + (long long)x * (C * (int)sizeof(T));
+    for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) taps_px_f<KS, C, T>(s, a.spitch, a.sw, a.sh, sx, sy, vy, vx, o);
+  }
 }
 
-template <int MODE, int C, int KS, int LENS>
-__global__ void __launch_bounds__(256) k_gather_taps(GatherArgs a, const short* __restrict__ wtab) {
+template <int MODE, int C, int KS, int LENS, class T>
+__global__ void __launch_bounds__(256) k_gather_taps(GatherArgs a, const TapWeights<T>* __restrict__ wtab) {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31);
   const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= a.dw || y >= a.dh) return;
-  gather_taps_frames<MODE, C, KS, LENS>(a, wtab, x, y, blockIdx.z * GATHER_NB);
+  gather_taps_frames<MODE, C, KS, LENS, T>(a, wtab, x, y, blockIdx.z * GATHER_NB);
 }
 
 // ---------------------------------------------------------------------------------

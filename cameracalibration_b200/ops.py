@@ -80,12 +80,12 @@ def _undistort_map(model, K, D, P, size, ctx, R=None, m1type=CV_16SC2):
     return m1, m2
 
 
-def _out(shape, out):
+def _out(shape, out, dtype=np.uint8):
     """cv2-style optional destination (e.g. a page-locked array from pinned_empty for full-rate D2H)."""
     if out is None:
-        return np.empty(shape, np.uint8)
-    if out.dtype != np.uint8 or out.shape != tuple(shape) or not out.flags.c_contiguous:
-        raise L.BevkError(f"out must be a C-contiguous uint8 array of shape {tuple(shape)}")
+        return np.empty(shape, dtype)
+    if out.dtype != dtype or out.shape != tuple(shape) or not out.flags.c_contiguous:
+        raise L.BevkError(f"out must be a C-contiguous {np.dtype(dtype).name} array of shape {tuple(shape)}")
     return out
 
 
@@ -183,33 +183,49 @@ def jpeg_encode_bound(width: int, height: int, params=None) -> int:
     return n.value
 
 
-def _cuda_images(arr, what):
+# the image gathers' sources beyond uint8: dtype -> cv2 depth (CV_16U, CV_16S, CV_32F), and their CUDA typestrs
+_WIDE = {np.dtype(np.uint16): 2, np.dtype(np.int16): 3, np.dtype(np.float32): 5}
+_WIDE_TYPESTRS = {"<u2": np.uint16, "<i2": np.int16, "<f4": np.float32}
+
+
+def _cuda_dtype(arr):
+    """The NumPy dtype of a CUDA array's elements as the image calls read them (uint8 for any 1-byte unsigned typestr)."""
+    ts = arr.__cuda_array_interface__["typestr"]
+    return np.dtype(_WIDE_TYPESTRS.get(ts, np.uint8))
+
+
+def _cuda_images(arr, what, wide=False):
     """(device pointer, rank, n, h, w, channels, image stride, row stride) of a uint8 CUDA array [H][W], [H][W][C] or
-    [N][H][W][C] (C in 1, 3, 4) whose pixels are dense (C-byte pixels, 1-byte channels); rows and images may be padded."""
+    [N][H][W][C] (C in 1, 3, 4) whose pixels are dense (C-byte pixels, 1-byte channels); rows and images may be padded.
+    wide: the image gathers' uint16, int16 and float32 arrays too (strides in bytes, dense C-element pixels)."""
     iface = getattr(arr, "__cuda_array_interface__", None)
     if iface is None:
         raise L.BevkError(f"{what} must be a CUDA array (an object with __cuda_array_interface__), got {type(arr).__name__}")
     shape = tuple(iface["shape"])
-    if iface["typestr"] not in ("|u1", "<u1", "=u1"):
-        raise L.BevkError(f"{what} must be uint8, got typestr {iface['typestr']}")
+    es, dtypes = 1, "uint8, uint16, int16 or float32" if wide else "uint8"
+    if wide and iface["typestr"] in _WIDE_TYPESTRS:
+        es = np.dtype(_WIDE_TYPESTRS[iface["typestr"]]).itemsize
+    elif iface["typestr"] not in ("|u1", "<u1", "=u1"):
+        raise L.BevkError(f"{what} must be {dtypes}, got typestr {iface['typestr']}")
     rank = len(shape)
     if rank not in (2, 3, 4) or (rank > 2 and shape[-1] not in (1, 3, 4)):
-        raise L.BevkError(f"{what} must be uint8[H][W], [H][W][C] or [N][H][W][C] with C in 1, 3, 4, got shape {shape}")
+        kind = "uint8" if not wide else f"({dtypes}) "
+        raise L.BevkError(f"{what} must be {kind}[H][W], [H][W][C] or [N][H][W][C] with C in 1, 3, 4, got shape {shape}")
     strides = iface.get("strides")
     if strides is None:
-        strides = tuple(int(np.prod(shape[i + 1:])) for i in range(rank))
+        strides = tuple(es * int(np.prod(shape[i + 1:])) for i in range(rank))
     strides = tuple(int(s) for s in strides)
     if rank == 2:
-        shape, strides = shape + (1,), strides + (1,)
+        shape, strides = shape + (1,), strides + (es,)
     if rank != 4:
         shape, strides = (1,) + shape, (0,) + strides
     n, h, w, ch = shape
-    if (ch > 1 and strides[3] != 1) or (w > 1 and strides[2] != ch):
-        raise L.BevkError(f"{what} must have dense pixels (strides {ch} and 1 along width and channels)")
+    if (ch > 1 and strides[3] != es) or (w > 1 and strides[2] != ch * es):
+        raise L.BevkError(f"{what} must have dense pixels (strides {ch * es} and {es} along width and channels)")
     ptr = iface["data"][0]
     if not ptr:
         raise L.BevkError(f"{what} has a null data pointer")
-    row = strides[1] if h > 1 else w * ch
+    row = strides[1] if h > 1 else w * ch * es
     img = strides[0] if n > 1 else h * row
     return int(ptr), rank, n, h, w, ch, img, row
 
@@ -385,7 +401,10 @@ def remap(src: np.ndarray, map1: np.ndarray, map2: np.ndarray | None, interpolat
     float32 maps (CV_32FC1: map1, map2 float32[h][w]; CV_32FC2: map1 float32[h][w][2], map2 None) give cv2.remap's bytes
     for float maps.  With them src may also be a CUDA array ([H][W], [H][W][C] or a batch [N][H][W][C], rows and images
     may be padded), read in place on torch's current stream, with the maps NumPy or CUDA arrays; the result then stays
-    on the device (``out``, default a new torch tensor)."""
+    on the device (``out``, default a new torch tensor).
+
+    src may be uint8, uint16, int16 or float32 (CUDA typestr <u2, <i2, <f4); the result has src's dtype and cv2's bits
+    at that depth (DESIGN.md section 2)."""
     ctx = ctx or L.default_context()
     if _is_float32(map1):
         return _remap_f32(src, map1, map2, interpolation, ctx, out)
@@ -396,8 +415,8 @@ def remap(src: np.ndarray, map1: np.ndarray, map2: np.ndarray | None, interpolat
     m2 = None if map2 is None else np.ascontiguousarray(map2, np.uint16)
     if m2 is not None and m2.shape != (dh, dw):
         raise L.BevkError("map2 must be uint16[h][w] (CV_16UC1)")
-    return _host_image(src, dw, dh, out, lambda s, d, dstride: ctx.lib.bevk_remap(
-        ctx.h, *s, L.vptr(m1), None if m2 is None else L.vptr(m2), dw, dh, d, dstride, _interp(interpolation)))
+    return _host_image(src, dw, dh, out, lambda f, s, d, dstride: f(
+        ctx.h, *s, L.vptr(m1), None if m2 is None else L.vptr(m2), dw, dh, d, dstride, _interp(interpolation)), ctx.lib, "bevk_remap")
 
 
 def _is_float32(a) -> bool:
@@ -461,14 +480,15 @@ def _remap_f32(src, map1, map2, interpolation, ctx, out):
     dh, dw = _float_map_shapes(map1, map2)
     if hasattr(src, "__cuda_array_interface__"):
         (m1, m2), keep = _device_maps((map1, map2), (np.float32, np.float32), ctx)
-        return _device_images(src, dw, dh, out, ctx, "remap", lambda s, d: ctx.lib.bevk_remap_f32_stack(
-            ctx.h, *s, m1, m2, *d, _interp(interpolation)))
+        return _device_images(src, dw, dh, out, ctx, "remap", lambda f, s, d: f(
+            ctx.h, *s, m1, m2, *d, _interp(interpolation)), name="bevk_remap_f32_stack")
     if hasattr(map1, "__cuda_array_interface__") or hasattr(map2, "__cuda_array_interface__"):
         raise L.BevkError("remap: CUDA maps need a CUDA source image")
     m1 = np.ascontiguousarray(map1, np.float32)
     m2 = None if map2 is None else np.ascontiguousarray(map2, np.float32)
-    return _host_image(src, dw, dh, out, lambda s, d, dstride: ctx.lib.bevk_remap_f32(
-        ctx.h, *s, L.vptr(m1), None if m2 is None else L.vptr(m2), dw, dh, d, dstride, _interp(interpolation)))
+    return _host_image(src, dw, dh, out, lambda f, s, d, dstride: f(
+        ctx.h, *s, L.vptr(m1), None if m2 is None else L.vptr(m2), dw, dh, d, dstride, _interp(interpolation)), ctx.lib,
+        "bevk_remap_f32")
 
 
 def convert_maps(map1, map2, dstmap1type: int, nninterpolation: bool = False, ctx: L.Context | None = None):
@@ -514,53 +534,75 @@ def convert_maps(map1, map2, dstmap1type: int, nninterpolation: bool = False, ct
 
 def warp_perspective(src: np.ndarray, H, dsize, flags: int = INTER_LINEAR, ctx: L.Context | None = None,
                      out: np.ndarray | None = None):
-    """cv2.warpPerspective(src, H, dsize, flags) for uint8 images, BORDER_CONSTANT 0.  flags: INTER_NEAREST,
-    INTER_LINEAR, INTER_CUBIC, INTER_AREA (read as INTER_LINEAR, as cv2 reads it) or INTER_LANCZOS4."""
+    """cv2.warpPerspective(src, H, dsize, flags) for uint8, uint16, int16 and float32 images, BORDER_CONSTANT 0.  flags:
+    INTER_NEAREST, INTER_LINEAR, INTER_CUBIC, INTER_AREA (read as INTER_LINEAR, as cv2 reads it) or INTER_LANCZOS4; LINEAR / AREA at
+    uint16 with 3 or 4 channels and NEAREST at float32 with 1 or 4 channels raise BevkError (cv2 computes them with
+    other bodies than cv2.remap's)."""
     ctx = ctx or L.default_context()
     dw, dh = int(dsize[0]), int(dsize[1])
-    return _host_image(src, dw, dh, out, lambda s, d, dstride: ctx.lib.bevk_warp_perspective(
-        ctx.h, *s, L.dptr(H), d, dw, dh, dstride, _interp(flags)))
+    return _host_image(src, dw, dh, out, lambda f, s, d, dstride: f(
+        ctx.h, *s, L.dptr(H), d, dw, dh, dstride, _interp(flags)), ctx.lib, "bevk_warp_perspective")
 
 
 INTER_LINEAR_EXACT, INTER_NEAREST_EXACT, WARP_INVERSE_MAP = L.INTER_LINEAR_EXACT, L.INTER_NEAREST_EXACT, L.WARP_INVERSE_MAP
 BORDER_CONSTANT = 0
 
 
-def _host_image(src, dw, dh, out, call):
+def _gather_fn(lib, name, dtype):
+    """The library entry point of an image gather: `name` for uint8 images, its _typed sibling (a cv2 type code in place
+    of the channel count) for uint16, int16 and float32 ones."""
+    return getattr(lib, name) if dtype == np.uint8 else getattr(lib, name + "_typed")
+
+
+def _host_image(src, dw, dh, out, call, lib=None, name=None):
     """The body of the host forms: src a NumPy image [H][W] or [H][W][C]; out (default a new array) [dh][dw] of the same
-    rank; call(src, dst, dst_stride) with src's (pointer, width, height, stride, channels) and dst's pointer."""
-    img, sw, sh, ss, ch = L.image_view(src)
-    out = _out((dh, dw) if src.ndim == 2 else (dh, dw, ch), out)
-    L.check(call((L.vptr(img), sw, sh, ss, ch), L.vptr(out), dw * ch))
+    rank and dtype; call(src, dst, dst_stride) with src's (pointer, width, height, stride, channels) and dst's pointer.
+    With lib and name (an image gather) src may also be uint16, int16 or float32: call then takes the entry point first
+    (_gather_fn), and the channel count becomes the cv2 type code for the _typed sibling."""
+    if name is None:
+        img, sw, sh, ss, ch = L.image_view(src)
+        out = _out((dh, dw) if src.ndim == 2 else (dh, dw, ch), out)
+        L.check(call((L.vptr(img), sw, sh, ss, ch), L.vptr(out), dw * ch))
+        return out
+    img, sw, sh, ss, ch = L.image_view(src, (np.uint8, *_WIDE))
+    out = _out((dh, dw) if src.ndim == 2 else (dh, dw, ch), out, img.dtype)
+    kind = ch if img.dtype == np.uint8 else _WIDE[img.dtype] + ((ch - 1) << 3)
+    L.check(call(_gather_fn(lib, name, img.dtype), (L.vptr(img), sw, sh, ss, kind), L.vptr(out), dw * ch * img.itemsize))
     return out
 
 
-def _device_images(src, dw, dh, out, ctx, what, call, stream=None):
+def _device_images(src, dw, dh, out, ctx, what, call, stream=None, name=None):
     """The body of the device forms: src a uint8 CUDA array [H][W], [H][W][C] or [N][H][W][C] read in place; out
     (default a new torch tensor) of the same rank with dh x dw images; call(src, out) with the (pointer, image stride,
-    ...) layouts is run on ``stream`` (default torch's current stream) and only enqueues."""
-    ptr, rank, n, sh, sw, ch, simg, srow = _cuda_images(src, what)
+    ...) layouts is run on ``stream`` (default torch's current stream) and only enqueues.  With name (an image gather)
+    src may also be uint16, int16 or float32 (typestr <u2, <i2, <f4), out of the same dtype, and call takes the entry
+    point first, as _host_image's does."""
+    wide = name is not None
+    ptr, rank, n, sh, sw, ch, simg, srow = _cuda_images(src, what, wide)
+    dtype = _cuda_dtype(src) if wide else np.dtype(np.uint8)
     shape = {2: (dh, dw), 3: (dh, dw, ch), 4: (n, dh, dw, ch)}[rank]
     if out is None:
         import torch
-        out = torch.empty(shape, dtype=torch.uint8, device=torch.device("cuda", ctx.device))
-    optr, orank, on, oh, ow, och, oimg, orow = _cuda_images(out, "out")
-    if orank != rank or (on, oh, ow, och) != (n, dh, dw, ch):
-        raise L.BevkError(f"out must be a uint8 CUDA array of shape {shape}")
+        out = torch.empty(shape, dtype=getattr(torch, dtype.name), device=torch.device("cuda", ctx.device))
+    optr, orank, on, oh, ow, och, oimg, orow = _cuda_images(out, "out", wide)
+    if orank != rank or (on, oh, ow, och) != (n, dh, dw, ch) or (wide and _cuda_dtype(out) != dtype):
+        raise L.BevkError(f"out must be a {dtype.name} CUDA array of shape {shape}")
     if stream is None:
         from .sharding import _torch_current_stream
         stream = _torch_current_stream(ctx.device)
+    kind = ch if dtype == np.uint8 else _WIDE[dtype] + ((ch - 1) << 3)
+    s, d = (C.c_void_p(ptr), simg, sw, sh, srow, kind, n), (C.c_void_p(optr), oimg, dw, dh, orow)
     with ctx.on_stream(stream):
-        L.check(call((C.c_void_p(ptr), simg, sw, sh, srow, ch, n), (C.c_void_p(optr), oimg, dw, dh, orow)))
+        L.check(call(_gather_fn(ctx.lib, name, dtype), s, d) if wide else call(s, d))
     return out
 
 
-def _image_call(src, dw, dh, out, ctx, what, host, device):
+def _image_call(src, dw, dh, out, ctx, what, host, device, name=None):
     """A CUDA array goes to the device form (_device_images, with ``device``), anything else to the host form
-    (_host_image, with ``host``)."""
+    (_host_image, with ``host``); name: the host entry point of an image gather (its device form is name + "_stack")."""
     if hasattr(src, "__cuda_array_interface__"):
-        return _device_images(src, dw, dh, out, ctx, what, device)
-    return _host_image(src, dw, dh, out, host)
+        return _device_images(src, dw, dh, out, ctx, what, device, name=name and name + "_stack")
+    return _host_image(src, dw, dh, out, host, ctx.lib, name)
 
 
 def _src_size(src):
@@ -601,7 +643,9 @@ def resize(src, dsize, fx: float = 0, fy: float = 0, interpolation: int = INTER_
 
 def warp_affine(src, M, dsize, flags: int = INTER_LINEAR, borderMode: int = BORDER_CONSTANT, borderValue=0,
                 ctx: L.Context | None = None, out=None):
-    """cv2.warpAffine(src, M, dsize, flags=flags) for uint8 images with a zero constant border, byte for byte.  M: 2x3.
+    """cv2.warpAffine(src, M, dsize, flags=flags) for uint8, uint16, int16 and float32 images with a zero
+    constant border, bit for bit; NEAREST at int16 and at uint16 with 4 channels raises BevkError (cv2 computes it with
+    another body than cv2.remap's).  M: 2x3.
     flags: any interpolation warp_perspective takes, optionally | WARP_INVERSE_MAP.  Other borders raise BevkError.
     Takes NumPy images and CUDA arrays as resize() does."""
     if borderMode != BORDER_CONSTANT or np.any(np.asarray(borderValue) != 0):
@@ -612,8 +656,8 @@ def warp_affine(src, M, dsize, flags: int = INTER_LINEAR, borderMode: int = BORD
         raise L.BevkError(f"M must be 2x3, got shape {m.shape}")
     dw, dh = int(dsize[0]), int(dsize[1])
     return _image_call(src, dw, dh, out, ctx, "warp_affine",
-                       lambda s, d, ds: ctx.lib.bevk_warp_affine(ctx.h, *s, L.dptr(m), d, dw, dh, ds, int(flags)),
-                       lambda s, d: ctx.lib.bevk_warp_affine_stack(ctx.h, *s, L.dptr(m), *d, int(flags)))
+                       lambda f, s, d, ds: f(ctx.h, *s, L.dptr(m), d, dw, dh, ds, int(flags)),
+                       lambda f, s, d: f(ctx.h, *s, L.dptr(m), *d, int(flags)), "bevk_warp_affine")
 
 
 _GATHER_PATHS = {4: "word", 1: "byte", 2: "taps", 3: "resize"}
@@ -760,9 +804,10 @@ class Undistorter:
         the result stays on the device; NumPy input is uploaded, undistorted and downloaded in one call."""
         self._live()
         lib, h = self.ctx.lib, self.ctx.h
-        return _image_call(src, self.w, self.h, out, self.ctx, "frames",
-                           lambda s, d, ds: lib.bevk_undistort(h, self.slot, *s, d, self.w, self.h, ds, _interp(interpolation)),
-                           lambda s, d: lib.bevk_undistort_stack_interp(h, self.slot, *s, *d, _interp(interpolation)))
+        if hasattr(src, "__cuda_array_interface__"):
+            return self.cuda(src, out, interpolation)
+        return _host_image(src, self.w, self.h, out, lambda f, s, d, ds: f(h, self.slot, *s, d, self.w, self.h, ds,
+                                                                           _interp(interpolation)), lib, "bevk_undistort")
 
     def jpeg(self, src: np.ndarray, quality: int = 95, interpolation: int = INTER_LINEAR, params=None) -> bytes:
         """The undistorted image as the bytes cv2.imwrite(path, self(src), [IMWRITE_JPEG_QUALITY, quality] + params)
@@ -796,15 +841,16 @@ class Undistorter:
     def cuda(self, frames, out=None, interpolation: int = INTER_LINEAR, stream: int | None = None):
         """Undistort frames that already live on the GPU: no PCIe in the call.
 
-        frames: a uint8 CUDA array (``__cuda_array_interface__``) [H][W] (one grey image), [H][W][C] (one image) or
+        frames: a uint8, uint16, int16 or float32 CUDA array (``__cuda_array_interface__``; ``out`` of the same dtype)
+        [H][W] (one grey image), [H][W][C] (one image) or
         [N][H][W][C] (a batch; a grey batch is [N][H][W][1]), C in 1, 3, 4.  Pixels must be dense; rows and images may
         be padded.  ``out``: a CUDA array of the matching shape (rows and images may be padded too), default a new torch
         tensor.  ``interpolation``: as for __call__.  Each output pixel's map entry (or camera model) and, for INTER_CUBIC /
         INTER_LANCZOS4, its row of weights are read once for several frames of the batch.  Runs on
         ``stream`` (a raw CUDA stream handle), default torch's current stream, and only enqueues.  Returns ``out``."""
         self._live()
-        return _device_images(frames, self.w, self.h, out, self.ctx, "frames", lambda s, d: self.ctx.lib.bevk_undistort_stack_interp(
-            self.ctx.h, self.slot, *s, *d, _interp(interpolation)), stream)
+        return _device_images(frames, self.w, self.h, out, self.ctx, "frames", lambda f, s, d: f(
+            self.ctx.h, self.slot, *s, *d, _interp(interpolation)), stream, "bevk_undistort_stack_interp")
 
     def cuda_to_jpeg(self, frames, quality: int = 95, interpolation: int = INTER_LINEAR, params=None) -> list[bytes]:
         """cuda() followed by cv2.imencode('.jpg', img, [IMWRITE_JPEG_QUALITY, quality] + params) per frame, with the

@@ -50,6 +50,17 @@ enum { BEVK_MODEL_FISHEYE = 0, BEVK_MODEL_PINHOLE = 1 };
 /* cv2's map types (m1type / dstmap1type values): CV_16SC2 (+ a CV_16UC1 map2), CV_32FC1 (map1 = x, map2 = y planes)
  * and CV_32FC2 (map1 = interleaved x, y; no map2). */
 enum { BEVK_CV_32FC1 = 5, BEVK_CV_16SC2 = 11, BEVK_CV_32FC2 = 13 };
+
+/* The image type of the _typed gathers: cv2's type code, depth + ((channels - 1) << 3), with channels 1, 3 or 4 and
+ * depth CV_8U, CV_16U, CV_16S or CV_32F (CV_8UC3 = 16, CV_16UC1 = 2, CV_32FC4 = 29).  cv2.remap's arithmetic at each depth
+ * is kept bit for bit: taps at 1/32 px as for 8 bits; 16U, 16S and 32F LINEAR, CUBIC and LANCZOS4 in cv2's float sums
+ * (cvRound and saturation for 16U / 16S; a float result, NaN where cv2 gives NaN); NEAREST copies the element's bits.
+ * CV_8S and CV_16F (refused by cv2.remap) and CV_64F are BEVK_ERR_UNSUPPORTED, as are the warps cv2 computes with other
+ * bodies than cv2.remap's: warpPerspective LINEAR / AREA at CV_16UC3 / C4 and NEAREST at CV_32FC1 / C4, warpAffine
+ * NEAREST at CV_16UC4 and CV_16S.  Base pointers, row strides and image
+ * strides must be multiples of the element size (BEVK_ERR_ARG); all sizes and strides stay in bytes.  The uint8 calls
+ * are their _typed siblings at CV_8UC(channels). */
+enum { BEVK_CV_8U = 0, BEVK_CV_16U = 2, BEVK_CV_16S = 3, BEVK_CV_32F = 5 };
 /* bevk_bev_run flags.  BEVK_FLAG_NV12 / BEVK_FLAG_I420 (exclusive; they combine with BALANCE) say the frames are YUV
  * 4:2:0 in cv2's single-buffer layout, uint8[frame_h*3/2][frame_w] (frame_w, frame_h even, else BEVK_ERR_UNSUPPORTED):
  * the Y plane, then NV12: interleaved U,V rows; I420: the U plane, then the V plane, each frame_w/2 x frame_h/2 and
@@ -127,18 +138,25 @@ int bevk_undistort_rectify_map_f32(bevk_ctx *ctx, int model, const double K[9], 
 int bevk_remap(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t sstride, int channels,
                const int16_t *map1, const uint16_t *map2, int dw, int dh,
                uint8_t *dst, int64_t dstride, int interp);
+int bevk_remap_typed(bevk_ctx *ctx, const void *src, int sw, int sh, int64_t sstride, int type,
+                     const int16_t *map1, const uint16_t *map2, int dw, int dh, void *dst, int64_t dstride, int interp);
 /* cv2.remap with float maps: map1, map2 float[dh][dw] (CV_32FC1), or map2 NULL and map1 float[dh][dw][2] (CV_32FC2).
  * Byte for byte cv2.convertMaps(map1, map2, CV_16SC2, nninterpolation = (interp == NEAREST)) followed by the integer
  * remap, which is what cv2.remap does: cvRound(x * 32.f) (NEAREST: cvRound(x), half to even, without the integer maps'
  * nearest-neighbour rule), saturated to int16; NaN, +-inf and values beyond the int range become -32768. */
 int bevk_remap_f32(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t sstride, int channels,
                    const float *map1, const float *map2, int dw, int dh, uint8_t *dst, int64_t dstride, int interp);
+int bevk_remap_f32_typed(bevk_ctx *ctx, const void *src, int sw, int sh, int64_t sstride, int type,
+                         const float *map1, const float *map2, int dw, int dh, void *dst, int64_t dstride, int interp);
 /* The same for n DEVICE frames through DEVICE maps (dense, as above), with the strides, checks and word path of
  * bevk_undistort_stack (the maps need 16-byte alignment for the word path); a destination range that overlaps the
  * source frames or the maps is refused.  Only enqueues; can be graph-captured. */
 int bevk_remap_f32_stack(bevk_ctx *ctx, const void *d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
                          int channels, int n, const float *d_map1, const float *d_map2, void *d_dst, int64_t dst_image_stride,
                          int dw, int dh, int64_t dst_row_stride, int interp);
+int bevk_remap_f32_stack_typed(bevk_ctx *ctx, const void *d_src, int64_t src_image_stride, int sw, int sh,
+                               int64_t src_row_stride, int type, int n, const float *d_map1, const float *d_map2,
+                               void *d_dst, int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride, int interp);
 /* cv2.convertMaps(map1, map2, dstmap1type, nninterpolation) for w x h maps between BEVK_CV_16SC2 (map2: uint16[h][w] or
  * NULL), BEVK_CV_32FC1 and BEVK_CV_32FC2.  To CV_16SC2 as bevk_remap_f32 converts (dst2 unused with nninterpolation);
  * from CV_16SC2 as x + (map2 & 31) / 32, exactly.  The same type on both sides is BEVK_ERR_ARG.  on_device = 0: host
@@ -171,6 +189,8 @@ int bevk_undistorter_maps_f32(bevk_ctx *ctx, int slot, float *map1, float *map2)
  * a slot that was re-set can never make the library write past dst). */
 int bevk_undistort(bevk_ctx *ctx, int slot, const uint8_t *src, int sw, int sh, int64_t sstride, int channels,
                    uint8_t *dst, int dw, int dh, int64_t dstride, int interp);
+int bevk_undistort_typed(bevk_ctx *ctx, int slot, const void *src, int sw, int sh, int64_t sstride, int type,
+                         void *dst, int dw, int dh, int64_t dstride, int interp);
 /* n DEVICE frames (frame i at d_src + i*src_image_stride, rows src_row_stride apart, channels 1/3/4) undistorted
  * through the slot's map or fused model into n DEVICE images (dst_image_stride / dst_row_stride, dw x dh = the slot's
  * size, checked).  Each output pixel's taps are resolved once (map read or camera model) for several frames.  Row
@@ -188,6 +208,9 @@ int bevk_undistort_stack(bevk_ctx *ctx, int slot, const void *d_src, int64_t src
 int bevk_undistort_stack_interp(bevk_ctx *ctx, int slot, const void *d_src, int64_t src_image_stride, int sw, int sh,
                                 int64_t src_row_stride, int channels, int n, void *d_dst, int64_t dst_image_stride,
                                 int dw, int dh, int64_t dst_row_stride, int interp);
+int bevk_undistort_stack_interp_typed(bevk_ctx *ctx, int slot, const void *d_src, int64_t src_image_stride, int sw, int sh,
+                                      int64_t src_row_stride, int type, int n, void *d_dst, int64_t dst_image_stride,
+                                      int dw, int dh, int64_t dst_row_stride, int interp);
 /* Which gather the last undistort call (or bevk_remap / bevk_warp_perspective / bevk_warp_affine(_stack) /
  * bevk_resize(_stack)) launched: 4 = k_gather4 (word path), 1 = k_gather (byte path), 2 = k_gather_taps (INTER_CUBIC /
  * INTER_LANCZOS4), 3 = k_resize, 0 = none yet. */
@@ -197,6 +220,8 @@ int bevk_undistort_last_path(bevk_ctx *ctx);
  *   ExtrinsicCalibration/extrinsicCalib.py:166-169, surroundBEV.py:113-114      */
 int bevk_warp_perspective(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t sstride, int channels,
                           const double H[9], uint8_t *dst, int dw, int dh, int64_t dstride, int interp);
+int bevk_warp_perspective_typed(bevk_ctx *ctx, const void *src, int sw, int sh, int64_t sstride, int type,
+                                const double H[9], void *dst, int dw, int dh, int64_t dstride, int interp);
 /* ---- cv2.warpAffine(src, M, (dw,dh), flags), BORDER_CONSTANT 0 ------------------
  *   ExtrinsicCalibration/extrinsicCalib.py:58 (CenterImage.translate)
  * M: the 2x3 matrix, row-major.  flags: a BEVK_INTER_* (INTER_AREA read as INTER_LINEAR, as cv2 reads it), optionally
@@ -204,12 +229,17 @@ int bevk_warp_perspective(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int
  * source position of cv2's fixed-point affine walk. */
 int bevk_warp_affine(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t sstride, int channels,
                      const double M[6], uint8_t *dst, int dw, int dh, int64_t dstride, int flags);
+int bevk_warp_affine_typed(bevk_ctx *ctx, const void *src, int sw, int sh, int64_t sstride, int type,
+                           const double M[6], void *dst, int dw, int dh, int64_t dstride, int flags);
 /* The same for n DEVICE frames, laid out as bevk_undistort_stack lays them out (image and row strides on both sides,
  * strides smaller than one image and a destination overlapping the source refused with BEVK_ERR_ARG); word and byte
  * paths as there (bevk_undistort_last_path).  Only enqueues on the ctx stream; can be graph-captured. */
 int bevk_warp_affine_stack(bevk_ctx *ctx, const void *d_src, int64_t src_image_stride, int sw, int sh,
                            int64_t src_row_stride, int channels, int n, const double M[6], void *d_dst,
                            int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride, int flags);
+int bevk_warp_affine_stack_typed(bevk_ctx *ctx, const void *d_src, int64_t src_image_stride, int sw, int sh,
+                                 int64_t src_row_stride, int type, int n, const double M[6], void *d_dst,
+                                 int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride, int flags);
 
 /* ---- cv2.resize(src, (dw,dh), fx=fx, fy=fy, interpolation=interp) -----------------
  *   IntrinsicCalibration/intrinsicCalib.py:236, ExtrinsicCalibration/extrinsicCalib.py:125 (ScaleImage)
