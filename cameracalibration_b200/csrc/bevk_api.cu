@@ -613,10 +613,9 @@ struct ImageOp {
   GatherArgs g{};                   // a gather's maps, camera model or inverse matrix
   ResizeArgs r{};                   // a resize's scales
   int slot = -1, dw = 0, dh = 0;    // an undistorter slot and the size of the images it writes
-  const int16_t* hmap1 = nullptr;   // bevk_remap: the caller's host maps, uploaded once every check has passed
-  const uint16_t* hmap2 = nullptr;
-  const float* hfmap1 = nullptr;    // bevk_remap_f32: the same for the caller's float maps (hfmap2 null: CV_32FC2)
-  const float* hfmap2 = nullptr;
+  // bevk_remap*: the bytes of the caller's maps in g.map1 / g.map2, 0 for none.  host_launch uploads host maps once every
+  // check has passed; device_image refuses images written over device maps.
+  size_t map1_bytes = 0, map2_bytes = 0;
 };
 
 // a (GatherArgs or ResizeArgs) with its frame fields taken from b
@@ -727,23 +726,27 @@ static int launch(bevk_ctx* c, const ImageOp& op, const ImageBatch& b, PixType t
 }
 
 // ---- the operations' builders: each makes the refusals of its operation's own arguments and fills a default op
-static int remap_op(const int16_t* map1, const uint16_t* map2, int interp, ImageOp* op) {
+// dw x dh CV_16SC2 + CV_16UC1 maps, map2 null for NEAREST without fractions
+static int remap_op(const int16_t* map1, const uint16_t* map2, int interp, int dw, int dh, ImageOp* op) {
   if (!map1) return fail(BEVK_ERR_ARG, "null map1");
   RET(gather_interp(&interp));
   if (interp != BEVK_INTER_NEAREST && !map2) return fail(BEVK_ERR_ARG, "interpolation %d needs map2", interp);
   op->interp = interp;
-  op->hmap1 = map1; op->hmap2 = map2;
+  const size_t n = (size_t)dw * dh;
+  op->g.map1 = reinterpret_cast<const short2*>(map1); op->g.map2 = map2;
+  op->map1_bytes = n * 4; op->map2_bytes = map2 ? n * 2 : 0;
   return BEVK_OK;
 }
 
-// float maps: map2 null means map1 is CV_32FC2; host maps are uploaded by host_launch, device maps read in place
-static int remap_f32_op(const float* map1, const float* map2, int interp, bool host, ImageOp* op) {
+// dw x dh float maps: map2 null means map1 is CV_32FC2
+static int remap_f32_op(const float* map1, const float* map2, int interp, int dw, int dh, ImageOp* op) {
   if (!map1) return fail(BEVK_ERR_ARG, "null map1");
   RET(gather_interp(&interp));
   op->mode = 4;
   op->interp = interp;
-  if (host) { op->hfmap1 = map1; op->hfmap2 = map2; }
-  else { op->g.fmap1 = map1; op->g.fmap2 = map2; }
+  const size_t n = (size_t)dw * dh;
+  op->g.fmap1 = map1; op->g.fmap2 = map2;
+  op->map1_bytes = map2 ? n * 4 : n * 8; op->map2_bytes = map2 ? n * 4 : 0;
   return BEVK_OK;
 }
 
@@ -846,21 +849,15 @@ static int download_image(bevk_ctx* c, const DevBuf& buf, void* dst, int w, int 
 static int host_launch(bevk_ctx* c, ImageOp op, const void* src, int sw, int sh, int64_t sstride, PixType t, int dw, int dh) {
   RET(upload_image(c, c->s_src, src, sw, sh, sstride, t));
   RET(c->s_dst.ensure((size_t)dw * dh * t.px()));
-  if (op.hmap1) {
-    const size_t n = (size_t)dw * dh;
-    RET(c->s_m1.ensure(n * 4));
-    RET(c->s_m2.ensure(n * 2));
-    CU(cudaMemcpyAsync(c->s_m1.p, op.hmap1, n * 4, cudaMemcpyHostToDevice, c->stream));
-    if (op.hmap2) CU(cudaMemcpyAsync(c->s_m2.p, op.hmap2, n * 2, cudaMemcpyHostToDevice, c->stream));
-    op.g.map1 = c->s_m1.as<short2>(); op.g.map2 = op.hmap2 ? c->s_m2.as<unsigned short>() : nullptr;
+  if (op.map1_bytes) {
+    RET(c->s_m1.ensure(op.map1_bytes));
+    CU(cudaMemcpyAsync(c->s_m1.p, op.g.map1, op.map1_bytes, cudaMemcpyHostToDevice, c->stream));
+    op.g.map1 = c->s_m1.as<short2>();
   }
-  if (op.hfmap1) {
-    const size_t n = (size_t)dw * dh, b1 = op.hfmap2 ? n * 4 : n * 8;
-    RET(c->s_m1.ensure(b1));
-    if (op.hfmap2) RET(c->s_m2.ensure(n * 4));
-    CU(cudaMemcpyAsync(c->s_m1.p, op.hfmap1, b1, cudaMemcpyHostToDevice, c->stream));
-    if (op.hfmap2) CU(cudaMemcpyAsync(c->s_m2.p, op.hfmap2, n * 4, cudaMemcpyHostToDevice, c->stream));
-    op.g.fmap1 = c->s_m1.as<float>(); op.g.fmap2 = op.hfmap2 ? c->s_m2.as<float>() : nullptr;
+  if (op.map2_bytes) {
+    RET(c->s_m2.ensure(op.map2_bytes));
+    CU(cudaMemcpyAsync(c->s_m2.p, op.g.map2, op.map2_bytes, cudaMemcpyHostToDevice, c->stream));
+    op.g.map2 = c->s_m2.as<unsigned short>();
   }
   const ImageBatch b{c->s_src.as<uint8_t>(), sw, sh, sw * t.px(), 0, c->s_dst.as<uint8_t>(), dw, dh, dw * t.px(), 0, 1};
   return launch(c, op, b, t);
@@ -917,12 +914,11 @@ static int device_image(bevk_ctx* c, const ImageOp& op, const void* d_src, int64
   RET(check_stack_src(d_src, sis, sw, sh, srs, t, n));
   RET(check_op_size(op, dw, dh));
   RET(check_stack_dst(d_src, sis, sw, sh, srs, t, n, d_dst, dis, dw, dh, drs));
-  if (op.mode == 4 && op.slot < 0) {   // the caller's float maps: the images written must not overwrite them
+  if (op.map1_bytes) {   // the caller's maps: the images written must not overwrite them
     const uintptr_t d0 = reinterpret_cast<uintptr_t>(d_dst);
     const uintptr_t d1 = d0 + (uintptr_t)(n > 1 ? (n - 1) * dis : 0) + (uintptr_t)((int64_t)(dh - 1) * drs + dw * t.px());
-    const size_t np = (size_t)dw * dh;
-    const uintptr_t x0 = reinterpret_cast<uintptr_t>(op.g.fmap1), x1 = x0 + np * (op.g.fmap2 ? 4 : 8);
-    const uintptr_t y0 = reinterpret_cast<uintptr_t>(op.g.fmap2), y1 = op.g.fmap2 ? y0 + np * 4 : y0;
+    const uintptr_t x0 = reinterpret_cast<uintptr_t>(op.g.map1), x1 = x0 + op.map1_bytes;
+    const uintptr_t y0 = reinterpret_cast<uintptr_t>(op.g.map2), y1 = y0 + op.map2_bytes;
     if ((x0 < d1 && d0 < x1) || (y0 < d1 && d0 < y1)) return fail(BEVK_ERR_ARG, "the destination range overlaps the maps");
   }
   return launch(c, op, device_batch(d_src, sis, sw, sh, srs, n, d_dst, dis, dw, dh, drs), t);
@@ -933,7 +929,7 @@ static int device_image(bevk_ctx* c, const ImageOp& op, const void* d_src, int64
 static int remap_image(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, PixType t, const int16_t* map1,
                        const uint16_t* map2, int dw, int dh, void* dst, int64_t dstride, int interp) {
   ImageOp op;
-  RET(remap_op(map1, map2, interp, &op));
+  RET(remap_op(map1, map2, interp, dw, dh, &op));
   return host_image(c, op, src, sw, sh, sstride, t, dst, dw, dh, dstride);
 }
 int bevk_remap(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, const int16_t* map1,
@@ -952,7 +948,7 @@ int bevk_remap_typed(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstri
 static int remap_f32_image(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, PixType t, const float* map1,
                            const float* map2, int dw, int dh, void* dst, int64_t dstride, int interp) {
   ImageOp op;
-  RET(remap_f32_op(map1, map2, interp, true, &op));
+  RET(remap_f32_op(map1, map2, interp, dw, dh, &op));
   return host_image(c, op, src, sw, sh, sstride, t, dst, dw, dh, dstride);
 }
 int bevk_remap_f32(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, const float* map1,
@@ -972,7 +968,7 @@ static int remap_f32_frames(bevk_ctx* c, const void* d_src, int64_t src_image_st
                             PixType t, int n, const float* d_map1, const float* d_map2, void* d_dst, int64_t dst_image_stride,
                             int dw, int dh, int64_t dst_row_stride, int interp) {
   ImageOp op;
-  RET(remap_f32_op(d_map1, d_map2, interp, false, &op));
+  RET(remap_f32_op(d_map1, d_map2, interp, dw, dh, &op));
   return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, t, n, d_dst, dst_image_stride, dw, dh,
                       dst_row_stride);
 }

@@ -91,26 +91,12 @@ __host__ __device__ __forceinline__ void gather4_frames(const GatherArgs& a, int
 #pragma unroll
     for (int q = 0; q < 4; ++q) quantise_xy(X[q], Y[q], false, mx[q], my[q], fr[q]);
   }
-  int sx[4], sy[4];
-  unsigned fx[4], fy[4], px[4];
+  int sx[4], sy[4], fx[4], fy[4];
+  unsigned px[4];
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
-    if (MODE == 2 || MODE == 3) {
-      int X, Y;
-      warp_xy<MODE>(a.hm, x4 + q, y, false, X, Y);
-      sx[q] = sat_i16(X >> INTER_BITS); sy[q] = sat_i16(Y >> INTER_BITS);
-      fx[q] = X & (TAB - 1); fy[q] = Y & (TAB - 1);
-    } else {
-      if (MODE == 1) {
-        double u, v;
-        undistort_point<LENS>(a.cm, a.lx, x4 + q, y, u, v);
-        quantise_uv(u, v, mx[q], my[q], fr[q], pack_saturates(a.cm.model, x4 + q, a.cm.w));
-      } else if (MODE == 5) {
-        float_taps<MODE, LENS>(a, x4 + q, y, false, mx[q], my[q], fr[q]);
-      }
-      sx[q] = mx[q]; sy[q] = my[q];
-      fx[q] = fr[q] & (TAB - 1); fy[q] = (fr[q] >> INTER_BITS) & (TAB - 1);
-    }
+    if (MODE == 0 || MODE == 4) split_entry(mx[q], my[q], fr[q], false, sx[q], sy[q], fx[q], fy[q]);
+    else source_pos<MODE, LENS>(a, x4 + q, y, false, sx[q], sy[q], fx[q], fy[q]);
     // one frame (launched only for n = 1, so f0 = 0): gather each pixel as soon as its taps are known, as the
     // single-frame kernel always did -- about half the registers of the batch form, twice the occupancy
     if (NB == 1) px[q] = gather_px<LD>(a.src, (unsigned)a.spitch, a.sw, a.sh, sx[q], sy[q], fx[q], fy[q]);

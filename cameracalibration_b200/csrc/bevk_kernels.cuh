@@ -23,32 +23,49 @@ constexpr int BEVK_MAX_CAMERAS_K = 8;   // == BEVK_MAX_CAMERAS in include/bevk.h
 // ---------------------------------------------------------------------------------
 // K1
 // ---------------------------------------------------------------------------------
+// The camera model's CV_16SC2 + CV_16UC1 map entry of pixel (x, y), as cv2.initUndistortRectifyMap stores it.  Every
+// in-kernel evaluation of the model (the map build, the fused gathers' MODE 1, k_warp_maps' fused taps) goes through it.
+template <int LENS>
+__host__ __device__ __forceinline__ void model_entry(const CamModel& cm, const LensExt& lx, int x, int y, short& mx, short& my,
+                                                     unsigned short& fr) {
+  double u, v;
+  undistort_point<LENS>(cm, lx, x, y, u, v);
+  quantise_uv(u, v, mx, my, fr, pack_saturates(cm.model, x, cm.w));
+}
+
+// The camera model's CV_32FC1 / CV_32FC2 map entry of pixel (x, y): cv2 stores (float)u, (float)v of the very (u, v)
+// the CV_16SC2 build quantises.
+template <int LENS>
+__host__ __device__ __forceinline__ void model_entry_f32(const CamModel& cm, const LensExt& lx, int x, int y, float& fx,
+                                                         float& fy) {
+  double u, v;
+  undistort_point<LENS>(cm, lx, x, y, u, v);
+  fx = d2f(u); fy = d2f(v);
+}
+
 template <int LENS>
 __global__ void __launch_bounds__(256) k_undistort_map(CamModel cm, LensExt lx, short2* __restrict__ map1,
                                                        unsigned short* __restrict__ map2) {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31);
   const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= cm.w || y >= cm.h) return;
-  double u, v;
-  undistort_point<LENS>(cm, lx, x, y, u, v);
   short mx, my;
   unsigned short fr;
-  quantise_uv(u, v, mx, my, fr, pack_saturates(cm.model, x, cm.w));
+  model_entry<LENS>(cm, lx, x, y, mx, my, fr);
   const size_t i = (size_t)y * cm.w + x;
   map1[i] = make_short2(mx, my);
   map2[i] = fr;
 }
 
-// K1 into CV_32FC1 (map2 = the y plane) or CV_32FC2 (map2 null, map1 interleaved): cv2 stores (float)u, (float)v of the
-// very (u, v) the CV_16SC2 build quantises.
+// K1 into CV_32FC1 (map2 = the y plane) or CV_32FC2 (map2 null, map1 interleaved).
 template <int LENS>
 __host__ __device__ __forceinline__ void undistort_map_f32_px(const CamModel& cm, const LensExt& lx, int x, int y,
                                                              float* __restrict__ map1, float* __restrict__ map2) {
-  double u, v;
-  undistort_point<LENS>(cm, lx, x, y, u, v);
+  float fx, fy;
+  model_entry_f32<LENS>(cm, lx, x, y, fx, fy);
   const size_t i = (size_t)y * cm.w + x;
-  if (map2) { map1[i] = d2f(u); map2[i] = d2f(v); }
-  else { map1[2 * i] = d2f(u); map1[2 * i + 1] = d2f(v); }
+  if (map2) { map1[i] = fx; map2[i] = fy; }
+  else { map1[2 * i] = fx; map1[2 * i + 1] = fy; }
 }
 
 template <int LENS>
@@ -126,24 +143,6 @@ struct GatherArgs {
   int n; long long sistride, distride;   // frames, and the 64-bit image strides of source and destination
 };
 
-// MODE 4 / 5: the integer map entry of output pixel (x, y): the float map's (x, y), or the camera model's (u, v) rounded
-// to float, through quantise_xy.
-template <int MODE, int LENS>
-__host__ __device__ __forceinline__ void float_taps(const GatherArgs& a, int x, int y, bool nearest, short& mx, short& my,
-                                                    unsigned short& fr) {
-  float fx, fy;
-  if (MODE == 4) {
-    const size_t i = (size_t)y * a.dw + x;
-    if (a.fmap2) { fx = a.fmap1[i]; fy = a.fmap2[i]; }
-    else { fx = a.fmap1[2 * i]; fy = a.fmap1[2 * i + 1]; }
-  } else {
-    double u, v;
-    undistort_point<LENS>(a.cm, a.lx, x, y, u, v);
-    fx = d2f(u); fy = d2f(v);
-  }
-  quantise_xy(fx, fy, nearest, mx, my, fr);
-}
-
 // Frames per thread (grid.z = ceil(n / GATHER_NB)); DESIGN.md section 4 has the measurement that chose it.
 #ifndef BEVK_GATHER_NB
 #define BEVK_GATHER_NB 8
@@ -155,6 +154,61 @@ template <int MODE>
 __host__ __device__ __forceinline__ void warp_xy(const Homog& hm, int x, int y, bool nearest, int& X, int& Y) {
   if (MODE == 3) affine_point(hm, x, y, nearest, X, Y);
   else warp_point(hm, x, y, nearest ? 1.0 : (double)TAB, X, Y);
+}
+
+// A CV_16SC2 + CV_16UC1 map entry as source pixel (sx, sy) and 1/32 fractions (fx, fy).  nn_delta: INTER_NEAREST
+// through an entry that has a fraction, which moves the pixel by OpenCV's NNDeltaTab_i -- inverted: frac < 16 picks the
+// +1 neighbour.
+__host__ __device__ __forceinline__ void split_entry(short mx, short my, unsigned short fr, bool nn_delta, int& sx, int& sy,
+                                                     int& fx, int& fy) {
+  sx = mx; sy = my;
+  fx = fr & (TAB - 1); fy = (fr >> INTER_BITS) & (TAB - 1);
+  if (nn_delta) { sx += (fx < 16); sy += (fy < 16); }
+}
+
+// The source position of output pixel (x, y) in every MODE: source pixel (sx, sy) and 1/32 fractions (fx, fy), as
+// cv2.remap / cv2.warpPerspective / cv2.warpAffine pick them.  MODE 0 reads the map entry, MODE 1 evaluates the camera
+// model (model_entry), MODE 4 and 5 quantise a float map entry or the model rounded to float (model_entry_f32) as
+// cv2.remap converts float maps (quantise_xy), MODE 2 / 3 warp the pixel (warp_xy).  nearest (INTER_NEAREST): MODE 0 / 1
+// apply NNDeltaTab when the entry has a fraction (map2 may be null only then), MODE 4 / 5 round to whole pixels with no
+// fraction, MODE 2 / 3 warp in whole pixels; (fx, fy) are then 0 or unused.
+template <int MODE, int LENS>
+__host__ __device__ __forceinline__ void source_pos(const GatherArgs& a, int x, int y, bool nearest, int& sx, int& sy, int& fx,
+                                                    int& fy) {
+  if (MODE == 2 || MODE == 3) {
+    int X, Y;
+    warp_xy<MODE>(a.hm, x, y, nearest, X, Y);
+    if (nearest) { sx = sat_i16(X); sy = sat_i16(Y); fx = fy = 0; }
+    else {
+      sx = sat_i16(X >> INTER_BITS); sy = sat_i16(Y >> INTER_BITS);
+      fx = X & (TAB - 1); fy = Y & (TAB - 1);
+    }
+    return;
+  }
+  short mx, my;
+  unsigned short fr;
+  bool frac = true;
+  if (MODE == 0) {
+    const size_t i = (size_t)y * a.dw + x;
+    const short2 m = a.map1[i];
+    mx = m.x; my = m.y;
+    frac = !nearest || a.map2 != nullptr;
+    fr = frac ? a.map2[i] : 0;
+  } else if (MODE == 1) {
+    model_entry<LENS>(a.cm, a.lx, x, y, mx, my, fr);
+  } else {
+    float X, Y;
+    if (MODE == 4) {
+      const size_t i = (size_t)y * a.dw + x;
+      if (a.fmap2) { X = a.fmap1[i]; Y = a.fmap2[i]; }
+      else { X = a.fmap1[2 * i]; Y = a.fmap1[2 * i + 1]; }
+    } else {
+      model_entry_f32<LENS>(a.cm, a.lx, x, y, X, Y);
+    }
+    quantise_xy(X, Y, nearest, mx, my, fr);
+    frac = !nearest;
+  }
+  split_entry(mx, my, fr, nearest && frac, sx, sy, fx, fy);
 }
 
 template <int C>
@@ -191,40 +245,8 @@ __host__ __device__ __forceinline__ void load_px_f(const uint8_t* __restrict__ s
 // depth.  8-bit LINEAR is the Q10 sum; the wider depths take cv2's float bilinear (gather_px_f).
 template <int MODE, int C, int LINEAR, int LENS = 0, class T = uint8_t>
 __host__ __device__ __forceinline__ void gather_frames(const GatherArgs& a, int x, int y, int f0) {
-  int sx, sy, fx = 0, fy = 0;
-  if (MODE == 2 || MODE == 3) {
-    int X, Y;
-    warp_xy<MODE>(a.hm, x, y, !LINEAR, X, Y);
-    if (LINEAR) {
-      sx = sat_i16(X >> INTER_BITS); sy = sat_i16(Y >> INTER_BITS);
-      fx = X & (TAB - 1); fy = Y & (TAB - 1);
-    } else {
-      sx = sat_i16(X); sy = sat_i16(Y);
-    }
-  } else {
-    short mx, my;
-    unsigned short fr;
-    bool have_frac = true;
-    if (MODE == 0) {
-      const size_t i = (size_t)y * a.dw + x;
-      const short2 m = a.map1[i];
-      mx = m.x; my = m.y;
-      have_frac = (a.map2 != nullptr);
-      fr = have_frac ? a.map2[i] : 0;
-    } else if (MODE == 1) {
-      double u, v;
-      undistort_point<LENS>(a.cm, a.lx, x, y, u, v);
-      quantise_uv(u, v, mx, my, fr, pack_saturates(a.cm.model, x, a.cm.w));
-    } else {
-      float_taps<MODE, LENS>(a, x, y, !LINEAR, mx, my, fr);
-      have_frac = LINEAR;
-    }
-    sx = mx; sy = my;
-    fx = fr & (TAB - 1); fy = (fr >> INTER_BITS) & (TAB - 1);
-    if (!LINEAR && have_frac) {  // OpenCV's NNDeltaTab_i is inverted: frac < 16 picks the +1 neighbour
-      sx += (fx < 16); sy += (fy < 16);
-    }
-  }
+  int sx, sy, fx, fy;
+  source_pos<MODE, LENS>(a, x, y, !LINEAR, sx, sy, fx, fy);
   constexpr int PX = C * (int)sizeof(T);   // bytes per pixel
   const int nf = a.n - f0 < GATHER_NB ? a.n - f0 : GATHER_NB;
   const uint8_t* s = a.src + (long long)f0 * a.sistride;
@@ -301,33 +323,11 @@ using TapWeights = typename std::conditional<sizeof(T) == 1, short, float>::type
 template <int MODE, int C, int KS, int LENS = 0, class T = uint8_t>
 __host__ __device__ __forceinline__ void gather_taps_frames(const GatherArgs& a, const TapWeights<T>* __restrict__ wtab, int x,
                                                             int y, int f0) {
-  int sx, sy;
-  unsigned fr;
-  if (MODE == 2 || MODE == 3) {
-    int X, Y;
-    warp_xy<MODE>(a.hm, x, y, false, X, Y);
-    sx = sat_i16(X >> INTER_BITS); sy = sat_i16(Y >> INTER_BITS);
-    fr = (unsigned)((Y & (TAB - 1)) * TAB + (X & (TAB - 1)));
-  } else {
-    short mx, my;
-    unsigned short f;
-    if (MODE == 0) {
-      const size_t i = (size_t)y * a.dw + x;
-      const short2 m = a.map1[i];
-      mx = m.x; my = m.y;
-      f = a.map2[i];
-    } else if (MODE == 1) {
-      double u, v;
-      undistort_point<LENS>(a.cm, a.lx, x, y, u, v);
-      quantise_uv(u, v, mx, my, f, pack_saturates(a.cm.model, x, a.cm.w));
-    } else {
-      float_taps<MODE, LENS>(a, x, y, false, mx, my, f);
-    }
-    sx = mx; sy = my;
-    fr = f & (INTER_TAB_SIZE2 - 1);
-  }
+  int sx, sy, fx, fy;
+  source_pos<MODE, LENS>(a, x, y, false, sx, sy, fx, fy);
   sx -= KS / 2 - 1; sy -= KS / 2 - 1;
   if constexpr (sizeof(T) == 1) {
+    const unsigned fr = (unsigned)(fy * TAB + fx);
     short w[KS * KS];
 #ifdef __CUDA_ARCH__
     const uint4* wr = reinterpret_cast<const uint4*>(wtab + fr * (KS * KS));
@@ -343,12 +343,12 @@ __host__ __device__ __forceinline__ void gather_taps_frames(const GatherArgs& a,
 #endif
     const int nf = a.n - f0 < GATHER_NB ? a.n - f0 : GATHER_NB;
     const uint8_t* s = a.src + (long long)f0 * a.sistride;
-    uint8_t* o = a.dst + (long long)f0 * a.distride + (long long)y * a.dpitch + (long long)x * C;
+    uint8_t* o = a.dst + (long long)f0 * a.distride + (long long)y * a.dpitch + (long long)x * (C * (int)sizeof(T));
     for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) taps_px<KS, C>(s, a.spitch, a.sw, a.sh, sx, sy, w, o);
   } else {
     float vy[KS], vx[KS];
-    const float* ry = wtab + (fr >> INTER_BITS) * KS;
-    const float* rx = wtab + (fr & (TAB - 1)) * KS;
+    const float* ry = wtab + fy * KS;
+    const float* rx = wtab + fx * KS;
 #ifdef __CUDA_ARCH__
 #pragma unroll
     for (int i = 0; i < KS / 4; ++i) {
@@ -406,9 +406,7 @@ __host__ __device__ __forceinline__ void warp_maps_pixel(const WarpMapsArgs& a, 
       short mx, my;
       unsigned short fr;
       if (FROM_MODEL) {
-        double u, v;
-        undistort_point<LENS>(a.cm, a.lx, tx, ty, u, v);
-        quantise_uv(u, v, mx, my, fr, pack_saturates(a.cm.model, tx, a.cm.w));
+        model_entry<LENS>(a.cm, a.lx, tx, ty, mx, my, fr);
       } else {
         const size_t i = (size_t)ty * a.sw + tx;
         const short2 m = a.in1[i];
