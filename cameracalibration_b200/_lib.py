@@ -149,6 +149,9 @@ SIGNATURES = {
 SIGNATURES.update({n + "_typed": SIGNATURES[n] for n in (
     "bevk_remap", "bevk_remap_f32", "bevk_remap_f32_stack", "bevk_undistort", "bevk_undistort_stack_interp",
     "bevk_warp_perspective", "bevk_warp_affine", "bevk_warp_affine_stack")})
+# ... and their _border siblings: the _typed arguments, then cv2's borderMode and borderValue (4 doubles, or NULL)
+SIGNATURES.update({n.replace("_typed", "_border"): (SIGNATURES[n][0], SIGNATURES[n][1] + [C.c_int, C.POINTER(C.c_double)])
+                   for n in list(SIGNATURES) if n.endswith("_typed")})
 
 _lib = None
 

@@ -557,7 +557,8 @@ int bevk_undistort_map(bevk_ctx* c, int model, const double K[9], const double* 
 
 // k_gather4's word path: 32-bit tap loads need every source row to start on a 4-byte boundary (base, row pitch and, over
 // a batch, image stride), and its 32-bit stores the same of the destination (padded rows are fine).  Anything else,
-// e.g. caller memory at an odd address, takes k_gather's byte path.
+// e.g. caller memory at an odd address, takes k_gather's byte path; so does BORDER_TRANSPARENT, which leaves pixels
+// alone that k_gather4's three-word stores of four pixels would write.
 // An image's cv2 type (CV_8UC1 .. CV_32FC4): the depth (CV_8U 0, CV_16U 2, CV_16S 3, CV_32F 5), the channels and the bytes
 // of one element.  Rows, images and base pointers of a wider depth are element-aligned (check_image).
 struct PixType {
@@ -582,7 +583,7 @@ static bool gather4_ok(const GatherArgs& a, PixType t, int interp, int mode) {
   const int channels = t.esize == 1 ? t.channels : 0;   // the word path is 8-bit only
   const uintptr_t al = reinterpret_cast<uintptr_t>(a.src) | reinterpret_cast<uintptr_t>(a.dst) | (uintptr_t)a.spitch |
                        (uintptr_t)a.dpitch | (a.n > 1 ? (uintptr_t)(a.sistride | a.distride) : 0);
-  return channels == 3 && interp == BEVK_INTER_LINEAR && (a.dw % 4) == 0 && (al & 3) == 0 &&
+  return channels == 3 && interp == BEVK_INTER_LINEAR && a.bd.mode != BORDER_TRANSPARENT && (a.dw % 4) == 0 && (al & 3) == 0 &&
          a.spitch < (1ll << 31) / std::max(1, a.sh) && (mode != 0 || a.map2 != nullptr) &&
          (mode != 4 || ((reinterpret_cast<uintptr_t>(a.fmap1) | reinterpret_cast<uintptr_t>(a.fmap2)) & 15) == 0);   // float4 loads
 }
@@ -627,11 +628,17 @@ static Args with_frames(Args a, const ImageBatch& b) {
   return a;
 }
 
+// bd: a border other than a zero BORDER_CONSTANT, which the _border kernels take; the zero-constant kernels keep their
+// machine code
 template <int MODE, int LENS, class T>
-static void gather_t(bevk_ctx* c, const GatherArgs& a, int channels, int interp, unsigned gz) {
+static void gather_t(bevk_ctx* c, const GatherArgs& a, int channels, int interp, bool bd, unsigned gz) {
   const dim3 g((a.dw + 31) / 32, (a.dh + 7) / 8, gz);
-#define GO(C, L) k_gather<MODE, C, L, LENS, T><<<g, 256, 0, c->stream>>>(a)
-#define TAPS(C, KS) k_gather_taps<MODE, C, KS, LENS, T><<<g, 256, 0, c->stream>>>(a, wt)
+#define GO(C, L)                                                                      \
+  (bd ? k_gather_border<MODE, C, L, LENS, T><<<g, 256, 0, c->stream>>>(a)             \
+      : k_gather<MODE, C, L, LENS, T><<<g, 256, 0, c->stream>>>(a))
+#define TAPS(C, KS)                                                                   \
+  (bd ? k_gather_taps_border<MODE, C, KS, LENS, T><<<g, 256, 0, c->stream>>>(a, wt)   \
+      : k_gather_taps<MODE, C, KS, LENS, T><<<g, 256, 0, c->stream>>>(a, wt))
   if (interp == BEVK_INTER_CUBIC || interp == BEVK_INTER_LANCZOS4) {
     const TapWeights<T>* wt;
     if constexpr (sizeof(T) == 1) wt = c->d_wtab.as<short>() + (interp == BEVK_INTER_CUBIC ? 0 : INTERP_TAB_LANCZOS4);
@@ -653,18 +660,25 @@ static void gather_t(bevk_ctx* c, const GatherArgs& a, int channels, int interp,
 
 template <int MODE, int LENS>
 static void gather(bevk_ctx* c, const GatherArgs& a, PixType t, int interp, bool words, unsigned gz) {
+  bool bd = a.bd.mode != BORDER_CONSTANT;
+  for (unsigned char v : a.bd.v) bd |= v != 0;
   if (words) {
     // 4 output pixels per thread, 32-bit tap loads and 12-byte stores
     const dim3 g4((a.dw / 4 + 31) / 32, (a.dh + 7) / 8, gz);
-    if (a.n == 1) k_gather4<MODE, 1, LENS><<<g4, 256, 0, c->stream>>>(a);
-    else k_gather4<MODE, GATHER_NB, LENS><<<g4, 256, 0, c->stream>>>(a);
+    if (bd) {
+      if (a.n == 1) k_gather4_border<MODE, 1, LENS><<<g4, 256, 0, c->stream>>>(a);
+      else k_gather4_border<MODE, GATHER_NB, LENS><<<g4, 256, 0, c->stream>>>(a);
+    } else {
+      if (a.n == 1) k_gather4<MODE, 1, LENS><<<g4, 256, 0, c->stream>>>(a);
+      else k_gather4<MODE, GATHER_NB, LENS><<<g4, 256, 0, c->stream>>>(a);
+    }
     return;
   }
   switch (t.depth) {
-    case 0: gather_t<MODE, LENS, uint8_t>(c, a, t.channels, interp, gz); break;
-    case 2: gather_t<MODE, LENS, uint16_t>(c, a, t.channels, interp, gz); break;
-    case 3: gather_t<MODE, LENS, int16_t>(c, a, t.channels, interp, gz); break;
-    default: gather_t<MODE, LENS, float>(c, a, t.channels, interp, gz);
+    case 0: gather_t<MODE, LENS, uint8_t>(c, a, t.channels, interp, bd, gz); break;
+    case 2: gather_t<MODE, LENS, uint16_t>(c, a, t.channels, interp, bd, gz); break;
+    case 3: gather_t<MODE, LENS, int16_t>(c, a, t.channels, interp, bd, gz); break;
+    default: gather_t<MODE, LENS, float>(c, a, t.channels, interp, bd, gz);
   }
 }
 
@@ -846,9 +860,12 @@ static int download_image(bevk_ctx* c, const DevBuf& buf, void* dst, int w, int 
 
 // Host path, without the read-back: a checked host frame uploaded to c->s_src and op run into c->s_dst.  Both are dense
 // (row pitch w times the pixel bytes), so k_gather4's word-path choice sees the same pitches whatever the caller's strides.
-static int host_launch(bevk_ctx* c, ImageOp op, const void* src, int sw, int sh, int64_t sstride, PixType t, int dw, int dh) {
+// BORDER_TRANSPARENT leaves some destination pixels as they are: the caller's dst (dstride) is uploaded into c->s_dst first.
+static int host_launch(bevk_ctx* c, ImageOp op, const void* src, int sw, int sh, int64_t sstride, PixType t, int dw, int dh,
+                       const void* dst = nullptr, int64_t dstride = 0) {
   RET(upload_image(c, c->s_src, src, sw, sh, sstride, t));
-  RET(c->s_dst.ensure((size_t)dw * dh * t.px()));
+  if (op.mode != OP_RESIZE && op.g.bd.mode == BORDER_TRANSPARENT) RET(upload_image(c, c->s_dst, dst, dw, dh, dstride, t));
+  else RET(c->s_dst.ensure((size_t)dw * dh * t.px()));
   if (op.map1_bytes) {
     RET(c->s_m1.ensure(op.map1_bytes));
     CU(cudaMemcpyAsync(c->s_m1.p, op.g.map1, op.map1_bytes, cudaMemcpyHostToDevice, c->stream));
@@ -869,7 +886,7 @@ static int host_image(bevk_ctx* c, const ImageOp& op, const void* src, int sw, i
   RET(check_image(src, sw, sh, sstride, t, "src"));
   RET(check_op_size(op, dw, dh));
   RET(check_image(dst, dw, dh, dstride, t, "dst"));
-  RET(host_launch(c, op, src, sw, sh, sstride, t, dw, dh));
+  RET(host_launch(c, op, src, sw, sh, sstride, t, dw, dh, dst, dstride));
   return download_image(c, c->s_dst, dst, dw, dh, dstride, t);
 }
 
@@ -924,51 +941,84 @@ static int device_image(bevk_ctx* c, const ImageOp& op, const void* d_src, int64
   return launch(c, op, device_batch(d_src, sis, sw, sh, srs, n, d_dst, dis, dw, dh, drs), t);
 }
 
+// cv2's borderMode and borderValue for a gather op of images of type t: the mode (BORDER_CONSTANT 0 .. BORDER_TRANSPARENT
+// 5; anything else, BORDER_ISOLATED included, refused as cv2 refuses it) and the value converted to t's depth, once, here
+// (make_border; NULL means zeros).  cv2 4.13 leaves remap's arithmetic in a few border cases; exactly those are refused:
+// LINEAR (and AREA, read as LINEAR) under BORDER_TRANSPARENT at 32F, whose windows across the edge cv2 sums another way,
+// and warpPerspective NEAREST / LINEAR at 16S under BORDER_REPLICATE and BORDER_TRANSPARENT (DESIGN.md section 2).
+static int set_border(ImageOp* op, PixType t, int mode, const double* value) {
+  if (mode < BORDER_CONSTANT || mode > BORDER_TRANSPARENT)
+    return fail(BEVK_ERR_ARG, "border mode %d: the gathers take cv2's BORDER_CONSTANT (0) .. BORDER_TRANSPARENT (5)", mode);
+  const bool linear = op->interp == BEVK_INTER_LINEAR, nearest = op->interp == BEVK_INTER_NEAREST;
+  if ((t.depth == 5 && linear && mode == BORDER_TRANSPARENT) ||
+      (op->mode == 2 && t.depth == 3 && (linear || nearest) && (mode == BORDER_REPLICATE || mode == BORDER_TRANSPARENT)))
+    return fail(BEVK_ERR_UNSUPPORTED, "%s with interp %d at depth %d under border mode %d: cv2 computes it with another body "
+                "than cv2.remap's", op->mode == 2 ? "warpPerspective" : "a gather", op->interp, t.depth, mode);
+  double v[4] = {0, 0, 0, 0};
+  if (value) memcpy(v, value, sizeof v);
+  op->g.bd = make_border(mode, t.depth, v);
+  return BEVK_OK;
+}
+
 // ---- the entry points
-// Each uint8 entry point is its _typed sibling at CV_8UC(channels); the sibling reads a cv2 type code (pix_type) first.
+// Each uint8 entry point is its _typed sibling at CV_8UC(channels); the sibling reads a cv2 type code (pix_type) first,
+// and is its _border sibling at BORDER_CONSTANT with a zero value.
 static int remap_image(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, PixType t, const int16_t* map1,
-                       const uint16_t* map2, int dw, int dh, void* dst, int64_t dstride, int interp) {
+                       const uint16_t* map2, int dw, int dh, void* dst, int64_t dstride, int interp, int border, const double* bval) {
   ImageOp op;
   RET(remap_op(map1, map2, interp, dw, dh, &op));
+  RET(set_border(&op, t, border, bval));
   return host_image(c, op, src, sw, sh, sstride, t, dst, dw, dh, dstride);
 }
 int bevk_remap(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, const int16_t* map1,
                const uint16_t* map2, int dw, int dh, uint8_t* dst, int64_t dstride, int interp) {
   RET(use(c));
-  return remap_image(c, src, sw, sh, sstride, u8(channels), map1, map2, dw, dh, dst, dstride, interp);
+  return remap_image(c, src, sw, sh, sstride, u8(channels), map1, map2, dw, dh, dst, dstride, interp, BORDER_CONSTANT, nullptr);
 }
 int bevk_remap_typed(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, int type, const int16_t* map1,
                      const uint16_t* map2, int dw, int dh, void* dst, int64_t dstride, int interp) {
+  return bevk_remap_border(c, src, sw, sh, sstride, type, map1, map2, dw, dh, dst, dstride, interp, BORDER_CONSTANT, nullptr);
+}
+int bevk_remap_border(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, int type, const int16_t* map1,
+                     const uint16_t* map2, int dw, int dh, void* dst, int64_t dstride, int interp, int border_mode,
+                      const double border_value[4]) {
   RET(use(c));
   PixType t;
   RET(pix_type(type, &t));
-  return remap_image(c, src, sw, sh, sstride, t, map1, map2, dw, dh, dst, dstride, interp);
+  return remap_image(c, src, sw, sh, sstride, t, map1, map2, dw, dh, dst, dstride, interp, border_mode, border_value);
 }
 
 static int remap_f32_image(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, PixType t, const float* map1,
-                           const float* map2, int dw, int dh, void* dst, int64_t dstride, int interp) {
+                           const float* map2, int dw, int dh, void* dst, int64_t dstride, int interp, int border, const double* bval) {
   ImageOp op;
   RET(remap_f32_op(map1, map2, interp, dw, dh, &op));
+  RET(set_border(&op, t, border, bval));
   return host_image(c, op, src, sw, sh, sstride, t, dst, dw, dh, dstride);
 }
 int bevk_remap_f32(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, const float* map1,
                    const float* map2, int dw, int dh, uint8_t* dst, int64_t dstride, int interp) {
   RET(use(c));
-  return remap_f32_image(c, src, sw, sh, sstride, u8(channels), map1, map2, dw, dh, dst, dstride, interp);
+  return remap_f32_image(c, src, sw, sh, sstride, u8(channels), map1, map2, dw, dh, dst, dstride, interp, BORDER_CONSTANT, nullptr);
 }
 int bevk_remap_f32_typed(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, int type, const float* map1,
                          const float* map2, int dw, int dh, void* dst, int64_t dstride, int interp) {
+  return bevk_remap_f32_border(c, src, sw, sh, sstride, type, map1, map2, dw, dh, dst, dstride, interp, BORDER_CONSTANT, nullptr);
+}
+int bevk_remap_f32_border(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, int type, const float* map1,
+                         const float* map2, int dw, int dh, void* dst, int64_t dstride, int interp, int border_mode,
+                          const double border_value[4]) {
   RET(use(c));
   PixType t;
   RET(pix_type(type, &t));
-  return remap_f32_image(c, src, sw, sh, sstride, t, map1, map2, dw, dh, dst, dstride, interp);
+  return remap_f32_image(c, src, sw, sh, sstride, t, map1, map2, dw, dh, dst, dstride, interp, border_mode, border_value);
 }
 
 static int remap_f32_frames(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
                             PixType t, int n, const float* d_map1, const float* d_map2, void* d_dst, int64_t dst_image_stride,
-                            int dw, int dh, int64_t dst_row_stride, int interp) {
+                            int dw, int dh, int64_t dst_row_stride, int interp, int border, const double* bval) {
   ImageOp op;
   RET(remap_f32_op(d_map1, d_map2, interp, dw, dh, &op));
+  RET(set_border(&op, t, border, bval));
   return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, t, n, d_dst, dst_image_stride, dw, dh,
                       dst_row_stride);
 }
@@ -977,16 +1027,23 @@ int bevk_remap_f32_stack(bevk_ctx* c, const void* d_src, int64_t src_image_strid
                          int dw, int dh, int64_t dst_row_stride, int interp) {
   RET(use(c));
   return remap_f32_frames(c, d_src, src_image_stride, sw, sh, src_row_stride, u8(channels), n, d_map1, d_map2, d_dst,
-                          dst_image_stride, dw, dh, dst_row_stride, interp);
+                          dst_image_stride, dw, dh, dst_row_stride, interp, BORDER_CONSTANT, nullptr);
 }
 int bevk_remap_f32_stack_typed(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
                                int type, int n, const float* d_map1, const float* d_map2, void* d_dst, int64_t dst_image_stride,
                                int dw, int dh, int64_t dst_row_stride, int interp) {
+  return bevk_remap_f32_stack_border(c, d_src, src_image_stride, sw, sh, src_row_stride, type, n, d_map1, d_map2, d_dst,
+                                     dst_image_stride, dw, dh, dst_row_stride, interp, BORDER_CONSTANT, nullptr);
+}
+int bevk_remap_f32_stack_border(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
+                               int type, int n, const float* d_map1, const float* d_map2, void* d_dst, int64_t dst_image_stride,
+                               int dw, int dh, int64_t dst_row_stride, int interp, int border_mode,
+                                const double border_value[4]) {
   RET(use(c));
   PixType t;
   RET(pix_type(type, &t));
   return remap_f32_frames(c, d_src, src_image_stride, sw, sh, src_row_stride, t, n, d_map1, d_map2, d_dst, dst_image_stride,
-                          dw, dh, dst_row_stride, interp);
+                          dw, dh, dst_row_stride, interp, border_mode, border_value);
 }
 
 // ------------------------------------------------------------------ cached-map undistortion
@@ -1108,22 +1165,28 @@ int bevk_convert_maps(bevk_ctx* c, const void* map1, const void* map2, int m1typ
 }
 
 static int undistort_image(bevk_ctx* c, int slot, const void* src, int sw, int sh, int64_t sstride, PixType t, void* dst, int dw,
-                           int dh, int64_t dstride, int interp) {
+                           int dh, int64_t dstride, int interp, int border, const double* bval) {
   ImageOp op;
   RET(undistort_op(c, slot, interp, &op));
+  RET(set_border(&op, t, border, bval));
   return host_image(c, op, src, sw, sh, sstride, t, dst, dw, dh, dstride);
 }
 int bevk_undistort(bevk_ctx* c, int slot, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
                    uint8_t* dst, int dw, int dh, int64_t dstride, int interp) {
   RET(use(c));
-  return undistort_image(c, slot, src, sw, sh, sstride, u8(channels), dst, dw, dh, dstride, interp);
+  return undistort_image(c, slot, src, sw, sh, sstride, u8(channels), dst, dw, dh, dstride, interp, BORDER_CONSTANT, nullptr);
 }
 int bevk_undistort_typed(bevk_ctx* c, int slot, const void* src, int sw, int sh, int64_t sstride, int type, void* dst, int dw,
                          int dh, int64_t dstride, int interp) {
+  return bevk_undistort_border(c, slot, src, sw, sh, sstride, type, dst, dw, dh, dstride, interp, BORDER_CONSTANT, nullptr);
+}
+int bevk_undistort_border(bevk_ctx* c, int slot, const void* src, int sw, int sh, int64_t sstride, int type, void* dst, int dw,
+                         int dh, int64_t dstride, int interp, int border_mode,
+                          const double border_value[4]) {
   RET(use(c));
   PixType t;
   RET(pix_type(type, &t));
-  return undistort_image(c, slot, src, sw, sh, sstride, t, dst, dw, dh, dstride, interp);
+  return undistort_image(c, slot, src, sw, sh, sstride, t, dst, dw, dh, dstride, interp, border_mode, border_value);
 }
 
 // ------------------------------------------------------------------ undistortion of device frame batches
@@ -1141,9 +1204,10 @@ int bevk_undistort_stack(bevk_ctx* c, int slot, const void* d_src, int64_t src_i
 
 static int undistort_frames(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh,
                             int64_t src_row_stride, PixType t, int n, void* d_dst, int64_t dst_image_stride, int dw, int dh,
-                            int64_t dst_row_stride, int interp) {
+                            int64_t dst_row_stride, int interp, int border, const double* bval) {
   ImageOp op;
   RET(undistort_op(c, slot, interp, &op));
+  RET(set_border(&op, t, border, bval));
   return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, t, n, d_dst, dst_image_stride, dw, dh,
                       dst_row_stride);
 }
@@ -1152,16 +1216,23 @@ int bevk_undistort_stack_interp(bevk_ctx* c, int slot, const void* d_src, int64_
                                 int64_t dst_row_stride, int interp) {
   RET(use(c));
   return undistort_frames(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, u8(channels), n, d_dst, dst_image_stride,
-                          dw, dh, dst_row_stride, interp);
+                          dw, dh, dst_row_stride, interp, BORDER_CONSTANT, nullptr);
 }
 int bevk_undistort_stack_interp_typed(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh,
                                       int64_t src_row_stride, int type, int n, void* d_dst, int64_t dst_image_stride, int dw,
                                       int dh, int64_t dst_row_stride, int interp) {
+  return bevk_undistort_stack_interp_border(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, type, n, d_dst,
+                                            dst_image_stride, dw, dh, dst_row_stride, interp, BORDER_CONSTANT, nullptr);
+}
+int bevk_undistort_stack_interp_border(bevk_ctx* c, int slot, const void* d_src, int64_t src_image_stride, int sw, int sh,
+                                      int64_t src_row_stride, int type, int n, void* d_dst, int64_t dst_image_stride, int dw,
+                                      int dh, int64_t dst_row_stride, int interp, int border_mode,
+                                       const double border_value[4]) {
   RET(use(c));
   PixType t;
   RET(pix_type(type, &t));
   return undistort_frames(c, slot, d_src, src_image_stride, sw, sh, src_row_stride, t, n, d_dst, dst_image_stride, dw, dh,
-                          dst_row_stride, interp);
+                          dst_row_stride, interp, border_mode, border_value);
 }
 
 int bevk_undistort_last_path(bevk_ctx* c) { return c ? c->gather_path : 0; }
@@ -1183,52 +1254,65 @@ static int check_warp_depth(const ImageOp& op, PixType t) {
 }
 
 static int perspective_image(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, PixType t, const double H[9],
-                             void* dst, int dw, int dh, int64_t dstride, int interp) {
+                             void* dst, int dw, int dh, int64_t dstride, int interp, int border, const double* bval) {
   ImageOp op;
   RET(perspective_op(H, interp, &op));
   RET(check_warp_depth(op, t));
+  RET(set_border(&op, t, border, bval));
   return host_image(c, op, src, sw, sh, sstride, t, dst, dw, dh, dstride);
 }
 int bevk_warp_perspective(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels,
                           const double H[9], uint8_t* dst, int dw, int dh, int64_t dstride, int interp) {
   RET(use(c));
-  return perspective_image(c, src, sw, sh, sstride, u8(channels), H, dst, dw, dh, dstride, interp);
+  return perspective_image(c, src, sw, sh, sstride, u8(channels), H, dst, dw, dh, dstride, interp, BORDER_CONSTANT, nullptr);
 }
 int bevk_warp_perspective_typed(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, int type, const double H[9],
                                 void* dst, int dw, int dh, int64_t dstride, int interp) {
+  return bevk_warp_perspective_border(c, src, sw, sh, sstride, type, H, dst, dw, dh, dstride, interp, BORDER_CONSTANT, nullptr);
+}
+int bevk_warp_perspective_border(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, int type, const double H[9],
+                                void* dst, int dw, int dh, int64_t dstride, int interp, int border_mode,
+                                 const double border_value[4]) {
   RET(use(c));
   PixType t;
   RET(pix_type(type, &t));
-  return perspective_image(c, src, sw, sh, sstride, t, H, dst, dw, dh, dstride, interp);
+  return perspective_image(c, src, sw, sh, sstride, t, H, dst, dw, dh, dstride, interp, border_mode, border_value);
 }
 
 // ------------------------------------------------------------------ cv2.warpAffine
 static int affine_image(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, PixType t, const double M[6], void* dst,
-                        int dw, int dh, int64_t dstride, int flags) {
+                        int dw, int dh, int64_t dstride, int flags, int border, const double* bval) {
   ImageOp op;
   RET(affine_op(M, flags, &op));
   RET(check_warp_depth(op, t));
+  RET(set_border(&op, t, border, bval));
   return host_image(c, op, src, sw, sh, sstride, t, dst, dw, dh, dstride);
 }
 int bevk_warp_affine(bevk_ctx* c, const uint8_t* src, int sw, int sh, int64_t sstride, int channels, const double M[6],
                      uint8_t* dst, int dw, int dh, int64_t dstride, int flags) {
   RET(use(c));
-  return affine_image(c, src, sw, sh, sstride, u8(channels), M, dst, dw, dh, dstride, flags);
+  return affine_image(c, src, sw, sh, sstride, u8(channels), M, dst, dw, dh, dstride, flags, BORDER_CONSTANT, nullptr);
 }
 int bevk_warp_affine_typed(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, int type, const double M[6], void* dst,
                            int dw, int dh, int64_t dstride, int flags) {
+  return bevk_warp_affine_border(c, src, sw, sh, sstride, type, M, dst, dw, dh, dstride, flags, BORDER_CONSTANT, nullptr);
+}
+int bevk_warp_affine_border(bevk_ctx* c, const void* src, int sw, int sh, int64_t sstride, int type, const double M[6], void* dst,
+                           int dw, int dh, int64_t dstride, int flags, int border_mode,
+                            const double border_value[4]) {
   RET(use(c));
   PixType t;
   RET(pix_type(type, &t));
-  return affine_image(c, src, sw, sh, sstride, t, M, dst, dw, dh, dstride, flags);
+  return affine_image(c, src, sw, sh, sstride, t, M, dst, dw, dh, dstride, flags, border_mode, border_value);
 }
 
 static int affine_frames(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
                          PixType t, int n, const double M[6], void* d_dst, int64_t dst_image_stride, int dw, int dh,
-                         int64_t dst_row_stride, int flags) {
+                         int64_t dst_row_stride, int flags, int border, const double* bval) {
   ImageOp op;
   RET(affine_op(M, flags, &op));
   RET(check_warp_depth(op, t));
+  RET(set_border(&op, t, border, bval));
   return device_image(c, op, d_src, src_image_stride, sw, sh, src_row_stride, t, n, d_dst, dst_image_stride, dw, dh,
                       dst_row_stride);
 }
@@ -1237,16 +1321,23 @@ int bevk_warp_affine_stack(bevk_ctx* c, const void* d_src, int64_t src_image_str
                            int64_t dst_row_stride, int flags) {
   RET(use(c));
   return affine_frames(c, d_src, src_image_stride, sw, sh, src_row_stride, u8(channels), n, M, d_dst, dst_image_stride, dw, dh,
-                       dst_row_stride, flags);
+                       dst_row_stride, flags, BORDER_CONSTANT, nullptr);
 }
 int bevk_warp_affine_stack_typed(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
                                  int type, int n, const double M[6], void* d_dst, int64_t dst_image_stride, int dw, int dh,
                                  int64_t dst_row_stride, int flags) {
+  return bevk_warp_affine_stack_border(c, d_src, src_image_stride, sw, sh, src_row_stride, type, n, M, d_dst, dst_image_stride,
+                                       dw, dh, dst_row_stride, flags, BORDER_CONSTANT, nullptr);
+}
+int bevk_warp_affine_stack_border(bevk_ctx* c, const void* d_src, int64_t src_image_stride, int sw, int sh, int64_t src_row_stride,
+                                 int type, int n, const double M[6], void* d_dst, int64_t dst_image_stride, int dw, int dh,
+                                 int64_t dst_row_stride, int flags, int border_mode,
+                                  const double border_value[4]) {
   RET(use(c));
   PixType t;
   RET(pix_type(type, &t));
   return affine_frames(c, d_src, src_image_stride, sw, sh, src_row_stride, t, n, M, d_dst, dst_image_stride, dw, dh,
-                       dst_row_stride, flags);
+                       dst_row_stride, flags, border_mode, border_value);
 }
 
 // ------------------------------------------------------------------ cv2.resize

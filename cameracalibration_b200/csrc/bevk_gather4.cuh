@@ -21,17 +21,37 @@ struct Ldg {
   __host__ __device__ __forceinline__ static int b8(const uint8_t* p) { return ldg8(p); }
 };
 
-// one output pixel: fixed-point source position -> packed B | G<<8 | R<<16.
+// one output pixel: fixed-point source position -> packed B | G<<8 | R<<16.  BD (k_gather4_border): a window not wholly
+// inside takes its taps through border_window instead (bd: any mode but BORDER_TRANSPARENT, which gather4_ok sends to
+// k_gather_border); a window the border value fills is the Q10 sum of four border taps, which is the value itself.
 // The word loads read nothing outside the taps' own rows, rounded out to whole 32-bit words, so frames need no
 // slack after them: `inside` means both taps of each row, bytes [off, off + 6) with off = 3 * sx, lie in the row.
 // The loaded words start at off_al = off & ~3 and off_al + 4, and at off_al + 8 only when off % 4 == 3.  Each of
 // them holds a byte of [off, off + 6): off itself; off_al + 4, which is in [off + 1, off + 4]; off_al + 8 = off + 5.
 // With the row's first byte on a 4-byte boundary (src, spitch 4-aligned; checked by the host), every word loaded
 // is therefore one of the row's own words.
-template <class LD = Ldg>
+template <class LD = Ldg, bool BD = false>
 __host__ __device__ __forceinline__ unsigned gather_px(const uint8_t* __restrict__ src, unsigned spitch, int sw, int sh, int sx, int sy,
-                                              unsigned fx, unsigned fy) {
+                                              unsigned fx, unsigned fy, const Border& bd = Border{}) {
   const bool inside = sx >= 0 && sy >= 0 && sx + 1 < sw && sy + 1 < sh;
+  if constexpr (BD) {
+    if (!inside) {
+      int xs[2], ys[2], p[4][3];
+      const bool fill = border_window<2>(bd, sx, sy, sw, sh, xs, ys) != BW_TAPS;
+#pragma unroll
+      for (int t = 0; t < 4; ++t) {
+        const int tx = xs[t & 1], ty = ys[t >> 1];
+        if (!fill && (tx | ty) >= 0) {
+          const uint8_t* q = src + (size_t)ty * spitch + 3 * tx;
+          p[t][0] = LD::b8(q); p[t][1] = LD::b8(q + 1); p[t][2] = LD::b8(q + 2);
+        } else { p[t][0] = bd.v[0]; p[t][1] = bd.v[1]; p[t][2] = bd.v[2]; }
+      }
+      const unsigned ob = (unsigned)bilerp_q10(p[0][0], p[1][0], p[2][0], p[3][0], (int)fx, (int)fy);
+      const unsigned og = (unsigned)bilerp_q10(p[0][1], p[1][1], p[2][1], p[3][1], (int)fx, (int)fy);
+      const unsigned orr = (unsigned)bilerp_q10(p[0][2], p[1][2], p[2][2], p[3][2], (int)fx, (int)fy);
+      return ob | (og << 8) | (orr << 16);
+    }
+  }
   if (inside) {
     const unsigned off = (unsigned)sy * spitch + 3u * (unsigned)sx;
     const unsigned off_al = off & ~3u, sh8 = (off & 3u) * 8u;
@@ -62,7 +82,7 @@ __host__ __device__ __forceinline__ unsigned gather_px(const uint8_t* __restrict
 // (tests/host/undistort_stack.cu).  Requirements checked by the host (gather4_ok in bevk_api.cu): channels == 3,
 // INTER_LINEAR, dw % 4 == 0; src, dst, both row pitches and (n > 1) both image strides multiples of 4; spitch * sh < 2^31
 // (gather_px's 32-bit offsets within a frame).
-template <int MODE, int NB, class LD = Ldg, int LENS = 0>
+template <int MODE, int NB, class LD = Ldg, int LENS = 0, bool BD = false>
 __host__ __device__ __forceinline__ void gather4_frames(const GatherArgs& a, int x4, int y, int f0) {
   short mx[4], my[4];
   unsigned short fr[4];
@@ -99,7 +119,7 @@ __host__ __device__ __forceinline__ void gather4_frames(const GatherArgs& a, int
     else source_pos<MODE, LENS>(a, x4 + q, y, false, sx[q], sy[q], fx[q], fy[q]);
     // one frame (launched only for n = 1, so f0 = 0): gather each pixel as soon as its taps are known, as the
     // single-frame kernel always did -- about half the registers of the batch form, twice the occupancy
-    if (NB == 1) px[q] = gather_px<LD>(a.src, (unsigned)a.spitch, a.sw, a.sh, sx[q], sy[q], fx[q], fy[q]);
+    if (NB == 1) px[q] = gather_px<LD, BD>(a.src, (unsigned)a.spitch, a.sw, a.sh, sx[q], sy[q], fx[q], fy[q], a.bd);
   }
   const int nf = a.n - f0 < NB ? a.n - f0 : NB;
   const uint8_t* s = a.src + (long long)f0 * a.sistride;
@@ -107,7 +127,7 @@ __host__ __device__ __forceinline__ void gather4_frames(const GatherArgs& a, int
   for (int f = 0; f < nf; ++f, s += a.sistride, d += a.distride) {
     if (NB != 1) {
 #pragma unroll
-      for (int q = 0; q < 4; ++q) px[q] = gather_px<LD>(s, (unsigned)a.spitch, a.sw, a.sh, sx[q], sy[q], fx[q], fy[q]);
+      for (int q = 0; q < 4; ++q) px[q] = gather_px<LD, BD>(s, (unsigned)a.spitch, a.sw, a.sh, sx[q], sy[q], fx[q], fy[q], a.bd);
     }
     unsigned* o = reinterpret_cast<unsigned*>(NB == 1 ? a.dst + (long long)y * a.dpitch + (long long)x4 * 3 : d);
     o[0] = lane_perm(px[0], px[1], 0x4210);   // B0 G0 R0 B1
@@ -125,6 +145,15 @@ __global__ void __launch_bounds__(256) k_gather4(GatherArgs a) {
   const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x4 >= a.dw || y >= a.dh) return;
   gather4_frames<MODE, NB, Ldg, LENS>(a, x4, y, blockIdx.z * NB);
+}
+
+// k_gather4 under cv2's other border modes and values but BORDER_TRANSPARENT (gather_px's BD form)
+template <int MODE, int NB, int LENS>
+__global__ void __launch_bounds__(256) k_gather4_border(GatherArgs a) {
+  const int x4 = (blockIdx.x * 32 + (threadIdx.x & 31)) * 4;
+  const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x4 >= a.dw || y >= a.dh) return;
+  gather4_frames<MODE, NB, Ldg, LENS, true>(a, x4, y, blockIdx.z * NB);
 }
 
 }  // namespace bevk

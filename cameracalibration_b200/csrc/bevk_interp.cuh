@@ -1,6 +1,6 @@
-// bevk_interp.cuh -- cv2.remap's INTER_CUBIC and INTER_LANCZOS4 for 8-bit images (OpenCV 4.13, CV_16SC2 + CV_16UC1
-// maps, BORDER_CONSTANT 0): the fixed-point weight tables and the per-pixel tap sum, shared by the device gathers
-// (k_gather_taps) and the host harness tests/host/remap_interp.cu.  DESIGN.md section 2 has the arithmetic.
+// bevk_interp.cuh -- cv2.remap's INTER_CUBIC and INTER_LANCZOS4 (OpenCV 4.13, CV_16SC2 + CV_16UC1 maps): the weight
+// tables and the per-pixel tap sums, and cv2's border modes for every gather (border_window), shared by the device
+// gathers and the host harnesses under tests/host/.  DESIGN.md section 2 has the arithmetic.
 #pragma once
 #include <float.h>
 #include <math.h>
@@ -136,13 +136,185 @@ __host__ __device__ __forceinline__ void st_sum(uint8_t* p, float v) {
 #endif
 }
 
+// ---- Borders: what the gathers read for a tap outside the source, as cv2.remap / warpPerspective / warpAffine do.
+// cv2's border modes, with cv2's values (BEVK_BORDER_* in include/bevk.h).
+constexpr int BORDER_CONSTANT = 0, BORDER_REPLICATE = 1, BORDER_REFLECT = 2, BORDER_WRAP = 3, BORDER_REFLECT_101 = 4,
+              BORDER_TRANSPARENT = 5;
+
+// A gather's border mode and value.  v holds four elements of the image's depth (bytes 0..4*esize), converted from
+// cv2's Scalar as cv2 converts it (make_border); channel c reads element c.
+struct Border {
+  int mode;
+  unsigned char v[16];
+};
+
+template <class T>
+__host__ __device__ __forceinline__ T border_elem(const Border& b, int c) {
+  T r;
+  memcpy(&r, b.v + c * sizeof(T), sizeof r);
+  return r;
+}
+
+// cv2's Scalar border value at depth (0 8U, 2 16U, 3 16S, 5 32F) as cv2's scalarToRawData converts it: cvRound (half
+// to even; INT_MIN for NaN, +-inf and anything beyond int) then saturation at the integer depths, (float) at 32F.
+inline Border make_border(int mode, int depth, const double (&val)[4]) {
+  Border b{};
+  b.mode = mode;
+  for (int c = 0; c < 4; ++c) {
+    const double v = val[c];
+    if (depth == 5) {
+      const float f = (float)v;
+      memcpy(b.v + 4 * c, &f, 4);
+    } else if (depth == 0) {
+      b.v[c] = (unsigned char)max(0, min(255, cv_round(v)));
+    } else {
+      const int lo = depth == 2 ? 0 : -32768, hi = depth == 2 ? 65535 : 32767;
+      const unsigned short e = (unsigned short)max(lo, min(hi, cv_round(v)));
+      memcpy(b.v + 2 * c, &e, 2);
+    }
+  }
+  return b;
+}
+
+// cv2.borderInterpolate in closed form: the source index position p reads on an axis of n >= 1 pixels, or -1 for the
+// border value (BORDER_CONSTANT).  cv2 walks REFLECT and REFLECT_101 back one period per loop pass (about 16k passes for
+// a 2-pixel axis at the int16 floor); the remainder modulo the period gives the same index for every p.
+__host__ __device__ __forceinline__ int border_index(int p, int n, int mode) {
+  if ((unsigned)p < (unsigned)n) return p;
+  if (mode == BORDER_REPLICATE) return p < 0 ? 0 : n - 1;
+  if (mode == BORDER_WRAP) {
+    const int q = p % n;
+    return q < 0 ? q + n : q;
+  }
+  if (mode == BORDER_REFLECT || mode == BORDER_REFLECT_101) {
+    if (n == 1) return 0;
+    const int d = mode == BORDER_REFLECT_101, per = 2 * (n - d);   // REFLECT: ..cb|abc..; REFLECT_101: ..c|abc..
+    int q = p % per;
+    if (q < 0) q += per;
+    return q < n ? q : per - 1 + d - q;
+  }
+  return -1;
+}
+
+// A K x K window (K = 1 NEAREST, 2 LINEAR, 4 CUBIC, 8 LANCZOS4) with top-left tap (sx, sy), on a source of sw x sh:
+// BW_SKIP, cv2 leaves the destination pixel as it is (BORDER_TRANSPARENT with the window's anchor -- the map's own
+// pixel, tap K/2 - 1 -- outside the source); BW_FILL, cv2 writes the border value (BORDER_CONSTANT, window wholly
+// outside); BW_TAPS, the taps are the source's columns xs and rows ys, -1 standing for the border value.
+// BORDER_TRANSPARENT reads its other windows as REPLICATE (NEAREST, LINEAR) or REFLECT_101 (CUBIC, LANCZOS4).
+enum { BW_TAPS = 0, BW_FILL = 1, BW_SKIP = 2 };
+template <int K>
+__host__ __device__ __forceinline__ int border_window(const Border& b, int sx, int sy, int sw, int sh, int (&xs)[K],
+                                                      int (&ys)[K]) {
+  constexpr int A = K > 1 ? K / 2 - 1 : 0;
+  int m = b.mode;
+  if (m == BORDER_TRANSPARENT) {
+    if ((unsigned)(sx + A) >= (unsigned)sw || (unsigned)(sy + A) >= (unsigned)sh) return BW_SKIP;
+    m = K > 2 ? BORDER_REFLECT_101 : BORDER_REPLICATE;
+  } else if (m == BORDER_CONSTANT && (sx >= sw || sx + K <= 0 || sy >= sh || sy + K <= 0)) {
+    return BW_FILL;
+  }
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    xs[k] = border_index(sx + k, sw, m);
+    ys[k] = border_index(sy + k, sh, m);
+  }
+  return BW_TAPS;
+}
+
+// The border value's C elements written as the pixel at o
+template <int C, class T>
+__host__ __device__ __forceinline__ void st_border(uint8_t* o, const Border& b) {
+#pragma unroll
+  for (int c = 0; c < C; ++c) {
+#ifdef __CUDA_ARCH__
+    reinterpret_cast<T*>(o)[c] = border_elem<T>(b, c);
+#else
+    memcpy(o + c * sizeof(T), b.v + c * sizeof(T), sizeof(T));
+#endif
+  }
+}
+
+// ---- A window of taps_px / taps_px_f that is not wholly inside the source, under any border (border_window): OpenCV
+// sums it as cv * ONE + sum (S - cv) w over the taps it reads, cv the border value in every mode.  With int16 weights
+// summing to 2^15 (8U) that is the sum with cv in place of the taps outside; in float (16U, 16S, 32F) it is not, so cv
+// changes such windows even under REPLICATE, where no tap is outside.  The float sum takes the taps one by one in
+// row-major order.
+template <int KS, int C>
+__host__ __device__ __forceinline__ void taps_px_edge(const uint8_t* __restrict__ src, long long spitch, int sw, int sh, int sx,
+                                                      int sy, const short (&w)[KS * KS], uint8_t* __restrict__ o,
+                                                      const Border& bd) {
+  int xs[KS], ys[KS];
+  const int act = border_window<KS>(bd, sx, sy, sw, sh, xs, ys);
+  if (act == BW_SKIP) return;
+  if (act == BW_FILL) {
+    st_border<C, uint8_t>(o, bd);
+    return;
+  }
+  int sum[C];
+#pragma unroll
+  for (int c = 0; c < C; ++c) sum[c] = (int)bd.v[c] << COEF_BITS;
+#pragma unroll
+  for (int k1 = 0; k1 < KS; ++k1) {
+    if (ys[k1] < 0) continue;
+    const uint8_t* q = src + (long long)ys[k1] * spitch;
+#pragma unroll
+    for (int k2 = 0; k2 < KS; ++k2) {
+      if (xs[k2] < 0) continue;
+#pragma unroll
+      for (int c = 0; c < C; ++c) sum[c] += (tap8(q + (long long)xs[k2] * C + c) - (int)bd.v[c]) * w[k1 * KS + k2];
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < C; ++c) o[c] = (uint8_t)max(0, min(255, (sum[c] + (1 << (COEF_BITS - 1))) >> COEF_BITS));
+}
+
+template <int KS, int C, class T>
+__host__ __device__ __forceinline__ void taps_px_f_edge(const uint8_t* __restrict__ src, long long spitch, int sw, int sh,
+                                                        int sx, int sy, const float (&vy)[KS], const float (&vx)[KS],
+                                                        uint8_t* __restrict__ o, const Border& bd) {
+  constexpr int E = (int)sizeof(T);
+  int xs[KS], ys[KS];
+  const int act = border_window<KS>(bd, sx, sy, sw, sh, xs, ys);
+  if (act == BW_SKIP) return;
+  if (act == BW_FILL) {
+    st_border<C, T>(o, bd);
+    return;
+  }
+  float sum[C], cv[C];
+#pragma unroll
+  for (int c = 0; c < C; ++c) sum[c] = cv[c] = (float)border_elem<T>(bd, c);
+#pragma unroll
+  for (int k1 = 0; k1 < KS; ++k1) {
+    if (ys[k1] < 0) continue;
+    const uint8_t* q = src + (long long)ys[k1] * spitch;
+#pragma unroll
+    for (int k2 = 0; k2 < KS; ++k2) {
+      if (xs[k2] < 0) continue;
+      const float w = fmul(vy[k1], vx[k2]);
+#pragma unroll
+      for (int c = 0; c < C; ++c)
+        sum[c] = fadd(sum[c], fmul(fsub((float)ld_elem<T>(q + ((long long)xs[k2] * C + c) * E), cv[c]), w));
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < C; ++c) st_sum<T>(o + c * E, sum[c]);
+}
+
 // ---- one output pixel of a KS x KS kernel (remapBicubic / remapLanczos4).  (sx, sy): the window's top-left tap, map1 -
 // (KS/2 - 1) in int, so the int16 extremes do not wrap; w: the fraction class's row of weights, k1 * KS + k2.
 // A tap outside the source adds nothing (OpenCV's BORDER_CONSTANT sum is cval * 2^15 + sum (S - cval) w with cval 0, and
 // a window wholly outside is cval); windows wholly inside take OpenCV's fast-path test and read without checks.
-template <int KS, int C>
+// BD (k_gather_taps_border): a window not wholly inside follows border_window (taps_px_edge) instead.
+template <int KS, int C, bool BD = false>
 __host__ __device__ __forceinline__ void taps_px(const uint8_t* __restrict__ src, long long spitch, int sw, int sh, int sx,
-                                                 int sy, const short (&w)[KS * KS], uint8_t* __restrict__ o) {
+                                                 int sy, const short (&w)[KS * KS], uint8_t* __restrict__ o,
+                                                 const Border& bd) {
+  if constexpr (BD) {
+    if (!((unsigned)sx < (unsigned)max(sw - (KS - 1), 0) && (unsigned)sy < (unsigned)max(sh - (KS - 1), 0))) {
+      taps_px_edge<KS, C>(src, spitch, sw, sh, sx, sy, w, o, bd);
+      return;
+    }
+  }
   int sum[C];
 #pragma unroll
   for (int c = 0; c < C; ++c) sum[c] = 0;
@@ -176,9 +348,16 @@ __host__ __device__ __forceinline__ void taps_px(const uint8_t* __restrict__ src
 // left to right; cubic then adds rows 1..3 onto row 0, Lanczos4 adds rows 0..7 onto +0 (so an all -0.0 window gives -0.0
 // with cubic and +0.0 with Lanczos4).  Across an edge the sum starts at +0 and takes the in-frame taps one by one in
 // row-major order; a window wholly outside is +0.  A NaN or inf tap inside the frame poisons the sum whatever its weight.
-template <int KS, int C, class T>
+template <int KS, int C, class T, bool BD = false>
 __host__ __device__ __forceinline__ void taps_px_f(const uint8_t* __restrict__ src, long long spitch, int sw, int sh, int sx,
-                                                   int sy, const float (&vy)[KS], const float (&vx)[KS], uint8_t* __restrict__ o) {
+                                                   int sy, const float (&vy)[KS], const float (&vx)[KS], uint8_t* __restrict__ o,
+                                                   const Border& bd) {
+  if constexpr (BD) {
+    if (!((unsigned)sx < (unsigned)max(sw - (KS - 1), 0) && (unsigned)sy < (unsigned)max(sh - (KS - 1), 0))) {
+      taps_px_f_edge<KS, C, T>(src, spitch, sw, sh, sx, sy, vy, vx, o, bd);
+      return;
+    }
+  }
   constexpr int E = (int)sizeof(T);
   float sum[C];
 #pragma unroll

@@ -141,6 +141,7 @@ struct GatherArgs {
   LensExt lx;                            // MODE 1 with LENS = 1 only
   Homog hm;
   int n; long long sistride, distride;   // frames, and the 64-bit image strides of source and destination
+  Border bd;                             // taps outside the source (border_window); zero-initialised: BORDER_CONSTANT 0
 };
 
 // Frames per thread (grid.z = ceil(n / GATHER_NB)); DESIGN.md section 4 has the measurement that chose it.
@@ -301,12 +302,120 @@ __host__ __device__ __forceinline__ void gather_frames(const GatherArgs& a, int 
   }
 }
 
+// One tap of k_gather at source column x and row y as border_window resolves them (-1: the border value), as ints (8-bit)
+// or as floats (16U, 16S, 32F)
+template <int C>
+__host__ __device__ __forceinline__ void load_tap(const uint8_t* __restrict__ src, long long spitch, int x, int y,
+                                                 const Border& bd, int (&p)[C]) {
+  if ((x | y) >= 0) {
+    const uint8_t* q = src + (long long)y * spitch + (long long)x * C;
+#ifdef __CUDA_ARCH__
+#pragma unroll
+    for (int c = 0; c < C; ++c) p[c] = __ldg(q + c);
+#else
+    for (int c = 0; c < C; ++c) p[c] = q[c];
+#endif
+  } else {
+#pragma unroll
+    for (int c = 0; c < C; ++c) p[c] = bd.v[c];
+  }
+}
+
+template <int C, class T>
+__host__ __device__ __forceinline__ void load_tap_f(const uint8_t* __restrict__ src, long long spitch, int x, int y,
+                                                   const Border& bd, float (&p)[C]) {
+  const bool in = (x | y) >= 0;
+  const uint8_t* q = src + (long long)y * spitch + (long long)x * (C * (int)sizeof(T));
+#pragma unroll
+  for (int c = 0; c < C; ++c) p[c] = (float)(in ? ld_elem<T>(q + c * sizeof(T)) : border_elem<T>(bd, c));
+}
+
+// gather_frames under a border other than a zero BORDER_CONSTANT (k_gather_border): the border (a.bd) is resolved once
+// per pixel for all its frames -- the taps' source columns and rows, the border value, or no write at all.  NEAREST
+// through an entry with a fraction wraps NNDeltaTab's +1 to int16, as cv2's map buffer does (32767 + 1 reads -32768);
+// every other position is int16 already.
+template <int MODE, int C, int LINEAR, int LENS = 0, class T = uint8_t>
+__host__ __device__ __forceinline__ void gather_frames_border(const GatherArgs& a, int x, int y, int f0) {
+  int sx, sy, fx, fy;
+  source_pos<MODE, LENS>(a, x, y, !LINEAR, sx, sy, fx, fy);
+  if (!LINEAR) { sx = (short)sx; sy = (short)sy; }
+  constexpr int K = LINEAR ? 2 : 1;
+  int xs[K], ys[K];
+  const int act = border_window<K>(a.bd, sx, sy, a.sw, a.sh, xs, ys);
+  if (act == BW_SKIP) return;
+  constexpr int PX = C * (int)sizeof(T);   // bytes per pixel
+  const int nf = a.n - f0 < GATHER_NB ? a.n - f0 : GATHER_NB;
+  const uint8_t* s = a.src + (long long)f0 * a.sistride;
+  uint8_t* o = a.dst + (long long)f0 * a.distride + (long long)y * a.dpitch + (long long)x * PX;
+  if (act == BW_FILL) {
+    for (int f = 0; f < nf; ++f, o += a.distride) st_border<C, T>(o, a.bd);
+    return;
+  }
+  if constexpr (sizeof(T) == 1) {
+    for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) {
+      if (LINEAR) {
+        int p00[C], p01[C], p10[C], p11[C];
+        load_tap<C>(s, a.spitch, xs[0], ys[0], a.bd, p00);
+        load_tap<C>(s, a.spitch, xs[K - 1], ys[0], a.bd, p01);
+        load_tap<C>(s, a.spitch, xs[0], ys[K - 1], a.bd, p10);
+        load_tap<C>(s, a.spitch, xs[K - 1], ys[K - 1], a.bd, p11);
+#pragma unroll
+        for (int c = 0; c < C; ++c) o[c] = (uint8_t)bilerp_q10(p00[c], p01[c], p10[c], p11[c], fx, fy);
+      } else {
+        int p[C];
+        load_tap<C>(s, a.spitch, xs[0], ys[0], a.bd, p);
+#pragma unroll
+        for (int c = 0; c < C; ++c) o[c] = (uint8_t)p[c];
+      }
+    }
+  } else if constexpr (LINEAR) {
+    // cv2's float table: w = vy * vx with vx = {1 - fx / 32, fx / 32}, each product rounded to float
+    const float ax = fmul((float)fx, 1.f / TAB), ay = fmul((float)fy, 1.f / TAB);
+    const float bx = fsub(1.f, ax), by = fsub(1.f, ay);
+    const float w00 = fmul(by, bx), w01 = fmul(by, ax), w10 = fmul(ay, bx), w11 = fmul(ay, ax);
+    for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) {
+      float p00[C], p01[C], p10[C], p11[C];
+      load_tap_f<C, T>(s, a.spitch, xs[0], ys[0], a.bd, p00);
+      load_tap_f<C, T>(s, a.spitch, xs[K - 1], ys[0], a.bd, p01);
+      load_tap_f<C, T>(s, a.spitch, xs[0], ys[K - 1], a.bd, p10);
+      load_tap_f<C, T>(s, a.spitch, xs[K - 1], ys[K - 1], a.bd, p11);
+#pragma unroll
+      for (int c = 0; c < C; ++c)   // ((t00 w00 + t01 w01) + t10 w10) + t11 w11, taps outside the frame the border value
+        st_sum<T>(o + c * sizeof(T), fadd(fadd(fadd(fmul(p00[c], w00), fmul(p01[c], w01)), fmul(p10[c], w10)), fmul(p11[c], w11)));
+    }
+  } else {
+    // NEAREST moves the element's bits: a float NaN keeps its payload, -0.0 its sign
+    for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) {
+      const uint8_t* q = s + (long long)ys[0] * a.spitch + (long long)xs[0] * PX;
+#pragma unroll
+      for (int c = 0; c < C; ++c) {
+        const T v = (xs[0] | ys[0]) >= 0 ? ld_elem<T>(q + c * sizeof(T)) : border_elem<T>(a.bd, c);
+#ifdef __CUDA_ARCH__
+        reinterpret_cast<T*>(o)[c] = v;
+#else
+        memcpy(o + c * sizeof(T), &v, sizeof v);
+#endif
+      }
+    }
+  }
+}
+
 template <int MODE, int C, int LINEAR, int LENS, class T>
 __global__ void __launch_bounds__(256) k_gather(GatherArgs a) {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31);
   const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= a.dw || y >= a.dh) return;
   gather_frames<MODE, C, LINEAR, LENS, T>(a, x, y, blockIdx.z * GATHER_NB);
+}
+
+// k_gather under cv2's other border modes and values: a kernel of its own, so that the zero-constant instances keep
+// their machine code and speed
+template <int MODE, int C, int LINEAR, int LENS, class T>
+__global__ void __launch_bounds__(256) k_gather_border(GatherArgs a) {
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31);
+  const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x >= a.dw || y >= a.dh) return;
+  gather_frames_border<MODE, C, LINEAR, LENS, T>(a, x, y, blockIdx.z * GATHER_NB);
 }
 
 // The weights k_gather_taps reads: 8-bit sources the int16 2-D rows of build_interp_tabs, wider ones the float 1-D rows
@@ -320,7 +429,7 @@ using TapWeights = typename std::conditional<sizeof(T) == 1, short, float>::type
 // A 16U, 16S or 32F source instead reads the fraction's two 1-D float rows (2 * KS floats) and forms each 2-D weight as
 // cv2's float table holds it (taps_px_f): 2 * KS registers rather than KS * KS.
 // Host-capable, like gather_frames (tests/host/remap_interp.cu, tests/host/remap_depth.cu).
-template <int MODE, int C, int KS, int LENS = 0, class T = uint8_t>
+template <int MODE, int C, int KS, int LENS = 0, class T = uint8_t, bool BD = false>
 __host__ __device__ __forceinline__ void gather_taps_frames(const GatherArgs& a, const TapWeights<T>* __restrict__ wtab, int x,
                                                             int y, int f0) {
   int sx, sy, fx, fy;
@@ -344,7 +453,7 @@ __host__ __device__ __forceinline__ void gather_taps_frames(const GatherArgs& a,
     const int nf = a.n - f0 < GATHER_NB ? a.n - f0 : GATHER_NB;
     const uint8_t* s = a.src + (long long)f0 * a.sistride;
     uint8_t* o = a.dst + (long long)f0 * a.distride + (long long)y * a.dpitch + (long long)x * (C * (int)sizeof(T));
-    for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) taps_px<KS, C>(s, a.spitch, a.sw, a.sh, sx, sy, w, o);
+    for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) taps_px<KS, C, BD>(s, a.spitch, a.sw, a.sh, sx, sy, w, o, a.bd);
   } else {
     float vy[KS], vx[KS];
     const float* ry = wtab + fy * KS;
@@ -363,7 +472,7 @@ __host__ __device__ __forceinline__ void gather_taps_frames(const GatherArgs& a,
     const int nf = a.n - f0 < GATHER_NB ? a.n - f0 : GATHER_NB;
     const uint8_t* s = a.src + (long long)f0 * a.sistride;
     uint8_t* o = a.dst + (long long)f0 * a.distride + (long long)y * a.dpitch + (long long)x * (C * (int)sizeof(T));
-    for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) taps_px_f<KS, C, T>(s, a.spitch, a.sw, a.sh, sx, sy, vy, vx, o);
+    for (int f = 0; f < nf; ++f, s += a.sistride, o += a.distride) taps_px_f<KS, C, T, BD>(s, a.spitch, a.sw, a.sh, sx, sy, vy, vx, o, a.bd);
   }
 }
 
@@ -373,6 +482,15 @@ __global__ void __launch_bounds__(256) k_gather_taps(GatherArgs a, const TapWeig
   const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= a.dw || y >= a.dh) return;
   gather_taps_frames<MODE, C, KS, LENS, T>(a, wtab, x, y, blockIdx.z * GATHER_NB);
+}
+
+// k_gather_taps under cv2's other border modes and values (BD: the edge windows follow border_window)
+template <int MODE, int C, int KS, int LENS, class T>
+__global__ void __launch_bounds__(256) k_gather_taps_border(GatherArgs a, const TapWeights<T>* __restrict__ wtab) {
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31);
+  const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x >= a.dw || y >= a.dh) return;
+  gather_taps_frames<MODE, C, KS, LENS, T, true>(a, wtab, x, y, blockIdx.z * GATHER_NB);
 }
 
 // ---------------------------------------------------------------------------------

@@ -15,6 +15,9 @@ _INTERPOLATIONS = (INTER_NEAREST, INTER_LINEAR, INTER_CUBIC, INTER_AREA, INTER_L
 CV_16SC2, CV_32FC1, CV_32FC2 = L.CV_16SC2, L.CV_32FC1, L.CV_32FC2
 _MAP_TYPES = (CV_16SC2, CV_32FC1, CV_32FC2)
 
+# cv2's border modes (cv2.BORDER_*), for remap, warp_perspective, warp_affine and Undistorter
+BORDER_CONSTANT, BORDER_REPLICATE, BORDER_REFLECT, BORDER_WRAP, BORDER_REFLECT_101, BORDER_TRANSPARENT = 0, 1, 2, 3, 4, 5
+
 
 def _interp(flag: int) -> int:
     if flag not in _INTERPOLATIONS:
@@ -393,8 +396,9 @@ def imencode(ext: str, images, params=None, ctx: L.Context | None = None) -> lis
 
 
 def remap(src: np.ndarray, map1: np.ndarray, map2: np.ndarray | None, interpolation: int = INTER_LINEAR,
-          ctx: L.Context | None = None, out: np.ndarray | None = None) -> np.ndarray:
-    """cv2.remap with CV_16SC2 (+CV_16UC1) maps, BORDER_CONSTANT 0.  interpolation: INTER_NEAREST, INTER_LINEAR,
+          ctx: L.Context | None = None, out: np.ndarray | None = None, borderMode: int = BORDER_CONSTANT,
+          borderValue=0) -> np.ndarray:
+    """cv2.remap with CV_16SC2 (+CV_16UC1) maps.  interpolation: INTER_NEAREST, INTER_LINEAR,
     INTER_CUBIC, INTER_AREA (read as INTER_LINEAR, as cv2.remap reads it) or INTER_LANCZOS4; all but NEAREST need map2.
     The result is byte-identical to cv2.remap's.
 
@@ -404,10 +408,15 @@ def remap(src: np.ndarray, map1: np.ndarray, map2: np.ndarray | None, interpolat
     on the device (``out``, default a new torch tensor).
 
     src may be uint8, uint16, int16 or float32 (CUDA typestr <u2, <i2, <f4); the result has src's dtype and cv2's bits
-    at that depth (DESIGN.md section 2)."""
+    at that depth (DESIGN.md section 2).
+
+    borderMode, borderValue: cv2's, bit for bit (BORDER_CONSTANT, _REPLICATE, _REFLECT, _WRAP, _REFLECT_101 and
+    _TRANSPARENT; a number v means (v, 0, 0, 0)).  BORDER_TRANSPARENT writes into ``out``, which it needs; LINEAR under it
+    at float32, which cv2 sums another way, raises BevkError (include/bevk.h has the rules)."""
+    border = _border(borderMode, borderValue, out)
     ctx = ctx or L.default_context()
     if _is_float32(map1):
-        return _remap_f32(src, map1, map2, interpolation, ctx, out)
+        return _remap_f32(src, map1, map2, interpolation, ctx, out, border)
     m1 = np.ascontiguousarray(map1, np.int16)
     if m1.ndim != 3 or m1.shape[2] != 2:
         raise L.BevkError("map1 must be int16[h][w][2] (CV_16SC2)")
@@ -416,7 +425,8 @@ def remap(src: np.ndarray, map1: np.ndarray, map2: np.ndarray | None, interpolat
     if m2 is not None and m2.shape != (dh, dw):
         raise L.BevkError("map2 must be uint16[h][w] (CV_16UC1)")
     return _host_image(src, dw, dh, out, lambda f, s, d, dstride: f(
-        ctx.h, *s, L.vptr(m1), None if m2 is None else L.vptr(m2), dw, dh, d, dstride, _interp(interpolation)), ctx.lib, "bevk_remap")
+        ctx.h, *s, L.vptr(m1), None if m2 is None else L.vptr(m2), dw, dh, d, dstride, _interp(interpolation)), ctx.lib, "bevk_remap",
+        border)
 
 
 def _is_float32(a) -> bool:
@@ -476,19 +486,19 @@ def _device_maps(maps, dtypes, ctx):
     return ptrs, keep
 
 
-def _remap_f32(src, map1, map2, interpolation, ctx, out):
+def _remap_f32(src, map1, map2, interpolation, ctx, out, border=None):
     dh, dw = _float_map_shapes(map1, map2)
     if hasattr(src, "__cuda_array_interface__"):
         (m1, m2), keep = _device_maps((map1, map2), (np.float32, np.float32), ctx)
         return _device_images(src, dw, dh, out, ctx, "remap", lambda f, s, d: f(
-            ctx.h, *s, m1, m2, *d, _interp(interpolation)), name="bevk_remap_f32_stack")
+            ctx.h, *s, m1, m2, *d, _interp(interpolation)), name="bevk_remap_f32_stack", border=border)
     if hasattr(map1, "__cuda_array_interface__") or hasattr(map2, "__cuda_array_interface__"):
         raise L.BevkError("remap: CUDA maps need a CUDA source image")
     m1 = np.ascontiguousarray(map1, np.float32)
     m2 = None if map2 is None else np.ascontiguousarray(map2, np.float32)
     return _host_image(src, dw, dh, out, lambda f, s, d, dstride: f(
         ctx.h, *s, L.vptr(m1), None if m2 is None else L.vptr(m2), dw, dh, d, dstride, _interp(interpolation)), ctx.lib,
-        "bevk_remap_f32")
+        "bevk_remap_f32", border)
 
 
 def convert_maps(map1, map2, dstmap1type: int, nninterpolation: bool = False, ctx: L.Context | None = None):
@@ -533,32 +543,64 @@ def convert_maps(map1, map2, dstmap1type: int, nninterpolation: bool = False, ct
 
 
 def warp_perspective(src: np.ndarray, H, dsize, flags: int = INTER_LINEAR, ctx: L.Context | None = None,
-                     out: np.ndarray | None = None):
-    """cv2.warpPerspective(src, H, dsize, flags) for uint8, uint16, int16 and float32 images, BORDER_CONSTANT 0.  flags:
+                     out: np.ndarray | None = None, borderMode: int = BORDER_CONSTANT, borderValue=0):
+    """cv2.warpPerspective(src, H, dsize, flags, borderMode=, borderValue=) for uint8, uint16, int16 and float32 images,
+    borders as remap() takes them; NEAREST and LINEAR at int16 under BORDER_REPLICATE / BORDER_TRANSPARENT raise
+    BevkError (cv2 computes them with another body than cv2.remap's).  flags:
     INTER_NEAREST, INTER_LINEAR, INTER_CUBIC, INTER_AREA (read as INTER_LINEAR, as cv2 reads it) or INTER_LANCZOS4; LINEAR / AREA at
     uint16 with 3 or 4 channels and NEAREST at float32 with 1 or 4 channels raise BevkError (cv2 computes them with
     other bodies than cv2.remap's)."""
+    border = _border(borderMode, borderValue, out)
     ctx = ctx or L.default_context()
     dw, dh = int(dsize[0]), int(dsize[1])
     return _host_image(src, dw, dh, out, lambda f, s, d, dstride: f(
-        ctx.h, *s, L.dptr(H), d, dw, dh, dstride, _interp(flags)), ctx.lib, "bevk_warp_perspective")
+        ctx.h, *s, L.dptr(H), d, dw, dh, dstride, _interp(flags)), ctx.lib, "bevk_warp_perspective", border)
 
 
 INTER_LINEAR_EXACT, INTER_NEAREST_EXACT, WARP_INVERSE_MAP = L.INTER_LINEAR_EXACT, L.INTER_NEAREST_EXACT, L.WARP_INVERSE_MAP
-BORDER_CONSTANT = 0
 
 
-def _gather_fn(lib, name, dtype):
+def _border(borderMode, borderValue, out):
+    """cv2's borderMode and borderValue as a gather's _border arguments (mode, double[4]), or None for the zero constant
+    border, which the _typed and uint8 entry points give.  borderValue follows cv2's Scalar: a number v is (v, 0, 0, 0),
+    a sequence gives up to four values.  The library checks the mode (BORDER_ISOLATED and unknown modes raise) and
+    converts the values to the image's depth as cv2 does.  BORDER_TRANSPARENT leaves pixels of the destination as they
+    were, so it needs ``out``: cv2 leaves them undefined in a new array."""
+    vals = np.atleast_1d(np.asarray(borderValue, np.float64)).ravel()
+    if vals.size > 4:
+        raise L.BevkError(f"borderValue takes up to 4 values (cv2's Scalar), got {vals.size}")
+    mode = int(borderMode)
+    if mode == BORDER_TRANSPARENT and out is None:
+        raise L.BevkError("BORDER_TRANSPARENT needs out=: it writes only some pixels of the destination")
+    if mode == BORDER_CONSTANT and not vals.any():
+        return None
+    v = (C.c_double * 4)(*vals, *[0.0] * (4 - vals.size))
+    return mode, v
+
+
+def _gather_fn(lib, name, dtype, border=None):
     """The library entry point of an image gather: `name` for uint8 images, its _typed sibling (a cv2 type code in place
-    of the channel count) for uint16, int16 and float32 ones."""
+    of the channel count) for uint16, int16 and float32 ones, and with a border (_border's) its _border sibling, which
+    takes the type code at every depth and the border after the _typed arguments."""
+    if border is not None:
+        fn = getattr(lib, name + "_border")
+        return lambda *a: fn(*a, *border)
     return getattr(lib, name) if dtype == np.uint8 else getattr(lib, name + "_typed")
 
 
-def _host_image(src, dw, dh, out, call, lib=None, name=None):
+def _type_code(dtype, ch, border):
+    """The kind argument of a gather entry point: the channel count for uint8 images without a border, else cv2's type
+    code."""
+    if dtype == np.uint8:
+        return ch if border is None else (ch - 1) << 3
+    return _WIDE[dtype] + ((ch - 1) << 3)
+
+
+def _host_image(src, dw, dh, out, call, lib=None, name=None, border=None):
     """The body of the host forms: src a NumPy image [H][W] or [H][W][C]; out (default a new array) [dh][dw] of the same
     rank and dtype; call(src, dst, dst_stride) with src's (pointer, width, height, stride, channels) and dst's pointer.
     With lib and name (an image gather) src may also be uint16, int16 or float32: call then takes the entry point first
-    (_gather_fn), and the channel count becomes the cv2 type code for the _typed sibling."""
+    (_gather_fn), and the channel count becomes the cv2 type code for the _typed sibling.  border: _border's."""
     if name is None:
         img, sw, sh, ss, ch = L.image_view(src)
         out = _out((dh, dw) if src.ndim == 2 else (dh, dw, ch), out)
@@ -566,17 +608,18 @@ def _host_image(src, dw, dh, out, call, lib=None, name=None):
         return out
     img, sw, sh, ss, ch = L.image_view(src, (np.uint8, *_WIDE))
     out = _out((dh, dw) if src.ndim == 2 else (dh, dw, ch), out, img.dtype)
-    kind = ch if img.dtype == np.uint8 else _WIDE[img.dtype] + ((ch - 1) << 3)
-    L.check(call(_gather_fn(lib, name, img.dtype), (L.vptr(img), sw, sh, ss, kind), L.vptr(out), dw * ch * img.itemsize))
+    kind = _type_code(img.dtype, ch, border)
+    L.check(call(_gather_fn(lib, name, img.dtype, border), (L.vptr(img), sw, sh, ss, kind), L.vptr(out),
+                 dw * ch * img.itemsize))
     return out
 
 
-def _device_images(src, dw, dh, out, ctx, what, call, stream=None, name=None):
+def _device_images(src, dw, dh, out, ctx, what, call, stream=None, name=None, border=None):
     """The body of the device forms: src a uint8 CUDA array [H][W], [H][W][C] or [N][H][W][C] read in place; out
     (default a new torch tensor) of the same rank with dh x dw images; call(src, out) with the (pointer, image stride,
     ...) layouts is run on ``stream`` (default torch's current stream) and only enqueues.  With name (an image gather)
     src may also be uint16, int16 or float32 (typestr <u2, <i2, <f4), out of the same dtype, and call takes the entry
-    point first, as _host_image's does."""
+    point first, as _host_image's does (border too)."""
     wide = name is not None
     ptr, rank, n, sh, sw, ch, simg, srow = _cuda_images(src, what, wide)
     dtype = _cuda_dtype(src) if wide else np.dtype(np.uint8)
@@ -590,19 +633,19 @@ def _device_images(src, dw, dh, out, ctx, what, call, stream=None, name=None):
     if stream is None:
         from .sharding import _torch_current_stream
         stream = _torch_current_stream(ctx.device)
-    kind = ch if dtype == np.uint8 else _WIDE[dtype] + ((ch - 1) << 3)
+    kind = _type_code(dtype, ch, border)
     s, d = (C.c_void_p(ptr), simg, sw, sh, srow, kind, n), (C.c_void_p(optr), oimg, dw, dh, orow)
     with ctx.on_stream(stream):
-        L.check(call(_gather_fn(ctx.lib, name, dtype), s, d) if wide else call(s, d))
+        L.check(call(_gather_fn(ctx.lib, name, dtype, border), s, d) if wide else call(s, d))
     return out
 
 
-def _image_call(src, dw, dh, out, ctx, what, host, device, name=None):
+def _image_call(src, dw, dh, out, ctx, what, host, device, name=None, border=None):
     """A CUDA array goes to the device form (_device_images, with ``device``), anything else to the host form
     (_host_image, with ``host``); name: the host entry point of an image gather (its device form is name + "_stack")."""
     if hasattr(src, "__cuda_array_interface__"):
-        return _device_images(src, dw, dh, out, ctx, what, device, name=name and name + "_stack")
-    return _host_image(src, dw, dh, out, host, ctx.lib, name)
+        return _device_images(src, dw, dh, out, ctx, what, device, name=name and name + "_stack", border=border)
+    return _host_image(src, dw, dh, out, host, ctx.lib, name, border)
 
 
 def _src_size(src):
@@ -646,10 +689,23 @@ def warp_affine(src, M, dsize, flags: int = INTER_LINEAR, borderMode: int = BORD
     """cv2.warpAffine(src, M, dsize, flags=flags) for uint8, uint16, int16 and float32 images with a zero
     constant border, bit for bit; NEAREST at int16 and at uint16 with 4 channels raises BevkError (cv2 computes it with
     another body than cv2.remap's).  M: 2x3.
-    flags: any interpolation warp_perspective takes, optionally | WARP_INVERSE_MAP.  Other borders raise BevkError.
+    flags: any interpolation warp_perspective takes, optionally | WARP_INVERSE_MAP.  Other borders raise BevkError:
+    warp_affine_border takes them.
     Takes NumPy images and CUDA arrays as resize() does."""
     if borderMode != BORDER_CONSTANT or np.any(np.asarray(borderValue) != 0):
-        raise L.BevkError("warp_affine supports BORDER_CONSTANT with value 0 only")
+        raise L.BevkError("warp_affine supports BORDER_CONSTANT with value 0 only; warp_affine_border takes cv2's other "
+                          "borders")
+    return _warp_affine(src, M, dsize, flags, None, ctx, out)
+
+
+def warp_affine_border(src, M, dsize, flags: int = INTER_LINEAR, borderMode: int = BORDER_CONSTANT, borderValue=0,
+                       ctx: L.Context | None = None, out=None):
+    """cv2.warpAffine(src, M, dsize, flags=flags, borderMode=borderMode, borderValue=borderValue), bit for bit: warp_affine
+    with cv2's border modes and values as remap() takes them.  BORDER_TRANSPARENT writes into ``out``, which it needs."""
+    return _warp_affine(src, M, dsize, flags, _border(borderMode, borderValue, out), ctx, out)
+
+
+def _warp_affine(src, M, dsize, flags, border, ctx, out):
     ctx = ctx or L.default_context()
     m = np.asarray(M, np.float64)
     if m.shape != (2, 3):
@@ -657,7 +713,7 @@ def warp_affine(src, M, dsize, flags: int = INTER_LINEAR, borderMode: int = BORD
     dw, dh = int(dsize[0]), int(dsize[1])
     return _image_call(src, dw, dh, out, ctx, "warp_affine",
                        lambda f, s, d, ds: f(ctx.h, *s, L.dptr(m), d, dw, dh, ds, int(flags)),
-                       lambda f, s, d: f(ctx.h, *s, L.dptr(m), *d, int(flags)), "bevk_warp_affine")
+                       lambda f, s, d: f(ctx.h, *s, L.dptr(m), *d, int(flags)), "bevk_warp_affine", border)
 
 
 _GATHER_PATHS = {4: "word", 1: "byte", 2: "taps", 3: "resize"}
@@ -799,15 +855,19 @@ class Undistorter:
         L.check(self.ctx.lib.bevk_undistorter_maps(self.ctx.h, self.slot, L.vptr(m1), L.vptr(m2)))
         return m1, m2
 
-    def __call__(self, src: np.ndarray, interpolation: int = INTER_LINEAR, out: np.ndarray | None = None) -> np.ndarray:
-        """cv2.remap(src, map1, map2, interpolation), any of remap()'s interpolations.  A CUDA array (e.g. a torch tensor on the GPU) goes to cuda() and
+    def __call__(self, src: np.ndarray, interpolation: int = INTER_LINEAR, out: np.ndarray | None = None,
+                 borderMode: int = BORDER_CONSTANT, borderValue=0) -> np.ndarray:
+        """cv2.remap(src, map1, map2, interpolation, borderMode=, borderValue=), any of remap()'s interpolations and
+        borders.  A CUDA array (e.g. a torch tensor on the GPU) goes to cuda() and
         the result stays on the device; NumPy input is uploaded, undistorted and downloaded in one call."""
         self._live()
         lib, h = self.ctx.lib, self.ctx.h
         if hasattr(src, "__cuda_array_interface__"):
-            return self.cuda(src, out, interpolation)
+            return self.cuda(src, out, interpolation, borderMode=borderMode, borderValue=borderValue)
+        border = _border(borderMode, borderValue, out)
         return _host_image(src, self.w, self.h, out, lambda f, s, d, ds: f(h, self.slot, *s, d, self.w, self.h, ds,
-                                                                           _interp(interpolation)), lib, "bevk_undistort")
+                                                                           _interp(interpolation)), lib, "bevk_undistort",
+                           border)
 
     def jpeg(self, src: np.ndarray, quality: int = 95, interpolation: int = INTER_LINEAR, params=None) -> bytes:
         """The undistorted image as the bytes cv2.imwrite(path, self(src), [IMWRITE_JPEG_QUALITY, quality] + params)
@@ -838,7 +898,8 @@ class Undistorter:
         d = torch.from_numpy(np.ascontiguousarray(a)).to(torch.device("cuda", self.ctx.device))
         return png_encode(self.cuda(d, interpolation=interpolation), ctx=self.ctx, params=params)[0]
 
-    def cuda(self, frames, out=None, interpolation: int = INTER_LINEAR, stream: int | None = None):
+    def cuda(self, frames, out=None, interpolation: int = INTER_LINEAR, stream: int | None = None,
+             borderMode: int = BORDER_CONSTANT, borderValue=0):
         """Undistort frames that already live on the GPU: no PCIe in the call.
 
         frames: a uint8, uint16, int16 or float32 CUDA array (``__cuda_array_interface__``; ``out`` of the same dtype)
@@ -847,10 +908,12 @@ class Undistorter:
         be padded.  ``out``: a CUDA array of the matching shape (rows and images may be padded too), default a new torch
         tensor.  ``interpolation``: as for __call__.  Each output pixel's map entry (or camera model) and, for INTER_CUBIC /
         INTER_LANCZOS4, its row of weights are read once for several frames of the batch.  Runs on
-        ``stream`` (a raw CUDA stream handle), default torch's current stream, and only enqueues.  Returns ``out``."""
+        ``stream`` (a raw CUDA stream handle), default torch's current stream, and only enqueues.  Returns ``out``.
+        borderMode, borderValue: as remap() takes them; BORDER_TRANSPARENT writes into ``out`` in place."""
         self._live()
+        border = _border(borderMode, borderValue, out)
         return _device_images(frames, self.w, self.h, out, self.ctx, "frames", lambda f, s, d: f(
-            self.ctx.h, self.slot, *s, *d, _interp(interpolation)), stream, "bevk_undistort_stack_interp")
+            self.ctx.h, self.slot, *s, *d, _interp(interpolation)), stream, "bevk_undistort_stack_interp", border)
 
     def cuda_to_jpeg(self, frames, quality: int = 95, interpolation: int = INTER_LINEAR, params=None) -> list[bytes]:
         """cuda() followed by cv2.imencode('.jpg', img, [IMWRITE_JPEG_QUALITY, quality] + params) per frame, with the

@@ -61,6 +61,23 @@ enum { BEVK_CV_32FC1 = 5, BEVK_CV_16SC2 = 11, BEVK_CV_32FC2 = 13 };
  * strides must be multiples of the element size (BEVK_ERR_ARG); all sizes and strides stay in bytes.  The uint8 calls
  * are their _typed siblings at CV_8UC(channels). */
 enum { BEVK_CV_8U = 0, BEVK_CV_16U = 2, BEVK_CV_16S = 3, BEVK_CV_32F = 5 };
+/* cv2's border modes, for the _border gathers (bevk_remap_border, bevk_remap_f32_border, bevk_remap_f32_stack_border,
+ * bevk_undistort_border, bevk_undistort_stack_interp_border, bevk_warp_perspective_border, bevk_warp_affine_border,
+ * bevk_warp_affine_stack_border).  Each takes its _typed sibling's arguments plus border_mode and border_value (cv2's
+ * Scalar: four doubles, NULL for zeros, channel c reading value c), converted to the image's depth as cv2 converts it:
+ * cvRound, half to even, then saturation for 8U, 16U and 16S (NaN, +-inf and values beyond int become INT_MIN first, so
+ * 0 at 8U / 16U and -32768 at 16S), (float) for 32F.  Every pixel is cv2's, bit for bit:
+ *   CONSTANT: taps outside the source read the value (a window wholly outside is the value); REPLICATE, REFLECT, WRAP
+ *   and REFLECT_101 index the source as cv2.borderInterpolate does; CUBIC and LANCZOS4 sum a window across the edge as
+ *   v + sum (S - v) w in every mode, so at 16U, 16S and 32F the value changes such pixels even under REPLICATE.
+ *   TRANSPARENT: a pixel whose map position (the window's anchor) lies outside the source is not written; the others
+ *   read as REPLICATE (NEAREST, LINEAR) or REFLECT_101 (CUBIC, LANCZOS4).  The host calls upload dst first, so its
+ *   untouched pixels come back as they were; the device calls write in place.  It always takes the byte path.
+ * Any other mode, BORDER_ISOLATED included, is BEVK_ERR_ARG.  BEVK_ERR_UNSUPPORTED, because cv2 4.13 leaves remap's
+ * arithmetic there: LINEAR / AREA under TRANSPARENT at CV_32F, and warpPerspective NEAREST / LINEAR at CV_16S under
+ * REPLICATE and TRANSPARENT.  The _typed calls are their _border siblings at CONSTANT with a zero value. */
+enum { BEVK_BORDER_CONSTANT = 0, BEVK_BORDER_REPLICATE = 1, BEVK_BORDER_REFLECT = 2, BEVK_BORDER_WRAP = 3,
+       BEVK_BORDER_REFLECT_101 = 4, BEVK_BORDER_TRANSPARENT = 5 };
 /* bevk_bev_run flags.  BEVK_FLAG_NV12 / BEVK_FLAG_I420 (exclusive; they combine with BALANCE) say the frames are YUV
  * 4:2:0 in cv2's single-buffer layout, uint8[frame_h*3/2][frame_w] (frame_w, frame_h even, else BEVK_ERR_UNSUPPORTED):
  * the Y plane, then NV12: interleaved U,V rows; I420: the U plane, then the V plane, each frame_w/2 x frame_h/2 and
@@ -132,7 +149,7 @@ int bevk_undistort_rectify_map(bevk_ctx *ctx, int model, const double K[9], cons
 int bevk_undistort_rectify_map_f32(bevk_ctx *ctx, int model, const double K[9], const double *D, int n_dist,
                                    const double *R, const double P[9], int w, int h, int m1type, float *map1, float *map2);
 
-/* ---- K3: cv2.remap(src, map1, map2, interp), BORDER_CONSTANT 0 --------------
+/* ---- K3: cv2.remap(src, map1, map2, interp), BORDER_CONSTANT 0 (_border: any mode) 
  *   surroundBEV.py:110-111,116-117; undistort.py:66; intrinsicCalib.py:193-195
  * channels in {1,3,4}; map2 may be NULL for NEAREST with integer maps.  interp: any BEVK_INTER_* (see above).    */
 int bevk_remap(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t sstride, int channels,
@@ -140,6 +157,9 @@ int bevk_remap(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t sstrid
                uint8_t *dst, int64_t dstride, int interp);
 int bevk_remap_typed(bevk_ctx *ctx, const void *src, int sw, int sh, int64_t sstride, int type,
                      const int16_t *map1, const uint16_t *map2, int dw, int dh, void *dst, int64_t dstride, int interp);
+int bevk_remap_border(bevk_ctx *ctx, const void *src, int sw, int sh, int64_t sstride, int type,
+                      const int16_t *map1, const uint16_t *map2, int dw, int dh, void *dst, int64_t dstride, int interp,
+                      int border_mode, const double border_value[4]);
 /* cv2.remap with float maps: map1, map2 float[dh][dw] (CV_32FC1), or map2 NULL and map1 float[dh][dw][2] (CV_32FC2).
  * Byte for byte cv2.convertMaps(map1, map2, CV_16SC2, nninterpolation = (interp == NEAREST)) followed by the integer
  * remap, which is what cv2.remap does: cvRound(x * 32.f) (NEAREST: cvRound(x), half to even, without the integer maps'
@@ -148,6 +168,9 @@ int bevk_remap_f32(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t ss
                    const float *map1, const float *map2, int dw, int dh, uint8_t *dst, int64_t dstride, int interp);
 int bevk_remap_f32_typed(bevk_ctx *ctx, const void *src, int sw, int sh, int64_t sstride, int type,
                          const float *map1, const float *map2, int dw, int dh, void *dst, int64_t dstride, int interp);
+int bevk_remap_f32_border(bevk_ctx *ctx, const void *src, int sw, int sh, int64_t sstride, int type,
+                          const float *map1, const float *map2, int dw, int dh, void *dst, int64_t dstride, int interp,
+                          int border_mode, const double border_value[4]);
 /* The same for n DEVICE frames through DEVICE maps (dense, as above), with the strides, checks and word path of
  * bevk_undistort_stack (the maps need 16-byte alignment for the word path); a destination range that overlaps the
  * source frames or the maps is refused.  Only enqueues; can be graph-captured. */
@@ -157,6 +180,10 @@ int bevk_remap_f32_stack(bevk_ctx *ctx, const void *d_src, int64_t src_image_str
 int bevk_remap_f32_stack_typed(bevk_ctx *ctx, const void *d_src, int64_t src_image_stride, int sw, int sh,
                                int64_t src_row_stride, int type, int n, const float *d_map1, const float *d_map2,
                                void *d_dst, int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride, int interp);
+int bevk_remap_f32_stack_border(bevk_ctx *ctx, const void *d_src, int64_t src_image_stride, int sw, int sh,
+                                int64_t src_row_stride, int type, int n, const float *d_map1, const float *d_map2,
+                                void *d_dst, int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride, int interp,
+                                int border_mode, const double border_value[4]);
 /* cv2.convertMaps(map1, map2, dstmap1type, nninterpolation) for w x h maps between BEVK_CV_16SC2 (map2: uint16[h][w] or
  * NULL), BEVK_CV_32FC1 and BEVK_CV_32FC2.  To CV_16SC2 as bevk_remap_f32 converts (dst2 unused with nninterpolation);
  * from CV_16SC2 as x + (map2 & 31) / 32, exactly.  The same type on both sides is BEVK_ERR_ARG.  on_device = 0: host
@@ -191,6 +218,9 @@ int bevk_undistort(bevk_ctx *ctx, int slot, const uint8_t *src, int sw, int sh, 
                    uint8_t *dst, int dw, int dh, int64_t dstride, int interp);
 int bevk_undistort_typed(bevk_ctx *ctx, int slot, const void *src, int sw, int sh, int64_t sstride, int type,
                          void *dst, int dw, int dh, int64_t dstride, int interp);
+int bevk_undistort_border(bevk_ctx *ctx, int slot, const void *src, int sw, int sh, int64_t sstride, int type,
+                          void *dst, int dw, int dh, int64_t dstride, int interp, int border_mode,
+                          const double border_value[4]);
 /* n DEVICE frames (frame i at d_src + i*src_image_stride, rows src_row_stride apart, channels 1/3/4) undistorted
  * through the slot's map or fused model into n DEVICE images (dst_image_stride / dst_row_stride, dw x dh = the slot's
  * size, checked).  Each output pixel's taps are resolved once (map read or camera model) for several frames.  Row
@@ -211,18 +241,25 @@ int bevk_undistort_stack_interp(bevk_ctx *ctx, int slot, const void *d_src, int6
 int bevk_undistort_stack_interp_typed(bevk_ctx *ctx, int slot, const void *d_src, int64_t src_image_stride, int sw, int sh,
                                       int64_t src_row_stride, int type, int n, void *d_dst, int64_t dst_image_stride,
                                       int dw, int dh, int64_t dst_row_stride, int interp);
+int bevk_undistort_stack_interp_border(bevk_ctx *ctx, int slot, const void *d_src, int64_t src_image_stride, int sw,
+                                       int sh, int64_t src_row_stride, int type, int n, void *d_dst,
+                                       int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride, int interp,
+                                       int border_mode, const double border_value[4]);
 /* Which gather the last undistort call (or bevk_remap / bevk_warp_perspective / bevk_warp_affine(_stack) /
  * bevk_resize(_stack)) launched: 4 = k_gather4 (word path), 1 = k_gather (byte path), 2 = k_gather_taps (INTER_CUBIC /
  * INTER_LANCZOS4), 3 = k_resize, 0 = none yet. */
 int bevk_undistort_last_path(bevk_ctx *ctx);
 
-/* ---- K4: cv2.warpPerspective(src, H, (dw,dh), flags=interp), border 0 --------
+/* ---- K4: cv2.warpPerspective(src, H, (dw,dh), flags=interp), border 0 (_border: any)
  *   ExtrinsicCalibration/extrinsicCalib.py:166-169, surroundBEV.py:113-114      */
 int bevk_warp_perspective(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t sstride, int channels,
                           const double H[9], uint8_t *dst, int dw, int dh, int64_t dstride, int interp);
 int bevk_warp_perspective_typed(bevk_ctx *ctx, const void *src, int sw, int sh, int64_t sstride, int type,
                                 const double H[9], void *dst, int dw, int dh, int64_t dstride, int interp);
-/* ---- cv2.warpAffine(src, M, (dw,dh), flags), BORDER_CONSTANT 0 ------------------
+int bevk_warp_perspective_border(bevk_ctx *ctx, const void *src, int sw, int sh, int64_t sstride, int type,
+                                 const double H[9], void *dst, int dw, int dh, int64_t dstride, int interp,
+                                 int border_mode, const double border_value[4]);
+/* ---- cv2.warpAffine(src, M, (dw,dh), flags), BORDER_CONSTANT 0 (_border: any mode) -
  *   ExtrinsicCalibration/extrinsicCalib.py:58 (CenterImage.translate)
  * M: the 2x3 matrix, row-major.  flags: a BEVK_INTER_* (INTER_AREA read as INTER_LINEAR, as cv2 reads it), optionally
  * | BEVK_WARP_INVERSE_MAP; anything else is BEVK_ERR_UNSUPPORTED.  The same gathers as bevk_warp_perspective, with the
@@ -231,6 +268,9 @@ int bevk_warp_affine(bevk_ctx *ctx, const uint8_t *src, int sw, int sh, int64_t 
                      const double M[6], uint8_t *dst, int dw, int dh, int64_t dstride, int flags);
 int bevk_warp_affine_typed(bevk_ctx *ctx, const void *src, int sw, int sh, int64_t sstride, int type,
                            const double M[6], void *dst, int dw, int dh, int64_t dstride, int flags);
+int bevk_warp_affine_border(bevk_ctx *ctx, const void *src, int sw, int sh, int64_t sstride, int type,
+                            const double M[6], void *dst, int dw, int dh, int64_t dstride, int flags, int border_mode,
+                            const double border_value[4]);
 /* The same for n DEVICE frames, laid out as bevk_undistort_stack lays them out (image and row strides on both sides,
  * strides smaller than one image and a destination overlapping the source refused with BEVK_ERR_ARG); word and byte
  * paths as there (bevk_undistort_last_path).  Only enqueues on the ctx stream; can be graph-captured. */
@@ -240,6 +280,10 @@ int bevk_warp_affine_stack(bevk_ctx *ctx, const void *d_src, int64_t src_image_s
 int bevk_warp_affine_stack_typed(bevk_ctx *ctx, const void *d_src, int64_t src_image_stride, int sw, int sh,
                                  int64_t src_row_stride, int type, int n, const double M[6], void *d_dst,
                                  int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride, int flags);
+int bevk_warp_affine_stack_border(bevk_ctx *ctx, const void *d_src, int64_t src_image_stride, int sw, int sh,
+                                  int64_t src_row_stride, int type, int n, const double M[6], void *d_dst,
+                                  int64_t dst_image_stride, int dw, int dh, int64_t dst_row_stride, int flags,
+                                  int border_mode, const double border_value[4]);
 
 /* ---- cv2.resize(src, (dw,dh), fx=fx, fy=fy, interpolation=interp) -----------------
  *   IntrinsicCalibration/intrinsicCalib.py:236, ExtrinsicCalibration/extrinsicCalib.py:125 (ScaleImage)
