@@ -126,6 +126,17 @@ class InCalibrator:
             self.camera._get_undistort_maps()
         return d._und(img)
 
+    def undistort_points(self, pts):
+        """Raw-frame pixels -> pixels of undistort(img)'s image: cv2.fisheye.undistortPoints(pts, K, D, P=P) (a "normal"
+        camera: cv2.undistortPoints) with the P that undistort uses, bit for bit; NumPy or CUDA points."""
+        d = self.camera.data
+        if d.camera_mat is None:
+            raise Exception("no calibration: call set_calibration(K, D) first")
+        P = self.camera._get_camera_mat_dst(d.camera_mat)
+        if self.camera.kind == "fisheye":
+            return ops.fisheye_undistort_points(pts, d.camera_mat, d.dist_coeff, P=P)
+        return ops.undistort_points(pts, d.camera_mat, d.dist_coeff, P=P)
+
     def calibrate(self, img):
         return self.camera.data
 

@@ -306,6 +306,14 @@ class BevGenerator:
     def __call__(self, front, back, left, right, car=None):
         return self.engine.run([[front, back, left, right]], car, self.balance)[0]
 
+    def points_to_bev(self, name, pts):
+        """Pixels of camera `name`'s raw frame -> BEV canvas pixels (BevEngine.camera_to_canvas)."""
+        return self.engine.camera_to_canvas(NAMES.index(name), pts)
+
+    def points_from_bev(self, name, pts):
+        """BEV canvas pixels -> pixels of camera `name`'s raw frame (BevEngine.canvas_to_camera)."""
+        return self.engine.canvas_to_camera(NAMES.index(name), pts)
+
     def run_batch(self, frame_sets, car=None, out=None, pixel_format="bgr", out_format="bgr"):
         """frame_sets: iterable of (front, back, left, right) tuples -> uint8[n][BH][BW][3].  pixel_format "nv12" /
         "i420": the frames are YUV 4:2:0 buffers uint8[FH*3//2][FW] (cv2's layout), converted to BGR on the GPU exactly

@@ -47,6 +47,13 @@ SIGNATURES = {
     "bevk_remap_f32_stack": (C.c_int, [_p, _p, C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, _p, _p, _p, C.c_int64,
                                        C.c_int, C.c_int, C.c_int64, C.c_int]),
     "bevk_convert_maps": (C.c_int, [_p, _p, _p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _p, _p, C.c_int]),
+    "bevk_undistort_points": (C.c_int, [_p, C.c_int, _p, _p, C.c_int64, C.c_int, _dp, _dp, C.c_int, _dp, C.c_int, _dp,
+                                        C.c_int, C.c_int, C.c_double, C.c_int]),
+    "bevk_project_points": (C.c_int, [_p, C.c_int, _p, _p, C.c_int64, C.c_int, _dp, _dp, _dp, _dp, C.c_int, C.c_double,
+                                      C.c_int]),
+    "bevk_fisheye_distort_points": (C.c_int, [_p, _p, _p, C.c_int64, C.c_int, _dp, _dp, C.c_int, C.c_double, C.c_int]),
+    "bevk_perspective_transform": (C.c_int, [_p, _p, _p, C.c_int64, C.c_int, _dp, C.c_int]),
+    "bevk_invert3": (C.c_int, [_dp, _dp]),
     "bevk_undistorter_set": (C.c_int, [_p, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, C.c_int, C.c_int, C.c_int]),
     "bevk_undistorter_set_rectify": (C.c_int, [_p, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, _dp, C.c_int, C.c_int, C.c_int]),
     "bevk_undistorter_maps": (C.c_int, [_p, C.c_int, _p, _p]),

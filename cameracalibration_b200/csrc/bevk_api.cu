@@ -28,6 +28,7 @@
 #include "bevk_jpeg_prog.cuh"
 #include "bevk_png_enc.cuh"
 #include "bevk_resize.cuh"
+#include "bevk_points.cuh"
 
 #include <cub/device/device_scan.cuh>
 #include <cub/iterator/counting_input_iterator.cuh>
@@ -1161,6 +1162,124 @@ int bevk_convert_maps(bevk_ctx* c, const void* map1, const void* map2, int m1typ
     if (o2) CU(cudaMemcpyAsync(dst2, c->s_o2.p, n * o2, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
   }
+  return BEVK_OK;
+}
+
+// ------------------------------------------------------------------ point functions (bevk_points.cuh)
+template <int OP, int MODEL, class T>
+static void launch_points(bevk_ctx* c, const PointCam& pc, const void* src, void* dst, long long n) {
+  const long long blocks = std::min<long long>((n + 255) / 256, (long long)c->n_sm * 16);
+  k_points<OP, MODEL, T><<<(unsigned)blocks, 256, 0, c->stream>>>(pc, (const T*)src, (T*)dst, n);
+}
+
+// One point call: checks, then host points through scratch (waits) or device points (only enqueued).  The output
+// may alias the input exactly (same element count per point); any other overlap is refused.
+static int points_call(bevk_ctx* c, int op, int model, const PointCam& pc, const void* src, void* dst, int64_t n, int depth,
+                       int on_device) {
+  if (depth != BEVK_CV_32F && depth != BEVK_CV_64F)
+    return fail(BEVK_ERR_ARG, "point depth %d: BEVK_CV_32F (%d) or BEVK_CV_64F (%d)", depth, BEVK_CV_32F, BEVK_CV_64F);
+  if (depth == BEVK_CV_64F && model == BEVK_MODEL_FISHEYE && op != PT_PERSPECTIVE)
+    return fail(BEVK_ERR_UNSUPPORTED, "float64 fisheye points: cv2 uses glibc's tan / atan, which the device cannot "
+                "reproduce to the last bit");
+  if (n < 0) return fail(BEVK_ERR_ARG, "n must be >= 0, got %lld", (long long)n);
+  if (n == 0) return BEVK_OK;
+  if (!src || !dst) return fail(BEVK_ERR_ARG, "null points");
+  const size_t es = depth == BEVK_CV_64F ? 8 : 4, in_bytes = (size_t)n * (op == PT_PROJECT ? 3 : 2) * es,
+               out_bytes = (size_t)n * 2 * es;
+  const char *s0 = (const char*)src, *d0 = (const char*)dst;
+  const bool same = src == dst && op != PT_PROJECT;
+  if (!same && s0 < d0 + out_bytes && d0 < s0 + in_bytes) return fail(BEVK_ERR_ARG, "the output overlaps the input points");
+  const void* in = src;
+  void* out = dst;
+  if (!on_device) {
+    if (c->capturing) return fail(BEVK_ERR_ARG, "host points cannot be mapped inside a graph capture");
+    RET(c->s_src.ensure(in_bytes));
+    RET(c->s_dst.ensure(out_bytes));
+    CU(cudaMemcpyAsync(c->s_src.p, src, in_bytes, cudaMemcpyHostToDevice, c->stream));
+    in = c->s_src.p;
+    out = c->s_dst.p;
+  }
+  const bool f64 = depth == BEVK_CV_64F;
+  if (op == PT_UNDISTORT && model == BEVK_MODEL_FISHEYE) launch_points<PT_UNDISTORT, 0, float>(c, pc, in, out, n);
+  else if (op == PT_UNDISTORT) f64 ? launch_points<PT_UNDISTORT, 1, double>(c, pc, in, out, n)
+                                   : launch_points<PT_UNDISTORT, 1, float>(c, pc, in, out, n);
+  else if (op == PT_PROJECT && model == BEVK_MODEL_FISHEYE) launch_points<PT_PROJECT, 0, float>(c, pc, in, out, n);
+  else if (op == PT_PROJECT) f64 ? launch_points<PT_PROJECT, 1, double>(c, pc, in, out, n)
+                                 : launch_points<PT_PROJECT, 1, float>(c, pc, in, out, n);
+  else if (op == PT_DISTORT) launch_points<PT_DISTORT, 0, float>(c, pc, in, out, n);
+  else f64 ? launch_points<PT_PERSPECTIVE, 0, double>(c, pc, in, out, n) : launch_points<PT_PERSPECTIVE, 0, float>(c, pc, in, out, n);
+  CU(cudaGetLastError());
+  LAUNCHED(c);
+  if (!on_device) {
+    CU(cudaMemcpyAsync(dst, out, out_bytes, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+  }
+  return BEVK_OK;
+}
+
+static int point_camera(int op, int model, const double* K, const double* D, int n_dist, const double* R, int n_r,
+                        const double* P, const double* t, double alpha, int crit, int max_count, double eps, PointCam* pc) {
+  if (model != BEVK_MODEL_FISHEYE && model != BEVK_MODEL_PINHOLE) return fail(BEVK_ERR_ARG, "bad camera model %d", model);
+  if (!K) return fail(BEVK_ERR_ARG, "null K");
+  if (n_dist > 0 && !D) return fail(BEVK_ERR_ARG, "null D");
+  if (R && !(n_r == 9 || (n_r == 3 && model == BEVK_MODEL_FISHEYE)))
+    return fail(BEVK_ERR_ARG, "R has %d entries: a 3x3 matrix (9)%s", n_r, model == BEVK_MODEL_FISHEYE ? " or an rvec (3)" : "");
+  switch (points_camera(op, model, K, D, n_dist, R, n_r, P, t, alpha, crit, max_count, eps, pc)) {
+    case PTS_BAD_COUNT:
+      return fail(BEVK_ERR_ARG, model == BEVK_MODEL_FISHEYE ? "fisheye D has %d coefficients, cv2 takes 4 (or 0)"
+                                                            : "pinhole D has %d coefficients, cv2 takes 4, 5, 8, 12 or 14 (or 0)",
+                  n_dist);
+    case PTS_BAD_CRITERIA:
+      return fail(BEVK_ERR_UNSUPPORTED, "criteria type %d without COUNT: cv2 iterates without bound", crit);
+    case PTS_TOO_MANY_ITERATIONS:
+      return fail(BEVK_ERR_UNSUPPORTED, "criteria max_count %d: at most %d iterations per point", max_count,
+                  MAX_POINT_ITERATIONS);
+    case PTS_EPS_UNFOLLOWED:
+      return fail(BEVK_ERR_UNSUPPORTED, "cv2.undistortPointsIter's EPS criterion (its reprojection-error stop) is not "
+                  "followed; use COUNT");
+    default: return BEVK_OK;
+  }
+}
+
+int bevk_undistort_points(bevk_ctx* c, int model, const void* src, void* dst, int64_t n, int depth, const double* K,
+                          const double* D, int n_dist, const double* R, int n_r, const double* P, int criteria_type,
+                          int max_count, double epsilon, int on_device) {
+  RET(use(c));
+  PointCam pc;
+  RET(point_camera(PT_UNDISTORT, model, K, D, n_dist, R, n_r, P, nullptr, 0., criteria_type, max_count, epsilon, &pc));
+  return points_call(c, PT_UNDISTORT, model, pc, src, dst, n, depth, on_device);
+}
+
+int bevk_project_points(bevk_ctx* c, int model, const void* obj, void* dst, int64_t n, int depth, const double* rvec,
+                        const double* tvec, const double* K, const double* D, int n_dist, double alpha, int on_device) {
+  RET(use(c));
+  if (!rvec || !tvec) return fail(BEVK_ERR_ARG, "null rvec / tvec");
+  PointCam pc;
+  RET(point_camera(PT_PROJECT, model, K, D, n_dist, nullptr, 0, nullptr, tvec, alpha, CRIT_COUNT, 0, 0., &pc));
+  rodrigues(rvec, pc.RR);
+  return points_call(c, PT_PROJECT, model, pc, obj, dst, n, depth, on_device);
+}
+
+int bevk_fisheye_distort_points(bevk_ctx* c, const void* src, void* dst, int64_t n, int depth, const double* K,
+                                const double* D, int n_dist, double alpha, int on_device) {
+  RET(use(c));
+  PointCam pc;
+  RET(point_camera(PT_DISTORT, BEVK_MODEL_FISHEYE, K, D, n_dist, nullptr, 0, nullptr, nullptr, alpha, CRIT_COUNT, 0, 0., &pc));
+  return points_call(c, PT_DISTORT, BEVK_MODEL_FISHEYE, pc, src, dst, n, depth, on_device);
+}
+
+int bevk_perspective_transform(bevk_ctx* c, const void* src, void* dst, int64_t n, int depth, const double* M, int on_device) {
+  RET(use(c));
+  if (!M) return fail(BEVK_ERR_ARG, "null M");
+  PointCam pc;
+  memset(&pc, 0, sizeof pc);
+  memcpy(pc.RR, M, sizeof pc.RR);
+  return points_call(c, PT_PERSPECTIVE, BEVK_MODEL_PINHOLE, pc, src, dst, n, depth, on_device);
+}
+
+int bevk_invert3(const double* S, double* T) {
+  if (!S || !T) return fail(BEVK_ERR_ARG, "null matrix");
+  if (!inv3(S, T)) return fail(BEVK_ERR_ARG, "singular matrix");
   return BEVK_OK;
 }
 

@@ -778,6 +778,159 @@ def luminance_balance(images, ctx: L.Context | None = None):
     return outs
 
 
+# ---- points: cv2's point functions (bevk_points.cuh), bit for bit.  NumPy points come back as NumPy arrays; CUDA
+# points (__cuda_array_interface__) are mapped on torch's current stream into new torch tensors, without a synchronise.
+TERM_COUNT, TERM_EPS = 1, 2   # cv2.TermCriteria_COUNT / _EPS
+_POINT_DEPTHS = {"<f4": 5, "<f8": 6}
+
+
+def _points(pts, k, what, flat=True):
+    """(pts, n, typestr, out shape) of cv2 points of k elements: [N][1][k] or [1][N][k] (and [N][k] where cv2's pinhole
+    functions take it, flat=True, which they return as [N][1][2]); float32 or float64, dense."""
+    iface = getattr(pts, "__cuda_array_interface__", None)
+    if iface is None:
+        pts = np.asarray(pts)
+        typestr = pts.dtype.str
+        pts = np.ascontiguousarray(pts)
+    else:
+        typestr = iface["typestr"]
+    if typestr not in _POINT_DEPTHS:
+        raise L.BevkError(f"{what}: points must be float32 or float64, got {typestr}")
+    shape = _shape(pts)
+    if len(shape) == 3 and shape[2] == k and 1 in shape[:2]:
+        n = shape[0] * shape[1]
+        out = (n, 1, 2) if flat else (shape[0], shape[1], 2)
+    elif flat and len(shape) == 2 and shape[1] == k:
+        n, out = shape[0], (shape[0], 1, 2)
+    else:
+        raise L.BevkError(f"{what}: points must be [N][1][{k}] or [1][N][{k}]{f' or [N][{k}]' if flat else ''}, got {shape}")
+    return pts, n, typestr, out
+
+
+def _point_call(pts, k, what, flat, call, ctx, out=None):
+    """Run call(src, dst, n, depth, on_device) on host or CUDA points; out: an existing destination (in place: pts).
+    A NumPy destination must be a writeable C-contiguous float32 / float64 ndarray (the call writes it densely)."""
+    ctx = ctx or L.default_context()
+    if out is not None and not hasattr(out, "__cuda_array_interface__") and not (
+            isinstance(out, np.ndarray) and out.dtype.str in _POINT_DEPTHS and out.flags.c_contiguous
+            and out.flags.writeable):
+        raise L.BevkError(f"{what}: inplace needs a writeable C-contiguous float32 or float64 array")
+    pts, n, typestr, shape = _points(pts, k, what, flat)
+    depth = _POINT_DEPTHS[typestr]
+    if hasattr(pts, "__cuda_array_interface__"):
+        import torch
+        from .sharding import _torch_current_stream
+        if out is None:
+            out = torch.empty(shape, dtype=torch.float32 if depth == 5 else torch.float64, device=torch.device("cuda", ctx.device))
+        src = _cuda_dense(pts, typestr, what) if n else None
+        dst = _cuda_dense(out, typestr, what) if n else None
+        with ctx.on_stream(_torch_current_stream(ctx.device)):
+            L.check(call(ctx, src, dst, n, depth, 1))
+        return out
+    if out is None:
+        out = np.empty(shape, np.dtype(typestr))
+    L.check(call(ctx, L.vptr(pts) if n else None, L.vptr(out) if n else None, n, depth, 0))
+    return out
+
+
+def _dist(D):
+    d = None if D is None else np.asarray(D, np.float64).reshape(-1)
+    return (None, 0) if d is None or d.size == 0 else (L.dptr(d), int(d.size))
+
+
+def _mat3(M, what):
+    if M is None:
+        return None
+    m = np.asarray(M, np.float64)
+    if m.shape == (3, 4):   # a projection matrix: its first three columns, as cv2 takes them
+        m = m[:, :3]
+    if m.shape != (3, 3):
+        raise L.BevkError(f"{what} must be 3x3, got shape {m.shape}")
+    return L.dptr(m)
+
+
+def _undistort_points(model, src, K, D, R, P, criteria, ctx, inplace, what):
+    typ, count, eps = criteria
+    d, nd = _dist(D)
+    r, nr = None, 0
+    if R is not None:
+        rr = np.asarray(R, np.float64)
+        if rr.size == 3 and model == L.MODEL_FISHEYE:
+            r, nr = L.dptr(rr), 3
+        else:
+            r, nr = _mat3(rr, "R"), 9
+    return _point_call(src, 2, what, model == L.MODEL_PINHOLE, lambda c, s, o, n, dep, dev: c.lib.bevk_undistort_points(
+        c.h, model, s, o, n, dep, L.dptr(K), d, nd, r, nr, _mat3(P, "P"), int(typ), int(count), float(eps), dev), ctx,
+        src if inplace else None)
+
+
+def undistort_points(src, cameraMatrix, distCoeffs, dst=None, R=None, P=None, ctx: L.Context | None = None,
+                     inplace: bool = False):
+    """cv2.undistortPoints(src, cameraMatrix, distCoeffs, R=, P=): D of 0, 4, 5, 8, 12 or 14 coefficients (None: no
+    distortion), R 3x3, P 3x3 or 3x4.  Returns [N][1][2] of src's dtype.  inplace=True writes into src ([N][1][2] or
+    [1][N][2]) and returns it."""
+    return undistort_points_iter(src, cameraMatrix, distCoeffs, R, P, (TERM_COUNT, 5, 0.01), ctx=ctx, inplace=inplace)
+
+
+def undistort_points_iter(src, cameraMatrix, distCoeffs, R, P, criteria, dst=None, ctx: L.Context | None = None,
+                          inplace: bool = False):
+    """cv2.undistortPointsIter(src, cameraMatrix, distCoeffs, R, P, criteria) with a COUNT criteria of at most 1000
+    iterations; EPS raises BevkError (its reprojection-error stop is not followed)."""
+    return _undistort_points(L.MODEL_PINHOLE, src, cameraMatrix, distCoeffs, R, P, criteria, ctx, inplace,
+                             "undistort_points")
+
+
+def fisheye_undistort_points(distorted, K, D, undistorted=None, R=None, P=None, criteria=(TERM_COUNT | TERM_EPS, 10, 1e-8),
+                             ctx: L.Context | None = None, inplace: bool = False):
+    """cv2.fisheye.undistortPoints(distorted, K, D, R=, P=, criteria=) for float32 points ([N][1][2] or [1][N][2], returned
+    in the same shape); R a 3x3 matrix or an rvec.  float64 raises BevkError (cv2's glibc tan is not reproducible)."""
+    return _undistort_points(L.MODEL_FISHEYE, distorted, K, D, R, P, criteria, ctx, inplace, "fisheye_undistort_points")
+
+
+def _project(model, objectPoints, rvec, tvec, K, D, alpha, ctx, what):
+    d, nd = _dist(D)
+    rv, tv = np.asarray(rvec, np.float64).reshape(-1), np.asarray(tvec, np.float64).reshape(-1)
+    if rv.size != 3 or tv.size != 3:
+        raise L.BevkError(f"{what}: rvec and tvec must have 3 entries")
+    pts = _point_call(objectPoints, 3, what, model == L.MODEL_PINHOLE, lambda c, s, o, n, dep, dev: c.lib.bevk_project_points(
+        c.h, model, s, o, n, dep, L.dptr(rv), L.dptr(tv), L.dptr(K), d, nd, float(alpha), dev), ctx)
+    return pts, None
+
+
+def project_points(objectPoints, rvec, tvec, cameraMatrix, distCoeffs, imagePoints=None, jacobian=None, aspectRatio=0,
+                   ctx: L.Context | None = None):
+    """cv2.projectPoints(objectPoints, rvec, tvec, cameraMatrix, distCoeffs) -> (imagePoints [N][1][2], None): no
+    jacobian is computed."""
+    if aspectRatio:
+        raise L.BevkError("project_points: aspectRatio is only used by cv2's jacobian, which is not computed")
+    return _project(L.MODEL_PINHOLE, objectPoints, rvec, tvec, cameraMatrix, distCoeffs, 0., ctx, "project_points")
+
+
+def fisheye_project_points(objectPoints, rvec, tvec, K, D, imagePoints=None, alpha: float = 0, jacobian=None,
+                           ctx: L.Context | None = None):
+    """cv2.fisheye.projectPoints(objectPoints, rvec, tvec, K, D, alpha=) -> (imagePoints, None) for float32 points
+    [N][1][3] or [1][N][3]; float64 raises BevkError."""
+    return _project(L.MODEL_FISHEYE, objectPoints, rvec, tvec, K, D, alpha, ctx, "fisheye_project_points")
+
+
+def fisheye_distort_points(undistorted, K, D, distorted=None, alpha: float = 0, ctx: L.Context | None = None,
+                           inplace: bool = False):
+    """cv2.fisheye.distortPoints(undistorted, K, D, alpha=) of float32 normalised points [N][1][2] or [1][N][2]."""
+    d, nd = _dist(D)
+    return _point_call(undistorted, 2, "fisheye_distort_points", False, lambda c, s, o, n, dep, dev:
+                       c.lib.bevk_fisheye_distort_points(c.h, s, o, n, dep, L.dptr(K), d, nd, float(alpha), dev), ctx,
+                       undistorted if inplace else None)
+
+
+def perspective_transform(src, m, dst=None, ctx: L.Context | None = None, inplace: bool = False):
+    """cv2.perspectiveTransform(src, m) of float32 or float64 2-D points [N][1][2] or [1][N][2] by a 3x3 m."""
+    mm = np.asarray(m, np.float64)
+    if mm.shape != (3, 3):
+        raise L.BevkError(f"perspective_transform: m must be 3x3 (2-D points), got shape {mm.shape}")
+    return _point_call(src, 2, "perspective_transform", False, lambda c, s, o, n, dep, dev:
+                       c.lib.bevk_perspective_transform(c.h, s, o, n, dep, L.dptr(mm), dev), ctx, src if inplace else None)
+
+
 class Undistorter:
     """Device-resident undistortion map (or fused camera model) + per-frame gather.
 
@@ -947,6 +1100,7 @@ class BevEngine:
         self.n_cam = n_cam
         self.FW, self.FH = int(frame_size[0]), int(frame_size[1])
         self.BW, self.BH = int(bev_size[0]), int(bev_size[1])
+        self._point_cams = {}   # cam -> (model, K, D, P, H, inv(H)): what camera_to_canvas / canvas_to_camera chain
         L.check(self.ctx.lib.bevk_bev_configure(self.ctx.h, n_cam, self.FW, self.FH, self.BW, self.BH))
         self.finalized = False
 
@@ -964,7 +1118,42 @@ class BevEngine:
                                                            L.dptr(P), int(und_size[0]), int(und_size[1]), L.dptr(H)))
         else:
             raise L.BevkError(f'camera model must be "fisheye" or "pinhole", got {model!r}')
+        Hd, Hi = np.array(H, np.float64).reshape(3, 3), np.empty((3, 3))
+        L.check(self.ctx.lib.bevk_invert3(L.dptr(Hd), Hi.ctypes.data_as(L._dp)))
+        self._point_cams[cam] = (model, np.array(K, np.float64), d if model == "fisheye" else dd, np.array(P, np.float64),
+                                 Hd, Hi)
         self.finalized = False
+
+    def _point_cam(self, cam):
+        if cam not in self._point_cams:
+            raise L.BevkError(f"camera {cam} is not set")
+        return self._point_cams[cam]
+
+    def camera_to_canvas(self, cam, pts):
+        """Camera `cam`'s raw-frame pixels -> canvas pixels, as the chain cv2.perspectiveTransform(
+        cv2.fisheye.undistortPoints(pts, K, D, P=P), H) (a pinhole: cv2.undistortPoints) of set_camera's K, D, P, H
+        computes them, bit for bit.  pts: float32 [N][1][2] or [1][N][2] (a pinhole also takes float64 and [N][2]),
+        NumPy or CUDA; the result has the chain's shape and dtype."""
+        model, K, D, P, H, _ = self._point_cam(cam)
+        und = (fisheye_undistort_points(pts, K, D, P=P, ctx=self.ctx) if model == "fisheye"
+               else undistort_points(pts, K, D, P=P, ctx=self.ctx))
+        return perspective_transform(und, H, ctx=self.ctx)
+
+    def canvas_to_camera(self, cam, pts):
+        """Canvas pixels -> camera `cam`'s raw-frame pixels, as the chain cv2.fisheye.distortPoints(cv2.undistortPoints(
+        cv2.perspectiveTransform(pts, cv2.invert(H)[1]), P, None), K, D) computes them (a pinhole: cv2.projectPoints of
+        (x, y, 1) with zero rvec and tvec), bit for bit.  pts: float32 [N][1][2] or [1][N][2] (a pinhole also takes
+        float64), NumPy or CUDA; returns [N][1][2]."""
+        model, K, D, P, _, Hi = self._point_cam(cam)
+        xy = undistort_points(perspective_transform(pts, Hi, ctx=self.ctx), P, None, ctx=self.ctx)
+        if model == "fisheye":
+            return fisheye_distort_points(xy, K, D, ctx=self.ctx)
+        if hasattr(xy, "__cuda_array_interface__"):
+            import torch
+            xyz = torch.cat([xy, torch.ones_like(xy[..., :1])], -1)
+        else:
+            xyz = np.concatenate([xy, np.ones_like(xy[..., :1])], -1)
+        return project_points(xyz, np.zeros(3), np.zeros(3), K, D, ctx=self.ctx)[0]
 
     def set_maps(self, cam: int, map1, map2):
         m1 = np.ascontiguousarray(map1, np.int16)

@@ -191,6 +191,41 @@ int bevk_remap_f32_stack_border(bevk_ctx *ctx, const void *d_src, int64_t src_im
 int bevk_convert_maps(bevk_ctx *ctx, const void *map1, const void *map2, int m1type, int w, int h, int dstm1type,
                       int nninterpolation, void *dst1, void *dst2, int on_device);
 
+/* ---- points: cv2's point functions, one thread per point, bit for bit as cv2 4.13 computes them.
+ * Points are dense arrays of n points (n >= 0) of 2 elements (3 for object points) at depth BEVK_CV_32F or BEVK_CV_64F;
+ * the output is n points of 2 elements of the same depth.  on_device = 0: host buffers, done when the call returns;
+ * 1: device buffers, only enqueued on the ctx stream (graph-capturable).  dst may be src itself (not for
+ * bevk_project_points); any other overlap is BEVK_ERR_ARG.  D lengths cv2 refuses are BEVK_ERR_ARG.
+ * Refused with BEVK_ERR_UNSUPPORTED:
+ *   - float64 fisheye points (undistort, project, distort): cv2 evaluates tan / atan with glibc, which is not
+ *     correctly rounded and which the device cannot reproduce to the last bit; at float32 a result differs only when
+ *     a float rounding boundary falls inside the few-ulp gap;
+ *   - the pinhole EPS criterion (cv2.undistortPointsIter's reprojection-error stop is not followed);
+ *   - a criteria type without COUNT: cv2 then iterates without bound;
+ *   - max_count above 1000: each iteration costs FP64 divisions per point, and the bound keeps one call from holding
+ *     the device for minutes (cv2's defaults are 5 and 10). */
+enum { BEVK_CV_64F = 6 };
+enum { BEVK_TERM_COUNT = 1, BEVK_TERM_EPS = 2 };   /* cv2.TermCriteria_COUNT / _EPS */
+/* cv2.undistortPoints / undistortPointsIter (pinhole: D of 0, 4, 5, 8, 12 or 14; R 3x3 (n_r = 9) or NULL) and
+ * cv2.fisheye.undistortPoints (D of 4 or 0; R a 3x3 matrix (n_r = 9), an rvec (n_r = 3) or NULL).  P: 3x3 or NULL.
+ * cv2's defaults: pinhole COUNT, 5; fisheye COUNT | EPS, 10, 1e-8. */
+int bevk_undistort_points(bevk_ctx *ctx, int model, const void *src, void *dst, int64_t n, int depth, const double K[9],
+                          const double *D, int n_dist, const double *R, int n_r, const double *P, int criteria_type,
+                          int max_count, double epsilon, int on_device);
+/* cv2.projectPoints (pinhole, R = cv2.Rodrigues(rvec)) / cv2.fisheye.projectPoints (with its alpha; ignored for the
+ * pinhole) of n object points [n][3]; image points only, no jacobian. */
+int bevk_project_points(bevk_ctx *ctx, int model, const void *obj, void *dst, int64_t n, int depth, const double rvec[3],
+                        const double tvec[3], const double K[9], const double *D, int n_dist, double alpha, int on_device);
+/* cv2.fisheye.distortPoints(undistorted, K, D, alpha) of normalised points. */
+int bevk_fisheye_distort_points(bevk_ctx *ctx, const void *src, void *dst, int64_t n, int depth, const double K[9],
+                                const double *D, int n_dist, double alpha, int on_device);
+/* cv2.perspectiveTransform of 2-D points by a 3x3 M: (0, 0) where |w| <= FLT_EPSILON.  Float32 and float64, each
+ * with cv2's own body. */
+int bevk_perspective_transform(bevk_ctx *ctx, const void *src, void *dst, int64_t n, int depth, const double M[9],
+                               int on_device);
+/* cv2.invert(S)[1] of a 3x3 S (cv2's closed form, DECOMP_LU); a singular S is BEVK_ERR_ARG. */
+int bevk_invert3(const double S[9], double T[9]);
+
 /* ---- cached-map undistortion (the per-frame call of InCalibrator.undistort /
  * Camera.undistort / Tools/undistort.py's loop).  The map is built on the device
  * once per "slot" and never leaves HBM; each frame is one H2D, one gather kernel,
